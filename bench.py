@@ -10,11 +10,14 @@ A "step" = one batched fit of the rank's shard.  `value` = whole-job series/s wi
 (CUDA events on the library's stream, max over ranks); `e2e` = the same through pb200_fit_host with pinned
 HOST buffers (H2D + D2H inside the timed region).
 
-Scaling.  north_star asks for "50k synthetic series x 1440 points reported at 1/2/4/8 B200": the SAME 50k
+Scaling.  The headline is 50k synthetic series x 1440 points at 1/2/4/8 H100: the SAME 50k
 series split over the ranks (contiguous row-balanced ranges, dist.shard_bounds; no data-path collective), i.e.
 STRONG scaling -- that is the headline `value` at N > 1 (`"scaling": "strong"`).  The weak-scaling figure
 (every rank its own 50k series) is measured in the same run and reported under `weak`.
 `--scaling weak` makes the weak figure the headline instead.  Prints ONE JSON line on rank 0.
+
+`--dump-outputs DIR` writes what the last timed step returned (rank 0's fitted-model arrays) as DIR/<name>.npy, so that
+two builds can be compared output for output on the same seeded inputs.
 """
 from __future__ import annotations
 
@@ -40,8 +43,8 @@ WORKLOAD = "config#3: 50k synthetic series x 1440 15-min pts, logistic growth w/
 ALG_BYTES_PER_SERIES = T_POINTS * 12 + (8 * 62 + 8 * 25 + 8 * 4 + 2 * 8 + 4 * 8)
 # flops per objective+gradient evaluation (SURVEY 8d): ~T*(4K+28), K=14
 FLOPS_PER_EVAL = T_POINTS * (4 * 14 + 28)
-HBM_FALLBACK_GBS = 6650.0      # /opt/skills/guides/B200_PROFILING.md fallback
-FP64_PEAK_GFLOPS = 148 * 64 * 2 * 1.965   # 148 SMs x 64 DFMA/clk x 2 flop x max SM clock (GHz): 37.2 TFLOP/s
+HBM_FALLBACK_GBS = 3350.0      # H100 SXM data sheet (HBM3, 700 W card)
+FP64_PEAK_GFLOPS = 132 * 64 * 2 * 1.98    # 132 SMs x 64 DFMA/clk x 2 flop x max SM clock (GHz): 33.5 TFLOP/s
 
 
 def _peaks():
@@ -54,7 +57,7 @@ def _peaks():
                     return float(d[k]), "measured (MEASURED_PEAKS.json)"
         except Exception:
             pass
-    return HBM_FALLBACK_GBS, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return HBM_FALLBACK_GBS, "fallback (H100 SXM data sheet 3.35 TB/s)"
 
 
 def usable_cores() -> dict:
@@ -72,18 +75,12 @@ def _build_digest():
         return None
 
 
-def _ncu_traffic_per_series():
-    """DRAM bytes per series of the dominant kernel from the committed ncu capture, with what it was captured on.
-    Not measured in this run (ncu replays kernels; a number printed under it is not a bench value)."""
-    p = os.path.join(ROOT, "profiles", "fit_kernel_traffic.json")
-    if os.path.exists(p):
-        try:
-            d = json.load(open(p))
-            return float(d["dram_bytes_per_series"]), {"file": "profiles/fit_kernel_traffic.json", "kernel": d.get("kernel"),
-                                                       "build_digest": d.get("build_digest"), "capture": d.get("capture")}
-        except Exception:
-            return None, None
-    return None, None
+def dump_outputs(dirpath: str, fitted) -> None:
+    """The fitted-model arrays of the last timed step as DIR/<name>.npy (float64; 50k series: ~40 MB in all).
+    meta_i64 holds start_ns / t_scale_ns in whole seconds, which float64 holds exactly up to ~4.6e9 s (the year 2115)."""
+    os.makedirs(dirpath, exist_ok=True)
+    for name in ("params", "tchange", "meta_i32", "meta_i64", "meta_f64"):
+        np.save(os.path.join(dirpath, f"{name}.npy"), np.ascontiguousarray(getattr(fitted, name), dtype=np.float64))
 
 
 class ClockSampler:
@@ -236,7 +233,7 @@ def run_gpu(args):
     world = int(os.environ.get("WORLD_SIZE", "1"))
     local = int(os.environ.get("LOCAL_RANK", "0"))
     if not torch.cuda.is_available():
-        raise RuntimeError("bench.py needs a B200: there is no CPU fallback for the product path")
+        raise RuntimeError("bench.py needs an H100: there is no CPU fallback for the product path")
     torch.cuda.set_device(local)
     if world > 1:
         os.environ.setdefault("MASTER_ADDR", "127.0.0.1")
@@ -309,6 +306,8 @@ def run_gpu(args):
     ms_max, ms_mine, out, launches = timed_fit(b, args.steps, args.warmup, sampler)
     n_job = int(allsum(float(n_mine)))
     host = out.to_host()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, host)
     vc = ctx.last_fit_variant_counts()          # which fit-kernel variant the series of the last step ran on
     variants = {name: int(vc[i].sum()) for i, name in enumerate(("planes", "rotation", "week_table", "day_table")) if vc[i].sum()}
     st = host.meta_i32[:, 4]
@@ -371,22 +370,20 @@ def run_gpu(args):
     peak, peak_src = _peaks()
     per_launch_s = ms_max * 1e-3 / args.steps
     achieved = n_mine * ALG_BYTES_PER_SERIES / per_launch_s / 1e9
-    tps, tsrc = _ncu_traffic_per_series()
     digest = _build_digest()
-    if tsrc is not None:
-        tsrc["matches_this_build"] = bool(digest and tsrc.get("build_digest") == digest)
     gflops = n_mine * float(evals.mean()) * FLOPS_PER_EVAL / per_launch_s / 1e9
     cores = usable_cores()
     cpu = cpu_baseline(int(os.environ.get("PB200_CPU_SAMPLE", str(max(256, 16 * cores["usable"])))), cores) if world == 1 else None
     mean_ms = float(np.mean(rank_ms))
+    l2_mb = torch.cuda.get_device_properties(dev).L2_cache_size / 2**20
     line = {
         "metric": METRIC, "value": value, "unit": UNIT, "n_gpus": world, "steps": args.steps, "warmup": args.warmup,
         "ms_per_step": ms_max / args.steps, "higher_is_better": True, "scaling": "strong" if strong else "weak",
         "vs_baseline": None, "dtype": "f64", "data": "synthetic",
         "config": {"workload": WORKLOAD, "series_per_gpu": n_mine, "points_per_series": T_POINTS,
                    "global_series": n_job, "parallelism": f"series-sharded x{world} (contiguous row-balanced ranges), no data-path collective",
-                   "l2": f"inputs {(b.ds.nbytes + b.y.nbytes) / 1e6:.0f} MB per GPU vs 126 MB L2; every step re-reads them "
-                         f"from HBM (the per-series workspace of the resident series is what lives in L2)",
+                   "l2": f"inputs {(b.ds.nbytes + b.y.nbytes) / 1e6:.0f} MB per GPU vs {l2_mb:.0f} MB L2; every step re-reads them "
+                         f"from HBM (L2 serves the per-series workspace of the resident series, as much of it as fits)",
                    "mean_objective_evals_per_series": float(evals.mean()), "max_objective_evals": int(evals.max()),
                    "series_with_model": fitted_ok, "fit_kernel_variants": variants, "build_digest": digest},
         "e2e": {"value": n_job * e2e_steps / e2e_s, "unit": UNIT, "h2d_bytes_per_step": h2d,
@@ -397,11 +394,11 @@ def run_gpu(args):
                       "limiter": "no collective on the data path: a rank's step ends with its slowest series "
                                  "(max evaluations per series x per-evaluation latency), which does not shrink with the shard"},
         "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-                     "traffic": (tps * n_mine) if tps else None, "traffic_source": tsrc, "peak_source": peak_src,
+                     "peak_source": peak_src,
                      "kernel": _kernel_name(variants, group_of(n_mine)),
                      "algorithmic_bytes_per_launch": n_mine * ALG_BYTES_PER_SERIES,
                      "note": "ds/y are read from HBM once per series; the ~700 objective evaluations stream the "
-                             "series' y (8 B/point) from the L2-resident workspace: the kernel is FP64-issue / latency bound, "
+                             "series' y (8 B/point) from the per-series workspace: the kernel is FP64-issue / latency bound, "
                              "not HBM bound; see fp64 below (model flops of the plain T x K formulation -- the day-table "
                              "variant executes fewer)",
                      "fp64": {"achieved_gflops": gflops, "peak_gflops": FP64_PEAK_GFLOPS, "frac": gflops / FP64_PEAK_GFLOPS,
@@ -558,6 +555,8 @@ def main():
     ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
     ap.add_argument("--scaling", default="strong", choices=["strong", "weak"],
                     help="what `value` means at N > 1: the same 50k series split over the ranks (north_star), or 50k per rank")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the fitted-model arrays of the last timed step (rank 0) to DIR/<name>.npy")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3) if args.impl == "b200" else args.warmup
     if args.impl == "reference":

@@ -1,5 +1,5 @@
 /*
- * prophet_b200.h -- C ABI of the B200-native batched Prophet fitter / scorer.
+ * prophet_b200.h -- C ABI of the H100-native batched Prophet fitter / scorer.
  *
  * Drop-in boundary for the per-series hot path of mageky/time-series-spark:
  *
@@ -18,7 +18,7 @@
  * (the reference turns a per-series RuntimeError into "no output row",
  * prophet_modeler.py:81-85 / prophet_scorer.py:99-102).
  *
- * There is NO CPU fallback behind this ABI: every entry point launches sm_100a
+ * There is NO CPU fallback behind this ABI: every entry point launches sm_90a
  * kernels and fails with PB200_E_CUDA if no device is usable.
  */
 #ifndef PROPHET_B200_H

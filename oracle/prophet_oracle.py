@@ -2,7 +2,7 @@
 
 PARITY UNPINNED.  The reference (mageky/time-series-spark) keeps all of its
 arithmetic in two un-vendored third-party pins, ``fbprophet==0.5`` and
-``pystan==2.19.1.1`` (/root/reference/environment.yml:12-13).  Neither is
+``pystan==2.19.1.1`` (reference environment.yml:12-13).  Neither is
 installed here, neither can be fetched (no network), and the reference's own
 tests pin no numerical value (tests/unit/*.py assert row counts and column
 names only).  This file therefore *restates the published algorithm* of those

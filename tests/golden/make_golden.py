@@ -1,6 +1,6 @@
-"""Generates the committed golden fixtures (run HERE, where /root/reference exists):
+"""Generates the committed golden fixtures from a checkout of the reference repository:
 
-    python tests/golden/make_golden.py
+    python tests/golden/make_golden.py <path to mageky/time-series-spark>
 
   model_input_751.npz      the reference's only data fixture
                            (tests/fixtures/model-input/series_id=751/sample-model-input.csv,
@@ -26,12 +26,13 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, os.path.dirname(os.path.dirname(HERE)))
 from oracle import prophet_oracle as po  # noqa: E402
 
-SRC = "/root/reference/tests/fixtures/model-input/series_id=751/sample-model-input.csv"
+FIXTURE = os.path.join("tests", "fixtures", "model-input", "series_id=751", "sample-model-input.csv")
 
 
 def main():
-    raw = open(SRC, "rb").read()
-    df = pd.read_csv(SRC, header=None, names=["dim_id", "ds", "y"], parse_dates=["ds"])
+    src = os.path.join(sys.argv[1], FIXTURE)
+    raw = open(src, "rb").read()
+    df = pd.read_csv(src, header=None, names=["dim_id", "ds", "y"], parse_dates=["ds"])
     ds_ns = df["ds"].values.astype("datetime64[ns]").astype(np.int64)
     np.savez_compressed(os.path.join(HERE, "model_input_751.npz"), dim_id=df["dim_id"].values.astype(np.int32),
                         ds_ns=ds_ns, y=df["y"].values.astype(np.int32), n_bytes=np.int64(len(raw)),

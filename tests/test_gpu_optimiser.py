@@ -1,4 +1,4 @@
-"""GPU tests that pin the OPTIMISER (run with -m gpu on a B200), not just the cloud of points it ends in.
+"""GPU tests that pin the OPTIMISER (run with -m gpu on an H100), not just the cloud of points it ends in.
 
 tests/test_gpu_parity.py holds the fitted forecasts to distribution-level tolerances, because Stan's loose
 relative-gradient stop amplifies last-bit differences.  That leaves room for a wrong line-search or update

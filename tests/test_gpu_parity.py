@@ -1,4 +1,4 @@
-"""GPU parity tests (run with -m gpu on a B200).  Everything goes through the C ABI
+"""GPU parity tests (run with -m gpu on an H100).  Everything goes through the C ABI
 (libprophet_b200.so via ctypes); the numpy oracle is only the checker.
 
 What can and cannot be pinned.  The model arithmetic (objective, gradient, predict) is

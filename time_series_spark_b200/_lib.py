@@ -1,7 +1,7 @@
 """ctypes binding of libprophet_b200.so (C ABI in include/prophet_b200.h).
 
 There is no CPU fallback: importing this module never builds or emulates anything, and
-``load()`` raises if the CUDA library is missing; ``Context()`` raises if no B200 is visible.
+``load()`` raises if the CUDA library is missing; ``Context()`` raises if no H100 is visible.
 """
 from __future__ import annotations
 

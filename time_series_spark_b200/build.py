@@ -1,4 +1,4 @@
-"""Builds libprophet_b200.so (hand-written sm_100a CUDA + C ABI) in-tree with nvcc.
+"""Builds libprophet_b200.so (hand-written sm_90a CUDA + C ABI) in-tree with nvcc.
 
     python -m time_series_spark_b200.build [--force]
 
@@ -21,8 +21,9 @@ OBJ = os.path.join(CSRC, "_build", _VARIANT) if _VARIANT else os.path.join(CSRC,
 LIB = os.path.join(HERE, f"libprophet_b200{'_' + _VARIANT if _VARIANT else ''}.so")
 INCLUDE = os.path.join(os.path.dirname(HERE), "include")
 
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]     # H100 (Hopper)
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+    *ARCH, "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC", "-Xcompiler", "-fvisibility=hidden", "--expt-relaxed-constexpr",
 ] + [f for f in os.environ.get("PB200_NVCC_EXTRA", "").split() if f]
 
@@ -48,13 +49,13 @@ def _sources_digest() -> str:
 
 
 def build(force: bool = False, verbose: bool = False) -> str:
-    os.makedirs(OBJ, exist_ok=True)
-    # the stamp lives next to the library, not in _build/: the objects stay behind when a snapshot of the tree is sent to
-    # a GPU box (.gpurunignore) but the library travels, and without its stamp every test session there recompiled it
+    # the stamp lives next to the library, not in _build/: a copy of the tree that leaves the object files behind still
+    # finds the library up to date instead of recompiling it
     stamp = LIB + ".digest"
     digest = _sources_digest()
     if not force and os.path.exists(LIB) and os.path.exists(stamp) and open(stamp).read() == digest:
         return LIB
+    os.makedirs(OBJ, exist_ok=True)
     nvcc = _nvcc()
     jobs = []
     for m in range(8):
@@ -77,7 +78,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
                 raise RuntimeError("nvcc failed: " + " ".join(cmd))
     objs = [os.path.join(OBJ, f"fit_inst_{m}.o") for m in range(8)] + [os.path.join(OBJ, "capi.o"),
                                                                       os.path.join(OBJ, "fit_group_inst.o")]
-    link = [nvcc, "-shared", "-gencode", "arch=compute_100a,code=sm_100a", "-o", LIB, *objs, "-lcudart"]
+    link = [nvcc, "-shared", *ARCH, "-o", LIB, *objs, "-lcudart"]
     r = subprocess.run(link, capture_output=True, text=True)
     if r.returncode != 0:
         sys.stderr.write(r.stdout + r.stderr)

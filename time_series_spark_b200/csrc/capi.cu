@@ -86,7 +86,7 @@ int env_int(const char* name, int dflt) {
 // Everything one in-flight fit call needs besides its inputs and outputs.  NWS of them: the *_host entry point cuts
 // a big batch into series chunks, one (stream, workspace) pair each, so that the H2D copy of chunk i + 1 overlaps the
 // fit of chunk i and the later chunks' kernels fill the SMs an earlier chunk's stragglers leave idle.  (With two
-// pairs chunk i + 2 had to wait for chunk i's LAST series before it could start: r2i, e2e / value 0.86.)
+// pairs chunk i + 2 had to wait for chunk i's LAST series before it could start.)
 struct FitWs {
     cudaStream_t stream = nullptr;
     cudaEvent_t ctl_ev = nullptr;   // recorded after the H2D copies out of h_ctl
@@ -120,14 +120,14 @@ struct pb200_ctx {
     DevBuf d_trace;        // trajectory rows of pb200_fit_trace_host
     DevBuf d_nq_all, d_offsets_full;   // pb200_fit_host: per-chunk Newton retry queues, the call's offsets on the device
     int plain_grp = 0;     // PB200_PLAIN_GROUP=1: the class WITHOUT seasonality (regular grid; reference config #4) on the grouped kernel
-                           // too.  Off: measured 6 % faster than one warp per series at 500k short series, 3 % slower at 100k and
-                           // 35 % slower at 30k (r2s) -- its rounds are longer, and small batches are latency bound
+                           // too.  Off: it beat one warp per series only at the largest batches measured (500k short series) --
+                           // its rounds are longer, and small batches are latency bound
     int grp_min = 16384;   // PB200_GROUP_MIN: smallest batch that gets 8 lanes per series; smaller ones get 16 (a warp with 4
-                           // series drains longer once the queue is empty).  r2o, ms per step at 6 250 / 12 500 / 50 000 series:
-                           // G = 8: 78 / 113 / 333, G = 16: 73 / 110 / 352, one warp per series (round-1 kernel): 76 / 125 / 455
-    int host_chunks = 1;   // PB200_HOST_CHUNKS: series chunks of pb200_fit_host.  Default 1 (one pass): measured on 50k x 1440
-                           // (r2j / r2k) 1 / 2 / 4 / 8 chunks = 397 / 407 / 440 / 500 ms -- the 865 MB copy is only ~25 ms at
-                           // PCIe 5 speed, and every chunk pays its own straggler drain, which costs more than it hides
+                           // series drains longer once the queue is empty).  H100 (400 W), 1440-point series, ms per step at 12 500 / 50 000
+                           // series: G = 8: 156 / 529, G = 16: 147 / 526 (the same within the run-to-run spread of ~5 %)
+    int host_chunks = 1;   // PB200_HOST_CHUNKS: series chunks of pb200_fit_host.  Default 1 (one pass): more chunks measured slower on 50k x
+                           // 1440 -- the 865 MB copy is short next to the fit, and every chunk pays its own straggler drain,
+                           // which costs more than it hides
 };
 
 namespace {
@@ -252,8 +252,8 @@ PB200_API pb200_ctx* pb200_create(int device) {
     cudaDeviceProp prop;
     cudaGetDeviceProperties(&prop, device);
     c->sms = prop.multiProcessorCount;
-    if (prop.major != 10) {
-        fail(PB200_E_CUDA, "device is not sm_100 (this library is compiled for sm_100a only)");
+    if (prop.major != 9 || prop.minor != 0) {
+        fail(PB200_E_CUDA, "device is not sm_90 (this library is compiled for sm_90a only)");
         delete c;
         return nullptr;
     }
@@ -744,7 +744,7 @@ PB200_API int pb200_fit_host(pb200_ctx* c, const pb200_options* opts, const int6
         }
     }
     // results back, chunk by chunk, only after EVERY chunk is enqueued: a copy into pageable caller memory blocks the
-    // host until its stream gets there, and issued inside the loop above it serialised the chunks (r2h: e2e / value 0.71)
+    // host until its stream gets there, and issued inside the loop above it serialised the chunks
     for (int k = 0; k < nch; ++k) {
         const int64_t s0 = cut[k], nk = cut[k + 1] - s0;
         if (nk <= 0) continue;

@@ -1,14 +1,14 @@
-// Grouped-lanes Prophet MAP fit for sm_100a: G lanes per series, 32 / G series per warp.
+// Grouped-lanes Prophet MAP fit for sm_90a: G lanes per series, 32 / G series per warp.
 //
 // Same per-series algorithm as fit_kernel.cuh (prep done by prep_kernel; Stan L-BFGS restated from
 // bfgs.hpp / bfgs_linesearch.hpp / lbfgs_update.hpp; objective of python/stan/unix/prophet.stan, reached
 // from reference src/jobs/prophet_modeler.py:65-66), for the class that carries the headline workload:
 // regular time grid whose step divides the day into GPT_MIN..GPT steps, weekly + daily seasonality
-// ("day table", variant 3).  Why a second kernel (profiles/r1km_table_variants.md, profiles/r2*.md):
-// with one warp per series 39 % of all warp time went into the ~2.5 k-instruction per-evaluation serial
+// ("day table", variant 3).  Why a second kernel:
+// with one warp per series much of the warp time went into the ~2.5 k-instruction per-evaluation serial
 // code (line search, L-BFGS update, trend adjoints) whose operands are 42-element vectors and 26 trend
 // segments -- most lanes idle or redundant, instruction fetch the top stall, and phase-aligning the warps of
-// an SM did not help (r2a: 475 vs 467 ms).  Here one pass through that code serves 32 / G series:
+// an SM did not help.  Here one pass through that code serves 32 / G series:
 //   * every lane owns T / G contiguous points of ITS series; the point loop is the same instruction
 //     stream for all lanes, so the groups of a warp stay converged through an evaluation;
 //   * vectors live G-strided (element q on lane q mod G), trend segments blocked (32 / G per lane), and
@@ -42,7 +42,7 @@ template <bool SEAS> constexpr int gkx() { return SEAS ? GK : 1; }
 constexpr int ST_IDLE = 0, ST_FIRST = 1, ST_SEARCH = 2, ST_OBJ = 3;
 
 // SEAS = false (the class without seasonality) drops the table and shortens the vectors: 3.7 instead of 5.8 KB per series,
-// the difference between 9 and 14 resident warps per SM (r2s: that class's time is inversely proportional to them)
+// the difference between 9 and 14 resident warps per SM (that class's time falls as they rise)
 template <int G, bool SEAS>
 struct GState {
     static constexpr int PPAD = SEAS ? GPPAD : GPPAD_PLAIN;
@@ -92,7 +92,7 @@ __device__ __forceinline__ double2* gring() {
     return reinterpret_cast<double2*>(pb200_smem + (size_t)(32 / G) * ((sizeof(GState<G, SEAS>) + 15) & ~(size_t)15));
 }
 // the fit options, copied out of the kernel parameters once per warp (the optimiser's routines take them by reference;
-// a reference into the parameter bank would force a local-memory copy that misses L1 on every use: r2c profile)
+// a reference into the parameter bank would force a local-memory copy that misses L1 on every use)
 template <int G, bool SEAS>
 __device__ __forceinline__ FitOptsDev& gopts() {
     return *reinterpret_cast<FitOptsDev*>(reinterpret_cast<unsigned char*>(gring<G, SEAS>()) + (size_t)2 * (grp_u(G) / 2) * 32 * 16);
@@ -336,7 +336,7 @@ __device__ __noinline__ void g_point_pass(GState<G, SEAS>& s, const double* plan
     }
     nfull = min(nfull, nstep);
     // cp.async ring: 2 stages of U points per lane (stage st, half q: row (st (U / 2) + q) of 32 double2).  The 32-bit
-    // shared-window address is taken once: inside the loop the generic-to-shared conversion cost an S2R per step (r2c profile)
+    // shared-window address is taken once: inside the loop the generic-to-shared conversion cost an S2R per step
     double2* const ring = gring<G, SEAS>() + lane;
     const unsigned ring_sa = (unsigned)__cvta_generic_to_shared(ring);
     constexpr unsigned STAGE_B = (U / 2) * 32 * 16;
@@ -356,7 +356,7 @@ __device__ __noinline__ void g_point_pass(GState<G, SEAS>& s, const double* plan
     //   * the gradient sum_i c_i y(i): Clenshaw's recurrence on the reversed sequence, B_i = c_h B_{i-1} + c_i - B_{i-2}
     //     (two operations per harmonic and point, serving sine AND cosine), closed after the lane's last point with
     //     sum = y(n-1) (B_{n-1} - c_h B_{n-2}) + y(n-2) B_{n-2}.
-    // 12 FP64 operations per point instead of 19 (r2m: features by recurrence 6 + dot 7 + gradient 6), 25 (r2b: rotation).
+    // 12 FP64 operations per point instead of 19 (features by recurrence 6 + dot 7 + gradient 6), 25 (rotation).
     // Rounding: recurrences grow errors like n eps / sin(h delta), delta = 2 pi / 672: ~1e-12 of the term over a
     // 180-point chunk (measured against 40-digit arithmetic: 6e-13 for h = 1) -- inside the 1e-10 objective and 1e-8
     // gradient tolerances, and every evaluation restarts from the lane's exact start / end phases.
@@ -1236,14 +1236,14 @@ __device__ __noinline__ void g_write_record(GState<G, SEAS>& s, const FitArgs& a
 // ---------------------------------------------------------------------------------------
 template <int G, bool LOGI, bool MULT, bool SEAS>
 #ifndef PB200_GRP_BLOCKS
-// resident one-warp CTAs per SM the G = 8 register budget is set for.  8 -> 215 registers; 9 -> 168 registers with spills in
-// g_post_accept: 405 vs 376 ms per 50k-series step on the same box (r2l), whether 8 or 9 CTAs are actually resident (the
-// shared-memory footprint allows 9 either way: occupancy is not what limits this kernel)
+// resident one-warp CTAs per SM the G = 8 register budget is set for.  8 -> 240 registers on sm_90a; 9 -> spills in
+// g_post_accept, which measured slower.  Occupancy is not what limits this kernel: on an H100 (400 W) a 50k x 1440 step
+// took the same time, within the run-to-run spread, with 4 to 8 CTAs resident per SM
 #define PB200_GRP_BLOCKS 8
 #endif
 #ifndef PB200_GRP_PLAIN_BLOCKS
-// ... and for the class without seasonality, whose time IS inversely proportional to the resident warps (r2s: 466 / 525 / 607 /
-// 806 ms per 500k short series at 8 / 7 / 6 / 4 CTAs per SM): short point loops, the latency of the serial code dominates
+// ... and for the class without seasonality, whose time DOES fall as resident warps rise (500k short series at
+// 4 to 8 CTAs per SM): short point loops, the latency of the serial code dominates
 #define PB200_GRP_PLAIN_BLOCKS 14
 #endif
 __global__ void __launch_bounds__(32, G != 8 ? 16 : (SEAS ? PB200_GRP_BLOCKS : PB200_GRP_PLAIN_BLOCKS)) fit_group_kernel(const FitArgs a) {

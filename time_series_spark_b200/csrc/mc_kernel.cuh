@@ -1,4 +1,4 @@
-// Monte-Carlo predictive intervals (yhat_lower / yhat_upper) for sm_100a.
+// Monte-Carlo predictive intervals (yhat_lower / yhat_upper) for sm_90a.
 // Restates fbprophet 0.5 Prophet.predict_uncertainty -> sample_posterior_predictive ->
 // sample_model -> sample_predictive_trend (reached from reference
 // src/jobs/prophet_scorer.py:70 and discarded at :86): per draw, new changepoints from a

@@ -1,4 +1,4 @@
-// Batched Prophet predict for sm_100a.  Replaces the per-model body of
+// Batched Prophet predict for sm_90a.  Replaces the per-model body of
 // forecast_time_series_udf (reference src/jobs/prophet_scorer.py:35-102): fbprophet 0.5
 // Prophet.predict = predict_trend (piecewise_linear / piecewise_logistic) +
 // predict_seasonal_components + yhat = trend*(1+multiplicative)+additive, then the

@@ -2,7 +2,7 @@
 
 The reference parallelises over (series_id, dim_id) groups only -- one Spark task per group
 after a hash shuffle (src/jobs/prophet_modeler.py:139-141, src/jobs/prophet_scorer.py:159-161,
-README.md:119-130).  Groups never interact, so the B200 equivalent is a contiguous range
+README.md:119-130).  Groups never interact, so the GPU equivalent is a contiguous range
 shard of the sorted group list balanced by ROWS (not by group count: ragged batches), no
 collective during fit/predict, and -- optionally -- one gather of the final forecast frame to
 rank 0 over NCCL (the only collective; otherwise each rank writes its own part file exactly

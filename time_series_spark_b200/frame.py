@@ -3,7 +3,7 @@
 The reference drives its per-series operators through a handful of Spark DataFrame calls
 (``groupby(...).apply(udf)`` src/jobs/prophet_modeler.py:139-141, src/jobs/prophet_scorer.py:159-161;
 ``count``/``columns``/``filter``/``select(...).distinct()``/``collect`` in tests/unit/*.py).
-There is no Spark (no JVM) on the B200 path, so this class offers exactly that subset on an
+There is no Spark (no JVM) on the GPU path, so this class offers exactly that subset on an
 Arrow table; ``groupby(keys).apply(op)`` hands ALL groups to the batched operator at once
 instead of one pandas frame per Python worker.
 """

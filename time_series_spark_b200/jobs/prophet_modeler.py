@@ -1,4 +1,4 @@
-"""B200 drop-in for the reference's src/jobs/prophet_modeler.py.
+"""H100 drop-in for the reference's src/jobs/prophet_modeler.py.
 
 Same names and contracts -- ``MODEL_INPUT_SCHEMA``, ``model_time_series(config)``,
 ``ProphetModeler(config).read_input_dataframe / persist_models``, ``ProphetModeler.model`` --

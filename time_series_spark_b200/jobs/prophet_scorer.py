@@ -1,4 +1,4 @@
-"""B200 drop-in for the reference's src/jobs/prophet_scorer.py.
+"""H100 drop-in for the reference's src/jobs/prophet_scorer.py.
 
 Same names and contracts -- ``forecast_time_series(config)``, ``extract_date``,
 ``ProphetScorer(config).read_model_dataframe / convert_forecasts / write_forecasts``,
@@ -175,7 +175,7 @@ _ROWS_PER_PART = 1 << 20
 
 
 def _strftime_via_dictionary(ts, fmt: str):
-    """``pc.strftime`` costs 0.5-0.9 us per VALUE (16 s for 8 M forecast rows, against 3 ms for the GPU to compute them), and a
+    """``pc.strftime`` costs 0.5-0.9 us per VALUE (seconds for millions of forecast rows, which the GPU computes in milliseconds), and a
     forecast frame repeats few distinct timestamps -- every model's horizon is the same handful of grid points.  Format the
     distinct values only and expand through the dictionary indices (a 20 ns per row memcpy).  Falls back to the direct call
     when most values are distinct."""

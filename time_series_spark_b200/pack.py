@@ -138,7 +138,7 @@ def _device_column(col, arrow_type, dev):
     """A null-free primitive Arrow column (ChunkedArray) -> one contiguous device tensor.  The chunks are memcpy'd
     back to back into a small ring of pinned slots and DMA'd from there while the next slot fills: the only host pass
     over the column is that memcpy (no combine_chunks, no pageable cudaMemcpy of a 64-bit key built in numpy -- the
-    two things that made the pack 42 % of the modeler job's wall time in profiles/r2u_e2e_stage_breakdown.log)."""
+    two things that dominated the pack's time)."""
     import torch
     tdtype = {pa.int64(): torch.int64, pa.int32(): torch.int32, pa.float64(): torch.float64}[arrow_type]
     width = 8 if arrow_type != pa.int32() else 4
@@ -189,7 +189,7 @@ def _device_column(col, arrow_type, dev):
 
 def pack_groups_cuda(table: pa.Table, device=None, keys=("series_id", "dim_id"), ds_col="ds", y_col="y"):
     """GPU version of :func:`pack_groups` (SURVEY 8f-2): the columns go to HBM as they are (32-bit ids and y, 64-bit
-    ds), the sort key is formed there and the (series_id, dim_id, ds) sort of the whole frame runs on the B200 as two
+    ds), the sort key is formed there and the (series_id, dim_id, ds) sort of the whole frame runs on the GPU as two
     stable radix sorts (``torch.sort`` -- plumbing, not a hand-written kernel; skipped when the frame already is in
     that order, as a hive-partitioned input written per series is).  ``ds`` / ``y`` stay resident in HBM for
     ``pb200_fit_device``.  Returns a PackedGroups whose ``ds`` / ``y`` are CUDA tensors; ids, offsets and last_ds are

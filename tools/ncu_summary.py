@@ -1,4 +1,4 @@
-"""Prints the key metrics of an .ncu-rep (first kernel) -- used to write profiles/*.md."""
+"""Prints the key metrics of an .ncu-rep (first kernel)."""
 import csv, subprocess, sys
 rep = sys.argv[1]
 out = subprocess.run(["ncu", "-i", rep, "--page", "raw", "--csv"], capture_output=True, text=True).stdout
