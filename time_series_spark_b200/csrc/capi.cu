@@ -133,6 +133,10 @@ struct pb200_ctx {
     int host_chunks = 1;   // PB200_HOST_CHUNKS: series chunks of pb200_fit_host.  Default 1 (one pass): more chunks measured slower on 50k x
                            // 1440 -- the 865 MB copy is short next to the fit, and every chunk pays its own straggler drain,
                            // which costs more than it hides
+    int grid_max = 0;      // PB200_FIT_GRID_MAX (tests): at most this many CTAs per fit launch (grouped and one-series kernels) and per
+                           // Newton launch; unset or <= 0: no cap.  The workspace is sized from the capped grid; the kernel variant, G and
+                           // the evict_last slot count are chosen as without it.  With a small cap every slot fits many series in turn
+                           // (a series' result must not depend on which slot or launch geometry it gets)
 };
 
 namespace {
@@ -290,6 +294,7 @@ PB200_API pb200_ctx* pb200_create(int device) {
     c->grp_min = env_int("PB200_GROUP_MIN", 16384);
     c->plain_grp = env_int("PB200_PLAIN_GROUP", 0) != 0;
     c->l2_keep_pct = std::min(100, env_int("PB200_L2_KEEP_PCT", 65));
+    c->grid_max = std::max(0, env_int("PB200_FIT_GRID_MAX", 0));
     return c;
 }
 
@@ -376,7 +381,8 @@ static int launch_newton(pb200_ctx* c, cudaStream_t st, const pb200_options* opt
     na.o = to_dev(opts);
     const size_t nsm = pb200::nw::newton_smem_bytes(L.pstride);
     CK(cudaFuncSetAttribute(pb200::nw::newton_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)nsm));
-    const int ngrid = (int)std::min<int64_t>(n_series, opts->algorithm == PB200_ALG_NEWTON ? (int64_t)c->sms * 2 : (int64_t)c->sms);
+    int ngrid = (int)std::min<int64_t>(n_series, opts->algorithm == PB200_ALG_NEWTON ? (int64_t)c->sms * 2 : (int64_t)c->sms);
+    if (c->grid_max > 0) ngrid = std::min(ngrid, c->grid_max);
     pb200::nw::newton_kernel<<<ngrid, 32 * pb200::nw::NW_WARPS, nsm, st>>>(na);
     CK(cudaGetLastError());
     c->launches++;
@@ -521,6 +527,7 @@ static int fit_impl(pb200_ctx* c, FitWs& w, const pb200_options* opts, const int
     struct Geo { int grid, Tp, ppad; size_t smem, slice, off; bool on, grouped; };
     Geo geo[NLC][NQ];       // [length class][variant * 8 + seasonality class]
     size_t planes_bytes = 0;
+    auto cap_grid = [&](int64_t grid) { return (int)(c->grid_max > 0 ? std::min<int64_t>(grid, c->grid_max) : grid); };
     for (int lc = 0; lc < NLC; ++lc)
         for (int rm = 0; rm < NQ; ++rm) {
             const int mask = rm & 7, reg = rm >> 3;
@@ -553,14 +560,14 @@ static int fit_impl(pb200_ctx* c, FitWs& w, const pb200_options* opts, const int
                 if (occ < 1) return fail(PB200_E_UNSUPPORTED, "grouped fit kernel does not fit on an SM");
                 g.grouped = true;
                 g.slice = pb200::fit_group_plane_doubles(lc_tmax[lc], grp_g);           // doubles per slot
-                g.grid = (int)std::min<int64_t>(((int64_t)lc_n[lc] + nser - 1) / nser, (int64_t)c->sms * occ);
+                g.grid = cap_grid(std::min<int64_t>(((int64_t)lc_n[lc] + nser - 1) / nser, (int64_t)c->sms * occ));
                 planes_bytes += (size_t)g.grid * nser * g.slice * 8;
                 g.on = true;
                 continue;
             }
             CK(LAUNCH[mask](NT, opts->growth, reg, dummy, 0, g.smem, w.stream, &occ));
             if (occ < 1) return fail(PB200_E_UNSUPPORTED, "fit kernel does not fit on an SM");
-            g.grid = (int)std::min<int64_t>((int64_t)lc_n[lc], (int64_t)c->sms * occ);
+            g.grid = cap_grid(std::min<int64_t>((int64_t)lc_n[lc], (int64_t)c->sms * occ));
             planes_bytes += (size_t)g.grid * g.slice * 16;
             g.on = true;
         }

@@ -361,6 +361,10 @@ struct GPoint {
         } else {
             dz = MULT ? r * opm : r;
         }
+        // A point past the lane's own (only the checked tail steps have them; `valid` is a constant true elsewhere) runs on
+        // at virtual t > 1 when a longer series shares the warp, where the exp-ratio recurrence is unchecked: e = inf gives
+        // sig = NaN, and 0 * NaN would poison the sums.  Its contributions are zeros by definition
+        if (!valid) { cb = 0.0; dz = 0.0; }
     }
 };
 
