@@ -176,8 +176,10 @@ enum PhaseClock {
     PC_PASS_WAIT,      // inside PC_PASS: cp.async.wait_group of the y ring
     PC_POST_HIST,      // inside PC_POST: waiting for the history loads at their first use
     PC_DRAIN,          // inside PC_TOTAL: rounds after the queue ran dry with fewer than 32 / G active groups
+    PC_PASS_LOOP,      // inside PC_PASS: g_point_pass's two step loops; the rest of the pass is the table and the reductions
     PC_ROUNDS,         // (a count, not cycles) evaluation rounds
     PC_WARPS,          // (a count) warps = CTAs of the launches
+    PC_PASS_STEPS,     // (a count) steps run by the step loops
     PC_N
 };
 #ifdef PB200_PHASE_CLOCKS
@@ -492,8 +494,10 @@ __device__ __noinline__ void g_point_pass(GState<G, SEAS>& s, const double* plan
 #pragma unroll
     for (int u = 0; u < U; ++u) tt[u] = (double)(i0 + u) * h;
     const double hU = (double)U * h;
-    auto step = [&](const int m, auto checked_tag) {
+    // direct_tag false: every lane of the warp is on the exp-ratio recurrence (erec), so the step leaves out the test
+    auto step = [&](const int m, auto checked_tag, auto direct_tag) {
         constexpr bool CHECK = decltype(checked_tag)::value;
+        constexpr bool DIRECT = decltype(direct_tag)::value;
         const int n = U * m;
         double2* const cur = ring + (m & (NR - 1)) * (U / 2) * 32;
         const unsigned fill_sa = ring_sa + ((m + D) & (NR - 1)) * STAGE_B;
@@ -508,7 +512,7 @@ __device__ __noinline__ void g_point_pass(GState<G, SEAS>& s, const double* plan
         bool val[U];
         [[maybe_unused]] int pu[U];
         [[maybe_unused]] double sp[U], Rv[U];
-        int jlo[U + 1];
+        int jlo[U + 1];                                    // (jlo[0] is not used)
         double ee[U], kcu[U], mcu[U];
 #pragma unroll
         for (int q = 0; q < U / 2; ++q) {
@@ -528,9 +532,9 @@ __device__ __noinline__ void g_point_pass(GState<G, SEAS>& s, const double* plan
         }
         // exp ratio recurrence: the step INTO a point uses the rate of the segment the previous point is in; then the
         // changepoints AT the point switch rate, offset and ratio.  Nearly all steps hold no changepoint of this lane:
-        // one test, and one divergent region for the steps that do (their partial sums are recorded after the
-        // step's arithmetic, when the contributions of the step's earlier points are known)
-        jlo[0] = j;
+        // one test, and one divergent region for the steps that do.  The boundaries AT the step's first point get the
+        // lane's sums before the step right there; those at later points are recorded after the step's arithmetic, when
+        // the contributions of the step's earlier points are known
         if (nb >= i0 + n + U) {
 #pragma unroll
             for (int u = 0; u < U; ++u) {
@@ -546,6 +550,7 @@ __device__ __noinline__ void g_point_pass(GState<G, SEAS>& s, const double* plan
                 if constexpr (LOGI) { e = e * qj; ee[u] = e; }
                 else ee[u] = 0.0;
                 const int iu = i0 + n + u;
+                const int j_before = j;
                 while (val[u] && iu == nb) {
                     ++j;
                     kcj = s.kc[j];
@@ -553,13 +558,20 @@ __device__ __noinline__ void g_point_pass(GState<G, SEAS>& s, const double* plan
                     if constexpr (LOGI) qj = s.qs[j];
                     nb = j < S ? s.bidx[j] : 0x7fffffff;
                 }
+                if (u == 0) {
+#pragma unroll 1
+                    for (int jj = j_before; jj < j; ++jj) {
+                        s.bndU[jj] = locU;
+                        s.bndV[jj] = locV;
+                    }
+                }
                 kcu[u] = kcj;
                 mcu[u] = mcj;
                 jlo[u + 1] = j;
             }
         }
         if constexpr (LOGI) {
-            if (!erec) {                                       // exponent out of the recurrence's range: direct exp
+            if (DIRECT && !erec) {                             // exponent out of the recurrence's range: direct exp
 #pragma unroll
                 for (int u = 0; u < U; ++u) ee[u] = exp_fastpath(-(kcu[u] * (tt[u] - mcu[u])));
             }
@@ -599,9 +611,9 @@ __device__ __noinline__ void g_point_pass(GState<G, SEAS>& s, const double* plan
         }
         locU = preU[U];
         locV = preV[U];
-        if (jlo[U] != jlo[0]) {                                  // changepoints at point u: sums over the points before it
+        if (jlo[U] != jlo[1]) {                                  // changepoints at point u > 0: sums over the points before it
 #pragma unroll
-            for (int u = 0; u < U; ++u) {
+            for (int u = 1; u < U; ++u) {
 #pragma unroll 1
                 for (int jj = jlo[u]; jj < jlo[u + 1]; ++jj) {
                     s.bndU[jj] = preU[u];
@@ -611,11 +623,20 @@ __device__ __noinline__ void g_point_pass(GState<G, SEAS>& s, const double* plan
         }
         if constexpr (SEAS) __syncwarp();                      // (the bins: all lanes of the warp step together)
     };
+    PB200_PCLK_DECL(loop_t0);
+    PB200_PCLK_NOW(loop_t0);
     int m = 0;
+    if (LOGI && __all_sync(FULL, erec)) {              // (warp-uniform: the steps stay in lockstep for the bins)
 #pragma unroll 1
-    for (; m < nfull; ++m) step(m, std::false_type{});
+        for (; m < nfull; ++m) step(m, std::false_type{}, std::false_type{});
+    } else {
 #pragma unroll 1
-    for (; m < nstep; ++m) step(m, std::true_type{});
+        for (; m < nfull; ++m) step(m, std::false_type{}, std::true_type{});
+    }
+#pragma unroll 1
+    for (; m < nstep; ++m) step(m, std::true_type{}, std::true_type{});
+    PB200_PCLK_ADD(PC_PASS_LOOP, clock64() - loop_t0, lane == 0);
+    PB200_PCLK_ADD(PC_PASS_STEPS, nstep, lane == 0);
     PB200_PCLK_ADD(PC_PASS_WAIT, wait_cyc, lane == 0);
     if constexpr (SEAS) {   // weekly beta gradient: close the Clenshaw sums with the features of the lane's last two (padded) points
         const double2 rcw = *reinterpret_cast<const double2*>(s.rotw);

@@ -5,7 +5,8 @@
 
 Times `reps` fits (CUDA events, after one warm-up fit) and samples nvidia-smi (read-only queries: memory / SM utilisation,
 SM clock, power) while they run.  With a build that has the phase clocks (-DPB200_PHASE_CLOCKS), it also prints each
-phase's share of the kernel's warp cycles (clock64 per warp, summed over the warps; pb200::grp::PhaseClock).  The clocks
+phase's share of the kernel's warp cycles (clock64 per warp, summed over the warps; pb200::grp::PhaseClock), and the
+point pass's step loops in cycles per two-point step next to the rest of the pass per evaluation round.  The clocks
 add instructions to the kernel: compare step times between builds without them.  PB200_GRP_PAD pads each CTA's shared
 memory so that fewer CTAs fit an SM (24576: 4 per SM for G = 8).
 """
@@ -23,8 +24,10 @@ import torch  # noqa: E402
 from time_series_spark_b200 import _lib as L, batched, synth  # noqa: E402
 
 PHASES = ["total", "fetch", "eval_setup", "point_pass", "eval_finalize", "ls_step", "post_accept", "ls_begin", "write_record",
-          "point_pass.cp_async_wait", "post_accept.history_wait", "drain", "rounds", "warps"]
+          "point_pass.cp_async_wait", "post_accept.history_wait", "drain", "point_pass.step_loops", "rounds", "warps",
+          "point_pass.steps"]
 EXCLUSIVE = PHASES[1:9]
+COUNTS = ("rounds", "warps", "point_pass.steps")
 
 
 class Smi:
@@ -95,10 +98,15 @@ def main():
         read(buf, len(PHASES), 0)
         c = dict(zip(PHASES, (int(x) for x in buf)))
         tot = max(c["total"], 1)
-        res["warp_cycle_share"] = {k: round(c[k] / tot, 4) for k in PHASES[1:-2]}
+        res["warp_cycle_share"] = {k: round(c[k] / tot, 4) for k in PHASES[1:] if k not in COUNTS}
         res["warp_cycle_share"]["(exclusive phases sum)"] = round(sum(c[k] for k in EXCLUSIVE) / tot, 4)
         res["cycles_per_round_per_warp"] = tot / max(c["rounds"], 1)
         res["wait_cycles_per_round_per_warp"] = c["point_pass.cp_async_wait"] / max(c["rounds"], 1)
+        # the point pass split into its step loops (per two-point step of a warp) and the rest: seasonal table, bins'
+        # gradient and the reductions (per evaluation round)
+        res["step_loop_cycles_per_step"] = c["point_pass.step_loops"] / max(c["point_pass.steps"], 1)
+        res["steps_per_round"] = c["point_pass.steps"] / max(c["rounds"], 1)
+        res["pass_rest_cycles_per_round"] = (c["point_pass"] - c["point_pass.step_loops"]) / max(c["rounds"], 1)
         # the grid is SMs x the occupancy query's CTAs per SM when the batch fills it
         res["ctas_per_sm"] = c["warps"] / reps / torch.cuda.get_device_properties(0).multi_processor_count
     print(json.dumps(res))
