@@ -180,6 +180,8 @@ enum PhaseClock {
     PC_ROUNDS,         // (a count, not cycles) evaluation rounds
     PC_WARPS,          // (a count) warps = CTAs of the launches
     PC_PASS_STEPS,     // (a count) steps run by the step loops
+    PC_POST_CALLS,     // (a count) rounds in which the warp runs g_post_accept (PC_POST's cycles per call)
+    PC_ACCEPTS,        // (a count) accepted line searches, over the groups
     PC_N
 };
 #ifdef PB200_PHASE_CLOCKS
@@ -1035,15 +1037,20 @@ __device__ __noinline__ int g_ls_step(GState<G, SEAS>& s, const int gl, const un
     return ACT_EVAL;
 }
 
-// the rest of BFGSMinimizer::step after an accepted line search; history Y[5], S[5] in global memory `hist`
+// the rest of BFGSMinimizer::step after an accepted line search; history Y[5], S[5] in global memory `hist`.
+// The whole warp calls it, `acc` set in the groups whose line search was accepted: with every lane present the group
+// reductions shuffle under the full mask (a group's lane mask is not known at compile time, and a shuffle under it first
+// has to test which lanes take part).  The other groups run on zeros from their own slot and store nothing
 template <int G, bool SEAS>
-__device__ __noinline__ int g_post_accept(GState<G, SEAS>& s, double* hist, const int gl, const unsigned gm, const int P,
+__device__ __noinline__ int g_post_accept(GState<G, SEAS>& s, double* hist, const int gl, const bool acc, const int P_,
                                           const FitOptsDev& o, double* trace, const int trace_cap, const int l2f) {
     constexpr int NV = (GState<G, SEAS>::PPAD + G - 1) / G;
     LSState& ls = s.ls;
     double* HY = hist;
     double* HS = hist + HMAX * GPPAD;
-    const int ix = ls.ixt, ixt = ls.ix, ig = ls.igt, igt = ls.ig, ip = ls.ipp, ipp = ls.ip;
+    const int P = acc ? P_ : 0;
+    const int ix = acc ? ls.ixt : 0, ixt = acc ? ls.ix : 0, ig = acc ? ls.igt : 0, igt = acc ? ls.ig : 0;
+    const int ip = acc ? ls.ipp : 0, ipp = acc ? ls.ip : 0;
     const double* x = s.vec[ix];
     const double* xt = s.vec[ixt];
     const double* g = s.vec[ig];
@@ -1051,9 +1058,9 @@ __device__ __noinline__ int g_post_accept(GState<G, SEAS>& s, double* hist, cons
     double* p = s.vec[ip];
     double* pp = s.vec[ipp];
     const double fk_1 = ls.fk, fk = ls.ft, alpha = ls.alpha;
-    const int resetB = ls.resetB, H = o.history;
-    int hn = ls.hn, hhead = ls.hhead;
-    if (trace && gl == 0 && ls.iters <= trace_cap) {
+    const int resetB = acc ? ls.resetB : 0, H = o.history;
+    int hn = acc ? ls.hn : 0, hhead = acc ? ls.hhead : 0;
+    if (acc && trace && gl == 0 && ls.iters <= trace_cap) {
         double* tr = trace + (size_t)(ls.iters - 1) * 4;
         tr[0] = (double)ls.iters; tr[1] = fk; tr[2] = alpha; tr[3] = (double)ls.nevals;
     }
@@ -1062,23 +1069,31 @@ __device__ __noinline__ int g_post_accept(GState<G, SEAS>& s, double* hist, cons
     int slot;
     if (hn < H) { slot = hhead + hn; if (slot >= H) slot -= H; ++hn; }
     else { slot = hhead; hhead = hhead + 1 == H ? 0 : hhead + 1; }
-    // history vectors of the two-loop recursion: all loads issued up front (one L2 round trip), the new pair from registers
+    // The new pair is position hn - 1 of the recursion order, whether the history is filling or full: it stays in registers
+    // of its own (sn, yn, and 1 / s.y in rn).  The ho = hn - 1 older pairs, position h at slot (hhead + h) mod H, are loaded
+    // up front (one L2 round trip) with their 1 / s.y
+    const int ho = hn - 1;
     const unsigned long long pol_h = l2_policy(l2f);
-    double hy[HMAX][NV], hs[HMAX][NV];
+    double hy[HMAX - 1][NV], hs[HMAX - 1][NV], hr[HMAX - 1];
 #pragma unroll
-    for (int h = 0; h < HMAX; ++h) {
+    for (int h = 0; h < HMAX - 1; ++h) {
+        int sl = hhead + h;
+        if (sl >= H) sl -= H;
+        const double* const hyp = HY + (sl * GPPAD + gl);         // (element u of the lane: a constant offset u G)
+        const double* const hsp = HS + (sl * GPPAD + gl);
+        hr[h] = h < ho ? s.hrho[sl] : 0.0;
 #pragma unroll
         for (int u = 0; u < NV; ++u) {
             const int q = gl + u * G;
-            const bool ld = h < hn && q < P;
-            int sl = hhead + h;
-            if (sl >= H) sl -= H;
-            hy[h][u] = (ld && sl != slot) ? ldcg_hint(HY + sl * GPPAD + q, pol_h) : 0.0;
-            hs[h][u] = (ld && sl != slot) ? ldcg_hint(HS + sl * GPPAD + q, pol_h) : 0.0;
+            const bool ld = h < ho && q < P;
+            hy[h][u] = ld ? ldcg_hint(hyp + u * G, pol_h) : 0.0;
+            hs[h][u] = ld ? ldcg_hint(hsp + u * G, pol_h) : 0.0;
         }
     }
     double nrm0 = 0.0, nrm1 = 0.0, nrm2 = 0.0, nrm3 = 0.0;   // s.y, y.y, s.s, g.g
-    double gq[NV];
+    double gq[NV], sn[NV], yn[NV];
+    double* const hyn = HY + (slot * GPPAD + gl);
+    double* const hsn = HS + (slot * GPPAD + gl);
 #pragma unroll
     for (int u = 0; u < NV; ++u) {
         const int q = gl + u * G;
@@ -1088,22 +1103,17 @@ __device__ __noinline__ int g_post_accept(GState<G, SEAS>& s, double* hist, cons
             sv = x[q] - xt[q];
             yv = g[q] - gt[q];
             gq[u] = g[q];
-            stcg_hint(HS + slot * GPPAD + q, sv, pol_h);
-            stcg_hint(HY + slot * GPPAD + q, yv, pol_h);
+            stcg_hint(hsn + u * G, sv, pol_h);                  // (P = 0 outside the accepted groups)
+            stcg_hint(hyn + u * G, yv, pol_h);
         }
-        // the new pair is position hn - 1 of the recursion order
-#pragma unroll
-        for (int h = 0; h < HMAX; ++h) {
-            int sl = hhead + h;
-            if (sl >= H) sl -= H;
-            if (h < hn && sl == slot) { hy[h][u] = yv; hs[h][u] = sv; }
-        }
+        sn[u] = sv;
+        yn[u] = yv;
         nrm0 = fma(sv, yv, nrm0); nrm1 = fma(yv, yv, nrm1);
         nrm2 = fma(sv, sv, nrm2); nrm3 = fma(gq[u], gq[u], nrm3);
     }
-    const double skyk = gsum<G>(nrm0, gm), ykyk = gsum<G>(nrm1, gm);
-    const double stepNorm = sqrt(gsum<G>(nrm2, gm));
-    const double gradNorm = sqrt(gsum<G>(nrm3, gm));
+    const double skyk = gsum<G>(nrm0, FULL), ykyk = gsum<G>(nrm1, FULL);
+    const double stepNorm = sqrt(gsum<G>(nrm2, FULL));
+    const double gradNorm = sqrt(gsum<G>(nrm3, FULL));
     double alphak_1;
     if (resetB) {
         const double B0 = fdiv(ykyk, skyk), rB0 = rcp_any(B0);
@@ -1117,54 +1127,65 @@ __device__ __noinline__ int g_post_accept(GState<G, SEAS>& s, double* hist, cons
         alphak_1 = alpha;
     }
     const double gammak = fdiv(skyk, ykyk);
-    if (gl == 0) s.hrho[slot] = rcp_any(skyk);
-    __syncwarp(gm);
+    const double rn = rcp_any(skyk);
+    if (acc && gl == 0) s.hrho[slot] = rn;                          // (read by the calls that follow, after their own syncs)
 #ifdef PB200_PHASE_CLOCKS
     {   // the history loads' exposed round trip: wait for all of them here, where the recursion first needs them
         const long long t0 = clock64();
         double chk = 0.0;
 #pragma unroll
-        for (int h = 0; h < HMAX; ++h)
+        for (int h = 0; h < HMAX - 1; ++h)
 #pragma unroll
             for (int u = 0; u < NV; ++u) chk += hy[h][u] + hs[h][u];
         if (__double_as_longlong(chk) == 0x7ff8dead00000000ll) s.hrho[7] = chk;     // (never true: makes the wait real)
         PB200_PCLK_ADD(PC_POST_HIST, clock64() - t0, (threadIdx.x & 31) == __ffs(__activemask()) - 1);
     }
 #endif
-    // ---- LBFGSUpdate::search_direction (two-loop recursion) ----
-    double pv[NV], hal[HMAX];
+    // ---- LBFGSUpdate::search_direction (two-loop recursion): newest pair first in the first loop, last in the second ----
+    double pv[NV], hal[HMAX - 1];
 #pragma unroll
     for (int u = 0; u < NV; ++u) pv[u] = -gq[u];
+    double aln;
+    {
+        double l = 0.0;
 #pragma unroll
-    for (int h = HMAX - 1; h >= 0; --h) {
-        hal[h] = 0.0;
-        if (h < hn) {
-            int sl = hhead + h;
-            if (sl >= H) sl -= H;
-            double l = 0.0;
+        for (int u = 0; u < NV; ++u) l = fma(sn[u], pv[u], l);
+        aln = rn * gsum<G>(l, FULL);
 #pragma unroll
-            for (int u = 0; u < NV; ++u) l = fma(hs[h][u], pv[u], l);
-            const double al = s.hrho[sl] * gsum<G>(l, gm);
+        for (int u = 0; u < NV; ++u) pv[u] -= aln * yn[u];
+    }
 #pragma unroll
-            for (int u = 0; u < NV; ++u) pv[u] -= al * hy[h][u];
-            hal[h] = al;
-        }
+    for (int h = HMAX - 2; h >= 0; --h) {       // (positions h >= ho: every lane shuffles, nothing is kept)
+        double l = 0.0;
+#pragma unroll
+        for (int u = 0; u < NV; ++u) l = fma(hs[h][u], pv[u], l);
+        const double al = hr[h] * gsum<G>(l, FULL);
+        const bool on = h < ho;
+#pragma unroll
+        for (int u = 0; u < NV; ++u) pv[u] = on ? pv[u] - al * hy[h][u] : pv[u];
+        hal[h] = on ? al : 0.0;
     }
 #pragma unroll
     for (int u = 0; u < NV; ++u) pv[u] *= gammak;
 #pragma unroll
-    for (int h = 0; h < HMAX; ++h) {
-        if (h < hn) {
-            int sl = hhead + h;
-            if (sl >= H) sl -= H;
-            double l = 0.0;
+    for (int h = 0; h < HMAX - 1; ++h) {
+        double l = 0.0;
 #pragma unroll
-            for (int u = 0; u < NV; ++u) l = fma(hy[h][u], pv[u], l);
-            const double be = s.hrho[sl] * gsum<G>(l, gm);
-            const double cf = hal[h] - be;
+        for (int u = 0; u < NV; ++u) l = fma(hy[h][u], pv[u], l);
+        const double be = hr[h] * gsum<G>(l, FULL);
+        const double cf = hal[h] - be;
+        const bool on = h < ho;
 #pragma unroll
-            for (int u = 0; u < NV; ++u) pv[u] += cf * hs[h][u];
-        }
+        for (int u = 0; u < NV; ++u) pv[u] = on ? pv[u] + cf * hs[h][u] : pv[u];
+    }
+    {
+        double l = 0.0;
+#pragma unroll
+        for (int u = 0; u < NV; ++u) l = fma(yn[u], pv[u], l);
+        const double be = rn * gsum<G>(l, FULL);
+        const double cf = aln - be;
+#pragma unroll
+        for (int u = 0; u < NV; ++u) pv[u] += cf * sn[u];
     }
     double gpl = 0.0;
 #pragma unroll
@@ -1173,7 +1194,7 @@ __device__ __noinline__ int g_post_accept(GState<G, SEAS>& s, double* hist, cons
         if (q < P) p[q] = pv[u];
         gpl = fma(gq[u], pv[u], gpl);
     }
-    const double gp = gsum<G>(gpl, gm);
+    const double gp = gsum<G>(gpl, FULL);
     // ---- convergence tests ----
     const double df = fabs(fk_1 - fk);
     int status = PB200_ST_SUCCESS;
@@ -1183,13 +1204,13 @@ __device__ __noinline__ int g_post_accept(GState<G, SEAS>& s, double* hist, cons
     else if (fabs(gp) < o.tol_rel_grad_eps * fmax(fabs(fk), 1.0)) status = PB200_ST_RELGRAD;
     else if (stepNorm < o.tol_param) status = PB200_ST_ABSX;
     else if (ls.iters >= o.max_iter) status = PB200_ST_MAXIT;
-    __syncwarp(gm);
-    if (gl == 0) {
+    __syncwarp();
+    if (acc && gl == 0) {
         ls.ix = ix; ls.ixt = ixt; ls.ig = ig; ls.igt = igt; ls.ip = ip; ls.ipp = ipp;
         ls.fk_1 = fk_1; ls.fk = fk; ls.alphak_1 = alphak_1; ls.hn = hn; ls.hhead = hhead;
         ls.status = status;
     }
-    __syncwarp(gm);
+    __syncwarp();
     return status;
 }
 
@@ -1380,7 +1401,7 @@ __device__ __noinline__ void g_write_record(GState<G, SEAS>& s, const FitArgs& a
 // ---------------------------------------------------------------------------------------
 template <int G, bool LOGI, bool MULT, bool SEAS>
 #ifndef PB200_GRP_BLOCKS
-// resident one-warp CTAs per SM the G = 8 register budget is set for.  8 -> 247 registers on sm_90a; 9 -> spills in
+// resident one-warp CTAs per SM the G = 8 register budget is set for.  8 -> 242 registers on sm_90a; 9 -> spills in
 // g_post_accept, which measured slower.  On an H100 a 50k x 1440 step takes 35 % less time with 8 CTAs per SM than with 4
 // (DESIGN §3)
 #define PB200_GRP_BLOCKS 8
@@ -1390,7 +1411,8 @@ template <int G, bool LOGI, bool MULT, bool SEAS>
 // 4 to 8 CTAs per SM): short point loops, the latency of the serial code dominates
 #define PB200_GRP_PLAIN_BLOCKS 14
 #endif
-__global__ void __launch_bounds__(32, G != 8 ? 16 : (SEAS ? PB200_GRP_BLOCKS : PB200_GRP_PLAIN_BLOCKS)) fit_group_kernel(const FitArgs a) {
+__global__ void __launch_bounds__(32, G != 8 ? 16 : (SEAS ? PB200_GRP_BLOCKS : PB200_GRP_PLAIN_BLOCKS)) fit_group_kernel(const __grid_constant__ FitArgs a) {
+    // (__grid_constant__: g_fetch and g_write_record take `a` by reference without a copy of it in local memory)
     static_assert(G == 8 || G == 16 || G == 32, "lanes per series");
     static_assert(SEAS || !MULT, "without seasonality the additive form is the model");
     static_assert((SEAS ? 6 * G * 8 : 0) + G * 4 <= 5 * GState<G, SEAS>::PPAD * 8, "LanePhase hand-over through vec[1..5]");
@@ -1500,14 +1522,25 @@ __global__ void __launch_bounds__(32, G != 8 ? 16 : (SEAS ? PB200_GRP_BLOCKS : P
         }
         __syncwarp();
         PB200_PCLK_MARK(PC_LS_STEP, t_mark, lane);
-        if (act == ACT_ACCEPT) {
-            double* tr = trace_base ? trace_base + (size_t)s.series * trace_cap * 4 : nullptr;
-            status = g_post_accept<G, SEAS>(s, hist, gl, gm, P, opt, tr, trace_cap, l2f);
-            if (status != PB200_ST_SUCCESS) done = true;
-            else {
-                if (gl == 0) { s.ls.iters += 1; s.ls.resetB = 0; }
-                __syncwarp(gm);
-                act = ACT_FAIL + 1;
+#ifdef PB200_PHASE_CLOCKS
+        {
+            const unsigned acc = __ballot_sync(FULL, act == ACT_ACCEPT);
+            PB200_PCLK_ADD(PC_POST_CALLS, 1, acc != 0 && lane == 0);
+            PB200_PCLK_ADD(PC_ACCEPTS, 1, act == ACT_ACCEPT && gl == 0);
+        }
+#endif
+        if (__any_sync(FULL, act == ACT_ACCEPT)) {
+            const bool acc = act == ACT_ACCEPT;
+            double* tr = (trace_base && acc) ? trace_base + (size_t)s.series * trace_cap * 4 : nullptr;
+            const int st = g_post_accept<G, SEAS>(s, hist, gl, acc, P, opt, tr, trace_cap, l2f);
+            if (acc) {
+                status = st;
+                if (status != PB200_ST_SUCCESS) done = true;
+                else {
+                    if (gl == 0) { s.ls.iters += 1; s.ls.resetB = 0; }
+                    __syncwarp(gm);
+                    act = ACT_FAIL + 1;
+                }
             }
         }
         __syncwarp();

@@ -25,9 +25,9 @@ from time_series_spark_b200 import _lib as L, batched, synth  # noqa: E402
 
 PHASES = ["total", "fetch", "eval_setup", "point_pass", "eval_finalize", "ls_step", "post_accept", "ls_begin", "write_record",
           "point_pass.cp_async_wait", "post_accept.history_wait", "drain", "point_pass.step_loops", "rounds", "warps",
-          "point_pass.steps"]
+          "point_pass.steps", "post_accept.calls", "accepts"]
 EXCLUSIVE = PHASES[1:9]
-COUNTS = ("rounds", "warps", "point_pass.steps")
+COUNTS = ("rounds", "warps", "point_pass.steps", "post_accept.calls", "accepts")
 
 
 class Smi:
@@ -107,6 +107,12 @@ def main():
         res["step_loop_cycles_per_step"] = c["point_pass.step_loops"] / max(c["point_pass.steps"], 1)
         res["steps_per_round"] = c["point_pass.steps"] / max(c["rounds"], 1)
         res["pass_rest_cycles_per_round"] = (c["point_pass"] - c["point_pass.step_loops"]) / max(c["rounds"], 1)
+        # warp cycles per evaluation round of every phase (shares alone do not compare builds routine by routine), and
+        # g_post_accept per call: a warp's call serves every group of it whose line search was accepted that round
+        res["cycles_per_round"] = {k: round(c[k] / max(c["rounds"], 1), 1) for k in PHASES[1:13] if k not in COUNTS}
+        res["post_accept_cycles_per_call"] = c["post_accept"] / max(c["post_accept.calls"], 1)
+        res["post_accept_calls_per_round"] = c["post_accept.calls"] / max(c["rounds"], 1)
+        res["accepts_per_call"] = c["accepts"] / max(c["post_accept.calls"], 1)
         # the grid is SMs x the occupancy query's CTAs per SM when the batch fills it
         res["ctas_per_sm"] = c["warps"] / reps / torch.cuda.get_device_properties(0).multi_processor_count
     print(json.dumps(res))
