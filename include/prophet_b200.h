@@ -103,8 +103,8 @@ typedef struct pb200_options {
     double  tol_grad;               /* 1e-8 */
     double  tol_rel_grad;           /* 1e7  (x machine epsilon) */
     double  tol_param;              /* 1e-8 */
-    double  interval_width;         /* 0.8 */
-    int32_t uncertainty_samples;    /* 1000; 0 = skip yhat_lower / yhat_upper */
+    double  interval_width;         /* 0.8; must be in [0, 1] when intervals are requested (else PB200_E_ARG, nothing launched) */
+    int32_t uncertainty_samples;    /* 1000; 0 = skip yhat_lower / yhat_upper; else [2, 1024] (else PB200_E_UNSUPPORTED) */
     int32_t algorithm;              /* PB200_ALG_*: 0 = fbprophet 0.5's fit(): Stan L-BFGS, Newton retry after a line-search failure */
 } pb200_options;
 
@@ -221,8 +221,10 @@ PB200_API int pb200_fit_trace_host(pb200_ctx* ctx, const pb200_options* opts,
  *               float32 model-table columns (prophet_scorer.py:46-47,67-68)
  * Outputs [n_models * horizon]:
  *   d_yhat        double  trend*(1+multiplicative)+additive
- *   d_yhat_lower / d_yhat_upper  double, MC interval (NULL or uncertainty_samples=0 to skip)
- *   d_yhat_int    int32   (int)yhat, then < floor -> floor   (prophet_scorer.py:73-84)
+ *   d_yhat_lower / d_yhat_upper  double, MC interval (NULL or uncertainty_samples=0 to skip);
+ *                 a function of the seed and the model's own record, not of its place in the batch
+ *   d_yhat_int    int32   (int)yhat, then < floor -> floor   (prophet_scorer.py:73-84),
+ *                 saturated to [INT32_MIN, INT32_MAX]
  * Models whose meta status < 0 produce no forecast: their rows are filled with
  * NaN / INT32_MIN and the caller drops them (empty frame in the reference).
  */

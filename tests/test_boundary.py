@@ -127,6 +127,23 @@ def test_model_record_roundtrip():
         model_record.decode(pa.array([b"not a record, e.g. a pickle"], pa.binary()))
 
 
+@pytest.mark.parametrize("width", [-0.1, 1.5, 95, float("nan")])
+def test_scorer_refuses_out_of_range_interval_width(width):
+    """fbprophet refuses an interval width outside [0, 1] (numpy's percentile range check), e.g. 95 meant as a percent:
+    the scorer names the key before any model is decoded or any GPU work starts."""
+    from time_series_spark_b200.jobs.prophet_scorer import forecast_time_series
+    opts = batched.make_options()
+    lay = L.get_layout(opts)
+    fb = batched.FittedBatch(np.zeros((1, lay.pstride)), np.zeros((1, lay.smax)), np.zeros((1, 8), np.int32),
+                             np.zeros((1, 2), np.int64), np.ones((1, 4)), lay.smax, lay.kmax)
+    tbl = pa.table({"series_id": pa.array([1], pa.int32()), "dim_id": pa.array([2], pa.int32()),
+                    "floor": pa.array([0.0], pa.float32()), "cap": pa.array([10.0], pa.float32()),
+                    "model": model_record.encode(fb, np.zeros(1, np.int64), opts)})
+    op = forecast_time_series({"forecast": {"periods": 4, "frequency": "h", "intervals": True, "interval_width": width}})
+    with pytest.raises(ValueError, match="forecast.interval_width"):
+        op.apply_batched(tbl, ["series_id", "dim_id"])
+
+
 def test_frequency_to_future_matches_pandas():
     import pandas as pd
     last = np.array([pd.Timestamp("2002-12-28 21:45:00").value, pd.Timestamp("2021-03-15 23:45:00").value])

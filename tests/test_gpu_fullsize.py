@@ -63,15 +63,18 @@ def test_config5_shape_scorer_epilogue(gpu_ctx, c3_full):
     assert np.array_equal(fc.yhat_int, expect)
     # logistic trend with cap: forecasts stay below cap * (1 + max seasonal swing)
     assert np.all(fc.yhat.max(axis=1) < 3.0 * cap32)
-    # MC intervals on a slice: ordered, reproducible for a fixed seed and independent of what else is in the batch
+    # MC intervals on a slice: ordered, reproducible for a fixed seed and independent of what else is in the batch and of
+    # the model's place in it (the Philox key is a hash of the model's record): a reversed, non-prefix subset placed
+    # after other models gives every model the bounds it had in the full slice
     sub = batched.FittedBatch(fb.params[:256], fb.tchange[:256], fb.meta_i32[:256], fb.meta_i64[:256], fb.meta_f64[:256],
                               fb.smax, fb.kmax)
     m1 = batched.predict_batch_host(gpu_ctx, opts, sub, fut[:256], np.zeros(256), cap32[:256], seed=11, intervals=True)
-    sub2 = batched.FittedBatch(fb.params[:64], fb.tchange[:64], fb.meta_i32[:64], fb.meta_i64[:64], fb.meta_f64[:64],
-                               fb.smax, fb.kmax)
-    m2 = batched.predict_batch_host(gpu_ctx, opts, sub2, fut[:64], np.zeros(64), cap32[:64], seed=11, intervals=True)
+    idx = np.concatenate([np.arange(200, 230), np.arange(37, 101)[::-1]])
+    sub2 = batched.FittedBatch(*(np.ascontiguousarray(a[idx]) for a in (fb.params, fb.tchange, fb.meta_i32, fb.meta_i64,
+                                                                         fb.meta_f64)), fb.smax, fb.kmax)
+    m2 = batched.predict_batch_host(gpu_ctx, opts, sub2, fut[idx], np.zeros(idx.size), cap32[idx], seed=11, intervals=True)
     assert np.all(m1.yhat_lower < m1.yhat_upper)
-    assert np.array_equal(m1.yhat_lower[:64], m2.yhat_lower) and np.array_equal(m1.yhat_upper[:64], m2.yhat_upper)
+    assert np.array_equal(m1.yhat_lower[idx], m2.yhat_lower) and np.array_equal(m1.yhat_upper[idx], m2.yhat_upper)
 
 
 def test_config4_full_size_ragged(gpu_ctx):

@@ -201,8 +201,11 @@ def test_predict_kernel_matches_oracle_given_same_parameters(gpu_ctx, case):
                           theta=None, neg_logp=0.0, iters=0, n_evals=0, ret=0)
         pr = po.predict(fr, fut[i], 0.0, cap32[i], oopts)
         assert np.max(np.abs(pr["yhat"] - fc.yhat[i])) <= 1e-12 * p.y_scale * max(1.0, np.max(np.abs(pr["yhat"])) / p.y_scale)
+        # the int epilogue exactly, on the kernel's own yhat; and the oracle's wherever the two yhat truncate alike
+        assert np.array_equal(fc.yhat_int[i], np.maximum(np.trunc(fc.yhat[i]), 0.0).astype(np.int32))
         exp_int = po.scorer_epilogue(pr["yhat"], 0.0)
-        assert np.sum(exp_int != fc.yhat_int[i]) == 0 or np.max(np.abs(exp_int - fc.yhat_int[i])) <= 1
+        same = np.trunc(pr["yhat"]) == np.trunc(fc.yhat[i])
+        assert same.sum() >= same.size - 1 and np.array_equal(exp_int[same], fc.yhat_int[i][same])
 
 
 def test_mc_intervals_statistically_match_oracle(gpu_ctx):

@@ -165,6 +165,15 @@ int check_opts(const pb200_options* o) {
     return PB200_OK;
 }
 
+// the MC interval options, checked before anything is copied or launched: the kernel turns interval_width into ranks of the
+// sorted draws, so a width outside [0, 1] (or NaN) would index outside a point's row of draws
+int check_mc_opts(const pb200_options* o) {
+    if (o->uncertainty_samples < 2 || o->uncertainty_samples > pb200::MC_NP)
+        return fail(PB200_E_UNSUPPORTED, "uncertainty_samples must be in [2, 1024]");
+    if (!(o->interval_width >= 0.0 && o->interval_width <= 1.0)) return fail(PB200_E_ARG, "interval_width must be in [0, 1]");
+    return PB200_OK;
+}
+
 FitOptsDev to_dev(const pb200_options* o) {
     FitOptsDev d;
     const double eps = 2.220446049250313e-16;
@@ -856,6 +865,8 @@ PB200_API int pb200_predict_device(pb200_ctx* c, const pb200_options* opts, cons
     if (!d_params || !d_tchange || !d_meta_i32 || !d_meta_i64 || !d_meta_f64 || !d_future_ds || !d_floor || !d_cap ||
         !d_yhat || !d_yhat_int)
         return fail(PB200_E_ARG, "null pointer");
+    const bool mc = d_yhat_lower && d_yhat_upper && opts->uncertainty_samples > 0;
+    if (mc && (rc = check_mc_opts(opts))) return rc;
     pb200_layout L;
     pb200_get_layout(opts, &L);
     CK(cudaSetDevice(c->device));
@@ -886,10 +897,10 @@ PB200_API int pb200_predict_device(pb200_ctx* c, const pb200_options* opts, cons
         CK(cudaGetLastError());
         c->launches++;
     }
-    if (d_yhat_lower && d_yhat_upper && opts->uncertainty_samples > 0) {
+    if (mc) {
         rc = pb200::launch_mc(c->stream, c->sms, a, opts->uncertainty_samples, opts->interval_width, seed, d_yhat_lower,
                               d_yhat_upper);
-        if (rc == -1) return fail(PB200_E_UNSUPPORTED, "uncertainty_samples must be in [2, 1024]");
+        if (rc == -1) return fail(PB200_E_ARG, "uncertainty_samples / interval_width out of range");
         if (rc) return fail(PB200_E_CUDA, "mc kernel launch", cudaGetLastError());
         c->launches++;
     }
@@ -912,6 +923,7 @@ PB200_API int pb200_predict_host(pb200_ctx* c, const pb200_options* opts, const 
     CK(cudaSetDevice(c->device));
     const size_t N = (size_t)n_models, NH = N * (size_t)horizon;
     const bool mc = h_yhat_lower && h_yhat_upper && opts->uncertainty_samples > 0;
+    if (mc && (rc = check_mc_opts(opts))) return rc;
     CK(c->d_params.reserve(N * L.pstride * 8));
     CK(c->d_tchange.reserve(N * L.smax * 8));
     CK(c->d_mi32.reserve(N * 8 * 4));

@@ -10,7 +10,9 @@
 // SAME process by exponential inter-arrival gaps (rate S), which needs O(1) state per draw
 // and no sort of changepoints.  The reference uses the unseeded global numpy RNG, so only
 // the distribution -- not the stream -- can be matched; here the stream is counter-based
-// Philox4x32-10 keyed by (seed, model, draw), reproducible and shard-independent.
+// Philox4x32-10, keyed by the seed and a hash of the model's own record (model_key) and counted by draw:
+// a model's intervals are a function of the model and the seed, whatever else is in the batch and on
+// whichever shard it runs.  oracle/mc_stream.py restates the stream and the sampler in numpy.
 //
 // One CTA per model; thread j owns draws j and j + 512; the draws of a tile of 16 future
 // points are staged in shared memory ([16][1024] fp64) and each warp sorts one row's order
@@ -68,6 +70,41 @@ struct McArgs {
     double* lower;
     double* upper;
 };
+
+__device__ __forceinline__ uint64_t splitmix64(uint64_t z) {
+    z += 0x9E3779B97F4A7C15ull;
+    z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
+    z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
+    return z ^ (z >> 31);
+}
+
+// Philox key of one model, a function of the seed and the model's own record only -- not of its index in the batch -- so
+// that a model gets the same intervals in any batch, on any shard.  Words of the record, in order: params[0, pstride),
+// tchange[0, smax), start_ns, t_scale_ns and the bits of y_scale, floor, cap.  Word i contributes
+// splitmix64(w_i ^ splitmix64(i)); the contributions are XORed (lane l of warp 0 takes words l, l + 32, ...) and the key is
+// splitmix64(xor ^ splitmix64(seed)): k0 its low, k1 its high 32 bits.  oracle/mc_stream.py restates it.
+__device__ __forceinline__ uint64_t model_key(const McArgs& a, const int model, const int lane) {
+    const PredictArgs& p = a.p;
+    const int nw = p.pstride + p.smax + 5;
+    uint64_t h = 0;
+    for (int i = lane; i < nw; i += 32) {
+        uint64_t w;
+        if (i < p.pstride) {
+            w = (uint64_t)__double_as_longlong(p.params[(size_t)model * p.pstride + i]);
+        } else if (i < p.pstride + p.smax) {
+            w = (uint64_t)__double_as_longlong(p.tchange[(size_t)model * p.smax + (i - p.pstride)]);
+        } else {
+            const int j = i - p.pstride - p.smax;
+            if (j < 2) w = (uint64_t)p.meta_i64[(size_t)model * 2 + j];
+            else if (j == 2) w = (uint64_t)__double_as_longlong(p.meta_f64[(size_t)model * 4]);
+            else w = (uint64_t)__double_as_longlong(j == 3 ? p.floor[model] : p.cap[model]);
+        }
+        h ^= splitmix64(w ^ splitmix64((uint64_t)i));
+    }
+#pragma unroll
+    for (int o = 16; o >= 1; o >>= 1) h ^= __shfl_xor_sync(0xffffffffu, h, o);
+    return splitmix64(h ^ splitmix64(a.seed));
+}
 
 template <bool LOGI>
 __device__ __forceinline__ void advance(DrawState& d, const ModelSm& ms, const double t, const Philox& ph,
@@ -196,6 +233,7 @@ __global__ void __launch_bounds__(MC_THREADS, 1) mc_kernel(const McArgs a) {
     __shared__ ModelSm ms;
     __shared__ double seas[MC_TILE], tt[MC_TILE];
     __shared__ double red_t[MC_THREADS / 32];
+    __shared__ uint64_t key_sm;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int H = a.p.horizon;
     for (int model = blockIdx.x; model < a.p.n_models; model += gridDim.x) {
@@ -212,13 +250,17 @@ __global__ void __launch_bounds__(MC_THREADS, 1) mc_kernel(const McArgs a) {
 #pragma unroll
         for (int o = 16; o >= 1; o >>= 1) tm = fmax(tm, __shfl_xor_sync(0xffffffffu, tm, o));
         if (lane == 0) red_t[warp] = tm;
+        if (warp == 0) {
+            const uint64_t key = model_key(a, model, lane);
+            if (lane == 0) key_sm = key;
+        }
         __syncthreads();
         tm = red_t[0];
         for (int w = 1; w < MC_THREADS / 32; ++w) tm = fmax(tm, red_t[w]);
         const double rate = (double)ms.S;
         Philox ph;
-        ph.k0 = (uint32_t)a.seed ^ (uint32_t)model * 0x9E3779B1u;
-        ph.k1 = (uint32_t)(a.seed >> 32) ^ 0x85EBCA6Bu ^ (uint32_t)((uint64_t)model >> 7);
+        ph.k0 = (uint32_t)key_sm;
+        ph.k1 = (uint32_t)(key_sm >> 32);
         DrawState d[2];
         bool live[2];
 #pragma unroll
@@ -307,10 +349,10 @@ __global__ void __launch_bounds__(MC_THREADS, 1) mc_kernel(const McArgs a) {
     }
 }
 
-// returns 0 ok, -1 unsupported sample count, 1 CUDA error
+// returns 0 ok, -1 sample count or interval width out of range, 1 CUDA error
 inline int launch_mc(cudaStream_t st, int sms, const PredictArgs& p, int n_samples, double width, uint64_t seed,
                      double* lower, double* upper) {
-    if (n_samples < 2 || n_samples > MC_NP) return -1;
+    if (n_samples < 2 || n_samples > MC_NP || !(width >= 0.0 && width <= 1.0)) return -1;
     McArgs a;
     a.p = p;
     a.n_samples = n_samples;

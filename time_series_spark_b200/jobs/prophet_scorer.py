@@ -100,6 +100,10 @@ class _ForecastTimeSeriesOp:
             raise ValueError("forecast_time_series groups by ('series_id', 'dim_id')")
         fc = self.config["forecast"]
         want_intervals = bool(fc.get("intervals", False))
+        if want_intervals:
+            width = float(fc.get("interval_width", 0.8))
+            if not 0.0 <= width <= 1.0:     # fbprophet refuses it too (numpy's percentile range check); NaN fails here
+                raise ValueError(f"forecast.interval_width must be in [0, 1] (got {fc.get('interval_width')!r})")
         rank, ws, _ = pdist.world()
         if ws > 1 and table.num_rows:      # shard the model rows across ranks (equal horizon => equal work)
             lo, hi = pdist.shard_bounds(np.arange(table.num_rows + 1, dtype=np.int64), ws)[rank]
