@@ -273,6 +273,60 @@ PB200_API int pb200_forecast_csv_rows_device(pb200_ctx* ctx, const int32_t* d_se
 PB200_API int32_t pb200_forecast_csv_row_host(int32_t series_id, int32_t dim_id, int64_t ds_ns, int32_t quantity,
                                               const char* created, int32_t created_len, char* out);
 
+/*
+ * Backtest (fbprophet.diagnostics.cross_validation / performance_metrics) of a batch of series; DESIGN §9.
+ *
+ * Cutoff plan, two passes over the series (d_ds sorted ascending per series, rows [d_offsets[i], d_offsets[i+1])):
+ *   pb200_cv_plan_counts_device  d_n_cutoffs[i] = cutoffs of generate_cutoffs(horizon, period, initial) (0 on error),
+ *                                d_mask[i] = the full history's seasonality mask (1 yearly | 2 weekly | 4 daily, the rule
+ *                                of the fit's set_auto_seasonalities under opts->yearly / weekly / daily), d_err[i] =
+ *                                PB200_CV_ERR_* bits.
+ *   pb200_cv_plan_device         given d_pair_off = exclusive scan of d_n_cutoffs ([n_series + 1]), writes per
+ *                                (series, cutoff) pair, cutoffs ascending within a series: d_pair_series, d_cutoff (ns),
+ *                                d_hist_end (first row > cutoff: the history is [offsets[i], hist_end)), d_win_end (first
+ *                                row > cutoff + horizon: the held-out window is [hist_end, win_end)); ORs
+ *                                PB200_CV_ERR_FEW into d_err.
+ * horizon / period / initial: int64 ns, > 0.
+ */
+#define PB200_CV_ERR_HORIZON 1   /* "Less data than horizon" */
+#define PB200_CV_ERR_INITIAL 2   /* "Less data than horizon after initial window" */
+#define PB200_CV_ERR_FEW     4   /* "Less than two datapoints before cutoff" at some cutoff */
+PB200_API int pb200_cv_plan_counts_device(pb200_ctx* ctx, const pb200_options* opts, const int64_t* d_ds,
+                                          const int64_t* d_offsets, int64_t n_series, int64_t horizon_ns, int64_t period_ns,
+                                          int64_t initial_ns, int32_t* d_n_cutoffs, int32_t* d_mask, int32_t* d_err);
+PB200_API int pb200_cv_plan_device(pb200_ctx* ctx, const pb200_options* opts, const int64_t* d_ds, const int64_t* d_offsets,
+                                   int64_t n_series, int64_t horizon_ns, int64_t period_ns, int64_t initial_ns,
+                                   const int64_t* d_pair_off, int32_t* d_err, int32_t* d_pair_series, int64_t* d_cutoff,
+                                   int64_t* d_hist_end, int64_t* d_win_end);
+
+/*
+ * Truncated-history fit batch of n plan pairs d_pairs[k]: entry k's history rows (ds, and y in its element type y_dtype)
+ * go to [d_fit_off[k], d_fit_off[k+1]) of d_ds_out / d_y_out (d_fit_off = exclusive scan of hist_end - offsets[series]),
+ * its held-out timestamps to row k of d_future_ds [n * hmax], a window shorter than hmax padded by repeating its last
+ * timestamp (so that pb200_predict_device runs on the frame as it is; hmax >= every window's length).
+ */
+PB200_API int pb200_cv_gather_device(pb200_ctx* ctx, const int64_t* d_ds, const void* d_y, int32_t y_dtype,
+                                     const int64_t* d_offsets, const int32_t* d_pair_series, const int64_t* d_hist_end,
+                                     const int64_t* d_win_end, const int64_t* d_pairs, int64_t n, const int64_t* d_fit_off,
+                                     int32_t hmax, int64_t* d_ds_out, void* d_y_out, int64_t* d_future_ds);
+
+/*
+ * performance_metrics per series over held-out rows: d_horizon (ns, ds - cutoff), d_y, d_yhat and optionally
+ * d_yhat_lower / d_yhat_upper (both or neither) of n_rows rows; d_order lists the rows sorted by (series, horizon) and
+ * series i owns d_order[d_srow_off[i] .. d_srow_off[i+1]).  With w = min(n_i, max(1, (int)(rolling_window * n_i))) the
+ * metrics of a distinct horizon h are means over w rows: every row of h, then rows of smaller horizons nearest first, the
+ * group where the window stops contributing its mean times the rows still needed (rolling_mean_by_h).  Outputs per slot
+ * q = d_srow_off[i] + g for the g-th distinct horizon of series i (slots past the last horizon and horizons with fewer
+ * than w rows at or below them get d_valid[q] = 0): d_out_horizon, d_mse, d_rmse, d_mae, d_mape (NaN for every horizon
+ * of a series with some |y| < 1e-8), d_coverage (NaN without intervals).  d_scratch: int64 [rows].  Sums run in the
+ * rows' listed order, one thread per series: bit-reproducible and independent of the other series.
+ */
+PB200_API int pb200_cv_metrics_device(pb200_ctx* ctx, const int64_t* d_horizon, const double* d_y, const double* d_yhat,
+                                      const double* d_yhat_lower, const double* d_yhat_upper, const int64_t* d_order,
+                                      const int64_t* d_srow_off, int64_t n_series, double rolling_window,
+                                      int64_t* d_out_horizon, int64_t* d_scratch, double* d_mse, double* d_rmse,
+                                      double* d_mae, double* d_mape, double* d_coverage, int32_t* d_valid);
+
 #ifdef __cplusplus
 }
 #endif

@@ -49,7 +49,9 @@ EXPORTS = [
     "pb200_stream", "pb200_launch_count", "pb200_last_fit_variant_counts", "pb200_tab_chunk", "pb200_fit_device", "pb200_fit_host", "pb200_predict_device",
     "pb200_predict_host", "pb200_make_future_device", "pb200_synchronize", "pb200_objective_host",
     "pb200_fit_trace_host", "pb200_forecast_csv_lengths_device", "pb200_forecast_csv_rows_device", "pb200_forecast_csv_row_host",
+    "pb200_cv_plan_counts_device", "pb200_cv_plan_device", "pb200_cv_gather_device", "pb200_cv_metrics_device",
 ]
+CV_ERR_HORIZON, CV_ERR_INITIAL, CV_ERR_FEW = 1, 2, 4
 
 _lib = None
 
@@ -106,6 +108,14 @@ def load() -> C.CDLL:
     lib.pb200_forecast_csv_rows_device.restype = C.c_int
     lib.pb200_forecast_csv_row_host.argtypes = [i32, i32, i64, i32, C.c_char_p, i32, C.c_char_p]
     lib.pb200_forecast_csv_row_host.restype = i32
+    lib.pb200_cv_plan_counts_device.argtypes = [vp, OP, vp, vp, i64, i64, i64, i64, vp, vp, vp]
+    lib.pb200_cv_plan_counts_device.restype = C.c_int
+    lib.pb200_cv_plan_device.argtypes = [vp, OP, vp, vp, i64, i64, i64, i64, vp, vp, vp, vp, vp, vp]
+    lib.pb200_cv_plan_device.restype = C.c_int
+    lib.pb200_cv_gather_device.argtypes = [vp, vp, vp, i32, vp, vp, vp, vp, vp, i64, vp, i32, vp, vp, vp]
+    lib.pb200_cv_gather_device.restype = C.c_int
+    lib.pb200_cv_metrics_device.argtypes = [vp, vp, vp, vp, vp, vp, vp, vp, i64, dbl, vp, vp, vp, vp, vp, vp, vp, vp]
+    lib.pb200_cv_metrics_device.restype = C.c_int
     lib.pb200_synchronize.argtypes = [vp]
     lib.pb200_synchronize.restype = C.c_int
     _lib = lib

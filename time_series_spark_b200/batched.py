@@ -323,3 +323,307 @@ def objective_host(ctx: L.Context, opts: L.Options, ds_ns: np.ndarray, y: np.nda
                                        _np_ptr(f), _np_ptr(g), _np_ptr(mi32))
     L.check(rc, "pb200_objective_host")
     return f, g, mi32
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# Backtest: fbprophet.diagnostics.cross_validation / performance_metrics for every series of a batch (DESIGN §9)
+# ---------------------------------------------------------------------------------------------------------------------
+# Rows (history prefixes plus held-out windows) gathered per chunk.  50k series x 22 cutoffs of ~840 history rows are
+# ~1e9 rows (~11 GB with int32 y); chunks of whole series keep the gathered batch and the fit outputs bounded.
+CV_ROW_BUDGET = 1 << 27
+
+
+@dataclass
+class CvPlan:
+    """Per series (host numpy): cutoff count, full-history seasonality mask, error bits (L.CV_ERR_*), and the
+    exclusive scan of the counts; per (series, cutoff) pair (CUDA tensors, cutoffs ascending within a series): series
+    index, cutoff ns, first row > cutoff (``hist_end``) and first row > cutoff + horizon (``win_end``), absolute rows."""
+    n_cutoffs: np.ndarray
+    mask: np.ndarray
+    err: np.ndarray
+    pair_off: np.ndarray
+    pair_series: object
+    cutoff: object
+    hist_end: object
+    win_end: object
+
+    @property
+    def n_pairs(self) -> int:
+        return int(self.pair_off[-1])
+
+
+def cv_plan_device(ctx: L.Context, opts: L.Options, ds_ns, offsets_host: np.ndarray, horizon_ns: int, period_ns: int,
+                   initial_ns: int) -> CvPlan:
+    """pb200_cv_plan_counts_device, the scan, pb200_cv_plan_device: generate_cutoffs for every series of a packed batch
+    (``ds_ns`` a CUDA int64 tensor sorted within each series)."""
+    import torch
+    offsets_host = np.ascontiguousarray(offsets_host, dtype=np.int64)
+    n = offsets_host.size - 1
+    dev = ds_ns.device
+    lib = L.load()
+    d_off = torch.from_numpy(offsets_host).to(dev)
+    n_cut = torch.zeros(n, dtype=torch.int32, device=dev)
+    mask = torch.zeros(n, dtype=torch.int32, device=dev)
+    err = torch.zeros(n, dtype=torch.int32, device=dev)
+    torch.cuda.current_stream(dev).synchronize()
+    L.check(lib.pb200_cv_plan_counts_device(ctx.handle, C.byref(opts), ds_ns.data_ptr(), d_off.data_ptr(), n, int(horizon_ns),
+                                            int(period_ns), int(initial_ns), n_cut.data_ptr(), mask.data_ptr(), err.data_ptr()),
+            "pb200_cv_plan_counts_device")
+    ctx.synchronize()
+    counts = n_cut.cpu().numpy()
+    pair_off = np.zeros(n + 1, np.int64)
+    np.cumsum(counts, out=pair_off[1:])
+    p = int(pair_off[-1])
+    ps = torch.empty(p, dtype=torch.int32, device=dev)
+    cut, he, we = (torch.empty(p, dtype=torch.int64, device=dev) for _ in range(3))
+    d_poff = torch.from_numpy(pair_off).to(dev)
+    torch.cuda.current_stream(dev).synchronize()
+    L.check(lib.pb200_cv_plan_device(ctx.handle, C.byref(opts), ds_ns.data_ptr(), d_off.data_ptr(), n, int(horizon_ns),
+                                     int(period_ns), int(initial_ns), d_poff.data_ptr(), err.data_ptr(), ps.data_ptr(),
+                                     cut.data_ptr(), he.data_ptr(), we.data_ptr()), "pb200_cv_plan_device")
+    ctx.synchronize()
+    return CvPlan(counts, mask.cpu().numpy(), err.cpu().numpy(), pair_off, ps, cut, he, we)
+
+
+def cv_plan_errors(plan: CvPlan):
+    """(message, per-series bool mask) of the first kind of plan error present, or None: fbprophet's exceptions."""
+    for bit, msg in ((L.CV_ERR_HORIZON, "Less data than horizon."),
+                     (L.CV_ERR_INITIAL, "Less data than horizon after initial window. Make horizon or initial shorter."),
+                     (L.CV_ERR_FEW, "Less than two datapoints before cutoff. Increase initial window.")):
+        bad = (plan.err & bit) != 0
+        if bad.any():
+            return msg, bad
+    return None
+
+
+def _with_mask(opts: L.Options, mask: int) -> L.Options:
+    """The options of a cutoff fit: the full model's, seasonalities forced to the full history's auto mask."""
+    o = L.Options.from_buffer_copy(opts)
+    o.yearly, o.weekly, o.daily = int(mask & 1 != 0), int(mask & 2 != 0), int(mask & 4 != 0)
+    return o
+
+
+@dataclass
+class CvResult:
+    """Output of cross_validation_device (host numpy).
+
+    Pairs, in plan order (series ascending, cutoffs ascending): ``pair_series``, ``pair_cutoff``, ``pair_status`` (the
+    cutoff fit's solver status; < 0: failed), ``pair_mask`` (the seasonality mask it was fitted with).
+    Held-out rows, ordered by (series, cutoff, ds): ``row_series``, ``ds``, ``cutoff``, ``y`` (float64 of the input
+    value), ``yhat`` and, with intervals, ``yhat_lower`` / ``yhat_upper``.
+    Metrics rows (when requested), ordered by (series, horizon): ``m_series``, ``horizon`` (ns), ``mse``, ``rmse``,
+    ``mae``, ``mape``, ``coverage`` (None without intervals).
+    ``fitted``: with ``keep_fits``, the cutoff fits in plan order, each record in the layout of ``opts`` (beta packed
+    by its mask, zero beyond)."""
+    pair_series: np.ndarray
+    pair_cutoff: np.ndarray
+    pair_status: np.ndarray
+    pair_mask: np.ndarray
+    row_series: np.ndarray
+    ds: np.ndarray
+    cutoff: np.ndarray
+    y: np.ndarray
+    yhat: np.ndarray
+    yhat_lower: Optional[np.ndarray]
+    yhat_upper: Optional[np.ndarray]
+    metrics: Optional[dict] = None
+    fitted: Optional[FittedBatch] = None
+
+
+def _cv_chunks(plan: CvPlan, offsets_host: np.ndarray, budget: int):
+    """Series ranges [s0, s1) whose gathered rows (history prefixes + held-out windows) stay within ``budget``; a
+    series is never split (its metrics need all of its rows)."""
+    he = plan.hist_end.cpu().numpy()
+    we = plan.win_end.cpu().numpy()
+    ps = np.repeat(np.arange(plan.n_cutoffs.size), plan.n_cutoffs)
+    per_pair = (he - offsets_host[:-1][ps]) + (we - he)
+    per_series = np.zeros(plan.n_cutoffs.size, np.int64)
+    np.add.at(per_series, ps, per_pair)
+    out, s0, acc = [], 0, 0
+    for s in range(per_series.size):
+        if acc and acc + per_series[s] > budget:
+            out.append((s0, s))
+            s0, acc = s, 0
+        acc += int(per_series[s])
+    if s0 < per_series.size:
+        out.append((s0, per_series.size))
+    return out, he, we
+
+
+def cross_validation_device(ctx: L.Context, opts: L.Options, ds_ns, y, offsets_host: np.ndarray, floor: float, cap,
+                            horizon_ns: int, period_ns: int, initial_ns: int, intervals: bool = False, seed: int = 0,
+                            rolling_window: Optional[float] = None, plan: Optional[CvPlan] = None,
+                            keep_fits: bool = False, timings: Optional[dict] = None,
+                            _row_budget: Optional[int] = None) -> CvResult:
+    """fbprophet.diagnostics.cross_validation (and, with ``rolling_window``, performance_metrics) for every series of a
+    packed batch: ``ds_ns`` / ``y`` CUDA tensors sorted within each series, ``cap`` the float64 CUDA tensor of each
+    series' full-history cap.  Per chunk of series: one gather, one pb200_fit_device per full-history seasonality mask
+    class, one predict, and the metrics kernel.  Plan errors raise ValueError (see ``cv_plan_errors``).  ``timings``
+    (a dict) accumulates seconds per stage -- plan, gather, fit, predict, metrics, each ending in a synchronisation."""
+    import time
+    import torch
+    tm = timings if timings is not None else {}
+    clock = [time.perf_counter()]
+
+    def lap(stage):
+        t = time.perf_counter()
+        tm[stage] = tm.get(stage, 0.0) + t - clock[0]
+        clock[0] = t
+    offsets_host = np.ascontiguousarray(offsets_host, dtype=np.int64)
+    dev = ds_ns.device
+    if plan is None:
+        plan = cv_plan_device(ctx, opts, ds_ns, offsets_host, horizon_ns, period_ns, initial_ns)
+        lap("plan")
+    bad = cv_plan_errors(plan)
+    if bad is not None:
+        raise ValueError(f"{bad[0]} (first offender: series {int(np.flatnonzero(bad[1])[0])}; "
+                         f"{int(bad[1].sum())} series in all)")
+    lib = L.load()
+    lay = L.get_layout(opts)
+    ydt = _y_dtype(y)
+    d_off = torch.from_numpy(offsets_host).to(dev)
+    chunks, he_h, we_h = _cv_chunks(plan, offsets_host, int(_row_budget or CV_ROW_BUDGET))
+    cap = cap.to(device=dev, dtype=torch.float64)
+    pieces = []
+    clock[0] = time.perf_counter()
+    for s0, s1 in chunks:
+        p0, p1 = int(plan.pair_off[s0]), int(plan.pair_off[s1])
+        if p1 == p0:
+            continue
+        ps_h = np.repeat(np.arange(s0, s1), plan.n_cutoffs[s0:s1])
+        pmask = plan.mask[ps_h]
+        # gathered order: pairs grouped by mask class (stable), so that every class is one contiguous fit batch
+        perm = np.argsort(pmask, kind="stable")
+        pairs_h = (p0 + perm).astype(np.int64)
+        hist_len = he_h[pairs_h] - offsets_host[ps_h[perm]]
+        win_len = we_h[pairs_h] - he_h[pairs_h]
+        fit_off = np.zeros(pairs_h.size + 1, np.int64)
+        np.cumsum(hist_len, out=fit_off[1:])
+        hmax = int(win_len.max())
+        n = pairs_h.size
+        d_pairs = torch.from_numpy(pairs_h).to(dev)
+        d_fit_off = torch.from_numpy(fit_off).to(dev)
+        ds_g = torch.empty(int(fit_off[-1]), dtype=torch.int64, device=dev)
+        y_g = torch.empty(int(fit_off[-1]), dtype=y.dtype, device=dev)
+        fut = torch.empty((n, hmax), dtype=torch.int64, device=dev)
+        torch.cuda.current_stream(dev).synchronize()
+        L.check(lib.pb200_cv_gather_device(ctx.handle, ds_ns.data_ptr(), y.data_ptr(), ydt, d_off.data_ptr(),
+                                           plan.pair_series.data_ptr(), plan.hist_end.data_ptr(), plan.win_end.data_ptr(),
+                                           d_pairs.data_ptr(), n, d_fit_off.data_ptr(), hmax, ds_g.data_ptr(),
+                                           y_g.data_ptr(), fut.data_ptr()), "pb200_cv_gather_device")
+        ctx.synchronize()
+        lap("gather")
+        # fits, one call per mask class; records re-laid into the layout of ``opts`` for the one predict call
+        sp = pmask[perm]
+        fitted = FittedBatch(torch.zeros((n, lay.pstride), dtype=torch.float64, device=dev),
+                             torch.zeros((n, lay.smax), dtype=torch.float64, device=dev),
+                             torch.empty((n, 8), dtype=torch.int32, device=dev),
+                             torch.empty((n, 2), dtype=torch.int64, device=dev),
+                             torch.empty((n, 4), dtype=torch.float64, device=dev), lay.smax, lay.kmax)
+        cap_p = cap[torch.from_numpy(ps_h[perm]).to(dev)].contiguous()
+        bounds = np.flatnonzero(np.diff(np.concatenate(([-1], sp, [-1])))).tolist()
+        for a, b in zip(bounds[:-1], bounds[1:]):
+            oc = _with_mask(opts, int(sp[a]))
+            r0, r1 = int(fit_off[a]), int(fit_off[b])
+            fc = fit_batch_device(ctx, oc, ds_g[r0:r1], y_g[r0:r1], fit_off[a:b + 1] - r0, float(floor), 1.0,
+                                  cap=cap_p[a:b])
+            w = fc.params.shape[1]
+            fitted.params[a:b, :w] = fc.params
+            fitted.tchange[a:b] = fc.tchange
+            fitted.meta_i32[a:b] = fc.meta_i32
+            fitted.meta_i64[a:b] = fc.meta_i64
+            fitted.meta_f64[a:b] = fc.meta_f64
+        torch.cuda.current_stream(dev).synchronize()
+        lap("fit")
+        floor_p = torch.full((n,), float(floor), dtype=torch.float64, device=dev)
+        fcst = predict_batch_device(ctx, opts, fitted, fut, floor_p, cap_p, seed=seed, intervals=intervals)
+        lap("predict")
+        # back to plan order, then the held-out rows
+        inv = torch.from_numpy(np.argsort(perm, kind="stable")).to(dev)
+        yhat = fcst.yhat[inv]
+        lo = fcst.yhat_lower[inv] if fcst.yhat_lower is not None else None
+        hi = fcst.yhat_upper[inv] if fcst.yhat_upper is not None else None
+        futp = fut[inv]
+        wl = torch.from_numpy(we_h[p0:p1] - he_h[p0:p1]).to(dev)
+        valid = torch.arange(hmax, device=dev)[None, :] < wl[:, None]
+        kk, jj = torch.nonzero(valid, as_tuple=True)
+        src_row = plan.hist_end[p0:p1][kk] + jj
+        rows = {"series": plan.pair_series[p0:p1][kk].to(torch.int64), "ds": futp[kk, jj],
+                "cutoff": plan.cutoff[p0:p1][kk], "y": y[src_row].to(torch.float64), "yhat": yhat[kk, jj],
+                "yhat_lower": lo[kk, jj] if lo is not None else None, "yhat_upper": hi[kk, jj] if hi is not None else None}
+        met = None
+        if rolling_window is not None:
+            met = performance_metrics_device(ctx, rows["series"] - s0, rows["ds"] - rows["cutoff"], rows["y"], rows["yhat"],
+                                             rows["yhat_lower"], rows["yhat_upper"], s1 - s0, rolling_window)
+            met["series"] = met["series"] + s0
+            lap("metrics")
+        fh = None
+        if keep_fits:
+            fh = FittedBatch(*(x[inv].cpu().numpy() for x in (fitted.params, fitted.tchange, fitted.meta_i32,
+                                                               fitted.meta_i64, fitted.meta_f64)), lay.smax, lay.kmax)
+        pieces.append(({k: (v.cpu().numpy() if v is not None else None) for k, v in rows.items()}, met,
+                       fitted.meta_i32[inv, 4].cpu().numpy(), fh))
+        lap("rows")
+    cat = lambda xs: np.concatenate(xs) if xs else None                       # noqa: E731
+    rows = {k: cat([p[0][k] for p in pieces]) if (pieces and pieces[0][0][k] is not None) else None
+            for k in ("series", "ds", "cutoff", "y", "yhat", "yhat_lower", "yhat_upper")}
+    if not pieces:
+        rows.update({k: np.zeros(0, np.int64) for k in ("series", "ds", "cutoff")})
+        rows.update({k: np.zeros(0) for k in ("y", "yhat")})
+    metrics = None
+    if rolling_window is not None:
+        keys = ("series", "horizon", "mse", "rmse", "mae", "mape", "coverage")
+        metrics = {k: (cat([p[1][k] for p in pieces]) if pieces and pieces[0][1][k] is not None else None) for k in keys}
+        if not pieces:
+            metrics = performance_metrics_device(ctx, *(torch.zeros(0, dtype=t, device=dev) for t in
+                                                        (torch.int64, torch.int64, torch.float64, torch.float64)),
+                                                 None, None, 0, rolling_window)
+    fitted_all = None
+    if keep_fits and pieces:
+        fitted_all = FittedBatch(*(np.concatenate([getattr(p[3], f) for p in pieces])
+                                   for f in ("params", "tchange", "meta_i32", "meta_i64", "meta_f64")), lay.smax, lay.kmax)
+    ps_all = np.repeat(np.arange(plan.n_cutoffs.size), plan.n_cutoffs)
+    status = cat([p[2] for p in pieces]) if pieces else np.zeros(0, np.int32)
+    return CvResult(ps_all, plan.cutoff.cpu().numpy(), status, plan.mask[ps_all], rows["series"], rows["ds"], rows["cutoff"],
+                    rows["y"], rows["yhat"], rows["yhat_lower"], rows["yhat_upper"], metrics, fitted_all)
+
+
+def performance_metrics_device(ctx: L.Context, series, horizon_ns, y, yhat, yhat_lower, yhat_upper, n_series: int,
+                               rolling_window: float = 0.1) -> dict:
+    """fbprophet.diagnostics.performance_metrics per series (pb200_cv_metrics_device) over held-out rows given as CUDA
+    tensors: ``series`` int64 in [0, n_series), ``horizon_ns`` int64 (ds - cutoff), ``y`` / ``yhat`` (and optionally
+    ``yhat_lower`` / ``yhat_upper``) float64.  Rows of one series are summed in their given order within a horizon.
+    Returns host numpy columns series, horizon, mse, rmse, mae, mape, coverage (None without intervals), ordered by
+    (series, horizon)."""
+    import torch
+    if not (0.0 <= float(rolling_window) <= 1.0):
+        raise ValueError(f"rolling_window must be in [0, 1] (got {rolling_window!r})")
+    dev = y.device
+    R = int(y.shape[0])
+    # rows sorted by (series, horizon), stable: two stable sorts (plumbing)
+    o1 = torch.sort(horizon_ns, stable=True).indices
+    o2 = torch.sort(series[o1], stable=True).indices
+    order = o1[o2].contiguous()
+    counts = torch.bincount(series, minlength=n_series) if R else torch.zeros(n_series, dtype=torch.int64, device=dev)
+    srow_off = torch.zeros(n_series + 1, dtype=torch.int64, device=dev)
+    srow_off[1:] = torch.cumsum(counts, 0)
+    out_h, scratch = (torch.empty(R, dtype=torch.int64, device=dev) for _ in range(2))
+    mse, rmse, mae, mape, cov = (torch.empty(R, dtype=torch.float64, device=dev) for _ in range(5))
+    valid = torch.zeros(R, dtype=torch.int32, device=dev)
+    has_iv = yhat_lower is not None
+    if R and n_series:
+        h, yy, yh = horizon_ns.contiguous(), y.contiguous(), yhat.contiguous()
+        lo = yhat_lower.contiguous() if has_iv else None
+        hi = yhat_upper.contiguous() if has_iv else None
+        torch.cuda.current_stream(dev).synchronize()
+        L.check(L.load().pb200_cv_metrics_device(
+            ctx.handle, h.data_ptr(), yy.data_ptr(), yh.data_ptr(), lo.data_ptr() if has_iv else None,
+            hi.data_ptr() if has_iv else None, order.data_ptr(), srow_off.data_ptr(), int(n_series), float(rolling_window),
+            out_h.data_ptr(), scratch.data_ptr(), mse.data_ptr(), rmse.data_ptr(), mae.data_ptr(), mape.data_ptr(),
+            cov.data_ptr(), valid.data_ptr()), "pb200_cv_metrics_device")
+        ctx.synchronize()
+    keep = valid.bool()
+    slot_series = torch.repeat_interleave(torch.arange(n_series, device=dev), counts) if R else torch.zeros(0, dtype=torch.int64, device=dev)
+    out = {"series": slot_series[keep], "horizon": out_h[keep], "mse": mse[keep], "rmse": rmse[keep], "mae": mae[keep],
+           "mape": mape[keep], "coverage": cov[keep] if has_iv else None}
+    return {k: (v.cpu().numpy() if v is not None else None) for k, v in out.items()}

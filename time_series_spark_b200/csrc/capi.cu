@@ -7,6 +7,7 @@
 #include "mc_kernel.cuh"
 #include "newton_kernel.cuh"
 #include "csv_kernel.cuh"
+#include "cv_kernel.cuh"
 
 #include <algorithm>
 #include <cstdio>
@@ -1023,6 +1024,145 @@ PB200_API int32_t pb200_forecast_csv_row_host(int32_t series_id, int32_t dim_id,
     char* e = pb200::csv::put_row(out, series_id, dim_id, ds_ns, quantity, created, created_len);
     const int n = (int)(e - out);
     return n == pb200::csv::row_len(series_id, dim_id, quantity, created_len) ? n : -1;
+}
+
+// ---- backtest: cutoff plan, truncated-history gather, performance metrics (cv_kernel.cuh) ----
+static int cv_plan_args(pb200::cv::PlanArgs& a, const pb200_options* opts, const int64_t* d_ds, const int64_t* d_offsets,
+                        int64_t n_series, int64_t horizon_ns, int64_t period_ns, int64_t initial_ns) {
+    int rc = check_opts(opts);
+    if (rc) return rc;
+    if (n_series < 0) return fail(PB200_E_ARG, "n_series");
+    if (horizon_ns <= 0 || period_ns <= 0 || initial_ns <= 0) return fail(PB200_E_ARG, "horizon, period and initial must be > 0");
+    if (n_series && (!d_ds || !d_offsets)) return fail(PB200_E_ARG, "null pointer");
+    memset(&a, 0, sizeof a);
+    a.ds = (const long long*)d_ds;
+    a.offsets = (const long long*)d_offsets;
+    a.n_series = n_series;
+    a.horizon = horizon_ns;
+    a.period = period_ns;
+    a.initial = initial_ns;
+    a.yearly = opts->yearly;
+    a.weekly = opts->weekly;
+    a.daily = opts->daily;
+    return PB200_OK;
+}
+
+static int cv_plan_launch(pb200_ctx* c, const pb200::cv::PlanArgs& a) {
+    const int64_t warps = a.n_series;
+    const int grid = (int)std::max<int64_t>(1, std::min<int64_t>((warps + 7) / 8, (int64_t)c->sms * 16));
+    pb200::cv::cv_plan_kernel<<<grid, 256, 0, c->stream>>>(a);
+    CK(cudaGetLastError());
+    c->launches++;
+    return PB200_OK;
+}
+
+PB200_API int pb200_cv_plan_counts_device(pb200_ctx* c, const pb200_options* opts, const int64_t* d_ds, const int64_t* d_offsets,
+                                          int64_t n_series, int64_t horizon_ns, int64_t period_ns, int64_t initial_ns,
+                                          int32_t* d_n_cutoffs, int32_t* d_mask, int32_t* d_err) {
+    if (!c) return fail(PB200_E_ARG, "ctx is null");
+    pb200::cv::PlanArgs a;
+    int rc = cv_plan_args(a, opts, d_ds, d_offsets, n_series, horizon_ns, period_ns, initial_ns);
+    if (rc) return rc;
+    if (n_series == 0) return PB200_OK;
+    if (!d_n_cutoffs || !d_mask || !d_err) return fail(PB200_E_ARG, "null pointer");
+    CK(cudaSetDevice(c->device));
+    a.n_cut = d_n_cutoffs;
+    a.mask = d_mask;
+    a.err = d_err;
+    return cv_plan_launch(c, a);
+}
+
+PB200_API int pb200_cv_plan_device(pb200_ctx* c, const pb200_options* opts, const int64_t* d_ds, const int64_t* d_offsets,
+                                   int64_t n_series, int64_t horizon_ns, int64_t period_ns, int64_t initial_ns,
+                                   const int64_t* d_pair_off, int32_t* d_err, int32_t* d_pair_series, int64_t* d_cutoff,
+                                   int64_t* d_hist_end, int64_t* d_win_end) {
+    if (!c) return fail(PB200_E_ARG, "ctx is null");
+    pb200::cv::PlanArgs a;
+    int rc = cv_plan_args(a, opts, d_ds, d_offsets, n_series, horizon_ns, period_ns, initial_ns);
+    if (rc) return rc;
+    if (n_series == 0) return PB200_OK;
+    if (!d_pair_off || !d_err || !d_pair_series || !d_cutoff || !d_hist_end || !d_win_end) return fail(PB200_E_ARG, "null pointer");
+    CK(cudaSetDevice(c->device));
+    a.pair_off = (const long long*)d_pair_off;
+    a.err = d_err;
+    a.pair_series = d_pair_series;
+    a.cutoff = (long long*)d_cutoff;
+    a.hist_end = (long long*)d_hist_end;
+    a.win_end = (long long*)d_win_end;
+    return cv_plan_launch(c, a);
+}
+
+PB200_API int pb200_cv_gather_device(pb200_ctx* c, const int64_t* d_ds, const void* d_y, int32_t y_dtype,
+                                     const int64_t* d_offsets, const int32_t* d_pair_series, const int64_t* d_hist_end,
+                                     const int64_t* d_win_end, const int64_t* d_pairs, int64_t n, const int64_t* d_fit_off,
+                                     int32_t hmax, int64_t* d_ds_out, void* d_y_out, int64_t* d_future_ds) {
+    if (!c) return fail(PB200_E_ARG, "ctx is null");
+    if (n < 0 || hmax < 1) return fail(PB200_E_ARG, "sizes");
+    if (y_dtype < 0 || y_dtype > 2) return fail(PB200_E_ARG, "y_dtype");
+    if (n == 0) return PB200_OK;
+    if (!d_ds || !d_y || !d_offsets || !d_pair_series || !d_hist_end || !d_win_end || !d_pairs || !d_fit_off || !d_ds_out ||
+        !d_y_out || !d_future_ds)
+        return fail(PB200_E_ARG, "null pointer");
+    CK(cudaSetDevice(c->device));
+    pb200::cv::GatherArgs a;
+    a.ds = (const long long*)d_ds;
+    a.y = d_y;
+    a.y_dtype = y_dtype;
+    a.offsets = (const long long*)d_offsets;
+    a.pair_series = d_pair_series;
+    a.hist_end = (const long long*)d_hist_end;
+    a.win_end = (const long long*)d_win_end;
+    a.pairs = (const long long*)d_pairs;
+    a.n = n;
+    a.fit_off = (const long long*)d_fit_off;
+    a.hmax = hmax;
+    a.ds_out = (long long*)d_ds_out;
+    a.y_out = d_y_out;
+    a.fut = (long long*)d_future_ds;
+    const int grid = (int)std::min<int64_t>(n, (int64_t)c->sms * 32);
+    pb200::cv::cv_gather_kernel<<<grid, 256, 0, c->stream>>>(a);
+    CK(cudaGetLastError());
+    c->launches++;
+    return PB200_OK;
+}
+
+PB200_API int pb200_cv_metrics_device(pb200_ctx* c, const int64_t* d_horizon, const double* d_y, const double* d_yhat,
+                                      const double* d_yhat_lower, const double* d_yhat_upper, const int64_t* d_order,
+                                      const int64_t* d_srow_off, int64_t n_series, double rolling_window, int64_t* d_out_horizon,
+                                      int64_t* d_scratch, double* d_mse, double* d_rmse, double* d_mae, double* d_mape,
+                                      double* d_coverage, int32_t* d_valid) {
+    if (!c) return fail(PB200_E_ARG, "ctx is null");
+    if (n_series < 0) return fail(PB200_E_ARG, "n_series");
+    if (!(rolling_window >= 0.0 && rolling_window <= 1.0)) return fail(PB200_E_ARG, "rolling_window must be in [0, 1]");
+    if (!d_yhat_lower != !d_yhat_upper) return fail(PB200_E_ARG, "yhat_lower and yhat_upper go together");
+    if (n_series == 0) return PB200_OK;
+    if (!d_horizon || !d_y || !d_yhat || !d_order || !d_srow_off || !d_out_horizon || !d_scratch || !d_mse || !d_rmse ||
+        !d_mae || !d_mape || !d_coverage || !d_valid)
+        return fail(PB200_E_ARG, "null pointer");
+    CK(cudaSetDevice(c->device));
+    pb200::cv::MetricsArgs a;
+    a.horizon = (const long long*)d_horizon;
+    a.y = d_y;
+    a.yhat = d_yhat;
+    a.lo = d_yhat_lower;
+    a.hi = d_yhat_upper;
+    a.order = (const long long*)d_order;
+    a.srow_off = (const long long*)d_srow_off;
+    a.n_series = n_series;
+    a.rolling_window = rolling_window;
+    a.out_h = (long long*)d_out_horizon;
+    a.out_n = (long long*)d_scratch;
+    a.out_mse = d_mse;
+    a.out_rmse = d_rmse;
+    a.out_mae = d_mae;
+    a.out_mape = d_mape;
+    a.out_cov = d_coverage;
+    a.out_valid = d_valid;
+    const int grid = (int)std::min<int64_t>((n_series + 127) / 128, (int64_t)c->sms * 16);
+    pb200::cv::cv_metrics_kernel<<<grid, 128, 0, c->stream>>>(a);
+    CK(cudaGetLastError());
+    c->launches++;
+    return PB200_OK;
 }
 
 }  // extern "C"

@@ -1,0 +1,259 @@
+// Backtest (fbprophet.diagnostics cross_validation / performance_metrics) over a whole batch of series.  Three pieces, the
+// fit / predict / MC kernels being reused unchanged in between:
+//   cv_plan_kernel     per series: the cutoffs of generate_cutoffs, each cutoff's history end and held-out window, the
+//                      full history's seasonality mask and the error flags.  Two passes, like csv_kernel.cuh: counts,
+//                      then (given the exclusive scan of the counts) the (series, cutoff) pairs.
+//   cv_gather_kernel   the truncated histories of a list of pairs packed into one ragged fit batch, and the held-out
+//                      timestamps as a [pairs, hmax] frame for predict (short windows padded by their last timestamp).
+//   cv_metrics_kernel  performance_metrics per series: per-horizon trailing-window means of the squared / absolute /
+//                      relative errors and of the interval coverage.
+// Every series is one warp (plan) or one thread (metrics) and every sum runs in one fixed order with no floating-point
+// atomics: a series' plan and metrics do not depend on the other series of the batch.
+#pragma once
+#include <cuda_runtime.h>
+#include <math.h>
+#include <stdint.h>
+
+#include "fit_kernel.cuh"
+
+namespace pb200 {
+namespace cv {
+
+// error flags of a series (cv_plan err[]); the fbprophet exceptions they stand for
+constexpr int ERR_HORIZON = 1;   // "Less data than horizon"
+constexpr int ERR_INITIAL = 2;   // "Less data than horizon after initial window"
+constexpr int ERR_FEW = 4;       // "Less than two datapoints before cutoff" (some cutoff)
+
+// first index in [lo, hi) whose timestamp is > v (hi if none)
+__device__ __forceinline__ long long upper_bound(const long long* ds, long long lo, long long hi, const long long v) {
+    while (lo < hi) {
+        const long long mid = lo + ((hi - lo) >> 1);
+        if (ds[mid] <= v) lo = mid + 1;
+        else hi = mid;
+    }
+    return lo;
+}
+
+// generate_cutoffs over the sorted rows [a, b): returns the number of cutoffs (< 0: an ERR_* flag, negated) and, when
+// out != nullptr, writes them in ascending order to out[0 .. n).  The walk produces them in descending order, so the
+// writing pass is told n (from the counting pass) and fills out from the back.
+__device__ __forceinline__ int cutoff_walk(const long long* ds, const long long a, const long long b, const long long H,
+                                           const long long P, const long long I, long long* out, const int n_known) {
+    const long long first = ds[a], last = ds[b - 1];
+    long long prev = last - H;
+    if (prev < first) return -ERR_HORIZON;
+    int n = 0;
+    while (prev >= first + I) {
+        long long c = prev - P;
+        const long long u = upper_bound(ds, a, b, c);         // first row > c
+        bool stop = false;
+        if (!(u < b && ds[u] <= c + H)) {
+            // no row in (c, c + H]: the next cutoff is (latest row <= c) - H.  With no such row fbprophet's cutoff
+            // becomes NaT, which ends the loop and is the element dropped: prev is kept
+            if (u == a) stop = true;
+            else c = ds[u - 1] - H;
+        }
+        if (out) out[n_known - 1 - n] = prev;
+        ++n;
+        if (stop) return n;
+        prev = c;
+    }
+    return n > 0 ? n : -ERR_INITIAL;                           // prev, the last element, is dropped
+}
+
+struct PlanArgs {
+    const long long* ds;
+    const long long* offsets;    // [n_series + 1]
+    long long n_series;
+    long long horizon, period, initial;
+    int yearly, weekly, daily;   // pb200_options switches
+    // counting pass (pair_off == nullptr)
+    int* n_cut;                  // [n_series] cutoffs (0 on error)
+    int* mask;                   // [n_series] full-history seasonality mask
+    int* err;                    // [n_series] ERR_* bits
+    // writing pass
+    const long long* pair_off;   // [n_series + 1] exclusive scan of n_cut
+    int* pair_series;            // [pairs]
+    long long* cutoff;           // [pairs] ns
+    long long* hist_end;         // [pairs] first row > cutoff
+    long long* win_end;          // [pairs] first row > cutoff + horizon
+};
+
+__global__ void __launch_bounds__(256) cv_plan_kernel(const PlanArgs a) {
+    const int lane = threadIdx.x & 31;
+    const long long gw = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    const long long nw = ((long long)gridDim.x * blockDim.x) >> 5;
+    for (long long s = gw; s < a.n_series; s += nw) {
+        const long long off = a.offsets[s], end = a.offsets[s + 1];
+        if (a.pair_off == nullptr) {
+            // the full history's smallest non-zero step, as prep_kernel measures it
+            long long mindt = INT64_MAX;
+            for (long long i = off + 1 + lane; i < end; i += 32) {
+                const long long dt = a.ds[i] - a.ds[i - 1];
+                if (dt != 0 && dt < mindt) mindt = dt;
+            }
+            mindt = wminll(mindt);
+            if (lane == 0) {
+                int err = 0, n = 0;
+                if (end - off < 1) {
+                    err = ERR_HORIZON;
+                } else {
+                    n = cutoff_walk(a.ds, off, end, a.horizon, a.period, a.initial, nullptr, 0);
+                    if (n < 0) {
+                        err = -n;
+                        n = 0;
+                    }
+                }
+                a.mask[s] = end - off < 1 ? 0 : auto_seasonality_mask(a.ds[end - 1] - a.ds[off], mindt, a.yearly, a.weekly, a.daily);
+                a.n_cut[s] = n;
+                a.err[s] = err;
+            }
+        } else if (lane == 0) {
+            const long long p0 = a.pair_off[s];
+            const int n = (int)(a.pair_off[s + 1] - p0);
+            if (n <= 0) continue;
+            cutoff_walk(a.ds, off, end, a.horizon, a.period, a.initial, a.cutoff + p0, n);
+            int few = 0;
+            for (int j = 0; j < n; ++j) {
+                const long long c = a.cutoff[p0 + j];
+                const long long he = upper_bound(a.ds, off, end, c);
+                a.pair_series[p0 + j] = (int)s;
+                a.hist_end[p0 + j] = he;
+                a.win_end[p0 + j] = upper_bound(a.ds, he, end, c + a.horizon);
+                if (he - off < 2) few = 1;
+            }
+            if (few) a.err[s] |= ERR_FEW;
+        }
+    }
+}
+
+struct GatherArgs {
+    const long long* ds;
+    const void* y;
+    int y_dtype;
+    const long long* offsets;    // [n_series + 1] of ds / y
+    const int* pair_series;      // [pairs] (plan)
+    const long long* hist_end;
+    const long long* win_end;
+    const long long* pairs;      // [n] the pair of each entry of the gathered batch
+    long long n;
+    const long long* fit_off;    // [n + 1] exclusive scan of the entries' history lengths
+    int hmax;
+    long long* ds_out;           // [fit_off[n]]
+    void* y_out;                 // [fit_off[n]], element type y_dtype
+    long long* fut;              // [n * hmax]
+};
+
+// one CTA per entry: its history prefix, then its held-out timestamps
+__global__ void __launch_bounds__(256) cv_gather_kernel(const GatherArgs a) {
+    for (long long k = blockIdx.x; k < a.n; k += gridDim.x) {
+        const long long p = a.pairs[k];
+        const long long off = a.offsets[a.pair_series[p]], he = a.hist_end[p], we = a.win_end[p];
+        const long long dst = a.fit_off[k], len = he - off;
+        for (long long i = threadIdx.x; i < len; i += blockDim.x) a.ds_out[dst + i] = a.ds[off + i];
+        if (a.y_dtype == PB200_Y_F64) {
+            const double* ys = (const double*)a.y;
+            double* yd = (double*)a.y_out;
+            for (long long i = threadIdx.x; i < len; i += blockDim.x) yd[dst + i] = ys[off + i];
+        } else {   // int32 / float32: moved as 32-bit words
+            const uint32_t* ys = (const uint32_t*)a.y;
+            uint32_t* yd = (uint32_t*)a.y_out;
+            for (long long i = threadIdx.x; i < len; i += blockDim.x) yd[dst + i] = ys[off + i];
+        }
+        for (int j = threadIdx.x; j < a.hmax; j += blockDim.x) {
+            const long long r = he + j < we ? he + j : we - 1;
+            a.fut[k * a.hmax + j] = a.ds[r];
+        }
+    }
+}
+
+struct MetricsArgs {
+    const long long* horizon;    // [n_rows] ns (ds - cutoff)
+    const double* y;             // [n_rows]
+    const double* yhat;
+    const double* lo;            // nullable (no coverage)
+    const double* hi;
+    const long long* order;      // [n_rows] the rows sorted by (series, horizon), stable
+    const long long* srow_off;   // [n_series + 1] into order
+    long long n_series;
+    double rolling_window;
+    // outputs, slot srow_off[s] + g for the g-th distinct horizon of series s
+    long long* out_h;
+    long long* out_n;            // scratch: rows of the horizon
+    double* out_mse;
+    double* out_rmse;
+    double* out_mae;
+    double* out_mape;
+    double* out_cov;
+    int* out_valid;              // 1 where the horizon has a metrics row
+};
+
+__global__ void __launch_bounds__(128) cv_metrics_kernel(const MetricsArgs a) {
+    for (long long s = blockIdx.x * (long long)blockDim.x + threadIdx.x; s < a.n_series; s += (long long)gridDim.x * blockDim.x) {
+        const long long r0 = a.srow_off[s], r1 = a.srow_off[s + 1], n = r1 - r0;
+        if (n <= 0) continue;
+        // group sums per distinct horizon, rows in their sorted order
+        long long G = 0;
+        bool tiny_y = false;
+        for (long long r = r0; r < r1;) {
+            const long long h = a.horizon[a.order[r]];
+            double se = 0.0, ae = 0.0, ape = 0.0, cv = 0.0;
+            long long c = 0;
+            for (; r < r1 && a.horizon[a.order[r]] == h; ++r, ++c) {
+                const long long i = a.order[r];
+                const double yv = a.y[i], e = yv - a.yhat[i], ay = fabs(yv);
+                if (ay < 1e-8) tiny_y = true;
+                se += e * e;
+                ae += fabs(e);
+                ape += fabs(e) / ay;
+                if (a.lo) cv += (a.lo[i] <= yv && yv <= a.hi[i]) ? 1.0 : 0.0;
+            }
+            const long long g = r0 + G++;
+            a.out_h[g] = h;
+            a.out_n[g] = c;
+            a.out_mse[g] = se;
+            a.out_mae[g] = ae;
+            a.out_mape[g] = ape;
+            a.out_cov[g] = cv;
+        }
+        long long w = (long long)(a.rolling_window * (double)n);
+        if (w < 1) w = 1;
+        if (w > n) w = n;
+        // horizon k: the mean over w rows -- all of k's, then smaller horizons nearest first, the group where the
+        // window stops contributing its mean times the rows still needed.  Descending k: slot k is overwritten with
+        // its result only once no larger horizon needs its sums
+        for (long long k = G - 1; k >= 0; --k) {
+            double se = 0.0, ae = 0.0, ape = 0.0, cv = 0.0;
+            long long need = w;
+            for (long long g = k; g >= 0 && need > 0; --g) {
+                const long long q = r0 + g, c = a.out_n[q];
+                if (c >= need) {
+                    const double f = (double)need / (double)c;
+                    se += a.out_mse[q] * f;
+                    ae += a.out_mae[q] * f;
+                    ape += a.out_mape[q] * f;
+                    cv += a.out_cov[q] * f;
+                    need = 0;
+                } else {
+                    se += a.out_mse[q];
+                    ae += a.out_mae[q];
+                    ape += a.out_mape[q];
+                    cv += a.out_cov[q];
+                    need -= c;
+                }
+            }
+            const long long q = r0 + k;
+            a.out_valid[q] = need == 0 ? 1 : 0;
+            const double mse = se / (double)w;
+            a.out_mse[q] = mse;
+            a.out_rmse[q] = sqrt(mse);
+            a.out_mae[q] = ae / (double)w;
+            a.out_mape[q] = tiny_y ? NAN : ape / (double)w;
+            a.out_cov[q] = a.lo ? cv / (double)w : NAN;
+        }
+        for (long long q = r0 + G; q < r1; ++q) a.out_valid[q] = 0;
+    }
+}
+
+}  // namespace cv
+}  // namespace pb200

@@ -1,0 +1,205 @@
+"""Backtest job: fbprophet.diagnostics.cross_validation + performance_metrics for every (series_id, dim_id) group.
+
+Reads the modeler's input (``io.input``, same header-less hive-partitioned CSV) and fits each group at every cutoff of
+its history with the modeler's options (``model.*``), then predicts the held-out rows after each cutoff and reduces
+the errors to metrics by forecast horizon.  All of it on the GPU: the cutoff plan, the gathered truncated histories,
+the fits, the prediction and the metrics (time_series_spark_b200/csrc/cv_kernel.cuh; semantics in DESIGN §9).
+
+Keys (``backtest.*``):
+  horizon            pandas Timedelta string, required ("1 days")
+  period             default horizon / 2
+  initial            default 3 * horizon
+  rolling_window     fraction of a series' held-out rows each metric averages over, in [0, 1]; default 0.1
+  intervals          false (default): no yhat_lower / yhat_upper, no coverage column
+  uncertainty_samples, interval_width, seed   1000, 0.8, 0 (used with intervals only)
+Outputs (parquet, one part file per rank):
+  io.metrics   series_id, dim_id, horizon duration[ns], mse, rmse, mae, mape[, coverage]
+  io.cv_rows   (optional) series_id, dim_id, ds, cutoff, y, yhat[, yhat_lower, yhat_upper]
+"""
+from __future__ import annotations
+
+import logging
+import os
+import time
+
+import numpy as np
+import pyarrow as pa
+import pyarrow.parquet as pq
+
+from .. import _lib as L
+from .. import batched
+from .. import dist as pdist
+from ..pack import pack_groups_cuda
+from .prophet_modeler import ProphetModeler, get_context, options_from_config
+
+
+def _duration_ns(key: str, value) -> int:
+    import pandas as pd
+    try:
+        ns = int(pd.Timedelta(value).value)
+    except (ValueError, TypeError) as e:
+        raise ValueError(f"backtest.{key} must be a duration such as '1 days' (got {value!r})") from e
+    if ns <= 0:
+        raise ValueError(f"backtest.{key} must be positive (got {value!r})")
+    return ns
+
+
+def backtest_spec_from_config(config) -> dict:
+    """The ``backtest`` section checked and converted: durations in int64 ns, the metric window, interval options."""
+    b = dict(config.get("backtest", {}) or {})
+    if "horizon" not in b:
+        raise ValueError("backtest.horizon is required")
+    horizon = _duration_ns("horizon", b["horizon"])
+    period = _duration_ns("period", b["period"]) if b.get("period") is not None else horizon // 2
+    initial = _duration_ns("initial", b["initial"]) if b.get("initial") is not None else 3 * horizon
+    if period <= 0:
+        raise ValueError(f"backtest.period must be positive (horizon / 2 of {b['horizon']!r} is 0)")
+    try:
+        rw = float(b.get("rolling_window", 0.1))
+    except (TypeError, ValueError):
+        rw = float("nan")
+    if not (0.0 <= rw <= 1.0):
+        raise ValueError(f"backtest.rolling_window must be in [0, 1] (got {b.get('rolling_window')!r})")
+    intervals = bool(b.get("intervals", False))
+    spec = {"horizon": horizon, "period": period, "initial": initial, "rolling_window": rw, "intervals": intervals,
+            "uncertainty_samples": 0, "interval_width": 0.8, "seed": int(b.get("seed", 0))}
+    if intervals:
+        width = float(b.get("interval_width", 0.8))
+        if not (0.0 <= width <= 1.0):
+            raise ValueError(f"backtest.interval_width must be in [0, 1] (got {b.get('interval_width')!r})")
+        ns = int(b.get("uncertainty_samples", 1000))
+        if not (2 <= ns <= 1024):
+            raise ValueError(f"backtest.uncertainty_samples must be in [2, 1024] (got {b.get('uncertainty_samples')!r})")
+        spec["interval_width"], spec["uncertainty_samples"] = width, ns
+    return spec
+
+
+def _who(series_id, dim_id, mask) -> str:
+    i = int(np.flatnonzero(mask)[0])
+    return (f" (first offender: series_id {int(series_id[i])}, dim_id {int(dim_id[i])}; "
+            f"{int(np.count_nonzero(mask))} group(s) in all)")
+
+
+def assemble_outputs(series_id, dim_id, res: batched.CvResult, y_dtype, with_rows: bool = True):
+    """Metrics (and row) tables of a CvResult.  A series with a failed cutoff fit (status < 0) -- where fbprophet's
+    cross_validation would raise -- gets no row in either table, and a printed line names it and the cutoff."""
+    n = len(series_id)
+    failed = np.zeros(n, bool)
+    for p in np.flatnonzero(res.pair_status < 0):
+        s = int(res.pair_series[p])
+        if not failed[s]:
+            cut = np.datetime64(int(res.pair_cutoff[p]), "ns")
+            print(f"Runtime error (solver status {int(res.pair_status[p])}) for series_id: {int(series_id[s])}, "
+                  f"dim_id: {int(dim_id[s])}, cutoff: {cut}")
+        failed[s] = True
+    m = res.metrics
+    keep = ~failed[m["series"]]
+    ms = m["series"][keep]
+    cols = {"series_id": pa.array(np.asarray(series_id)[ms], pa.int32()),
+            "dim_id": pa.array(np.asarray(dim_id)[ms], pa.int32()),
+            "horizon": pa.array(m["horizon"][keep], pa.duration("ns"))}
+    for k in ("mse", "rmse", "mae", "mape"):
+        cols[k] = pa.array(m[k][keep], pa.float64())
+    if m["coverage"] is not None:
+        cols["coverage"] = pa.array(m["coverage"][keep], pa.float64())
+    metrics = pa.table(cols)
+    rows = None
+    if with_rows:
+        keep = ~failed[res.row_series]
+        rs = res.row_series[keep]
+        rc = {"series_id": pa.array(np.asarray(series_id)[rs], pa.int32()),
+              "dim_id": pa.array(np.asarray(dim_id)[rs], pa.int32()),
+              "ds": pa.array(res.ds[keep], pa.timestamp("ns")),
+              "cutoff": pa.array(res.cutoff[keep], pa.timestamp("ns")),
+              "y": pa.array(res.y[keep].astype(y_dtype)),
+              "yhat": pa.array(res.yhat[keep], pa.float64())}
+        if res.yhat_lower is not None:
+            rc["yhat_lower"] = pa.array(res.yhat_lower[keep], pa.float64())
+            rc["yhat_upper"] = pa.array(res.yhat_upper[keep], pa.float64())
+        rows = pa.table(rc)
+    return metrics, rows
+
+
+class ProphetBacktester:
+    """Backtest every group of the modeler's input (one batched GPU job; see the module docstring)."""
+
+    def __init__(self, config, logger=None):
+        self.logger = logger or logging.getLogger(self.__class__.__name__)
+        self.config = config
+        self.rank_local_input = False
+
+    def read_input_dataframe(self, spark=None):
+        reader = ProphetModeler(self.config)
+        frame = reader.read_input_dataframe(spark)
+        self.rank_local_input = getattr(reader, "rank_local_input", False)
+        return frame
+
+    def backtest(self, table: pa.Table):
+        """(metrics table, row table or None) of the groups in ``table`` (columns series_id, dim_id, ds, y)."""
+        t0 = time.time()
+        spec = backtest_spec_from_config(self.config)
+        floor = float(self.config["model"]["floor"])
+        cap_multiplier = float(self.config["model"]["cap_multiplier"])
+        opts = options_from_config(self.config)
+        opts.uncertainty_samples = spec["uncertainty_samples"]
+        opts.interval_width = spec["interval_width"]
+        ctx = get_context()
+        import torch
+        torch.cuda.set_device(ctx.device)
+        pk = pack_groups_cuda(table, device=f"cuda:{ctx.device}")
+        rank, ws, _ = pdist.world()
+        if ws > 1 and not self.rank_local_input:
+            lo, hi = pdist.shard_bounds(pk.offsets, ws)[rank]
+            pk = pk.take(lo, hi)
+        with_rows = bool((self.config.get("io", {}) or {}).get("cv_rows"))
+        if pk.n == 0:
+            res = batched.CvResult(*(np.zeros(0, np.int64),) * 4, *(np.zeros(0, np.int64),) * 3, *(np.zeros(0),) * 2,
+                                   None, None, metrics={k: np.zeros(0, np.int64 if k in ("series", "horizon") else np.float64)
+                                                        for k in ("series", "horizon", "mse", "rmse", "mae", "mape")})
+            res.metrics["coverage"] = np.zeros(0) if spec["intervals"] else None
+            if spec["intervals"]:
+                res.yhat_lower, res.yhat_upper = np.zeros(0), np.zeros(0)
+            return assemble_outputs(pk.series_id, pk.dim_id, res, np.dtype(str(pk.y.dtype).replace("torch.", "")), with_rows)
+        ds, y = pk.ds.contiguous(), pk.y.contiguous()
+        short = np.diff(pk.offsets) < 2
+        if np.any(short):
+            raise ValueError("Dataframe has less than 2 non-NaN rows." + _who(pk.series_id, pk.dim_id, short))
+        plan = batched.cv_plan_device(ctx, opts, ds, pk.offsets, spec["horizon"], spec["period"], spec["initial"])
+        bad = batched.cv_plan_errors(plan)
+        if bad is not None:
+            raise ValueError(bad[0] + _who(pk.series_id, pk.dim_id, bad[1]))
+        # the full history's float64 cap, as the modeler computes it: max(y) * cap_multiplier
+        lens = torch.from_numpy(np.diff(pk.offsets)).to(ds.device)
+        cap = torch.segment_reduce(y.to(torch.float64), "max", lengths=lens) * cap_multiplier
+        print(f"Backtesting {pk.n} series at {plan.n_pairs} cutoffs")
+        res = batched.cross_validation_device(ctx, opts, ds, y, pk.offsets, floor, cap, spec["horizon"], spec["period"],
+                                              spec["initial"], intervals=spec["intervals"], seed=spec["seed"],
+                                              rolling_window=spec["rolling_window"], plan=plan)
+        for code, msg in ((L.ST_CAP_LE_FLOOR, "cap must be greater than floor (which defaults to 0)."),
+                          (L.ST_BAD_INPUT, "Found non-finite y or a zero time span in a series.")):
+            hit = np.zeros(pk.n, bool)
+            hit[res.pair_series[res.pair_status == code]] = True
+            if hit.any():
+                raise ValueError(msg + _who(pk.series_id, pk.dim_id, hit))
+        out = assemble_outputs(pk.series_id, pk.dim_id, res, np.dtype(str(y.dtype).replace("torch.", "")), with_rows)
+        print(f"Backtest: {out[0].num_rows} metrics rows in {time.time() - t0:.1f} s")
+        return out
+
+    def persist(self, metrics: pa.Table, rows) -> None:
+        """Parquet part file per rank under io.metrics (and io.cv_rows)."""
+        io = self.config["io"]
+        rank = pdist.world()[0]
+        for key, tbl in (("metrics", metrics), ("cv_rows", rows)):
+            if tbl is None or not io.get(key):
+                continue
+            pdist.prepare_output_dir(io[key])
+            pq.write_table(tbl, os.path.join(io[key], f"part-{rank:05d}.parquet"))
+
+    @staticmethod
+    def run(spark_session, config):
+        pdist.init_process_group()
+        job = ProphetBacktester(config)
+        frame = job.read_input_dataframe(spark_session)
+        metrics, rows = job.backtest(frame.table)
+        job.persist(metrics, rows)
+        return metrics, rows
