@@ -4,8 +4,6 @@ sanity and the scorer epilogue at the sizes the benchmark is quoted on.  What th
 against it: the objective and gradient of all 50k config-#3 series (C oracle), and the first iterations of a sample of
 them.  At this size the grouped kernel runs in production geometry: ~12 series per workspace slot, and about two thirds of
 the slots evict-first in L2."""
-import os
-
 import numpy as np
 import pytest
 
@@ -97,43 +95,6 @@ def test_config4_full_size_ragged(gpu_ctx):
     sub = b.take(lo, hi)
     fs = batched.fit_batch_host(gpu_ctx, opts, sub.ds, sub.y, sub.offsets, 0.0, 1.1)
     assert np.array_equal(fs.params, fb.params[lo:hi]) and np.array_equal(fs.meta_i32[:, 4:7], fb.meta_i32[lo:hi, 4:7])
-
-
-def _check_chunked_equals_single_pass(gpu_ctx, b):
-    opts = batched.make_options()
-    f1 = batched.fit_batch_host(gpu_ctx, opts, b.ds, b.y, b.offsets, 0.0, 1.1)            # one pass
-    v1 = gpu_ctx.last_fit_variant_counts()
-    os.environ["PB200_HOST_CHUNKS"] = "4"
-    try:
-        four = L.Context(0)
-    finally:
-        del os.environ["PB200_HOST_CHUNKS"]
-    try:
-        fb = batched.fit_batch_host(four, opts, b.ds, b.y, b.offsets, 0.0, 1.1)           # 4 chunks
-        v4 = four.last_fit_variant_counts()
-        assert v4.sum() == b.n      # counted over all chunks of the call
-    finally:
-        four.close()
-    assert np.array_equal(v4, v1)
-    assert np.array_equal(fb.params, f1.params) and np.array_equal(fb.meta_i32, f1.meta_i32)
-    assert np.array_equal(fb.meta_f64, f1.meta_f64, equal_nan=True) and np.array_equal(fb.tchange, f1.tchange)
-    assert np.array_equal(fb.meta_i64, f1.meta_i64)
-    return v1
-
-
-def test_chunked_host_fit_equals_single_pass(gpu_ctx):
-    """pb200_fit_host can cut a big batch into series chunks over several streams (PB200_HOST_CHUNKS; copy / compute
-    overlap -- off by default because it measured slower); a series' result must not depend on the chunking.  Config #4:
-    4 chunks of ~10k short series on the one-warp-per-series kernel."""
-    _check_chunked_equals_single_pass(gpu_ctx, synth.config4(n=40_000))
-
-
-def test_chunked_host_fit_equals_single_pass_on_the_grouped_kernel(gpu_ctx):
-    """The same on 20k config-#3 series, 4 chunks of ~5k: they run the grouped day-table kernel at 8 lanes per series
-    (the lane count follows the whole call's size, 20k >= 16384, not a chunk's)."""
-    b = synth.config3(n=20_000)
-    v1 = _check_chunked_equals_single_pass(gpu_ctx, b)
-    assert v1[3, 6] == b.n      # the day-table class: the grouped kernel
 
 
 def test_config3_full_size_objective_matches_c_oracle(gpu_ctx, c3_full):

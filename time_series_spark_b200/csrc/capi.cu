@@ -74,8 +74,12 @@ struct HostBuf {   // pinned
     }
 };
 
-constexpr int NLC = 3;
-const int LC_NT[NLC] = {32, 64, 128};
+constexpr int NLC = 2;
+const int LC_NT[NLC] = {32, 128};
+
+// the work queues' expected-cost key is points x (1 + QKEY_CV_WEIGHT x cv), cv the coefficient of variation of y: a noisier
+// series takes more evaluations (DESIGN §3)
+constexpr double QKEY_CV_WEIGHT = 2.0;
 
 int env_int(const char* name, int dflt) {
     const char* v = getenv(name);
@@ -84,12 +88,12 @@ int env_int(const char* name, int dflt) {
 
 }  // namespace
 
-// Everything one in-flight fit call needs besides its inputs and outputs.  NWS of them: the *_host entry point cuts
-// a big batch into series chunks, one (stream, workspace) pair each, so that the H2D copy of chunk i + 1 overlaps the
-// fit of chunk i and the later chunks' kernels fill the SMs an earlier chunk's stragglers leave idle.  (With two
-// pairs chunk i + 2 had to wait for chunk i's LAST series before it could start.)
-struct FitWs {
-    cudaStream_t stream = nullptr;
+struct pb200_ctx {
+    int device = 0;
+    int sms = 0;
+    cudaStream_t stream = nullptr;  // the stream of every call
+    int64_t launches = 0;
+    // fit workspace
     cudaEvent_t ctl_ev = nullptr;   // recorded after the H2D copies out of h_ctl
     bool ctl_pending = false;
     DevBuf d_offsets, d_order, d_lenclass, d_qitems, d_qctl;   // control workspace (device)
@@ -97,29 +101,17 @@ struct FitWs {
     DevBuf d_nq;                    // [0] count, [1] head, [2..] series whose L-BFGS failed its line search (Newton retry queue)
     DevBuf d_planes;                // fit kernels' per-series workspace (one slice per resident CTA / series slot)
     HostBuf h_ctl;                  // pinned staging for offsets / order / lenclass
-};
-
-constexpr int NWS = 4;
-
-struct pb200_ctx {
-    int device = 0;
-    int sms = 0;
-    FitWs ws[NWS];
-    cudaStream_t stream = nullptr;  // = ws[0].stream: the stream of every single-workspace call
-    cudaEvent_t fork_ev = nullptr;
-    int64_t launches = 0;
     DevBuf d_vcount;                // series of the last fit call per kernel variant x seasonality class
     // data staging for the *_host entry points
     DevBuf d_ds, d_y, d_cap, d_params, d_tchange, d_mi32, d_mi64, d_mf64;
     DevBuf d_fut, d_floor, d_yhat, d_lo, d_hi, d_yint;
     DevBuf d_mc;     // MC workspace
-    int lc_max[NLC];
-    bool lc_auto = true;   // false when PB200_LC*_MAX pins the CTA width
+    int lc0_max = 1 << 30; // PB200_LC0_MAX: longest series on one warp per series, longer ones get four (unset: no limit)
+    bool lc_auto = true;   // false when PB200_LC0_MAX pins the CTA width
     bool tab_on = true;    // PB200_NO_TAB=1 disables the seasonal-table variants (A/B runs)
-    int grp_g = -1;        // lanes per series of the grouped day-table kernel (fit_group.cuh); PB200_GROUP=0|8|16|32 pins it
+    int grp_g = -1;        // lanes per series of the grouped day-table kernel (fit_group.cuh); PB200_GROUP=0|8|16 pins it
                            // (0 = point_pass_tab), unset = by batch size: 8 from grp_min series on, 16 below
     DevBuf d_trace;        // trajectory rows of pb200_fit_trace_host
-    DevBuf d_nq_all, d_offsets_full;   // pb200_fit_host: per-chunk Newton retry queues, the call's offsets on the device
     int plain_grp = 0;     // PB200_PLAIN_GROUP=1: the class WITHOUT seasonality (regular grid; reference config #4) on the grouped kernel
                            // too.  Off: it beat one warp per series only at the largest batches measured (500k short series) --
                            // its rounds are longer, and small batches are latency bound
@@ -131,9 +123,6 @@ struct pb200_ctx {
     size_t l2_bytes = 0;   // the device's L2
     int l2_keep_pct = 65;  // PB200_L2_KEEP_PCT: share of the L2 the grouped kernel's workspace slots may hold at evict_last priority
                            // (< 0: no cache hints -- A/B runs).  40 to 85 measured the same on an H100
-    int host_chunks = 1;   // PB200_HOST_CHUNKS: series chunks of pb200_fit_host.  Default 1 (one pass): more chunks measured slower on 50k x
-                           // 1440 -- the 865 MB copy is short next to the fit, and every chunk pays its own straggler drain,
-                           // which costs more than it hides
     int grid_max = 0;      // PB200_FIT_GRID_MAX (tests): at most this many CTAs per fit launch (grouped and one-series kernels) and per
                            // Newton launch; unset or <= 0: no cap.  The workspace is sized from the capped grid; the kernel variant, G and
                            // the evict_last slot count are chosen as without it.  With a small cap every slot fits many series in turn
@@ -277,30 +266,18 @@ PB200_API pb200_ctx* pb200_create(int device) {
         delete c;
         return nullptr;
     }
-    bool ok = cudaEventCreateWithFlags(&c->fork_ev, cudaEventDisableTiming) == cudaSuccess;
-    for (FitWs& w : c->ws) {
-        ok = ok && cudaStreamCreateWithFlags(&w.stream, cudaStreamNonBlocking) == cudaSuccess;
-        ok = ok && cudaEventCreateWithFlags(&w.ctl_ev, cudaEventDisableTiming) == cudaSuccess;
-    }
-    if (!ok) {
+    if (cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking) != cudaSuccess ||
+        cudaEventCreateWithFlags(&c->ctl_ev, cudaEventDisableTiming) != cudaSuccess) {
         fail(PB200_E_CUDA, "cudaStreamCreate / cudaEventCreate");
-        for (FitWs& w : c->ws) {
-            if (w.ctl_ev) cudaEventDestroy(w.ctl_ev);
-            if (w.stream) cudaStreamDestroy(w.stream);
-        }
-        if (c->fork_ev) cudaEventDestroy(c->fork_ev);
+        if (c->stream) cudaStreamDestroy(c->stream);
         delete c;
         return nullptr;
     }
-    c->stream = c->ws[0].stream;
-    c->host_chunks = std::max(1, std::min(16, env_int("PB200_HOST_CHUNKS", 1)));
-    c->lc_max[0] = env_int("PB200_LC0_MAX", 1 << 30);   // warp-per-series for every length
-    c->lc_max[1] = env_int("PB200_LC1_MAX", 1 << 30);
-    c->lc_max[2] = 1 << 30;
-    c->lc_auto = !(getenv("PB200_LC0_MAX") || getenv("PB200_LC1_MAX"));
+    c->lc0_max = env_int("PB200_LC0_MAX", 1 << 30);
+    c->lc_auto = !getenv("PB200_LC0_MAX");
     c->tab_on = env_int("PB200_NO_TAB", 0) == 0;
     c->grp_g = env_int("PB200_GROUP", -1);
-    if (c->grp_g != -1 && c->grp_g != 8 && c->grp_g != 16 && c->grp_g != 32) c->grp_g = 0;
+    if (c->grp_g != -1 && c->grp_g != 8 && c->grp_g != 16) c->grp_g = 0;
     c->grp_min = env_int("PB200_GROUP_MIN", 16384);
     c->plain_grp = env_int("PB200_PLAIN_GROUP", 0) != 0;
     c->l2_keep_pct = std::min(100, env_int("PB200_L2_KEEP_PCT", 65));
@@ -311,19 +288,14 @@ PB200_API pb200_ctx* pb200_create(int device) {
 PB200_API void pb200_destroy(pb200_ctx* c) {
     if (!c) return;
     cudaSetDevice(c->device);
-    for (FitWs& w : c->ws) cudaStreamSynchronize(w.stream);
+    cudaStreamSynchronize(c->stream);
     for (DevBuf* b : {&c->d_ds, &c->d_y, &c->d_cap, &c->d_params, &c->d_tchange, &c->d_mi32, &c->d_mi64, &c->d_mf64, &c->d_fut,
-                      &c->d_floor, &c->d_yhat, &c->d_lo, &c->d_hi, &c->d_yint, &c->d_mc, &c->d_trace, &c->d_vcount, &c->d_nq_all,
-                      &c->d_offsets_full})
+                      &c->d_floor, &c->d_yhat, &c->d_lo, &c->d_hi, &c->d_yint, &c->d_mc, &c->d_trace, &c->d_vcount, &c->d_offsets,
+                      &c->d_order, &c->d_lenclass, &c->d_qitems, &c->d_qctl, &c->d_nq, &c->d_planes, &c->d_qkey, &c->d_qhist})
         b->release();
-    for (FitWs& w : c->ws) {
-        for (DevBuf* b : {&w.d_offsets, &w.d_order, &w.d_lenclass, &w.d_qitems, &w.d_qctl, &w.d_nq, &w.d_planes, &w.d_qkey, &w.d_qhist})
-            b->release();
-        w.h_ctl.release();
-        cudaEventDestroy(w.ctl_ev);
-        cudaStreamDestroy(w.stream);
-    }
-    cudaEventDestroy(c->fork_ev);
+    c->h_ctl.release();
+    cudaEventDestroy(c->ctl_ev);
+    cudaStreamDestroy(c->stream);
     delete c;
 }
 
@@ -341,7 +313,7 @@ PB200_API int pb200_last_fit_variant_counts(pb200_ctx* c, int32_t* h_counts) {
     for (int i = 0; i < NQ; ++i) h_counts[i] = 0;
     if (!c->d_vcount.p) return PB200_OK;      // no fit yet
     CK(cudaSetDevice(c->device));
-    for (FitWs& w : c->ws) CK(cudaStreamSynchronize(w.stream));
+    CK(cudaStreamSynchronize(c->stream));
     CK(cudaMemcpy(h_counts, c->d_vcount.p, NQ * 4, cudaMemcpyDeviceToHost));
     return PB200_OK;
 }
@@ -349,24 +321,14 @@ PB200_API int pb200_last_fit_variant_counts(pb200_ctx* c, int32_t* h_counts) {
 PB200_API int pb200_synchronize(pb200_ctx* c) {
     if (!c) return fail(PB200_E_ARG, "ctx is null");
     CK(cudaSetDevice(c->device));
-    for (FitWs& w : c->ws) CK(cudaStreamSynchronize(w.stream));
+    CK(cudaStreamSynchronize(c->stream));
     return PB200_OK;
 }
 
 }  // extern "C"
 
-// zero the per-call variant counters (on workspace 0's stream; the other workspaces are ordered behind it)
-static int begin_fit_call(pb200_ctx* c) {
-    CK(c->d_vcount.reserve(NQ * 4));
-    CK(cudaMemsetAsync(c->d_vcount.p, 0, NQ * 4, c->ws[0].stream));
-    CK(cudaEventRecord(c->fork_ev, c->ws[0].stream));
-    for (int i = 1; i < NWS; ++i) CK(cudaStreamWaitEvent(c->ws[i].stream, c->fork_ev, 0));
-    return PB200_OK;
-}
-
-// newton_kernel over the queue {count, head, items...} at d_nq (16-warp CTAs with ~100 KB of shared memory: they do not
-// fit beside a full house of fit CTAs, which is why the chunked host path runs them after all chunks, and only if needed)
-static int launch_newton(pb200_ctx* c, cudaStream_t st, const pb200_options* opts, const int64_t* d_ds, const void* d_y,
+// newton_kernel over the queue {count, head, items...} at d_nq (16-warp CTAs with ~100 KB of shared memory)
+static int launch_newton(pb200_ctx* c, const pb200_options* opts, const int64_t* d_ds, const void* d_y,
                          int32_t y_dtype, const int64_t* d_offsets, int64_t n_series, int* d_nq, double* d_params,
                          double* d_tchange, int32_t* d_meta_i32, int64_t* d_meta_i64, double* d_meta_f64) {
     pb200_layout L;
@@ -393,20 +355,23 @@ static int launch_newton(pb200_ctx* c, cudaStream_t st, const pb200_options* opt
     CK(cudaFuncSetAttribute(pb200::nw::newton_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)nsm));
     int ngrid = (int)std::min<int64_t>(n_series, opts->algorithm == PB200_ALG_NEWTON ? (int64_t)c->sms * 2 : (int64_t)c->sms);
     if (c->grid_max > 0) ngrid = std::min(ngrid, c->grid_max);
-    pb200::nw::newton_kernel<<<ngrid, 32 * pb200::nw::NW_WARPS, nsm, st>>>(na);
+    pb200::nw::newton_kernel<<<ngrid, 32 * pb200::nw::NW_WARPS, nsm, c->stream>>>(na);
     CK(cudaGetLastError());
     c->launches++;
     return PB200_OK;
 }
 
-static int fit_impl(pb200_ctx* c, FitWs& w, const pb200_options* opts, const int64_t* d_ds, const void* d_y, int32_t y_dtype,
+// every fit call: zeroes the variant counters, then queues, fit kernels and (unless this is an objective evaluation,
+// d_theta_in set) the Newton retry on the context's stream
+static int fit_impl(pb200_ctx* c, const pb200_options* opts, const int64_t* d_ds, const void* d_y, int32_t y_dtype,
                     const int64_t* h_offsets, int64_t n_series, double floor, double cap_multiplier,
                     const double* d_cap, double* d_params, double* d_tchange, int32_t* d_meta_i32,
                     int64_t* d_meta_i64, double* d_meta_f64, const double* d_theta_in, double* d_grad_out,
-                    double* d_trace = nullptr, int trace_cap = 0, int64_t n_call = 0, int* ext_nq = nullptr) {
-    // ext_nq (chunked host call): {count, head} of this chunk's Newton retry queue followed at ext_nq + 2 by its items;
-    // the queue is then only FILLED here and the caller launches newton_kernel after all chunks (see pb200_fit_host)
+                    double* d_trace = nullptr, int trace_cap = 0) {
     if (!c) return fail(PB200_E_ARG, "ctx is null");
+    CK(cudaSetDevice(c->device));
+    CK(c->d_vcount.reserve(NQ * 4));
+    CK(cudaMemsetAsync(c->d_vcount.p, 0, NQ * 4, c->stream));
     int rc = check_opts(opts);
     if (rc) return rc;
     if (n_series < 0 || n_series > (1LL << 30)) return fail(PB200_E_ARG, "n_series");
@@ -416,21 +381,20 @@ static int fit_impl(pb200_ctx* c, FitWs& w, const pb200_options* opts, const int
     if (y_dtype < 0 || y_dtype > 2) return fail(PB200_E_ARG, "y_dtype");
     pb200_layout L;
     pb200_get_layout(opts, &L);
-    CK(cudaSetDevice(c->device));
     const int N = (int)n_series;
 
     // ---- host: length classes and longest-first order (counting sort on T) ----
     size_t ctl_bytes = (size_t)(N + 1) * 8 + (size_t)N * 4 * 2;
-    if (w.ctl_pending) {   // the pinned staging of the previous call must have been consumed
-        CK(cudaEventSynchronize(w.ctl_ev));
-        w.ctl_pending = false;
+    if (c->ctl_pending) {   // the pinned staging of the previous call must have been consumed
+        CK(cudaEventSynchronize(c->ctl_ev));
+        c->ctl_pending = false;
     }
-    CK(w.h_ctl.reserve(ctl_bytes));
-    int64_t* ho = (int64_t*)w.h_ctl.p;
+    CK(c->h_ctl.reserve(ctl_bytes));
+    int64_t* ho = (int64_t*)c->h_ctl.p;
     int* horder = (int*)(ho + N + 1);
     int* hlc = horder + N;
     memcpy(ho, h_offsets, (size_t)(N + 1) * 8);
-    int lc_n[NLC] = {0, 0, 0}, lc_tmax[NLC] = {0, 0, 0};
+    int lc_n[NLC] = {0, 0}, lc_tmax[NLC] = {0, 0};
     int64_t tmax_all = 0;
     for (int i = 0; i < N; ++i) {
         const int64_t T = ho[i + 1] - ho[i];
@@ -450,53 +414,47 @@ static int fit_impl(pb200_ctx* c, FitWs& w, const pb200_options* opts, const int
             horder[posv[(size_t)T]++] = i;
             // CTA width: one warp per series fills the chip once there are >= ~8 series per SM; a small
             // batch of long series gets 4 warps per series instead (same kernels, NT = 128)
-            int lc = 0;
-            while (lc < NLC - 1 && T > c->lc_max[lc]) ++lc;
-            if (c->lc_auto && N < c->sms * 8 && T >= 256) lc = NLC - 1;
+            const int lc = (T > c->lc0_max || (c->lc_auto && N < c->sms * 8 && T >= 256)) ? 1 : 0;
             hlc[i] = lc;
             lc_n[lc]++;
             if (T > lc_tmax[lc]) lc_tmax[lc] = T;
         }
     }
     // ---- device control buffers ----
-    CK(w.d_offsets.reserve((size_t)(N + 1) * 8));
-    CK(w.d_order.reserve((size_t)N * 4));
-    CK(w.d_lenclass.reserve((size_t)N * 4));
-    CK(w.d_qitems.reserve((size_t)NLC * NQ * N * 4));
-    CK(w.d_qctl.reserve((size_t)NLC * NQ * 2 * 4));
-    CK(w.d_qkey.reserve((size_t)N * 4));
-    CK(w.d_qhist.reserve((size_t)NLC * NQ * pb200::QBINS * 4));
-    CK(cudaMemsetAsync(w.d_qkey.p, 0xff, (size_t)N * 4, w.stream));
-    CK(cudaMemsetAsync(w.d_qhist.p, 0, (size_t)NLC * NQ * pb200::QBINS * 4, w.stream));
-    int* nq = ext_nq;
-    if (!nq) {
-        CK(w.d_nq.reserve((size_t)(N + 2) * 4));             // count, head, items[N]
-        nq = (int*)w.d_nq.p;
-    }
-    CK(cudaMemsetAsync(nq, 0, 8, w.stream));
-    CK(cudaMemcpyAsync(w.d_offsets.p, ho, (size_t)(N + 1) * 8, cudaMemcpyHostToDevice, w.stream));
-    CK(cudaMemcpyAsync(w.d_order.p, horder, (size_t)N * 4, cudaMemcpyHostToDevice, w.stream));
-    CK(cudaMemcpyAsync(w.d_lenclass.p, hlc, (size_t)N * 4, cudaMemcpyHostToDevice, w.stream));
-    CK(cudaEventRecord(w.ctl_ev, w.stream));
-    w.ctl_pending = true;
-    CK(cudaMemsetAsync(w.d_qctl.p, 0, (size_t)NLC * NQ * 2 * 4, w.stream));
-    CK(cudaMemsetAsync(d_params, 0, (size_t)N * L.pstride * 8, w.stream));
-    CK(cudaMemsetAsync(d_tchange, 0, (size_t)N * L.smax * 8, w.stream));
-    int* q_count = (int*)w.d_qctl.p;
+    CK(c->d_offsets.reserve((size_t)(N + 1) * 8));
+    CK(c->d_order.reserve((size_t)N * 4));
+    CK(c->d_lenclass.reserve((size_t)N * 4));
+    CK(c->d_qitems.reserve((size_t)NLC * NQ * N * 4));
+    CK(c->d_qctl.reserve((size_t)NLC * NQ * 2 * 4));
+    CK(c->d_qkey.reserve((size_t)N * 4));
+    CK(c->d_qhist.reserve((size_t)NLC * NQ * pb200::QBINS * 4));
+    CK(cudaMemsetAsync(c->d_qkey.p, 0xff, (size_t)N * 4, c->stream));
+    CK(cudaMemsetAsync(c->d_qhist.p, 0, (size_t)NLC * NQ * pb200::QBINS * 4, c->stream));
+    CK(c->d_nq.reserve((size_t)(N + 2) * 4));             // count, head, items[N]
+    int* nq = (int*)c->d_nq.p;
+    CK(cudaMemsetAsync(nq, 0, 8, c->stream));
+    CK(cudaMemcpyAsync(c->d_offsets.p, ho, (size_t)(N + 1) * 8, cudaMemcpyHostToDevice, c->stream));
+    CK(cudaMemcpyAsync(c->d_order.p, horder, (size_t)N * 4, cudaMemcpyHostToDevice, c->stream));
+    CK(cudaMemcpyAsync(c->d_lenclass.p, hlc, (size_t)N * 4, cudaMemcpyHostToDevice, c->stream));
+    CK(cudaEventRecord(c->ctl_ev, c->stream));
+    c->ctl_pending = true;
+    CK(cudaMemsetAsync(c->d_qctl.p, 0, (size_t)NLC * NQ * 2 * 4, c->stream));
+    CK(cudaMemsetAsync(d_params, 0, (size_t)N * L.pstride * 8, c->stream));
+    CK(cudaMemsetAsync(d_tchange, 0, (size_t)N * L.smax * 8, c->stream));
+    int* q_count = (int*)c->d_qctl.p;
     int* q_head = q_count + NLC * NQ;
 
     const FitOptsDev od = to_dev(opts);
     // lanes per series of the grouped day-table kernel
-    // (n_call: series of the whole API call when this is one chunk of it)
-    const int grp_g = !c->tab_on ? 0 : (c->grp_g >= 0 ? c->grp_g : (std::max<int64_t>(N, n_call) >= c->grp_min ? 8 : 16));
+    const int grp_g = !c->tab_on ? 0 : (c->grp_g >= 0 ? c->grp_g : (N >= c->grp_min ? 8 : 16));
     // ---- prep kernel ----
     {
         pb200::PrepArgs pa;
         pa.ds = (const long long*)d_ds;
         pa.y = d_y;
         pa.y_dtype = y_dtype;
-        pa.offsets = (const long long*)w.d_offsets.p;
-        pa.order = (const int*)w.d_order.p;
+        pa.offsets = (const long long*)c->d_offsets.p;
+        pa.order = (const int*)c->d_order.p;
         pa.cap = d_cap;
         pa.floor = floor;
         pa.cap_multiplier = cap_multiplier;
@@ -504,8 +462,8 @@ static int fit_impl(pb200_ctx* c, FitWs& w, const pb200_options* opts, const int
         pa.meta_i32 = d_meta_i32;
         pa.meta_i64 = (long long*)d_meta_i64;
         pa.meta_f64 = d_meta_f64;
-        pa.lenclass = (const int*)w.d_lenclass.p;
-        pa.q_items = (int*)w.d_qitems.p;
+        pa.lenclass = (const int*)c->d_lenclass.p;
+        pa.q_items = (int*)c->d_qitems.p;
         pa.q_count = q_count;
         pa.o = od;
         pa.tab_lc_mask = 0;
@@ -513,22 +471,22 @@ static int fit_impl(pb200_ctx* c, FitWs& w, const pb200_options* opts, const int
             if (c->tab_on && LC_NT[lc] == 32) pa.tab_lc_mask |= 1 << lc;
         pa.grp_g = grp_g;
         pa.grp_plain = (c->plain_grp && grp_g > 0) ? 1 : 0;
-        { static const char* e = getenv("PB200_QKEY_CV"); pa.cv_weight = e ? atof(e) : 2.0; }
+        pa.cv_weight = QKEY_CV_WEIGHT;
         pa.newton_only = (opts->algorithm == PB200_ALG_NEWTON && !d_theta_in) ? 1 : 0;
         pa.nq_count = nq;
         pa.nq_items = nq + 2;
         pa.vcount = (int*)c->d_vcount.p;
-        pa.qkey = (int*)w.d_qkey.p;
-        pa.qhist = (int*)w.d_qhist.p;
+        pa.qkey = (int*)c->d_qkey.p;
+        pa.qhist = (int*)c->d_qhist.p;
         const int warps_per_block = 8;
         int grid = (N + warps_per_block - 1) / warps_per_block;
         grid = std::min(grid, c->sms * 8);
-        pb200::prep_kernel<<<grid, warps_per_block * 32, 0, w.stream>>>(pa);
+        pb200::prep_kernel<<<grid, warps_per_block * 32, 0, c->stream>>>(pa);
         CK(cudaGetLastError());
-        pb200::queue_scan_kernel<<<(NLC * NQ + 127) / 128, 128, 0, w.stream>>>((int*)w.d_qhist.p, NLC * NQ);
+        pb200::queue_scan_kernel<<<(NLC * NQ + 127) / 128, 128, 0, c->stream>>>((int*)c->d_qhist.p, NLC * NQ);
         CK(cudaGetLastError());
-        pb200::queue_scatter_kernel<<<std::min((N + 255) / 256, c->sms * 8), 256, 0, w.stream>>>(
-            (const int*)w.d_qkey.p, (int*)w.d_qhist.p, (int*)w.d_qitems.p, N);
+        pb200::queue_scatter_kernel<<<std::min((N + 255) / 256, c->sms * 8), 256, 0, c->stream>>>(
+            (const int*)c->d_qkey.p, (int*)c->d_qhist.p, (int*)c->d_qitems.p, N);
         CK(cudaGetLastError());
         c->launches += 3;
     }
@@ -566,7 +524,7 @@ static int fit_impl(pb200_ctx* c, FitWs& w, const pb200_options* opts, const int
             if (reg == 3 && grp_g > 0) {
                 // grouped day-table kernel: one warp per CTA, 32 / grp_g series per warp, one workspace slot per series
                 const int nser = 32 / grp_g;
-                CK(pb200::launch_fit_group(grp_g, opts->growth, opts->multiplicative ? 1 : 0, mask != 0, dummy, 0, w.stream, &occ));
+                CK(pb200::launch_fit_group(grp_g, opts->growth, opts->multiplicative ? 1 : 0, mask != 0, dummy, 0, c->stream, &occ));
                 if (occ < 1) return fail(PB200_E_UNSUPPORTED, "grouped fit kernel does not fit on an SM");
                 g.grouped = true;
                 g.slice = pb200::fit_group_plane_doubles(lc_tmax[lc], grp_g);           // doubles per slot
@@ -575,13 +533,13 @@ static int fit_impl(pb200_ctx* c, FitWs& w, const pb200_options* opts, const int
                 g.on = true;
                 continue;
             }
-            CK(LAUNCH[mask](NT, opts->growth, reg, dummy, 0, g.smem, w.stream, &occ));
+            CK(LAUNCH[mask](NT, opts->growth, reg, dummy, 0, g.smem, c->stream, &occ));
             if (occ < 1) return fail(PB200_E_UNSUPPORTED, "fit kernel does not fit on an SM");
             g.grid = cap_grid(std::min<int64_t>((int64_t)lc_n[lc], (int64_t)c->sms * occ));
             planes_bytes += (size_t)g.grid * g.slice * 16;
             g.on = true;
         }
-    CK(w.d_planes.reserve(planes_bytes));
+    CK(c->d_planes.reserve(planes_bytes));
     for (int lc = 0; lc < NLC; ++lc) {
         if (lc_n[lc] == 0) continue;
         const int NT = LC_NT[lc];
@@ -595,9 +553,9 @@ static int fit_impl(pb200_ctx* c, FitWs& w, const pb200_options* opts, const int
             fa.ds = (const long long*)d_ds;
             fa.y = d_y;
             fa.y_dtype = y_dtype;
-            fa.offsets = (const long long*)w.d_offsets.p;
+            fa.offsets = (const long long*)c->d_offsets.p;
             const int q = lc * NQ + rm;
-            fa.q_items = (const int*)w.d_qitems.p + (size_t)q * N;
+            fa.q_items = (const int*)c->d_qitems.p + (size_t)q * N;
             fa.q_count = q_count + q;
             fa.q_head = q_head + q;
             fa.params = d_params;
@@ -610,7 +568,7 @@ static int fit_impl(pb200_ctx* c, FitWs& w, const pb200_options* opts, const int
             fa.pstride = L.pstride;
             fa.Tp = Tp;
             fa.ppad = ppad;
-            fa.planes = (double2*)((char*)w.d_planes.p + g.off);
+            fa.planes = (double2*)((char*)c->d_planes.p + g.off);
             fa.nseas_stride = (int)g.slice;
             fa.theta_in = d_theta_in;
             fa.grad_out = d_grad_out;
@@ -629,44 +587,35 @@ static int fit_impl(pb200_ctx* c, FitWs& w, const pb200_options* opts, const int
                 fa.l2_rest_first = 1;
             }
             if (g.grouped) {
-                CK(pb200::launch_fit_group(grp_g, opts->growth, opts->multiplicative ? 1 : 0, mask != 0, fa, g.grid, w.stream, nullptr));
+                CK(pb200::launch_fit_group(grp_g, opts->growth, opts->multiplicative ? 1 : 0, mask != 0, fa, g.grid, c->stream, nullptr));
             } else {
-                CK(LAUNCH[mask](NT, opts->growth, reg, fa, g.grid, smem, w.stream, nullptr));
+                CK(LAUNCH[mask](NT, opts->growth, reg, fa, g.grid, smem, c->stream, nullptr));
             }
             c->launches++;
         }
     }
     // ---- fbprophet's Newton retry over the series whose L-BFGS failed its line search (normally an empty queue) ----
-    if (!ext_nq && !d_theta_in)
-        return launch_newton(c, w.stream, opts, d_ds, d_y, y_dtype, (const int64_t*)w.d_offsets.p, n_series, nq, d_params, d_tchange,
+    if (!d_theta_in)
+        return launch_newton(c, opts, d_ds, d_y, y_dtype, (const int64_t*)c->d_offsets.p, n_series, nq, d_params, d_tchange,
                              d_meta_i32, d_meta_i64, d_meta_f64);
     return PB200_OK;
 }
 
-extern "C" {
-
-PB200_API int pb200_fit_device(pb200_ctx* c, const pb200_options* opts, const int64_t* d_ds, const void* d_y, int32_t y_dtype,
-                     const int64_t* h_offsets, int64_t n_series, double floor, double cap_multiplier,
-                     const double* d_cap, double* d_params, double* d_tchange, int32_t* d_meta_i32,
-                     int64_t* d_meta_i64, double* d_meta_f64) {
-    if (!c) return fail(PB200_E_ARG, "ctx is null");
-    CK(cudaSetDevice(c->device));
-    int rc = begin_fit_call(c);
-    if (rc) return rc;
-    return fit_impl(c, c->ws[0], opts, d_ds, d_y, y_dtype, h_offsets, n_series, floor, cap_multiplier, d_cap, d_params, d_tchange,
-                    d_meta_i32, d_meta_i64, d_meta_f64, nullptr, nullptr);
-}
-
-PB200_API int pb200_objective_host(pb200_ctx* c, const pb200_options* opts, const int64_t* h_ds, const void* h_y,
-                                   int32_t y_dtype, const int64_t* h_offsets, int64_t n_series, double floor,
-                                   double cap_multiplier, const double* h_theta, double* h_f, double* h_grad,
-                                   int32_t* h_meta_i32) {
+// argument checks of the *_host fit entry points (outs: the caller's own pointers are all set); n_series == 0 passes
+static int check_host_fit(pb200_ctx* c, const pb200_options* opts, const int64_t* h_ds, const void* h_y, int32_t y_dtype,
+                          const int64_t* h_offsets, int64_t n_series, bool outs) {
     if (!c) return fail(PB200_E_ARG, "ctx is null");
     int rc = check_opts(opts);
     if (rc) return rc;
     if (n_series <= 0) return n_series == 0 ? PB200_OK : fail(PB200_E_ARG, "n_series");
-    if (!h_ds || !h_y || !h_offsets || !h_theta || !h_f || !h_grad || !h_meta_i32) return fail(PB200_E_ARG, "null pointer");
+    if (!h_ds || !h_y || !h_offsets || !outs) return fail(PB200_E_ARG, "null pointer");
     if (y_dtype < 0 || y_dtype > 2) return fail(PB200_E_ARG, "y_dtype");
+    return PB200_OK;
+}
+
+// ... and their common staging: ds and y copied in, room for the fitted records
+static int stage_host_fit(pb200_ctx* c, const pb200_options* opts, const int64_t* h_ds, const void* h_y, int32_t y_dtype,
+                          const int64_t* h_offsets, int64_t n_series) {
     pb200_layout L;
     pb200_get_layout(opts, &L);
     CK(cudaSetDevice(c->device));
@@ -679,15 +628,72 @@ PB200_API int pb200_objective_host(pb200_ctx* c, const pb200_options* opts, cons
     CK(c->d_mi32.reserve(N * 8 * 4));
     CK(c->d_mi64.reserve(N * 2 * 8));
     CK(c->d_mf64.reserve(N * 4 * 8));
-    CK(c->d_yhat.reserve(N * L.pstride * 8));   // theta_in
-    CK(c->d_lo.reserve(N * L.pstride * 8));     // grad_out
     CK(cudaMemcpyAsync(c->d_ds.p, h_ds, (size_t)R * 8, cudaMemcpyHostToDevice, c->stream));
     CK(cudaMemcpyAsync(c->d_y.p, h_y, (size_t)R * y_elem(y_dtype), cudaMemcpyHostToDevice, c->stream));
+    return PB200_OK;
+}
+
+// pb200_fit_host and pb200_fit_trace_host (traced: trace_cap trajectory rows per series into h_trace): copy in, fit, copy out
+static int fit_host(pb200_ctx* c, const pb200_options* opts, const int64_t* h_ds, const void* h_y, int32_t y_dtype,
+                    const int64_t* h_offsets, int64_t n_series, double floor, double cap_multiplier, const double* h_cap,
+                    double* h_params, double* h_tchange, int32_t* h_meta_i32, int64_t* h_meta_i64, double* h_meta_f64,
+                    bool traced, double* h_trace, int32_t trace_cap) {
+    int rc = check_host_fit(c, opts, h_ds, h_y, y_dtype, h_offsets, n_series,
+                            h_params && h_tchange && h_meta_i32 && h_meta_i64 && h_meta_f64 && (h_trace || !traced));
+    if (rc || n_series == 0) return rc;
+    if (traced && (trace_cap < 1 || (int64_t)trace_cap * n_series > (1LL << 26))) return fail(PB200_E_ARG, "trace_cap");
+    if ((rc = stage_host_fit(c, opts, h_ds, h_y, y_dtype, h_offsets, n_series))) return rc;
+    pb200_layout L;
+    pb200_get_layout(opts, &L);
+    const size_t N = (size_t)n_series, tbytes = traced ? N * (size_t)trace_cap * 4 * 8 : 0;
+    if (h_cap) {
+        CK(c->d_cap.reserve(N * 8));
+        CK(cudaMemcpyAsync(c->d_cap.p, h_cap, N * 8, cudaMemcpyHostToDevice, c->stream));
+    }
+    if (traced) {
+        CK(c->d_trace.reserve(tbytes));
+        CK(cudaMemsetAsync(c->d_trace.p, 0, tbytes, c->stream));
+    }
+    rc = fit_impl(c, opts, (const int64_t*)c->d_ds.p, c->d_y.p, y_dtype, h_offsets, n_series, floor, cap_multiplier,
+                  h_cap ? (const double*)c->d_cap.p : nullptr, (double*)c->d_params.p, (double*)c->d_tchange.p,
+                  (int32_t*)c->d_mi32.p, (int64_t*)c->d_mi64.p, (double*)c->d_mf64.p, nullptr, nullptr,
+                  traced ? (double*)c->d_trace.p : nullptr, trace_cap);
+    if (rc) return rc;
+    CK(cudaMemcpyAsync(h_params, c->d_params.p, N * L.pstride * 8, cudaMemcpyDeviceToHost, c->stream));
+    CK(cudaMemcpyAsync(h_tchange, c->d_tchange.p, N * L.smax * 8, cudaMemcpyDeviceToHost, c->stream));
+    CK(cudaMemcpyAsync(h_meta_i32, c->d_mi32.p, N * 8 * 4, cudaMemcpyDeviceToHost, c->stream));
+    CK(cudaMemcpyAsync(h_meta_i64, c->d_mi64.p, N * 2 * 8, cudaMemcpyDeviceToHost, c->stream));
+    CK(cudaMemcpyAsync(h_meta_f64, c->d_mf64.p, N * 4 * 8, cudaMemcpyDeviceToHost, c->stream));
+    if (traced) CK(cudaMemcpyAsync(h_trace, c->d_trace.p, tbytes, cudaMemcpyDeviceToHost, c->stream));
+    CK(cudaStreamSynchronize(c->stream));
+    return PB200_OK;
+}
+
+extern "C" {
+
+PB200_API int pb200_fit_device(pb200_ctx* c, const pb200_options* opts, const int64_t* d_ds, const void* d_y, int32_t y_dtype,
+                     const int64_t* h_offsets, int64_t n_series, double floor, double cap_multiplier,
+                     const double* d_cap, double* d_params, double* d_tchange, int32_t* d_meta_i32,
+                     int64_t* d_meta_i64, double* d_meta_f64) {
+    return fit_impl(c, opts, d_ds, d_y, y_dtype, h_offsets, n_series, floor, cap_multiplier, d_cap, d_params, d_tchange,
+                    d_meta_i32, d_meta_i64, d_meta_f64, nullptr, nullptr);
+}
+
+PB200_API int pb200_objective_host(pb200_ctx* c, const pb200_options* opts, const int64_t* h_ds, const void* h_y,
+                                   int32_t y_dtype, const int64_t* h_offsets, int64_t n_series, double floor,
+                                   double cap_multiplier, const double* h_theta, double* h_f, double* h_grad,
+                                   int32_t* h_meta_i32) {
+    int rc = check_host_fit(c, opts, h_ds, h_y, y_dtype, h_offsets, n_series, h_theta && h_f && h_grad && h_meta_i32);
+    if (rc || n_series == 0) return rc;
+    if ((rc = stage_host_fit(c, opts, h_ds, h_y, y_dtype, h_offsets, n_series))) return rc;
+    pb200_layout L;
+    pb200_get_layout(opts, &L);
+    const size_t N = (size_t)n_series;
+    CK(c->d_yhat.reserve(N * L.pstride * 8));   // theta_in
+    CK(c->d_lo.reserve(N * L.pstride * 8));     // grad_out
     CK(cudaMemcpyAsync(c->d_yhat.p, h_theta, N * L.pstride * 8, cudaMemcpyHostToDevice, c->stream));
     CK(cudaMemsetAsync(c->d_lo.p, 0, N * L.pstride * 8, c->stream));
-    rc = begin_fit_call(c);
-    if (rc) return rc;
-    rc = fit_impl(c, c->ws[0], opts, (const int64_t*)c->d_ds.p, c->d_y.p, y_dtype, h_offsets, n_series, floor, cap_multiplier,
+    rc = fit_impl(c, opts, (const int64_t*)c->d_ds.p, c->d_y.p, y_dtype, h_offsets, n_series, floor, cap_multiplier,
                   nullptr, (double*)c->d_params.p, (double*)c->d_tchange.p, (int32_t*)c->d_mi32.p,
                   (int64_t*)c->d_mi64.p, (double*)c->d_mf64.p, (const double*)c->d_yhat.p, (double*)c->d_lo.p);
     if (rc) return rc;
@@ -703,138 +709,16 @@ PB200_API int pb200_objective_host(pb200_ctx* c, const pb200_options* opts, cons
 PB200_API int pb200_fit_host(pb200_ctx* c, const pb200_options* opts, const int64_t* h_ds, const void* h_y, int32_t y_dtype,
                    const int64_t* h_offsets, int64_t n_series, double floor, double cap_multiplier, const double* h_cap,
                    double* h_params, double* h_tchange, int32_t* h_meta_i32, int64_t* h_meta_i64, double* h_meta_f64) {
-    if (!c) return fail(PB200_E_ARG, "ctx is null");
-    int rc = check_opts(opts);
-    if (rc) return rc;
-    if (n_series <= 0) return n_series == 0 ? PB200_OK : fail(PB200_E_ARG, "n_series");
-    if (!h_ds || !h_y || !h_offsets || !h_params || !h_tchange || !h_meta_i32 || !h_meta_i64 || !h_meta_f64)
-        return fail(PB200_E_ARG, "null pointer");
-    if (y_dtype < 0 || y_dtype > 2) return fail(PB200_E_ARG, "y_dtype");
-    pb200_layout L;
-    pb200_get_layout(opts, &L);
-    CK(cudaSetDevice(c->device));
-    const int64_t R = h_offsets[n_series];
-    const size_t N = (size_t)n_series;
-    CK(c->d_ds.reserve((size_t)R * 8));
-    CK(c->d_y.reserve((size_t)R * y_elem(y_dtype)));
-    CK(c->d_params.reserve(N * L.pstride * 8));
-    CK(c->d_tchange.reserve(N * L.smax * 8));
-    CK(c->d_mi32.reserve(N * 8 * 4));
-    CK(c->d_mi64.reserve(N * 2 * 8));
-    CK(c->d_mf64.reserve(N * 4 * 8));
-    if (h_cap) CK(c->d_cap.reserve(N * 8));
-    CK(c->d_nq_all.reserve((N + 2 * 16 + 2) * 4));
-    CK(c->d_offsets_full.reserve((N + 1) * 8));
-    rc = begin_fit_call(c);
-    if (rc) return rc;
-    CK(cudaMemcpyAsync(c->d_offsets_full.p, h_offsets, (N + 1) * 8, cudaMemcpyHostToDevice, c->ws[0].stream));
-    // series chunks with (nearly) equal rows, alternating over the two workspaces / streams: copy in, fit, copy out
-    int nch = c->host_chunks;
-    if (n_series < 4096 * (int64_t)nch || R < (int64_t)nch * (1 << 20)) nch = 1;
-    const size_t ye = y_elem(y_dtype);
-    std::vector<int64_t> cut(nch + 1, 0), hoff;
-    cut[nch] = n_series;
-    for (int k = 1; k < nch; ++k)
-        cut[k] = std::lower_bound(h_offsets, h_offsets + n_series + 1, R * k / nch) - h_offsets;
-    for (int k = 0; k < nch; ++k) {
-        const int64_t s0 = cut[k], s1 = cut[k + 1], nk = s1 - s0;
-        if (nk <= 0) continue;
-        FitWs& w = c->ws[k % NWS];
-        const int64_t r0 = h_offsets[s0], rk = h_offsets[s1] - r0;
-        CK(cudaMemcpyAsync((char*)c->d_ds.p + (size_t)r0 * 8, h_ds + r0, (size_t)rk * 8, cudaMemcpyHostToDevice, w.stream));
-        CK(cudaMemcpyAsync((char*)c->d_y.p + (size_t)r0 * ye, (const char*)h_y + (size_t)r0 * ye, (size_t)rk * ye,
-                           cudaMemcpyHostToDevice, w.stream));
-        const double* dcap = nullptr;
-        if (h_cap) {
-            CK(cudaMemcpyAsync((double*)c->d_cap.p + s0, h_cap + s0, (size_t)nk * 8, cudaMemcpyHostToDevice, w.stream));
-            dcap = (const double*)c->d_cap.p + s0;
-        }
-        hoff.resize((size_t)nk + 1);
-        for (int64_t i = 0; i <= nk; ++i) hoff[(size_t)i] = h_offsets[s0 + i] - r0;
-        rc = fit_impl(c, w, opts, (const int64_t*)c->d_ds.p + r0, (const char*)c->d_y.p + (size_t)r0 * ye, y_dtype, hoff.data(), nk,
-                      floor, cap_multiplier, dcap, (double*)c->d_params.p + (size_t)s0 * L.pstride,
-                      (double*)c->d_tchange.p + (size_t)s0 * L.smax, (int32_t*)c->d_mi32.p + (size_t)s0 * 8,
-                      (int64_t*)c->d_mi64.p + (size_t)s0 * 2, (double*)c->d_mf64.p + (size_t)s0 * 4, nullptr, nullptr, nullptr, 0,
-                      n_series, (int*)c->d_nq_all.p + s0 + 2 * k);
-        if (rc) return rc;
-    }
-    // Newton retries, normally none: the per-chunk queue lengths are read back once every chunk's fit is done
-    if (opts->algorithm != PB200_ALG_LBFGS) {
-        for (FitWs& w : c->ws) CK(cudaStreamSynchronize(w.stream));
-        for (int k = 0; k < nch; ++k) {
-            const int64_t s0 = cut[k], nk = cut[k + 1] - s0;
-            if (nk <= 0) continue;
-            int* nq = (int*)c->d_nq_all.p + s0 + 2 * k;
-            int cnt = 0;
-            CK(cudaMemcpy(&cnt, nq, 4, cudaMemcpyDeviceToHost));
-            if (cnt <= 0) continue;
-            // chunk-local series indices, the call's un-rebased offsets: ds / y are passed whole
-            rc = launch_newton(c, c->ws[k % NWS].stream, opts, (const int64_t*)c->d_ds.p, c->d_y.p, y_dtype,
-                               (const int64_t*)c->d_offsets_full.p + s0, nk, nq, (double*)c->d_params.p + (size_t)s0 * L.pstride,
-                               (double*)c->d_tchange.p + (size_t)s0 * L.smax, (int32_t*)c->d_mi32.p + (size_t)s0 * 8,
-                               (int64_t*)c->d_mi64.p + (size_t)s0 * 2, (double*)c->d_mf64.p + (size_t)s0 * 4);
-            if (rc) return rc;
-        }
-    }
-    // results back, chunk by chunk, only after EVERY chunk is enqueued: a copy into pageable caller memory blocks the
-    // host until its stream gets there, and issued inside the loop above it serialised the chunks
-    for (int k = 0; k < nch; ++k) {
-        const int64_t s0 = cut[k], nk = cut[k + 1] - s0;
-        if (nk <= 0) continue;
-        FitWs& w = c->ws[k % NWS];
-        const size_t n0 = (size_t)s0, nn = (size_t)nk;
-        CK(cudaMemcpyAsync(h_params + n0 * L.pstride, (double*)c->d_params.p + n0 * L.pstride, nn * L.pstride * 8, cudaMemcpyDeviceToHost, w.stream));
-        CK(cudaMemcpyAsync(h_tchange + n0 * L.smax, (double*)c->d_tchange.p + n0 * L.smax, nn * L.smax * 8, cudaMemcpyDeviceToHost, w.stream));
-        CK(cudaMemcpyAsync(h_meta_i32 + n0 * 8, (int32_t*)c->d_mi32.p + n0 * 8, nn * 8 * 4, cudaMemcpyDeviceToHost, w.stream));
-        CK(cudaMemcpyAsync(h_meta_i64 + n0 * 2, (int64_t*)c->d_mi64.p + n0 * 2, nn * 2 * 8, cudaMemcpyDeviceToHost, w.stream));
-        CK(cudaMemcpyAsync(h_meta_f64 + n0 * 4, (double*)c->d_mf64.p + n0 * 4, nn * 4 * 8, cudaMemcpyDeviceToHost, w.stream));
-    }
-    for (FitWs& w : c->ws) CK(cudaStreamSynchronize(w.stream));
-    return PB200_OK;
+    return fit_host(c, opts, h_ds, h_y, y_dtype, h_offsets, n_series, floor, cap_multiplier, h_cap, h_params, h_tchange,
+                    h_meta_i32, h_meta_i64, h_meta_f64, false, nullptr, 0);
 }
 
 PB200_API int pb200_fit_trace_host(pb200_ctx* c, const pb200_options* opts, const int64_t* h_ds, const void* h_y, int32_t y_dtype,
                          const int64_t* h_offsets, int64_t n_series, double floor, double cap_multiplier, double* h_params,
                          double* h_tchange, int32_t* h_meta_i32, int64_t* h_meta_i64, double* h_meta_f64, double* h_trace,
                          int32_t trace_cap) {
-    if (!c) return fail(PB200_E_ARG, "ctx is null");
-    int rc = check_opts(opts);
-    if (rc) return rc;
-    if (n_series <= 0) return n_series == 0 ? PB200_OK : fail(PB200_E_ARG, "n_series");
-    if (!h_ds || !h_y || !h_offsets || !h_params || !h_tchange || !h_meta_i32 || !h_meta_i64 || !h_meta_f64 || !h_trace)
-        return fail(PB200_E_ARG, "null pointer");
-    if (y_dtype < 0 || y_dtype > 2) return fail(PB200_E_ARG, "y_dtype");
-    if (trace_cap < 1 || (int64_t)trace_cap * n_series > (1LL << 26)) return fail(PB200_E_ARG, "trace_cap");
-    pb200_layout L;
-    pb200_get_layout(opts, &L);
-    CK(cudaSetDevice(c->device));
-    const int64_t R = h_offsets[n_series];
-    const size_t N = (size_t)n_series, tbytes = N * (size_t)trace_cap * 4 * 8;
-    CK(c->d_ds.reserve((size_t)R * 8));
-    CK(c->d_y.reserve((size_t)R * y_elem(y_dtype)));
-    CK(c->d_params.reserve(N * L.pstride * 8));
-    CK(c->d_tchange.reserve(N * L.smax * 8));
-    CK(c->d_mi32.reserve(N * 8 * 4));
-    CK(c->d_mi64.reserve(N * 2 * 8));
-    CK(c->d_mf64.reserve(N * 4 * 8));
-    CK(c->d_trace.reserve(tbytes));
-    CK(cudaMemcpyAsync(c->d_ds.p, h_ds, (size_t)R * 8, cudaMemcpyHostToDevice, c->stream));
-    CK(cudaMemcpyAsync(c->d_y.p, h_y, (size_t)R * y_elem(y_dtype), cudaMemcpyHostToDevice, c->stream));
-    CK(cudaMemsetAsync(c->d_trace.p, 0, tbytes, c->stream));
-    rc = begin_fit_call(c);
-    if (rc) return rc;
-    rc = fit_impl(c, c->ws[0], opts, (const int64_t*)c->d_ds.p, c->d_y.p, y_dtype, h_offsets, n_series, floor, cap_multiplier, nullptr,
-                  (double*)c->d_params.p, (double*)c->d_tchange.p, (int32_t*)c->d_mi32.p, (int64_t*)c->d_mi64.p,
-                  (double*)c->d_mf64.p, nullptr, nullptr, (double*)c->d_trace.p, trace_cap);
-    if (rc) return rc;
-    CK(cudaMemcpyAsync(h_params, c->d_params.p, N * L.pstride * 8, cudaMemcpyDeviceToHost, c->stream));
-    CK(cudaMemcpyAsync(h_tchange, c->d_tchange.p, N * L.smax * 8, cudaMemcpyDeviceToHost, c->stream));
-    CK(cudaMemcpyAsync(h_meta_i32, c->d_mi32.p, N * 8 * 4, cudaMemcpyDeviceToHost, c->stream));
-    CK(cudaMemcpyAsync(h_meta_i64, c->d_mi64.p, N * 2 * 8, cudaMemcpyDeviceToHost, c->stream));
-    CK(cudaMemcpyAsync(h_meta_f64, c->d_mf64.p, N * 4 * 8, cudaMemcpyDeviceToHost, c->stream));
-    CK(cudaMemcpyAsync(h_trace, c->d_trace.p, tbytes, cudaMemcpyDeviceToHost, c->stream));
-    CK(cudaStreamSynchronize(c->stream));
-    return PB200_OK;
+    return fit_host(c, opts, h_ds, h_y, y_dtype, h_offsets, n_series, floor, cap_multiplier, nullptr, h_params, h_tchange,
+                    h_meta_i32, h_meta_i64, h_meta_f64, true, h_trace, trace_cap);
 }
 
 PB200_API int pb200_make_future_device(pb200_ctx* c, const int64_t* d_last_ds, int64_t n_models, int32_t horizon, int64_t freq_ns,

@@ -1413,12 +1413,12 @@ template <int G, bool LOGI, bool MULT, bool SEAS>
 #endif
 __global__ void __launch_bounds__(32, G != 8 ? 16 : (SEAS ? PB200_GRP_BLOCKS : PB200_GRP_PLAIN_BLOCKS)) fit_group_kernel(const __grid_constant__ FitArgs a) {
     // (__grid_constant__: g_fetch and g_write_record take `a` by reference without a copy of it in local memory)
-    static_assert(G == 8 || G == 16 || G == 32, "lanes per series");
+    static_assert(G == 8 || G == 16, "lanes per series");
     static_assert(SEAS || !MULT, "without seasonality the additive form is the model");
     static_assert((SEAS ? 6 * G * 8 : 0) + G * 4 <= 5 * GState<G, SEAS>::PPAD * 8, "LanePhase hand-over through vec[1..5]");
     constexpr int NSER = 32 / G;
     const int lane = threadIdx.x & 31, gi = lane / G, gl = lane % G;
-    const unsigned gm = G == 32 ? FULL : (((1u << G) - 1u) << (gi * G));
+    const unsigned gm = ((1u << G) - 1u) << (gi * G);
     GState<G, SEAS>& s = gstate<G, SEAS>(gi);
     const size_t slot = (size_t)blockIdx.x * NSER + gi;
     double* const plane = reinterpret_cast<double*>(a.planes) + slot * (size_t)a.nseas_stride;

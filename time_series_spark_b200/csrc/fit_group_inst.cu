@@ -1,4 +1,4 @@
-// Instantiations of the grouped-lanes fit kernel (fit_group.cuh): G in {8, 16, 32} lanes per series x growth x
+// Instantiations of the grouped-lanes fit kernel (fit_group.cuh): G in {8, 16} lanes per series x growth x
 // seasonality mode for the weekly + daily day-table class, x growth for the class without seasonality.
 #include <cstdlib>
 
@@ -30,7 +30,6 @@ static cudaError_t launch_group_g(int logi, int mult, int seas, const FitArgs& a
 cudaError_t launch_fit_group(int g, int logi, int mult, int seas, const FitArgs& a, int grid, cudaStream_t st, int* occ) {
     if (g == 8) return launch_group_g<8>(logi, mult, seas, a, grid, st, occ);
     if (g == 16) return launch_group_g<16>(logi, mult, seas, a, grid, st, occ);
-    if (g == 32) return launch_group_g<32>(logi, mult, seas, a, grid, st, occ);
     return cudaErrorInvalidValue;
 }
 

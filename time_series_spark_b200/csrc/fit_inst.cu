@@ -1,7 +1,7 @@
 // One translation unit per seasonality class (compile with -DPB200_MASK=0..7):
 // bit0 yearly (order 10), bit1 weekly (order 3), bit2 daily (order 4) -- the Fourier
 // orders Prophet.set_auto_seasonalities uses.  Instantiates fit_kernel for
-// NT in {32, 64, 128} x growth in {linear, logistic}.
+// NT in {32, 128} x growth in {linear, logistic}.
 #include "fit_kernel.cuh"
 #include "launch.h"
 
@@ -47,7 +47,6 @@ static cudaError_t launch_nt(int logi, int reg, const FitArgs& a, int grid, size
 cudaError_t PB200_CAT(launch_fit_mask, PB200_MASK)(int nt, int logi, int reg, const FitArgs& a, int grid, size_t smem,
                                                    cudaStream_t st, int* occ) {
     if (nt == 32) return launch_nt<32>(logi, reg, a, grid, smem, st, occ);
-    if (nt == 64) return launch_nt<64>(logi, reg, a, grid, smem, st, occ);
     if (nt == 128) return launch_nt<128>(logi, reg, a, grid, smem, st, occ);
     return cudaErrorInvalidValue;
 }

@@ -1,5 +1,5 @@
 """Dev helper: config-3 (or, with AB_CONFIG=c4, config-4) fit under several context environments in one process (same inputs), e.g.
-    python tools/ab_env.py 50000 3 g8: g16:PB200_GROUP=16 g32:PB200_GROUP=32 tab32:PB200_GROUP=0 notab:PB200_NO_TAB=1
+    python tools/ab_env.py 50000 3 g8: g16:PB200_GROUP=16 tab32:PB200_GROUP=0 notab:PB200_NO_TAB=1
 prints timings, the kernel-variant counts and how the results compare with the first configuration."""
 import sys, os, time
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
@@ -8,7 +8,7 @@ from time_series_spark_b200 import synth, batched, _lib as L
 n = int(sys.argv[1]) if len(sys.argv) > 1 else 50000
 reps = int(sys.argv[2]) if len(sys.argv) > 2 else 3
 specs = sys.argv[3:] or ["base:"]
-KNOWN = ("PB200_NO_TAB", "PB200_GROUP", "PB200_GRP_PAD", "PB200_PLAIN_GROUP", "PB200_LC0_MAX", "PB200_LC1_MAX")
+KNOWN = ("PB200_NO_TAB", "PB200_GROUP", "PB200_GRP_PAD", "PB200_PLAIN_GROUP", "PB200_LC0_MAX")
 cfg = os.environ.get("AB_CONFIG", "c3")          # c3 (50k x 1440 shape) or c4 (short ragged series, no seasonality)
 b = synth.config4(n=n) if cfg == "c4" else synth.config3(n=n); opts = batched.make_options()
 mask = 0 if cfg == "c4" else 6
