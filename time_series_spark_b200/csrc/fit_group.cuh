@@ -12,10 +12,11 @@
 //   * every lane owns T / G contiguous points of ITS series; the point loop is the same instruction
 //     stream for all lanes, so the groups of a warp stay converged through an evaluation;
 //   * vectors live G-strided (element q on lane q mod G), trend segments blocked (32 / G per lane), and
-//     reductions / scans are log2(G) shuffle steps on the group's lane mask;
+//     reductions / scans are log2(G) shuffle steps within the group, under the full warp mask;
 //   * the groups of a warp run the optimiser's state machine in lockstep at evaluation granularity:
-//     [fetch + stage a series if idle] -> evaluate -> line-search step -> (accepted: update + new direction);
-//     a group whose action differs simply sits out that routine.
+//     [fetch + stage a series if idle] -> evaluate -> line-search step -> (accepted: update) -> new search / trial point;
+//     the whole warp runs every routine of a round, and a group whose action differs (or an idle one) computes on its
+//     own slot's state and stores nothing.
 // Data layout per series slot: global workspace: y_scaled in steps of U points per lane (U = 2; 4 was measured and lost),
 // step m of lane l at ((m G + l) U) doubles (a lane's cp.async is 16 B, a group's G lanes read 8 U G contiguous bytes), and the
 // L-BFGS history Y[5], S[5] (read once per iteration); shared memory (GState): optimiser state, the six
@@ -201,58 +202,61 @@ __device__ unsigned long long g_phase_cycles[PC_N];
 #define PB200_PCLK_ADD(ph, v, cond)
 #endif
 
-// ---- group collectives (lanes of one series; `gm` is the group's lane mask) ----
+// ---- group collectives (lanes of one series).  The whole warp calls them: every shuffle runs under the full mask, with
+// offsets below G (xor) or width G (scans), so that each group sees only its own lanes.  A group's lane mask is a run-time
+// value, and a shuffle under it would first compile to a convergence test and a collective fallback ----
 template <int G>
-__device__ __forceinline__ double gsum(double v, const unsigned gm) {
+__device__ __forceinline__ double gsum(double v) {
 #pragma unroll
-    for (int o = G / 2; o >= 1; o >>= 1) v += __shfl_xor_sync(gm, v, o);
+    for (int o = G / 2; o >= 1; o >>= 1) v += __shfl_xor_sync(FULL, v, o);
     return v;
 }
 template <int G>
-__device__ __forceinline__ double gmax(double v, const unsigned gm) {
+__device__ __forceinline__ double gmax(double v) {
 #pragma unroll
-    for (int o = G / 2; o >= 1; o >>= 1) v = fmax(v, __shfl_xor_sync(gm, v, o));
+    for (int o = G / 2; o >= 1; o >>= 1) v = fmax(v, __shfl_xor_sync(FULL, v, o));
     return v;
 }
 // sum of v over the lower lanes of the group (exclusive prefix); *tot = the group total
 template <int G>
-__device__ __forceinline__ double gscan_excl(double v, const int gl, const unsigned gm, double* tot) {
+__device__ __forceinline__ double gscan_excl(double v, const int gl, double* tot) {
     double inc = v;
 #pragma unroll
     for (int o = 1; o < G; o <<= 1) {
-        const double a = __shfl_up_sync(gm, inc, o, G);
+        const double a = __shfl_up_sync(FULL, inc, o, G);
         if (gl >= o) inc += a;
     }
-    if (tot) *tot = __shfl_sync(gm, inc, G - 1, G);
+    if (tot) *tot = __shfl_sync(FULL, inc, G - 1, G);
     return inc - v;
 }
 // sum of v over the HIGHER lanes of the group
 template <int G>
-__device__ __forceinline__ double gscan_excl_rev(double v, const int gl, const unsigned gm) {
+__device__ __forceinline__ double gscan_excl_rev(double v, const int gl) {
     double inc = v;
 #pragma unroll
     for (int o = 1; o < G; o <<= 1) {
-        const double a = __shfl_down_sync(gm, inc, o, G);
+        const double a = __shfl_down_sync(FULL, inc, o, G);
         if (gl + o < G) inc += a;
     }
     return inc - v;
 }
 template <int G, int PPAD>
-__device__ __noinline__ double gvdot(const double* a, const double* b, const int P, const int gl, const unsigned gm) {
+__device__ __forceinline__ double gvdot(const double* a, const double* b, const int P, const int gl) {
     double s = 0.0;
 #pragma unroll
     for (int u = 0; u < (PPAD + G - 1) / G; ++u) {
         const int q = gl + u * G;
         if (q < P) s = fma(a[q], b[q], s);
     }
-    return gsum<G>(s, gm);
+    return gsum<G>(s);
 }
 
 // ---------------------------------------------------------------------------------------
-// evaluation, part 1: trend segments of theta (rate, offset, per-step exp ratio), sigma, beta
+// evaluation, part 1: trend segments of theta (rate, offset, per-step exp ratio), sigma, beta.  The whole warp calls it;
+// an idle group (`active` false) computes on its own slot's state and stores nothing
 // ---------------------------------------------------------------------------------------
 template <int G, bool LOGI, bool SEAS>
-__device__ __noinline__ void g_eval_setup(GState<G, SEAS>& s, const double* xv, const int gl, const unsigned gm) {
+__device__ __noinline__ void g_eval_setup(GState<G, SEAS>& s, const double* xv, const int gl, const bool active) {
     constexpr int NS = GSEG / G;
     const int S = s.S, jb = gl * NS;
     const double k = xv[0], m = xv[1];
@@ -267,11 +271,11 @@ __device__ __noinline__ void g_eval_setup(GState<G, SEAS>& s, const double* xv, 
         run += d[u];
         if constexpr (!LOGI) { pree[u] = rune; rune = fma(-tcl[u], d[u], rune); }
     }
-    const double ex = gscan_excl<G>(run, gl, gm, nullptr);
+    const double ex = gscan_excl<G>(run, gl, nullptr);
 #pragma unroll
     for (int u = 0; u < NS; ++u) kcl[u] = k + (ex + pre[u]);
-    kcl[NS] = __shfl_down_sync(gm, kcl[0], 1, G);                 // first rate of the next lane's block
-    if (gl == 0) s.sigma = exp_fastpath(xv[2 + S]);
+    kcl[NS] = __shfl_down_sync(FULL, kcl[0], 1, G);               // first rate of the next lane's block
+    if (active && gl == 0) s.sigma = exp_fastpath(xv[2 + S]);
     double mcl[NS + 1];
     if constexpr (LOGI) {
         // logistic_gamma: m_{j+1} = rho_j m_j + (1 - rho_j) t_change_j, rho_j = k_j / k_{j+1}
@@ -288,11 +292,11 @@ __device__ __noinline__ void g_eval_setup(GState<G, SEAS>& s, const double* xv, 
         double Ai = A, Bi = B;                                     // inclusive scan of the block maps
 #pragma unroll
         for (int o = 1; o < G; o <<= 1) {
-            const double Ap = __shfl_up_sync(gm, Ai, o, G);
-            const double Bp = __shfl_up_sync(gm, Bi, o, G);
+            const double Ap = __shfl_up_sync(FULL, Ai, o, G);
+            const double Bp = __shfl_up_sync(FULL, Bi, o, G);
             if (gl >= o) { Bi = fma(Ai, Bp, Bi); Ai = Ai * Ap; }
         }
-        double Ae = __shfl_up_sync(gm, Ai, 1, G), Be = __shfl_up_sync(gm, Bi, 1, G);
+        double Ae = __shfl_up_sync(FULL, Ai, 1, G), Be = __shfl_up_sync(FULL, Bi, 1, G);
         if (gl == 0) { Ae = 1.0; Be = 0.0; }
         mcl[0] = fma(Ae, m, Be);
 #pragma unroll
@@ -303,9 +307,11 @@ __device__ __noinline__ void g_eval_setup(GState<G, SEAS>& s, const double* xv, 
         for (int u = 0; u < NS; ++u) {
             const int j = jb + u;
             if (j <= S) {
-                s.kc[j] = kcl[u];
-                s.mc[j] = mcl[u];
-                s.qs[j] = exp_fastpath(-(kcl[u] * h));
+                if (active) {
+                    s.kc[j] = kcl[u];
+                    s.mc[j] = mcl[u];
+                    s.qs[j] = exp_fastpath(-(kcl[u] * h));
+                }
                 // the exponent k_j (t - m_j) is piecewise linear in t: its extremes sit at the segment ends
                 const double tl = j == 0 ? -h : s.tc[j - 1];
                 const double tr = j == S ? 1.0 : tcl[u];
@@ -314,23 +320,23 @@ __device__ __noinline__ void g_eval_setup(GState<G, SEAS>& s, const double* xv, 
                 if (!(fabs(z0) < 600.0) || !(fabs(z1) < 600.0)) zm = 1e300;   // NaN too
             }
         }
-        zm = gmax<G>(zm, gm);
-        if (gl == 0) s.exprec = zm < 600.0 ? 1 : 0;
+        zm = gmax<G>(zm);
+        if (active && gl == 0) s.exprec = zm < 600.0 ? 1 : 0;
     } else {
-        const double exe = gscan_excl<G>(rune, gl, gm, nullptr);
+        const double exe = gscan_excl<G>(rune, gl, nullptr);
 #pragma unroll
         for (int u = 0; u < NS; ++u) {
             const int j = jb + u;
-            if (j <= S) { s.kc[j] = kcl[u]; s.mc[j] = m + (exe + pree[u]); }
+            if (active && j <= S) { s.kc[j] = kcl[u]; s.mc[j] = m + (exe + pree[u]); }
         }
-        if (gl == 0) s.exprec = 0;
+        if (active && gl == 0) s.exprec = 0;
     }
 #pragma unroll
     for (int u = 0; u < (gkx<SEAS>() + G - 1) / G; ++u) {
         const int q = gl + u * G;
-        if (q < gkx<SEAS>()) s.bcoef[q] = xv[3 + S + q];
+        if (active && q < gkx<SEAS>()) s.bcoef[q] = xv[3 + S + q];
     }
-    __syncwarp(gm);
+    __syncwarp();
 }
 
 // features of table phase p from the (sin, cos) of the daily angle
@@ -377,7 +383,7 @@ struct GPoint {
 // ---------------------------------------------------------------------------------------
 template <int G, bool LOGI, bool MULT, bool SEAS, int U>
 __device__ __noinline__ void g_point_pass(GState<G, SEAS>& s, const double* plane, const bool active, const int gl, const int lane,
-                                          const unsigned gm, const LanePhase lp, const int l2f) {
+                                          const LanePhase lp, const int l2f) {
     static_assert(U == 2 || U == 4, "points per lane per step");
     const int P = active ? s.tabP : GState<G, SEAS>::PT, PL = active ? s.tabPL : 0;     // (an idle group's lanes only keep step)
     const double2 rct = *reinterpret_cast<const double2*>(s.rotd);
@@ -675,7 +681,7 @@ __device__ __noinline__ void g_point_pass(GState<G, SEAS>& s, const double* plan
     }
     // boundaries recorded by this lane get the sums of the lanes before it; totals to slot S
     double totU, totV;
-    const double exU = gscan_excl<G>(locU, gl, gm, &totU), exV = gscan_excl<G>(locV, gl, gm, &totV);
+    const double exU = gscan_excl<G>(locU, gl, &totU), exV = gscan_excl<G>(locV, gl, &totV);
     if (active) {
 #pragma unroll 1
         for (int q = j0; q < j; ++q) {
@@ -687,7 +693,7 @@ __device__ __noinline__ void g_point_pass(GState<G, SEAS>& s, const double* plan
     __syncwarp();
     if constexpr (!SEAS) {
         // only the residual sum of squares to total; the zero column's gradient sum is zero
-        ss = gsum<G>(ss, gm);
+        ss = gsum<G>(ss);
         double* scr = s.stab;                                   // (stab and rtab are contiguous: value v at scr[v])
         if (active && gl == 0) { scr[0] = 0.0; scr[GState<G, SEAS>::TOTSS] = ss; }
         __syncwarp();
@@ -743,11 +749,13 @@ __device__ __noinline__ void g_point_pass(GState<G, SEAS>& s, const double* plan
 }
 
 // ---------------------------------------------------------------------------------------
-// evaluation, part 3: objective value and gradient from the pass's sums; returns err (group-uniform)
+// evaluation, part 3: objective value and gradient from the pass's sums; returns err (group-uniform).  The whole warp calls
+// it; an idle group (`active` false) computes on its own slot's state and stores nothing.  `gm`: the group's lane mask
 // ---------------------------------------------------------------------------------------
 template <int G, bool LOGI, bool SEAS>
 __device__ __noinline__ int g_eval_finalize(GState<G, SEAS>& s, const double* xv, double* gv, const int gl, const unsigned gm,
-                                            const double tau, const double rtau, const double inv_seas2, double* f_out) {
+                                            const bool active, const double tau, const double rtau, const double inv_seas2,
+                                            double* f_out) {
     constexpr int NS = GSEG / G;
     const int S = s.S, T = s.T, jb = gl * NS;
     const double* tot = s.stab;                     // value v of the pass: tot[v], v < 14 beta sums, tot[14] = ss
@@ -780,7 +788,7 @@ __device__ __noinline__ int g_eval_finalize(GState<G, SEAS>& s, const double* xv
             Gkc[u] = j <= S ? scale * (PU[u + 1] - PU[u]) : 0.0;
             Gmc[u] = j <= S ? scale * (-kcl[u]) * (PV[u + 1] - PV[u]) : 0.0;
         }
-        kcl[NS] = __shfl_down_sync(gm, kcl[0], 1, G);
+        kcl[NS] = __shfl_down_sync(FULL, kcl[0], 1, G);
         if (jb + NS > S) kcl[NS] = 1.0;
 #pragma unroll
         for (int u = 0; u < NS; ++u)
@@ -800,12 +808,12 @@ __device__ __noinline__ int g_eval_finalize(GState<G, SEAS>& s, const double* xv
         double Ai = A, Bi = B;
 #pragma unroll
         for (int o = 1; o < G; o <<= 1) {
-            const double An = __shfl_down_sync(gm, Ai, o, G);
-            const double Bn = __shfl_down_sync(gm, Bi, o, G);
+            const double An = __shfl_down_sync(FULL, Ai, o, G);
+            const double Bn = __shfl_down_sync(FULL, Bi, o, G);
             if (gl + o < G) { Bi = fma(Ai, Bn, Bi); Ai = Ai * An; }
         }
         // value entering this block from above = (inclusive map of the next lane)(0)
-        double xin = __shfl_down_sync(gm, Bi, 1, G);
+        double xin = __shfl_down_sync(FULL, Bi, 1, G);
         if (gl == G - 1) xin = 0.0;
         double ab[NS + 1];
         ab[NS] = xin;
@@ -822,7 +830,7 @@ __device__ __noinline__ int g_eval_finalize(GState<G, SEAS>& s, const double* xv
             t2[u] = j < S ? div_const(-(rb * rhl[u]), kcl[u + 1], rk) : 0.0;
             kbar[u] = j <= S ? Gkc[u] + t1 : 0.0;
         }
-        double t2prev = __shfl_up_sync(gm, t2[NS - 1], 1, G);
+        double t2prev = __shfl_up_sync(FULL, t2[NS - 1], 1, G);
         if (gl == 0) t2prev = 0.0;
 #pragma unroll
         for (int u = 0; u < NS; ++u) {
@@ -833,7 +841,7 @@ __device__ __noinline__ int g_eval_finalize(GState<G, SEAS>& s, const double* xv
         double suf[NS + 1], run = 0.0;
 #pragma unroll
         for (int u = NS - 1; u >= 0; --u) { run += kbar[u]; suf[u] = run; }
-        const double above = gscan_excl_rev<G>(run, gl, gm);
+        const double above = gscan_excl_rev<G>(run, gl);
         suf[NS] = 0.0;
 #pragma unroll
         for (int u = 0; u < NS; ++u) {
@@ -842,13 +850,13 @@ __device__ __noinline__ int g_eval_finalize(GState<G, SEAS>& s, const double* xv
                 const double d = xv[2 + j];
                 const double sg = d > 0.0 ? 1.0 : (d < 0.0 ? -1.0 : 0.0);
                 const double gd = (above + suf[u + 1]) + div_const(sg, tau, rtau);
-                gv[2 + j] = gd;
+                if (active) gv[2 + j] = gd;
                 if (!isfinite(gd)) bad = 1;
                 ad_part += fabs(d);
             }
         }
         kb_part = run;
-        gm_ = __shfl_sync(gm, ab[0], 0, G) + div_const(m, 25.0, 0.04);
+        gm_ = __shfl_sync(FULL, ab[0], 0, G) + div_const(m, 25.0, 0.04);
     } else {
 #pragma unroll
         for (int u = 0; u < NS; ++u) {
@@ -857,7 +865,7 @@ __device__ __noinline__ int g_eval_finalize(GState<G, SEAS>& s, const double* xv
                 const double d = xv[2 + j];
                 const double sg = d > 0.0 ? 1.0 : (d < 0.0 ? -1.0 : 0.0);
                 const double gd = scale * ((totU - s.bndU[j]) - s.tc[j] * (totV - s.bndV[j])) + div_const(sg, tau, rtau);
-                gv[2 + j] = gd;
+                if (active) gv[2 + j] = gd;
                 if (!isfinite(gd)) bad = 1;
                 ad_part += fabs(d);
             }
@@ -872,169 +880,180 @@ __device__ __noinline__ int g_eval_finalize(GState<G, SEAS>& s, const double* xv
         if (q < gkx<SEAS>()) {
             const double b = xv[3 + S + q];
             const double gb = scale * tot[q] + b * inv_seas2;
-            gv[3 + S + q] = gb;
+            if (active) gv[3 + S + q] = gb;
             pb += 0.5 * b * b * inv_seas2;
             if (!isfinite(gb)) bad = 1;
         }
     }
-    const double kb_sum = gsum<G>(kb_part, gm), pb_sum = gsum<G>(pb, gm), ad = gsum<G>(ad_part, gm);
+    const double kb_sum = gsum<G>(kb_part), pb_sum = gsum<G>(pb), ad = gsum<G>(ad_part);
     const double k25 = div_const(k, 25.0, 0.04);
     const double gk = LOGI ? kb_sum + k25 : scale * totU + k25;
     const double gu = -ss * inv_s2 + (double)T + 4.0 * sigma * sigma;
     const double f = 0.5 * ss * inv_s2 + (double)T * u_ + div_const(k * k, 50.0, 0.02) + div_const(m * m, 50.0, 0.02) +
                      div_const(ad, tau, rtau) + 2.0 * sigma * sigma + pb_sum;
     if (gl == 0) {
-        gv[0] = gk; gv[1] = gm_; gv[2 + S] = gu;
+        if (active) { gv[0] = gk; gv[1] = gm_; gv[2 + S] = gu; }
         if (!isfinite(gk) || !isfinite(gm_) || !isfinite(gu)) bad = 1;
     }
     if (!isfinite(f) || !(sigma > 0.0) || !isfinite(sigma)) bad = 1;
-    bad = __any_sync(gm, bad);
-    __syncwarp(gm);
-    if (gl == 0) *f_out = f;
-    __syncwarp(gm);
+    bad = (__ballot_sync(FULL, bad) & gm) != 0;
+    if (active && gl == 0) *f_out = f;             // (nothing here reads it: the caller's __syncwarp publishes it)
     return bad;
 }
 
 // ---------------------------------------------------------------------------------------
-// Stan's L-BFGS over the group's LSState (see fit_kernel.cuh for the routine-by-routine mapping)
+// Stan's L-BFGS over the group's LSState (see fit_kernel.cuh for the routine-by-routine mapping).  The whole warp calls
+// each routine once per round, and a group's action is a register value: every group computes the routine's dot products
+// under the full mask, and only the groups whose action uses one keep it.  A routine reads the LSState scalars once, and
+// lane 0 stores the new ones once, behind one __syncwarp (the lanes of its group have read the old ones by then)
 // ---------------------------------------------------------------------------------------
-template <int G, bool SEAS>
-__device__ __noinline__ void g_make_trial(GState<G, SEAS>& s, const double alpha, const int P, const int gl, const unsigned gm) {
-    const double* x = s.vec[s.ls.ix];
-    const double* p = s.vec[s.ls.ip];
-    double* xt = s.vec[s.ls.ixt];
-#pragma unroll
-    for (int u = 0; u < (GState<G, SEAS>::PPAD + G - 1) / G; ++u) {
-        const int q = gl + u * G;
-        if (q < P) xt[q] = x[q] + alpha * p[q];
-    }
-    __syncwarp(gm);
-}
+// actions besides fit_kernel.cuh's ACT_EVAL / ACT_ACCEPT / ACT_FAIL: none (idle, or done this round), and the three ways
+// into a new line search: the first iteration, the retry from a reset Hessian after a failed search, the next iteration
+// after an accepted one
+constexpr int ACT_NONE = -1, ACT_BEGIN_FIRST = ACT_FAIL + 1, ACT_BEGIN_RETRY = ACT_FAIL + 2, ACT_BEGIN_NEXT = ACT_FAIL + 3;
 
-template <int G, bool SEAS>
-__device__ __noinline__ void g_ls_begin(GState<G, SEAS>& s, const int gl, const unsigned gm, const int P, const double init_alpha) {
-    LSState& ls = s.ls;
-    const double minAlpha = 1e-12;
-    const double* g = s.vec[ls.ig];
-    double* p = s.vec[ls.ip];
-    if (ls.resetB) {
-#pragma unroll
-        for (int u = 0; u < (GState<G, SEAS>::PPAD + G - 1) / G; ++u) {
-            const int q = gl + u * G;
-            if (q < P) p[q] = -g[q];
-        }
-        __syncwarp(gm);
-    }
-    const double dfp = gvdot<G, GState<G, SEAS>::PPAD>(g, p, P, gl, gm);
+// WolfeLineSearch / WolfLSZoom after the evaluation at the trial point.  Groups that are not in a line search (`search`
+// false) return ACT_NONE.  ACT_EVAL: alpha is the step of the next trial point, which g_ls_begin forms.  (Returned by value:
+// an out-pointer to the caller's register would put it on the stack)
+struct LsStep {
+    int act;
     double alpha;
-    if (ls.iters > 1 && ls.resetB != 2) {
-        const double dprev = gvdot<G, GState<G, SEAS>::PPAD>(s.vec[ls.igt], s.vec[ls.ipp], P, gl, gm);
-        alpha = fmin(1.0, 1.01 * cubic_interp(dprev, ls.alphak_1, ls.fk - ls.fk_1, dfp, minAlpha, 1.0));
-    } else {
-        alpha = init_alpha;
-    }
-    __syncwarp(gm);
-    if (gl == 0) {
-        ls.dfp = dfp; ls.alpha = alpha; ls.alpha0 = minAlpha; ls.prevF = ls.fk; ls.prevDFp = dfp;
-        ls.nits = 0; ls.lsRestarts = 0; ls.phase = PH_LS;
-    }
-    __syncwarp(gm);
-    g_make_trial<G, SEAS>(s, alpha, P, gl, gm);
-}
-
+};
 template <int G, bool SEAS>
-__device__ __noinline__ int g_ls_step(GState<G, SEAS>& s, const int gl, const unsigned gm, const int P, const int err) {
+__device__ __noinline__ LsStep g_ls_step(GState<G, SEAS>& s, const int gl, const bool search, const int P, const int err) {
     LSState& ls = s.ls;
     const double c1 = 1e-4, c2 = 0.9, min_range = 1e-16;
     const int maxLSIts = 20, maxLSRestarts = 10;
+    // the directional derivative at the trial point (the groups with err, or not searching, discard it)
+    const double newDFp = gvdot<G, GState<G, SEAS>::PPAD>(s.vec[ls.igt], s.vec[ls.ip], P, gl);
     const double fk = ls.fk, ft = ls.ft, dfp = ls.dfp;
     const double c1dfp = c1 * dfp, c2dfp = c2 * dfp;
-    double alpha = ls.alpha;
+    double alpha = ls.alpha, alpha0 = ls.alpha0, prevF = ls.prevF, prevDFp = ls.prevDFp;
     double alo = ls.alo, aloF = ls.aloF, aloD = ls.aloD, ahi = ls.ahi, ahiF = ls.ahiF, ahiD = ls.ahiD;
-    int itNum = ls.itNum;
-    if (ls.phase == PH_LS) {
-        // ---------------- WolfeLineSearch ----------------
-        const double alpha0 = ls.alpha0, prevF = ls.prevF, prevDFp = ls.prevDFp;
-        const int nits = ls.nits;
-        if (err) {
-            if (ls.lsRestarts >= maxLSRestarts) return ACT_FAIL;
-            alpha = 0.5 * (alpha0 + alpha);
-            __syncwarp(gm);
-            if (gl == 0) { ls.alpha = alpha; ls.lsRestarts += 1; }
-            __syncwarp(gm);
-            g_make_trial<G, SEAS>(s, alpha, P, gl, gm);
-            return ACT_EVAL;
-        }
-        const double newDFp = gvdot<G, GState<G, SEAS>::PPAD>(s.vec[ls.igt], s.vec[ls.ip], P, gl, gm);
-        if (ft > fk + alpha * c1dfp || (ft >= prevF && nits > 0)) {
-            alo = alpha0; aloF = prevF; aloD = prevDFp;
-            ahi = alpha; ahiF = ft; ahiD = newDFp;
-        } else if (fabs(newDFp) <= -c2dfp) {
-            return ACT_ACCEPT;
-        } else if (newDFp >= 0) {
-            alo = alpha; aloF = ft; aloD = newDFp;
-            ahi = alpha0; ahiF = prevF; ahiD = prevDFp;
-        } else {
-            if (nits + 1 >= maxLSIts) return ACT_FAIL;
-            const double a10 = alpha * 10.0;
-            __syncwarp(gm);
-            if (gl == 0) {
-                ls.alpha0 = alpha; ls.prevF = ft; ls.prevDFp = newDFp; ls.alpha = a10; ls.nits = nits + 1;
-                ls.lsRestarts = 0;
+    int itNum = ls.itNum, nits = ls.nits, lsRestarts = ls.lsRestarts, phase = ls.phase;
+    // Stan's decisions on the local copies; every ACT_EVAL leaves the new state in them
+    auto decide = [&]() -> int {
+        if (phase == PH_LS) {
+            // ---------------- WolfeLineSearch ----------------
+            if (err) {
+                if (lsRestarts >= maxLSRestarts) return ACT_FAIL;
+                alpha = 0.5 * (alpha0 + alpha);
+                lsRestarts += 1;
+                return ACT_EVAL;
             }
-            __syncwarp(gm);
-            g_make_trial<G, SEAS>(s, a10, P, gl, gm);
-            return ACT_EVAL;
-        }
-        itNum = 0;
-    } else {
-        // ---------------- WolfLSZoom: result of the evaluation at alpha ----------------
-        if (err) {
-            const double lo = fmin(alo, ahi);
-            alpha = 0.5 * (alpha + lo);
-            if (fabs(lo - alpha) < min_range) return ACT_FAIL;
-            __syncwarp(gm);
-            if (gl == 0) ls.alpha = alpha;
-            __syncwarp(gm);
-            g_make_trial<G, SEAS>(s, alpha, P, gl, gm);
-            return ACT_EVAL;
-        }
-        const double newDFp = gvdot<G, GState<G, SEAS>::PPAD>(s.vec[ls.igt], s.vec[ls.ip], P, gl, gm);
-        if (ft > (fk + alpha * c1dfp) || ft >= aloF) {
-            ahi = alpha; ahiF = ft; ahiD = newDFp;
+            if (ft > fk + alpha * c1dfp || (ft >= prevF && nits > 0)) {
+                alo = alpha0; aloF = prevF; aloD = prevDFp;
+                ahi = alpha; ahiF = ft; ahiD = newDFp;
+            } else if (fabs(newDFp) <= -c2dfp) {
+                return ACT_ACCEPT;
+            } else if (newDFp >= 0) {
+                alo = alpha; aloF = ft; aloD = newDFp;
+                ahi = alpha0; ahiF = prevF; ahiD = prevDFp;
+            } else {
+                if (nits + 1 >= maxLSIts) return ACT_FAIL;
+                const double a10 = alpha * 10.0;
+                alpha0 = alpha; prevF = ft; prevDFp = newDFp; alpha = a10; nits += 1;
+                lsRestarts = 0;
+                return ACT_EVAL;
+            }
+            itNum = 0;
         } else {
-            if (fabs(newDFp) <= -c2dfp) return ACT_ACCEPT;
-            if (newDFp * (ahi - alo) >= 0) { ahi = alo; ahiF = aloF; ahiD = aloD; }
-            alo = alpha; aloF = ft; aloD = newDFp;
+            // ---------------- WolfLSZoom: result of the evaluation at alpha ----------------
+            if (err) {
+                const double lo = fmin(alo, ahi);
+                alpha = 0.5 * (alpha + lo);
+                if (fabs(lo - alpha) < min_range) return ACT_FAIL;
+                return ACT_EVAL;
+            }
+            if (ft > (fk + alpha * c1dfp) || ft >= aloF) {
+                ahi = alpha; ahiF = ft; ahiD = newDFp;
+            } else {
+                if (fabs(newDFp) <= -c2dfp) return ACT_ACCEPT;
+                if (newDFp * (ahi - alo) >= 0) { ahi = alo; ahiF = aloF; ahiD = aloD; }
+                alo = alpha; aloF = ft; aloD = newDFp;
+            }
+        }
+        // ---------------- WolfLSZoom: next trial step ----------------
+        ++itNum;
+        if (fabs(alo - ahi) < min_range) return ACT_FAIL;
+        {
+            // [guard, not in Stan] bracket = two adjacent doubles wider than min_range (see fit_kernel.cuh)
+            const double mid = 0.5 * (alo + ahi);
+            if (mid == alo || mid == ahi) return ACT_FAIL;
+        }
+        if (itNum % 5 == 0) {
+            alpha = 0.5 * (alo + ahi);
+        } else {
+            const double d1 = aloD + ahiD - fdiv(3 * (aloF - ahiF), alo - ahi);
+            double d2 = sqrt(d1 * d1 - aloD * ahiD);
+            if (ahi < alo) d2 = -d2;
+            alpha = ahi - fdiv((ahi - alo) * (ahiD + d2 - d1), ahiD - aloD + 2 * d2);
+            const double lo = fmin(alo, ahi), hi = fmax(alo, ahi);
+            if (!isfinite(alpha) || alpha < lo + 0.01 * fabs(alo - ahi) || alpha > hi - 0.01 * fabs(alo - ahi))
+                alpha = 0.5 * (alo + ahi);
+        }
+        phase = PH_ZOOM;
+        return ACT_EVAL;
+    };
+    const int act = search ? decide() : ACT_NONE;
+    __syncwarp();
+    if (act == ACT_EVAL && gl == 0) {          // (fields a branch leaves alone are stored back unchanged)
+        ls.alpha = alpha; ls.alpha0 = alpha0; ls.prevF = prevF; ls.prevDFp = prevDFp;
+        ls.alo = alo; ls.aloF = aloF; ls.aloD = aloD; ls.ahi = ahi; ls.ahiF = ahiF; ls.ahiD = ahiD;
+        ls.itNum = itNum; ls.nits = nits; ls.lsRestarts = lsRestarts; ls.phase = phase;
+    }
+    return {act, alpha};
+}
+
+// A new line search for the groups that start one (act ACT_BEGIN_*): the direction is -g after a reset Hessian, and the
+// initial step comes from Stan's cubic interpolation over the previous iteration.  Then the trial point x + alpha p of
+// every group that evaluates one next: those groups and the ACT_EVAL ones (alpha = talpha)
+template <int G, bool SEAS>
+__device__ __noinline__ void g_ls_begin(GState<G, SEAS>& s, const int gl, const int P, const double init_alpha, const int act,
+                                        const double talpha) {
+    constexpr int NV = (GState<G, SEAS>::PPAD + G - 1) / G;
+    LSState& ls = s.ls;
+    const double minAlpha = 1e-12;
+    const bool begin = act >= ACT_BEGIN_FIRST, trial = begin || act == ACT_EVAL;
+    const int iters = act == ACT_BEGIN_FIRST ? 1 : (act == ACT_BEGIN_NEXT ? ls.iters + 1 : ls.iters);
+    const int resetB = act == ACT_BEGIN_FIRST ? 1 : (act == ACT_BEGIN_RETRY ? 2 : (act == ACT_BEGIN_NEXT ? 0 : ls.resetB));
+    const double fk = ls.fk;
+    const double* x = s.vec[ls.ix];
+    const double* g = s.vec[ls.ig];
+    double* p = s.vec[ls.ip];
+    double* xt = s.vec[ls.ixt];
+    const bool neg = begin && resetB != 0;                 // the direction starts over at -g
+    double pv[NV], l = 0.0;
+#pragma unroll
+    for (int u = 0; u < NV; ++u) {
+        const int q = gl + u * G;
+        pv[u] = 0.0;
+        if (q < P) {
+            pv[u] = neg ? -g[q] : p[q];
+            l = fma(g[q], pv[u], l);
         }
     }
-    // ---------------- WolfLSZoom: next trial step ----------------
-    ++itNum;
-    if (fabs(alo - ahi) < min_range) return ACT_FAIL;
-    {
-        // [guard, not in Stan] bracket = two adjacent doubles wider than min_range (see fit_kernel.cuh)
-        const double mid = 0.5 * (alo + ahi);
-        if (mid == alo || mid == ahi) return ACT_FAIL;
+    const double dfp = gsum<G>(l);
+    const double dprev = gvdot<G, GState<G, SEAS>::PPAD>(s.vec[ls.igt], s.vec[ls.ipp], P, gl);
+    double alpha = talpha;
+    if (begin) {
+        if (iters > 1 && resetB != 2) alpha = fmin(1.0, 1.01 * cubic_interp(dprev, ls.alphak_1, fk - ls.fk_1, dfp, minAlpha, 1.0));
+        else alpha = init_alpha;
     }
-    if (itNum % 5 == 0) {
-        alpha = 0.5 * (alo + ahi);
-    } else {
-        const double d1 = aloD + ahiD - fdiv(3 * (aloF - ahiF), alo - ahi);
-        double d2 = sqrt(d1 * d1 - aloD * ahiD);
-        if (ahi < alo) d2 = -d2;
-        alpha = ahi - fdiv((ahi - alo) * (ahiD + d2 - d1), ahiD - aloD + 2 * d2);
-        const double lo = fmin(alo, ahi), hi = fmax(alo, ahi);
-        if (!isfinite(alpha) || alpha < lo + 0.01 * fabs(alo - ahi) || alpha > hi - 0.01 * fabs(alo - ahi))
-            alpha = 0.5 * (alo + ahi);
+#pragma unroll
+    for (int u = 0; u < NV; ++u) {
+        const int q = gl + u * G;
+        if (trial && q < P) {
+            if (neg) p[q] = pv[u];
+            xt[q] = x[q] + alpha * pv[u];
+        }
     }
-    __syncwarp(gm);
-    if (gl == 0) {
-        ls.phase = PH_ZOOM; ls.itNum = itNum; ls.alpha = alpha;
-        ls.alo = alo; ls.aloF = aloF; ls.aloD = aloD; ls.ahi = ahi; ls.ahiF = ahiF; ls.ahiD = ahiD;
+    __syncwarp();
+    if (begin && gl == 0) {
+        ls.dfp = dfp; ls.alpha = alpha; ls.alpha0 = minAlpha; ls.prevF = fk; ls.prevDFp = dfp;
+        ls.nits = 0; ls.lsRestarts = 0; ls.phase = PH_LS; ls.iters = iters; ls.resetB = resetB;
+        if (act == ACT_BEGIN_FIRST) s.state = ST_SEARCH;
     }
-    __syncwarp(gm);
-    g_make_trial<G, SEAS>(s, alpha, P, gl, gm);
-    return ACT_EVAL;
 }
 
 // the rest of BFGSMinimizer::step after an accepted line search; history Y[5], S[5] in global memory `hist`.
@@ -1111,9 +1130,9 @@ __device__ __noinline__ int g_post_accept(GState<G, SEAS>& s, double* hist, cons
         nrm0 = fma(sv, yv, nrm0); nrm1 = fma(yv, yv, nrm1);
         nrm2 = fma(sv, sv, nrm2); nrm3 = fma(gq[u], gq[u], nrm3);
     }
-    const double skyk = gsum<G>(nrm0, FULL), ykyk = gsum<G>(nrm1, FULL);
-    const double stepNorm = sqrt(gsum<G>(nrm2, FULL));
-    const double gradNorm = sqrt(gsum<G>(nrm3, FULL));
+    const double skyk = gsum<G>(nrm0), ykyk = gsum<G>(nrm1);
+    const double stepNorm = sqrt(gsum<G>(nrm2));
+    const double gradNorm = sqrt(gsum<G>(nrm3));
     double alphak_1;
     if (resetB) {
         const double B0 = fdiv(ykyk, skyk), rB0 = rcp_any(B0);
@@ -1150,7 +1169,7 @@ __device__ __noinline__ int g_post_accept(GState<G, SEAS>& s, double* hist, cons
         double l = 0.0;
 #pragma unroll
         for (int u = 0; u < NV; ++u) l = fma(sn[u], pv[u], l);
-        aln = rn * gsum<G>(l, FULL);
+        aln = rn * gsum<G>(l);
 #pragma unroll
         for (int u = 0; u < NV; ++u) pv[u] -= aln * yn[u];
     }
@@ -1159,7 +1178,7 @@ __device__ __noinline__ int g_post_accept(GState<G, SEAS>& s, double* hist, cons
         double l = 0.0;
 #pragma unroll
         for (int u = 0; u < NV; ++u) l = fma(hs[h][u], pv[u], l);
-        const double al = hr[h] * gsum<G>(l, FULL);
+        const double al = hr[h] * gsum<G>(l);
         const bool on = h < ho;
 #pragma unroll
         for (int u = 0; u < NV; ++u) pv[u] = on ? pv[u] - al * hy[h][u] : pv[u];
@@ -1172,7 +1191,7 @@ __device__ __noinline__ int g_post_accept(GState<G, SEAS>& s, double* hist, cons
         double l = 0.0;
 #pragma unroll
         for (int u = 0; u < NV; ++u) l = fma(hy[h][u], pv[u], l);
-        const double be = hr[h] * gsum<G>(l, FULL);
+        const double be = hr[h] * gsum<G>(l);
         const double cf = hal[h] - be;
         const bool on = h < ho;
 #pragma unroll
@@ -1182,7 +1201,7 @@ __device__ __noinline__ int g_post_accept(GState<G, SEAS>& s, double* hist, cons
         double l = 0.0;
 #pragma unroll
         for (int u = 0; u < NV; ++u) l = fma(yn[u], pv[u], l);
-        const double be = rn * gsum<G>(l, FULL);
+        const double be = rn * gsum<G>(l);
         const double cf = aln - be;
 #pragma unroll
         for (int u = 0; u < NV; ++u) pv[u] += cf * sn[u];
@@ -1194,7 +1213,7 @@ __device__ __noinline__ int g_post_accept(GState<G, SEAS>& s, double* hist, cons
         if (q < P) p[q] = pv[u];
         gpl = fma(gq[u], pv[u], gpl);
     }
-    const double gp = gsum<G>(gpl, FULL);
+    const double gp = gsum<G>(gpl);
     // ---- convergence tests ----
     const double df = fabs(fk_1 - fk);
     int status = PB200_ST_SUCCESS;
@@ -1426,6 +1445,14 @@ __global__ void __launch_bounds__(32, G != 8 ? 16 : (SEAS ? PB200_GRP_BLOCKS : P
     double* const trace_base = a.trace;
     // (the all-zero column of the class without seasonality has prior scale 1: fbprophet's make_all_seasonality_features)
     const double tau = a.o.tau, rtau = a.o.rtau, inv_seas2 = SEAS ? a.o.inv_seas2 : 1.0;
+    {   // every group's state starts zeroed: the idle groups run the round's routines on it (no trend segments, every vector
+        // role on vec[0]: in bounds), and store nothing
+        constexpr int NZ = (int)(NSER * ((sizeof(GState<G, SEAS>) + 15) & ~(size_t)15) / 16);
+        double2* const z = reinterpret_cast<double2*>(pb200_smem);
+#pragma unroll 1
+        for (int i = lane; i < NZ; i += 32) z[i] = make_double2(0.0, 0.0);
+    }
+    __syncwarp();
     if (gl == 0) { s.state = ST_IDLE; s.series = -1; }
     if (lane == 0) gopts<G, SEAS>() = a.o;
     __syncwarp();
@@ -1476,49 +1503,36 @@ __global__ void __launch_bounds__(32, G != 8 ? 16 : (SEAS ? PB200_GRP_BLOCKS : P
             continue;
         }
         PB200_PCLK_ADD(PC_ROUNDS, 1, lane == 0);
-        // ---- one objective + gradient evaluation per active group ----
+        // ---- one objective + gradient evaluation per active group.  The whole warp runs every routine of the round: the
+        // idle groups compute on their own slot's state and store nothing ----
         const bool first = state == ST_FIRST || state == ST_OBJ;
         const int ixv = first ? s.ls.ix : s.ls.ixt, igv = first ? s.ls.ig : s.ls.igt;
         const int P = s.S + gkx<SEAS>() + 3;
-        if (active) {
-            g_eval_setup<G, LOGI, SEAS>(s, s.vec[ixv], gl, gm);
-            if (gl == 0) s.ls.nevals += 1;
-        }
+        g_eval_setup<G, LOGI, SEAS>(s, s.vec[ixv], gl, active);
+        if (active && gl == 0) s.ls.nevals += 1;
         __syncwarp();
         PB200_PCLK_MARK(PC_SETUP, t_mark, lane);
-        g_point_pass<G, LOGI, MULT, SEAS, grp_u(G)>(s, plane, active, gl, lane, gm, lp, l2f);
+        g_point_pass<G, LOGI, MULT, SEAS, grp_u(G)>(s, plane, active, gl, lane, lp, l2f);
         __syncwarp();
         PB200_PCLK_MARK(PC_PASS, t_mark, lane);
-        int err = 0;
-        if (active) err = g_eval_finalize<G, LOGI, SEAS>(s, s.vec[ixv], s.vec[igv], gl, gm, tau, rtau, inv_seas2, first ? &s.ls.fk : &s.ls.ft);
+        const int err = g_eval_finalize<G, LOGI, SEAS>(s, s.vec[ixv], s.vec[igv], gl, gm, active, tau, rtau, inv_seas2,
+                                                       first ? &s.ls.fk : &s.ls.ft);
         __syncwarp();
         PB200_PCLK_MARK(PC_FINAL, t_mark, lane);
-        // ---- the optimiser's reaction (BFGSMinimizer::step split at its evaluations) ----
-        int act = -1, status = PB200_ST_SUCCESS;
+        // ---- the optimiser's reaction (BFGSMinimizer::step split at its evaluations); `act` carries each group's action
+        // from one routine to the next ----
+        const LsStep lss = g_ls_step<G, SEAS>(s, gl, state == ST_SEARCH, P, err);
+        int act = lss.act, status = PB200_ST_SUCCESS;
         bool done = false;
-        if (state == ST_OBJ) {
+        if (state == ST_OBJ || (state == ST_FIRST && err)) {
             status = err ? PB200_ST_INIT_ERROR : PB200_ST_SUCCESS;
             done = true;
         } else if (state == ST_FIRST) {
-            if (err) { status = PB200_ST_INIT_ERROR; done = true; }
-            else {
-                if (gl == 0) { s.ls.iters = 1; s.ls.resetB = 1; s.state = ST_SEARCH; }
-                __syncwarp(gm);
-                act = ACT_FAIL + 1;                                  // -> ls_begin below
-            }
-        } else if (state == ST_SEARCH) {
-            act = g_ls_step<G, SEAS>(s, gl, gm, P, err);
-        }
-        __syncwarp();
-        if (act == ACT_FAIL) {
+            act = ACT_BEGIN_FIRST;
+        } else if (act == ACT_FAIL) {
             // line search failed: retry once from a reset Hessian, else give up (PyStan raises; fbprophet retries with Newton)
-            if (s.ls.resetB) { status = PB200_ST_LSFAIL; done = true; act = -1; }
-            else {
-                __syncwarp(gm);
-                if (gl == 0) s.ls.resetB = 2;
-                __syncwarp(gm);
-                act = ACT_FAIL + 1;
-            }
+            if (s.ls.resetB) { status = PB200_ST_LSFAIL; done = true; act = ACT_NONE; }
+            else act = ACT_BEGIN_RETRY;
         }
         __syncwarp();
         PB200_PCLK_MARK(PC_LS_STEP, t_mark, lane);
@@ -1536,22 +1550,17 @@ __global__ void __launch_bounds__(32, G != 8 ? 16 : (SEAS ? PB200_GRP_BLOCKS : P
             if (acc) {
                 status = st;
                 if (status != PB200_ST_SUCCESS) done = true;
-                else {
-                    if (gl == 0) { s.ls.iters += 1; s.ls.resetB = 0; }
-                    __syncwarp(gm);
-                    act = ACT_FAIL + 1;
-                }
+                else act = ACT_BEGIN_NEXT;
             }
         }
         __syncwarp();
         PB200_PCLK_MARK(PC_POST, t_mark, lane);
-        if (act == ACT_FAIL + 1) g_ls_begin<G, SEAS>(s, gl, gm, P, init_alpha);
+        g_ls_begin<G, SEAS>(s, gl, P, init_alpha, act, lss.alpha);
         __syncwarp();
         PB200_PCLK_MARK(PC_LS_BEGIN, t_mark, lane);
         if (done) {
             g_write_record<G, SEAS>(s, a, status, gl, gm);
             if (gl == 0) s.state = ST_IDLE;
-            __syncwarp(gm);
         }
         __syncwarp();
         PB200_PCLK_MARK(PC_WRITE, t_mark, lane);
