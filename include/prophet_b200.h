@@ -67,6 +67,7 @@ extern "C" {
 #define PB200_ST_TOO_FEW     -3   /* < 2 rows  (fbprophet ValueError) */
 #define PB200_ST_CAP_LE_FLOOR -4  /* cap <= floor (fbprophet ValueError) */
 #define PB200_ST_BAD_INPUT   -5   /* unsorted timestamps / non-finite y / zero time span */
+#define PB200_ST_BAD_PRIOR   -6   /* pb200_fit_prior_device: the series' prior scales are not finite and > 0 */
 
 /* y element type */
 #define PB200_Y_I32 0
@@ -174,6 +175,19 @@ PB200_API int pb200_fit_device(pb200_ctx* ctx, const pb200_options* opts,
                      const int64_t* h_offsets, int64_t n_series,
                      double floor, double cap_multiplier, const double* d_cap,
                      double* d_params, double* d_tchange,
+                     int32_t* d_meta_i32, int64_t* d_meta_i64, double* d_meta_f64);
+
+/* pb200_fit_device with per-series prior scales (hyperparameter tuning fits each series with its own):
+ *   d_prior   double [n_series][2] = (changepoint_prior_scale, seasonality_prior_scale) of series i
+ *             at [2 i], [2 i + 1] (device); NULL = the options' scales for every series, which is
+ *             exactly pb200_fit_device.  A series whose pair is not finite and > 0 gets status
+ *             PB200_ST_BAD_PRIOR and no fit; the other series are not affected.  A pair equal to
+ *             the options' gives the same bits as NULL. */
+PB200_API int pb200_fit_prior_device(pb200_ctx* ctx, const pb200_options* opts,
+                     const int64_t* d_ds, const void* d_y, int32_t y_dtype,
+                     const int64_t* h_offsets, int64_t n_series,
+                     double floor, double cap_multiplier, const double* d_cap,
+                     const double* d_prior, double* d_params, double* d_tchange,
                      int32_t* d_meta_i32, int64_t* d_meta_i64, double* d_meta_f64);
 
 /* Same with HOST buffers in and out (pinned or pageable); the call stages

@@ -151,8 +151,10 @@ def fit_batch_trace_host(ctx: L.Context, opts: L.Options, ds_ns: np.ndarray, y: 
 
 def fit_batch_device(ctx: L.Context, opts: L.Options, ds_ns, y, offsets_host: np.ndarray,
                      floor: float, cap_multiplier: float, cap=None, out: Optional[FittedBatch] = None,
-                     sync: bool = True) -> FittedBatch:
-    """pb200_fit_device: ``ds_ns`` / ``y`` / ``cap`` are torch CUDA tensors already in HBM."""
+                     sync: bool = True, prior=None) -> FittedBatch:
+    """pb200_fit_prior_device: ``ds_ns`` / ``y`` / ``cap`` are torch CUDA tensors already in HBM.  ``prior``: None (the
+    options' prior scales) or a float64 CUDA tensor ``[n, 2]`` of (changepoint_prior_scale, seasonality_prior_scale)
+    per series; a series whose pair is not finite and > 0 gets status ``L.ST_BAD_PRIOR``."""
     import torch
     offsets_host = np.ascontiguousarray(offsets_host, dtype=np.int64)
     n = offsets_host.size - 1
@@ -166,13 +168,17 @@ def fit_batch_device(ctx: L.Context, opts: L.Options, ds_ns, y, offsets_host: np
                           torch.empty((n, 4), dtype=torch.float64, device=dev), lay.smax, lay.kmax)
     if n > 0:
         # inputs were produced on torch's current stream; the library has its own stream
+        if prior is not None and (prior.dtype != torch.float64 or tuple(prior.shape) != (n, 2) or not prior.is_contiguous()
+                                  or prior.device != dev):
+            raise ValueError(f"prior must be a contiguous float64 tensor of shape ({n}, 2) on {dev}")
         torch.cuda.current_stream(dev).synchronize()
-        rc = L.load().pb200_fit_device(ctx.handle, C.byref(opts), ds_ns.data_ptr(), y.data_ptr(), _y_dtype(y),
-                                       _np_ptr(offsets_host), n, float(floor), float(cap_multiplier),
-                                       cap.data_ptr() if cap is not None else None,
-                                       out.params.data_ptr(), out.tchange.data_ptr(), out.meta_i32.data_ptr(),
-                                       out.meta_i64.data_ptr(), out.meta_f64.data_ptr())
-        L.check(rc, "pb200_fit_device")
+        rc = L.load().pb200_fit_prior_device(ctx.handle, C.byref(opts), ds_ns.data_ptr(), y.data_ptr(), _y_dtype(y),
+                                             _np_ptr(offsets_host), n, float(floor), float(cap_multiplier),
+                                             cap.data_ptr() if cap is not None else None,
+                                             prior.data_ptr() if prior is not None else None,
+                                             out.params.data_ptr(), out.tchange.data_ptr(), out.meta_i32.data_ptr(),
+                                             out.meta_i64.data_ptr(), out.meta_f64.data_ptr())
+        L.check(rc, "pb200_fit_prior_device")
         if sync:
             ctx.synchronize()
     return out
@@ -414,7 +420,9 @@ class CvResult:
     Metrics rows (when requested), ordered by (series, horizon): ``m_series``, ``horizon`` (ns), ``mse``, ``rmse``,
     ``mae``, ``mape``, ``coverage`` (None without intervals).
     ``fitted``: with ``keep_fits``, the cutoff fits in plan order, each record in the layout of ``opts`` (beta packed
-    by its mask, zero beyond)."""
+    by its mask, zero beyond).
+    With a ``grid`` of n_grid prior-scale pairs every series index above is a virtual one, ``s * n_grid + g`` for series
+    ``s`` fitted with grid point ``g``, and "plan order" is (series, grid point, cutoff)."""
     pair_series: np.ndarray
     pair_cutoff: np.ndarray
     pair_status: np.ndarray
@@ -430,15 +438,16 @@ class CvResult:
     fitted: Optional[FittedBatch] = None
 
 
-def _cv_chunks(plan: CvPlan, offsets_host: np.ndarray, budget: int):
-    """Series ranges [s0, s1) whose gathered rows (history prefixes + held-out windows) stay within ``budget``; a
-    series is never split (its metrics need all of its rows)."""
+def _cv_chunks(plan: CvPlan, offsets_host: np.ndarray, budget: int, n_grid: int = 1):
+    """Series ranges [s0, s1) whose gathered rows (history prefixes + held-out windows, once per grid point) stay within
+    ``budget``; a series is never split (its metrics need all of its rows)."""
     he = plan.hist_end.cpu().numpy()
     we = plan.win_end.cpu().numpy()
     ps = np.repeat(np.arange(plan.n_cutoffs.size), plan.n_cutoffs)
     per_pair = (he - offsets_host[:-1][ps]) + (we - he)
     per_series = np.zeros(plan.n_cutoffs.size, np.int64)
     np.add.at(per_series, ps, per_pair)
+    per_series *= n_grid
     out, s0, acc = [], 0, 0
     for s in range(per_series.size):
         if acc and acc + per_series[s] > budget:
@@ -450,16 +459,32 @@ def _cv_chunks(plan: CvPlan, offsets_host: np.ndarray, budget: int):
     return out, he, we
 
 
+def _cv_entries(plan: CvPlan, s0: int, s1: int, n_grid: int):
+    """The cutoff fits of series [s0, s1) under ``n_grid`` grid points, in plan order (series, grid point, cutoff): the
+    plan pair, the series and the grid point of each."""
+    vs = np.repeat(np.arange(s0, s1), n_grid)                 # (series, grid point) -> series
+    vg = np.tile(np.arange(n_grid), s1 - s0)
+    vn = np.repeat(plan.n_cutoffs[s0:s1].astype(np.int64), n_grid)
+    e = np.repeat(np.arange(vs.size), vn)
+    voff = np.zeros(vs.size + 1, np.int64)
+    np.cumsum(vn, out=voff[1:])
+    series = vs[e]
+    return plan.pair_off[series] + (np.arange(int(voff[-1])) - voff[:-1][e]), series, vg[e]
+
+
 def cross_validation_device(ctx: L.Context, opts: L.Options, ds_ns, y, offsets_host: np.ndarray, floor: float, cap,
                             horizon_ns: int, period_ns: int, initial_ns: int, intervals: bool = False, seed: int = 0,
                             rolling_window: Optional[float] = None, plan: Optional[CvPlan] = None,
                             keep_fits: bool = False, timings: Optional[dict] = None,
-                            _row_budget: Optional[int] = None) -> CvResult:
+                            _row_budget: Optional[int] = None, grid=None) -> CvResult:
     """fbprophet.diagnostics.cross_validation (and, with ``rolling_window``, performance_metrics) for every series of a
     packed batch: ``ds_ns`` / ``y`` CUDA tensors sorted within each series, ``cap`` the float64 CUDA tensor of each
     series' full-history cap.  Per chunk of series: one gather, one pb200_fit_device per full-history seasonality mask
     class, one predict, and the metrics kernel.  Plan errors raise ValueError (see ``cv_plan_errors``).  ``timings``
-    (a dict) accumulates seconds per stage -- plan, gather, fit, predict, metrics, each ending in a synchronisation."""
+    (a dict) accumulates seconds per stage -- plan, gather, fit, predict, metrics, each ending in a synchronisation.
+    ``grid``: a list of (changepoint_prior_scale, seasonality_prior_scale) pairs.  Every cutoff fit is then made once per
+    pair, in the same fit calls (each entry with its own prior scales), and the result's series are the virtual
+    ``s * n_grid + g`` (see CvResult): one backtest per grid point for the price of one batch."""
     import time
     import torch
     tm = timings if timings is not None else {}
@@ -482,7 +507,13 @@ def cross_validation_device(ctx: L.Context, opts: L.Options, ds_ns, y, offsets_h
     lay = L.get_layout(opts)
     ydt = _y_dtype(y)
     d_off = torch.from_numpy(offsets_host).to(dev)
-    chunks, he_h, we_h = _cv_chunks(plan, offsets_host, int(_row_budget or CV_ROW_BUDGET))
+    n_grid, grid_h = 1, None
+    if grid is not None:
+        grid_h = np.ascontiguousarray(np.asarray(grid, dtype=np.float64))
+        if grid_h.ndim != 2 or grid_h.shape[1] != 2 or grid_h.shape[0] == 0:
+            raise ValueError("grid must be a non-empty list of (changepoint_prior_scale, seasonality_prior_scale) pairs")
+        n_grid = grid_h.shape[0]
+    chunks, he_h, we_h = _cv_chunks(plan, offsets_host, int(_row_budget or CV_ROW_BUDGET), n_grid)
     cap = cap.to(device=dev, dtype=torch.float64)
     pieces = []
     clock[0] = time.perf_counter()
@@ -490,11 +521,11 @@ def cross_validation_device(ctx: L.Context, opts: L.Options, ds_ns, y, offsets_h
         p0, p1 = int(plan.pair_off[s0]), int(plan.pair_off[s1])
         if p1 == p0:
             continue
-        ps_h = np.repeat(np.arange(s0, s1), plan.n_cutoffs[s0:s1])
+        ent_h, ps_h, g_h = _cv_entries(plan, s0, s1, n_grid)
         pmask = plan.mask[ps_h]
-        # gathered order: pairs grouped by mask class (stable), so that every class is one contiguous fit batch
+        # gathered order: fits grouped by mask class (stable), so that every class is one contiguous fit batch
         perm = np.argsort(pmask, kind="stable")
-        pairs_h = (p0 + perm).astype(np.int64)
+        pairs_h = ent_h[perm].astype(np.int64)
         hist_len = he_h[pairs_h] - offsets_host[ps_h[perm]]
         win_len = we_h[pairs_h] - he_h[pairs_h]
         fit_off = np.zeros(pairs_h.size + 1, np.int64)
@@ -521,12 +552,13 @@ def cross_validation_device(ctx: L.Context, opts: L.Options, ds_ns, y, offsets_h
                              torch.empty((n, 2), dtype=torch.int64, device=dev),
                              torch.empty((n, 4), dtype=torch.float64, device=dev), lay.smax, lay.kmax)
         cap_p = cap[torch.from_numpy(ps_h[perm]).to(dev)].contiguous()
+        prior_p = torch.from_numpy(grid_h[g_h[perm]]).to(dev) if grid_h is not None else None
         bounds = np.flatnonzero(np.diff(np.concatenate(([-1], sp, [-1])))).tolist()
         for a, b in zip(bounds[:-1], bounds[1:]):
             oc = _with_mask(opts, int(sp[a]))
             r0, r1 = int(fit_off[a]), int(fit_off[b])
             fc = fit_batch_device(ctx, oc, ds_g[r0:r1], y_g[r0:r1], fit_off[a:b + 1] - r0, float(floor), 1.0,
-                                  cap=cap_p[a:b])
+                                  cap=cap_p[a:b], prior=prior_p[a:b] if prior_p is not None else None)
             w = fc.params.shape[1]
             fitted.params[a:b, :w] = fc.params
             fitted.tchange[a:b] = fc.tchange
@@ -544,18 +576,20 @@ def cross_validation_device(ctx: L.Context, opts: L.Options, ds_ns, y, offsets_h
         lo = fcst.yhat_lower[inv] if fcst.yhat_lower is not None else None
         hi = fcst.yhat_upper[inv] if fcst.yhat_upper is not None else None
         futp = fut[inv]
-        wl = torch.from_numpy(we_h[p0:p1] - he_h[p0:p1]).to(dev)
+        d_ent = torch.from_numpy(ent_h).to(dev)
+        wl = torch.from_numpy(we_h[ent_h] - he_h[ent_h]).to(dev)
         valid = torch.arange(hmax, device=dev)[None, :] < wl[:, None]
         kk, jj = torch.nonzero(valid, as_tuple=True)
-        src_row = plan.hist_end[p0:p1][kk] + jj
-        rows = {"series": plan.pair_series[p0:p1][kk].to(torch.int64), "ds": futp[kk, jj],
-                "cutoff": plan.cutoff[p0:p1][kk], "y": y[src_row].to(torch.float64), "yhat": yhat[kk, jj],
+        src_row = plan.hist_end[d_ent][kk] + jj
+        rows = {"series": torch.from_numpy(ps_h * n_grid + g_h).to(dev)[kk], "ds": futp[kk, jj],
+                "cutoff": plan.cutoff[d_ent][kk], "y": y[src_row].to(torch.float64), "yhat": yhat[kk, jj],
                 "yhat_lower": lo[kk, jj] if lo is not None else None, "yhat_upper": hi[kk, jj] if hi is not None else None}
         met = None
         if rolling_window is not None:
-            met = performance_metrics_device(ctx, rows["series"] - s0, rows["ds"] - rows["cutoff"], rows["y"], rows["yhat"],
-                                             rows["yhat_lower"], rows["yhat_upper"], s1 - s0, rolling_window)
-            met["series"] = met["series"] + s0
+            v0 = s0 * n_grid
+            met = performance_metrics_device(ctx, rows["series"] - v0, rows["ds"] - rows["cutoff"], rows["y"], rows["yhat"],
+                                             rows["yhat_lower"], rows["yhat_upper"], (s1 - s0) * n_grid, rolling_window)
+            met["series"] = met["series"] + v0
             lap("metrics")
         fh = None
         if keep_fits:
@@ -582,10 +616,11 @@ def cross_validation_device(ctx: L.Context, opts: L.Options, ds_ns, y, offsets_h
     if keep_fits and pieces:
         fitted_all = FittedBatch(*(np.concatenate([getattr(p[3], f) for p in pieces])
                                    for f in ("params", "tchange", "meta_i32", "meta_i64", "meta_f64")), lay.smax, lay.kmax)
-    ps_all = np.repeat(np.arange(plan.n_cutoffs.size), plan.n_cutoffs)
+    ent_all, ps_all, g_all = _cv_entries(plan, 0, plan.n_cutoffs.size, n_grid)
     status = cat([p[2] for p in pieces]) if pieces else np.zeros(0, np.int32)
-    return CvResult(ps_all, plan.cutoff.cpu().numpy(), status, plan.mask[ps_all], rows["series"], rows["ds"], rows["cutoff"],
-                    rows["y"], rows["yhat"], rows["yhat_lower"], rows["yhat_upper"], metrics, fitted_all)
+    return CvResult(ps_all * n_grid + g_all, plan.cutoff.cpu().numpy()[ent_all], status, plan.mask[ps_all], rows["series"],
+                    rows["ds"], rows["cutoff"], rows["y"], rows["yhat"], rows["yhat_lower"], rows["yhat_upper"], metrics,
+                    fitted_all)
 
 
 def performance_metrics_device(ctx: L.Context, series, horizon_ns, y, yhat, yhat_lower, yhat_upper, n_series: int,
@@ -627,3 +662,66 @@ def performance_metrics_device(ctx: L.Context, series, horizon_ns, y, yhat, yhat
     out = {"series": slot_series[keep], "horizon": out_h[keep], "mse": mse[keep], "rmse": rmse[keep], "mae": mae[keep],
            "mape": mape[keep], "coverage": cov[keep] if has_iv else None}
     return {k: (v.cpu().numpy() if v is not None else None) for k, v in out.items()}
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# Hyperparameter tuning: fbprophet's documented grid search over the prior scales, every series in one job (DESIGN §10)
+# ---------------------------------------------------------------------------------------------------------------------
+TUNE_METRICS = ("mse", "rmse", "mae", "mape")
+
+
+@dataclass
+class TuneResult:
+    """Output of tune_device.  ``grid`` [n_grid, 2]: the (changepoint_prior_scale, seasonality_prior_scale) pairs in
+    enumeration order.  Per (series, grid point), host numpy [n, n_grid]: ``scores`` (the metric over all of the series'
+    held-out rows: performance_metrics with rolling_window = 1) and ``eligible`` (every cutoff fit succeeded and the
+    score is finite).  Per series: ``chosen`` (grid index of the lowest eligible score, the first on ties; -1: none
+    eligible, the options' scales were used), ``prior`` [n, 2] (the pair of the final fit) and ``fitted``, the
+    full-history fits with those pairs (CUDA tensors).  ``cv``: the grid backtest itself (virtual series)."""
+    grid: np.ndarray
+    scores: np.ndarray
+    eligible: np.ndarray
+    chosen: np.ndarray
+    prior: np.ndarray
+    fitted: FittedBatch
+    cv: CvResult
+
+
+def tune_device(ctx: L.Context, opts: L.Options, ds_ns, y, offsets_host: np.ndarray, floor: float, cap_multiplier: float,
+                horizon_ns: int, period_ns: int, initial_ns: int, grid, metric: str = "rmse",
+                plan: Optional[CvPlan] = None, timings: Optional[dict] = None,
+                _row_budget: Optional[int] = None) -> TuneResult:
+    """For every series of a packed batch: cross_validation + performance_metrics(rolling_window=1) at every grid point
+    (one cross_validation_device call with ``grid``), the grid point with the lowest ``metric``, then one
+    pb200_fit_prior_device over the full histories, each series with its chosen pair (the options' for a series with no
+    eligible point).  ``cap_multiplier`` gives every fit the full history's cap, max(y) * cap_multiplier, as the modeler
+    does.  ``timings`` as in cross_validation_device, plus ``final_fit``."""
+    import time
+    import torch
+    if metric not in TUNE_METRICS:
+        raise ValueError(f"metric must be one of {', '.join(TUNE_METRICS)} (got {metric!r})")
+    offsets_host = np.ascontiguousarray(offsets_host, dtype=np.int64)
+    n = offsets_host.size - 1
+    grid_h = np.ascontiguousarray(np.asarray(grid, dtype=np.float64).reshape(-1, 2))
+    g = grid_h.shape[0]
+    dev = ds_ns.device
+    lens = torch.from_numpy(np.diff(offsets_host)).to(dev)
+    cap = torch.segment_reduce(y.to(torch.float64), "max", lengths=lens) * float(cap_multiplier)
+    cv = cross_validation_device(ctx, opts, ds_ns, y, offsets_host, floor, cap, horizon_ns, period_ns, initial_ns,
+                                 rolling_window=1.0, plan=plan, timings=timings, _row_budget=_row_budget, grid=grid_h)
+    scores = np.full(n * g, np.nan)
+    scores[cv.metrics["series"]] = cv.metrics[metric]
+    fit_ok = np.ones(n * g, bool)
+    fit_ok[cv.pair_series[cv.pair_status < 0]] = False
+    scores = scores.reshape(n, g)
+    eligible = fit_ok.reshape(n, g) & np.isfinite(scores)
+    chosen = np.argmin(np.where(eligible, scores, np.inf), axis=1)        # the first of equal minima
+    chosen[~eligible.any(axis=1)] = -1
+    prior = np.where((chosen >= 0)[:, None], grid_h[np.maximum(chosen, 0)],
+                     np.array([[opts.changepoint_prior_scale, opts.seasonality_prior_scale]]))
+    t0 = time.perf_counter()
+    fitted = fit_batch_device(ctx, opts, ds_ns, y, offsets_host, float(floor), float(cap_multiplier),
+                              prior=torch.from_numpy(np.ascontiguousarray(prior)).to(dev))
+    if timings is not None:
+        timings["final_fit"] = timings.get("final_fit", 0.0) + time.perf_counter() - t0
+    return TuneResult(grid_h, scores, eligible, chosen, prior, fitted, cv)

@@ -329,8 +329,8 @@ PB200_API int pb200_synchronize(pb200_ctx* c) {
 
 // newton_kernel over the queue {count, head, items...} at d_nq (16-warp CTAs with ~100 KB of shared memory)
 static int launch_newton(pb200_ctx* c, const pb200_options* opts, const int64_t* d_ds, const void* d_y,
-                         int32_t y_dtype, const int64_t* d_offsets, int64_t n_series, int* d_nq, double* d_params,
-                         double* d_tchange, int32_t* d_meta_i32, int64_t* d_meta_i64, double* d_meta_f64) {
+                         int32_t y_dtype, const int64_t* d_offsets, int64_t n_series, int* d_nq, const double* d_prior,
+                         double* d_params, double* d_tchange, int32_t* d_meta_i32, int64_t* d_meta_i64, double* d_meta_f64) {
     pb200_layout L;
     pb200_get_layout(opts, &L);
     if (opts->algorithm == PB200_ALG_LBFGS || L.pstride > pb200::nw::NW_PMAX) return PB200_OK;
@@ -350,6 +350,7 @@ static int launch_newton(pb200_ctx* c, const pb200_options* opts, const int64_t*
     na.smax = L.smax;
     na.kmax = L.kmax;
     na.pstride = L.pstride;
+    na.prior = d_prior;
     na.o = to_dev(opts);
     const size_t nsm = pb200::nw::newton_smem_bytes(L.pstride);
     CK(cudaFuncSetAttribute(pb200::nw::newton_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)nsm));
@@ -362,10 +363,10 @@ static int launch_newton(pb200_ctx* c, const pb200_options* opts, const int64_t*
 }
 
 // every fit call: zeroes the variant counters, then queues, fit kernels and (unless this is an objective evaluation,
-// d_theta_in set) the Newton retry on the context's stream
+// d_theta_in set) the Newton retry on the context's stream.  d_prior: per-series prior scales, or null for the options'
 static int fit_impl(pb200_ctx* c, const pb200_options* opts, const int64_t* d_ds, const void* d_y, int32_t y_dtype,
                     const int64_t* h_offsets, int64_t n_series, double floor, double cap_multiplier,
-                    const double* d_cap, double* d_params, double* d_tchange, int32_t* d_meta_i32,
+                    const double* d_cap, const double* d_prior, double* d_params, double* d_tchange, int32_t* d_meta_i32,
                     int64_t* d_meta_i64, double* d_meta_f64, const double* d_theta_in, double* d_grad_out,
                     double* d_trace = nullptr, int trace_cap = 0) {
     if (!c) return fail(PB200_E_ARG, "ctx is null");
@@ -478,6 +479,7 @@ static int fit_impl(pb200_ctx* c, const pb200_options* opts, const int64_t* d_ds
         pa.vcount = (int*)c->d_vcount.p;
         pa.qkey = (int*)c->d_qkey.p;
         pa.qhist = (int*)c->d_qhist.p;
+        pa.prior = d_prior;
         const int warps_per_block = 8;
         int grid = (N + warps_per_block - 1) / warps_per_block;
         grid = std::min(grid, c->sms * 8);
@@ -577,6 +579,7 @@ static int fit_impl(pb200_ctx* c, const pb200_options* opts, const int64_t* d_ds
             fa.nq_count = nq;
             fa.nq_items = opts->algorithm == PB200_ALG_LBFGS_NEWTON ? nq + 2 : nullptr;
             fa.o = od;
+            fa.prior = d_prior;
             fa.l2_keep = fa.l2_rest_first = 0;
             if (g.grouped && c->l2_keep_pct >= 0) {
                 // the slots' y planes are read once per evaluation round, cyclically: an LRU-like L2 smaller than all of them
@@ -596,8 +599,8 @@ static int fit_impl(pb200_ctx* c, const pb200_options* opts, const int64_t* d_ds
     }
     // ---- fbprophet's Newton retry over the series whose L-BFGS failed its line search (normally an empty queue) ----
     if (!d_theta_in)
-        return launch_newton(c, opts, d_ds, d_y, y_dtype, (const int64_t*)c->d_offsets.p, n_series, nq, d_params, d_tchange,
-                             d_meta_i32, d_meta_i64, d_meta_f64);
+        return launch_newton(c, opts, d_ds, d_y, y_dtype, (const int64_t*)c->d_offsets.p, n_series, nq, d_prior, d_params,
+                             d_tchange, d_meta_i32, d_meta_i64, d_meta_f64);
     return PB200_OK;
 }
 
@@ -655,7 +658,7 @@ static int fit_host(pb200_ctx* c, const pb200_options* opts, const int64_t* h_ds
         CK(cudaMemsetAsync(c->d_trace.p, 0, tbytes, c->stream));
     }
     rc = fit_impl(c, opts, (const int64_t*)c->d_ds.p, c->d_y.p, y_dtype, h_offsets, n_series, floor, cap_multiplier,
-                  h_cap ? (const double*)c->d_cap.p : nullptr, (double*)c->d_params.p, (double*)c->d_tchange.p,
+                  h_cap ? (const double*)c->d_cap.p : nullptr, nullptr, (double*)c->d_params.p, (double*)c->d_tchange.p,
                   (int32_t*)c->d_mi32.p, (int64_t*)c->d_mi64.p, (double*)c->d_mf64.p, nullptr, nullptr,
                   traced ? (double*)c->d_trace.p : nullptr, trace_cap);
     if (rc) return rc;
@@ -671,12 +674,20 @@ static int fit_host(pb200_ctx* c, const pb200_options* opts, const int64_t* h_ds
 
 extern "C" {
 
+PB200_API int pb200_fit_prior_device(pb200_ctx* c, const pb200_options* opts, const int64_t* d_ds, const void* d_y,
+                                     int32_t y_dtype, const int64_t* h_offsets, int64_t n_series, double floor,
+                                     double cap_multiplier, const double* d_cap, const double* d_prior, double* d_params,
+                                     double* d_tchange, int32_t* d_meta_i32, int64_t* d_meta_i64, double* d_meta_f64) {
+    return fit_impl(c, opts, d_ds, d_y, y_dtype, h_offsets, n_series, floor, cap_multiplier, d_cap, d_prior, d_params,
+                    d_tchange, d_meta_i32, d_meta_i64, d_meta_f64, nullptr, nullptr);
+}
+
 PB200_API int pb200_fit_device(pb200_ctx* c, const pb200_options* opts, const int64_t* d_ds, const void* d_y, int32_t y_dtype,
                      const int64_t* h_offsets, int64_t n_series, double floor, double cap_multiplier,
                      const double* d_cap, double* d_params, double* d_tchange, int32_t* d_meta_i32,
                      int64_t* d_meta_i64, double* d_meta_f64) {
-    return fit_impl(c, opts, d_ds, d_y, y_dtype, h_offsets, n_series, floor, cap_multiplier, d_cap, d_params, d_tchange,
-                    d_meta_i32, d_meta_i64, d_meta_f64, nullptr, nullptr);
+    return pb200_fit_prior_device(c, opts, d_ds, d_y, y_dtype, h_offsets, n_series, floor, cap_multiplier, d_cap, nullptr,
+                                  d_params, d_tchange, d_meta_i32, d_meta_i64, d_meta_f64);
 }
 
 PB200_API int pb200_objective_host(pb200_ctx* c, const pb200_options* opts, const int64_t* h_ds, const void* h_y,
@@ -694,7 +705,7 @@ PB200_API int pb200_objective_host(pb200_ctx* c, const pb200_options* opts, cons
     CK(cudaMemcpyAsync(c->d_yhat.p, h_theta, N * L.pstride * 8, cudaMemcpyHostToDevice, c->stream));
     CK(cudaMemsetAsync(c->d_lo.p, 0, N * L.pstride * 8, c->stream));
     rc = fit_impl(c, opts, (const int64_t*)c->d_ds.p, c->d_y.p, y_dtype, h_offsets, n_series, floor, cap_multiplier,
-                  nullptr, (double*)c->d_params.p, (double*)c->d_tchange.p, (int32_t*)c->d_mi32.p,
+                  nullptr, nullptr, (double*)c->d_params.p, (double*)c->d_tchange.p, (int32_t*)c->d_mi32.p,
                   (int64_t*)c->d_mi64.p, (double*)c->d_mf64.p, (const double*)c->d_yhat.p, (double*)c->d_lo.p);
     if (rc) return rc;
     std::vector<double> mf(N * 4);

@@ -86,7 +86,8 @@ static_assert(PB200_GRP_RING >= 2 && (PB200_GRP_RING & (PB200_GRP_RING - 1)) == 
 template <int G, bool SEAS>
 inline size_t group_smem_bytes() {
     return (size_t)(32 / G) * ((sizeof(GState<G, SEAS>) + 15) & ~(size_t)15) + (size_t)grp_ring(G) * (grp_u(G) / 2) * 32 * 16   // + cp.async ring
-           + sizeof(FitOptsDev);                                                                                 // + the options
+           + sizeof(FitOptsDev)                                                                                  // + the options
+           + (size_t)(32 / G) * sizeof(SeriesPrior);                                                             // + gprior
 }
 // global workspace per series slot (doubles): y pairs, then history Y[5], S[5]
 __host__ __device__ inline size_t group_plane_doubles(int tmax, int G) {
@@ -108,6 +109,12 @@ __device__ __forceinline__ double2* gring() {
 template <int G, bool SEAS>
 __device__ __forceinline__ FitOptsDev& gopts() {
     return *reinterpret_cast<FitOptsDev*>(reinterpret_cast<unsigned char*>(gring<G, SEAS>()) + (size_t)grp_ring(G) * (grp_u(G) / 2) * 32 * 16);
+}
+// the prior scales of group gi's series (inv_seas2 = 1 without seasonality), behind the options rather than in GState: a
+// longer GState moves every group's state to other shared-memory banks, which measured 4 % slower at G = 8
+template <int G, bool SEAS>
+__device__ __forceinline__ SeriesPrior& gprior(int gi) {
+    return reinterpret_cast<SeriesPrior*>(&gopts<G, SEAS>() + 1)[gi];
 }
 
 // ---- L2 priority of the workspace slots (per-access cache hints only: nothing is set aside in L2 for the device) ----
@@ -754,10 +761,11 @@ __device__ __noinline__ void g_point_pass(GState<G, SEAS>& s, const double* plan
 // ---------------------------------------------------------------------------------------
 template <int G, bool LOGI, bool SEAS>
 __device__ __noinline__ int g_eval_finalize(GState<G, SEAS>& s, const double* xv, double* gv, const int gl, const unsigned gm,
-                                            const bool active, const double tau, const double rtau, const double inv_seas2,
-                                            double* f_out) {
+                                            const bool active, double* f_out) {
     constexpr int NS = GSEG / G;
     const int S = s.S, T = s.T, jb = gl * NS;
+    const SeriesPrior& pr = gprior<G, SEAS>((threadIdx.x & 31) / G);
+    const double tau = pr.tau, rtau = pr.rtau, inv_seas2 = pr.inv_seas2;
     const double* tot = s.stab;                     // value v of the pass: tot[v], v < 14 beta sums, tot[14] = ss
     const double ss = tot[GState<G, SEAS>::TOTSS];
     const double sigma = s.sigma;
@@ -1265,6 +1273,10 @@ __device__ __noinline__ bool g_fetch(GState<G, SEAS>& s, const FitArgs& a, doubl
     if (gl == 0) {
         s.T = T; s.S = S; s.ncp = ncp; s.chunk = chunk; s.tabP = tabP; s.tabPL = PL;
         s.cap_s = cap_s; s.hstep = (double)step / dts; s.st0 = st0; s.i1max = i1max; s.exprec = 0;
+        SeriesPrior& pr = gprior<G, SEAS>((threadIdx.x & 31) / G);
+        pr = series_prior(a.prior, a.o, sidx);
+        // (the all-zero column of the class without seasonality has prior scale 1: fbprophet's make_all_seasonality_features)
+        if constexpr (!SEAS) pr.inv_seas2 = 1.0;
         if constexpr (SEAS) {
             const double dt_d = (1e-9 * (double)step) / 86400.0;
             double s_, c_;
@@ -1443,8 +1455,6 @@ __global__ void __launch_bounds__(32, G != 8 ? 16 : (SEAS ? PB200_GRP_BLOCKS : P
     double* const plane = reinterpret_cast<double*>(a.planes) + slot * (size_t)a.nseas_stride;
     double* const hist = plane + (a.nseas_stride - GHIST);
     double* const trace_base = a.trace;
-    // (the all-zero column of the class without seasonality has prior scale 1: fbprophet's make_all_seasonality_features)
-    const double tau = a.o.tau, rtau = a.o.rtau, inv_seas2 = SEAS ? a.o.inv_seas2 : 1.0;
     {   // every group's state starts zeroed: the idle groups run the round's routines on it (no trend segments, every vector
         // role on vec[0]: in bounds), and store nothing
         constexpr int NZ = (int)(NSER * ((sizeof(GState<G, SEAS>) + 15) & ~(size_t)15) / 16);
@@ -1453,7 +1463,8 @@ __global__ void __launch_bounds__(32, G != 8 ? 16 : (SEAS ? PB200_GRP_BLOCKS : P
         for (int i = lane; i < NZ; i += 32) z[i] = make_double2(0.0, 0.0);
     }
     __syncwarp();
-    if (gl == 0) { s.state = ST_IDLE; s.series = -1; }
+    // (an idle group's prior scales: the options', so that its unstored evaluations stay finite as before any fetch)
+    if (gl == 0) { s.state = ST_IDLE; s.series = -1; gprior<G, SEAS>(gi) = {a.o.tau, a.o.rtau, SEAS ? a.o.inv_seas2 : 1.0}; }
     if (lane == 0) gopts<G, SEAS>() = a.o;
     __syncwarp();
     const FitOptsDev& opt = gopts<G, SEAS>();
@@ -1515,8 +1526,7 @@ __global__ void __launch_bounds__(32, G != 8 ? 16 : (SEAS ? PB200_GRP_BLOCKS : P
         g_point_pass<G, LOGI, MULT, SEAS, grp_u(G)>(s, plane, active, gl, lane, lp, l2f);
         __syncwarp();
         PB200_PCLK_MARK(PC_PASS, t_mark, lane);
-        const int err = g_eval_finalize<G, LOGI, SEAS>(s, s.vec[ixv], s.vec[igv], gl, gm, active, tau, rtau, inv_seas2,
-                                                       first ? &s.ls.fk : &s.ls.ft);
+        const int err = g_eval_finalize<G, LOGI, SEAS>(s, s.vec[ixv], s.vec[igv], gl, gm, active, first ? &s.ls.fk : &s.ls.ft);
         __syncwarp();
         PB200_PCLK_MARK(PC_FINAL, t_mark, lane);
         // ---- the optimiser's reaction (BFGSMinimizer::step split at its evaluations); `act` carries each group's action

@@ -40,6 +40,7 @@ struct NewtonArgs {
     const long long* meta_i64;
     double* meta_f64;
     int smax, kmax, pstride;
+    const double* prior;     // per-series prior scales (FitArgs::prior); null: o's
     FitOptsDev o;
 };
 
@@ -319,7 +320,8 @@ __global__ void __launch_bounds__(32 * NW_WARPS, 1) newton_kernel(const NewtonAr
             sr.span = a.meta_i64[(size_t)sidx * 2 + 1];
             sr.y_scale = mf[0]; sr.fl = mf[1];
             sr.cap_s = sr.logistic ? (mf[2] - mf[1]) / mf[0] : 0.0;
-            sr.tau = a.o.tau; sr.inv_seas2 = a.o.inv_seas2;
+            const SeriesPrior pr = series_prior(a.prior, a.o, sidx);
+            sr.tau = pr.tau; sr.inv_seas2 = pr.inv_seas2;
             sr.it = 0; sr.nev = 0; sr.status = PB200_ST_NEWTON; sr.stop = 0;
         }
         __syncthreads();

@@ -77,6 +77,41 @@ def options_from_config(config) -> L.Options:
     )
 
 
+def who(series_id, dim_id, mask) -> str:
+    """The first offending group of a per-series bool mask, and how many there are, for an error message."""
+    i = int(np.flatnonzero(mask)[0])
+    return (f" (first offender: series_id {int(series_id[i])}, dim_id {int(dim_id[i])}; "
+            f"{int(np.count_nonzero(mask))} group(s) in all)")
+
+
+def models_table(fitted: batched.FittedBatch, series_id, dim_id, last_ds, opts: L.Options, floor) -> pa.Table:
+    """The models table (MODEL_OUTPUT_SCHEMA) of a fitted batch (host arrays).  fbprophet's ValueErrors (cap <= floor,
+    bad input) raise, naming the group; a failed fit (status < 0) -- the reference's RuntimeError -- prints a line and
+    gets no row (prophet_modeler.py:81-85)."""
+    n = fitted.n
+    status = fitted.meta_i32[:, 4]
+    if np.any(status == L.ST_CAP_LE_FLOOR):
+        raise ValueError("cap must be greater than floor (which defaults to 0)." + who(series_id, dim_id, status == L.ST_CAP_LE_FLOOR))
+    if np.any(status == L.ST_BAD_INPUT):
+        raise ValueError("Found non-finite y or a zero time span in a series." + who(series_id, dim_id, status == L.ST_BAD_INPUT))
+    ok = status >= 0
+    for i in np.flatnonzero(~ok):
+        print(f"Runtime error (solver status {int(status[i])}) for series_id: {int(series_id[i])}, "
+              f"dim_id: {int(dim_id[i])}")
+    blobs = model_record.encode(fitted, last_ds, opts)
+    cap64 = fitted.meta_f64[:, 2]
+    out = pa.table({
+        "series_id": pa.array(series_id, pa.int32()),
+        "dim_id": pa.array(dim_id, pa.int32()),
+        "floor": pa.array(np.full(n, floor, dtype=np.float32), pa.float32()),
+        "cap": pa.array(cap64.astype(np.float32), pa.float32()),   # FloatType column, prophet_modeler.py:36
+        "model": blobs,
+    })
+    if not ok.all():
+        out = out.filter(pa.array(ok))
+    return out
+
+
 class _ModelTimeSeriesOp:
     """Batched GROUPED_MAP operator: all (series_id, dim_id) groups in one GPU launch."""
 
@@ -108,38 +143,13 @@ class _ModelTimeSeriesOp:
         print(f"Modeling {pk.n} series with {int(pk.offsets[-1])} modeling rows")
         # fbprophet raises ValueError (task failure, not RuntimeError) for < 2 rows:
         # keep that observable behaviour (prophet_modeler.py:81 only catches RuntimeError)
-        def _who(mask):
-            i = int(np.flatnonzero(mask)[0])
-            return (f" (first offender: series_id {int(pk.series_id[i])}, dim_id {int(pk.dim_id[i])}; "
-                    f"{int(np.count_nonzero(mask))} group(s) in all)")
-
         short = np.diff(pk.offsets) < 2
         if np.any(short):
-            raise ValueError("Dataframe has less than 2 non-NaN rows." + _who(short))
+            raise ValueError("Dataframe has less than 2 non-NaN rows." + who(pk.series_id, pk.dim_id, short))
         fitted = batched.fit_batch_device(ctx, opts, pk.ds.contiguous(), pk.y.contiguous(), pk.offsets,
                                           float(floor), float(cap_multiplier)).to_host()
         t_fit = time.time()
-        status = fitted.meta_i32[:, 4]
-        if np.any(status == L.ST_CAP_LE_FLOOR):
-            raise ValueError("cap must be greater than floor (which defaults to 0)." + _who(status == L.ST_CAP_LE_FLOOR))
-        if np.any(status == L.ST_BAD_INPUT):
-            raise ValueError("Found non-finite y or a zero time span in a series." + _who(status == L.ST_BAD_INPUT))
-        ok = status >= 0
-        for i in np.flatnonzero(~ok):
-            # reference: RuntimeError -> print + empty frame (prophet_modeler.py:81-85)
-            print(f"Runtime error (solver status {int(status[i])}) for series_id: {int(pk.series_id[i])}, "
-                  f"dim_id: {int(pk.dim_id[i])}")
-        blobs = model_record.encode(fitted, pk.last_ds, opts)
-        cap64 = fitted.meta_f64[:, 2]
-        out = pa.table({
-            "series_id": pa.array(pk.series_id, pa.int32()),
-            "dim_id": pa.array(pk.dim_id, pa.int32()),
-            "floor": pa.array(np.full(pk.n, floor, dtype=np.float32), pa.float32()),
-            "cap": pa.array(cap64.astype(np.float32), pa.float32()),   # FloatType column, prophet_modeler.py:36
-            "model": blobs,
-        })
-        if not ok.all():
-            out = out.filter(pa.array(ok))
+        out = models_table(fitted, pk.series_id, pk.dim_id, pk.last_ds, opts, floor)
         # wall time per stage of the last call (tools/e2e_scaling.py reports them): upload + group + sort, GPU fit + D2H, encode
         self.last_timings = {"pack_s": t_pack - execution_time, "fit_s": t_fit - t_pack, "encode_s": time.time() - t_fit}
         print(f"Output df {out.num_rows} models trained in {time.time() - execution_time}")
