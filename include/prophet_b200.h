@@ -69,6 +69,12 @@ extern "C" {
 #define PB200_ST_BAD_INPUT   -5   /* unsorted timestamps / non-finite y / zero time span */
 #define PB200_ST_BAD_PRIOR   -6   /* pb200_fit_prior_device: the series' prior scales are not finite and > 0 */
 
+/* where a series of pb200_fit_warm_device started (d_warm) */
+#define PB200_WARM_USED       1   /* from its previous model */
+#define PB200_WARM_NONE       0   /* cold: no previous model, or the series is not optimised (prep error, constant linear) */
+#define PB200_WARM_SHAPE     -1   /* cold: the previous model's S or seasonality mask differs from the new history's */
+#define PB200_WARM_BAD       -2   /* cold: the previous model has a non-finite k, m, delta or beta, or sigma_obs <= 0 */
+
 /* y element type */
 #define PB200_Y_I32 0
 #define PB200_Y_F32 1
@@ -189,6 +195,38 @@ PB200_API int pb200_fit_prior_device(pb200_ctx* ctx, const pb200_options* opts,
                      double floor, double cap_multiplier, const double* d_cap,
                      const double* d_prior, double* d_params, double* d_tchange,
                      int32_t* d_meta_i32, int64_t* d_meta_i64, double* d_meta_f64);
+
+/* pb200_fit_prior_device started from each series' previous model (fbprophet's "updating fitted
+ * models": m.fit(df, init=stan_init(m_old))):
+ *   d_init_params   double [n_series][pstride] previous model records (layout of d_params), row i
+ *                   for series i; NULL = exactly pb200_fit_prior_device (d_init_meta, d_warm ignored)
+ *   d_init_meta     int32 [n_series][8] their meta_i32 (S at [1], mask at [3], status at [4]); a
+ *                   status < 0 means "no previous model"
+ *   d_warm          int32 [n_series] PB200_WARM_* per series, or NULL
+ * A series starts from k, m, delta[0:S], log(sigma_obs), beta[0:K] of its record (raw values, no
+ * rescaling to the new y_scale / t_scale / cap) when the record's status is >= 0, its S and mask are
+ * the new history's, and those values are finite with sigma_obs > 0; otherwise from stan_init, bit for
+ * bit as without an init.  The L-BFGS run, its Newton retry and PB200_ALG_NEWTON all start there; the
+ * constant-linear shortcut ignores it.  A start point whose objective is not finite gives
+ * PB200_ST_INIT_ERROR (L-BFGS).  The model record and its layout are those of pb200_fit_device. */
+PB200_API int pb200_fit_warm_device(pb200_ctx* ctx, const pb200_options* opts,
+                     const int64_t* d_ds, const void* d_y, int32_t y_dtype,
+                     const int64_t* h_offsets, int64_t n_series,
+                     double floor, double cap_multiplier, const double* d_cap, const double* d_prior,
+                     const double* d_init_params, const int32_t* d_init_meta_i32,
+                     double* d_params, double* d_tchange,
+                     int32_t* d_meta_i32, int64_t* d_meta_i64, double* d_meta_f64, int32_t* d_warm);
+
+/* pb200_fit_warm_device on HOST buffers (h_cap, h_prior, h_init_params, h_warm may be NULL), plus
+ * an optional trajectory: h_trace with trace_cap > 0 gets pb200_fit_trace_host's rows (NULL / 0: none). */
+PB200_API int pb200_fit_warm_host(pb200_ctx* ctx, const pb200_options* opts,
+                     const int64_t* h_ds, const void* h_y, int32_t y_dtype,
+                     const int64_t* h_offsets, int64_t n_series,
+                     double floor, double cap_multiplier, const double* h_cap, const double* h_prior,
+                     const double* h_init_params, const int32_t* h_init_meta_i32,
+                     double* h_params, double* h_tchange,
+                     int32_t* h_meta_i32, int64_t* h_meta_i64, double* h_meta_f64, int32_t* h_warm,
+                     double* h_trace, int32_t trace_cap);
 
 /* Same with HOST buffers in and out (pinned or pageable); the call stages
  * through the context's device workspace, copies results back and synchronises. */

@@ -22,6 +22,8 @@ ST_ABSX, ST_ABSF, ST_RELF, ST_ABSGRAD, ST_RELGRAD, ST_MAXIT, ST_CONST_LINEAR = 1
 ST_NEWTON = 60
 ALG_LBFGS_NEWTON, ALG_LBFGS, ALG_NEWTON = 0, 1, 2
 ST_LSFAIL, ST_INIT_ERROR, ST_TOO_FEW, ST_CAP_LE_FLOOR, ST_BAD_INPUT, ST_BAD_PRIOR = -1, -2, -3, -4, -5, -6
+# where a series of a warm-started fit started (PB200_WARM_*)
+WARM_USED, WARM_NONE, WARM_SHAPE, WARM_BAD = 1, 0, -1, -2
 
 
 class Options(C.Structure):
@@ -46,7 +48,7 @@ class Layout(C.Structure):
 
 EXPORTS = [
     "pb200_default_options", "pb200_get_layout", "pb200_create", "pb200_destroy", "pb200_last_error",
-    "pb200_stream", "pb200_launch_count", "pb200_last_fit_variant_counts", "pb200_tab_chunk", "pb200_fit_device", "pb200_fit_prior_device", "pb200_fit_host", "pb200_predict_device",
+    "pb200_stream", "pb200_launch_count", "pb200_last_fit_variant_counts", "pb200_tab_chunk", "pb200_fit_device", "pb200_fit_prior_device", "pb200_fit_warm_device", "pb200_fit_host", "pb200_fit_warm_host", "pb200_predict_device",
     "pb200_predict_host", "pb200_make_future_device", "pb200_synchronize", "pb200_objective_host",
     "pb200_fit_trace_host", "pb200_forecast_csv_lengths_device", "pb200_forecast_csv_rows_device", "pb200_forecast_csv_row_host",
     "pb200_cv_plan_counts_device", "pb200_cv_plan_device", "pb200_cv_gather_device", "pb200_cv_metrics_device",
@@ -91,6 +93,10 @@ def load() -> C.CDLL:
     lib.pb200_fit_device.restype = C.c_int
     lib.pb200_fit_prior_device.argtypes = fit_args[:10] + [vp] + fit_args[10:]
     lib.pb200_fit_prior_device.restype = C.c_int
+    lib.pb200_fit_warm_device.argtypes = fit_args[:10] + [vp, vp, vp] + fit_args[10:] + [vp]
+    lib.pb200_fit_warm_device.restype = C.c_int
+    lib.pb200_fit_warm_host.argtypes = fit_args[:10] + [vp, vp, vp] + fit_args[10:] + [vp, vp, i32]
+    lib.pb200_fit_warm_host.restype = C.c_int
     lib.pb200_fit_host.argtypes = fit_args
     lib.pb200_fit_host.restype = C.c_int
     pred_args = [vp, OP, vp, vp, vp, vp, vp, i64, vp, i32, vp, vp, u64, vp, vp, vp, vp]

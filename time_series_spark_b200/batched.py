@@ -68,6 +68,7 @@ class FittedBatch:
     meta_f64: object     # [N, 4]  y_scale, floor, cap, neg_log_posterior
     smax: int
     kmax: int
+    warm: object = None  # [N] int32 L.WARM_* of a warm-started fit (where each series started); None for a cold fit
 
     @property
     def n(self) -> int:
@@ -82,7 +83,55 @@ class FittedBatch:
             return self
         return FittedBatch(*(x.cpu().numpy() for x in (self.params, self.tchange, self.meta_i32,
                                                        self.meta_i64, self.meta_f64)),
-                           smax=self.smax, kmax=self.kmax)
+                           smax=self.smax, kmax=self.kmax, warm=None if self.warm is None else self.warm.cpu().numpy())
+
+
+def _seasonal_k(mask):
+    """Fourier columns K of a seasonality mask (1 yearly 20 | 2 weekly 6 | 4 daily 8); fbprophet's single zero column
+    when there is none."""
+    mask = np.asarray(mask)
+    k = 20 * (mask & 1 != 0) + 6 * (mask & 2 != 0) + 8 * (mask & 4 != 0)
+    return np.where(k > 0, k, 1)
+
+
+def warm_start(init: FittedBatch, S, mask, fitted) -> tuple:
+    """Where each series of a warm-started fit starts (DESIGN §11, rules 1 and 2), restated on the host: the reference the
+    device's choice (prep_kernel) is tested against.  ``init``: the previous models (host arrays, rows aligned with the
+    batch); ``S`` / ``mask``: the new histories' changepoint count and seasonality mask; ``fitted``: whether a series is
+    optimised at all (False after a prep error or for the constant-linear shortcut).  Returns ``(codes, x)``: int32
+    ``L.WARM_*`` per series, and ``[n, pstride]`` start points in Stan's unconstrained order (k, m, delta[S],
+    log sigma_obs, beta[K]) for the series whose code is ``L.WARM_USED`` (other rows NaN)."""
+    init = init.to_host()
+    S, mask, fitted = np.asarray(S), np.asarray(mask), np.asarray(fitted, dtype=bool)
+    n, smax = init.n, init.smax
+    p, mi = init.params, init.meta_i32
+    K = _seasonal_k(mask)
+    codes = np.full(n, L.WARM_NONE, np.int32)
+    x = np.full(p.shape, np.nan)
+    cand = fitted & (mi[:, 4] >= 0)
+    shape_ok = (mi[:, 1] == S) & (mi[:, 3] == mask)
+    codes[cand & ~shape_ok] = L.WARM_SHAPE
+    col = np.arange(p.shape[1])[None, :]
+    delta_in = (col >= 3) & (col < 3 + S[:, None])
+    beta_in = (col >= 3 + smax) & (col < 3 + smax + K[:, None])
+    used_cols = (col < 2) | delta_in | beta_in
+    with np.errstate(invalid="ignore"):
+        finite = np.all(np.isfinite(p) | ~used_cols, axis=1) & np.isfinite(p[:, 2]) & (p[:, 2] > 0)
+    codes[cand & shape_ok & ~finite] = L.WARM_BAD
+    use = cand & shape_ok & finite
+    for i in np.flatnonzero(use):      # one row per used series: the test reference, not a hot path
+        s_, k_ = int(S[i]), int(K[i])
+        x[i, :3 + s_ + k_] = np.concatenate((p[i, :2], p[i, 3:3 + s_], [np.log(p[i, 2])], p[i, 3 + smax:3 + smax + k_]))
+    codes[use] = L.WARM_USED
+    return codes, x
+
+
+def _check_init(init, n: int, lay) -> None:
+    if not isinstance(init, FittedBatch):
+        raise ValueError("init must be a FittedBatch of the previous models")
+    if init.n != n or init.smax != lay.smax or init.kmax != lay.kmax:
+        raise ValueError(f"init has {init.n} rows with smax {init.smax}, kmax {init.kmax}; the batch has {n} series and the "
+                         f"options' layout smax {lay.smax}, kmax {lay.kmax}")
 
 
 def _y_dtype(y) -> int:
@@ -149,37 +198,91 @@ def fit_batch_trace_host(ctx: L.Context, opts: L.Options, ds_ns: np.ndarray, y: 
     return FittedBatch(params, tchange, mi32, mi64, mf64, lay.smax, lay.kmax), trace
 
 
+def fit_batch_warm_host(ctx: L.Context, opts: L.Options, ds_ns: np.ndarray, y: np.ndarray, offsets: np.ndarray,
+                        floor: float, cap_multiplier: float, init: Optional[FittedBatch], cap: Optional[np.ndarray] = None,
+                        prior: Optional[np.ndarray] = None, trace_cap: int = 0):
+    """pb200_fit_warm_host: ``fit_batch_device(init=...)`` on numpy buffers, plus (``trace_cap`` > 0) the trajectory rows
+    of ``fit_batch_trace_host``.  Returns ``(FittedBatch, trace or None)``; ``FittedBatch.warm`` holds the
+    ``L.WARM_*`` codes when ``init`` is given."""
+    ds_ns = np.ascontiguousarray(ds_ns, dtype=np.int64)
+    y = np.ascontiguousarray(y)
+    offsets = np.ascontiguousarray(offsets, dtype=np.int64)
+    n = offsets.size - 1
+    lay = L.get_layout(opts)
+    params = np.empty((n, lay.pstride), np.float64)
+    tchange = np.empty((n, lay.smax), np.float64)
+    mi32 = np.empty((n, 8), np.int32)
+    mi64 = np.empty((n, 2), np.int64)
+    mf64 = np.empty((n, 4), np.float64)
+    warm = trace = None
+    ip = im = None
+    if init is not None:
+        _check_init(init, n, lay)
+        init = init.to_host()
+        ip = np.ascontiguousarray(init.params, dtype=np.float64)
+        im = np.ascontiguousarray(init.meta_i32, dtype=np.int32)
+        warm = np.empty(n, np.int32)
+    if cap is not None:
+        cap = np.ascontiguousarray(cap, dtype=np.float64)
+    if prior is not None:
+        prior = np.ascontiguousarray(prior, dtype=np.float64).reshape(n, 2)
+    if trace_cap > 0:
+        trace = np.zeros((n, trace_cap, 4), np.float64)
+    if n > 0:
+        ptr = lambda a: None if a is None else _np_ptr(a)     # noqa: E731
+        rc = L.load().pb200_fit_warm_host(ctx.handle, C.byref(opts), _np_ptr(ds_ns), _np_ptr(y), _y_dtype(y),
+                                          _np_ptr(offsets), n, float(floor), float(cap_multiplier), ptr(cap), ptr(prior),
+                                          ptr(ip), ptr(im), _np_ptr(params), _np_ptr(tchange), _np_ptr(mi32), _np_ptr(mi64),
+                                          _np_ptr(mf64), ptr(warm), ptr(trace), int(trace_cap))
+        L.check(rc, "pb200_fit_warm_host")
+    return FittedBatch(params, tchange, mi32, mi64, mf64, lay.smax, lay.kmax, warm=warm), trace
+
+
 def fit_batch_device(ctx: L.Context, opts: L.Options, ds_ns, y, offsets_host: np.ndarray,
                      floor: float, cap_multiplier: float, cap=None, out: Optional[FittedBatch] = None,
-                     sync: bool = True, prior=None) -> FittedBatch:
-    """pb200_fit_prior_device: ``ds_ns`` / ``y`` / ``cap`` are torch CUDA tensors already in HBM.  ``prior``: None (the
+                     sync: bool = True, prior=None, init: Optional[FittedBatch] = None) -> FittedBatch:
+    """pb200_fit_warm_device: ``ds_ns`` / ``y`` / ``cap`` are torch CUDA tensors already in HBM.  ``prior``: None (the
     options' prior scales) or a float64 CUDA tensor ``[n, 2]`` of (changepoint_prior_scale, seasonality_prior_scale)
-    per series; a series whose pair is not finite and > 0 gets status ``L.ST_BAD_PRIOR``."""
+    per series; a series whose pair is not finite and > 0 gets status ``L.ST_BAD_PRIOR``.  ``init``: None (every
+    series starts from fbprophet's stan_init) or the previous models, a FittedBatch (host or device) whose rows are
+    aligned with the batch and whose layout is the options'; each series then starts from its previous optimum when
+    DESIGN §11's rule allows, and ``out.warm`` receives the ``L.WARM_*`` code of every series."""
     import torch
     offsets_host = np.ascontiguousarray(offsets_host, dtype=np.int64)
     n = offsets_host.size - 1
     lay = L.get_layout(opts)
     dev = ds_ns.device
+    if init is not None:
+        _check_init(init, n, lay)
     if out is None:
         out = FittedBatch(torch.empty((n, lay.pstride), dtype=torch.float64, device=dev),
                           torch.empty((n, lay.smax), dtype=torch.float64, device=dev),
                           torch.empty((n, 8), dtype=torch.int32, device=dev),
                           torch.empty((n, 2), dtype=torch.int64, device=dev),
                           torch.empty((n, 4), dtype=torch.float64, device=dev), lay.smax, lay.kmax)
+    ip = im = None
+    if init is not None:
+        ip = torch.as_tensor(init.params, dtype=torch.float64, device=dev).contiguous()
+        im = torch.as_tensor(init.meta_i32, dtype=torch.int32, device=dev).contiguous()
+        if out.warm is None:
+            out.warm = torch.empty(n, dtype=torch.int32, device=dev)
     if n > 0:
         # inputs were produced on torch's current stream; the library has its own stream
         if prior is not None and (prior.dtype != torch.float64 or tuple(prior.shape) != (n, 2) or not prior.is_contiguous()
                                   or prior.device != dev):
             raise ValueError(f"prior must be a contiguous float64 tensor of shape ({n}, 2) on {dev}")
         torch.cuda.current_stream(dev).synchronize()
-        rc = L.load().pb200_fit_prior_device(ctx.handle, C.byref(opts), ds_ns.data_ptr(), y.data_ptr(), _y_dtype(y),
-                                             _np_ptr(offsets_host), n, float(floor), float(cap_multiplier),
-                                             cap.data_ptr() if cap is not None else None,
-                                             prior.data_ptr() if prior is not None else None,
-                                             out.params.data_ptr(), out.tchange.data_ptr(), out.meta_i32.data_ptr(),
-                                             out.meta_i64.data_ptr(), out.meta_f64.data_ptr())
-        L.check(rc, "pb200_fit_prior_device")
-        if sync:
+        rc = L.load().pb200_fit_warm_device(ctx.handle, C.byref(opts), ds_ns.data_ptr(), y.data_ptr(), _y_dtype(y),
+                                            _np_ptr(offsets_host), n, float(floor), float(cap_multiplier),
+                                            cap.data_ptr() if cap is not None else None,
+                                            prior.data_ptr() if prior is not None else None,
+                                            ip.data_ptr() if ip is not None else None,
+                                            im.data_ptr() if im is not None else None,
+                                            out.params.data_ptr(), out.tchange.data_ptr(), out.meta_i32.data_ptr(),
+                                            out.meta_i64.data_ptr(), out.meta_f64.data_ptr(),
+                                            out.warm.data_ptr() if init is not None else None)
+        L.check(rc, "pb200_fit_warm_device")
+        if sync or init is not None:       # (the uploaded copies of init must outlive the call)
             ctx.synchronize()
     return out
 

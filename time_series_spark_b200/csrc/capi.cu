@@ -112,6 +112,8 @@ struct pb200_ctx {
     int grp_g = -1;        // lanes per series of the grouped day-table kernel (fit_group.cuh); PB200_GROUP=0|8|16 pins it
                            // (0 = point_pass_tab), unset = by batch size: 8 from grp_min series on, 16 below
     DevBuf d_trace;        // trajectory rows of pb200_fit_trace_host
+    DevBuf d_warm_x;       // warm start points of pb200_fit_warm_* (prep_kernel -> fit kernels, Newton retry)
+    DevBuf d_prior, d_iparams, d_imeta, d_warm;   // staging of pb200_fit_warm_host's prior scales, previous models, warm codes
     int plain_grp = 0;     // PB200_PLAIN_GROUP=1: the class WITHOUT seasonality (regular grid; reference config #4) on the grouped kernel
                            // too.  Off: it beat one warp per series only at the largest batches measured (500k short series) --
                            // its rounds are longer, and small batches are latency bound
@@ -290,7 +292,7 @@ PB200_API void pb200_destroy(pb200_ctx* c) {
     cudaSetDevice(c->device);
     cudaStreamSynchronize(c->stream);
     for (DevBuf* b : {&c->d_ds, &c->d_y, &c->d_cap, &c->d_params, &c->d_tchange, &c->d_mi32, &c->d_mi64, &c->d_mf64, &c->d_fut,
-                      &c->d_floor, &c->d_yhat, &c->d_lo, &c->d_hi, &c->d_yint, &c->d_mc, &c->d_trace, &c->d_vcount, &c->d_offsets,
+                      &c->d_floor, &c->d_yhat, &c->d_lo, &c->d_hi, &c->d_yint, &c->d_mc, &c->d_trace, &c->d_warm_x, &c->d_prior, &c->d_iparams, &c->d_imeta, &c->d_warm, &c->d_vcount, &c->d_offsets,
                       &c->d_order, &c->d_lenclass, &c->d_qitems, &c->d_qctl, &c->d_nq, &c->d_planes, &c->d_qkey, &c->d_qhist})
         b->release();
     c->h_ctl.release();
@@ -330,7 +332,7 @@ PB200_API int pb200_synchronize(pb200_ctx* c) {
 // newton_kernel over the queue {count, head, items...} at d_nq (16-warp CTAs with ~100 KB of shared memory)
 static int launch_newton(pb200_ctx* c, const pb200_options* opts, const int64_t* d_ds, const void* d_y,
                          int32_t y_dtype, const int64_t* d_offsets, int64_t n_series, int* d_nq, const double* d_prior,
-                         double* d_params, double* d_tchange, int32_t* d_meta_i32, int64_t* d_meta_i64, double* d_meta_f64) {
+                         const double* d_x0, double* d_params, double* d_tchange, int32_t* d_meta_i32, int64_t* d_meta_i64, double* d_meta_f64) {
     pb200_layout L;
     pb200_get_layout(opts, &L);
     if (opts->algorithm == PB200_ALG_LBFGS || L.pstride > pb200::nw::NW_PMAX) return PB200_OK;
@@ -351,6 +353,7 @@ static int launch_newton(pb200_ctx* c, const pb200_options* opts, const int64_t*
     na.kmax = L.kmax;
     na.pstride = L.pstride;
     na.prior = d_prior;
+    na.x0 = d_x0;
     na.o = to_dev(opts);
     const size_t nsm = pb200::nw::newton_smem_bytes(L.pstride);
     CK(cudaFuncSetAttribute(pb200::nw::newton_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)nsm));
@@ -363,12 +366,14 @@ static int launch_newton(pb200_ctx* c, const pb200_options* opts, const int64_t*
 }
 
 // every fit call: zeroes the variant counters, then queues, fit kernels and (unless this is an objective evaluation,
-// d_theta_in set) the Newton retry on the context's stream.  d_prior: per-series prior scales, or null for the options'
+// d_grad_out set) the Newton retry on the context's stream.  d_prior: per-series prior scales, or null for the options'.
+// d_init_params / d_init_meta: previous models to start from (pb200_fit_warm_device), or null
 static int fit_impl(pb200_ctx* c, const pb200_options* opts, const int64_t* d_ds, const void* d_y, int32_t y_dtype,
                     const int64_t* h_offsets, int64_t n_series, double floor, double cap_multiplier,
                     const double* d_cap, const double* d_prior, double* d_params, double* d_tchange, int32_t* d_meta_i32,
                     int64_t* d_meta_i64, double* d_meta_f64, const double* d_theta_in, double* d_grad_out,
-                    double* d_trace = nullptr, int trace_cap = 0) {
+                    double* d_trace = nullptr, int trace_cap = 0, const double* d_init_params = nullptr,
+                    const int32_t* d_init_meta = nullptr, int32_t* d_warm = nullptr) {
     if (!c) return fail(PB200_E_ARG, "ctx is null");
     CK(cudaSetDevice(c->device));
     CK(c->d_vcount.reserve(NQ * 4));
@@ -380,9 +385,15 @@ static int fit_impl(pb200_ctx* c, const pb200_options* opts, const int64_t* d_ds
     if (!d_ds || !d_y || !h_offsets || !d_params || !d_tchange || !d_meta_i32 || !d_meta_i64 || !d_meta_f64)
         return fail(PB200_E_ARG, "null pointer");
     if (y_dtype < 0 || y_dtype > 2) return fail(PB200_E_ARG, "y_dtype");
+    if (d_init_params && !d_init_meta) return fail(PB200_E_ARG, "d_init_meta_i32 is null");
     pb200_layout L;
     pb200_get_layout(opts, &L);
     const int N = (int)n_series;
+    const double* warm_x = nullptr;     // the start points prep_kernel writes for the fit kernels and the Newton retry
+    if (d_init_params) {
+        CK(c->d_warm_x.reserve((size_t)N * L.pstride * 8));
+        warm_x = (const double*)c->d_warm_x.p;
+    }
 
     // ---- host: length classes and longest-first order (counting sort on T) ----
     size_t ctl_bytes = (size_t)(N + 1) * 8 + (size_t)N * 4 * 2;
@@ -473,13 +484,19 @@ static int fit_impl(pb200_ctx* c, const pb200_options* opts, const int64_t* d_ds
         pa.grp_g = grp_g;
         pa.grp_plain = (c->plain_grp && grp_g > 0) ? 1 : 0;
         pa.cv_weight = QKEY_CV_WEIGHT;
-        pa.newton_only = (opts->algorithm == PB200_ALG_NEWTON && !d_theta_in) ? 1 : 0;
+        pa.newton_only = (opts->algorithm == PB200_ALG_NEWTON && !d_grad_out) ? 1 : 0;
         pa.nq_count = nq;
         pa.nq_items = nq + 2;
         pa.vcount = (int*)c->d_vcount.p;
         pa.qkey = (int*)c->d_qkey.p;
         pa.qhist = (int*)c->d_qhist.p;
         pa.prior = d_prior;
+        pa.init_params = d_init_params;
+        pa.init_meta = d_init_meta;
+        pa.warm_x = (double*)warm_x;
+        pa.warm = d_warm;
+        pa.smax = L.smax;
+        pa.pstride = L.pstride;
         const int warps_per_block = 8;
         int grid = (N + warps_per_block - 1) / warps_per_block;
         grid = std::min(grid, c->sms * 8);
@@ -572,7 +589,7 @@ static int fit_impl(pb200_ctx* c, const pb200_options* opts, const int64_t* d_ds
             fa.ppad = ppad;
             fa.planes = (double2*)((char*)c->d_planes.p + g.off);
             fa.nseas_stride = (int)g.slice;
-            fa.theta_in = d_theta_in;
+            fa.theta_in = d_theta_in ? d_theta_in : warm_x;
             fa.grad_out = d_grad_out;
             fa.trace = d_trace;
             fa.trace_cap = trace_cap;
@@ -598,9 +615,9 @@ static int fit_impl(pb200_ctx* c, const pb200_options* opts, const int64_t* d_ds
         }
     }
     // ---- fbprophet's Newton retry over the series whose L-BFGS failed its line search (normally an empty queue) ----
-    if (!d_theta_in)
-        return launch_newton(c, opts, d_ds, d_y, y_dtype, (const int64_t*)c->d_offsets.p, n_series, nq, d_prior, d_params,
-                             d_tchange, d_meta_i32, d_meta_i64, d_meta_f64);
+    if (!d_grad_out)
+        return launch_newton(c, opts, d_ds, d_y, y_dtype, (const int64_t*)c->d_offsets.p, n_series, nq, d_prior, warm_x,
+                             d_params, d_tchange, d_meta_i32, d_meta_i64, d_meta_f64);
     return PB200_OK;
 }
 
@@ -636,14 +653,17 @@ static int stage_host_fit(pb200_ctx* c, const pb200_options* opts, const int64_t
     return PB200_OK;
 }
 
-// pb200_fit_host and pb200_fit_trace_host (traced: trace_cap trajectory rows per series into h_trace): copy in, fit, copy out
+// pb200_fit_host, pb200_fit_trace_host and pb200_fit_warm_host (traced: trace_cap trajectory rows per series into h_trace;
+// h_prior, h_init_params / h_init_meta, h_warm optional): copy in, fit, copy out
 static int fit_host(pb200_ctx* c, const pb200_options* opts, const int64_t* h_ds, const void* h_y, int32_t y_dtype,
                     const int64_t* h_offsets, int64_t n_series, double floor, double cap_multiplier, const double* h_cap,
                     double* h_params, double* h_tchange, int32_t* h_meta_i32, int64_t* h_meta_i64, double* h_meta_f64,
-                    bool traced, double* h_trace, int32_t trace_cap) {
+                    bool traced, double* h_trace, int32_t trace_cap, const double* h_prior = nullptr,
+                    const double* h_init_params = nullptr, const int32_t* h_init_meta = nullptr, int32_t* h_warm = nullptr) {
     int rc = check_host_fit(c, opts, h_ds, h_y, y_dtype, h_offsets, n_series,
                             h_params && h_tchange && h_meta_i32 && h_meta_i64 && h_meta_f64 && (h_trace || !traced));
     if (rc || n_series == 0) return rc;
+    if (h_init_params && !h_init_meta) return fail(PB200_E_ARG, "h_init_meta_i32 is null");
     if (traced && (trace_cap < 1 || (int64_t)trace_cap * n_series > (1LL << 26))) return fail(PB200_E_ARG, "trace_cap");
     if ((rc = stage_host_fit(c, opts, h_ds, h_y, y_dtype, h_offsets, n_series))) return rc;
     pb200_layout L;
@@ -657,11 +677,27 @@ static int fit_host(pb200_ctx* c, const pb200_options* opts, const int64_t* h_ds
         CK(c->d_trace.reserve(tbytes));
         CK(cudaMemsetAsync(c->d_trace.p, 0, tbytes, c->stream));
     }
+    if (h_prior) {
+        CK(c->d_prior.reserve(N * 2 * 8));
+        CK(cudaMemcpyAsync(c->d_prior.p, h_prior, N * 2 * 8, cudaMemcpyHostToDevice, c->stream));
+    }
+    if (h_init_params) {
+        CK(c->d_iparams.reserve(N * L.pstride * 8));
+        CK(c->d_imeta.reserve(N * 8 * 4));
+        CK(cudaMemcpyAsync(c->d_iparams.p, h_init_params, N * L.pstride * 8, cudaMemcpyHostToDevice, c->stream));
+        CK(cudaMemcpyAsync(c->d_imeta.p, h_init_meta, N * 8 * 4, cudaMemcpyHostToDevice, c->stream));
+    }
+    const bool warm_out = h_init_params && h_warm;
+    if (warm_out) CK(c->d_warm.reserve(N * 4));
     rc = fit_impl(c, opts, (const int64_t*)c->d_ds.p, c->d_y.p, y_dtype, h_offsets, n_series, floor, cap_multiplier,
-                  h_cap ? (const double*)c->d_cap.p : nullptr, nullptr, (double*)c->d_params.p, (double*)c->d_tchange.p,
+                  h_cap ? (const double*)c->d_cap.p : nullptr, h_prior ? (const double*)c->d_prior.p : nullptr,
+                  (double*)c->d_params.p, (double*)c->d_tchange.p,
                   (int32_t*)c->d_mi32.p, (int64_t*)c->d_mi64.p, (double*)c->d_mf64.p, nullptr, nullptr,
-                  traced ? (double*)c->d_trace.p : nullptr, trace_cap);
+                  traced ? (double*)c->d_trace.p : nullptr, trace_cap,
+                  h_init_params ? (const double*)c->d_iparams.p : nullptr,
+                  h_init_params ? (const int32_t*)c->d_imeta.p : nullptr, warm_out ? (int32_t*)c->d_warm.p : nullptr);
     if (rc) return rc;
+    if (warm_out) CK(cudaMemcpyAsync(h_warm, c->d_warm.p, N * 4, cudaMemcpyDeviceToHost, c->stream));
     CK(cudaMemcpyAsync(h_params, c->d_params.p, N * L.pstride * 8, cudaMemcpyDeviceToHost, c->stream));
     CK(cudaMemcpyAsync(h_tchange, c->d_tchange.p, N * L.smax * 8, cudaMemcpyDeviceToHost, c->stream));
     CK(cudaMemcpyAsync(h_meta_i32, c->d_mi32.p, N * 8 * 4, cudaMemcpyDeviceToHost, c->stream));
@@ -680,6 +716,28 @@ PB200_API int pb200_fit_prior_device(pb200_ctx* c, const pb200_options* opts, co
                                      double* d_tchange, int32_t* d_meta_i32, int64_t* d_meta_i64, double* d_meta_f64) {
     return fit_impl(c, opts, d_ds, d_y, y_dtype, h_offsets, n_series, floor, cap_multiplier, d_cap, d_prior, d_params,
                     d_tchange, d_meta_i32, d_meta_i64, d_meta_f64, nullptr, nullptr);
+}
+
+PB200_API int pb200_fit_warm_device(pb200_ctx* c, const pb200_options* opts, const int64_t* d_ds, const void* d_y,
+                                    int32_t y_dtype, const int64_t* h_offsets, int64_t n_series, double floor,
+                                    double cap_multiplier, const double* d_cap, const double* d_prior,
+                                    const double* d_init_params, const int32_t* d_init_meta_i32, double* d_params,
+                                    double* d_tchange, int32_t* d_meta_i32, int64_t* d_meta_i64, double* d_meta_f64,
+                                    int32_t* d_warm) {
+    return fit_impl(c, opts, d_ds, d_y, y_dtype, h_offsets, n_series, floor, cap_multiplier, d_cap, d_prior, d_params,
+                    d_tchange, d_meta_i32, d_meta_i64, d_meta_f64, nullptr, nullptr, nullptr, 0, d_init_params,
+                    d_init_meta_i32, d_init_params ? d_warm : nullptr);
+}
+
+PB200_API int pb200_fit_warm_host(pb200_ctx* c, const pb200_options* opts, const int64_t* h_ds, const void* h_y,
+                                  int32_t y_dtype, const int64_t* h_offsets, int64_t n_series, double floor,
+                                  double cap_multiplier, const double* h_cap, const double* h_prior,
+                                  const double* h_init_params, const int32_t* h_init_meta_i32, double* h_params,
+                                  double* h_tchange, int32_t* h_meta_i32, int64_t* h_meta_i64, double* h_meta_f64,
+                                  int32_t* h_warm, double* h_trace, int32_t trace_cap) {
+    return fit_host(c, opts, h_ds, h_y, y_dtype, h_offsets, n_series, floor, cap_multiplier, h_cap, h_params, h_tchange,
+                    h_meta_i32, h_meta_i64, h_meta_f64, h_trace != nullptr, h_trace, trace_cap, h_prior, h_init_params,
+                    h_init_meta_i32, h_warm);
 }
 
 PB200_API int pb200_fit_device(pb200_ctx* c, const pb200_options* opts, const int64_t* d_ds, const void* d_y, int32_t y_dtype,

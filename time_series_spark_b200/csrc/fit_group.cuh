@@ -1373,6 +1373,7 @@ __device__ __noinline__ bool g_fetch(GState<G, SEAS>& s, const FitArgs& a, doubl
         }
         double* x = s.vec[0];
         const double* th = a.theta_in ? a.theta_in + (size_t)sidx * a.pstride : nullptr;
+        if (th && !a.grad_out && !(th[0] == th[0])) th = nullptr;     // warm start: this series starts cold
 #pragma unroll 1
         for (int q = gl; q < P; q += G) x[q] = th ? th[q] : (q == 0 ? k0 : (q == 1 ? m0 : 0.0));
     }
@@ -1407,7 +1408,7 @@ __device__ __noinline__ void g_write_record(GState<G, SEAS>& s, const FitArgs& a
         }
         pr[q] = v;
     }
-    if (a.theta_in) {
+    if (a.grad_out) {
         const double* g = s.vec[s.ls.ig];
         double* go = a.grad_out + (size_t)sidx * a.pstride;
         const int P = S + gkx<SEAS>() + 3;
@@ -1493,7 +1494,7 @@ __global__ void __launch_bounds__(32, G != 8 ? 16 : (SEAS ? PB200_GRP_BLOCKS : P
                 }
                 lp.j0 = reinterpret_cast<const int*>(&s.vec[1][0] + (SEAS ? 6 * G : 0))[gl];
                 int st = ST_FIRST;
-                if (a.theta_in) st = ST_OBJ;
+                if (a.grad_out) st = ST_OBJ;
                 else if (s.st0 == PB200_ST_CONST_LINEAR) {
                     g_write_record<G, SEAS>(s, a, PB200_ST_CONST_LINEAR, gl, gm);
                     st = ST_IDLE;

@@ -41,6 +41,7 @@ struct NewtonArgs {
     double* meta_f64;
     int smax, kmax, pstride;
     const double* prior;     // per-series prior scales (FitArgs::prior); null: o's
+    const double* x0;        // warm start points (PrepArgs::warm_x, k = NaN: cold); null: every series from stan_init
     FitOptsDev o;
 };
 
@@ -348,8 +349,10 @@ __global__ void __launch_bounds__(32 * NW_WARPS, 1) newton_kernel(const NewtonAr
                 sr.tc[tid] = 0.0;
             }
         }
-        // ---- initial point: the same stan_init the L-BFGS run started from ----
+        // ---- initial point: the same stan_init (or warm start point) the L-BFGS run started from ----
         if (tid == 0) {
+            const double* w = a.x0 ? a.x0 + (size_t)sidx * a.pstride : nullptr;
+            if (w && !(w[0] == w[0])) w = nullptr;
             const int i1max = mi[7];
             const double y0 = (load_y(a.y, a.y_dtype, sr.off) - sr.fl) / sr.y_scale;
             const double y1 = (load_y(a.y, a.y_dtype, sr.off + i1max) - sr.fl) / sr.y_scale;
@@ -368,7 +371,7 @@ __global__ void __launch_bounds__(32 * NW_WARPS, 1) newton_kernel(const NewtonAr
                 k0 = (y1 - y0) / t1v;
                 m0 = y0 - k0 * 0.0;
             }
-            for (int q = 0; q < P; ++q) sr.x[q] = q == 0 ? k0 : (q == 1 ? m0 : 0.0);
+            for (int q = 0; q < P; ++q) sr.x[q] = w ? w[q] : (q == 0 ? k0 : (q == 1 ? m0 : 0.0));
         }
         __syncthreads();
         // services::optimize::newton: lp at the initial point (an error there is caught: lp = -inf)

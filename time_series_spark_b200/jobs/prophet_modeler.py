@@ -13,6 +13,14 @@ Optional keys beyond the reference (defaults reproduce prophet_modeler.py:65 exa
 ``model.growth``, ``model.seasonality_mode``, ``model.yearly_seasonality``,
 ``model.weekly_seasonality``, ``model.daily_seasonality``, ``model.n_changepoints``,
 ``model.changepoint_range``, ``model.changepoint_prior_scale``, ``model.seasonality_prior_scale``.
+
+``io.warm_start`` (optional): the path of a previous models table, for a job re-run on a schedule over the same groups
+plus new rows (fbprophet's "updating fitted models", ``m.fit(df, init=stan_init(m_old))``).  Every group starts its
+fit from its row of that table when the row's changepoint count and seasonalities are those of the new history
+(DESIGN §11), else from fbprophet's cold start; one line reports how many were warm, how many cold and why, and
+how many table rows matched no input group.  The table must have been fitted with the job's growth, seasonality mode,
+seasonality switches and ``n_changepoints``.  It may be ``io.models`` itself: the old table is read before it is
+replaced.  Without the key the job is the cold fit it has always been.
 """
 from __future__ import annotations
 
@@ -84,6 +92,72 @@ def who(series_id, dim_id, mask) -> str:
             f"{int(np.count_nonzero(mask))} group(s) in all)")
 
 
+def _group_keys(series_id, dim_id) -> np.ndarray:
+    """One int64 key per (series_id, dim_id) group."""
+    return (np.asarray(series_id, dtype=np.int64) << 32) | (np.asarray(dim_id, dtype=np.int64) & 0xFFFFFFFF)
+
+
+def warm_start_init(table: pa.Table, opts: L.Options, series_id, dim_id, path: str = "io.warm_start"):
+    """The previous models of the packed groups ``(series_id, dim_id)`` from a models table (MODEL_OUTPUT_SCHEMA), as
+    the ``init`` of ``batched.fit_batch_device``: a host FittedBatch in the groups' order whose rows without a previous
+    model have status -1.  Returns ``(init, unmatched)``, ``unmatched`` the number of table rows that match no group.
+    Raises ValueError (naming ``path``) for a table fitted with other options, and for duplicate keys."""
+    lay = L.get_layout(opts)
+    n = len(series_id)
+    gkey = _group_keys(series_id, dim_id)
+    init = batched.FittedBatch(np.zeros((n, lay.pstride)), np.zeros((n, lay.smax)), np.zeros((n, 8), np.int32),
+                               np.zeros((n, 2), np.int64), np.zeros((n, 4)), lay.smax, lay.kmax)
+    init.meta_i32[:, 4] = -1
+    if table.num_rows == 0:
+        return init, 0
+    tsid = table["series_id"].combine_chunks().to_numpy(zero_copy_only=False)
+    tdid = table["dim_id"].combine_chunks().to_numpy(zero_copy_only=False)
+    tkey = _group_keys(tsid, tdid)
+    order = np.argsort(tkey, kind="stable")
+    skey = tkey[order]
+    dup = np.zeros(tkey.size, bool)
+    dup[order[1:][skey[1:] == skey[:-1]]] = True
+    if dup.any():
+        raise ValueError(f"{path} holds more than one model for a (series_id, dim_id) group." + who(tsid, tdid, dup))
+    prev, _, info = model_record.decode(table["model"])
+    want = {"logistic": opts.growth == L.GROWTH_LOGISTIC, "multiplicative": bool(opts.multiplicative),
+            "yearly": int(opts.yearly), "weekly": int(opts.weekly), "daily": int(opts.daily),
+            "n_changepoints": int(opts.n_changepoints)}
+    diff = sorted(k for k in want if info[k] != want[k])
+    if diff:
+        raise ValueError(f"{path} was fitted with other options than this job's: " +
+                         ", ".join(f"{k} {info[k]!r} (job: {want[k]!r})" for k in diff))
+    pos = np.minimum(np.searchsorted(skey, gkey), skey.size - 1)
+    hit = skey[pos] == gkey
+    rows = order[pos[hit]]
+    init.params[hit] = prev.params[rows]
+    init.meta_i32[hit] = prev.meta_i32[rows]
+    init.meta_i64[hit] = prev.meta_i64[rows]
+    init.meta_f64[hit] = prev.meta_f64[rows]
+    init.tchange[hit] = prev.tchange[rows]
+    gsorted = np.sort(gkey)
+    gp = np.minimum(np.searchsorted(gsorted, tkey), max(gsorted.size - 1, 0))
+    unmatched = int(np.count_nonzero(gsorted[gp] != tkey)) if gsorted.size else int(tkey.size)
+    return init, unmatched
+
+
+def read_warm_start(path: str, series_id) -> pa.Table:
+    """The rows of the models table at ``path`` whose series_id is one of ``series_id`` (under torchrun: this rank's)."""
+    import pyarrow.compute as pc
+    sids = pa.array(np.unique(np.asarray(series_id, dtype=np.int32)), pa.int32())
+    return pads.dataset(path, format="parquet").to_table(filter=pc.field("series_id").isin(sids))
+
+
+def warm_report(warm, unmatched: int) -> str:
+    """The job's one line about where its fits started."""
+    w = np.asarray(warm)
+    return (f"Warm start: {int(np.count_nonzero(w == L.WARM_USED))} series warm; cold: "
+            f"{int(np.count_nonzero(w == L.WARM_NONE))} without a previous model or not optimised, "
+            f"{int(np.count_nonzero(w == L.WARM_SHAPE))} whose changepoints or seasonalities changed, "
+            f"{int(np.count_nonzero(w == L.WARM_BAD))} with unusable previous values; "
+            f"{unmatched} table row(s) matched no input group")
+
+
 def models_table(fitted: batched.FittedBatch, series_id, dim_id, last_ds, opts: L.Options, floor) -> pa.Table:
     """The models table (MODEL_OUTPUT_SCHEMA) of a fitted batch (host arrays).  fbprophet's ValueErrors (cap <= floor,
     bad input) raise, naming the group; a failed fit (status < 0) -- the reference's RuntimeError -- prints a line and
@@ -146,8 +220,14 @@ class _ModelTimeSeriesOp:
         short = np.diff(pk.offsets) < 2
         if np.any(short):
             raise ValueError("Dataframe has less than 2 non-NaN rows." + who(pk.series_id, pk.dim_id, short))
+        warm_path = (self.config.get("io") or {}).get("warm_start")
+        init = None
+        if warm_path:
+            init, unmatched = warm_start_init(read_warm_start(warm_path, pk.series_id), opts, pk.series_id, pk.dim_id)
         fitted = batched.fit_batch_device(ctx, opts, pk.ds.contiguous(), pk.y.contiguous(), pk.offsets,
-                                          float(floor), float(cap_multiplier)).to_host()
+                                          float(floor), float(cap_multiplier), init=init).to_host()
+        if warm_path:
+            print(warm_report(fitted.warm, unmatched))
         t_fit = time.time()
         out = models_table(fitted, pk.series_id, pk.dim_id, pk.last_ds, opts, floor)
         # wall time per stage of the last call (tools/e2e_scaling.py reports them): upload + group + sort, GPU fit + D2H, encode
@@ -238,6 +318,8 @@ class ProphetModeler:
         """Parquet, mode='overwrite' (reference :118-125); one part file per writer."""
         out = self.config["io"]["models"]
         rank = pdist.world()[0]
+        if self.config["io"].get("warm_start"):
+            pdist.barrier()                 # io.warm_start may be io.models: every rank has read it before rank 0 clears it
         pdist.prepare_output_dir(out)
         pq.write_table(model_df.table, os.path.join(out, f"part-{rank:05d}.parquet"))
 
