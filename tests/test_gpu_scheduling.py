@@ -15,10 +15,14 @@ options are not always the defaults.  These tests reach all of that at test size
     options the C ABI accepts (changepoints, changepoint range, history size, max_iter, seasonality prior scale).
 """
 import os
+import sys
 
 import numpy as np
 import pytest
 
+sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))     # the helper module next to this file
+import fit_oracle  # noqa: E402
+from fit_oracle import grp_chunk  # noqa: E402
 from oracle import prophet_oracle as po
 from time_series_spark_b200 import _lib as L
 from time_series_spark_b200 import batched, synth
@@ -38,19 +42,6 @@ FAMILIES = {
 }
 
 
-def _ctx_with_env(**env):
-    old = {k: os.environ.get(k) for k in env}
-    os.environ.update({k: str(v) for k, v in env.items()})
-    try:
-        return L.Context(0)
-    finally:
-        for k, v in old.items():
-            if v is None:
-                del os.environ[k]
-            else:
-                os.environ[k] = v
-
-
 @pytest.fixture(scope="module")
 def ctx_for():
     """ctx_for(family, **more_env) -> a context of the module (one per distinct environment)."""
@@ -60,7 +51,7 @@ def ctx_for():
         env = dict(FAMILIES[family], **more)
         key = tuple(sorted((k, str(v)) for k, v in env.items()))
         if key not in cache:
-            cache[key] = _ctx_with_env(**env)
+            cache[key] = fit_oracle.ctx_with_env(**env)
         return cache[key]
 
     yield get
@@ -69,14 +60,6 @@ def ctx_for():
 
 
 # ---- host mirrors of the grouped kernel's geometry (fit_kernel.cuh grp_chunk, fit_group.cuh group_plane_doubles) ----
-def grp_chunk(T, P, G, U=2):
-    c0 = (T + G - 1) // G
-    for c in range(c0, c0 + 25):
-        if all(U - 1 < (c * dl) % P < P - (U - 1) for dl in range(1, G)):
-            return c
-    return -1
-
-
 def last_lane_points(T, step_min, G):
     return max(0, T - (G - 1) * grp_chunk(T, NS_DAY // (step_min * NS_MIN), G))
 
@@ -144,24 +127,6 @@ def test_mixed_lengths_are_the_edges_they_claim():
         assert grp_chunk(T, NS_DAY // (st * NS_MIN), 16) > (T + 15) // 16    # widened: the last lane runs short
 
 
-def _thetas(b, oopts, lay, rng, steep=False):
-    rows, preps = [], []
-    for i in range(b.n):
-        a, e = b.offsets[i], b.offsets[i + 1]
-        y = b.y[a:e].astype(np.float64)
-        p = po.prepare(b.ds[a:e], y, 0.0, y.max() * 1.1, oopts)
-        th = po.initial_theta(p) + 0.05 * rng.randn(p.S + p.K + 3)
-        if steep:
-            # a steep falling logistic trend: k (t - m) = -520 t stays inside +-600 on the series' own t in [0, 1], so the
-            # kernel takes its exp-ratio recurrence; past t ~ 1.36 exp(520 t) overflows a double
-            th[0], th[1], th[2:2 + p.S] = -520.0, 0.0, 0.0
-        row = np.zeros(lay.pstride)
-        row[:th.size] = th
-        rows.append(row)
-        preps.append((p, th))
-    return np.array(rows), preps
-
-
 @pytest.mark.parametrize("point", ["near_initial", "steep"])
 @pytest.mark.parametrize("which", list(MIXED))
 def test_mixed_warp_objective_matches_oracle_and_series_alone(ctx_for, which, point):
@@ -170,7 +135,7 @@ def test_mixed_warp_objective_matches_oracle_and_series_alone(ctx_for, which, po
     b = _batch(specs)
     opts, oopts = batched.make_options(), po.ProphetOptions()
     lay = L.get_layout(opts)
-    th, preps = _thetas(b, oopts, lay, np.random.RandomState(3), steep=point == "steep")
+    th, preps = fit_oracle.thetas(b, oopts, lay, np.random.RandomState(3), steep=point == "steep")
     f, g, mi = batched.objective_host(ctx, opts, b.ds, b.y, b.offsets, 0.0, 1.1, th)
     vc = ctx.last_fit_variant_counts()
     assert vc[3, 6] == b.n and vc.sum() == b.n, vc
@@ -278,23 +243,6 @@ def test_grid_cap_changes_no_result(ctx_for, case):
         _assert_same_fit(runs[0], runs[cap], (case, cap))
 
 
-def _oracle_rows(ds, y, oopts):
-    rows = []
-    fr = po.fit(ds, y, opts=oopts, algorithm="LBFGS", trace=rows)
-    return fr, np.array(rows).reshape(-1, 4)
-
-
-def _assert_trajectory_head(tr, n_gpu, rows, what, n_head=6):
-    """The first accepted iterations against the oracle, at the tolerances of test_lbfgs_trajectory_matches_oracle."""
-    head = min(n_gpu, len(rows), n_head)
-    assert head >= 1, what
-    g, o = tr[:head], rows[:head]
-    assert np.array_equal(g[:, 0], np.arange(1, head + 1)), what
-    assert np.array_equal(g[:, 3], o[:, 3]), (what, g[:, 3], o[:, 3])
-    assert np.all(np.abs(g[:, 1] - o[:, 1]) <= 1e-11 * np.maximum(1.0, np.abs(o[:, 1]))), what
-    assert np.all(np.abs(g[:, 2] - o[:, 2]) <= 1e-7 * np.abs(o[:, 2])), what
-
-
 def test_reused_slots_follow_the_oracle(ctx_for):
     """At one CTA a G = 8 warp fits the 16 series of the mixed batch four at a time, groups refilling on different
     rounds: every series' first iterations still match the oracle's."""
@@ -305,10 +253,10 @@ def test_reused_slots_follow_the_oracle(ctx_for):
     oopts = po.ProphetOptions(max_iter=6)
     for i in range(b.n):
         a, e = b.offsets[i], b.offsets[i + 1]
-        fr, rows = _oracle_rows(b.ds[a:e], b.y[a:e].astype(np.float64), oopts)
+        fr, rows = fit_oracle.oracle_rows(b.ds[a:e], b.y[a:e].astype(np.float64), oopts)
         assert fb.meta_i32[i, 4] >= 0
         assert np.array_equal(fb.tchange[i, :fr.prep.S], fr.prep.t_change)
-        _assert_trajectory_head(tr[i], int(fb.meta_i32[i, 5]), rows, i)
+        fit_oracle.assert_trajectory_head(tr[i], int(fb.meta_i32[i, 5]), rows, i)
 
 
 def test_stale_workspace_from_a_longer_batch_changes_nothing(ctx_for):
@@ -317,8 +265,8 @@ def test_stale_workspace_from_a_longer_batch_changes_nothing(ctx_for):
     opts = batched.make_options()
     short = _batch([ODD30, ODD20, ODD15, ZERO30, ONE30, (1500, 15, "2021-03-05T01:15")])
     long_ = _batch([(8000, 15, f"2021-03-0{d}T0{d}:15") for d in range(1, 9)])
-    used = _ctx_with_env(**FAMILIES["g8"])
-    fresh = _ctx_with_env(**FAMILIES["g8"])
+    used = fit_oracle.ctx_with_env(**FAMILIES["g8"])
+    fresh = fit_oracle.ctx_with_env(**FAMILIES["g8"])
     try:
         batched.fit_batch_trace_host(used, opts, long_.ds, long_.y, long_.offsets, 0.0, 1.1, trace_cap=16)
         x = batched.fit_batch_trace_host(used, opts, short.ds, short.y, short.offsets, 0.0, 1.1, trace_cap=16)
@@ -380,7 +328,7 @@ def test_options_on_the_grouped_kernel(ctx_for, case):
     cell = (1, 6) if kw.get("n_changepoints") == 28 else (3, 6)
     lay = L.get_layout(opts)
     # objective and gradient at random points near the initial one
-    th, preps = _thetas(b, oopts, lay, np.random.RandomState(9))
+    th, preps = fit_oracle.thetas(b, oopts, lay, np.random.RandomState(9))
     f, g, mi = batched.objective_host(ctx, opts, b.ds, b.y, b.offsets, 0.0, 1.1, th)
     assert ctx.last_fit_variant_counts()[cell] == b.n, (case, ctx.last_fit_variant_counts())
     for i, (p, t) in enumerate(preps):
@@ -400,11 +348,11 @@ def test_options_on_the_grouped_kernel(ctx_for, case):
     for i in range(b.n):
         a, e = b.offsets[i], b.offsets[i + 1]
         o_run = oopts if short_run else po.ProphetOptions(history_size=hist, **dict(kw, max_iter=6))
-        fr, rows = _oracle_rows(b.ds[a:e], b.y[a:e].astype(np.float64), o_run)
+        fr, rows = fit_oracle.oracle_rows(b.ds[a:e], b.y[a:e].astype(np.float64), o_run)
         S = fr.prep.S
         assert fb.meta_i32[i, 1] == S and np.array_equal(fb.tchange[i, :S], fr.prep.t_change), (case, i)
         assert np.all(fb.tchange[i, S:] == 0.0)
-        _assert_trajectory_head(tr[i], int(fb.meta_i32[i, 5]), rows, (case, i), n_head=n_head)
+        fit_oracle.assert_trajectory_head(tr[i], int(fb.meta_i32[i, 5]), rows, (case, i), n_head=n_head)
         if short_run:
             assert fb.meta_i32[i, 4] == fr.ret and fb.meta_i32[i, 5] == fr.iters, (case, i, fb.meta_i32[i], fr.ret, fr.iters)
             if kw["max_iter"] == 1:

@@ -40,19 +40,25 @@ def _report_measured_deviations():
           f"max |predict_kernel - oracle| under the stated rule = {_measured['predict']:.3e}")
 
 
-# history shapes whose auto seasonalities give each mask: (step, points)
-_MASK_HIST = {7: (12 * H_NS, 1600),   # 800 days at 12 h: yearly + weekly + daily
-              6: (H_NS, 720),         # 30 days hourly: weekly + daily
-              2: (DAY, 60),           # 60 days daily: weekly
-              0: (MIN15, 96)}         # one day: none
+# history shapes whose seasonalities give each mask: (step, points, weekly_seasonality switch)
+_MASK_HIST = {7: (12 * H_NS, 1600, "auto"),   # 800 days at 12 h: yearly + weekly + daily
+              6: (H_NS, 720, "auto"),         # 30 days hourly: weekly + daily
+              5: (12 * H_NS, 1600, False),    # 800 days at 12 h without weekly: yearly + daily
+              4: (H_NS, 240, "auto"),         # 10 days hourly: daily
+              3: (DAY, 801, "auto"),          # 800 days daily: yearly + weekly
+              2: (DAY, 60, "auto"),           # 60 days daily: weekly
+              1: (7 * DAY, 115, "auto"),      # 798 days weekly: yearly
+              0: (MIN15, 96, "auto")}         # one day: none
+ALL_MASKS = (7, 6, 5, 4, 3, 2, 1, 0)
 
 
 @functools.lru_cache(maxsize=None)
 def _prep(mask, growth, mode, ncp=25, start="2021-03-01", cpr=0.8):
-    step, T = _MASK_HIST[mask]
+    step, T, weekly = _MASK_HIST[mask]
     ds = np.datetime64(start, "ns").astype(np.int64) + step * np.arange(T, dtype=np.int64)
     y = 100.0 + 20.0 * np.sin(np.arange(T) / 7.0) + np.arange(T) % 5
-    oopts = po.ProphetOptions(growth=growth, seasonality_mode=mode, n_changepoints=ncp, changepoint_range=cpr)
+    oopts = po.ProphetOptions(growth=growth, seasonality_mode=mode, n_changepoints=ncp, changepoint_range=cpr,
+                              weekly_seasonality=weekly)
     p = po.prepare(ds, y, 0.0, 1.1 * y.max(), oopts)
     assert sum(mcs._MASK_BIT[s.name] for s in p.seasonalities) == mask
     return p, oopts
@@ -145,15 +151,14 @@ def test_unsupported_sample_count_is_refused(gpu_ctx, n):
 @pytest.mark.parametrize("growth,mode", [("logistic", "multiplicative"), ("logistic", "additive"),
                                          ("linear", "multiplicative"), ("linear", "additive")])
 def test_mc_matches_restatement_many_models(gpu_ctx, growth, mode, seed):
-    """300 models (more than the grid: every CTA loops over models), masks 7 / 6 / 2 / 0 mixed, 30 changepoints, every
+    """300 models (more than the grid: every CTA loops over models), all eight masks mixed, 30 changepoints, every
     fifth model forecast inside its history (Tmax <= 1: no simulated changepoint), failed rows interleaved; a horizon of
     17 points (one full 16-point tile and a tail of one)."""
     rng = np.random.RandomState(1)
     H, N = 17, 300
-    masks = [7, 6, 2, 0]
     frs, fut = [], []
     for i in range(N):
-        p, _ = _prep(masks[i % 4], growth, mode, ncp=30)
+        p, _ = _prep(ALL_MASKS[i % len(ALL_MASKS)], growth, mode, ncp=30)
         frs.append(_model(p, rng))
         fut.append(_future(p, H, in_history=(i % 5 == 3)))
     status = np.where(np.arange(N) % 7 == 5, L.ST_TOO_FEW, 0)
@@ -297,13 +302,13 @@ def _epilogue(yhat, floor):
 @pytest.mark.parametrize("growth,mode", [("logistic", "multiplicative"), ("logistic", "additive"),
                                          ("linear", "multiplicative"), ("linear", "additive")])
 def test_predict_matches_oracle_every_segment_and_era(gpu_ctx, growth, mode):
-    """One batch under auto seasonality with masks 7, 6, 2 and 0 (K = 34 / 14 / 6 / 0 packed into 34 columns); histories
-    in 1959, 2021 and 2250; timestamps across the whole history (every trend segment, the first point before the first
-    changepoint included) and past its end."""
+    """One batch with all eight masks (K = 34 / 14 / 28 / 8 / 26 / 6 / 20 / 0 packed into 34 columns: every block of beta
+    at every offset a missing block leaves); histories in 1959, 2021 and 2250; timestamps across the whole history
+    (every trend segment, the first point before the first changepoint included) and past its end."""
     rng = np.random.RandomState(5)
     frs, fut = [], []
     for start in ("1959-06-01", "2021-03-01", "2250-01-01"):
-        for mask in (7, 6, 2, 0):
+        for mask in ALL_MASKS:
             p, oopts = _prep(mask, growth, mode, start=start)
             frs.append(_model(p, rng))
             inside = p.ds_sorted[np.linspace(0, p.T - 1, 64).round().astype(int)]
