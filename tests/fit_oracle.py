@@ -71,3 +71,76 @@ def assert_trajectory_head(tr, n_gpu, rows, what, n_head=6):
     assert np.all(df <= 1e-11), (what, df)
     da = np.abs(g[:, 2] - o[:, 2]) / np.abs(o[:, 2])
     assert np.all(da <= 1e-7), (what, da)
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# fbprophet's Newton run held per iteration (tests/test_newton_steps.py, tests/test_wide_params.py)
+# ---------------------------------------------------------------------------------------------------------------------
+def seasonal_k(mask):
+    """Fourier columns of a seasonality mask (yearly 20 | weekly 6 | daily 8), fbprophet's one zero column without any."""
+    k = 20 * bool(mask & 1) + 6 * bool(mask & 2) + 8 * bool(mask & 4)
+    return k if k else 1
+
+
+def record_theta(fb, i):
+    """Row i of a fitted batch as Stan's unconstrained point (k, m, delta[S], log sigma_obs, beta[K]), in the record's
+    folded form: without changepoints (n_cp_real 0) k holds k + delta[0] and delta is zero, and the single zero column of a
+    history without seasonality is recorded as 0."""
+    mi, p = fb.meta_i32[i], fb.params[i]
+    S, K = int(mi[1]), seasonal_k(int(mi[3]))
+    return np.concatenate(([p[0], p[1]], p[3:3 + S], [np.log(p[2])], p[3 + fb.smax:3 + fb.smax + K]))
+
+
+def folded(theta, S, ncp, mask):
+    """An oracle's unconstrained point in record_theta's form."""
+    th = np.array(theta, dtype=np.float64)
+    if ncp == 0:
+        th[0] += th[2]
+        th[2:2 + S] = 0.0
+    if mask == 0:
+        th[3 + S:] = 0.0
+    return th
+
+
+def c_newton_opts(growth, mode, extra, n_changepoints, max_iter):
+    """The C oracle's options for fbprophet's Newton run alone (``extra``: the Prophet seasonality switches)."""
+    from oracle import c_oracle as co
+    sw = {True: 1, False: 0}
+    o = co.options(growth=growth, seasonality_mode=mode, yearly=sw.get(extra.get("yearly_seasonality"), -1),
+                   weekly=sw.get(extra.get("weekly_seasonality"), -1), daily=sw.get(extra.get("daily_seasonality"), -1))
+    o.n_changepoints = n_changepoints
+    o.max_iter = max_iter
+    o.algorithm = co.ALG_NEWTON
+    return o
+
+
+def newton_bound(gpu, ref, other, scale, floor=1e-10):
+    """|gpu - ref|, and the bound it is held to: ten times the two CPU oracles' disagreement |other - ref| plus a floor of
+    ``floor`` of the quantity's size (max norm over a vector)."""
+    d = float(np.max(np.abs(np.asarray(gpu) - ref)))
+    return d, 10.0 * float(np.max(np.abs(np.asarray(other) - ref))) + floor * max(1.0, float(np.max(np.abs(scale))))
+
+
+def assert_newton_row(fb, i, fr, c_theta, c_f, c_info, measured, what):
+    """Row i of a Newton fit against the numpy oracle's FitResult ``fr`` and the C oracle's (theta, f, info) row: status
+    60, iteration and evaluation counts equal to both, changepoints exact, theta and objective within newton_bound."""
+    p = fr.prep
+    S, P, mask = p.S, p.S + p.K + 3, sum({"yearly": 1, "weekly": 2, "daily": 4}[s.name] for s in p.seasonalities)
+    mi = fb.meta_i32[i]
+    assert (int(mi[0]), int(mi[1]), int(mi[3])) == (p.T, S, mask), (what, mi)
+    assert mi[4] == 60 == fr.ret == c_info[0], (what, mi, fr.ret, c_info)
+    assert (mi[5], mi[6]) == (fr.iters, fr.n_evals) == (c_info[1], c_info[2]), (what, mi, fr.iters, fr.n_evals, c_info)
+    assert np.array_equal(fb.tchange[i, :S], p.t_change) and np.all(fb.tchange[i, S:] == 0.0), what
+    # the objective's floor is 1e-8: away from the optimum f moves with g . dtheta, and the two oracles' objectives can
+    # agree far more closely than their theta does (GPU measured up to 5.3e-9 relative where numpy and C are 1e-10 apart)
+    df, bf = newton_bound(fb.meta_f64[i, 3], fr.neg_logp, c_f, fr.neg_logp, floor=1e-8)
+    th_np = folded(fr.theta, S, p.n_changepoints_real, mask)
+    th_c = folded(c_theta[:P], S, p.n_changepoints_real, mask)
+    # theta's floor is 1e-10, and 1e-7 on yearly + weekly + daily series: their Hessian is ill-conditioned along the
+    # Laplace kinks, the two oracles' theta spread there to 2.4e-7, and they can happen to agree much more closely
+    # (GPU measured 3.8e-8 at P = 65 after five iterations where numpy and C were 6e-10 apart)
+    dt, bt = newton_bound(record_theta(fb, i), th_np, th_c, th_np, floor=1e-7 if mask == 7 else 1e-10)
+    measured["f"] = max(measured.get("f", 0.0), df / bf)
+    measured["theta"] = max(measured.get("theta", 0.0), dt / bt)
+    assert df <= bf, (what, fb.meta_f64[i, 3], fr.neg_logp, c_f)
+    assert dt <= bt, (what, dt, bt, np.abs(record_theta(fb, i) - th_np))

@@ -329,13 +329,14 @@ PB200_API int pb200_synchronize(pb200_ctx* c) {
 
 }  // extern "C"
 
-// newton_kernel over the queue {count, head, items...} at d_nq (16-warp CTAs with ~100 KB of shared memory)
+// newton_kernel over the queue {count, head, items...} at d_nq (16-warp CTAs with up to ~113 KB of shared memory, at P = 67)
 static int launch_newton(pb200_ctx* c, const pb200_options* opts, const int64_t* d_ds, const void* d_y,
                          int32_t y_dtype, const int64_t* d_offsets, int64_t n_series, int* d_nq, const double* d_prior,
                          const double* d_x0, double* d_params, double* d_tchange, int32_t* d_meta_i32, int64_t* d_meta_i64, double* d_meta_f64) {
+    static_assert(30 + 34 + 3 <= pb200::nw::NW_PMAX, "newton_kernel holds every P check_opts admits");
     pb200_layout L;
     pb200_get_layout(opts, &L);
-    if (opts->algorithm == PB200_ALG_LBFGS || L.pstride > pb200::nw::NW_PMAX) return PB200_OK;
+    if (opts->algorithm == PB200_ALG_LBFGS) return PB200_OK;
     pb200::nw::NewtonArgs na;
     na.ds = (const long long*)d_ds;
     na.y = d_y;

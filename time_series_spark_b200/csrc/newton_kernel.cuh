@@ -23,7 +23,7 @@ namespace pb200 {
 namespace nw {
 
 constexpr int NW_WARPS = 16;
-constexpr int NW_PMAX = 64;          // S + K + 3 <= 30 + 34 + 3 = 67 > 64: yearly + 30 changepoints is refused by the host
+constexpr int NW_PMAX = 68;          // S + K + 3 <= 30 + 34 + 3 = 67 (yearly + weekly + daily, 30 changepoints)
 constexpr int NW_SEG = 32;
 
 struct NewtonArgs {
@@ -395,7 +395,8 @@ __global__ void __launch_bounds__(32 * NW_WARPS, 1) newton_kernel(const NewtonAr
                 if (lane == 0) { sr.f0 = ws.f; if (ws.err) sr.err = 1; }
             }
             for (int d = warp; d < P; d += NW_WARPS) {
-                double r0 = 0.0, r1 = 0.0;                        // row d, columns lane and lane + 32
+                double* const Rd = Vm + d * P;                     // row d of R (staged in V's storage), this warp's own
+                for (int q = lane; q < P; q += 32) Rd[q] = 0.0;
                 int e = 0;
                 for (int i = 0; i < 4; ++i) {
                     const double pert = i == 0 ? -2 * eps : (i == 1 ? -eps : (i == 2 ? eps : 2 * eps));
@@ -404,12 +405,9 @@ __global__ void __launch_bounds__(32 * NW_WARPS, 1) newton_kernel(const NewtonAr
                     __syncwarp();
                     nw_eval(a, sr, ws, lane);
                     if (ws.err) e = 1;
-                    if (lane < P) r0 += half_inv_eps * coef * ws.g[lane];
-                    if (lane + 32 < P) r1 += half_inv_eps * coef * ws.g[lane + 32];
+                    for (int q = lane; q < P; q += 32) Rd[q] += half_inv_eps * coef * ws.g[q];
                     __syncwarp();
                 }
-                if (lane < P) Vm[d * P + lane] = r0;               // R (staged in V's storage)
-                if (lane + 32 < P) Vm[d * P + lane + 32] = r1;
                 if (e && lane == 0) atomicExch(&sr.err, 1);
             }
             __syncthreads();
