@@ -298,6 +298,47 @@ PB200_API int pb200_predict_host(pb200_ctx* ctx, const pb200_options* opts,
                        double* h_yhat, double* h_yhat_lower, double* h_yhat_upper,
                        int32_t* h_yhat_int);
 
+/*
+ * pb200_predict_* plus fbprophet's component columns of Prophet.predict (DESIGN §12).  Same arguments and the same
+ * yhat / yhat_lower / yhat_upper / yhat_int bits as pb200_predict_*, and:
+ *   d_components  double [PB200_N_COMPONENTS][n_models * horizon], plane PB200_COMP_* (required):
+ *     TREND           predict_trend: piecewise trend * y_scale + floor (floor 0 for linear growth)
+ *     MULTIPLICATIVE  multiplicative_terms: yearly + weekly + daily in multiplicative mode, else 0;
+ *                     yhat == trend * (1 + multiplicative_terms) exactly
+ *     ADDITIVE        additive_terms: (yearly + weekly + daily) * y_scale in additive mode, else 0;
+ *                     yhat == trend + additive_terms up to the rounding of additive_terms (yhat fuses the product)
+ *     YEARLY / WEEKLY / DAILY  X_c beta_c of that seasonality: times y_scale in additive mode, the relative factor
+ *                     in multiplicative mode; exactly 0 when the model's seasonality mask lacks it
+ *   d_trend_lower / d_trend_upper  double [n_models * horizon] or both NULL: percentiles at 100(1 -+ w)/2 of the
+ *     noise-free trend of the same draws as yhat_lower / yhat_upper; they need those intervals (both pointers and
+ *     uncertainty_samples > 0, else PB200_E_ARG) and take their option checks.
+ * Failed models (status < 0) get NaN in every plane and bound.
+ */
+#define PB200_N_COMPONENTS        6
+#define PB200_COMP_TREND          0
+#define PB200_COMP_MULTIPLICATIVE 1
+#define PB200_COMP_ADDITIVE       2
+#define PB200_COMP_YEARLY         3
+#define PB200_COMP_WEEKLY         4
+#define PB200_COMP_DAILY          5
+PB200_API int pb200_predict_components_device(pb200_ctx* ctx, const pb200_options* opts,
+                         const double* d_params, const double* d_tchange,
+                         const int32_t* d_meta_i32, const int64_t* d_meta_i64,
+                         const double* d_meta_f64, int64_t n_models,
+                         const int64_t* d_future_ds, int32_t horizon,
+                         const double* d_floor, const double* d_cap, uint64_t seed,
+                         double* d_yhat, double* d_yhat_lower, double* d_yhat_upper,
+                         int32_t* d_yhat_int, double* d_components, double* d_trend_lower, double* d_trend_upper);
+
+PB200_API int pb200_predict_components_host(pb200_ctx* ctx, const pb200_options* opts,
+                       const double* h_params, const double* h_tchange,
+                       const int32_t* h_meta_i32, const int64_t* h_meta_i64,
+                       const double* h_meta_f64, int64_t n_models,
+                       const int64_t* h_future_ds, int32_t horizon,
+                       const double* h_floor, const double* h_cap, uint64_t seed,
+                       double* h_yhat, double* h_yhat_lower, double* h_yhat_upper,
+                       int32_t* h_yhat_int, double* h_components, double* h_trend_lower, double* h_trend_upper);
+
 /* future_ds[i*horizon + j] = last_ds[i] + (j+1)*freq_ns  -- make_future_dataframe
  * (include_history=False) for a fixed-width pandas frequency. */
 PB200_API int pb200_make_future_device(pb200_ctx* ctx, const int64_t* d_last_ds, int64_t n_models,

@@ -24,6 +24,9 @@ ALG_LBFGS_NEWTON, ALG_LBFGS, ALG_NEWTON = 0, 1, 2
 ST_LSFAIL, ST_INIT_ERROR, ST_TOO_FEW, ST_CAP_LE_FLOOR, ST_BAD_INPUT, ST_BAD_PRIOR = -1, -2, -3, -4, -5, -6
 # where a series of a warm-started fit started (PB200_WARM_*)
 WARM_USED, WARM_NONE, WARM_SHAPE, WARM_BAD = 1, 0, -1, -2
+# planes of pb200_predict_components_* (PB200_COMP_*), in order
+COMPONENTS = ("trend", "multiplicative_terms", "additive_terms", "yearly", "weekly", "daily")
+N_COMPONENTS = len(COMPONENTS)
 
 
 class Options(C.Structure):
@@ -49,7 +52,7 @@ class Layout(C.Structure):
 EXPORTS = [
     "pb200_default_options", "pb200_get_layout", "pb200_create", "pb200_destroy", "pb200_last_error",
     "pb200_stream", "pb200_launch_count", "pb200_last_fit_variant_counts", "pb200_tab_chunk", "pb200_fit_device", "pb200_fit_prior_device", "pb200_fit_warm_device", "pb200_fit_host", "pb200_fit_warm_host", "pb200_predict_device",
-    "pb200_predict_host", "pb200_make_future_device", "pb200_synchronize", "pb200_objective_host",
+    "pb200_predict_host", "pb200_predict_components_device", "pb200_predict_components_host", "pb200_make_future_device", "pb200_synchronize", "pb200_objective_host",
     "pb200_fit_trace_host", "pb200_forecast_csv_lengths_device", "pb200_forecast_csv_rows_device", "pb200_forecast_csv_row_host",
     "pb200_cv_plan_counts_device", "pb200_cv_plan_device", "pb200_cv_gather_device", "pb200_cv_metrics_device",
 ]
@@ -104,6 +107,10 @@ def load() -> C.CDLL:
     lib.pb200_predict_device.restype = C.c_int
     lib.pb200_predict_host.argtypes = pred_args
     lib.pb200_predict_host.restype = C.c_int
+    lib.pb200_predict_components_device.argtypes = pred_args + [vp, vp, vp]
+    lib.pb200_predict_components_device.restype = C.c_int
+    lib.pb200_predict_components_host.argtypes = pred_args + [vp, vp, vp]
+    lib.pb200_predict_components_host.restype = C.c_int
     lib.pb200_make_future_device.argtypes = [vp, vp, i64, i32, i64, vp]
     lib.pb200_make_future_device.restype = C.c_int
     lib.pb200_objective_host.argtypes = [vp, OP, vp, vp, i32, vp, i64, dbl, dbl, vp, vp, vp, vp]

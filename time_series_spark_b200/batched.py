@@ -294,6 +294,14 @@ class ForecastBatch:
     yhat_lower: object   # [N, H] f64 or None
     yhat_upper: object
     yhat_int: object     # [N, H] int32 (truncated, floor-clamped)
+    components: object = None   # [6, N, H] f64, planes in L.COMPONENTS order (components=True), else None
+    trend_lower: object = None  # [N, H] f64 (components=True with intervals), else None
+    trend_upper: object = None
+
+    def component(self, name: str):
+        """One component plane by its fbprophet column name (trend, multiplicative_terms, additive_terms, yearly, weekly,
+        daily)."""
+        return self.components[L.COMPONENTS.index(name)]
 
 
 def make_future(last_ds_ns: np.ndarray, periods: int, freq_ns: int) -> np.ndarray:
@@ -358,9 +366,11 @@ def forecast_csv_row_host(series_id: int, dim_id: int, ds_ns: int, quantity: int
 
 
 def predict_batch_host(ctx: L.Context, opts: L.Options, fitted: FittedBatch, future_ds: np.ndarray,
-                       floor: np.ndarray, cap: np.ndarray, seed: int = 0, intervals: bool = True) -> ForecastBatch:
+                       floor: np.ndarray, cap: np.ndarray, seed: int = 0, intervals: bool = True,
+                       components: bool = False) -> ForecastBatch:
     """pb200_predict_host.  ``floor`` / ``cap`` per model as the scorer reads them back from
-    the float32 model-table columns (prophet_scorer.py:46-47,67-68)."""
+    the float32 model-table columns (prophet_scorer.py:46-47,67-68).  ``components``: pb200_predict_components_host,
+    which also fills ``components`` and, with intervals, ``trend_lower`` / ``trend_upper``."""
     fitted = fitted.to_host()
     n = fitted.n
     future_ds = np.ascontiguousarray(future_ds, dtype=np.int64).reshape(n, -1)
@@ -372,21 +382,29 @@ def predict_batch_host(ctx: L.Context, opts: L.Options, fitted: FittedBatch, fut
     do_mc = intervals and opts.uncertainty_samples > 0
     lo = np.empty((n, h), np.float64) if do_mc else None
     hi = np.empty((n, h), np.float64) if do_mc else None
+    comp = np.empty((L.N_COMPONENTS, n, h), np.float64) if components else None
+    tlo = np.empty((n, h), np.float64) if components and do_mc else None
+    thi = np.empty((n, h), np.float64) if components and do_mc else None
     if n > 0 and h > 0:
-        rc = L.load().pb200_predict_host(
-            ctx.handle, C.byref(opts), _np_ptr(np.ascontiguousarray(fitted.params)),
-            _np_ptr(np.ascontiguousarray(fitted.tchange)), _np_ptr(np.ascontiguousarray(fitted.meta_i32)),
-            _np_ptr(np.ascontiguousarray(fitted.meta_i64)), _np_ptr(np.ascontiguousarray(fitted.meta_f64)),
-            n, _np_ptr(future_ds), h, _np_ptr(floor), _np_ptr(cap), int(seed) & (2**64 - 1),
-            _np_ptr(yhat), _np_ptr(lo) if do_mc else None, _np_ptr(hi) if do_mc else None, _np_ptr(yint))
-        L.check(rc, "pb200_predict_host")
-    return ForecastBatch(future_ds, yhat, lo, hi, yint)
+        args = (ctx.handle, C.byref(opts), _np_ptr(np.ascontiguousarray(fitted.params)),
+                _np_ptr(np.ascontiguousarray(fitted.tchange)), _np_ptr(np.ascontiguousarray(fitted.meta_i32)),
+                _np_ptr(np.ascontiguousarray(fitted.meta_i64)), _np_ptr(np.ascontiguousarray(fitted.meta_f64)),
+                n, _np_ptr(future_ds), h, _np_ptr(floor), _np_ptr(cap), int(seed) & (2**64 - 1),
+                _np_ptr(yhat), _np_ptr(lo) if do_mc else None, _np_ptr(hi) if do_mc else None, _np_ptr(yint))
+        if components:
+            rc = L.load().pb200_predict_components_host(*args, _np_ptr(comp), _np_ptr(tlo) if do_mc else None,
+                                                        _np_ptr(thi) if do_mc else None)
+            L.check(rc, "pb200_predict_components_host")
+        else:
+            L.check(L.load().pb200_predict_host(*args), "pb200_predict_host")
+    return ForecastBatch(future_ds, yhat, lo, hi, yint, comp, tlo, thi)
 
 
 def predict_batch_device(ctx: L.Context, opts: L.Options, fitted: FittedBatch, future_ds, floor, cap,
                          seed: int = 0, intervals: bool = True, sync: bool = True,
-                         out: Optional["ForecastBatch"] = None) -> ForecastBatch:
-    """pb200_predict_device with torch CUDA tensors (``out`` reuses a previous result's buffers)."""
+                         out: Optional["ForecastBatch"] = None, components: bool = False) -> ForecastBatch:
+    """pb200_predict_device with torch CUDA tensors (``out`` reuses a previous result's buffers, which must have been
+    made with the same ``components``).  ``components``: pb200_predict_components_device, as in predict_batch_host."""
     import torch
     n = fitted.n
     h = int(future_ds.shape[1])
@@ -394,23 +412,31 @@ def predict_batch_device(ctx: L.Context, opts: L.Options, fitted: FittedBatch, f
     do_mc = intervals and opts.uncertainty_samples > 0
     if out is not None:
         yhat, yint, lo, hi = out.yhat, out.yhat_int, out.yhat_lower, out.yhat_upper
+        comp, tlo, thi = out.components, out.trend_lower, out.trend_upper
     else:
         yhat = torch.empty((n, h), dtype=torch.float64, device=dev)
         yint = torch.empty((n, h), dtype=torch.int32, device=dev)
         lo = torch.empty((n, h), dtype=torch.float64, device=dev) if do_mc else None
         hi = torch.empty((n, h), dtype=torch.float64, device=dev) if do_mc else None
+        comp = torch.empty((L.N_COMPONENTS, n, h), dtype=torch.float64, device=dev) if components else None
+        tlo = torch.empty((n, h), dtype=torch.float64, device=dev) if components and do_mc else None
+        thi = torch.empty((n, h), dtype=torch.float64, device=dev) if components and do_mc else None
     if n > 0 and h > 0:
         if out is None:
             torch.cuda.current_stream(dev).synchronize()
-        rc = L.load().pb200_predict_device(
-            ctx.handle, C.byref(opts), fitted.params.data_ptr(), fitted.tchange.data_ptr(),
-            fitted.meta_i32.data_ptr(), fitted.meta_i64.data_ptr(), fitted.meta_f64.data_ptr(), n,
-            future_ds.data_ptr(), h, floor.data_ptr(), cap.data_ptr(), int(seed) & (2**64 - 1),
-            yhat.data_ptr(), lo.data_ptr() if do_mc else None, hi.data_ptr() if do_mc else None, yint.data_ptr())
-        L.check(rc, "pb200_predict_device")
+        args = (ctx.handle, C.byref(opts), fitted.params.data_ptr(), fitted.tchange.data_ptr(),
+                fitted.meta_i32.data_ptr(), fitted.meta_i64.data_ptr(), fitted.meta_f64.data_ptr(), n,
+                future_ds.data_ptr(), h, floor.data_ptr(), cap.data_ptr(), int(seed) & (2**64 - 1),
+                yhat.data_ptr(), lo.data_ptr() if do_mc else None, hi.data_ptr() if do_mc else None, yint.data_ptr())
+        if components:
+            rc = L.load().pb200_predict_components_device(*args, comp.data_ptr(), tlo.data_ptr() if do_mc else None,
+                                                          thi.data_ptr() if do_mc else None)
+            L.check(rc, "pb200_predict_components_device")
+        else:
+            L.check(L.load().pb200_predict_device(*args), "pb200_predict_device")
         if sync:
             ctx.synchronize()
-    return ForecastBatch(future_ds, yhat, lo, hi, yint)
+    return ForecastBatch(future_ds, yhat, lo, hi, yint, comp, tlo, thi)
 
 
 def objective_host(ctx: L.Context, opts: L.Options, ds_ns: np.ndarray, y: np.ndarray, offsets: np.ndarray,

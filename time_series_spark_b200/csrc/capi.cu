@@ -105,6 +105,7 @@ struct pb200_ctx {
     // data staging for the *_host entry points
     DevBuf d_ds, d_y, d_cap, d_params, d_tchange, d_mi32, d_mi64, d_mf64;
     DevBuf d_fut, d_floor, d_yhat, d_lo, d_hi, d_yint;
+    DevBuf d_comp, d_tlo, d_thi;   // staging of pb200_predict_components_host's planes and trend bounds
     DevBuf d_mc;     // MC workspace
     int lc0_max = 1 << 30; // PB200_LC0_MAX: longest series on one warp per series, longer ones get four (unset: no limit)
     bool lc_auto = true;   // false when PB200_LC0_MAX pins the CTA width
@@ -292,7 +293,7 @@ PB200_API void pb200_destroy(pb200_ctx* c) {
     cudaSetDevice(c->device);
     cudaStreamSynchronize(c->stream);
     for (DevBuf* b : {&c->d_ds, &c->d_y, &c->d_cap, &c->d_params, &c->d_tchange, &c->d_mi32, &c->d_mi64, &c->d_mf64, &c->d_fut,
-                      &c->d_floor, &c->d_yhat, &c->d_lo, &c->d_hi, &c->d_yint, &c->d_mc, &c->d_trace, &c->d_warm_x, &c->d_prior, &c->d_iparams, &c->d_imeta, &c->d_warm, &c->d_vcount, &c->d_offsets,
+                      &c->d_floor, &c->d_yhat, &c->d_lo, &c->d_hi, &c->d_yint, &c->d_comp, &c->d_tlo, &c->d_thi, &c->d_mc,&c->d_trace, &c->d_warm_x, &c->d_prior, &c->d_iparams, &c->d_imeta, &c->d_warm, &c->d_vcount, &c->d_offsets,
                       &c->d_order, &c->d_lenclass, &c->d_qitems, &c->d_qctl, &c->d_nq, &c->d_planes, &c->d_qkey, &c->d_qhist})
         b->release();
     c->h_ctl.release();
@@ -807,11 +808,26 @@ PB200_API int pb200_make_future_device(pb200_ctx* c, const int64_t* d_last_ds, i
     return PB200_OK;
 }
 
-PB200_API int pb200_predict_device(pb200_ctx* c, const pb200_options* opts, const double* d_params, const double* d_tchange,
-                         const int32_t* d_meta_i32, const int64_t* d_meta_i64, const double* d_meta_f64,
-                         int64_t n_models, const int64_t* d_future_ds, int32_t horizon, const double* d_floor,
-                         const double* d_cap, uint64_t seed, double* d_yhat, double* d_yhat_lower, double* d_yhat_upper,
-                         int32_t* d_yhat_int) {
+namespace {
+
+// the component arguments of pb200_predict_components_*: the planes are required, the trend bounds come in pairs and
+// ride on the yhat intervals
+int check_comp_args(const pb200_options* o, const void* comp, const void* lo, const void* hi, const void* tlo,
+                    const void* thi) {
+    if (!comp) return fail(PB200_E_ARG, "null pointer (components)");
+    if (!tlo != !thi) return fail(PB200_E_ARG, "trend_lower and trend_upper go together");
+    if (tlo && !(lo && hi && o->uncertainty_samples > 0))
+        return fail(PB200_E_ARG, "trend bounds need the yhat intervals (yhat_lower / yhat_upper, uncertainty_samples > 0)");
+    return PB200_OK;
+}
+
+// pb200_predict_device; d_comp != null: the components instance of predict_kernel, d_tlo / d_thi != null: the
+// trend-bounds instance of mc_kernel
+int predict_device(pb200_ctx* c, const pb200_options* opts, const double* d_params, const double* d_tchange,
+                   const int32_t* d_meta_i32, const int64_t* d_meta_i64, const double* d_meta_f64, int64_t n_models,
+                   const int64_t* d_future_ds, int32_t horizon, const double* d_floor, const double* d_cap, uint64_t seed,
+                   double* d_yhat, double* d_yhat_lower, double* d_yhat_upper, int32_t* d_yhat_int, double* d_comp,
+                   double* d_tlo, double* d_thi) {
     if (!c) return fail(PB200_E_ARG, "ctx is null");
     int rc = check_opts(opts);
     if (rc) return rc;
@@ -842,19 +858,20 @@ PB200_API int pb200_predict_device(pb200_ctx* c, const pb200_options* opts, cons
     a.growth = opts->growth;
     a.mult = opts->multiplicative ? 1 : 0;
     a.yhat = d_yhat;
-    a.trend = nullptr;
+    a.trend = d_comp;
     a.yhat_int = d_yhat_int;
     {
         // one CTA per (model, 1024 future points): the per-model prologue (parameters, the serial gamma recurrence) is paid
         // once for config #5's 672 periods instead of three times
         dim3 grid((unsigned)n_models, (unsigned)std::min((horizon + 1023) / 1024, 64));
-        pb200::predict_kernel<<<grid, 256, 0, c->stream>>>(a);
+        if (d_comp) pb200::predict_kernel<true><<<grid, 256, 0, c->stream>>>(a);
+        else pb200::predict_kernel<false><<<grid, 256, 0, c->stream>>>(a);
         CK(cudaGetLastError());
         c->launches++;
     }
     if (mc) {
         rc = pb200::launch_mc(c->stream, c->sms, a, opts->uncertainty_samples, opts->interval_width, seed, d_yhat_lower,
-                              d_yhat_upper);
+                              d_yhat_upper, d_tlo, d_thi);
         if (rc == -1) return fail(PB200_E_ARG, "uncertainty_samples / interval_width out of range");
         if (rc) return fail(PB200_E_CUDA, "mc kernel launch", cudaGetLastError());
         c->launches++;
@@ -862,10 +879,12 @@ PB200_API int pb200_predict_device(pb200_ctx* c, const pb200_options* opts, cons
     return PB200_OK;
 }
 
-PB200_API int pb200_predict_host(pb200_ctx* c, const pb200_options* opts, const double* h_params, const double* h_tchange,
-                       const int32_t* h_meta_i32, const int64_t* h_meta_i64, const double* h_meta_f64, int64_t n_models,
-                       const int64_t* h_future_ds, int32_t horizon, const double* h_floor, const double* h_cap,
-                       uint64_t seed, double* h_yhat, double* h_yhat_lower, double* h_yhat_upper, int32_t* h_yhat_int) {
+// pb200_predict_host; h_comp / h_tlo / h_thi as predict_device's d_comp / d_tlo / d_thi
+int predict_host(pb200_ctx* c, const pb200_options* opts, const double* h_params, const double* h_tchange,
+                 const int32_t* h_meta_i32, const int64_t* h_meta_i64, const double* h_meta_f64, int64_t n_models,
+                 const int64_t* h_future_ds, int32_t horizon, const double* h_floor, const double* h_cap, uint64_t seed,
+                 double* h_yhat, double* h_yhat_lower, double* h_yhat_upper, int32_t* h_yhat_int, double* h_comp,
+                 double* h_tlo, double* h_thi) {
     if (!c) return fail(PB200_E_ARG, "ctx is null");
     int rc = check_opts(opts);
     if (rc) return rc;
@@ -893,6 +912,11 @@ PB200_API int pb200_predict_host(pb200_ctx* c, const pb200_options* opts, const 
         CK(c->d_lo.reserve(NH * 8));
         CK(c->d_hi.reserve(NH * 8));
     }
+    if (h_comp) CK(c->d_comp.reserve(NH * 8 * PB200_N_COMPONENTS));
+    if (h_tlo) {
+        CK(c->d_tlo.reserve(NH * 8));
+        CK(c->d_thi.reserve(NH * 8));
+    }
     cudaStream_t st = c->stream;
     CK(cudaMemcpyAsync(c->d_params.p, h_params, N * L.pstride * 8, cudaMemcpyHostToDevice, st));
     CK(cudaMemcpyAsync(c->d_tchange.p, h_tchange, N * L.smax * 8, cudaMemcpyHostToDevice, st));
@@ -902,11 +926,12 @@ PB200_API int pb200_predict_host(pb200_ctx* c, const pb200_options* opts, const 
     CK(cudaMemcpyAsync(c->d_fut.p, h_future_ds, NH * 8, cudaMemcpyHostToDevice, st));
     CK(cudaMemcpyAsync(c->d_floor.p, h_floor, N * 8, cudaMemcpyHostToDevice, st));
     CK(cudaMemcpyAsync(c->d_cap.p, h_cap, N * 8, cudaMemcpyHostToDevice, st));
-    rc = pb200_predict_device(c, opts, (const double*)c->d_params.p, (const double*)c->d_tchange.p,
-                              (const int32_t*)c->d_mi32.p, (const int64_t*)c->d_mi64.p, (const double*)c->d_mf64.p,
-                              n_models, (const int64_t*)c->d_fut.p, horizon, (const double*)c->d_floor.p,
-                              (const double*)c->d_cap.p, seed, (double*)c->d_yhat.p, mc ? (double*)c->d_lo.p : nullptr,
-                              mc ? (double*)c->d_hi.p : nullptr, (int32_t*)c->d_yint.p);
+    rc = predict_device(c, opts, (const double*)c->d_params.p, (const double*)c->d_tchange.p, (const int32_t*)c->d_mi32.p,
+                        (const int64_t*)c->d_mi64.p, (const double*)c->d_mf64.p, n_models, (const int64_t*)c->d_fut.p,
+                        horizon, (const double*)c->d_floor.p, (const double*)c->d_cap.p, seed, (double*)c->d_yhat.p,
+                        mc ? (double*)c->d_lo.p : nullptr, mc ? (double*)c->d_hi.p : nullptr, (int32_t*)c->d_yint.p,
+                        h_comp ? (double*)c->d_comp.p : nullptr, h_tlo ? (double*)c->d_tlo.p : nullptr,
+                        h_tlo ? (double*)c->d_thi.p : nullptr);
     if (rc) return rc;
     CK(cudaMemcpyAsync(h_yhat, c->d_yhat.p, NH * 8, cudaMemcpyDeviceToHost, st));
     CK(cudaMemcpyAsync(h_yhat_int, c->d_yint.p, NH * 4, cudaMemcpyDeviceToHost, st));
@@ -914,8 +939,62 @@ PB200_API int pb200_predict_host(pb200_ctx* c, const pb200_options* opts, const 
         CK(cudaMemcpyAsync(h_yhat_lower, c->d_lo.p, NH * 8, cudaMemcpyDeviceToHost, st));
         CK(cudaMemcpyAsync(h_yhat_upper, c->d_hi.p, NH * 8, cudaMemcpyDeviceToHost, st));
     }
+    if (h_comp) CK(cudaMemcpyAsync(h_comp, c->d_comp.p, NH * 8 * PB200_N_COMPONENTS, cudaMemcpyDeviceToHost, st));
+    if (h_tlo) {
+        CK(cudaMemcpyAsync(h_tlo, c->d_tlo.p, NH * 8, cudaMemcpyDeviceToHost, st));
+        CK(cudaMemcpyAsync(h_thi, c->d_thi.p, NH * 8, cudaMemcpyDeviceToHost, st));
+    }
     CK(cudaStreamSynchronize(st));
     return PB200_OK;
+}
+
+}  // namespace
+
+PB200_API int pb200_predict_device(pb200_ctx* c, const pb200_options* opts, const double* d_params, const double* d_tchange,
+                         const int32_t* d_meta_i32, const int64_t* d_meta_i64, const double* d_meta_f64,
+                         int64_t n_models, const int64_t* d_future_ds, int32_t horizon, const double* d_floor,
+                         const double* d_cap, uint64_t seed, double* d_yhat, double* d_yhat_lower, double* d_yhat_upper,
+                         int32_t* d_yhat_int) {
+    return predict_device(c, opts, d_params, d_tchange, d_meta_i32, d_meta_i64, d_meta_f64, n_models, d_future_ds, horizon,
+                          d_floor, d_cap, seed, d_yhat, d_yhat_lower, d_yhat_upper, d_yhat_int, nullptr, nullptr, nullptr);
+}
+
+PB200_API int pb200_predict_host(pb200_ctx* c, const pb200_options* opts, const double* h_params, const double* h_tchange,
+                       const int32_t* h_meta_i32, const int64_t* h_meta_i64, const double* h_meta_f64, int64_t n_models,
+                       const int64_t* h_future_ds, int32_t horizon, const double* h_floor, const double* h_cap,
+                       uint64_t seed, double* h_yhat, double* h_yhat_lower, double* h_yhat_upper, int32_t* h_yhat_int) {
+    return predict_host(c, opts, h_params, h_tchange, h_meta_i32, h_meta_i64, h_meta_f64, n_models, h_future_ds, horizon,
+                        h_floor, h_cap, seed, h_yhat, h_yhat_lower, h_yhat_upper, h_yhat_int, nullptr, nullptr, nullptr);
+}
+
+PB200_API int pb200_predict_components_device(pb200_ctx* c, const pb200_options* opts, const double* d_params,
+                         const double* d_tchange, const int32_t* d_meta_i32, const int64_t* d_meta_i64,
+                         const double* d_meta_f64, int64_t n_models, const int64_t* d_future_ds, int32_t horizon,
+                         const double* d_floor, const double* d_cap, uint64_t seed, double* d_yhat, double* d_yhat_lower,
+                         double* d_yhat_upper, int32_t* d_yhat_int, double* d_components, double* d_trend_lower,
+                         double* d_trend_upper) {
+    if (!c) return fail(PB200_E_ARG, "ctx is null");
+    int rc = check_opts(opts);
+    if (rc) return rc;
+    if ((rc = check_comp_args(opts, d_components, d_yhat_lower, d_yhat_upper, d_trend_lower, d_trend_upper))) return rc;
+    return predict_device(c, opts, d_params, d_tchange, d_meta_i32, d_meta_i64, d_meta_f64, n_models, d_future_ds, horizon,
+                          d_floor, d_cap, seed, d_yhat, d_yhat_lower, d_yhat_upper, d_yhat_int, d_components, d_trend_lower,
+                          d_trend_upper);
+}
+
+PB200_API int pb200_predict_components_host(pb200_ctx* c, const pb200_options* opts, const double* h_params,
+                       const double* h_tchange, const int32_t* h_meta_i32, const int64_t* h_meta_i64,
+                       const double* h_meta_f64, int64_t n_models, const int64_t* h_future_ds, int32_t horizon,
+                       const double* h_floor, const double* h_cap, uint64_t seed, double* h_yhat, double* h_yhat_lower,
+                       double* h_yhat_upper, int32_t* h_yhat_int, double* h_components, double* h_trend_lower,
+                       double* h_trend_upper) {
+    if (!c) return fail(PB200_E_ARG, "ctx is null");
+    int rc = check_opts(opts);
+    if (rc) return rc;
+    if ((rc = check_comp_args(opts, h_components, h_yhat_lower, h_yhat_upper, h_trend_lower, h_trend_upper))) return rc;
+    return predict_host(c, opts, h_params, h_tchange, h_meta_i32, h_meta_i64, h_meta_f64, n_models, h_future_ds, horizon,
+                        h_floor, h_cap, seed, h_yhat, h_yhat_lower, h_yhat_upper, h_yhat_int, h_components, h_trend_lower,
+                        h_trend_upper);
 }
 
 // ---- forecast CSV rows formatted on the device (csv_kernel.cuh) ----

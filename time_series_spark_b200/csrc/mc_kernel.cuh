@@ -69,6 +69,8 @@ struct McArgs {
     uint64_t seed;
     double* lower;
     double* upper;
+    double* tlower;       // trend bounds: written by mc_kernel<LOGI, true> only
+    double* tupper;
 };
 
 __device__ __forceinline__ uint64_t splitmix64(uint64_t z) {
@@ -134,7 +136,10 @@ __device__ __forceinline__ void advance(DrawState& d, const ModelSm& ms, const d
 constexpr int MC_CAND = 64;    // candidates kept per histogram bin before falling back to a full sort
 
 // k-th smallest of the n values of `row` (k 0-based) by a 256-bin histogram + exact selection inside
-// the bin that holds rank k.  Returns false if that bin holds more than MC_CAND values.
+// the bin that holds rank k.  Returns false if that bin holds more than MC_CAND values -- unless TIES and they are all
+// equal: then every rank in the bin is that value (exact).  Trend draws need it: before a draw's first simulated
+// changepoint its trend is the fitted one, so at early horizons most draws of a point are exactly equal.
+template <bool TIES>
 __device__ __forceinline__ bool kth_smallest(const double* row, const int n, const int k, const double mn,
                                              const double scale, const int* hist, const int base, const int lsum,
                                              double* cand, int* cnt, const int lane, double& out) {
@@ -154,17 +159,29 @@ __device__ __forceinline__ bool kth_smallest(const double* row, const int n, con
     rb = __shfl_sync(0xffffffffu, rb, src);
     if (lane == 0) *cnt = 0;
     __syncwarp();
+    double bmn = INFINITY, bmx = -INFINITY;
     for (int e = lane; e < n; e += 32) {
         const double v = row[e];
         const int bb = min(255, (int)((v - mn) * scale));
         if (bb == b) {
             const int pos = atomicAdd(cnt, 1);
             if (pos < MC_CAND) cand[pos] = v;
+            if (TIES) { bmn = fmin(bmn, v); bmx = fmax(bmx, v); }
         }
     }
     __syncwarp();
     const int m = *cnt;
-    if (m > MC_CAND) return false;
+    if (m > MC_CAND) {
+        if (TIES) {
+#pragma unroll
+            for (int o = 16; o >= 1; o >>= 1) {
+                bmn = fmin(bmn, __shfl_xor_sync(0xffffffffu, bmn, o));
+                bmx = fmax(bmx, __shfl_xor_sync(0xffffffffu, bmx, o));
+            }
+            if (bmn == bmx) { out = bmn; return true; }
+        }
+        return false;
+    }
     // exact selection: the candidate with exactly rb candidates ordered before it
     double found = 0.0;
     int have = 0;
@@ -184,6 +201,7 @@ __device__ __forceinline__ bool kth_smallest(const double* row, const int n, con
 }
 
 // numpy percentile (linear interpolation) at the two interval bounds from the draws of one point
+template <bool TIES>
 __device__ __forceinline__ bool select_quantiles(const double* row, const int n, const int lo_i, const double lo_f,
                                                  const int hi_i, const double hi_f, int* hist, double* cand, int* cnt,
                                                  const int lane, double& lo_v, double& hi_v) {
@@ -216,15 +234,20 @@ __device__ __forceinline__ bool select_quantiles(const double* row, const int n,
     const int ranks[4] = {lo_i, min(lo_i + 1, n - 1), hi_i, min(hi_i + 1, n - 1)};
     for (int q = 0; q < 4; ++q) {
         if (q > 0 && ranks[q] == ranks[q - 1]) { v[q] = v[q - 1]; continue; }
-        if (!kth_smallest(row, n, ranks[q], mn, scale, hist, base, lsum, cand, cnt, lane, v[q])) return false;
+        if (!kth_smallest<TIES>(row, n, ranks[q], mn, scale, hist, base, lsum, cand, cnt, lane, v[q])) return false;
     }
     lo_v = v[0] + (v[1] - v[0]) * lo_f;
     hi_v = v[2] + (v[3] - v[2]) * hi_f;
     return true;
 }
 
-template <bool LOGI>
+// TREND: also the bounds of the noise-free trend draws.  The tile is then TILE = 8 points: rows [0, 8) hold the yhat
+// draws and rows [8, 16) the trend draws of the same points, in the same 128 KB, and warp w still selects row w.  The
+// yhat draws are the same numbers (the noise counters go by pairs of points and 8 is even; the trend state advances per
+// draw across tiles; Tmax is over the whole frame), so are their bounds.
+template <bool LOGI, bool TREND>
 __global__ void __launch_bounds__(MC_THREADS, 1) mc_kernel(const McArgs a) {
+    constexpr int TILE = TREND ? MC_TILE / 2 : MC_TILE;
     extern __shared__ __align__(16) unsigned char mc_smem[];
     double* rows = (double*)mc_smem;                       // [MC_TILE][MC_NP]
     double* cand = rows + MC_TILE * MC_NP;                 // [MC_THREADS/32][MC_CAND]
@@ -241,7 +264,10 @@ __global__ void __launch_bounds__(MC_THREADS, 1) mc_kernel(const McArgs a) {
         load_model(ms, a.p, model, tid, MC_THREADS);
         const size_t base = (size_t)model * H;
         if (ms.status < 0) {
-            for (int h = tid; h < H; h += MC_THREADS) { a.lower[base + h] = NAN; a.upper[base + h] = NAN; }
+            for (int h = tid; h < H; h += MC_THREADS) {
+                a.lower[base + h] = NAN; a.upper[base + h] = NAN;
+                if (TREND) { a.tlower[base + h] = NAN; a.tupper[base + h] = NAN; }
+            }
             continue;
         }
         // Tmax = max t over the frame
@@ -275,8 +301,8 @@ __global__ void __launch_bounds__(MC_THREADS, 1) mc_kernel(const McArgs a) {
             }
         }
         const double nscale = ms.sigma * ms.y_scale;
-        for (int h0 = 0; h0 < H; h0 += MC_TILE) {
-            const int np = min(MC_TILE, H - h0);
+        for (int h0 = 0; h0 < H; h0 += TILE) {
+            const int np = min(TILE, H - h0);
             if (tid < np) {
                 const long long dsv = a.p.future_ds[base + h0 + tid];
                 tt[tid] = (double)(dsv - ms.start) / ms.t_scale;
@@ -287,7 +313,10 @@ __global__ void __launch_bounds__(MC_THREADS, 1) mc_kernel(const McArgs a) {
             for (int q = 0; q < 2; ++q) {
                 const uint32_t draw = tid + q * MC_THREADS;
                 if (!live[q]) {
-                    for (int p = 0; p < np; ++p) rows[p * MC_NP + draw] = INFINITY;
+                    for (int p = 0; p < np; ++p) {
+                        rows[p * MC_NP + draw] = INFINITY;
+                        if (TREND) rows[(TILE + p) * MC_NP + draw] = INFINITY;
+                    }
                     continue;
                 }
                 for (int p = 0; p < np; p += 2) {
@@ -310,15 +339,17 @@ __global__ void __launch_bounds__(MC_THREADS, 1) mc_kernel(const McArgs a) {
                         const double sd = seas[p + e];
                         const double yh = (a.p.mult ? tr * (1.0 + sd) : tr + sd * ms.y_scale) + nscale * z[e];
                         rows[(p + e) * MC_NP + draw] = yh;
+                        if (TREND) rows[(TILE + p + e) * MC_NP + draw] = tr;
                     }
                 }
             }
             __syncthreads();
-            // ---- percentiles: warp w selects the order statistics of row w ----
-            if (warp < np) {
+            // ---- percentiles: warp w selects the order statistics of row w (point pt of the tile) ----
+            const int pt = TREND ? (warp & (TILE - 1)) : warp;
+            if (pt < np) {
                 double* row = rows + warp * MC_NP;
                 double lo_v, hi_v;
-                if (!select_quantiles(row, a.n_samples, a.lo_i, a.lo_f, a.hi_i, a.hi_f, hist + warp * 256,
+                if (!select_quantiles<TREND>(row, a.n_samples, a.lo_i, a.lo_f, a.hi_i, a.hi_f, hist + warp * 256,
                                       cand + warp * MC_CAND, cnt + warp, lane, lo_v, hi_v)) {
                     // fallback (a histogram bin too crowded): full bitonic sort of the row
                     for (int k = 2; k <= MC_NP; k <<= 1) {
@@ -340,8 +371,13 @@ __global__ void __launch_bounds__(MC_THREADS, 1) mc_kernel(const McArgs a) {
                     hi_v = u0 + (u1 - u0) * a.hi_f;
                 }
                 if (lane == 0) {
-                    a.lower[base + h0 + warp] = lo_v;
-                    a.upper[base + h0 + warp] = hi_v;
+                    if (!TREND || warp < TILE) {
+                        a.lower[base + h0 + pt] = lo_v;
+                        a.upper[base + h0 + pt] = hi_v;
+                    } else {
+                        a.tlower[base + h0 + pt] = lo_v;
+                        a.tupper[base + h0 + pt] = hi_v;
+                    }
                 }
             }
             __syncthreads();
@@ -349,9 +385,17 @@ __global__ void __launch_bounds__(MC_THREADS, 1) mc_kernel(const McArgs a) {
     }
 }
 
-// returns 0 ok, -1 sample count or interval width out of range, 1 CUDA error
+template <bool LOGI, bool TREND>
+cudaError_t launch_mc_inst(cudaStream_t st, int grid, size_t smem, const McArgs& a) {
+    const cudaError_t e = cudaFuncSetAttribute(mc_kernel<LOGI, TREND>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) return e;
+    mc_kernel<LOGI, TREND><<<grid, MC_THREADS, smem, st>>>(a);
+    return cudaGetLastError();
+}
+
+// returns 0 ok, -1 sample count or interval width out of range, 1 CUDA error.  tlower / tupper: trend bounds, or both null
 inline int launch_mc(cudaStream_t st, int sms, const PredictArgs& p, int n_samples, double width, uint64_t seed,
-                     double* lower, double* upper) {
+                     double* lower, double* upper, double* tlower = nullptr, double* tupper = nullptr) {
     if (n_samples < 2 || n_samples > MC_NP || !(width >= 0.0 && width <= 1.0)) return -1;
     McArgs a;
     a.p = p;
@@ -363,19 +407,15 @@ inline int launch_mc(cudaStream_t st, int sms, const PredictArgs& p, int n_sampl
     a.seed = seed;
     a.lower = lower;
     a.upper = upper;
+    a.tlower = tlower;
+    a.tupper = tupper;
+    const bool trend = tlower && tupper;
     const size_t smem = (size_t)MC_TILE * MC_NP * 8 + (size_t)(MC_THREADS / 32) * (MC_CAND * 8 + 256 * 4 + 4) + 16;
     const int grid = p.n_models < sms ? p.n_models : sms;
-    cudaError_t e;
-    if (p.growth == PB200_GROWTH_LOGISTIC) {
-        e = cudaFuncSetAttribute(mc_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        if (e != cudaSuccess) return 1;
-        mc_kernel<true><<<grid, MC_THREADS, smem, st>>>(a);
-    } else {
-        e = cudaFuncSetAttribute(mc_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        if (e != cudaSuccess) return 1;
-        mc_kernel<false><<<grid, MC_THREADS, smem, st>>>(a);
-    }
-    return cudaGetLastError() == cudaSuccess ? 0 : 1;
+    const bool logi = p.growth == PB200_GROWTH_LOGISTIC;
+    const cudaError_t e = logi ? (trend ? launch_mc_inst<true, true>(st, grid, smem, a) : launch_mc_inst<true, false>(st, grid, smem, a))
+                               : (trend ? launch_mc_inst<false, true>(st, grid, smem, a) : launch_mc_inst<false, false>(st, grid, smem, a));
+    return e == cudaSuccess ? 0 : 1;
 }
 
 }  // namespace pb200

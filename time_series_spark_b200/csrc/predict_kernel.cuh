@@ -30,7 +30,9 @@ struct PredictArgs {
     int smax, kmax, pstride;
     int growth, mult;
     double* yhat;
-    double* trend;           // optional (may be null)
+    // optional (may be null): the trend plane [n_models * horizon]; predict_kernel<true> writes the other five component
+    // planes after it, at a stride of n_models * horizon (PB200_COMP_* order)
+    double* trend;
     int* yhat_int;
 };
 
@@ -140,6 +142,22 @@ __device__ __forceinline__ double seasonal_term(const ModelSm& ms, const long lo
     return acc;
 }
 
+// seasonal_term with each seasonality's own term kept (0.0 where the mask lacks it): the sum takes the same additions in
+// the same order, so it is seasonal_term's value bit for bit
+__device__ __forceinline__ double seasonal_parts(const ModelSm& ms, const long long d, double* yearly, double* weekly,
+                                                 double* daily) {
+    const double tau = (1e-9 * (double)d) / 86400.0;
+    double acc = 0.0;
+    int col = 0;
+    *yearly = *weekly = *daily = 0.0;
+    if (ms.mask & 1) { *yearly = seas_dot(tau, 365.25, 10, ms.beta + col); acc += *yearly; col += 20; }
+    if (ms.mask & 2) { *weekly = seas_dot(tau, 7.0, 3, ms.beta + col); acc += *weekly; col += 6; }
+    if (ms.mask & 4) { *daily = seas_dot(tau, 1.0, 4, ms.beta + col); acc += *daily; col += 8; }
+    return acc;
+}
+
+// COMP: also write fbprophet's component columns -- planes PB200_COMP_* of a.trend, each [n_models * horizon]
+template <bool COMP>
 __global__ void __launch_bounds__(256) predict_kernel(const PredictArgs a) {
     __shared__ ModelSm ms;
     const int model = blockIdx.x;
@@ -147,11 +165,17 @@ __global__ void __launch_bounds__(256) predict_kernel(const PredictArgs a) {
     load_model(ms, a, model, tid, blockDim.x);
     const bool ok = ms.status >= 0;
     const int S = ms.S;
+    const size_t plane = (size_t)a.n_models * a.horizon;
     for (int h = blockIdx.y * blockDim.x + tid; h < a.horizon; h += gridDim.y * blockDim.x) {
         const size_t o = (size_t)model * a.horizon + h;
         if (!ok) {
             a.yhat[o] = NAN;
-            if (a.trend) a.trend[o] = NAN;
+            if (COMP) {
+#pragma unroll
+                for (int c = 0; c < PB200_N_COMPONENTS; ++c) a.trend[c * plane + o] = NAN;
+            } else if (a.trend) {
+                a.trend[o] = NAN;
+            }
             a.yhat_int[o] = INT32_MIN;
             continue;
         }
@@ -168,10 +192,25 @@ __global__ void __launch_bounds__(256) predict_kernel(const PredictArgs a) {
         if (a.growth == PB200_GROWTH_LOGISTIC) tr = ms.cap_s / (1.0 + exp(-kt * (t - mt)));
         else tr = kt * t + mt;
         tr = tr * ms.y_scale + ms.floor;
-        const double sd = ms.K > 0 ? seasonal_term(ms, d) : 0.0;
+        double sd, cy = 0.0, cw = 0.0, cd = 0.0;
+        if (COMP) sd = ms.K > 0 ? seasonal_parts(ms, d, &cy, &cw, &cd) : 0.0;
+        else sd = ms.K > 0 ? seasonal_term(ms, d) : 0.0;
+        // the expression of predict_kernel<false>, so that yhat keeps its bits.  In additive mode the compiler fuses it
+        // into fma(sd, y_scale, trend): the product is not rounded on its own, while the additive_terms plane holds it
+        // rounded (fbprophet's value), so yhat and trend + additive_terms may differ by that one rounding (DESIGN §12)
         const double yh = a.mult ? tr * (1.0 + sd) : tr + sd * ms.y_scale;
+        if (COMP) {
+            const double add = __dmul_rn(sd, ms.y_scale);
+            const double s = a.mult ? 1.0 : ms.y_scale;
+            a.trend[o] = tr;
+            a.trend[PB200_COMP_MULTIPLICATIVE * plane + o] = a.mult ? sd : 0.0;
+            a.trend[PB200_COMP_ADDITIVE * plane + o] = a.mult ? 0.0 : add;
+            a.trend[PB200_COMP_YEARLY * plane + o] = cy * s;
+            a.trend[PB200_COMP_WEEKLY * plane + o] = cw * s;
+            a.trend[PB200_COMP_DAILY * plane + o] = cd * s;
+        }
         a.yhat[o] = yh;
-        if (a.trend) a.trend[o] = tr;
+        if (!COMP && a.trend) a.trend[o] = tr;
         // prophet_scorer.py:73 astype(int) truncates toward zero; :76-84 values < floor -> floor
         double yt = trunc(yh);
         const double fcfg = a.floor[model];

@@ -11,7 +11,9 @@ floor-clamp body (reference :35-102) is one batched GPU call over all models.
 Optional keys beyond the reference: ``forecast.intervals`` (default false: the reference
 computes yhat_lower/yhat_upper inside Prophet.predict and drops them at :86; set true to get
 ``yhat_lower``/``yhat_upper`` columns), ``forecast.uncertainty_samples`` (1000),
-``forecast.interval_width`` (0.8), ``forecast.seed``.
+``forecast.interval_width`` (0.8), ``forecast.seed``, ``forecast.components`` (default false; true adds fbprophet's
+component columns ``trend, yearly, weekly, daily, multiplicative_terms, additive_terms``, and ``trend_lower`` /
+``trend_upper`` with intervals -- DESIGN §12).
 """
 from __future__ import annotations
 
@@ -37,6 +39,39 @@ FORECAST_SCHEMA = pa.schema([   # reference prophet_scorer.py:27-32
     pa.field("ds", pa.timestamp("ns"), True),
     pa.field("yhat", pa.int32(), True),
 ])
+
+
+# fbprophet's component columns of Prophet.predict, in the frame's order; a seasonal column is null on the rows of a model
+# that has no such seasonality (fbprophet would have no such column for it)
+COMPONENT_COLUMNS = ("trend", "yearly", "weekly", "daily", "multiplicative_terms", "additive_terms")
+_SEASONAL_BIT = {"yearly": 1, "weekly": 2, "daily": 4}
+
+
+def _want_components(fc) -> bool:
+    v = fc.get("components", False)
+    if not isinstance(v, (bool, np.bool_)):
+        raise ValueError(f"forecast.components must be true or false (got {v!r})")
+    return bool(v)
+
+
+def _component_fields(intervals: bool):
+    names = COMPONENT_COLUMNS + (("trend_lower", "trend_upper") if intervals else ())
+    return [pa.field(n, pa.float64()) for n in names]
+
+
+def component_columns(res: "batched.ForecastBatch", mask: np.ndarray, periods: int, intervals: bool) -> dict:
+    """The component columns of one shard's forecast frame, one row per (model, period), from a components predict
+    (``res``) and the models' seasonality masks (meta_i32[:, 3])."""
+    mask = np.asarray(mask)
+    cols = {}
+    for name in COMPONENT_COLUMNS:
+        v = np.ascontiguousarray(res.component(name)).reshape(-1)
+        absent = np.repeat((mask & _SEASONAL_BIT[name]) == 0, periods) if name in _SEASONAL_BIT else None
+        cols[name] = pa.array(v, pa.float64(), mask=absent)
+    if intervals:
+        cols["trend_lower"] = pa.array(res.trend_lower.reshape(-1), pa.float64())
+        cols["trend_upper"] = pa.array(res.trend_upper.reshape(-1), pa.float64())
+    return cols
 
 
 # pandas 0.25 (the reference's pin) offset aliases that later pandas renamed
@@ -104,6 +139,7 @@ class _ForecastTimeSeriesOp:
             width = float(fc.get("interval_width", 0.8))
             if not 0.0 <= width <= 1.0:     # fbprophet refuses it too (numpy's percentile range check); NaN fails here
                 raise ValueError(f"forecast.interval_width must be in [0, 1] (got {fc.get('interval_width')!r})")
+        want_components = _want_components(fc)
         rank, ws, _ = pdist.world()
         if ws > 1 and table.num_rows:      # shard the model rows across ranks (equal horizon => equal work)
             lo, hi = pdist.shard_bounds(np.arange(table.num_rows + 1, dtype=np.int64), ws)[rank]
@@ -113,6 +149,9 @@ class _ForecastTimeSeriesOp:
         empty_schema = FORECAST_SCHEMA
         if want_intervals:
             empty_schema = empty_schema.append(pa.field("yhat_lower", pa.float64())).append(pa.field("yhat_upper", pa.float64()))
+        if want_components:
+            for f in _component_fields(want_intervals):
+                empty_schema = empty_schema.append(f)
         if table.num_rows == 0:
             return empty_schema.empty_table()
         # model is None -> "no model found", empty frame for that group (reference :51-55)
@@ -138,7 +177,7 @@ class _ForecastTimeSeriesOp:
         future = frequency_to_future(last_ds, periods, fc["frequency"])
         ctx = get_context()
         res = batched.predict_batch_host(ctx, opts, fitted, future, floor, cap, seed=int(fc.get("seed", 0)),
-                                         intervals=want_intervals)
+                                         intervals=want_intervals, components=want_components)
         sid = table["series_id"].combine_chunks().to_numpy(zero_copy_only=False).astype(np.int32)
         did = table["dim_id"].combine_chunks().to_numpy(zero_copy_only=False).astype(np.int32)
         ok = fitted.meta_i32[:, 4] >= 0
@@ -155,6 +194,8 @@ class _ForecastTimeSeriesOp:
         if want_intervals:
             cols["yhat_lower"] = pa.array(res.yhat_lower.reshape(-1), pa.float64())
             cols["yhat_upper"] = pa.array(res.yhat_upper.reshape(-1), pa.float64())
+        if want_components:
+            cols.update(component_columns(res, fitted.meta_i32[:, 3], periods, want_intervals))
         out = pa.table(cols)
         if not ok.all():
             out = out.filter(pa.array(np.repeat(ok, periods)))
@@ -307,7 +348,7 @@ class ProphetScorer:
             "forecast_timestamp": ds,
             "forecast_quantity": t["yhat"],
         }
-        for extra in ("yhat_lower", "yhat_upper"):
+        for extra in ("yhat_lower", "yhat_upper") + COMPONENT_COLUMNS + ("trend_lower", "trend_upper"):
             if extra in t.column_names:
                 cols[extra] = t[extra]
         out = Frame(pa.table(cols))
@@ -368,8 +409,9 @@ class ProphetScorer:
             if got is None:
                 pdist.prepare_output_dir(scorer.config["io"]["forecasts"])
                 return
-            arrays = [pa.array(a, pa.int64()).cast(pa.timestamp("ns")) if n == "ds" else pa.array(a)
-                      for n, a in zip(t.column_names, got)]
+            # a seasonal component column's nulls travel as NaN (the rows of failed models, the only NaN ones, are gone)
+            arrays = [pa.array(a, pa.int64()).cast(pa.timestamp("ns")) if n == "ds" else
+                      pa.array(a, from_pandas=n in _SEASONAL_BIT) for n, a in zip(t.column_names, got)]
             forecast_df = Frame(pa.table(dict(zip(t.column_names, arrays))).cast(t.schema))
         converted_df = scorer.convert_forecasts(forecast_df)
         scorer.write_forecasts(converted_df)
