@@ -339,6 +339,48 @@ PB200_API int pb200_predict_components_host(pb200_ctx* ctx, const pb200_options*
                        double* h_yhat, double* h_yhat_lower, double* h_yhat_upper,
                        int32_t* h_yhat_int, double* h_components, double* h_trend_lower, double* h_trend_upper);
 
+/*
+ * pb200_predict_* plus forecast totals over fixed-width time windows with joint-draw intervals: fbprophet's
+ * predictive_samples(future)['yhat'] summed per window, then percentiles of the sums (DESIGN §13).  Same arguments and the
+ * same yhat / yhat_lower / yhat_upper / yhat_int bits as pb200_predict_* (d_yhat_lower / d_yhat_upper optional as there), and:
+ *   width_ns > 0, origin_ns   the window of a point is floor((ds - origin_ns) / width_ns); a model's windows are the
+ *                 maximal runs of equal window index in its (ascending) frame, in order
+ *   wmax > 0      slots per model in the arrays below
+ *   d_n_windows   int32 [n_models]  the model's number of windows -- the true count also when it exceeds wmax, in which
+ *                 case only the first wmax windows are written: the caller checks
+ * and, each [n_models * wmax], slot j of model i at i * wmax + j:
+ *   d_win_start     int64   origin_ns + index * width_ns of window j
+ *   d_win_points    int32   frame points in it (the first and last window of a frame may be partial)
+ *   d_yhat_sum      double  s = 0.0; s = s + yhat[h] over the window's points in frame order
+ *   d_quantity_sum  int64   sum of yhat_int over them
+ *   d_sum_lower / d_sum_upper  double  numpy linear-interpolation percentiles at 100(1 -+ interval_width)/2 over the
+ *                 uncertainty_samples sums of the draws behind yhat_lower / yhat_upper, each draw summed like yhat_sum
+ * Slots at or past n_windows hold INT64_MIN / 0 / NaN / INT64_MIN / NaN / NaN.  Failed models (status < 0) have no window.
+ * uncertainty_samples must be in [2, 1024] (PB200_E_UNSUPPORTED) and interval_width in [0, 1], width_ns and wmax > 0 and
+ * the window outputs non-null (PB200_E_ARG): nothing is launched otherwise.
+ */
+PB200_API int pb200_predict_sums_device(pb200_ctx* ctx, const pb200_options* opts,
+                         const double* d_params, const double* d_tchange,
+                         const int32_t* d_meta_i32, const int64_t* d_meta_i64,
+                         const double* d_meta_f64, int64_t n_models,
+                         const int64_t* d_future_ds, int32_t horizon,
+                         const double* d_floor, const double* d_cap, uint64_t seed,
+                         double* d_yhat, double* d_yhat_lower, double* d_yhat_upper,
+                         int32_t* d_yhat_int, int64_t width_ns, int64_t origin_ns, int32_t wmax,
+                         int32_t* d_n_windows, int64_t* d_win_start, int32_t* d_win_points,
+                         double* d_yhat_sum, int64_t* d_quantity_sum, double* d_sum_lower, double* d_sum_upper);
+
+PB200_API int pb200_predict_sums_host(pb200_ctx* ctx, const pb200_options* opts,
+                       const double* h_params, const double* h_tchange,
+                       const int32_t* h_meta_i32, const int64_t* h_meta_i64,
+                       const double* h_meta_f64, int64_t n_models,
+                       const int64_t* h_future_ds, int32_t horizon,
+                       const double* h_floor, const double* h_cap, uint64_t seed,
+                       double* h_yhat, double* h_yhat_lower, double* h_yhat_upper,
+                       int32_t* h_yhat_int, int64_t width_ns, int64_t origin_ns, int32_t wmax,
+                       int32_t* h_n_windows, int64_t* h_win_start, int32_t* h_win_points,
+                       double* h_yhat_sum, int64_t* h_quantity_sum, double* h_sum_lower, double* h_sum_upper);
+
 /* future_ds[i*horizon + j] = last_ds[i] + (j+1)*freq_ns  -- make_future_dataframe
  * (include_history=False) for a fixed-width pandas frequency. */
 PB200_API int pb200_make_future_device(pb200_ctx* ctx, const int64_t* d_last_ds, int64_t n_models,

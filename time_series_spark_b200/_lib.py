@@ -52,7 +52,8 @@ class Layout(C.Structure):
 EXPORTS = [
     "pb200_default_options", "pb200_get_layout", "pb200_create", "pb200_destroy", "pb200_last_error",
     "pb200_stream", "pb200_launch_count", "pb200_last_fit_variant_counts", "pb200_tab_chunk", "pb200_fit_device", "pb200_fit_prior_device", "pb200_fit_warm_device", "pb200_fit_host", "pb200_fit_warm_host", "pb200_predict_device",
-    "pb200_predict_host", "pb200_predict_components_device", "pb200_predict_components_host", "pb200_make_future_device", "pb200_synchronize", "pb200_objective_host",
+    "pb200_predict_host", "pb200_predict_components_device", "pb200_predict_components_host",
+    "pb200_predict_sums_device", "pb200_predict_sums_host", "pb200_make_future_device", "pb200_synchronize", "pb200_objective_host",
     "pb200_fit_trace_host", "pb200_forecast_csv_lengths_device", "pb200_forecast_csv_rows_device", "pb200_forecast_csv_row_host",
     "pb200_cv_plan_counts_device", "pb200_cv_plan_device", "pb200_cv_gather_device", "pb200_cv_metrics_device",
 ]
@@ -111,6 +112,10 @@ def load() -> C.CDLL:
     lib.pb200_predict_components_device.restype = C.c_int
     lib.pb200_predict_components_host.argtypes = pred_args + [vp, vp, vp]
     lib.pb200_predict_components_host.restype = C.c_int
+    lib.pb200_predict_sums_device.argtypes = pred_args + [i64, i64, i32, vp, vp, vp, vp, vp, vp, vp]
+    lib.pb200_predict_sums_device.restype = C.c_int
+    lib.pb200_predict_sums_host.argtypes = pred_args + [i64, i64, i32, vp, vp, vp, vp, vp, vp, vp]
+    lib.pb200_predict_sums_host.restype = C.c_int
     lib.pb200_make_future_device.argtypes = [vp, vp, i64, i32, i64, vp]
     lib.pb200_make_future_device.restype = C.c_int
     lib.pb200_objective_host.argtypes = [vp, OP, vp, vp, i32, vp, i64, dbl, dbl, vp, vp, vp, vp]

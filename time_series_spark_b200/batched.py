@@ -439,6 +439,108 @@ def predict_batch_device(ctx: L.Context, opts: L.Options, fitted: FittedBatch, f
     return ForecastBatch(future_ds, yhat, lo, hi, yint, comp, tlo, thi)
 
 
+@dataclass
+class WindowSums:
+    """Forecast totals over fixed-width time windows (pb200_predict_sums_*), each [N, wmax]; slots at or past a model's
+    ``n_windows`` hold INT64_MIN / 0 / NaN."""
+    n_windows: object     # [N] int32
+    start: object         # int64 ns: origin + window index * width
+    points: object        # int32: frame points in the window
+    yhat_sum: object      # f64: yhat summed in frame order
+    quantity_sum: object  # int64: yhat_int summed
+    lower: object         # f64: percentiles over the draws' window sums
+    upper: object
+
+
+def window_slots(first_ds, last_ds, width_ns: int, origin_ns: int) -> int:
+    """An upper bound on a model's windows from the first and last column of an ascending frame:
+    max_i (w(last_i) - w(first_i) + 1), w = floor((ds - origin) / width).  Exact when the grid is no coarser than the
+    width; windows that hold no point take no slot."""
+    if len(first_ds) == 0:
+        return 1
+    return int(((last_ds - origin_ns) // width_ns - (first_ds - origin_ns) // width_ns).max()) + 1
+
+
+def _check_window_slots(wmax: int, n_windows_max: int) -> None:
+    if n_windows_max > wmax:
+        raise ValueError(f"a model has {n_windows_max} windows, more than the {wmax} slots sized from the frame's first and "
+                         "last columns: is every model's future frame ascending?")
+
+
+def predict_sums_host(ctx: L.Context, opts: L.Options, fitted: FittedBatch, future_ds: np.ndarray, floor: np.ndarray,
+                      cap: np.ndarray, width_ns: int, origin_ns: int = 0, seed: int = 0, intervals: bool = False):
+    """pb200_predict_sums_host: predict_batch_host's ForecastBatch and the WindowSums of the windows
+    floor((ds - origin_ns) / width_ns) of each model's ascending frame -- totals of yhat / yhat_int per window and the
+    interval of each total from the joint draws (fbprophet's predictive_samples summed per window).  Needs
+    ``opts.uncertainty_samples`` in [2, 1024]; ``intervals`` asks for the pointwise yhat_lower / yhat_upper as well."""
+    fitted = fitted.to_host()
+    n = fitted.n
+    future_ds = np.ascontiguousarray(future_ds, dtype=np.int64)
+    future_ds = future_ds.reshape(n, -1) if n else future_ds.reshape(0, future_ds.shape[-1] if future_ds.ndim == 2 else 0)
+    h = future_ds.shape[1]
+    floor = np.ascontiguousarray(np.broadcast_to(np.asarray(floor, dtype=np.float64), (n,)))
+    cap = np.ascontiguousarray(np.broadcast_to(np.asarray(cap, dtype=np.float64), (n,)))
+    width_ns, origin_ns = int(width_ns), int(origin_ns)
+    if width_ns <= 0:
+        raise ValueError(f"width_ns must be > 0 (got {width_ns})")
+    wmax = window_slots(future_ds[:, 0], future_ds[:, -1], width_ns, origin_ns) if h else 1
+    yhat = np.empty((n, h), np.float64)
+    yint = np.empty((n, h), np.int32)
+    lo = np.empty((n, h), np.float64) if intervals else None
+    hi = np.empty((n, h), np.float64) if intervals else None
+    ws = WindowSums(np.zeros(n, np.int32), np.empty((n, wmax), np.int64), np.empty((n, wmax), np.int32),
+                    np.empty((n, wmax), np.float64), np.empty((n, wmax), np.int64), np.empty((n, wmax), np.float64),
+                    np.empty((n, wmax), np.float64))
+    rc = L.load().pb200_predict_sums_host(
+        ctx.handle, C.byref(opts), _np_ptr(np.ascontiguousarray(fitted.params)),
+        _np_ptr(np.ascontiguousarray(fitted.tchange)), _np_ptr(np.ascontiguousarray(fitted.meta_i32)),
+        _np_ptr(np.ascontiguousarray(fitted.meta_i64)), _np_ptr(np.ascontiguousarray(fitted.meta_f64)),
+        n, _np_ptr(future_ds), h, _np_ptr(floor), _np_ptr(cap), int(seed) & (2**64 - 1),
+        _np_ptr(yhat), _np_ptr(lo) if intervals else None, _np_ptr(hi) if intervals else None, _np_ptr(yint),
+        width_ns, origin_ns, wmax, _np_ptr(ws.n_windows), _np_ptr(ws.start), _np_ptr(ws.points), _np_ptr(ws.yhat_sum),
+        _np_ptr(ws.quantity_sum), _np_ptr(ws.lower), _np_ptr(ws.upper))
+    L.check(rc, "pb200_predict_sums_host")
+    _check_window_slots(wmax, int(ws.n_windows.max()) if n else 0)
+    return ForecastBatch(future_ds, yhat, lo, hi, yint), ws
+
+
+def predict_sums_device(ctx: L.Context, opts: L.Options, fitted: FittedBatch, future_ds, floor, cap, width_ns: int,
+                        origin_ns: int = 0, seed: int = 0, intervals: bool = False):
+    """pb200_predict_sums_device with torch CUDA tensors; as predict_sums_host."""
+    import torch
+    n = fitted.n
+    h = int(future_ds.shape[1])
+    dev = future_ds.device
+    width_ns, origin_ns = int(width_ns), int(origin_ns)
+    if width_ns <= 0:
+        raise ValueError(f"width_ns must be > 0 (got {width_ns})")
+    wmax = 1
+    if n and h:
+        ends = future_ds[:, [0, -1]].cpu().numpy()
+        wmax = window_slots(ends[:, 0], ends[:, 1], width_ns, origin_ns)
+    f64 = dict(dtype=torch.float64, device=dev)
+    yhat = torch.empty((n, h), **f64)
+    yint = torch.empty((n, h), dtype=torch.int32, device=dev)
+    lo = torch.empty((n, h), **f64) if intervals else None
+    hi = torch.empty((n, h), **f64) if intervals else None
+    ws = WindowSums(torch.zeros(n, dtype=torch.int32, device=dev), torch.empty((n, wmax), dtype=torch.int64, device=dev),
+                    torch.empty((n, wmax), dtype=torch.int32, device=dev), torch.empty((n, wmax), **f64),
+                    torch.empty((n, wmax), dtype=torch.int64, device=dev), torch.empty((n, wmax), **f64),
+                    torch.empty((n, wmax), **f64))
+    torch.cuda.current_stream(dev).synchronize()
+    rc = L.load().pb200_predict_sums_device(
+        ctx.handle, C.byref(opts), fitted.params.data_ptr(), fitted.tchange.data_ptr(), fitted.meta_i32.data_ptr(),
+        fitted.meta_i64.data_ptr(), fitted.meta_f64.data_ptr(), n, future_ds.data_ptr(), h, floor.data_ptr(),
+        cap.data_ptr(), int(seed) & (2**64 - 1), yhat.data_ptr(), lo.data_ptr() if intervals else None,
+        hi.data_ptr() if intervals else None, yint.data_ptr(), width_ns, origin_ns, wmax, ws.n_windows.data_ptr(),
+        ws.start.data_ptr(), ws.points.data_ptr(), ws.yhat_sum.data_ptr(), ws.quantity_sum.data_ptr(), ws.lower.data_ptr(),
+        ws.upper.data_ptr())
+    L.check(rc, "pb200_predict_sums_device")
+    ctx.synchronize()
+    _check_window_slots(wmax, int(ws.n_windows.max().item()) if n else 0)
+    return ForecastBatch(future_ds, yhat, lo, hi, yint), ws
+
+
 def objective_host(ctx: L.Context, opts: L.Options, ds_ns: np.ndarray, y: np.ndarray, offsets: np.ndarray,
                    floor: float, cap_multiplier: float, theta: np.ndarray):
     """pb200_objective_host (parity-test hook): objective and gradient at ``theta`` rows

@@ -107,6 +107,7 @@ struct pb200_ctx {
     DevBuf d_fut, d_floor, d_yhat, d_lo, d_hi, d_yint;
     DevBuf d_comp, d_tlo, d_thi;   // staging of pb200_predict_components_host's planes and trend bounds
     DevBuf d_mc;     // MC workspace
+    DevBuf d_sums;   // staging of pb200_predict_sums_host's window outputs
     int lc0_max = 1 << 30; // PB200_LC0_MAX: longest series on one warp per series, longer ones get four (unset: no limit)
     bool lc_auto = true;   // false when PB200_LC0_MAX pins the CTA width
     bool tab_on = true;    // PB200_NO_TAB=1 disables the seasonal-table variants (A/B runs)
@@ -293,7 +294,7 @@ PB200_API void pb200_destroy(pb200_ctx* c) {
     cudaSetDevice(c->device);
     cudaStreamSynchronize(c->stream);
     for (DevBuf* b : {&c->d_ds, &c->d_y, &c->d_cap, &c->d_params, &c->d_tchange, &c->d_mi32, &c->d_mi64, &c->d_mf64, &c->d_fut,
-                      &c->d_floor, &c->d_yhat, &c->d_lo, &c->d_hi, &c->d_yint, &c->d_comp, &c->d_tlo, &c->d_thi, &c->d_mc,&c->d_trace, &c->d_warm_x, &c->d_prior, &c->d_iparams, &c->d_imeta, &c->d_warm, &c->d_vcount, &c->d_offsets,
+                      &c->d_floor, &c->d_yhat, &c->d_lo, &c->d_hi, &c->d_yint, &c->d_comp, &c->d_tlo, &c->d_thi, &c->d_mc, &c->d_sums, &c->d_trace, &c->d_warm_x, &c->d_prior, &c->d_iparams, &c->d_imeta, &c->d_warm, &c->d_vcount, &c->d_offsets,
                       &c->d_order, &c->d_lenclass, &c->d_qitems, &c->d_qctl, &c->d_nq, &c->d_planes, &c->d_qkey, &c->d_qhist})
         b->release();
     c->h_ctl.release();
@@ -821,22 +822,49 @@ int check_comp_args(const pb200_options* o, const void* comp, const void* lo, co
     return PB200_OK;
 }
 
+// the window arguments of pb200_predict_sums_*: the rule, the slots per model and the seven outputs (device pointers in
+// predict_device, host pointers in predict_host)
+struct SumOut {
+    int64_t width_ns, origin_ns;
+    int32_t wmax;
+    int32_t* n_windows;
+    int64_t* win_start;
+    int32_t* win_points;
+    double* yhat_sum;
+    int64_t* quantity_sum;
+    double* sum_lower;
+    double* sum_upper;
+};
+
+// checked before anything is copied or launched
+int check_sum_args(const pb200_options* o, const SumOut& s) {
+    const int rc = check_mc_opts(o);
+    if (rc) return rc;
+    if (s.width_ns <= 0) return fail(PB200_E_ARG, "width_ns must be > 0");
+    if (s.wmax <= 0) return fail(PB200_E_ARG, "wmax must be > 0");
+    if (!s.n_windows || !s.win_start || !s.win_points || !s.yhat_sum || !s.quantity_sum || !s.sum_lower || !s.sum_upper)
+        return fail(PB200_E_ARG, "null pointer (window outputs)");
+    return PB200_OK;
+}
+
 // pb200_predict_device; d_comp != null: the components instance of predict_kernel, d_tlo / d_thi != null: the
-// trend-bounds instance of mc_kernel
+// trend-bounds instance of mc_kernel; sums != null: mc_sum_kernel after them (it also runs on an empty frame, where
+// every model has no window)
 int predict_device(pb200_ctx* c, const pb200_options* opts, const double* d_params, const double* d_tchange,
                    const int32_t* d_meta_i32, const int64_t* d_meta_i64, const double* d_meta_f64, int64_t n_models,
                    const int64_t* d_future_ds, int32_t horizon, const double* d_floor, const double* d_cap, uint64_t seed,
                    double* d_yhat, double* d_yhat_lower, double* d_yhat_upper, int32_t* d_yhat_int, double* d_comp,
-                   double* d_tlo, double* d_thi) {
+                   double* d_tlo, double* d_thi, const SumOut* sums = nullptr) {
     if (!c) return fail(PB200_E_ARG, "ctx is null");
     int rc = check_opts(opts);
     if (rc) return rc;
     if (n_models < 0 || horizon < 0 || n_models > (1LL << 30)) return fail(PB200_E_ARG, "sizes");
-    if (n_models == 0 || horizon == 0) return PB200_OK;
-    if (!d_params || !d_tchange || !d_meta_i32 || !d_meta_i64 || !d_meta_f64 || !d_future_ds || !d_floor || !d_cap ||
-        !d_yhat || !d_yhat_int)
+    if (sums && (rc = check_sum_args(opts, *sums))) return rc;
+    if (n_models == 0 || (horizon == 0 && !sums)) return PB200_OK;
+    if (!d_params || !d_tchange || !d_meta_i32 || !d_meta_i64 || !d_meta_f64 || !d_floor || !d_cap ||
+        (horizon > 0 && (!d_future_ds || !d_yhat || !d_yhat_int)))
         return fail(PB200_E_ARG, "null pointer");
-    const bool mc = d_yhat_lower && d_yhat_upper && opts->uncertainty_samples > 0;
+    const bool mc = horizon > 0 && d_yhat_lower && d_yhat_upper && opts->uncertainty_samples > 0;
     if (mc && (rc = check_mc_opts(opts))) return rc;
     pb200_layout L;
     pb200_get_layout(opts, &L);
@@ -860,7 +888,7 @@ int predict_device(pb200_ctx* c, const pb200_options* opts, const double* d_para
     a.yhat = d_yhat;
     a.trend = d_comp;
     a.yhat_int = d_yhat_int;
-    {
+    if (horizon > 0) {
         // one CTA per (model, 1024 future points): the per-model prologue (parameters, the serial gamma recurrence) is paid
         // once for config #5's 672 periods instead of three times
         dim3 grid((unsigned)n_models, (unsigned)std::min((horizon + 1023) / 1024, 64));
@@ -876,6 +904,23 @@ int predict_device(pb200_ctx* c, const pb200_options* opts, const double* d_para
         if (rc) return fail(PB200_E_CUDA, "mc kernel launch", cudaGetLastError());
         c->launches++;
     }
+    if (sums) {
+        pb200::McSumArgs s;
+        s.mc.lower = sums->sum_lower;
+        s.mc.upper = sums->sum_upper;
+        s.width_ns = sums->width_ns;
+        s.origin_ns = sums->origin_ns;
+        s.wmax = sums->wmax;
+        s.n_windows = sums->n_windows;
+        s.win_start = (long long*)sums->win_start;
+        s.win_points = sums->win_points;
+        s.yhat_sum = sums->yhat_sum;
+        s.quantity_sum = (long long*)sums->quantity_sum;
+        rc = pb200::launch_mc_sum(c->stream, c->sms, a, opts->uncertainty_samples, opts->interval_width, seed, s);
+        if (rc == -1) return fail(PB200_E_ARG, "uncertainty_samples / interval_width out of range");
+        if (rc) return fail(PB200_E_CUDA, "mc sum kernel launch", cudaGetLastError());
+        c->launches++;
+    }
     return PB200_OK;
 }
 
@@ -884,20 +929,40 @@ int predict_host(pb200_ctx* c, const pb200_options* opts, const double* h_params
                  const int32_t* h_meta_i32, const int64_t* h_meta_i64, const double* h_meta_f64, int64_t n_models,
                  const int64_t* h_future_ds, int32_t horizon, const double* h_floor, const double* h_cap, uint64_t seed,
                  double* h_yhat, double* h_yhat_lower, double* h_yhat_upper, int32_t* h_yhat_int, double* h_comp,
-                 double* h_tlo, double* h_thi) {
+                 double* h_tlo, double* h_thi, const SumOut* sums = nullptr) {
     if (!c) return fail(PB200_E_ARG, "ctx is null");
     int rc = check_opts(opts);
     if (rc) return rc;
-    if (n_models <= 0 || horizon <= 0) return (n_models == 0 || horizon == 0) ? PB200_OK : fail(PB200_E_ARG, "sizes");
-    if (!h_params || !h_tchange || !h_meta_i32 || !h_meta_i64 || !h_meta_f64 || !h_future_ds || !h_floor || !h_cap ||
-        !h_yhat || !h_yhat_int)
+    if (sums) {
+        if (n_models < 0 || horizon < 0) return fail(PB200_E_ARG, "sizes");
+        if ((rc = check_sum_args(opts, *sums))) return rc;
+        if (n_models == 0) return PB200_OK;
+    } else if (n_models <= 0 || horizon <= 0) {
+        return (n_models == 0 || horizon == 0) ? PB200_OK : fail(PB200_E_ARG, "sizes");
+    }
+    if (!h_params || !h_tchange || !h_meta_i32 || !h_meta_i64 || !h_meta_f64 || !h_floor || !h_cap ||
+        (horizon > 0 && (!h_future_ds || !h_yhat || !h_yhat_int)))
         return fail(PB200_E_ARG, "null pointer");
     pb200_layout L;
     pb200_get_layout(opts, &L);
     CK(cudaSetDevice(c->device));
     const size_t N = (size_t)n_models, NH = N * (size_t)horizon;
-    const bool mc = h_yhat_lower && h_yhat_upper && opts->uncertainty_samples > 0;
+    const bool mc = horizon > 0 && h_yhat_lower && h_yhat_upper && opts->uncertainty_samples > 0;
     if (mc && (rc = check_mc_opts(opts))) return rc;
+    // the window outputs on the device: five 8-byte arrays [N * wmax], then win_points [N * wmax] and n_windows [N]
+    const size_t NW = sums ? N * (size_t)sums->wmax : 0;
+    SumOut dsum;
+    if (sums) {
+        CK(c->d_sums.reserve(NW * 44 + N * 4));
+        dsum = *sums;
+        dsum.win_start = (int64_t*)c->d_sums.p;
+        dsum.quantity_sum = dsum.win_start + NW;
+        dsum.yhat_sum = (double*)(dsum.quantity_sum + NW);
+        dsum.sum_lower = dsum.yhat_sum + NW;
+        dsum.sum_upper = dsum.sum_lower + NW;
+        dsum.win_points = (int32_t*)(dsum.sum_upper + NW);
+        dsum.n_windows = dsum.win_points + NW;
+    }
     CK(c->d_params.reserve(N * L.pstride * 8));
     CK(c->d_tchange.reserve(N * L.smax * 8));
     CK(c->d_mi32.reserve(N * 8 * 4));
@@ -923,7 +988,7 @@ int predict_host(pb200_ctx* c, const pb200_options* opts, const double* h_params
     CK(cudaMemcpyAsync(c->d_mi32.p, h_meta_i32, N * 8 * 4, cudaMemcpyHostToDevice, st));
     CK(cudaMemcpyAsync(c->d_mi64.p, h_meta_i64, N * 2 * 8, cudaMemcpyHostToDevice, st));
     CK(cudaMemcpyAsync(c->d_mf64.p, h_meta_f64, N * 4 * 8, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(c->d_fut.p, h_future_ds, NH * 8, cudaMemcpyHostToDevice, st));
+    if (NH) CK(cudaMemcpyAsync(c->d_fut.p, h_future_ds, NH * 8, cudaMemcpyHostToDevice, st));
     CK(cudaMemcpyAsync(c->d_floor.p, h_floor, N * 8, cudaMemcpyHostToDevice, st));
     CK(cudaMemcpyAsync(c->d_cap.p, h_cap, N * 8, cudaMemcpyHostToDevice, st));
     rc = predict_device(c, opts, (const double*)c->d_params.p, (const double*)c->d_tchange.p, (const int32_t*)c->d_mi32.p,
@@ -931,10 +996,21 @@ int predict_host(pb200_ctx* c, const pb200_options* opts, const double* h_params
                         horizon, (const double*)c->d_floor.p, (const double*)c->d_cap.p, seed, (double*)c->d_yhat.p,
                         mc ? (double*)c->d_lo.p : nullptr, mc ? (double*)c->d_hi.p : nullptr, (int32_t*)c->d_yint.p,
                         h_comp ? (double*)c->d_comp.p : nullptr, h_tlo ? (double*)c->d_tlo.p : nullptr,
-                        h_tlo ? (double*)c->d_thi.p : nullptr);
+                        h_tlo ? (double*)c->d_thi.p : nullptr, sums ? &dsum : nullptr);
     if (rc) return rc;
-    CK(cudaMemcpyAsync(h_yhat, c->d_yhat.p, NH * 8, cudaMemcpyDeviceToHost, st));
-    CK(cudaMemcpyAsync(h_yhat_int, c->d_yint.p, NH * 4, cudaMemcpyDeviceToHost, st));
+    if (sums) {
+        CK(cudaMemcpyAsync(sums->win_start, dsum.win_start, NW * 8, cudaMemcpyDeviceToHost, st));
+        CK(cudaMemcpyAsync(sums->quantity_sum, dsum.quantity_sum, NW * 8, cudaMemcpyDeviceToHost, st));
+        CK(cudaMemcpyAsync(sums->yhat_sum, dsum.yhat_sum, NW * 8, cudaMemcpyDeviceToHost, st));
+        CK(cudaMemcpyAsync(sums->sum_lower, dsum.sum_lower, NW * 8, cudaMemcpyDeviceToHost, st));
+        CK(cudaMemcpyAsync(sums->sum_upper, dsum.sum_upper, NW * 8, cudaMemcpyDeviceToHost, st));
+        CK(cudaMemcpyAsync(sums->win_points, dsum.win_points, NW * 4, cudaMemcpyDeviceToHost, st));
+        CK(cudaMemcpyAsync(sums->n_windows, dsum.n_windows, N * 4, cudaMemcpyDeviceToHost, st));
+    }
+    if (NH) {     // an empty frame (window sums only: every model then has no window) has nothing to copy
+        CK(cudaMemcpyAsync(h_yhat, c->d_yhat.p, NH * 8, cudaMemcpyDeviceToHost, st));
+        CK(cudaMemcpyAsync(h_yhat_int, c->d_yint.p, NH * 4, cudaMemcpyDeviceToHost, st));
+    }
     if (mc) {
         CK(cudaMemcpyAsync(h_yhat_lower, c->d_lo.p, NH * 8, cudaMemcpyDeviceToHost, st));
         CK(cudaMemcpyAsync(h_yhat_upper, c->d_hi.p, NH * 8, cudaMemcpyDeviceToHost, st));
@@ -995,6 +1071,32 @@ PB200_API int pb200_predict_components_host(pb200_ctx* c, const pb200_options* o
     return predict_host(c, opts, h_params, h_tchange, h_meta_i32, h_meta_i64, h_meta_f64, n_models, h_future_ds, horizon,
                         h_floor, h_cap, seed, h_yhat, h_yhat_lower, h_yhat_upper, h_yhat_int, h_components, h_trend_lower,
                         h_trend_upper);
+}
+
+PB200_API int pb200_predict_sums_device(pb200_ctx* c, const pb200_options* opts, const double* d_params, const double* d_tchange,
+                         const int32_t* d_meta_i32, const int64_t* d_meta_i64, const double* d_meta_f64,
+                         int64_t n_models, const int64_t* d_future_ds, int32_t horizon, const double* d_floor,
+                         const double* d_cap, uint64_t seed, double* d_yhat, double* d_yhat_lower, double* d_yhat_upper,
+                         int32_t* d_yhat_int, int64_t width_ns, int64_t origin_ns, int32_t wmax, int32_t* d_n_windows,
+                         int64_t* d_win_start, int32_t* d_win_points, double* d_yhat_sum, int64_t* d_quantity_sum,
+                         double* d_sum_lower, double* d_sum_upper) {
+    const SumOut s = {width_ns, origin_ns, wmax, d_n_windows, d_win_start, d_win_points, d_yhat_sum, d_quantity_sum,
+                      d_sum_lower, d_sum_upper};
+    return predict_device(c, opts, d_params, d_tchange, d_meta_i32, d_meta_i64, d_meta_f64, n_models, d_future_ds, horizon,
+                          d_floor, d_cap, seed, d_yhat, d_yhat_lower, d_yhat_upper, d_yhat_int, nullptr, nullptr, nullptr, &s);
+}
+
+PB200_API int pb200_predict_sums_host(pb200_ctx* c, const pb200_options* opts, const double* h_params, const double* h_tchange,
+                       const int32_t* h_meta_i32, const int64_t* h_meta_i64, const double* h_meta_f64, int64_t n_models,
+                       const int64_t* h_future_ds, int32_t horizon, const double* h_floor, const double* h_cap,
+                       uint64_t seed, double* h_yhat, double* h_yhat_lower, double* h_yhat_upper, int32_t* h_yhat_int,
+                       int64_t width_ns, int64_t origin_ns, int32_t wmax, int32_t* h_n_windows, int64_t* h_win_start,
+                       int32_t* h_win_points, double* h_yhat_sum, int64_t* h_quantity_sum, double* h_sum_lower,
+                       double* h_sum_upper) {
+    const SumOut s = {width_ns, origin_ns, wmax, h_n_windows, h_win_start, h_win_points, h_yhat_sum, h_quantity_sum,
+                      h_sum_lower, h_sum_upper};
+    return predict_host(c, opts, h_params, h_tchange, h_meta_i32, h_meta_i64, h_meta_f64, n_models, h_future_ds, horizon,
+                        h_floor, h_cap, seed, h_yhat, h_yhat_lower, h_yhat_upper, h_yhat_int, nullptr, nullptr, nullptr, &s);
 }
 
 // ---- forecast CSV rows formatted on the device (csv_kernel.cuh) ----

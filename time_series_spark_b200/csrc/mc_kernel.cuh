@@ -241,6 +241,91 @@ __device__ __forceinline__ bool select_quantiles(const double* row, const int n,
     return true;
 }
 
+// numpy's two percentiles of one row of draws: select_quantiles, or -- when a histogram bin is too crowded for it -- a
+// full bitonic sort of the row (all MC_NP slots: the padding draws hold INFINITY and sort to the end)
+template <bool TIES>
+__device__ __forceinline__ void row_quantiles(double* row, const McArgs& a, int* hist, double* cand, int* cnt,
+                                              const int lane, double& lo_v, double& hi_v) {
+    if (select_quantiles<TIES>(row, a.n_samples, a.lo_i, a.lo_f, a.hi_i, a.hi_f, hist, cand, cnt, lane, lo_v, hi_v)) return;
+    for (int k = 2; k <= MC_NP; k <<= 1) {
+        for (int j = k >> 1; j > 0; j >>= 1) {
+            for (int e = lane; e < MC_NP / 2; e += 32) {
+                const int i = ((e & ~(j - 1)) << 1) | (e & (j - 1));
+                const int l = i | j;
+                const bool up = (i & k) == 0;
+                const double x = row[i], y = row[l];
+                const bool sw = up ? (x > y) : (x < y);
+                if (sw) { row[i] = y; row[l] = x; }
+            }
+            __syncwarp();
+        }
+    }
+    const double l0 = row[a.lo_i], l1 = row[min(a.lo_i + 1, a.n_samples - 1)];
+    const double u0 = row[a.hi_i], u1 = row[min(a.hi_i + 1, a.n_samples - 1)];
+    lo_v = l0 + (l1 - l0) * a.lo_f;
+    hi_v = u0 + (u1 - u0) * a.hi_f;
+}
+
+// What a CTA does for a model before its first point: Tmax = max t over the whole frame, the model's Philox key, and
+// the state of this thread's two draws (tid and tid + MC_THREADS) with the time of their first simulated changepoint.
+// red_t [MC_THREADS / 32] and key_sm are shared scratch; every thread of the CTA calls it.
+__device__ __forceinline__ void start_draws(const McArgs& a, const ModelSm& ms, const int model, const int tid,
+                                            double* red_t, uint64_t* key_sm, Philox& ph, DrawState* d, bool* live) {
+    const int lane = tid & 31, warp = tid >> 5;
+    const int H = a.p.horizon;
+    const size_t base = (size_t)model * H;
+    double tm = -INFINITY;
+    for (int h = tid; h < H; h += MC_THREADS) tm = fmax(tm, (double)(a.p.future_ds[base + h] - ms.start) / ms.t_scale);
+#pragma unroll
+    for (int o = 16; o >= 1; o >>= 1) tm = fmax(tm, __shfl_xor_sync(0xffffffffu, tm, o));
+    if (lane == 0) red_t[warp] = tm;
+    if (warp == 0) {
+        const uint64_t key = model_key(a, model, lane);
+        if (lane == 0) *key_sm = key;
+    }
+    __syncthreads();
+    tm = red_t[0];
+    for (int w = 1; w < MC_THREADS / 32; ++w) tm = fmax(tm, red_t[w]);
+    const double rate = (double)ms.S;
+    ph.k0 = (uint32_t)*key_sm;
+    ph.k1 = (uint32_t)(*key_sm >> 32);
+#pragma unroll
+    for (int q = 0; q < 2; ++q) {
+        const uint32_t draw = tid + q * MC_THREADS;
+        live[q] = (int)draw < a.n_samples;
+        d[q].k = ms.k; d[q].m = ms.m; d[q].s_hist = 0; d[q].cp_ctr = 0; d[q].next_cp = INFINITY;
+        if (live[q] && tm > 1.0) {
+            uint32_t r[4];
+            ph.gen(draw, 0xffffffffu, 1u, 0u, r);
+            d[q].next_cp = 1.0 - log(u01(r[0], r[1])) / rate;
+        }
+    }
+}
+
+// the two standard normals of one draw for the points 2 * pair and 2 * pair + 1 of the frame (Box-Muller: two per Philox call)
+__device__ __forceinline__ void noise_pair(const Philox& ph, const uint32_t draw, const uint32_t pair, double* z) {
+    uint32_t r[4];
+    ph.gen(draw, pair, 0u, 0u, r);
+    const double rad = sqrt(-2.0 * log(u01(r[0], r[1])));
+    double sn, cs;
+    sincospi(2.0 * u01(r[2], r[3]), &sn, &cs);
+    z[0] = rad * cs;
+    z[1] = rad * sn;
+}
+
+// one draw's yhat at the next point of the frame (time t, seasonal term sd, standard normal z): advances the draw's trend
+// state to t; tr gets the noise-free trend.  rate = S, nscale = sigma_obs * y_scale
+template <bool LOGI>
+__device__ __forceinline__ double draw_point(DrawState& d, const ModelSm& ms, const double t, const double sd, const double z,
+                                             const Philox& ph, const uint32_t draw, const double rate, const double nscale,
+                                             const int mult, double& tr) {
+    advance<LOGI>(d, ms, t, ph, draw, rate);
+    if (LOGI) tr = ms.cap_s / (1.0 + exp(-d.k * (t - d.m)));
+    else tr = d.k * t + d.m;
+    tr = tr * ms.y_scale + ms.floor;
+    return (mult ? tr * (1.0 + sd) : tr + sd * ms.y_scale) + nscale * z;
+}
+
 // TREND: also the bounds of the noise-free trend draws.  The tile is then TILE = 8 points: rows [0, 8) hold the yhat
 // draws and rows [8, 16) the trend draws of the same points, in the same 128 KB, and warp w still selects row w.  The
 // yhat draws are the same numbers (the noise counters go by pairs of points and 8 is even; the trend state advances per
@@ -270,37 +355,11 @@ __global__ void __launch_bounds__(MC_THREADS, 1) mc_kernel(const McArgs a) {
             }
             continue;
         }
-        // Tmax = max t over the frame
-        double tm = -INFINITY;
-        for (int h = tid; h < H; h += MC_THREADS) tm = fmax(tm, (double)(a.p.future_ds[base + h] - ms.start) / ms.t_scale);
-#pragma unroll
-        for (int o = 16; o >= 1; o >>= 1) tm = fmax(tm, __shfl_xor_sync(0xffffffffu, tm, o));
-        if (lane == 0) red_t[warp] = tm;
-        if (warp == 0) {
-            const uint64_t key = model_key(a, model, lane);
-            if (lane == 0) key_sm = key;
-        }
-        __syncthreads();
-        tm = red_t[0];
-        for (int w = 1; w < MC_THREADS / 32; ++w) tm = fmax(tm, red_t[w]);
-        const double rate = (double)ms.S;
         Philox ph;
-        ph.k0 = (uint32_t)key_sm;
-        ph.k1 = (uint32_t)(key_sm >> 32);
         DrawState d[2];
         bool live[2];
-#pragma unroll
-        for (int q = 0; q < 2; ++q) {
-            const uint32_t draw = tid + q * MC_THREADS;
-            live[q] = (int)draw < a.n_samples;
-            d[q].k = ms.k; d[q].m = ms.m; d[q].s_hist = 0; d[q].cp_ctr = 0; d[q].next_cp = INFINITY;
-            if (live[q] && tm > 1.0) {
-                uint32_t r[4];
-                ph.gen(draw, 0xffffffffu, 1u, 0u, r);
-                d[q].next_cp = 1.0 - log(u01(r[0], r[1])) / rate;
-            }
-        }
-        const double nscale = ms.sigma * ms.y_scale;
+        start_draws(a, ms, model, tid, red_t, &key_sm, ph, d, live);
+        const double rate = (double)ms.S, nscale = ms.sigma * ms.y_scale;
         for (int h0 = 0; h0 < H; h0 += TILE) {
             const int np = min(TILE, H - h0);
             if (tid < np) {
@@ -320,24 +379,13 @@ __global__ void __launch_bounds__(MC_THREADS, 1) mc_kernel(const McArgs a) {
                     continue;
                 }
                 for (int p = 0; p < np; p += 2) {
-                    uint32_t r[4];
-                    ph.gen(draw, (uint32_t)((h0 + p) >> 1), 0u, 0u, r);
-                    // Box-Muller: two normals per Philox call
-                    const double rad = sqrt(-2.0 * log(u01(r[0], r[1])));
-                    double sn, cs;
-                    sincospi(2.0 * u01(r[2], r[3]), &sn, &cs);
-                    const double z[2] = {rad * cs, rad * sn};
+                    double z[2];
+                    noise_pair(ph, draw, (uint32_t)((h0 + p) >> 1), z);
 #pragma unroll
                     for (int e = 0; e < 2; ++e) {
                         if (p + e >= np) break;
-                        const double t = tt[p + e];
-                        advance<LOGI>(d[q], ms, t, ph, draw, rate);
                         double tr;
-                        if (LOGI) tr = ms.cap_s / (1.0 + exp(-d[q].k * (t - d[q].m)));
-                        else tr = d[q].k * t + d[q].m;
-                        tr = tr * ms.y_scale + ms.floor;
-                        const double sd = seas[p + e];
-                        const double yh = (a.p.mult ? tr * (1.0 + sd) : tr + sd * ms.y_scale) + nscale * z[e];
+                        const double yh = draw_point<LOGI>(d[q], ms, tt[p + e], seas[p + e], z[e], ph, draw, rate, nscale, a.p.mult, tr);
                         rows[(p + e) * MC_NP + draw] = yh;
                         if (TREND) rows[(TILE + p + e) * MC_NP + draw] = tr;
                     }
@@ -347,29 +395,8 @@ __global__ void __launch_bounds__(MC_THREADS, 1) mc_kernel(const McArgs a) {
             // ---- percentiles: warp w selects the order statistics of row w (point pt of the tile) ----
             const int pt = TREND ? (warp & (TILE - 1)) : warp;
             if (pt < np) {
-                double* row = rows + warp * MC_NP;
                 double lo_v, hi_v;
-                if (!select_quantiles<TREND>(row, a.n_samples, a.lo_i, a.lo_f, a.hi_i, a.hi_f, hist + warp * 256,
-                                      cand + warp * MC_CAND, cnt + warp, lane, lo_v, hi_v)) {
-                    // fallback (a histogram bin too crowded): full bitonic sort of the row
-                    for (int k = 2; k <= MC_NP; k <<= 1) {
-                        for (int j = k >> 1; j > 0; j >>= 1) {
-                            for (int e = lane; e < MC_NP / 2; e += 32) {
-                                const int i = ((e & ~(j - 1)) << 1) | (e & (j - 1));
-                                const int l = i | j;
-                                const bool up = (i & k) == 0;
-                                const double x = row[i], y = row[l];
-                                const bool sw = up ? (x > y) : (x < y);
-                                if (sw) { row[i] = y; row[l] = x; }
-                            }
-                            __syncwarp();
-                        }
-                    }
-                    const double l0 = row[a.lo_i], l1 = row[min(a.lo_i + 1, a.n_samples - 1)];
-                    const double u0 = row[a.hi_i], u1 = row[min(a.hi_i + 1, a.n_samples - 1)];
-                    lo_v = l0 + (l1 - l0) * a.lo_f;
-                    hi_v = u0 + (u1 - u0) * a.hi_f;
-                }
+                row_quantiles<TREND>(rows + warp * MC_NP, a, hist + warp * 256, cand + warp * MC_CAND, cnt + warp, lane, lo_v, hi_v);
                 if (lane == 0) {
                     if (!TREND || warp < TILE) {
                         a.lower[base + h0 + pt] = lo_v;
@@ -385,6 +412,143 @@ __global__ void __launch_bounds__(MC_THREADS, 1) mc_kernel(const McArgs a) {
     }
 }
 
+// ---- window sums (DESIGN §13): fbprophet's predictive_samples summed per window, percentiles over the sums ----
+struct McSumArgs {
+    McArgs mc;                    // lower / upper: the window bounds [n_models * wmax]; tlower / tupper unused
+    long long width_ns, origin_ns;
+    int wmax;
+    int* n_windows;               // [n_models]
+    long long* win_start;         // [n_models * wmax] from here on
+    int* win_points;
+    double* yhat_sum;
+    long long* quantity_sum;
+};
+
+constexpr int MC_SUM_TILE = 512;  // points whose t, seasonal term, window and predict outputs are staged at once (even: noise pairs)
+
+// mathematical floor((ds - origin) / width), width > 0
+__device__ __forceinline__ long long window_of(const long long ds, const long long origin, const long long width) {
+    const long long a = ds - origin;
+    const long long q = a / width;
+    return (a % width != 0 && a < 0) ? q - 1 : q;
+}
+
+// The draws of mc_kernel (same key, counters, Tmax, trend state: the same numbers), but instead of selecting per point each
+// thread keeps the running sum of its two draws over the points of the current window -- plain fp64 adds in frame order --
+// and stores them into row (window mod 16) of the staging area when the window index of the next point differs.  After 16
+// closed windows, and at the frame's end, warp r selects the percentiles of row r.  Thread 0 sums yhat / yhat_int of
+// predict_kernel's output over the same windows, in the same order.  Windows at or past wmax are counted and not written.
+template <bool LOGI>
+__global__ void __launch_bounds__(MC_THREADS, 1) mc_sum_kernel(const McSumArgs a) {
+    extern __shared__ __align__(16) unsigned char mc_smem[];
+    double* rows = (double*)mc_smem;                       // [MC_TILE][MC_NP], as mc_kernel
+    double* cand = rows + MC_TILE * MC_NP;
+    int* hist = (int*)(cand + (MC_THREADS / 32) * MC_CAND);
+    int* cnt = hist + (MC_THREADS / 32) * 256;
+    __shared__ ModelSm ms;
+    __shared__ double seas[MC_SUM_TILE], tt[MC_SUM_TILE], yh_t[MC_SUM_TILE];
+    __shared__ long long win[MC_SUM_TILE];
+    __shared__ int yi_t[MC_SUM_TILE];
+    __shared__ double red_t[MC_THREADS / 32];
+    __shared__ uint64_t key_sm;
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const McArgs& mc = a.mc;
+    const int H = mc.p.horizon;
+    for (int model = blockIdx.x; model < mc.p.n_models; model += gridDim.x) {
+        __syncthreads();
+        load_model(ms, mc.p, model, tid, MC_THREADS);
+        const size_t base = (size_t)model * H, wbase = (size_t)model * a.wmax;
+        int nw = 0;                                        // closed windows (the same in every thread)
+        if (ms.status >= 0) {
+            Philox ph;
+            DrawState d[2];
+            bool live[2];
+            start_draws(mc, ms, model, tid, red_t, &key_sm, ph, d, live);
+            const double rate = (double)ms.S, nscale = ms.sigma * ms.y_scale;
+            double s[2] = {0.0, 0.0}, ys = 0.0;            // ys, qs: thread 0's sums of the point forecast
+            long long qs = 0, cur_w = 0;
+            int pts = 0;                                   // points of the open window (0: none open)
+            // rows [0, n) hold the draws' sums of windows [nw - n, nw): warp r selects row r
+            auto select_rows = [&](const int n) {
+                __syncthreads();
+                const int wi = nw - n + warp;
+                if (warp < n && wi < a.wmax) {
+                    double lo_v, hi_v;
+                    row_quantiles<false>(rows + warp * MC_NP, mc, hist + warp * 256, cand + warp * MC_CAND, cnt + warp, lane,
+                                         lo_v, hi_v);
+                    if (lane == 0) { mc.lower[wbase + wi] = lo_v; mc.upper[wbase + wi] = hi_v; }
+                }
+                __syncthreads();
+            };
+            auto close_window = [&]() {
+                const int r = nw & (MC_TILE - 1);
+#pragma unroll
+                for (int q = 0; q < 2; ++q) {
+                    rows[r * MC_NP + tid + q * MC_THREADS] = live[q] ? s[q] : INFINITY;
+                    s[q] = 0.0;
+                }
+                if (tid == 0 && nw < a.wmax) {
+                    a.win_start[wbase + nw] = a.origin_ns + cur_w * a.width_ns;
+                    a.win_points[wbase + nw] = pts;
+                    a.yhat_sum[wbase + nw] = ys;
+                    a.quantity_sum[wbase + nw] = qs;
+                }
+                ys = 0.0; qs = 0; pts = 0;
+                if ((++nw & (MC_TILE - 1)) == 0) select_rows(MC_TILE);
+            };
+            for (int h0 = 0; h0 < H; h0 += MC_SUM_TILE) {
+                const int np = min(MC_SUM_TILE, H - h0);
+                __syncthreads();                           // the previous tile has been walked
+                if (tid < np) {
+                    const long long dsv = mc.p.future_ds[base + h0 + tid];
+                    tt[tid] = (double)(dsv - ms.start) / ms.t_scale;
+                    seas[tid] = ms.K > 0 ? seasonal_term(ms, dsv) : 0.0;
+                    win[tid] = window_of(dsv, a.origin_ns, a.width_ns);
+                    yh_t[tid] = mc.p.yhat[base + h0 + tid];
+                    yi_t[tid] = mc.p.yhat_int[base + h0 + tid];
+                }
+                __syncthreads();
+                for (int p = 0; p < np; p += 2) {
+                    double z[2][2];
+#pragma unroll
+                    for (int q = 0; q < 2; ++q)
+                        if (live[q]) noise_pair(ph, tid + q * MC_THREADS, (uint32_t)((h0 + p) >> 1), z[q]);
+#pragma unroll
+                    for (int e = 0; e < 2; ++e) {
+                        if (p + e >= np) break;
+                        const long long wv = win[p + e];
+                        if (pts > 0 && wv != cur_w) close_window();
+                        cur_w = wv;
+                        ++pts;
+#pragma unroll
+                        for (int q = 0; q < 2; ++q) {
+                            if (!live[q]) continue;
+                            double tr;
+                            const double yh = draw_point<LOGI>(d[q], ms, tt[p + e], seas[p + e], z[q][e], ph,
+                                                               tid + q * MC_THREADS, rate, nscale, mc.p.mult, tr);
+                            s[q] = __dadd_rn(s[q], yh);    // never contracted into the draw's last multiply-add
+                        }
+                        if (tid == 0) { ys = __dadd_rn(ys, yh_t[p + e]); qs += yi_t[p + e]; }
+                    }
+                }
+            }
+            if (pts > 0) close_window();
+            if (nw & (MC_TILE - 1)) select_rows(nw & (MC_TILE - 1));
+        }
+        if (tid == 0) a.n_windows[model] = nw;
+        for (int w = min(nw, a.wmax) + tid; w < a.wmax; w += MC_THREADS) {
+            a.win_start[wbase + w] = INT64_MIN;
+            a.win_points[wbase + w] = 0;
+            a.yhat_sum[wbase + w] = NAN;
+            a.quantity_sum[wbase + w] = INT64_MIN;
+            mc.lower[wbase + w] = NAN;
+            mc.upper[wbase + w] = NAN;
+        }
+    }
+}
+
+constexpr size_t MC_SMEM = (size_t)MC_TILE * MC_NP * 8 + (size_t)(MC_THREADS / 32) * (MC_CAND * 8 + 256 * 4 + 4) + 16;
+
 template <bool LOGI, bool TREND>
 cudaError_t launch_mc_inst(cudaStream_t st, int grid, size_t smem, const McArgs& a) {
     const cudaError_t e = cudaFuncSetAttribute(mc_kernel<LOGI, TREND>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
@@ -393,11 +557,18 @@ cudaError_t launch_mc_inst(cudaStream_t st, int grid, size_t smem, const McArgs&
     return cudaGetLastError();
 }
 
-// returns 0 ok, -1 sample count or interval width out of range, 1 CUDA error.  tlower / tupper: trend bounds, or both null
-inline int launch_mc(cudaStream_t st, int sms, const PredictArgs& p, int n_samples, double width, uint64_t seed,
-                     double* lower, double* upper, double* tlower = nullptr, double* tupper = nullptr) {
-    if (n_samples < 2 || n_samples > MC_NP || !(width >= 0.0 && width <= 1.0)) return -1;
-    McArgs a;
+template <bool LOGI>
+cudaError_t launch_mc_sum_inst(cudaStream_t st, int grid, const McSumArgs& a) {
+    const cudaError_t e = cudaFuncSetAttribute(mc_sum_kernel<LOGI>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)MC_SMEM);
+    if (e != cudaSuccess) return e;
+    mc_sum_kernel<LOGI><<<grid, MC_THREADS, MC_SMEM, st>>>(a);
+    return cudaGetLastError();
+}
+
+// the sample count, the ranks of the two percentiles among the sorted draws, the seed.  False: sample count or interval
+// width out of range
+inline bool mc_args(McArgs& a, const PredictArgs& p, int n_samples, double width, uint64_t seed) {
+    if (n_samples < 2 || n_samples > MC_NP || !(width >= 0.0 && width <= 1.0)) return false;
     a.p = p;
     a.n_samples = n_samples;
     const double lower_p = 100.0 * (1.0 - width) / 2.0, upper_p = 100.0 * (1.0 + width) / 2.0;
@@ -405,16 +576,38 @@ inline int launch_mc(cudaStream_t st, int sms, const PredictArgs& p, int n_sampl
     a.lo_i = (int)floor(li); a.lo_f = li - floor(li);
     a.hi_i = (int)floor(ui); a.hi_f = ui - floor(ui);
     a.seed = seed;
+    a.lower = a.upper = a.tlower = a.tupper = nullptr;
+    return true;
+}
+
+// returns 0 ok, -1 sample count or interval width out of range, 1 CUDA error.  tlower / tupper: trend bounds, or both null
+inline int launch_mc(cudaStream_t st, int sms, const PredictArgs& p, int n_samples, double width, uint64_t seed,
+                     double* lower, double* upper, double* tlower = nullptr, double* tupper = nullptr) {
+    McArgs a;
+    if (!mc_args(a, p, n_samples, width, seed)) return -1;
     a.lower = lower;
     a.upper = upper;
     a.tlower = tlower;
     a.tupper = tupper;
     const bool trend = tlower && tupper;
-    const size_t smem = (size_t)MC_TILE * MC_NP * 8 + (size_t)(MC_THREADS / 32) * (MC_CAND * 8 + 256 * 4 + 4) + 16;
     const int grid = p.n_models < sms ? p.n_models : sms;
     const bool logi = p.growth == PB200_GROWTH_LOGISTIC;
-    const cudaError_t e = logi ? (trend ? launch_mc_inst<true, true>(st, grid, smem, a) : launch_mc_inst<true, false>(st, grid, smem, a))
-                               : (trend ? launch_mc_inst<false, true>(st, grid, smem, a) : launch_mc_inst<false, false>(st, grid, smem, a));
+    const cudaError_t e = logi ? (trend ? launch_mc_inst<true, true>(st, grid, MC_SMEM, a) : launch_mc_inst<true, false>(st, grid, MC_SMEM, a))
+                               : (trend ? launch_mc_inst<false, true>(st, grid, MC_SMEM, a) : launch_mc_inst<false, false>(st, grid, MC_SMEM, a));
+    return e == cudaSuccess ? 0 : 1;
+}
+
+// mc_sum_kernel over the frame of p, whose yhat / yhat_int predict_kernel has written on the same stream; s.mc is filled
+// here but for its lower / upper (the window bounds).  Returns as launch_mc
+inline int launch_mc_sum(cudaStream_t st, int sms, const PredictArgs& p, int n_samples, double width, uint64_t seed,
+                         McSumArgs& s) {
+    double* const lo = s.mc.lower;
+    double* const hi = s.mc.upper;
+    if (!mc_args(s.mc, p, n_samples, width, seed)) return -1;
+    s.mc.lower = lo;
+    s.mc.upper = hi;
+    const int grid = p.n_models < sms ? p.n_models : sms;
+    const cudaError_t e = p.growth == PB200_GROWTH_LOGISTIC ? launch_mc_sum_inst<true>(st, grid, s) : launch_mc_sum_inst<false>(st, grid, s);
     return e == cudaSuccess ? 0 : 1;
 }
 

@@ -13,7 +13,9 @@ computes yhat_lower/yhat_upper inside Prophet.predict and drops them at :86; set
 ``yhat_lower``/``yhat_upper`` columns), ``forecast.uncertainty_samples`` (1000),
 ``forecast.interval_width`` (0.8), ``forecast.seed``, ``forecast.components`` (default false; true adds fbprophet's
 component columns ``trend, yearly, weekly, daily, multiplicative_terms, additive_terms``, and ``trend_lower`` /
-``trend_upper`` with intervals -- DESIGN §12).
+``trend_upper`` with intervals -- DESIGN §12), ``forecast.aggregate`` (a fixed-width duration such as ``'1D'``: also
+write, to ``io.aggregates``, the forecast total of every such window of every model with the interval of the total from
+the joint draws -- DESIGN §13) and ``forecast.aggregate_origin`` (where window 0 starts, default 1970-01-01).
 """
 from __future__ import annotations
 
@@ -74,6 +76,62 @@ def component_columns(res: "batched.ForecastBatch", mask: np.ndarray, periods: i
     return cols
 
 
+AGGREGATE_SCHEMA = pa.schema([
+    pa.field("series_id", pa.int32()), pa.field("dim_id", pa.int32()), pa.field("window_start", pa.timestamp("ns")),
+    pa.field("window_points", pa.int32()), pa.field("forecast_quantity", pa.int64()), pa.field("yhat", pa.float64()),
+    pa.field("yhat_lower", pa.float64()), pa.field("yhat_upper", pa.float64()),
+])
+
+
+def aggregate_rule(config):
+    """``forecast.aggregate`` / ``forecast.aggregate_origin`` as (width_ns, origin_ns), or None without the key.  The
+    width is a fixed-width pandas duration ('1D', '7D', '8h'); calendar offsets ('M') have no fixed width and are refused."""
+    import pandas as pd
+    fc = config.get("forecast", {}) or {}
+    if fc.get("aggregate") is None:
+        return None
+    spec = fc["aggregate"]
+    try:
+        off = _to_offset(spec)
+        width = int(7 * 86400 * 10**9 * off.n if isinstance(off, pd.offsets.Week) and off.weekday is None else off.nanos)
+    except Exception:
+        raise ValueError(f"forecast.aggregate must be a fixed-width duration such as '1D', '7D' or '8h' (got {spec!r}; "
+                         "calendar offsets such as 'M' have no fixed width)") from None
+    if width <= 0:
+        raise ValueError(f"forecast.aggregate must be a positive duration (got {spec!r})")
+    try:
+        origin = pd.Timestamp(fc.get("aggregate_origin", "1970-01-01"))
+        if origin is pd.NaT:
+            raise ValueError("NaT")
+        if origin.tzinfo is not None:
+            origin = origin.tz_convert("UTC").tz_localize(None)
+        origin_ns = int(origin.value)
+    except Exception:
+        raise ValueError(f"forecast.aggregate_origin must be a timestamp (got {fc.get('aggregate_origin')!r})") from None
+    if not (config.get("io", {}) or {}).get("aggregates"):
+        raise ValueError("forecast.aggregate needs io.aggregates, the directory the window totals are written to")
+    if _want_components(fc):
+        raise ValueError("forecast.aggregate cannot be combined with forecast.components")
+    return width, origin_ns
+
+
+def aggregate_table(sid, did, ok, ws: "batched.WindowSums") -> pa.Table:
+    """One row per (model, window) of the models that have a forecast, from a shard's WindowSums."""
+    wmax = ws.start.shape[1]
+    keep = (np.arange(wmax)[None, :] < ws.n_windows[:, None]) & ok[:, None]
+    rows = np.nonzero(keep)[0]
+    return pa.table({
+        "series_id": pa.array(sid[rows], pa.int32()),
+        "dim_id": pa.array(did[rows], pa.int32()),
+        "window_start": pa.array(ws.start[keep], pa.int64()).cast(pa.timestamp("ns")),
+        "window_points": pa.array(ws.points[keep], pa.int32()),
+        "forecast_quantity": pa.array(ws.quantity_sum[keep], pa.int64()),
+        "yhat": pa.array(ws.yhat_sum[keep], pa.float64()),
+        "yhat_lower": pa.array(ws.lower[keep], pa.float64()),
+        "yhat_upper": pa.array(ws.upper[keep], pa.float64()),
+    })
+
+
 # pandas 0.25 (the reference's pin) offset aliases that later pandas renamed
 _LEGACY_ALIASES = {"H": "h", "T": "min", "S": "s", "L": "ms", "U": "us", "N": "ns", "M": "ME", "BM": "BME",
                    "Q": "QE", "BQ": "BQE", "A": "YE", "Y": "YE", "BA": "BYE", "BY": "BYE", "AS": "YS", "BAS": "BYS"}
@@ -129,13 +187,16 @@ class _ForecastTimeSeriesOp:
 
     def __init__(self, config):
         self.config = config
+        self.aggregates = None      # with forecast.aggregate: the window totals of the last apply_batched (this rank's models)
 
     def apply_batched(self, table: pa.Table, keys) -> pa.Table:
         if list(keys) != ["series_id", "dim_id"]:
             raise ValueError("forecast_time_series groups by ('series_id', 'dim_id')")
         fc = self.config["forecast"]
         want_intervals = bool(fc.get("intervals", False))
-        if want_intervals:
+        rule = aggregate_rule(self.config)
+        self.aggregates = AGGREGATE_SCHEMA.empty_table() if rule else None
+        if want_intervals or rule:
             width = float(fc.get("interval_width", 0.8))
             if not 0.0 <= width <= 1.0:     # fbprophet refuses it too (numpy's percentile range check); NaN fails here
                 raise ValueError(f"forecast.interval_width must be in [0, 1] (got {fc.get('interval_width')!r})")
@@ -168,7 +229,7 @@ class _ForecastTimeSeriesOp:
                                     seasonality_mode="multiplicative" if info["multiplicative"] else "additive",
                                     n_changepoints=info["n_changepoints"],
                                     interval_width=fc.get("interval_width", 0.8),
-                                    uncertainty_samples=fc.get("uncertainty_samples", 1000) if want_intervals else 0)
+                                    uncertainty_samples=fc.get("uncertainty_samples", 1000) if want_intervals or rule else 0)
         opts.yearly, opts.weekly, opts.daily = info["yearly"], info["weekly"], info["daily"]
         # reference :46-47: floor / cap are read back from the FLOAT32 columns of the models table
         floor = table["floor"].combine_chunks().to_numpy(zero_copy_only=False).astype(np.float64)
@@ -176,11 +237,16 @@ class _ForecastTimeSeriesOp:
         periods = int(fc["periods"])
         future = frequency_to_future(last_ds, periods, fc["frequency"])
         ctx = get_context()
-        res = batched.predict_batch_host(ctx, opts, fitted, future, floor, cap, seed=int(fc.get("seed", 0)),
-                                         intervals=want_intervals, components=want_components)
         sid = table["series_id"].combine_chunks().to_numpy(zero_copy_only=False).astype(np.int32)
         did = table["dim_id"].combine_chunks().to_numpy(zero_copy_only=False).astype(np.int32)
         ok = fitted.meta_i32[:, 4] >= 0
+        if rule:
+            res, sums = batched.predict_sums_host(ctx, opts, fitted, future, floor, cap, rule[0], rule[1],
+                                                  seed=int(fc.get("seed", 0)), intervals=want_intervals)
+            self.aggregates = aggregate_table(sid, did, ok, sums)
+        else:
+            res = batched.predict_batch_host(ctx, opts, fitted, future, floor, cap, seed=int(fc.get("seed", 0)),
+                                             intervals=want_intervals, components=want_components)
         # "Negative forecast values found" log line (reference :76-79)
         neg = np.flatnonzero(ok & (np.trunc(res.yhat).min(axis=1) < floor))
         for i in neg[:100]:
@@ -393,12 +459,31 @@ class ProphetScorer:
         with ThreadPoolExecutor(max_workers=max(1, pdist.size_host_pools())) as pool:
             list(pool.map(write, range(len(bounds) - 1)))
 
+    def write_aggregates(self, aggregates: pa.Table, created_timestamp: str):
+        """The window totals of forecast.aggregate as CSV with header under io.aggregates: one part file per rank,
+        ``created_timestamp, series_id, dim_id, window_start, window_points, forecast_quantity, yhat, yhat_lower,
+        yhat_upper``; window_start printed like forecast_timestamp."""
+        out = self.config["io"]["aggregates"]
+        rank = pdist.world()[0]
+        pdist.prepare_output_dir(out)
+        t = aggregates
+        ms = pc.cast(t["window_start"], pa.timestamp("ms"), safe=False)
+        t = t.set_column(t.column_names.index("window_start"), "window_start",
+                         _strftime_via_dictionary(ms, "%Y-%m-%dT%H:%M:%SZ"))
+        t = t.add_column(0, "created_timestamp", pa.array([created_timestamp] * t.num_rows, pa.string()))
+        pacsv.write_csv(t, os.path.join(out, f"part-{rank:05d}.csv"),
+                        write_options=pacsv.WriteOptions(include_header=True, quoting_style="needed"))
+
     @staticmethod
     def score(spark_session, config):
+        aggregate_rule(config)              # a bad forecast.aggregate fails before anything is read
         pdist.init_process_group()          # no-op unless launched by torchrun with WORLD_SIZE > 1
         scorer = ProphetScorer(config)
         model_df = scorer.read_model_dataframe(spark_session)
-        forecast_df = model_df.groupby("series_id", "dim_id").apply(forecast_time_series(scorer.config))
+        op = forecast_time_series(scorer.config)
+        forecast_df = model_df.groupby("series_id", "dim_id").apply(op)
+        if op.aggregates is not None:       # per-rank part files; forecast.gather below is for the forecast frame only
+            scorer.write_aggregates(op.aggregates, datetime.now(timezone.utc).replace(microsecond=0).isoformat())
         if config["forecast"].get("gather", False) and pdist.world()[1] > 1:
             # optional: one NCCL gather of the final forecast frame to rank 0 (the only collective on
             # the path); default is one part file per rank, like Spark's output directory
