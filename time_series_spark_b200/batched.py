@@ -613,12 +613,13 @@ def cv_plan_device(ctx: L.Context, opts: L.Options, ds_ns, offsets_host: np.ndar
     p = int(pair_off[-1])
     ps = torch.empty(p, dtype=torch.int32, device=dev)
     cut, he, we = (torch.empty(p, dtype=torch.int64, device=dev) for _ in range(3))
-    d_poff = torch.from_numpy(pair_off).to(dev)
-    torch.cuda.current_stream(dev).synchronize()
-    L.check(lib.pb200_cv_plan_device(ctx.handle, C.byref(opts), ds_ns.data_ptr(), d_off.data_ptr(), n, int(horizon_ns),
-                                     int(period_ns), int(initial_ns), d_poff.data_ptr(), err.data_ptr(), ps.data_ptr(),
-                                     cut.data_ptr(), he.data_ptr(), we.data_ptr()), "pb200_cv_plan_device")
-    ctx.synchronize()
+    if p:                  # with no cutoff anywhere there is nothing to write (and the error bits are complete)
+        d_poff = torch.from_numpy(pair_off).to(dev)
+        torch.cuda.current_stream(dev).synchronize()
+        L.check(lib.pb200_cv_plan_device(ctx.handle, C.byref(opts), ds_ns.data_ptr(), d_off.data_ptr(), n, int(horizon_ns),
+                                         int(period_ns), int(initial_ns), d_poff.data_ptr(), err.data_ptr(), ps.data_ptr(),
+                                         cut.data_ptr(), he.data_ptr(), we.data_ptr()), "pb200_cv_plan_device")
+        ctx.synchronize()
     return CvPlan(counts, mask.cpu().numpy(), err.cpu().numpy(), pair_off, ps, cut, he, we)
 
 

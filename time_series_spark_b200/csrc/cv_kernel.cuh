@@ -37,21 +37,34 @@ __device__ __forceinline__ long long upper_bound(const long long* ds, long long 
 // generate_cutoffs over the sorted rows [a, b): returns the number of cutoffs (< 0: an ERR_* flag, negated) and, when
 // out != nullptr, writes them in ascending order to out[0 .. n).  The walk produces them in descending order, so the
 // writing pass is told n (from the counting pass) and fills out from the back.
+// H, P and I may be any positive int64 (pandas Timedeltas reach ~106 751 days), so no sum or difference below is formed
+// before it is known to stay in int64: a timestamp minus a duration that would fall below INT64_MIN lies before every
+// row, and first + I beyond INT64_MAX after every cutoff.  (A wrapped last - H or prev - P would otherwise land after
+// the rows and send the walk back to the same cutoff forever.)  Every cutoff c satisfies c <= last - H, so c + H does
+// not overflow.
 __device__ __forceinline__ int cutoff_walk(const long long* ds, const long long a, const long long b, const long long H,
                                            const long long P, const long long I, long long* out, const int n_known) {
     const long long first = ds[a], last = ds[b - 1];
+    if (last < INT64_MIN + H || last - H < first) return -ERR_HORIZON;
     long long prev = last - H;
-    if (prev < first) return -ERR_HORIZON;
+    const bool can_start = first <= INT64_MAX - I;             // else first + I is after every cutoff
     int n = 0;
-    while (prev >= first + I) {
-        long long c = prev - P;
-        const long long u = upper_bound(ds, a, b, c);         // first row > c
+    while (can_start && prev >= first + I) {
+        long long c = 0;
         bool stop = false;
-        if (!(u < b && ds[u] <= c + H)) {
-            // no row in (c, c + H]: the next cutoff is (latest row <= c) - H.  With no such row fbprophet's cutoff
-            // becomes NaT, which ends the loop and is the element dropped: prev is kept
-            if (u == a) stop = true;
-            else c = ds[u - 1] - H;
+        if (prev < INT64_MIN + P) {
+            // prev - P lies before every row: whichever branch fbprophet takes, the next cutoff ends the loop
+            stop = true;
+        } else {
+            c = prev - P;
+            const long long u = upper_bound(ds, a, b, c);     // first row > c
+            if (!(u < b && ds[u] <= c + H)) {
+                // no row in (c, c + H]: the next cutoff is (latest row <= c) - H.  With no such row fbprophet's cutoff
+                // becomes NaT, which ends the loop and is the element dropped: prev is kept.  So does a next cutoff
+                // before every row
+                if (u == a || ds[u - 1] < INT64_MIN + H) stop = true;
+                else c = ds[u - 1] - H;
+            }
         }
         if (out) out[n_known - 1 - n] = prev;
         ++n;
