@@ -507,7 +507,8 @@ def _wolfe_line_search(func, alpha, p, x0, f0, g0, c1, c2, min_alpha, max_ls_its
         nits += 1
 
 
-def stan_lbfgs(fun, x0: np.ndarray, opts: ProphetOptions, trace: Optional[list] = None):
+def stan_lbfgs(fun, x0: np.ndarray, opts: ProphetOptions, trace: Optional[list] = None,
+               crit: Optional[list] = None):
     """stan::optimization::BFGSMinimizer<…, LBFGSUpdate>::initialize + step loop as
     driven by stan::services::optimize::lbfgs.  ``fun(x) -> (err, f, g)`` minimised.
 
@@ -515,6 +516,9 @@ def stan_lbfgs(fun, x0: np.ndarray, opts: ProphetOptions, trace: Optional[list] 
     RuntimeError fbprophet 0.5 answers with a Newton retry.  ``trace`` (a list) receives one
     ``(iteration, f_k, alpha_k, n_evals)`` tuple per accepted iteration -- the record the GPU
     kernel's trajectory hook (pb200_fit_trace_host) writes, compared in tests/test_gpu_trajectory.py.
+    ``crit`` (a list) receives, per accepted iteration, what the convergence tests compare with their
+    tolerances: ``(iteration, |f_{k-1} - f_k|, max(|f_{k-1}|, |f_k|, 1), ||g_k||, |g_k . p_k|,
+    max(|f_k|, 1), ||s_k||)`` (tests/test_gpu_stop_rules.py).
     """
     func = _Counter(fun)
     c1, c2, min_alpha, max_ls_its, max_ls_restarts = 1e-4, 0.9, 1e-12, 20, 10
@@ -583,6 +587,9 @@ def stan_lbfgs(fun, x0: np.ndarray, opts: ProphetOptions, trace: Optional[list] 
             pk = pk + (alphas[j] - b) * si
         # convergence tests
         df = abs(fk_1 - fk)
+        if crit is not None:
+            crit.append((it, df, max(abs(fk_1), max(abs(fk), 1.0)), grad_norm, abs(float(gk @ pk)),
+                         max(abs(fk), 1.0), step_norm))
         if df < opts.tol_obj:
             ret = TERM_ABSF
         elif df < opts.tol_rel_obj * EPS * max(abs(fk_1), max(abs(fk), 1.0)):
@@ -697,11 +704,12 @@ def stan_newton(fun, x0: np.ndarray, opts: ProphetOptions):
 # --------------------------------------------------------------------------
 def fit(ds_ns, y, floor: float = 0.0, cap: Optional[float] = None,
         opts: Optional[ProphetOptions] = None, cap_multiplier: float = 1.1,
-        algorithm: str = "LBFGS+Newton", trace: Optional[list] = None) -> FitResult:
+        algorithm: str = "LBFGS+Newton", trace: Optional[list] = None,
+        crit: Optional[list] = None) -> FitResult:
     """model_time_series_udf body (prophet_modeler.py:56-66): cap = max(y)*cap_multiplier,
     then Prophet(...).fit.  ``algorithm``: "LBFGS+Newton" is fbprophet 0.5's fit() -- L-BFGS, and on
     PyStan's RuntimeError (line-search failure) a Newton run from the same initial point; "LBFGS" /
-    "Newton" run one of them alone (tests)."""
+    "Newton" run one of them alone (tests).  ``trace`` / ``crit``: stan_lbfgs's records."""
     opts = opts or ProphetOptions()
     ds_ns = np.asarray(ds_ns, dtype=np.int64)
     y = np.asarray(y, dtype=np.float64)
@@ -717,7 +725,7 @@ def fit(ds_ns, y, floor: float = 0.0, cap: Optional[float] = None,
         if algorithm == "Newton":
             th, f, it, ret, ne = stan_newton(fun, th0, opts)
         else:
-            th, f, it, ret, ne = stan_lbfgs(fun, th0, opts, trace=trace)
+            th, f, it, ret, ne = stan_lbfgs(fun, th0, opts, trace=trace, crit=crit)
             if ret == TERM_LSFAIL and algorithm == "LBFGS+Newton":
                 th, f, it2, ret, ne2 = stan_newton(fun, th0, opts)
                 it, ne = it + it2, ne + ne2

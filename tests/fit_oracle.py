@@ -1,6 +1,7 @@
 """Helpers the GPU fit tests share: contexts built under the environment switches pb200_create reads, start points near
 the oracle's initial one, the oracle's per-iteration record, the trajectory comparison, and a host mirror of the grouped
 kernel's chunk rule.  TEST INFRASTRUCTURE ONLY."""
+import dataclasses
 import os
 
 import numpy as np
@@ -144,3 +145,66 @@ def assert_newton_row(fb, i, fr, c_theta, c_f, c_info, measured, what):
     measured["theta"] = max(measured.get("theta", 0.0), dt / bt)
     assert df <= bf, (what, fb.meta_f64[i, 3], fr.neg_logp, c_f)
     assert dt <= bt, (what, dt, bt, np.abs(record_theta(fb, i) - th_np))
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# Stan's L-BFGS stop rules bracketed through the status alone (tests/test_stop_rules_oracle.py,
+# tests/test_gpu_stop_rules.py): run with max_iter = j, every other tolerance 0 and one rule's tolerance just above (just
+# below) the oracle's value at iteration j, a fit must end with that rule's status (with MAXIT) at iteration j
+# ---------------------------------------------------------------------------------------------------------------------
+EPS = 2.220446049250313e-16
+RULES = ("ABSF", "RELF", "ABSGRAD", "RELGRAD", "ABSX")            # the order BFGSMinimizer::step tests them in
+RULE_TOL = dict(zip(RULES, ("tol_obj", "tol_rel_obj", "tol_grad", "tol_rel_grad", "tol_param")))
+RULE_STATUS = dict(zip(RULES, (po.TERM_ABSF, po.TERM_RELF, po.TERM_ABSGRAD, po.TERM_RELGRAD, po.TERM_ABSX)))
+ZERO_TOLS = {t: 0.0 for t in RULE_TOL.values()}
+RECORD_MARGIN = 1.01          # a target's earlier values are all at least 1 % above its own
+
+
+class StopRun:
+    """The oracle's L-BFGS run with every tolerance 0: its trace rows ``(iteration, f_k, alpha_k, n_evals)``, the fit,
+    and per rule the value each accepted iteration compares with the rule's tolerance."""
+
+    def __init__(self, ds, y, oopts, max_iter=12, history=5, init=None):
+        import warm_oracle as wo
+        o = dataclasses.replace(oopts, max_iter=max_iter, history_size=history, **ZERO_TOLS)
+        rows, crit = [], []
+        self.fr = wo.fit(ds, np.asarray(y, np.float64), opts=o, algorithm="LBFGS", trace=rows, crit=crit, init=init)
+        self.rows = np.array(rows).reshape(-1, 4)
+        self.crit = np.array(crit).reshape(-1, 7)
+        c = self.crit
+        self.values = {"ABSF": c[:, 1], "RELF": c[:, 1] / (EPS * c[:, 2]), "ABSGRAD": c[:, 3],
+                       "RELGRAD": c[:, 4] / (EPS * c[:, 5]), "ABSX": c[:, 6]}
+        self.history = history
+
+    def f(self, j):
+        """f_j; f_0 is the start point's objective (each accepted step lowers f, so f_{j-1} = f_j + df_j)."""
+        return self.rows[j - 1, 1] if j >= 1 else self.rows[0, 1] + self.crit[0, 1]
+
+    def record_lows(self, rule):
+        """The iterations j whose value of ``rule`` every earlier one exceeds by RECORD_MARGIN."""
+        v = self.values[rule]
+        return [j for j in range(1, v.size + 1) if np.isfinite(v[j - 1]) and v[j - 1] > 0
+                and np.all(v[:j - 1] >= RECORD_MARGIN * v[j - 1])]
+
+    def targets(self, rule):
+        """Iteration 1 (the reset path), 2 when it is a record low, and the last record low past the history size (the
+        ring buffer has wrapped)."""
+        lows = self.record_lows(rule)
+        out = [j for j in lows if j <= 2]
+        past = [j for j in lows if j > self.history]
+        return out + past[-1:]
+
+    def delta(self, rule, j):
+        """The bracket's half width: 1e-6, and for the rules on df, 1e-9 |f_j| / df_j (df is the difference of two
+        values each exact to about 1e-11 relative)."""
+        if rule in ("ABSF", "RELF"):
+            return max(1e-6, 1e-9 * abs(self.rows[j - 1, 1]) / self.crit[j - 1, 1])
+        return 1e-6
+
+    def bracket(self, rule, j, side, delta):
+        """(tolerances, expected (status, iters, n_evals)) of the run with max_iter j and ``rule``'s tolerance at
+        v_j (1 + side delta)."""
+        tols = dict(ZERO_TOLS)
+        tols[RULE_TOL[rule]] = float(self.values[rule][j - 1] * (1.0 + side * delta))
+        want = (RULE_STATUS[rule] if side > 0 else po.TERM_MAXIT, j, int(self.rows[j - 1, 3]))
+        return tols, want

@@ -17,10 +17,10 @@ from oracle import prophet_oracle as po
 
 def fit(ds_ns, y, floor: float = 0.0, cap: Optional[float] = None, opts: Optional[po.ProphetOptions] = None,
         cap_multiplier: float = 1.1, algorithm: str = "LBFGS+Newton", trace: Optional[list] = None,
-        init: Optional[np.ndarray] = None) -> po.FitResult:
+        init: Optional[np.ndarray] = None, crit: Optional[list] = None) -> po.FitResult:
     """``po.fit`` started from ``init`` (Stan's unconstrained order k, m, delta[S], log sigma_obs, beta[K]) when given."""
     if init is None:
-        return po.fit(ds_ns, y, floor, cap, opts, cap_multiplier, algorithm, trace)
+        return po.fit(ds_ns, y, floor, cap, opts, cap_multiplier, algorithm, trace, crit)
     opts = opts or po.ProphetOptions()
     ds_ns = np.asarray(ds_ns, dtype=np.int64)
     y = np.asarray(y, dtype=np.float64)
@@ -38,7 +38,7 @@ def fit(ds_ns, y, floor: float = 0.0, cap: Optional[float] = None, opts: Optiona
         if algorithm == "Newton":
             th, f, it, ret, ne = po.stan_newton(fun, x0, opts)
         else:
-            th, f, it, ret, ne = po.stan_lbfgs(fun, x0, opts, trace=trace)
+            th, f, it, ret, ne = po.stan_lbfgs(fun, x0, opts, trace=trace, crit=crit)
             if ret == po.TERM_LSFAIL and algorithm == "LBFGS+Newton":
                 th, f, it2, ret, ne2 = po.stan_newton(fun, x0, opts)
                 it, ne = it + it2, ne + ne2
