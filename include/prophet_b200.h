@@ -381,6 +381,26 @@ PB200_API int pb200_predict_sums_host(pb200_ctx* ctx, const pb200_options* opts,
                        int32_t* h_n_windows, int64_t* h_win_start, int32_t* h_win_points,
                        double* h_yhat_sum, int64_t* h_quantity_sum, double* h_sum_lower, double* h_sum_upper);
 
+/*
+ * pb200_predict_sums_device with a window origin and a frame length per model (DESIGN §14): model i's windows are
+ * floor((ds - d_origin_ns[i]) / width_ns) over its first d_frame_len[i] points; the points after them (a frame padded by
+ * repeating its last timestamp) are predicted as usual but summed into no window.  The draws are those of the whole
+ * frame, so with every origin equal to origin_ns and every length equal to horizon the outputs are
+ * pb200_predict_sums_device's, byte for byte; the pointwise outputs are always pb200_predict_device's.  win_start is
+ * d_origin_ns[i] + w * width_ns.  d_origin_ns / d_frame_len: [n_models] device arrays, both required.
+ */
+PB200_API int pb200_predict_sums_anchored_device(pb200_ctx* ctx, const pb200_options* opts,
+                         const double* d_params, const double* d_tchange,
+                         const int32_t* d_meta_i32, const int64_t* d_meta_i64,
+                         const double* d_meta_f64, int64_t n_models,
+                         const int64_t* d_future_ds, int32_t horizon,
+                         const double* d_floor, const double* d_cap, uint64_t seed,
+                         double* d_yhat, double* d_yhat_lower, double* d_yhat_upper,
+                         int32_t* d_yhat_int, int64_t width_ns, const int64_t* d_origin_ns,
+                         const int32_t* d_frame_len, int32_t wmax,
+                         int32_t* d_n_windows, int64_t* d_win_start, int32_t* d_win_points,
+                         double* d_yhat_sum, int64_t* d_quantity_sum, double* d_sum_lower, double* d_sum_upper);
+
 /* future_ds[i*horizon + j] = last_ds[i] + (j+1)*freq_ns  -- make_future_dataframe
  * (include_history=False) for a fixed-width pandas frequency. */
 PB200_API int pb200_make_future_device(pb200_ctx* ctx, const int64_t* d_last_ds, int64_t n_models,
@@ -461,6 +481,22 @@ PB200_API int pb200_cv_metrics_device(pb200_ctx* ctx, const int64_t* d_horizon, 
                                       const int64_t* d_srow_off, int64_t n_series, double rolling_window,
                                       int64_t* d_out_horizon, int64_t* d_scratch, double* d_mse, double* d_rmse,
                                       double* d_mae, double* d_mape, double* d_coverage, int32_t* d_valid);
+
+/*
+ * Backtest window totals (DESIGN §14) of n gathered entries: entry k is plan pair d_pairs[k], its held-out rows
+ * [d_hist_end[p], d_win_end[p]) of d_ds / d_y (y_dtype as pb200_cv_gather_device) and row k of d_yhat [n * hmax] (the
+ * predict frame of pb200_cv_gather_device's d_future_ds).  Window j of cutoff c is (c + j W, c + (j + 1) W], W =
+ * width_ns > 0: row r lies in j = (ds_r - c - 1) / W.  Per entry, its non-empty windows in ascending j go to slots
+ * k * wmax + i: d_win_start (c + j W), d_win_points, d_y_sum and d_yhat_sum (the rows' float64 y / yhat summed in
+ * ascending row order, plain fp64 adds); d_n_windows[k] is the count (slots at or past it hold INT64_MIN / 0 / NaN; a
+ * count above wmax writes the first wmax).  One warp per entry, no floating-point atomics: an entry's outputs depend
+ * on that entry only.
+ */
+PB200_API int pb200_cv_windows_device(pb200_ctx* ctx, const int64_t* d_ds, const void* d_y, int32_t y_dtype,
+                                      const int64_t* d_cutoff, const int64_t* d_hist_end, const int64_t* d_win_end,
+                                      const int64_t* d_pairs, int64_t n, const double* d_yhat, int32_t hmax,
+                                      int64_t width_ns, int32_t wmax, int32_t* d_n_windows, int64_t* d_win_start,
+                                      int32_t* d_win_points, double* d_y_sum, double* d_yhat_sum);
 
 #ifdef __cplusplus
 }

@@ -541,6 +541,52 @@ def predict_sums_device(ctx: L.Context, opts: L.Options, fitted: FittedBatch, fu
     return ForecastBatch(future_ds, yhat, lo, hi, yint), ws
 
 
+def predict_sums_anchored_device(ctx: L.Context, opts: L.Options, fitted: FittedBatch, future_ds, floor, cap,
+                                 width_ns: int, origins, frame_len, seed: int = 0, intervals: bool = False,
+                                 wmax: Optional[int] = None):
+    """pb200_predict_sums_anchored_device with torch CUDA tensors: predict_sums_device with a window origin per model
+    (``origins`` int64 [N]) whose windows cover only the first ``frame_len[i]`` points of row i (int32 [N]; the rest
+    of the row is padding that is predicted but summed into no window).  ``wmax`` defaults to the bound
+    ``window_slots`` gives over each model's first and last walked point."""
+    import torch
+    n = fitted.n
+    h = int(future_ds.shape[1])
+    dev = future_ds.device
+    width_ns = int(width_ns)
+    if width_ns <= 0:
+        raise ValueError(f"width_ns must be > 0 (got {width_ns})")
+    origins = origins.to(device=dev, dtype=torch.int64).contiguous()
+    frame_len = frame_len.to(device=dev, dtype=torch.int32).contiguous()
+    if wmax is None:
+        wmax = 1
+        if n and h:
+            last = future_ds.gather(1, (frame_len.long().clamp(1, h) - 1)[:, None])[:, 0]
+            w = (last - origins).div(width_ns, rounding_mode="floor") - (future_ds[:, 0] - origins).div(width_ns, rounding_mode="floor")
+            wmax = max(1, int(w.max().item()) + 1)
+    wmax = int(wmax)
+    f64 = dict(dtype=torch.float64, device=dev)
+    yhat = torch.empty((n, h), **f64)
+    yint = torch.empty((n, h), dtype=torch.int32, device=dev)
+    lo = torch.empty((n, h), **f64) if intervals else None
+    hi = torch.empty((n, h), **f64) if intervals else None
+    ws = WindowSums(torch.zeros(n, dtype=torch.int32, device=dev), torch.empty((n, wmax), dtype=torch.int64, device=dev),
+                    torch.empty((n, wmax), dtype=torch.int32, device=dev), torch.empty((n, wmax), **f64),
+                    torch.empty((n, wmax), dtype=torch.int64, device=dev), torch.empty((n, wmax), **f64),
+                    torch.empty((n, wmax), **f64))
+    torch.cuda.current_stream(dev).synchronize()
+    rc = L.load().pb200_predict_sums_anchored_device(
+        ctx.handle, C.byref(opts), fitted.params.data_ptr(), fitted.tchange.data_ptr(), fitted.meta_i32.data_ptr(),
+        fitted.meta_i64.data_ptr(), fitted.meta_f64.data_ptr(), n, future_ds.data_ptr(), h, floor.data_ptr(),
+        cap.data_ptr(), int(seed) & (2**64 - 1), yhat.data_ptr(), lo.data_ptr() if intervals else None,
+        hi.data_ptr() if intervals else None, yint.data_ptr(), width_ns, origins.data_ptr(), frame_len.data_ptr(), wmax,
+        ws.n_windows.data_ptr(), ws.start.data_ptr(), ws.points.data_ptr(), ws.yhat_sum.data_ptr(),
+        ws.quantity_sum.data_ptr(), ws.lower.data_ptr(), ws.upper.data_ptr())
+    L.check(rc, "pb200_predict_sums_anchored_device")
+    ctx.synchronize()
+    _check_window_slots(wmax, int(ws.n_windows.max().item()) if n else 0)
+    return ForecastBatch(future_ds, yhat, lo, hi, yint), ws
+
+
 def objective_host(ctx: L.Context, opts: L.Options, ds_ns: np.ndarray, y: np.ndarray, offsets: np.ndarray,
                    floor: float, cap_multiplier: float, theta: np.ndarray):
     """pb200_objective_host (parity-test hook): objective and gradient at ``theta`` rows
@@ -668,6 +714,60 @@ class CvResult:
     yhat_upper: Optional[np.ndarray]
     metrics: Optional[dict] = None
     fitted: Optional[FittedBatch] = None
+    windows: Optional["CvWindows"] = None
+
+
+@dataclass
+class CvWindows:
+    """Window rows of cross_validation_device(aggregate_ns=W) (DESIGN §14), host numpy, ordered by (series, cutoff,
+    window).  Window j of cutoff c is (c + j W, c + (j + 1) W]; only windows holding a held-out row have a row.
+    ``series`` (as CvResult.row_series), ``cutoff``, ``horizon`` ((j + 1) W, ns), ``points`` (held-out rows in the
+    window), ``y`` / ``yhat`` (their float64 y / yhat summed in row order) and, with intervals, ``yhat_lower`` /
+    ``yhat_upper`` (percentiles over the joint draws' window sums).  ``metrics`` (with ``rolling_window``):
+    performance_metrics over the window rows with ``horizon`` as the horizon, keyed as CvResult.metrics."""
+    width_ns: int
+    series: np.ndarray
+    cutoff: np.ndarray
+    horizon: np.ndarray
+    points: np.ndarray
+    y: np.ndarray
+    yhat: np.ndarray
+    yhat_lower: Optional[np.ndarray]
+    yhat_upper: Optional[np.ndarray]
+    metrics: Optional[dict] = None
+
+
+def cv_windows_device(ctx: L.Context, ds_ns, y, plan: CvPlan, pairs, yhat, width_ns: int, wmax: Optional[int] = None):
+    """pb200_cv_windows_device: the window totals (DESIGN §14) of the gathered entries ``pairs`` (int64 CUDA tensor of
+    plan pairs) over the original ``ds_ns`` / ``y`` and the predict frame ``yhat`` [len(pairs), hmax] of those entries.
+    Returns CUDA tensors n_windows [n] and, [n, wmax], start (cutoff + j W), points, y_sum, yhat_sum.  ``wmax``
+    defaults to the entries' largest held-out row count (a pair has no more windows than held-out rows)."""
+    import torch
+    dev = yhat.device
+    n, hmax = int(yhat.shape[0]), int(yhat.shape[1])
+    width_ns = int(width_ns)
+    if width_ns <= 0:
+        raise ValueError(f"width_ns must be > 0 (got {width_ns})")
+    pairs = pairs.to(device=dev, dtype=torch.int64).contiguous()
+    if wmax is None:
+        wmax = max(1, int((plan.win_end[pairs] - plan.hist_end[pairs]).max().item())) if n else 1
+    wmax = int(wmax)
+    out = {"n_windows": torch.zeros(n, dtype=torch.int32, device=dev),
+           "start": torch.empty((n, wmax), dtype=torch.int64, device=dev),
+           "points": torch.empty((n, wmax), dtype=torch.int32, device=dev),
+           "y_sum": torch.empty((n, wmax), dtype=torch.float64, device=dev),
+           "yhat_sum": torch.empty((n, wmax), dtype=torch.float64, device=dev)}
+    if n:
+        yh = yhat.contiguous()
+        torch.cuda.current_stream(dev).synchronize()
+        L.check(L.load().pb200_cv_windows_device(
+            ctx.handle, ds_ns.data_ptr(), y.data_ptr(), _y_dtype(y), plan.cutoff.data_ptr(), plan.hist_end.data_ptr(),
+            plan.win_end.data_ptr(), pairs.data_ptr(), n, yh.data_ptr(), hmax, width_ns, wmax,
+            out["n_windows"].data_ptr(), out["start"].data_ptr(), out["points"].data_ptr(), out["y_sum"].data_ptr(),
+            out["yhat_sum"].data_ptr()), "pb200_cv_windows_device")
+        ctx.synchronize()
+        _check_window_slots(wmax, int(out["n_windows"].max().item()))
+    return out
 
 
 def _cv_chunks(plan: CvPlan, offsets_host: np.ndarray, budget: int, n_grid: int = 1):
@@ -708,7 +808,8 @@ def cross_validation_device(ctx: L.Context, opts: L.Options, ds_ns, y, offsets_h
                             horizon_ns: int, period_ns: int, initial_ns: int, intervals: bool = False, seed: int = 0,
                             rolling_window: Optional[float] = None, plan: Optional[CvPlan] = None,
                             keep_fits: bool = False, timings: Optional[dict] = None,
-                            _row_budget: Optional[int] = None, grid=None) -> CvResult:
+                            _row_budget: Optional[int] = None, grid=None,
+                            aggregate_ns: Optional[int] = None) -> CvResult:
     """fbprophet.diagnostics.cross_validation (and, with ``rolling_window``, performance_metrics) for every series of a
     packed batch: ``ds_ns`` / ``y`` CUDA tensors sorted within each series, ``cap`` the float64 CUDA tensor of each
     series' full-history cap.  Per chunk of series: one gather, one pb200_fit_device per full-history seasonality mask
@@ -716,7 +817,12 @@ def cross_validation_device(ctx: L.Context, opts: L.Options, ds_ns, y, offsets_h
     (a dict) accumulates seconds per stage -- plan, gather, fit, predict, metrics, each ending in a synchronisation.
     ``grid``: a list of (changepoint_prior_scale, seasonality_prior_scale) pairs.  Every cutoff fit is then made once per
     pair, in the same fit calls (each entry with its own prior scales), and the result's series are the virtual
-    ``s * n_grid + g`` (see CvResult): one backtest per grid point for the price of one batch."""
+    ``s * n_grid + g`` (see CvResult): one backtest per grid point for the price of one batch.
+    ``aggregate_ns`` (a width W dividing ``horizon_ns``): also the held-out totals per window (c + j W, c + (j + 1) W]
+    after each cutoff c, with their metrics, as ``CvResult.windows`` (DESIGN §14).  Every other output is unchanged.
+    With intervals the chunk's predict is pb200_predict_sums_anchored_device, whose pointwise outputs are
+    pb200_predict_device's; the window totals are pb200_cv_windows_device's (stages ``windows`` and
+    ``window_metrics``)."""
     import time
     import torch
     tm = timings if timings is not None else {}
@@ -745,6 +851,13 @@ def cross_validation_device(ctx: L.Context, opts: L.Options, ds_ns, y, offsets_h
         if grid_h.ndim != 2 or grid_h.shape[1] != 2 or grid_h.shape[0] == 0:
             raise ValueError("grid must be a non-empty list of (changepoint_prior_scale, seasonality_prior_scale) pairs")
         n_grid = grid_h.shape[0]
+    W = None
+    if aggregate_ns is not None:
+        W = int(aggregate_ns)
+        if W <= 0 or int(horizon_ns) % W != 0:
+            raise ValueError(f"aggregate_ns must be a positive width that divides the horizon (got {aggregate_ns!r} for "
+                             f"a horizon of {int(horizon_ns)} ns)")
+    sums = W is not None and intervals and opts.uncertainty_samples > 0
     chunks, he_h, we_h = _cv_chunks(plan, offsets_host, int(_row_budget or CV_ROW_BUDGET), n_grid)
     cap = cap.to(device=dev, dtype=torch.float64)
     pieces = []
@@ -800,7 +913,15 @@ def cross_validation_device(ctx: L.Context, opts: L.Options, ds_ns, y, offsets_h
         torch.cuda.current_stream(dev).synchronize()
         lap("fit")
         floor_p = torch.full((n,), float(floor), dtype=torch.float64, device=dev)
-        fcst = predict_batch_device(ctx, opts, fitted, fut, floor_p, cap_p, seed=seed, intervals=intervals)
+        if W is not None:
+            wmax = max(1, min(hmax, int(horizon_ns) // W))      # a pair has no more windows than held-out rows
+        if sums:
+            origins = plan.cutoff[d_pairs] + 1
+            flen = torch.from_numpy(win_len.astype(np.int32)).to(dev)
+            fcst, ws = predict_sums_anchored_device(ctx, opts, fitted, fut, floor_p, cap_p, W, origins, flen, seed=seed,
+                                                    intervals=True, wmax=wmax)
+        else:
+            fcst = predict_batch_device(ctx, opts, fitted, fut, floor_p, cap_p, seed=seed, intervals=intervals)
         lap("predict")
         # back to plan order, then the held-out rows
         inv = torch.from_numpy(np.argsort(perm, kind="stable")).to(dev)
@@ -823,12 +944,33 @@ def cross_validation_device(ctx: L.Context, opts: L.Options, ds_ns, y, offsets_h
                                              rows["yhat_lower"], rows["yhat_upper"], (s1 - s0) * n_grid, rolling_window)
             met["series"] = met["series"] + v0
             lap("metrics")
+        wpiece = None
+        if W is not None:
+            cw = cv_windows_device(ctx, ds_ns, y, plan, d_pairs, fcst.yhat, W, wmax)
+            nwin = cw["n_windows"][inv].long()
+            wk, wj = torch.nonzero(torch.arange(wmax, device=dev)[None, :] < nwin[:, None], as_tuple=True)
+            wcut = plan.cutoff[d_ent][wk]
+            wrows = {"series": torch.from_numpy(ps_h * n_grid + g_h).to(dev)[wk], "cutoff": wcut,
+                     "horizon": cw["start"][inv][wk, wj] - wcut + W, "points": cw["points"][inv][wk, wj],
+                     "y": cw["y_sum"][inv][wk, wj], "yhat": cw["yhat_sum"][inv][wk, wj],
+                     "yhat_lower": ws.lower[inv][wk, wj] if sums else None,
+                     "yhat_upper": ws.upper[inv][wk, wj] if sums else None}
+            lap("windows")
+            wmet = None
+            if rolling_window is not None:
+                v0 = s0 * n_grid
+                wmet = performance_metrics_device(ctx, wrows["series"] - v0, wrows["horizon"], wrows["y"], wrows["yhat"],
+                                                  wrows["yhat_lower"], wrows["yhat_upper"], (s1 - s0) * n_grid,
+                                                  rolling_window)
+                wmet["series"] = wmet["series"] + v0
+                lap("window_metrics")
+            wpiece = ({k: (v.cpu().numpy() if v is not None else None) for k, v in wrows.items()}, wmet)
         fh = None
         if keep_fits:
             fh = FittedBatch(*(x[inv].cpu().numpy() for x in (fitted.params, fitted.tchange, fitted.meta_i32,
                                                                fitted.meta_i64, fitted.meta_f64)), lay.smax, lay.kmax)
         pieces.append(({k: (v.cpu().numpy() if v is not None else None) for k, v in rows.items()}, met,
-                       fitted.meta_i32[inv, 4].cpu().numpy(), fh))
+                       fitted.meta_i32[inv, 4].cpu().numpy(), fh, wpiece))
         lap("rows")
     cat = lambda xs: np.concatenate(xs) if xs else None                       # noqa: E731
     rows = {k: cat([p[0][k] for p in pieces]) if (pieces and pieces[0][0][k] is not None) else None
@@ -850,9 +992,27 @@ def cross_validation_device(ctx: L.Context, opts: L.Options, ds_ns, y, offsets_h
                                    for f in ("params", "tchange", "meta_i32", "meta_i64", "meta_f64")), lay.smax, lay.kmax)
     ent_all, ps_all, g_all = _cv_entries(plan, 0, plan.n_cutoffs.size, n_grid)
     status = cat([p[2] for p in pieces]) if pieces else np.zeros(0, np.int32)
+    windows = None
+    if W is not None:
+        i64, f64 = np.zeros(0, np.int64), np.zeros(0)
+        empty = {"series": i64, "cutoff": i64, "horizon": i64, "points": np.zeros(0, np.int32), "y": f64, "yhat": f64,
+                 "yhat_lower": f64 if sums else None, "yhat_upper": f64 if sums else None}
+        wr = {k: (cat([p[4][0][k] for p in pieces]) if pieces else v) if v is not None else None for k, v in empty.items()}
+        wm = None
+        if rolling_window is not None:
+            keys = ("series", "horizon", "mse", "rmse", "mae", "mape", "coverage")
+            if pieces:
+                wm = {k: (cat([p[4][1][k] for p in pieces]) if pieces[0][4][1][k] is not None else None) for k in keys}
+            else:
+                wm = performance_metrics_device(ctx, *(torch.zeros(0, dtype=t, device=dev) for t in
+                                                       (torch.int64, torch.int64, torch.float64, torch.float64)),
+                                                *((torch.zeros(0, dtype=torch.float64, device=dev),) * 2 if sums else
+                                                  (None, None)), 0, rolling_window)
+        windows = CvWindows(W, wr["series"], wr["cutoff"], wr["horizon"], wr["points"], wr["y"], wr["yhat"],
+                            wr["yhat_lower"], wr["yhat_upper"], wm)
     return CvResult(ps_all * n_grid + g_all, plan.cutoff.cpu().numpy()[ent_all], status, plan.mask[ps_all], rows["series"],
                     rows["ds"], rows["cutoff"], rows["y"], rows["yhat"], rows["yhat_lower"], rows["yhat_upper"], metrics,
-                    fitted_all)
+                    fitted_all, windows)
 
 
 def performance_metrics_device(ctx: L.Context, series, horizon_ns, y, yhat, yhat_lower, yhat_upper, n_series: int,

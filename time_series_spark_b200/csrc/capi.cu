@@ -834,6 +834,9 @@ struct SumOut {
     int64_t* quantity_sum;
     double* sum_lower;
     double* sum_upper;
+    // pb200_predict_sums_anchored_device: an origin and a frame length per model, in place of origin_ns and the horizon
+    const int64_t* origins = nullptr;
+    const int32_t* frame_len = nullptr;
 };
 
 // checked before anything is copied or launched
@@ -849,7 +852,7 @@ int check_sum_args(const pb200_options* o, const SumOut& s) {
 
 // pb200_predict_device; d_comp != null: the components instance of predict_kernel, d_tlo / d_thi != null: the
 // trend-bounds instance of mc_kernel; sums != null: mc_sum_kernel after them (it also runs on an empty frame, where
-// every model has no window)
+// every model has no window), its per-model instance when sums->origins != null
 int predict_device(pb200_ctx* c, const pb200_options* opts, const double* d_params, const double* d_tchange,
                    const int32_t* d_meta_i32, const int64_t* d_meta_i64, const double* d_meta_f64, int64_t n_models,
                    const int64_t* d_future_ds, int32_t horizon, const double* d_floor, const double* d_cap, uint64_t seed,
@@ -916,6 +919,8 @@ int predict_device(pb200_ctx* c, const pb200_options* opts, const double* d_para
         s.win_points = sums->win_points;
         s.yhat_sum = sums->yhat_sum;
         s.quantity_sum = (long long*)sums->quantity_sum;
+        s.origins = (const long long*)sums->origins;
+        s.frame_len = sums->frame_len;
         rc = pb200::launch_mc_sum(c->stream, c->sms, a, opts->uncertainty_samples, opts->interval_width, seed, s);
         if (rc == -1) return fail(PB200_E_ARG, "uncertainty_samples / interval_width out of range");
         if (rc) return fail(PB200_E_CUDA, "mc sum kernel launch", cudaGetLastError());
@@ -1082,6 +1087,23 @@ PB200_API int pb200_predict_sums_device(pb200_ctx* c, const pb200_options* opts,
                          double* d_sum_lower, double* d_sum_upper) {
     const SumOut s = {width_ns, origin_ns, wmax, d_n_windows, d_win_start, d_win_points, d_yhat_sum, d_quantity_sum,
                       d_sum_lower, d_sum_upper};
+    return predict_device(c, opts, d_params, d_tchange, d_meta_i32, d_meta_i64, d_meta_f64, n_models, d_future_ds, horizon,
+                          d_floor, d_cap, seed, d_yhat, d_yhat_lower, d_yhat_upper, d_yhat_int, nullptr, nullptr, nullptr, &s);
+}
+
+PB200_API int pb200_predict_sums_anchored_device(pb200_ctx* c, const pb200_options* opts, const double* d_params,
+                         const double* d_tchange, const int32_t* d_meta_i32, const int64_t* d_meta_i64,
+                         const double* d_meta_f64, int64_t n_models, const int64_t* d_future_ds, int32_t horizon,
+                         const double* d_floor, const double* d_cap, uint64_t seed, double* d_yhat, double* d_yhat_lower,
+                         double* d_yhat_upper, int32_t* d_yhat_int, int64_t width_ns, const int64_t* d_origin_ns,
+                         const int32_t* d_frame_len, int32_t wmax, int32_t* d_n_windows, int64_t* d_win_start,
+                         int32_t* d_win_points, double* d_yhat_sum, int64_t* d_quantity_sum, double* d_sum_lower,
+                         double* d_sum_upper) {
+    if (n_models > 0 && (!d_origin_ns || !d_frame_len)) return fail(PB200_E_ARG, "null pointer (origins / frame lengths)");
+    SumOut s = {width_ns, 0, wmax, d_n_windows, d_win_start, d_win_points, d_yhat_sum, d_quantity_sum, d_sum_lower,
+                d_sum_upper};
+    s.origins = d_origin_ns;
+    s.frame_len = d_frame_len;
     return predict_device(c, opts, d_params, d_tchange, d_meta_i32, d_meta_i64, d_meta_f64, n_models, d_future_ds, horizon,
                           d_floor, d_cap, seed, d_yhat, d_yhat_lower, d_yhat_upper, d_yhat_int, nullptr, nullptr, nullptr, &s);
 }
@@ -1295,6 +1317,45 @@ PB200_API int pb200_cv_metrics_device(pb200_ctx* c, const int64_t* d_horizon, co
     a.out_valid = d_valid;
     const int grid = (int)std::min<int64_t>((n_series + 127) / 128, (int64_t)c->sms * 16);
     pb200::cv::cv_metrics_kernel<<<grid, 128, 0, c->stream>>>(a);
+    CK(cudaGetLastError());
+    c->launches++;
+    return PB200_OK;
+}
+
+PB200_API int pb200_cv_windows_device(pb200_ctx* c, const int64_t* d_ds, const void* d_y, int32_t y_dtype,
+                                      const int64_t* d_cutoff, const int64_t* d_hist_end, const int64_t* d_win_end,
+                                      const int64_t* d_pairs, int64_t n, const double* d_yhat, int32_t hmax, int64_t width_ns,
+                                      int32_t wmax, int32_t* d_n_windows, int64_t* d_win_start, int32_t* d_win_points,
+                                      double* d_y_sum, double* d_yhat_sum) {
+    if (!c) return fail(PB200_E_ARG, "ctx is null");
+    if (n < 0 || hmax < 1 || wmax < 1) return fail(PB200_E_ARG, "sizes");
+    if (width_ns <= 0) return fail(PB200_E_ARG, "width_ns must be > 0");
+    if (y_dtype < 0 || y_dtype > 2) return fail(PB200_E_ARG, "y_dtype");
+    if (n == 0) return PB200_OK;
+    if (!d_ds || !d_y || !d_cutoff || !d_hist_end || !d_win_end || !d_pairs || !d_yhat || !d_n_windows || !d_win_start ||
+        !d_win_points || !d_y_sum || !d_yhat_sum)
+        return fail(PB200_E_ARG, "null pointer");
+    CK(cudaSetDevice(c->device));
+    pb200::cv::WindowArgs a;
+    a.ds = (const long long*)d_ds;
+    a.y = d_y;
+    a.y_dtype = y_dtype;
+    a.cutoff = (const long long*)d_cutoff;
+    a.hist_end = (const long long*)d_hist_end;
+    a.win_end = (const long long*)d_win_end;
+    a.pairs = (const long long*)d_pairs;
+    a.n = n;
+    a.yhat = d_yhat;
+    a.hmax = hmax;
+    a.width = width_ns;
+    a.wmax = wmax;
+    a.n_windows = d_n_windows;
+    a.win_start = (long long*)d_win_start;
+    a.points = d_win_points;
+    a.y_sum = d_y_sum;
+    a.yhat_sum = d_yhat_sum;
+    const int grid = (int)std::min<int64_t>((n + 7) / 8, (int64_t)c->sms * 4);   // 8 warps per CTA, one per entry
+    pb200::cv::cv_window_kernel<<<grid, 256, 0, c->stream>>>(a);
     CK(cudaGetLastError());
     c->launches++;
     return PB200_OK;

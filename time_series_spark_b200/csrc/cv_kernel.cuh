@@ -1,4 +1,4 @@
-// Backtest (fbprophet.diagnostics cross_validation / performance_metrics) over a whole batch of series.  Three pieces, the
+// Backtest (fbprophet.diagnostics cross_validation / performance_metrics) over a whole batch of series.  Four pieces, the
 // fit / predict / MC kernels being reused unchanged in between:
 //   cv_plan_kernel     per series: the cutoffs of generate_cutoffs, each cutoff's history end and held-out window, the
 //                      full history's seasonality mask and the error flags.  Two passes, like csv_kernel.cuh: counts,
@@ -7,8 +7,10 @@
 //                      timestamps as a [pairs, hmax] frame for predict (short windows padded by their last timestamp).
 //   cv_metrics_kernel  performance_metrics per series: per-horizon trailing-window means of the squared / absolute /
 //                      relative errors and of the interval coverage.
-// Every series is one warp (plan) or one thread (metrics) and every sum runs in one fixed order with no floating-point
-// atomics: a series' plan and metrics do not depend on the other series of the batch.
+//   cv_window_kernel   per gathered entry: the held-out rows' totals over fixed-width windows anchored at the cutoff
+//                      (DESIGN §14), the window rows cv_metrics_kernel then reduces like pointwise rows.
+// Every series is one warp (plan, windows) or one thread (metrics) and every sum runs in one fixed order with no
+// floating-point atomics: a series' plan, metrics and windows do not depend on the other series of the batch.
 #pragma once
 #include <cuda_runtime.h>
 #include <math.h>
@@ -265,6 +267,88 @@ __global__ void __launch_bounds__(128) cv_metrics_kernel(const MetricsArgs a) {
             a.out_cov[q] = a.lo ? cv / (double)w : NAN;
         }
         for (long long q = r0 + G; q < r1; ++q) a.out_valid[q] = 0;
+    }
+}
+
+struct WindowArgs {
+    const long long* ds;
+    const void* y;
+    int y_dtype;
+    const long long* cutoff;     // [pairs] (plan)
+    const long long* hist_end;
+    const long long* win_end;
+    const long long* pairs;      // [n] the pair of each gathered entry
+    long long n;
+    const double* yhat;          // [n * hmax] the predict frame of the gathered entries
+    int hmax;
+    long long width;             // W > 0
+    int wmax;
+    // outputs: n_windows [n]; from here on [n * wmax], slot k * wmax + i for entry k's i-th non-empty window
+    int* n_windows;
+    long long* win_start;        // c + j W: window j is (c + j W, c + (j + 1) W]
+    int* points;
+    double* y_sum;
+    double* yhat_sum;
+};
+
+// One warp per entry.  The held-out rows [hist_end, win_end) of the pair are read 32 at a time, one per lane (coalesced),
+// then broadcast in row order so that every lane keeps the same running sums: s = s + v in ascending row order, plain
+// fp64 adds, the order of tests/window_backtest_oracle.window_rows.  Row r lies in window j = (ds_r - (c + 1)) / W:
+// every held-out row has c < ds_r <= c + H, so the quotient is a non-negative floor and no term overflows.  Lane 0 writes a window when
+// the next row's differs; windows at or past wmax are counted and not written; slots past the count hold INT64_MIN / 0 /
+// NaN, as mc_sum_kernel's.
+__global__ void __launch_bounds__(256) cv_window_kernel(const WindowArgs a) {
+    const int lane = threadIdx.x & 31;
+    const long long gw = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    const long long nwarps = ((long long)gridDim.x * blockDim.x) >> 5;
+    for (long long k = gw; k < a.n; k += nwarps) {
+        const long long p = a.pairs[k];
+        const long long he = a.hist_end[p], we = a.win_end[p], c = a.cutoff[p];
+        const double* yh = a.yhat + (size_t)k * a.hmax;
+        const size_t wb = (size_t)k * a.wmax;
+        int nw = 0, pts = 0;
+        long long cur = 0;
+        double ys = 0.0, fs = 0.0;
+        auto close_window = [&]() {
+            if (lane == 0 && nw < a.wmax) {
+                a.win_start[wb + nw] = c + cur * a.width;
+                a.points[wb + nw] = pts;
+                a.y_sum[wb + nw] = ys;
+                a.yhat_sum[wb + nw] = fs;
+            }
+            ++nw;
+            pts = 0; ys = 0.0; fs = 0.0;
+        };
+        for (long long r0 = he; r0 < we; r0 += 32) {
+            const long long r = r0 + lane;
+            long long wv = 0;
+            double yv = 0.0, fv = 0.0;
+            if (r < we) {
+                wv = (a.ds[r] - c - 1) / a.width;
+                if (a.y_dtype == PB200_Y_F64) yv = ((const double*)a.y)[r];
+                else if (a.y_dtype == PB200_Y_F32) yv = (double)((const float*)a.y)[r];
+                else yv = (double)((const int*)a.y)[r];
+                fv = yh[r - he];
+            }
+            const int m = we - r0 < 32 ? (int)(we - r0) : 32;
+            for (int i = 0; i < m; ++i) {
+                const long long wi = __shfl_sync(0xffffffffu, wv, i);
+                const double yi = __shfl_sync(0xffffffffu, yv, i), fi = __shfl_sync(0xffffffffu, fv, i);
+                if (pts > 0 && wi != cur) close_window();
+                cur = wi;
+                ++pts;
+                ys = __dadd_rn(ys, yi);
+                fs = __dadd_rn(fs, fi);
+            }
+        }
+        if (pts > 0) close_window();
+        if (lane == 0) a.n_windows[k] = nw;
+        for (int i = (nw < a.wmax ? nw : a.wmax) + lane; i < a.wmax; i += 32) {
+            a.win_start[wb + i] = INT64_MIN;
+            a.points[wb + i] = 0;
+            a.y_sum[wb + i] = NAN;
+            a.yhat_sum[wb + i] = NAN;
+        }
     }
 }
 

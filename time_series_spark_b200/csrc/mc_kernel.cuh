@@ -422,6 +422,10 @@ struct McSumArgs {
     int* win_points;
     double* yhat_sum;
     long long* quantity_sum;
+    // mc_sum_kernel<LOGI, true> only (DESIGN §14): a window origin and a frame length per model, in place of origin_ns and
+    // the horizon; the points past frame_len (the backtest frame's padding) are not walked
+    const long long* origins;     // [n_models]
+    const int* frame_len;         // [n_models]
 };
 
 constexpr int MC_SUM_TILE = 512;  // points whose t, seasonal term, window and predict outputs are staged at once (even: noise pairs)
@@ -438,7 +442,10 @@ __device__ __forceinline__ long long window_of(const long long ds, const long lo
 // and stores them into row (window mod 16) of the staging area when the window index of the next point differs.  After 16
 // closed windows, and at the frame's end, warp r selects the percentiles of row r.  Thread 0 sums yhat / yhat_int of
 // predict_kernel's output over the same windows, in the same order.  Windows at or past wmax are counted and not written.
-template <bool LOGI>
+// PER_MODEL: model i's windows are taken from origins[i] over its first frame_len[i] points only.  Tmax, the key and the
+// counters stay those of the whole frame, so the draws at the walked points are unchanged (the backtest pads a frame by
+// repeating its last timestamp, which leaves Tmax as it is).
+template <bool LOGI, bool PER_MODEL>
 __global__ void __launch_bounds__(MC_THREADS, 1) mc_sum_kernel(const McSumArgs a) {
     extern __shared__ __align__(16) unsigned char mc_smem[];
     double* rows = (double*)mc_smem;                       // [MC_TILE][MC_NP], as mc_kernel
@@ -488,7 +495,7 @@ __global__ void __launch_bounds__(MC_THREADS, 1) mc_sum_kernel(const McSumArgs a
                     s[q] = 0.0;
                 }
                 if (tid == 0 && nw < a.wmax) {
-                    a.win_start[wbase + nw] = a.origin_ns + cur_w * a.width_ns;
+                    a.win_start[wbase + nw] = (PER_MODEL ? a.origins[model] : a.origin_ns) + cur_w * a.width_ns;
                     a.win_points[wbase + nw] = pts;
                     a.yhat_sum[wbase + nw] = ys;
                     a.quantity_sum[wbase + nw] = qs;
@@ -496,14 +503,15 @@ __global__ void __launch_bounds__(MC_THREADS, 1) mc_sum_kernel(const McSumArgs a
                 ys = 0.0; qs = 0; pts = 0;
                 if ((++nw & (MC_TILE - 1)) == 0) select_rows(MC_TILE);
             };
-            for (int h0 = 0; h0 < H; h0 += MC_SUM_TILE) {
-                const int np = min(MC_SUM_TILE, H - h0);
+            const int HW = PER_MODEL ? min(a.frame_len[model], H) : H;   // points walked
+            for (int h0 = 0; h0 < HW; h0 += MC_SUM_TILE) {
+                const int np = min(MC_SUM_TILE, HW - h0);
                 __syncthreads();                           // the previous tile has been walked
                 if (tid < np) {
                     const long long dsv = mc.p.future_ds[base + h0 + tid];
                     tt[tid] = (double)(dsv - ms.start) / ms.t_scale;
                     seas[tid] = ms.K > 0 ? seasonal_term(ms, dsv) : 0.0;
-                    win[tid] = window_of(dsv, a.origin_ns, a.width_ns);
+                    win[tid] = window_of(dsv, PER_MODEL ? a.origins[model] : a.origin_ns, a.width_ns);
                     yh_t[tid] = mc.p.yhat[base + h0 + tid];
                     yi_t[tid] = mc.p.yhat_int[base + h0 + tid];
                 }
@@ -557,11 +565,12 @@ cudaError_t launch_mc_inst(cudaStream_t st, int grid, size_t smem, const McArgs&
     return cudaGetLastError();
 }
 
-template <bool LOGI>
+template <bool LOGI, bool PER_MODEL>
 cudaError_t launch_mc_sum_inst(cudaStream_t st, int grid, const McSumArgs& a) {
-    const cudaError_t e = cudaFuncSetAttribute(mc_sum_kernel<LOGI>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)MC_SMEM);
+    const cudaError_t e = cudaFuncSetAttribute(mc_sum_kernel<LOGI, PER_MODEL>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                               (int)MC_SMEM);
     if (e != cudaSuccess) return e;
-    mc_sum_kernel<LOGI><<<grid, MC_THREADS, MC_SMEM, st>>>(a);
+    mc_sum_kernel<LOGI, PER_MODEL><<<grid, MC_THREADS, MC_SMEM, st>>>(a);
     return cudaGetLastError();
 }
 
@@ -598,7 +607,8 @@ inline int launch_mc(cudaStream_t st, int sms, const PredictArgs& p, int n_sampl
 }
 
 // mc_sum_kernel over the frame of p, whose yhat / yhat_int predict_kernel has written on the same stream; s.mc is filled
-// here but for its lower / upper (the window bounds).  Returns as launch_mc
+// here but for its lower / upper (the window bounds).  s.origins != null: the per-model instance (s.frame_len as well).
+// Returns as launch_mc
 inline int launch_mc_sum(cudaStream_t st, int sms, const PredictArgs& p, int n_samples, double width, uint64_t seed,
                          McSumArgs& s) {
     double* const lo = s.mc.lower;
@@ -607,7 +617,9 @@ inline int launch_mc_sum(cudaStream_t st, int sms, const PredictArgs& p, int n_s
     s.mc.lower = lo;
     s.mc.upper = hi;
     const int grid = p.n_models < sms ? p.n_models : sms;
-    const cudaError_t e = p.growth == PB200_GROWTH_LOGISTIC ? launch_mc_sum_inst<true>(st, grid, s) : launch_mc_sum_inst<false>(st, grid, s);
+    const bool logi = p.growth == PB200_GROWTH_LOGISTIC, per_model = s.origins != nullptr;
+    const cudaError_t e = logi ? (per_model ? launch_mc_sum_inst<true, true>(st, grid, s) : launch_mc_sum_inst<true, false>(st, grid, s))
+                               : (per_model ? launch_mc_sum_inst<false, true>(st, grid, s) : launch_mc_sum_inst<false, false>(st, grid, s));
     return e == cudaSuccess ? 0 : 1;
 }
 

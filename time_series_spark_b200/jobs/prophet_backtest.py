@@ -12,9 +12,15 @@ Keys (``backtest.*``):
   rolling_window     fraction of a series' held-out rows each metric averages over, in [0, 1]; default 0.1
   intervals          false (default): no yhat_lower / yhat_upper, no coverage column
   uncertainty_samples, interval_width, seed   1000, 0.8, 0 (used with intervals only)
+  aggregate          a fixed-width duration W dividing the horizon ('1h', '8h', '1D'): also the held-out totals per
+                     window (c + j W, c + (j + 1) W] after each cutoff c and their metrics by horizon (j + 1) W, with
+                     intervals the coverage of the totals' joint-draw intervals (DESIGN §14); needs io.window_metrics
 Outputs (parquet, one part file per rank):
-  io.metrics   series_id, dim_id, horizon duration[ns], mse, rmse, mae, mape[, coverage]
-  io.cv_rows   (optional) series_id, dim_id, ds, cutoff, y, yhat[, yhat_lower, yhat_upper]
+  io.metrics          series_id, dim_id, horizon duration[ns], mse, rmse, mae, mape[, coverage]
+  io.cv_rows          (optional) series_id, dim_id, ds, cutoff, y, yhat[, yhat_lower, yhat_upper]
+  io.window_metrics   (with aggregate) series_id, dim_id, horizon duration[ns], mse, rmse, mae, mape[, coverage]
+  io.window_rows      (optional, with aggregate) series_id, dim_id, cutoff, horizon, window_points, y, yhat[,
+                      yhat_lower, yhat_upper]
 """
 from __future__ import annotations
 
@@ -71,7 +77,38 @@ def backtest_spec_from_config(config) -> dict:
         if not (2 <= ns <= 1024):
             raise ValueError(f"backtest.uncertainty_samples must be in [2, 1024] (got {b.get('uncertainty_samples')!r})")
         spec["interval_width"], spec["uncertainty_samples"] = width, ns
+    spec["aggregate"] = _aggregate_width(config, b, horizon)
     return spec
+
+
+def _aggregate_width(config, b: dict, horizon: int):
+    """``backtest.aggregate`` in ns (None without the key): a fixed-width duration that divides the horizon, so that
+    every window (c + j W, c + (j + 1) W] lies inside the held-out span (c, c + horizon]."""
+    import pandas as pd
+    from .prophet_scorer import _to_offset
+    spec = b.get("aggregate")
+    if spec is None:
+        return None
+    try:
+        off = _to_offset(spec)
+    except Exception:
+        off = None                  # not a frequency alias: a Timedelta string such as '2 days', as backtest.horizon
+    try:
+        if off is None:
+            width = int(pd.Timedelta(spec).value)
+        else:
+            width = int(7 * 86400 * 10**9 * off.n if isinstance(off, pd.offsets.Week) and off.weekday is None else off.nanos)
+    except Exception:
+        raise ValueError(f"backtest.aggregate must be a fixed-width duration such as '1h', '8h' or '1D' (got {spec!r}; "
+                         "calendar offsets such as 'M' have no fixed width)") from None
+    if width <= 0:
+        raise ValueError(f"backtest.aggregate must be a positive duration (got {spec!r})")
+    if horizon % width != 0:
+        raise ValueError(f"backtest.aggregate ({spec!r}) must divide backtest.horizon ({b['horizon']!r}), so that every "
+                         "window lies inside the held-out span")
+    if not (config.get("io", {}) or {}).get("window_metrics"):
+        raise ValueError("backtest.aggregate needs io.window_metrics, the directory the window metrics are written to")
+    return width
 
 
 def _who(series_id, dim_id, mask) -> str:
@@ -80,19 +117,22 @@ def _who(series_id, dim_id, mask) -> str:
             f"{int(np.count_nonzero(mask))} group(s) in all)")
 
 
-def assemble_outputs(series_id, dim_id, res: batched.CvResult, y_dtype, with_rows: bool = True):
-    """Metrics (and row) tables of a CvResult.  A series with a failed cutoff fit (status < 0) -- where fbprophet's
-    cross_validation would raise -- gets no row in either table, and a printed line names it and the cutoff."""
+def _failed_series(series_id, dim_id, res: batched.CvResult, announce: bool = True):
+    """Per series: some cutoff fit failed (status < 0), where fbprophet's cross_validation would raise; a printed line
+    names each such series and its first failed cutoff."""
     n = len(series_id)
     failed = np.zeros(n, bool)
     for p in np.flatnonzero(res.pair_status < 0):
         s = int(res.pair_series[p])
-        if not failed[s]:
+        if not failed[s] and announce:
             cut = np.datetime64(int(res.pair_cutoff[p]), "ns")
             print(f"Runtime error (solver status {int(res.pair_status[p])}) for series_id: {int(series_id[s])}, "
                   f"dim_id: {int(dim_id[s])}, cutoff: {cut}")
         failed[s] = True
-    m = res.metrics
+    return failed
+
+
+def _metrics_table(series_id, dim_id, m: dict, failed) -> pa.Table:
     keep = ~failed[m["series"]]
     ms = m["series"][keep]
     cols = {"series_id": pa.array(np.asarray(series_id)[ms], pa.int32()),
@@ -102,7 +142,38 @@ def assemble_outputs(series_id, dim_id, res: batched.CvResult, y_dtype, with_row
         cols[k] = pa.array(m[k][keep], pa.float64())
     if m["coverage"] is not None:
         cols["coverage"] = pa.array(m["coverage"][keep], pa.float64())
-    metrics = pa.table(cols)
+    return pa.table(cols)
+
+
+def assemble_window_outputs(series_id, dim_id, res: batched.CvResult, with_rows: bool = True):
+    """Window metrics (and window row) tables of a CvResult made with aggregate_ns; the same failed-fit rule as
+    assemble_outputs (which prints the lines)."""
+    failed = _failed_series(series_id, dim_id, res, announce=False)
+    w = res.windows
+    metrics = _metrics_table(series_id, dim_id, w.metrics, failed)
+    rows = None
+    if with_rows:
+        keep = ~failed[w.series]
+        rs = w.series[keep]
+        rc = {"series_id": pa.array(np.asarray(series_id)[rs], pa.int32()),
+              "dim_id": pa.array(np.asarray(dim_id)[rs], pa.int32()),
+              "cutoff": pa.array(w.cutoff[keep], pa.timestamp("ns")),
+              "horizon": pa.array(w.horizon[keep], pa.duration("ns")),
+              "window_points": pa.array(w.points[keep], pa.int32()),
+              "y": pa.array(w.y[keep], pa.float64()),
+              "yhat": pa.array(w.yhat[keep], pa.float64())}
+        if w.yhat_lower is not None:
+            rc["yhat_lower"] = pa.array(w.yhat_lower[keep], pa.float64())
+            rc["yhat_upper"] = pa.array(w.yhat_upper[keep], pa.float64())
+        rows = pa.table(rc)
+    return metrics, rows
+
+
+def assemble_outputs(series_id, dim_id, res: batched.CvResult, y_dtype, with_rows: bool = True):
+    """Metrics (and row) tables of a CvResult.  A series with a failed cutoff fit (status < 0) -- where fbprophet's
+    cross_validation would raise -- gets no row in either table, and a printed line names it and the cutoff."""
+    failed = _failed_series(series_id, dim_id, res)
+    metrics = _metrics_table(series_id, dim_id, res.metrics, failed)
     rows = None
     if with_rows:
         keep = ~failed[res.row_series]
@@ -127,6 +198,7 @@ class ProphetBacktester:
         self.logger = logger or logging.getLogger(self.__class__.__name__)
         self.config = config
         self.rank_local_input = False
+        self.window_outputs = None     # (window metrics, window rows or None) with backtest.aggregate
 
     def read_input_dataframe(self, spark=None):
         reader = ProphetModeler(self.config)
@@ -135,7 +207,8 @@ class ProphetBacktester:
         return frame
 
     def backtest(self, table: pa.Table):
-        """(metrics table, row table or None) of the groups in ``table`` (columns series_id, dim_id, ds, y)."""
+        """(metrics table, row table or None) of the groups in ``table`` (columns series_id, dim_id, ds, y).  With
+        backtest.aggregate, ``self.window_outputs`` gets the (window metrics, window rows or None) tables."""
         t0 = time.time()
         spec = backtest_spec_from_config(self.config)
         floor = float(self.config["model"]["floor"])
@@ -151,14 +224,22 @@ class ProphetBacktester:
         if ws > 1 and not self.rank_local_input:
             lo, hi = pdist.shard_bounds(pk.offsets, ws)[rank]
             pk = pk.take(lo, hi)
-        with_rows = bool((self.config.get("io", {}) or {}).get("cv_rows"))
+        io = self.config.get("io", {}) or {}
+        with_rows = bool(io.get("cv_rows"))
+        W = spec["aggregate"]
         if pk.n == 0:
+            empty_metrics = lambda: dict({k: np.zeros(0, np.int64 if k in ("series", "horizon") else np.float64)  # noqa: E731
+                                          for k in ("series", "horizon", "mse", "rmse", "mae", "mape")},
+                                         coverage=np.zeros(0) if spec["intervals"] else None)
             res = batched.CvResult(*(np.zeros(0, np.int64),) * 4, *(np.zeros(0, np.int64),) * 3, *(np.zeros(0),) * 2,
-                                   None, None, metrics={k: np.zeros(0, np.int64 if k in ("series", "horizon") else np.float64)
-                                                        for k in ("series", "horizon", "mse", "rmse", "mae", "mape")})
-            res.metrics["coverage"] = np.zeros(0) if spec["intervals"] else None
+                                   None, None, metrics=empty_metrics())
             if spec["intervals"]:
                 res.yhat_lower, res.yhat_upper = np.zeros(0), np.zeros(0)
+            if W is not None:
+                iv = np.zeros(0) if spec["intervals"] else None
+                res.windows = batched.CvWindows(W, *(np.zeros(0, np.int64),) * 3, np.zeros(0, np.int32), np.zeros(0),
+                                                np.zeros(0), iv, iv, empty_metrics())
+                self.window_outputs = assemble_window_outputs(pk.series_id, pk.dim_id, res, bool(io.get("window_rows")))
             return assemble_outputs(pk.series_id, pk.dim_id, res, np.dtype(str(pk.y.dtype).replace("torch.", "")), with_rows)
         ds, y = pk.ds.contiguous(), pk.y.contiguous()
         short = np.diff(pk.offsets) < 2
@@ -174,7 +255,7 @@ class ProphetBacktester:
         print(f"Backtesting {pk.n} series at {plan.n_pairs} cutoffs")
         res = batched.cross_validation_device(ctx, opts, ds, y, pk.offsets, floor, cap, spec["horizon"], spec["period"],
                                               spec["initial"], intervals=spec["intervals"], seed=spec["seed"],
-                                              rolling_window=spec["rolling_window"], plan=plan)
+                                              rolling_window=spec["rolling_window"], plan=plan, aggregate_ns=W)
         for code, msg in ((L.ST_CAP_LE_FLOOR, "cap must be greater than floor (which defaults to 0)."),
                           (L.ST_BAD_INPUT, "Found non-finite y or a zero time span in a series.")):
             hit = np.zeros(pk.n, bool)
@@ -182,14 +263,18 @@ class ProphetBacktester:
             if hit.any():
                 raise ValueError(msg + _who(pk.series_id, pk.dim_id, hit))
         out = assemble_outputs(pk.series_id, pk.dim_id, res, np.dtype(str(y.dtype).replace("torch.", "")), with_rows)
+        if W is not None:
+            self.window_outputs = assemble_window_outputs(pk.series_id, pk.dim_id, res, bool(io.get("window_rows")))
         print(f"Backtest: {out[0].num_rows} metrics rows in {time.time() - t0:.1f} s")
         return out
 
     def persist(self, metrics: pa.Table, rows) -> None:
-        """Parquet part file per rank under io.metrics (and io.cv_rows)."""
+        """Parquet part file per rank under io.metrics (and io.cv_rows, and with backtest.aggregate io.window_metrics
+        and io.window_rows)."""
         io = self.config["io"]
         rank = pdist.world()[0]
-        for key, tbl in (("metrics", metrics), ("cv_rows", rows)):
+        wm, wr = self.window_outputs or (None, None)
+        for key, tbl in (("metrics", metrics), ("cv_rows", rows), ("window_metrics", wm), ("window_rows", wr)):
             if tbl is None or not io.get(key):
                 continue
             pdist.prepare_output_dir(io[key])
