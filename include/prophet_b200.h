@@ -401,6 +401,38 @@ PB200_API int pb200_predict_sums_anchored_device(pb200_ctx* ctx, const pb200_opt
                          int32_t* d_n_windows, int64_t* d_win_start, int32_t* d_win_points,
                          double* d_yhat_sum, int64_t* d_quantity_sum, double* d_sum_lower, double* d_sum_upper);
 
+/*
+ * pb200_predict_* plus forecast quantiles at n_q levels from the same draws (DESIGN §15): fbprophet's
+ * np.percentile(predictive_samples(future)['yhat'], p, axis=1) for each p of h_percentiles, in one pass over the draws.
+ * Same arguments and the same yhat / yhat_lower / yhat_upper / yhat_int bits as pb200_predict_* (the bounds optional as
+ * there), and:
+ *   n_q            levels, in [1, 32]
+ *   h_percentiles  host double [n_q], each in [0, 100]; any order, repeats allowed
+ *   d_quantiles    double [n_q * n_models * horizon]: plane q, model i, point h at (q * n_models + i) * horizon + h
+ * Plane q at a point is s_i + (s_{min(i+1, n-1)} - s_i) * f over the sorted draws s, with x = p_q / 100.0 * (n - 1),
+ * i = floor(x), f = x - i, n = uncertainty_samples: the expression of the interval bounds, so a plane at
+ * 100 (1 -+ interval_width) / 2 (computed as written) is yhat_lower / yhat_upper bit for bit.  Failed models get NaN.
+ * uncertainty_samples must be in [2, 1024] (PB200_E_UNSUPPORTED) and interval_width in [0, 1]; n_q, a NaN or
+ * out-of-range percentile, or a null h_percentiles / d_quantiles give PB200_E_ARG.  Nothing is launched on an error.
+ */
+PB200_API int pb200_predict_quantiles_device(pb200_ctx* ctx, const pb200_options* opts,
+                         const double* d_params, const double* d_tchange,
+                         const int32_t* d_meta_i32, const int64_t* d_meta_i64,
+                         const double* d_meta_f64, int64_t n_models,
+                         const int64_t* d_future_ds, int32_t horizon,
+                         const double* d_floor, const double* d_cap, uint64_t seed,
+                         double* d_yhat, double* d_yhat_lower, double* d_yhat_upper,
+                         int32_t* d_yhat_int, int32_t n_q, const double* h_percentiles, double* d_quantiles);
+
+PB200_API int pb200_predict_quantiles_host(pb200_ctx* ctx, const pb200_options* opts,
+                       const double* h_params, const double* h_tchange,
+                       const int32_t* h_meta_i32, const int64_t* h_meta_i64,
+                       const double* h_meta_f64, int64_t n_models,
+                       const int64_t* h_future_ds, int32_t horizon,
+                       const double* h_floor, const double* h_cap, uint64_t seed,
+                       double* h_yhat, double* h_yhat_lower, double* h_yhat_upper,
+                       int32_t* h_yhat_int, int32_t n_q, const double* h_percentiles, double* h_quantiles);
+
 /* future_ds[i*horizon + j] = last_ds[i] + (j+1)*freq_ns  -- make_future_dataframe
  * (include_history=False) for a fixed-width pandas frequency. */
 PB200_API int pb200_make_future_device(pb200_ctx* ctx, const int64_t* d_last_ds, int64_t n_models,
@@ -497,6 +529,21 @@ PB200_API int pb200_cv_windows_device(pb200_ctx* ctx, const int64_t* d_ds, const
                                       const int64_t* d_pairs, int64_t n, const double* d_yhat, int32_t hmax,
                                       int64_t width_ns, int32_t wmax, int32_t* d_n_windows, int64_t* d_win_start,
                                       int32_t* d_win_points, double* d_y_sum, double* d_yhat_sum);
+
+/*
+ * Calibration of held-out quantiles by horizon (DESIGN §15): pb200_cv_metrics_device's rows, order, slots and rolling
+ * window rule over two per-row values of each level tau_q = h_levels[q] (host double [n_q], each in [0, 1], n_q in
+ * [1, 32]) with the held-out quantile d_yq[q * n_rows + r] and e = y - yq:
+ *   pinball loss  max(tau e, (tau - 1) e)
+ *   below         1 if y <= yq else 0
+ * The means over the window go to d_pinball / d_share_below [n_q * n_rows] at q * n_rows + slot, with d_out_horizon and
+ * d_valid as pb200_cv_metrics_device's; d_scratch: int64 [n_rows].  One thread per series, no atomics.
+ */
+PB200_API int pb200_cv_quantile_metrics_device(pb200_ctx* ctx, const int64_t* d_horizon, const double* d_y,
+                                               const double* d_yq, int64_t n_rows, int32_t n_q, const double* h_levels,
+                                               const int64_t* d_order, const int64_t* d_srow_off, int64_t n_series,
+                                               double rolling_window, int64_t* d_out_horizon, int64_t* d_scratch,
+                                               double* d_pinball, double* d_share_below, int32_t* d_valid);
 
 #ifdef __cplusplus
 }

@@ -56,7 +56,8 @@ EXPORTS = [
     "pb200_predict_sums_device", "pb200_predict_sums_host", "pb200_make_future_device", "pb200_synchronize", "pb200_objective_host",
     "pb200_fit_trace_host", "pb200_forecast_csv_lengths_device", "pb200_forecast_csv_rows_device", "pb200_forecast_csv_row_host",
     "pb200_cv_plan_counts_device", "pb200_cv_plan_device", "pb200_cv_gather_device", "pb200_cv_metrics_device",
-    "pb200_predict_sums_anchored_device", "pb200_cv_windows_device",
+    "pb200_predict_sums_anchored_device", "pb200_cv_windows_device", "pb200_predict_quantiles_device",
+    "pb200_predict_quantiles_host", "pb200_cv_quantile_metrics_device",
 ]
 CV_ERR_HORIZON, CV_ERR_INITIAL, CV_ERR_FEW = 1, 2, 4
 
@@ -119,6 +120,10 @@ def load() -> C.CDLL:
     lib.pb200_predict_sums_host.restype = C.c_int
     lib.pb200_predict_sums_anchored_device.argtypes = pred_args + [i64, vp, vp, i32, vp, vp, vp, vp, vp, vp, vp]
     lib.pb200_predict_sums_anchored_device.restype = C.c_int
+    lib.pb200_predict_quantiles_device.argtypes = pred_args + [i32, vp, vp]
+    lib.pb200_predict_quantiles_device.restype = C.c_int
+    lib.pb200_predict_quantiles_host.argtypes = pred_args + [i32, vp, vp]
+    lib.pb200_predict_quantiles_host.restype = C.c_int
     lib.pb200_make_future_device.argtypes = [vp, vp, i64, i32, i64, vp]
     lib.pb200_make_future_device.restype = C.c_int
     lib.pb200_objective_host.argtypes = [vp, OP, vp, vp, i32, vp, i64, dbl, dbl, vp, vp, vp, vp]
@@ -141,6 +146,8 @@ def load() -> C.CDLL:
     lib.pb200_cv_metrics_device.restype = C.c_int
     lib.pb200_cv_windows_device.argtypes = [vp, vp, vp, i32, vp, vp, vp, vp, i64, vp, i32, i64, i32, vp, vp, vp, vp, vp]
     lib.pb200_cv_windows_device.restype = C.c_int
+    lib.pb200_cv_quantile_metrics_device.argtypes = [vp, vp, vp, vp, i64, i32, vp, vp, vp, i64, dbl, vp, vp, vp, vp, vp]
+    lib.pb200_cv_quantile_metrics_device.restype = C.c_int
     lib.pb200_synchronize.argtypes = [vp]
     lib.pb200_synchronize.restype = C.c_int
     _lib = lib

@@ -297,6 +297,7 @@ class ForecastBatch:
     components: object = None   # [6, N, H] f64, planes in L.COMPONENTS order (components=True), else None
     trend_lower: object = None  # [N, H] f64 (components=True with intervals), else None
     trend_upper: object = None
+    quantiles: object = None    # [Q, N, H] f64 (predict_quantiles_*), else None
 
     def component(self, name: str):
         """One component plane by its fbprophet column name (trend, multiplicative_terms, additive_terms, yearly, weekly,
@@ -437,6 +438,70 @@ def predict_batch_device(ctx: L.Context, opts: L.Options, fitted: FittedBatch, f
         if sync:
             ctx.synchronize()
     return ForecastBatch(future_ds, yhat, lo, hi, yint, comp, tlo, thi)
+
+
+QUANTILES_MAX = 32
+
+
+def quantile_percentiles(levels) -> np.ndarray:
+    """Levels (fractions in [0, 1], 1 to 32 of them, any order, repeats allowed) as the kernel's percentiles 100 q."""
+    lv = np.asarray(levels, dtype=np.float64)
+    if lv.ndim != 1 or not 1 <= lv.size <= QUANTILES_MAX or not np.all((lv >= 0.0) & (lv <= 1.0)):
+        raise ValueError(f"levels must be 1 to {QUANTILES_MAX} fractions in [0, 1] (got {levels!r})")
+    return np.ascontiguousarray(100.0 * lv)
+
+
+def predict_quantiles_host(ctx: L.Context, opts: L.Options, fitted: FittedBatch, future_ds: np.ndarray, floor, cap,
+                           levels, seed: int = 0, intervals: bool = False) -> ForecastBatch:
+    """pb200_predict_quantiles_host: predict_batch_host's ForecastBatch (the bounds with ``intervals``) and
+    ``quantiles`` [Q, N, H], the percentile 100 q of each point's uncertainty_samples draws for each level q of
+    ``levels`` (DESIGN §15).  The draws are those behind yhat_lower / yhat_upper."""
+    pct = quantile_percentiles(levels)
+    fitted = fitted.to_host()
+    n = fitted.n
+    future_ds = np.ascontiguousarray(future_ds, dtype=np.int64).reshape(n, -1)
+    h = future_ds.shape[1]
+    floor = np.ascontiguousarray(np.broadcast_to(np.asarray(floor, dtype=np.float64), (n,)))
+    cap = np.ascontiguousarray(np.broadcast_to(np.asarray(cap, dtype=np.float64), (n,)))
+    yhat = np.empty((n, h), np.float64)
+    yint = np.empty((n, h), np.int32)
+    lo = np.empty((n, h), np.float64) if intervals else None
+    hi = np.empty((n, h), np.float64) if intervals else None
+    qs = np.empty((pct.size, n, h), np.float64)
+    rc = L.load().pb200_predict_quantiles_host(
+        ctx.handle, C.byref(opts), _np_ptr(np.ascontiguousarray(fitted.params)),
+        _np_ptr(np.ascontiguousarray(fitted.tchange)), _np_ptr(np.ascontiguousarray(fitted.meta_i32)),
+        _np_ptr(np.ascontiguousarray(fitted.meta_i64)), _np_ptr(np.ascontiguousarray(fitted.meta_f64)), n,
+        _np_ptr(future_ds), h, _np_ptr(floor), _np_ptr(cap), int(seed) & (2**64 - 1), _np_ptr(yhat),
+        _np_ptr(lo) if intervals else None, _np_ptr(hi) if intervals else None, _np_ptr(yint), int(pct.size),
+        _np_ptr(pct), _np_ptr(qs))
+    L.check(rc, "pb200_predict_quantiles_host")
+    return ForecastBatch(future_ds, yhat, lo, hi, yint, quantiles=qs)
+
+
+def predict_quantiles_device(ctx: L.Context, opts: L.Options, fitted: FittedBatch, future_ds, floor, cap, levels,
+                             seed: int = 0, intervals: bool = False, sync: bool = True) -> ForecastBatch:
+    """pb200_predict_quantiles_device with torch CUDA tensors; as predict_quantiles_host."""
+    import torch
+    pct = quantile_percentiles(levels)
+    n = fitted.n
+    h = int(future_ds.shape[1])
+    dev = future_ds.device
+    yhat = torch.empty((n, h), dtype=torch.float64, device=dev)
+    yint = torch.empty((n, h), dtype=torch.int32, device=dev)
+    lo = torch.empty((n, h), dtype=torch.float64, device=dev) if intervals else None
+    hi = torch.empty((n, h), dtype=torch.float64, device=dev) if intervals else None
+    qs = torch.empty((pct.size, n, h), dtype=torch.float64, device=dev)
+    torch.cuda.current_stream(dev).synchronize()
+    rc = L.load().pb200_predict_quantiles_device(
+        ctx.handle, C.byref(opts), fitted.params.data_ptr(), fitted.tchange.data_ptr(), fitted.meta_i32.data_ptr(),
+        fitted.meta_i64.data_ptr(), fitted.meta_f64.data_ptr(), n, future_ds.data_ptr(), h, floor.data_ptr(),
+        cap.data_ptr(), int(seed) & (2**64 - 1), yhat.data_ptr(), lo.data_ptr() if intervals else None,
+        hi.data_ptr() if intervals else None, yint.data_ptr(), int(pct.size), _np_ptr(pct), qs.data_ptr())
+    L.check(rc, "pb200_predict_quantiles_device")
+    if sync:
+        ctx.synchronize()
+    return ForecastBatch(future_ds, yhat, lo, hi, yint, quantiles=qs)
 
 
 @dataclass
@@ -715,6 +780,8 @@ class CvResult:
     metrics: Optional[dict] = None
     fitted: Optional[FittedBatch] = None
     windows: Optional["CvWindows"] = None
+    yhat_q: Optional[np.ndarray] = None           # [Q, rows] held-out quantiles (quantiles=levels)
+    quantile_metrics: Optional[dict] = None       # quantile_metrics_device's columns (quantiles with rolling_window)
 
 
 @dataclass
@@ -809,7 +876,7 @@ def cross_validation_device(ctx: L.Context, opts: L.Options, ds_ns, y, offsets_h
                             rolling_window: Optional[float] = None, plan: Optional[CvPlan] = None,
                             keep_fits: bool = False, timings: Optional[dict] = None,
                             _row_budget: Optional[int] = None, grid=None,
-                            aggregate_ns: Optional[int] = None) -> CvResult:
+                            aggregate_ns: Optional[int] = None, quantiles=None) -> CvResult:
     """fbprophet.diagnostics.cross_validation (and, with ``rolling_window``, performance_metrics) for every series of a
     packed batch: ``ds_ns`` / ``y`` CUDA tensors sorted within each series, ``cap`` the float64 CUDA tensor of each
     series' full-history cap.  Per chunk of series: one gather, one pb200_fit_device per full-history seasonality mask
@@ -818,6 +885,10 @@ def cross_validation_device(ctx: L.Context, opts: L.Options, ds_ns, y, offsets_h
     ``grid``: a list of (changepoint_prior_scale, seasonality_prior_scale) pairs.  Every cutoff fit is then made once per
     pair, in the same fit calls (each entry with its own prior scales), and the result's series are the virtual
     ``s * n_grid + g`` (see CvResult): one backtest per grid point for the price of one batch.
+    ``quantiles`` (levels, fractions in [0, 1]): the chunk's predict is pb200_predict_quantiles_device, whose pointwise
+    outputs are pb200_predict_device's; ``CvResult.yhat_q`` holds each held-out row's quantiles and, with
+    ``rolling_window``, ``CvResult.quantile_metrics`` their calibration by horizon (stage ``quantile_metrics``, DESIGN
+    §15).  It does not combine with ``aggregate_ns`` or ``grid``.
     ``aggregate_ns`` (a width W dividing ``horizon_ns``): also the held-out totals per window (c + j W, c + (j + 1) W]
     after each cutoff c, with their metrics, as ``CvResult.windows`` (DESIGN §14).  Every other output is unchanged.
     With intervals the chunk's predict is pb200_predict_sums_anchored_device, whose pointwise outputs are
@@ -858,6 +929,12 @@ def cross_validation_device(ctx: L.Context, opts: L.Options, ds_ns, y, offsets_h
             raise ValueError(f"aggregate_ns must be a positive width that divides the horizon (got {aggregate_ns!r} for "
                              f"a horizon of {int(horizon_ns)} ns)")
     sums = W is not None and intervals and opts.uncertainty_samples > 0
+    levels = None
+    if quantiles is not None:
+        if W is not None or grid is not None:
+            raise ValueError("quantiles do not combine with aggregate_ns or grid")
+        levels = np.asarray(quantiles, dtype=np.float64)
+        quantile_percentiles(levels)
     chunks, he_h, we_h = _cv_chunks(plan, offsets_host, int(_row_budget or CV_ROW_BUDGET), n_grid)
     cap = cap.to(device=dev, dtype=torch.float64)
     pieces = []
@@ -920,6 +997,9 @@ def cross_validation_device(ctx: L.Context, opts: L.Options, ds_ns, y, offsets_h
             flen = torch.from_numpy(win_len.astype(np.int32)).to(dev)
             fcst, ws = predict_sums_anchored_device(ctx, opts, fitted, fut, floor_p, cap_p, W, origins, flen, seed=seed,
                                                     intervals=True, wmax=wmax)
+        elif levels is not None:
+            fcst = predict_quantiles_device(ctx, opts, fitted, fut, floor_p, cap_p, levels, seed=seed,
+                                            intervals=intervals and opts.uncertainty_samples > 0)
         else:
             fcst = predict_batch_device(ctx, opts, fitted, fut, floor_p, cap_p, seed=seed, intervals=intervals)
         lap("predict")
@@ -944,6 +1024,16 @@ def cross_validation_device(ctx: L.Context, opts: L.Options, ds_ns, y, offsets_h
                                              rows["yhat_lower"], rows["yhat_upper"], (s1 - s0) * n_grid, rolling_window)
             met["series"] = met["series"] + v0
             lap("metrics")
+        qpiece = None
+        if levels is not None:
+            yq = fcst.quantiles[:, inv][:, kk, jj]
+            qmet = None
+            if rolling_window is not None:
+                qmet = quantile_metrics_device(ctx, rows["series"] - s0, rows["ds"] - rows["cutoff"], rows["y"], yq, levels,
+                                               s1 - s0, rolling_window)
+                qmet["series"] = qmet["series"] + s0
+                lap("quantile_metrics")
+            qpiece = (yq.cpu().numpy(), qmet)
         wpiece = None
         if W is not None:
             cw = cv_windows_device(ctx, ds_ns, y, plan, d_pairs, fcst.yhat, W, wmax)
@@ -970,7 +1060,7 @@ def cross_validation_device(ctx: L.Context, opts: L.Options, ds_ns, y, offsets_h
             fh = FittedBatch(*(x[inv].cpu().numpy() for x in (fitted.params, fitted.tchange, fitted.meta_i32,
                                                                fitted.meta_i64, fitted.meta_f64)), lay.smax, lay.kmax)
         pieces.append(({k: (v.cpu().numpy() if v is not None else None) for k, v in rows.items()}, met,
-                       fitted.meta_i32[inv, 4].cpu().numpy(), fh, wpiece))
+                       fitted.meta_i32[inv, 4].cpu().numpy(), fh, wpiece, qpiece))
         lap("rows")
     cat = lambda xs: np.concatenate(xs) if xs else None                       # noqa: E731
     rows = {k: cat([p[0][k] for p in pieces]) if (pieces and pieces[0][0][k] is not None) else None
@@ -1010,9 +1100,66 @@ def cross_validation_device(ctx: L.Context, opts: L.Options, ds_ns, y, offsets_h
                                                   (None, None)), 0, rolling_window)
         windows = CvWindows(W, wr["series"], wr["cutoff"], wr["horizon"], wr["points"], wr["y"], wr["yhat"],
                             wr["yhat_lower"], wr["yhat_upper"], wm)
+    yhat_q = qmetrics = None
+    if levels is not None:
+        yhat_q = np.concatenate([p[5][0] for p in pieces], axis=1) if pieces else np.zeros((levels.size, 0))
+        if rolling_window is not None:
+            keys = ("series", "horizon", "level", "pinball", "share_below")
+            qmetrics = ({k: cat([p[5][1][k] for p in pieces]) for k in keys} if pieces else
+                        {k: np.zeros(0, np.int64 if k in ("series", "horizon") else np.float64) for k in keys})
     return CvResult(ps_all * n_grid + g_all, plan.cutoff.cpu().numpy()[ent_all], status, plan.mask[ps_all], rows["series"],
                     rows["ds"], rows["cutoff"], rows["y"], rows["yhat"], rows["yhat_lower"], rows["yhat_upper"], metrics,
-                    fitted_all, windows)
+                    fitted_all, windows, yhat_q, qmetrics)
+
+
+def _metric_slots(series, horizon_ns, n_series: int):
+    """The rows sorted by (series, horizon), stable (two stable sorts: plumbing), the rows per series and their
+    exclusive scan: the row order and slots of the metrics kernels."""
+    import torch
+    dev = series.device
+    o1 = torch.sort(horizon_ns, stable=True).indices
+    o2 = torch.sort(series[o1], stable=True).indices
+    order = o1[o2].contiguous()
+    R = int(series.shape[0])
+    counts = torch.bincount(series, minlength=n_series) if R else torch.zeros(n_series, dtype=torch.int64, device=dev)
+    srow_off = torch.zeros(n_series + 1, dtype=torch.int64, device=dev)
+    srow_off[1:] = torch.cumsum(counts, 0)
+    return order, counts, srow_off
+
+
+def quantile_metrics_device(ctx: L.Context, series, horizon_ns, y, yq, levels, n_series: int,
+                            rolling_window: float = 0.1) -> dict:
+    """Calibration of held-out quantiles per series and horizon (pb200_cv_quantile_metrics_device, DESIGN §15): rows as
+    performance_metrics_device's, ``yq`` [Q, rows] float64 the quantile of each level of ``levels`` (fractions).  Per
+    (series, horizon, level), the rolling-window means of the pinball loss max(q e, (q - 1) e), e = y - yq, and of
+    [y <= yq].  Returns host numpy columns series, horizon, level, pinball, share_below, ordered by (series, horizon,
+    level as given)."""
+    import torch
+    lv = np.ascontiguousarray(np.asarray(levels, dtype=np.float64))
+    quantile_percentiles(lv)
+    if not (0.0 <= float(rolling_window) <= 1.0):
+        raise ValueError(f"rolling_window must be in [0, 1] (got {rolling_window!r})")
+    dev = y.device
+    R, Q = int(y.shape[0]), lv.size
+    order, counts, srow_off = _metric_slots(series, horizon_ns, n_series)
+    out_h, scratch = (torch.empty(R, dtype=torch.int64, device=dev) for _ in range(2))
+    pin, below = (torch.empty((Q, R), dtype=torch.float64, device=dev) for _ in range(2))
+    valid = torch.zeros(R, dtype=torch.int32, device=dev)
+    if R and n_series:
+        h, yy, q = horizon_ns.contiguous(), y.contiguous(), yq.contiguous()
+        torch.cuda.current_stream(dev).synchronize()
+        L.check(L.load().pb200_cv_quantile_metrics_device(
+            ctx.handle, h.data_ptr(), yy.data_ptr(), q.data_ptr(), R, Q, _np_ptr(lv), order.data_ptr(), srow_off.data_ptr(),
+            int(n_series), float(rolling_window), out_h.data_ptr(), scratch.data_ptr(), pin.data_ptr(), below.data_ptr(),
+            valid.data_ptr()), "pb200_cv_quantile_metrics_device")
+        ctx.synchronize()
+    keep = valid.bool()
+    slot_series = torch.repeat_interleave(torch.arange(n_series, device=dev), counts) if R else torch.zeros(0, dtype=torch.int64, device=dev)
+    m = int(keep.sum().item())
+    out = {"series": slot_series[keep].repeat_interleave(Q), "horizon": out_h[keep].repeat_interleave(Q),
+           "level": torch.from_numpy(lv).to(dev).repeat(m), "pinball": pin[:, keep].T.reshape(-1),
+           "share_below": below[:, keep].T.reshape(-1)}
+    return {k: v.cpu().numpy() for k, v in out.items()}
 
 
 def performance_metrics_device(ctx: L.Context, series, horizon_ns, y, yhat, yhat_lower, yhat_upper, n_series: int,
@@ -1027,13 +1174,7 @@ def performance_metrics_device(ctx: L.Context, series, horizon_ns, y, yhat, yhat
         raise ValueError(f"rolling_window must be in [0, 1] (got {rolling_window!r})")
     dev = y.device
     R = int(y.shape[0])
-    # rows sorted by (series, horizon), stable: two stable sorts (plumbing)
-    o1 = torch.sort(horizon_ns, stable=True).indices
-    o2 = torch.sort(series[o1], stable=True).indices
-    order = o1[o2].contiguous()
-    counts = torch.bincount(series, minlength=n_series) if R else torch.zeros(n_series, dtype=torch.int64, device=dev)
-    srow_off = torch.zeros(n_series + 1, dtype=torch.int64, device=dev)
-    srow_off[1:] = torch.cumsum(counts, 0)
+    order, counts, srow_off = _metric_slots(series, horizon_ns, n_series)
     out_h, scratch = (torch.empty(R, dtype=torch.int64, device=dev) for _ in range(2))
     mse, rmse, mae, mape, cov = (torch.empty(R, dtype=torch.float64, device=dev) for _ in range(5))
     valid = torch.zeros(R, dtype=torch.int32, device=dev)

@@ -108,6 +108,7 @@ struct pb200_ctx {
     DevBuf d_comp, d_tlo, d_thi;   // staging of pb200_predict_components_host's planes and trend bounds
     DevBuf d_mc;     // MC workspace
     DevBuf d_sums;   // staging of pb200_predict_sums_host's window outputs
+    DevBuf d_quant;  // staging of pb200_predict_quantiles_host's planes
     int lc0_max = 1 << 30; // PB200_LC0_MAX: longest series on one warp per series, longer ones get four (unset: no limit)
     bool lc_auto = true;   // false when PB200_LC0_MAX pins the CTA width
     bool tab_on = true;    // PB200_NO_TAB=1 disables the seasonal-table variants (A/B runs)
@@ -850,19 +851,40 @@ int check_sum_args(const pb200_options* o, const SumOut& s) {
     return PB200_OK;
 }
 
+// the level arguments of pb200_predict_quantiles_*: n_q percentiles (a host array) and the planes (device pointer in
+// predict_device, host pointer in predict_host)
+struct QuantOut {
+    int32_t n_q;
+    const double* percentiles;
+    double* planes;
+};
+
+// checked before anything is copied or launched
+int check_quant_args(const pb200_options* o, const QuantOut& q) {
+    const int rc = check_mc_opts(o);
+    if (rc) return rc;
+    if (q.n_q < 1 || q.n_q > pb200::MC_QMAX) return fail(PB200_E_ARG, "n_q must be in [1, 32]");
+    if (!q.percentiles || !q.planes) return fail(PB200_E_ARG, "null pointer (percentiles / quantiles)");
+    for (int i = 0; i < q.n_q; ++i)
+        if (!(q.percentiles[i] >= 0.0 && q.percentiles[i] <= 100.0)) return fail(PB200_E_ARG, "percentiles must be in [0, 100]");
+    return PB200_OK;
+}
+
 // pb200_predict_device; d_comp != null: the components instance of predict_kernel, d_tlo / d_thi != null: the
 // trend-bounds instance of mc_kernel; sums != null: mc_sum_kernel after them (it also runs on an empty frame, where
-// every model has no window), its per-model instance when sums->origins != null
+// every model has no window), its per-model instance when sums->origins != null; quant != null: mc_kernel also writes the
+// quantile planes, from the same selection as the bounds
 int predict_device(pb200_ctx* c, const pb200_options* opts, const double* d_params, const double* d_tchange,
                    const int32_t* d_meta_i32, const int64_t* d_meta_i64, const double* d_meta_f64, int64_t n_models,
                    const int64_t* d_future_ds, int32_t horizon, const double* d_floor, const double* d_cap, uint64_t seed,
                    double* d_yhat, double* d_yhat_lower, double* d_yhat_upper, int32_t* d_yhat_int, double* d_comp,
-                   double* d_tlo, double* d_thi, const SumOut* sums = nullptr) {
+                   double* d_tlo, double* d_thi, const SumOut* sums = nullptr, const QuantOut* quant = nullptr) {
     if (!c) return fail(PB200_E_ARG, "ctx is null");
     int rc = check_opts(opts);
     if (rc) return rc;
     if (n_models < 0 || horizon < 0 || n_models > (1LL << 30)) return fail(PB200_E_ARG, "sizes");
     if (sums && (rc = check_sum_args(opts, *sums))) return rc;
+    if (quant && (rc = check_quant_args(opts, *quant))) return rc;
     if (n_models == 0 || (horizon == 0 && !sums)) return PB200_OK;
     if (!d_params || !d_tchange || !d_meta_i32 || !d_meta_i64 || !d_meta_f64 || !d_floor || !d_cap ||
         (horizon > 0 && (!d_future_ds || !d_yhat || !d_yhat_int)))
@@ -900,10 +922,11 @@ int predict_device(pb200_ctx* c, const pb200_options* opts, const double* d_para
         CK(cudaGetLastError());
         c->launches++;
     }
-    if (mc) {
-        rc = pb200::launch_mc(c->stream, c->sms, a, opts->uncertainty_samples, opts->interval_width, seed, d_yhat_lower,
-                              d_yhat_upper, d_tlo, d_thi);
-        if (rc == -1) return fail(PB200_E_ARG, "uncertainty_samples / interval_width out of range");
+    if (mc || (quant && horizon > 0)) {
+        rc = pb200::launch_mc(c->stream, c->sms, a, opts->uncertainty_samples, opts->interval_width, seed,
+                              mc ? d_yhat_lower : nullptr, mc ? d_yhat_upper : nullptr, d_tlo, d_thi, quant ? quant->n_q : 0,
+                              quant ? quant->percentiles : nullptr, quant ? quant->planes : nullptr);
+        if (rc == -1) return fail(PB200_E_ARG, "uncertainty_samples / interval_width / n_q out of range");
         if (rc) return fail(PB200_E_CUDA, "mc kernel launch", cudaGetLastError());
         c->launches++;
     }
@@ -934,10 +957,11 @@ int predict_host(pb200_ctx* c, const pb200_options* opts, const double* h_params
                  const int32_t* h_meta_i32, const int64_t* h_meta_i64, const double* h_meta_f64, int64_t n_models,
                  const int64_t* h_future_ds, int32_t horizon, const double* h_floor, const double* h_cap, uint64_t seed,
                  double* h_yhat, double* h_yhat_lower, double* h_yhat_upper, int32_t* h_yhat_int, double* h_comp,
-                 double* h_tlo, double* h_thi, const SumOut* sums = nullptr) {
+                 double* h_tlo, double* h_thi, const SumOut* sums = nullptr, const QuantOut* quant = nullptr) {
     if (!c) return fail(PB200_E_ARG, "ctx is null");
     int rc = check_opts(opts);
     if (rc) return rc;
+    if (quant && (rc = check_quant_args(opts, *quant))) return rc;
     if (sums) {
         if (n_models < 0 || horizon < 0) return fail(PB200_E_ARG, "sizes");
         if ((rc = check_sum_args(opts, *sums))) return rc;
@@ -983,6 +1007,12 @@ int predict_host(pb200_ctx* c, const pb200_options* opts, const double* h_params
         CK(c->d_hi.reserve(NH * 8));
     }
     if (h_comp) CK(c->d_comp.reserve(NH * 8 * PB200_N_COMPONENTS));
+    QuantOut dquant;
+    if (quant) {
+        CK(c->d_quant.reserve(NH * 8 * (size_t)quant->n_q));
+        dquant = *quant;
+        dquant.planes = (double*)c->d_quant.p;
+    }
     if (h_tlo) {
         CK(c->d_tlo.reserve(NH * 8));
         CK(c->d_thi.reserve(NH * 8));
@@ -1001,7 +1031,7 @@ int predict_host(pb200_ctx* c, const pb200_options* opts, const double* h_params
                         horizon, (const double*)c->d_floor.p, (const double*)c->d_cap.p, seed, (double*)c->d_yhat.p,
                         mc ? (double*)c->d_lo.p : nullptr, mc ? (double*)c->d_hi.p : nullptr, (int32_t*)c->d_yint.p,
                         h_comp ? (double*)c->d_comp.p : nullptr, h_tlo ? (double*)c->d_tlo.p : nullptr,
-                        h_tlo ? (double*)c->d_thi.p : nullptr, sums ? &dsum : nullptr);
+                        h_tlo ? (double*)c->d_thi.p : nullptr, sums ? &dsum : nullptr, quant ? &dquant : nullptr);
     if (rc) return rc;
     if (sums) {
         CK(cudaMemcpyAsync(sums->win_start, dsum.win_start, NW * 8, cudaMemcpyDeviceToHost, st));
@@ -1021,6 +1051,7 @@ int predict_host(pb200_ctx* c, const pb200_options* opts, const double* h_params
         CK(cudaMemcpyAsync(h_yhat_upper, c->d_hi.p, NH * 8, cudaMemcpyDeviceToHost, st));
     }
     if (h_comp) CK(cudaMemcpyAsync(h_comp, c->d_comp.p, NH * 8 * PB200_N_COMPONENTS, cudaMemcpyDeviceToHost, st));
+    if (quant) CK(cudaMemcpyAsync(quant->planes, dquant.planes, NH * 8 * (size_t)quant->n_q, cudaMemcpyDeviceToHost, st));
     if (h_tlo) {
         CK(cudaMemcpyAsync(h_tlo, c->d_tlo.p, NH * 8, cudaMemcpyDeviceToHost, st));
         CK(cudaMemcpyAsync(h_thi, c->d_thi.p, NH * 8, cudaMemcpyDeviceToHost, st));
@@ -1119,6 +1150,30 @@ PB200_API int pb200_predict_sums_host(pb200_ctx* c, const pb200_options* opts, c
                       h_sum_lower, h_sum_upper};
     return predict_host(c, opts, h_params, h_tchange, h_meta_i32, h_meta_i64, h_meta_f64, n_models, h_future_ds, horizon,
                         h_floor, h_cap, seed, h_yhat, h_yhat_lower, h_yhat_upper, h_yhat_int, nullptr, nullptr, nullptr, &s);
+}
+
+PB200_API int pb200_predict_quantiles_device(pb200_ctx* c, const pb200_options* opts, const double* d_params,
+                         const double* d_tchange, const int32_t* d_meta_i32, const int64_t* d_meta_i64,
+                         const double* d_meta_f64, int64_t n_models, const int64_t* d_future_ds, int32_t horizon,
+                         const double* d_floor, const double* d_cap, uint64_t seed, double* d_yhat, double* d_yhat_lower,
+                         double* d_yhat_upper, int32_t* d_yhat_int, int32_t n_q, const double* h_percentiles,
+                         double* d_quantiles) {
+    const QuantOut q = {n_q, h_percentiles, d_quantiles};
+    return predict_device(c, opts, d_params, d_tchange, d_meta_i32, d_meta_i64, d_meta_f64, n_models, d_future_ds, horizon,
+                          d_floor, d_cap, seed, d_yhat, d_yhat_lower, d_yhat_upper, d_yhat_int, nullptr, nullptr, nullptr,
+                          nullptr, &q);
+}
+
+PB200_API int pb200_predict_quantiles_host(pb200_ctx* c, const pb200_options* opts, const double* h_params,
+                       const double* h_tchange, const int32_t* h_meta_i32, const int64_t* h_meta_i64,
+                       const double* h_meta_f64, int64_t n_models, const int64_t* h_future_ds, int32_t horizon,
+                       const double* h_floor, const double* h_cap, uint64_t seed, double* h_yhat, double* h_yhat_lower,
+                       double* h_yhat_upper, int32_t* h_yhat_int, int32_t n_q, const double* h_percentiles,
+                       double* h_quantiles) {
+    const QuantOut q = {n_q, h_percentiles, h_quantiles};
+    return predict_host(c, opts, h_params, h_tchange, h_meta_i32, h_meta_i64, h_meta_f64, n_models, h_future_ds, horizon,
+                        h_floor, h_cap, seed, h_yhat, h_yhat_lower, h_yhat_upper, h_yhat_int, nullptr, nullptr, nullptr,
+                        nullptr, &q);
 }
 
 // ---- forecast CSV rows formatted on the device (csv_kernel.cuh) ----
@@ -1317,6 +1372,47 @@ PB200_API int pb200_cv_metrics_device(pb200_ctx* c, const int64_t* d_horizon, co
     a.out_valid = d_valid;
     const int grid = (int)std::min<int64_t>((n_series + 127) / 128, (int64_t)c->sms * 16);
     pb200::cv::cv_metrics_kernel<<<grid, 128, 0, c->stream>>>(a);
+    CK(cudaGetLastError());
+    c->launches++;
+    return PB200_OK;
+}
+
+PB200_API int pb200_cv_quantile_metrics_device(pb200_ctx* c, const int64_t* d_horizon, const double* d_y,
+                                               const double* d_yq, int64_t n_rows, int32_t n_q, const double* h_levels,
+                                               const int64_t* d_order, const int64_t* d_srow_off, int64_t n_series,
+                                               double rolling_window, int64_t* d_out_horizon, int64_t* d_scratch,
+                                               double* d_pinball, double* d_share_below, int32_t* d_valid) {
+    if (!c) return fail(PB200_E_ARG, "ctx is null");
+    if (n_series < 0 || n_rows < 0) return fail(PB200_E_ARG, "sizes");
+    if (!(rolling_window >= 0.0 && rolling_window <= 1.0)) return fail(PB200_E_ARG, "rolling_window must be in [0, 1]");
+    if (n_q < 1 || n_q > pb200::cv::CV_QMAX) return fail(PB200_E_ARG, "n_q must be in [1, 32]");
+    if (!h_levels) return fail(PB200_E_ARG, "null pointer (levels)");
+    pb200::cv::QuantMetricsArgs a;
+    for (int q = 0; q < n_q; ++q) {
+        if (!(h_levels[q] >= 0.0 && h_levels[q] <= 1.0)) return fail(PB200_E_ARG, "levels must be in [0, 1]");
+        a.level[q] = h_levels[q];
+    }
+    if (n_series == 0) return PB200_OK;
+    if (!d_horizon || !d_y || !d_yq || !d_order || !d_srow_off || !d_out_horizon || !d_scratch || !d_pinball ||
+        !d_share_below || !d_valid)
+        return fail(PB200_E_ARG, "null pointer");
+    CK(cudaSetDevice(c->device));
+    a.horizon = (const long long*)d_horizon;
+    a.y = d_y;
+    a.yq = d_yq;
+    a.n_rows = n_rows;
+    a.nq = n_q;
+    a.order = (const long long*)d_order;
+    a.srow_off = (const long long*)d_srow_off;
+    a.n_series = n_series;
+    a.rolling_window = rolling_window;
+    a.out_h = (long long*)d_out_horizon;
+    a.out_n = (long long*)d_scratch;
+    a.out_pinball = d_pinball;
+    a.out_below = d_share_below;
+    a.out_valid = d_valid;
+    const int grid = (int)std::min<int64_t>((n_series + 127) / 128, (int64_t)c->sms * 16);
+    pb200::cv::cv_quantile_metrics_kernel<<<grid, 128, 0, c->stream>>>(a);
     CK(cudaGetLastError());
     c->launches++;
     return PB200_OK;

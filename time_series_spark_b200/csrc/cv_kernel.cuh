@@ -9,6 +9,8 @@
 //                      relative errors and of the interval coverage.
 //   cv_window_kernel   per gathered entry: the held-out rows' totals over fixed-width windows anchored at the cutoff
 //                      (DESIGN §14), the window rows cv_metrics_kernel then reduces like pointwise rows.
+//   cv_quantile_metrics_kernel  cv_metrics_kernel's trailing-window means of the pinball loss and of [y <= quantile]
+//                      per level of held-out quantiles (DESIGN §15).
 // Every series is one warp (plan, windows) or one thread (metrics) and every sum runs in one fixed order with no
 // floating-point atomics: a series' plan, metrics and windows do not depend on the other series of the batch.
 #pragma once
@@ -265,6 +267,94 @@ __global__ void __launch_bounds__(128) cv_metrics_kernel(const MetricsArgs a) {
             a.out_mae[q] = ae / (double)w;
             a.out_mape[q] = tiny_y ? NAN : ape / (double)w;
             a.out_cov[q] = a.lo ? cv / (double)w : NAN;
+        }
+        for (long long q = r0 + G; q < r1; ++q) a.out_valid[q] = 0;
+    }
+}
+
+// ---- held-out quantiles (DESIGN §15): pinball loss and the share of y at or below the quantile, per level ----
+constexpr int CV_QMAX = 32;
+
+struct QuantMetricsArgs {
+    const long long* horizon;    // [n_rows] ns, as MetricsArgs
+    const double* y;             // [n_rows]
+    const double* yq;            // [nq][n_rows] the held-out quantile of each level
+    long long n_rows;
+    int nq;
+    double level[CV_QMAX];       // tau in [0, 1]
+    const long long* order;      // as MetricsArgs
+    const long long* srow_off;
+    long long n_series;
+    double rolling_window;
+    long long* out_h;            // slots as MetricsArgs
+    long long* out_n;            // scratch
+    double* out_pinball;         // [nq][n_rows]
+    double* out_below;           // [nq][n_rows]
+    int* out_valid;
+};
+
+// cv_metrics_kernel's groups and rolling window over, per level, max(tau e, (tau - 1) e) and [y <= yq]
+__global__ void __launch_bounds__(128) cv_quantile_metrics_kernel(const QuantMetricsArgs a) {
+    for (long long s = blockIdx.x * (long long)blockDim.x + threadIdx.x; s < a.n_series; s += (long long)gridDim.x * blockDim.x) {
+        const long long r0 = a.srow_off[s], r1 = a.srow_off[s + 1], n = r1 - r0;
+        if (n <= 0) continue;
+        long long G = 0;
+        for (long long r = r0; r < r1;) {
+            const long long h = a.horizon[a.order[r]];
+            long long re = r;
+            while (re < r1 && a.horizon[a.order[re]] == h) ++re;
+            const long long g = r0 + G++;
+            a.out_h[g] = h;
+            a.out_n[g] = re - r;
+            for (int q = 0; q < a.nq; ++q) {
+                const double tau = a.level[q];
+                const double* yq = a.yq + (size_t)q * a.n_rows;
+                double pin = 0.0, below = 0.0;
+                for (long long j = r; j < re; ++j) {
+                    const long long i = a.order[j];
+                    const double yv = a.y[i], e = yv - yq[i];
+                    pin += fmax(tau * e, (tau - 1.0) * e);
+                    below += yv <= yq[i] ? 1.0 : 0.0;
+                }
+                a.out_pinball[(size_t)q * a.n_rows + g] = pin;
+                a.out_below[(size_t)q * a.n_rows + g] = below;
+            }
+            r = re;
+        }
+        long long w = (long long)(a.rolling_window * (double)n);
+        if (w < 1) w = 1;
+        if (w > n) w = n;
+        // descending k, as cv_metrics_kernel: slot k is overwritten only once no larger horizon needs its sums
+        for (long long k = G - 1; k >= 0; --k) {
+            long long need = w;
+            long long gl = k;                      // the last group the window reaches
+            for (; gl >= 0; --gl) {
+                const long long c = a.out_n[r0 + gl];
+                if (c >= need) break;
+                need -= c;
+            }
+            a.out_valid[r0 + k] = gl >= 0 ? 1 : 0;
+            for (int q = 0; q < a.nq; ++q) {
+                double* pin = a.out_pinball + (size_t)q * a.n_rows + r0;
+                double* below = a.out_below + (size_t)q * a.n_rows + r0;
+                double sp = 0.0, sb = 0.0;
+                long long nd = w;
+                for (long long g = k; g >= 0 && nd > 0; --g) {
+                    const long long c = a.out_n[r0 + g];
+                    if (c >= nd) {
+                        const double f = (double)nd / (double)c;
+                        sp += pin[g] * f;
+                        sb += below[g] * f;
+                        nd = 0;
+                    } else {
+                        sp += pin[g];
+                        sb += below[g];
+                        nd -= c;
+                    }
+                }
+                pin[k] = sp / (double)w;
+                below[k] = sb / (double)w;
+            }
         }
         for (long long q = r0 + G; q < r1; ++q) a.out_valid[q] = 0;
     }

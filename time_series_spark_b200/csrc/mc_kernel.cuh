@@ -23,6 +23,8 @@
 #include <math.h>
 #include <stdint.h>
 
+#include <algorithm>
+
 #include "predict_kernel.cuh"
 
 namespace pb200 {
@@ -61,16 +63,31 @@ struct DrawState {
     uint32_t cp_ctr;      // counter of the changepoint stream
 };
 
+constexpr int MC_QMAX = 32;                // quantile levels per call (DESIGN §15)
+constexpr int MC_QLEV = MC_QMAX + 2;       // with the two interval bounds
+constexpr int MC_QRANK = 2 * MC_QLEV;      // distinct order statistics read (each level reads i and min(i + 1, n - 1))
+
+// The percentiles a row's selection writes, as order statistics of the sorted draws s: level l is
+// s[rank[ia[l]]] + (s[rank[ib[l]]] - s[rank[ia[l]]]) * frac[l].  Levels [0, nq) are the quantile planes, then (when
+// requested) the lower and the upper interval bound.  mc_args fills it.
+struct McLevels {
+    int nlev, nq;                // nlev = nq + 2 with the bounds
+    int nrank;                   // distinct order statistics, ascending
+    int rank[MC_QRANK];
+    unsigned char ia[MC_QLEV], ib[MC_QLEV];
+    double frac[MC_QLEV];
+};
+
 struct McArgs {
     PredictArgs p;
     int n_samples;
-    int lo_i, hi_i;
-    double lo_f, hi_f;
+    McLevels lv;
     uint64_t seed;
     double* lower;
     double* upper;
     double* tlower;       // trend bounds: written by mc_kernel<LOGI, true> only
     double* tupper;
+    double* planes;       // [nq][n_models * horizon]: the quantile planes (mc_kernel<LOGI, false> only)
 };
 
 __device__ __forceinline__ uint64_t splitmix64(uint64_t z) {
@@ -135,76 +152,16 @@ __device__ __forceinline__ void advance(DrawState& d, const ModelSm& ms, const d
 
 constexpr int MC_CAND = 64;    // candidates kept per histogram bin before falling back to a full sort
 
-// k-th smallest of the n values of `row` (k 0-based) by a 256-bin histogram + exact selection inside
-// the bin that holds rank k.  Returns false if that bin holds more than MC_CAND values -- unless TIES and they are all
-// equal: then every rank in the bin is that value (exact).  Trend draws need it: before a draw's first simulated
-// changepoint its trend is the fitted one, so at early horizons most draws of a point are exactly equal.
+// The order statistics lv.rank[0, nrank) of one row of n values into sel[0, nrank).  One 256-bin histogram, then one
+// candidate gather per distinct bin that holds a target rank: every target rank in that bin is selected from the one
+// candidate set.  Returns 1; 2 for a constant row (sel[0] is then every level's value); 0 when such a bin holds more
+// than MC_CAND values -- unless TIES and they are all equal: then every target rank in the bin is that value (exact).
+// Trend draws need it: before a draw's first simulated changepoint its trend is the fitted one, so at early horizons
+// most draws of a point are exactly equal.  0 also when a value compares with nothing (NaN).  On 0 the caller sorts.
+// hist and tb / trb (per target: its bin, its rank inside the bin) are the warp's scratch.
 template <bool TIES>
-__device__ __forceinline__ bool kth_smallest(const double* row, const int n, const int k, const double mn,
-                                             const double scale, const int* hist, const int base, const int lsum,
-                                             double* cand, int* cnt, const int lane, double& out) {
-    // which lane's 8 bins contain rank k, and which bin
-    int b = -1, rb = 0;
-    if (k >= base && k < base + lsum) {
-        int cum = base;
-        for (int q = 0; q < 8; ++q) {
-            const int c = hist[lane * 8 + q];
-            if (k < cum + c) { b = lane * 8 + q; rb = k - cum; break; }
-            cum += c;
-        }
-    }
-    const unsigned who = __ballot_sync(0xffffffffu, b >= 0);
-    const int src = __ffs(who) - 1;
-    b = __shfl_sync(0xffffffffu, b, src);
-    rb = __shfl_sync(0xffffffffu, rb, src);
-    if (lane == 0) *cnt = 0;
-    __syncwarp();
-    double bmn = INFINITY, bmx = -INFINITY;
-    for (int e = lane; e < n; e += 32) {
-        const double v = row[e];
-        const int bb = min(255, (int)((v - mn) * scale));
-        if (bb == b) {
-            const int pos = atomicAdd(cnt, 1);
-            if (pos < MC_CAND) cand[pos] = v;
-            if (TIES) { bmn = fmin(bmn, v); bmx = fmax(bmx, v); }
-        }
-    }
-    __syncwarp();
-    const int m = *cnt;
-    if (m > MC_CAND) {
-        if (TIES) {
-#pragma unroll
-            for (int o = 16; o >= 1; o >>= 1) {
-                bmn = fmin(bmn, __shfl_xor_sync(0xffffffffu, bmn, o));
-                bmx = fmax(bmx, __shfl_xor_sync(0xffffffffu, bmx, o));
-            }
-            if (bmn == bmx) { out = bmn; return true; }
-        }
-        return false;
-    }
-    // exact selection: the candidate with exactly rb candidates ordered before it
-    double found = 0.0;
-    int have = 0;
-    for (int i = lane; i < m; i += 32) {
-        const double vi = cand[i];
-        int r = 0;
-        for (int j = 0; j < m; ++j) {
-            const double vj = cand[j];
-            r += (vj < vi || (vj == vi && j < i)) ? 1 : 0;
-        }
-        if (r == rb) { found = vi; have = 1; }
-    }
-    const unsigned w2 = __ballot_sync(0xffffffffu, have);
-    out = __shfl_sync(0xffffffffu, found, __ffs(w2) - 1);
-    __syncwarp();
-    return w2 != 0;
-}
-
-// numpy percentile (linear interpolation) at the two interval bounds from the draws of one point
-template <bool TIES>
-__device__ __forceinline__ bool select_quantiles(const double* row, const int n, const int lo_i, const double lo_f,
-                                                 const int hi_i, const double hi_f, int* hist, double* cand, int* cnt,
-                                                 const int lane, double& lo_v, double& hi_v) {
+__device__ __forceinline__ int select_ranks(const double* row, const int n, const McLevels& lv, int* hist, int* tb, int* trb,
+                                            double* cand, int* cnt, const int lane, double* sel) {
     double mn = INFINITY, mx = -INFINITY;
     for (int e = lane; e < n; e += 32) { const double v = row[e]; mn = fmin(mn, v); mx = fmax(mx, v); }
 #pragma unroll
@@ -213,8 +170,12 @@ __device__ __forceinline__ bool select_quantiles(const double* row, const int n,
         mx = fmax(mx, __shfl_xor_sync(0xffffffffu, mx, o));
     }
     if (!(mx > mn) || !isfinite(mx - mn)) {
-        if (mx == mn) { lo_v = hi_v = mn; return true; }
-        return false;
+        if (mx == mn) {
+            if (lane == 0) sel[0] = mn;
+            __syncwarp();
+            return 2;
+        }
+        return 0;
     }
     const double scale = 256.0 / (mx - mn);
     for (int q = 0; q < 8; ++q) hist[lane * 8 + q] = 0;
@@ -229,24 +190,70 @@ __device__ __forceinline__ bool select_quantiles(const double* row, const int n,
         const int t = __shfl_up_sync(0xffffffffu, inc, o);
         if (lane >= o) inc += t;
     }
-    const int base = inc - lsum;
-    double v[4];
-    const int ranks[4] = {lo_i, min(lo_i + 1, n - 1), hi_i, min(hi_i + 1, n - 1)};
-    for (int q = 0; q < 4; ++q) {
-        if (q > 0 && ranks[q] == ranks[q - 1]) { v[q] = v[q - 1]; continue; }
-        if (!kth_smallest<TIES>(row, n, ranks[q], mn, scale, hist, base, lsum, cand, cnt, lane, v[q])) return false;
+    // the histogram becomes the first rank of each bin; a target's bin is the last one starting at or before it
+    int cum = inc - lsum;
+    for (int q = 0; q < 8; ++q) { const int c = hist[lane * 8 + q]; hist[lane * 8 + q] = cum; cum += c; }
+    __syncwarp();
+    for (int t = lane; t < lv.nrank; t += 32) {
+        const int k = lv.rank[t];
+        int lo = 0, hi = 255;
+        while (lo < hi) {
+            const int mid = (lo + hi + 1) >> 1;
+            if (hist[mid] <= k) lo = mid; else hi = mid - 1;
+        }
+        tb[t] = lo;
+        trb[t] = k - hist[lo];
     }
-    lo_v = v[0] + (v[1] - v[0]) * lo_f;
-    hi_v = v[2] + (v[3] - v[2]) * hi_f;
-    return true;
+    __syncwarp();
+    for (int t0 = 0; t0 < lv.nrank;) {
+        const int b = tb[t0];
+        int t1 = t0 + 1;
+        while (t1 < lv.nrank && tb[t1] == b) ++t1;
+        if (lane == 0) *cnt = 0;
+        __syncwarp();
+        double bmn = INFINITY, bmx = -INFINITY;
+        for (int e = lane; e < n; e += 32) {
+            const double v = row[e];
+            if (min(255, (int)((v - mn) * scale)) == b) {
+                const int pos = atomicAdd(cnt, 1);
+                if (pos < MC_CAND) cand[pos] = v;
+                if (TIES) { bmn = fmin(bmn, v); bmx = fmax(bmx, v); }
+            }
+        }
+        __syncwarp();
+        const int m = *cnt;
+        if (m > MC_CAND) {
+            if (!TIES) return 0;
+#pragma unroll
+            for (int o = 16; o >= 1; o >>= 1) {
+                bmn = fmin(bmn, __shfl_xor_sync(0xffffffffu, bmn, o));
+                bmx = fmax(bmx, __shfl_xor_sync(0xffffffffu, bmx, o));
+            }
+            if (bmn != bmx) return 0;
+            for (int t = t0 + lane; t < t1; t += 32) sel[t] = bmn;
+        } else {
+            // the candidate with exactly r candidates ordered before it is the bin's r-th smallest
+            int found = 0;
+            for (int i = lane; i < m; i += 32) {
+                const double vi = cand[i];
+                int r = 0;
+                for (int j = 0; j < m; ++j) {
+                    const double vj = cand[j];
+                    r += (vj < vi || (vj == vi && j < i)) ? 1 : 0;
+                }
+                for (int t = t0; t < t1; ++t)
+                    if (trb[t] == r) { sel[t] = vi; ++found; }
+            }
+            if (__reduce_add_sync(0xffffffffu, found) != t1 - t0) return 0;
+        }
+        __syncwarp();
+        t0 = t1;
+    }
+    return 1;
 }
 
-// numpy's two percentiles of one row of draws: select_quantiles, or -- when a histogram bin is too crowded for it -- a
-// full bitonic sort of the row (all MC_NP slots: the padding draws hold INFINITY and sort to the end)
-template <bool TIES>
-__device__ __forceinline__ void row_quantiles(double* row, const McArgs& a, int* hist, double* cand, int* cnt,
-                                              const int lane, double& lo_v, double& hi_v) {
-    if (select_quantiles<TIES>(row, a.n_samples, a.lo_i, a.lo_f, a.hi_i, a.hi_f, hist, cand, cnt, lane, lo_v, hi_v)) return;
+// ascending bitonic sort of one row's MC_NP slots by one warp
+__device__ __forceinline__ void sort_row(double* row, const int lane) {
     for (int k = 2; k <= MC_NP; k <<= 1) {
         for (int j = k >> 1; j > 0; j >>= 1) {
             for (int e = lane; e < MC_NP / 2; e += 32) {
@@ -260,10 +267,50 @@ __device__ __forceinline__ void row_quantiles(double* row, const McArgs& a, int*
             __syncwarp();
         }
     }
-    const double l0 = row[a.lo_i], l1 = row[min(a.lo_i + 1, a.n_samples - 1)];
-    const double u0 = row[a.hi_i], u1 = row[min(a.hi_i + 1, a.n_samples - 1)];
-    lo_v = l0 + (l1 - l0) * a.lo_f;
-    hi_v = u0 + (u1 - u0) * a.hi_f;
+}
+
+// Per-warp scratch of the selection, carved from the dynamic shared memory after the [MC_TILE][MC_NP] rows.
+struct SelScratch {
+    double* cand;    // [MC_CAND]
+    int* hist;       // [256]
+    int* cnt;
+    double* sel;     // [MC_QRANK]
+    int* tb;         // [MC_QRANK]
+    int* trb;        // [MC_QRANK]
+};
+
+constexpr int MC_WARPS = MC_THREADS / 32;
+constexpr size_t MC_SMEM = (size_t)MC_TILE * MC_NP * 8 + (size_t)MC_WARPS * (MC_CAND * 8 + MC_QRANK * 16 + 256 * 4 + 4) + 16;
+
+__device__ __forceinline__ SelScratch sel_scratch(unsigned char* smem, const int warp) {
+    double* rows_end = (double*)smem + MC_TILE * MC_NP;
+    double* cand = rows_end;                                       // [MC_WARPS][MC_CAND]
+    double* sel = cand + MC_WARPS * MC_CAND;                       // [MC_WARPS][MC_QRANK]
+    int* hist = (int*)(sel + MC_WARPS * MC_QRANK);                 // [MC_WARPS][256]
+    int* tb = hist + MC_WARPS * 256;                               // [MC_WARPS][MC_QRANK]
+    int* trb = tb + MC_WARPS * MC_QRANK;
+    int* cnt = trb + MC_WARPS * MC_QRANK;                          // [MC_WARPS]
+    return {cand + warp * MC_CAND, hist + warp * 256, cnt + warp, sel + warp * MC_QRANK, tb + warp * MC_QRANK,
+            trb + warp * MC_QRANK};
+}
+
+// Every level of lv over one row of n draws (numpy's linear-interpolation percentiles): select_ranks, or -- when a
+// histogram bin is too crowded for it -- a full bitonic sort of the row (all MC_NP slots: the padding draws hold
+// INFINITY and sort to the end).  put(l, v) receives level l's value; the warp's lanes take levels l, l + 32, ...
+template <bool TIES, class Put>
+__device__ __forceinline__ void row_levels(double* row, const int n, const McLevels& lv, const SelScratch& w, const int lane,
+                                           Put&& put) {
+    const int got = select_ranks<TIES>(row, n, lv, w.hist, w.tb, w.trb, w.cand, w.cnt, lane, w.sel);
+    if (got == 0) {
+        sort_row(row, lane);
+        for (int t = lane; t < lv.nrank; t += 32) w.sel[t] = row[lv.rank[t]];
+        __syncwarp();
+    }
+    for (int l = lane; l < lv.nlev; l += 32) {
+        const double v0 = w.sel[lv.ia[l]], v1 = w.sel[lv.ib[l]];
+        put(l, got == 2 ? w.sel[0] : v0 + (v1 - v0) * lv.frac[l]);
+    }
+    __syncwarp();
 }
 
 // What a CTA does for a model before its first point: Tmax = max t over the whole frame, the model's Philox key, and
@@ -335,24 +382,31 @@ __global__ void __launch_bounds__(MC_THREADS, 1) mc_kernel(const McArgs a) {
     constexpr int TILE = TREND ? MC_TILE / 2 : MC_TILE;
     extern __shared__ __align__(16) unsigned char mc_smem[];
     double* rows = (double*)mc_smem;                       // [MC_TILE][MC_NP]
-    double* cand = rows + MC_TILE * MC_NP;                 // [MC_THREADS/32][MC_CAND]
-    int* hist = (int*)(cand + (MC_THREADS / 32) * MC_CAND);   // [MC_THREADS/32][256]
-    int* cnt = hist + (MC_THREADS / 32) * 256;             // [MC_THREADS/32]
+    const SelScratch sw = sel_scratch(mc_smem, threadIdx.x >> 5);
     __shared__ ModelSm ms;
     __shared__ double seas[MC_TILE], tt[MC_TILE];
     __shared__ double red_t[MC_THREADS / 32];
     __shared__ uint64_t key_sm;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int H = a.p.horizon;
+    const size_t NH = (size_t)a.p.n_models * H;
+    const McLevels& lv = a.lv;
+    // level l of point i: a quantile plane, or (the last two levels) the yhat bounds -- the trend bounds for trend rows
+    auto out = [&](const int l, const size_t i, const bool trend) -> double& {
+        if (l < lv.nq) return a.planes[(size_t)l * NH + i];
+        if (TREND && trend) return l == lv.nq ? a.tlower[i] : a.tupper[i];
+        return l == lv.nq ? a.lower[i] : a.upper[i];
+    };
     for (int model = blockIdx.x; model < a.p.n_models; model += gridDim.x) {
         __syncthreads();
         load_model(ms, a.p, model, tid, MC_THREADS);
         const size_t base = (size_t)model * H;
         if (ms.status < 0) {
-            for (int h = tid; h < H; h += MC_THREADS) {
-                a.lower[base + h] = NAN; a.upper[base + h] = NAN;
-                if (TREND) { a.tlower[base + h] = NAN; a.tupper[base + h] = NAN; }
-            }
+            for (int l = 0; l < lv.nlev; ++l)
+                for (int h = tid; h < H; h += MC_THREADS) {
+                    out(l, base + h, false) = NAN;
+                    if (TREND) out(l, base + h, true) = NAN;
+                }
             continue;
         }
         Philox ph;
@@ -394,19 +448,10 @@ __global__ void __launch_bounds__(MC_THREADS, 1) mc_kernel(const McArgs a) {
             __syncthreads();
             // ---- percentiles: warp w selects the order statistics of row w (point pt of the tile) ----
             const int pt = TREND ? (warp & (TILE - 1)) : warp;
-            if (pt < np) {
-                double lo_v, hi_v;
-                row_quantiles<TREND>(rows + warp * MC_NP, a, hist + warp * 256, cand + warp * MC_CAND, cnt + warp, lane, lo_v, hi_v);
-                if (lane == 0) {
-                    if (!TREND || warp < TILE) {
-                        a.lower[base + h0 + pt] = lo_v;
-                        a.upper[base + h0 + pt] = hi_v;
-                    } else {
-                        a.tlower[base + h0 + pt] = lo_v;
-                        a.tupper[base + h0 + pt] = hi_v;
-                    }
-                }
-            }
+            if (pt < np)
+                row_levels<TREND>(rows + warp * MC_NP, a.n_samples, lv, sw, lane, [&](const int l, const double v) {
+                    out(l, base + h0 + pt, TREND && warp >= TILE) = v;
+                });
             __syncthreads();
         }
     }
@@ -449,9 +494,7 @@ template <bool LOGI, bool PER_MODEL>
 __global__ void __launch_bounds__(MC_THREADS, 1) mc_sum_kernel(const McSumArgs a) {
     extern __shared__ __align__(16) unsigned char mc_smem[];
     double* rows = (double*)mc_smem;                       // [MC_TILE][MC_NP], as mc_kernel
-    double* cand = rows + MC_TILE * MC_NP;
-    int* hist = (int*)(cand + (MC_THREADS / 32) * MC_CAND);
-    int* cnt = hist + (MC_THREADS / 32) * 256;
+    const SelScratch sw = sel_scratch(mc_smem, threadIdx.x >> 5);
     __shared__ ModelSm ms;
     __shared__ double seas[MC_SUM_TILE], tt[MC_SUM_TILE], yh_t[MC_SUM_TILE];
     __shared__ long long win[MC_SUM_TILE];
@@ -479,12 +522,10 @@ __global__ void __launch_bounds__(MC_THREADS, 1) mc_sum_kernel(const McSumArgs a
             auto select_rows = [&](const int n) {
                 __syncthreads();
                 const int wi = nw - n + warp;
-                if (warp < n && wi < a.wmax) {
-                    double lo_v, hi_v;
-                    row_quantiles<false>(rows + warp * MC_NP, mc, hist + warp * 256, cand + warp * MC_CAND, cnt + warp, lane,
-                                         lo_v, hi_v);
-                    if (lane == 0) { mc.lower[wbase + wi] = lo_v; mc.upper[wbase + wi] = hi_v; }
-                }
+                if (warp < n && wi < a.wmax)
+                    row_levels<false>(rows + warp * MC_NP, mc.n_samples, mc.lv, sw, lane, [&](const int l, const double v) {
+                        (l == 0 ? mc.lower : mc.upper)[wbase + wi] = v;
+                    });
                 __syncthreads();
             };
             auto close_window = [&]() {
@@ -555,8 +596,6 @@ __global__ void __launch_bounds__(MC_THREADS, 1) mc_sum_kernel(const McSumArgs a
     }
 }
 
-constexpr size_t MC_SMEM = (size_t)MC_TILE * MC_NP * 8 + (size_t)(MC_THREADS / 32) * (MC_CAND * 8 + 256 * 4 + 4) + 16;
-
 template <bool LOGI, bool TREND>
 cudaError_t launch_mc_inst(cudaStream_t st, int grid, size_t smem, const McArgs& a) {
     const cudaError_t e = cudaFuncSetAttribute(mc_kernel<LOGI, TREND>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
@@ -574,30 +613,58 @@ cudaError_t launch_mc_sum_inst(cudaStream_t st, int grid, const McSumArgs& a) {
     return cudaGetLastError();
 }
 
-// the sample count, the ranks of the two percentiles among the sorted draws, the seed.  False: sample count or interval
-// width out of range
-inline bool mc_args(McArgs& a, const PredictArgs& p, int n_samples, double width, uint64_t seed) {
-    if (n_samples < 2 || n_samples > MC_NP || !(width >= 0.0 && width <= 1.0)) return false;
+// the sample count, the levels (McLevels: the nq percentiles pct[0, nq), each in [0, 100], then with `bounds` the
+// interval's 100 (1 -+ width) / 2), the seed.  A level's rank and fraction are x = p / 100.0 * (n_samples - 1),
+// i = floor(x), f = x - floor(x), so a plane at a bound's percentile is that bound.  False: sample count, interval width
+// or level count out of range
+inline bool mc_args(McArgs& a, const PredictArgs& p, int n_samples, double width, uint64_t seed, bool bounds = true,
+                    int nq = 0, const double* pct = nullptr) {
+    if (n_samples < 2 || n_samples > MC_NP || !(width >= 0.0 && width <= 1.0) || nq < 0 || nq > MC_QMAX) return false;
     a.p = p;
     a.n_samples = n_samples;
+    McLevels& lv = a.lv;
+    lv.nq = nq;
+    lv.nlev = nq + (bounds ? 2 : 0);
     const double lower_p = 100.0 * (1.0 - width) / 2.0, upper_p = 100.0 * (1.0 + width) / 2.0;
-    const double li = lower_p / 100.0 * (n_samples - 1), ui = upper_p / 100.0 * (n_samples - 1);
-    a.lo_i = (int)floor(li); a.lo_f = li - floor(li);
-    a.hi_i = (int)floor(ui); a.hi_f = ui - floor(ui);
+    int r0[MC_QLEV], r1[MC_QLEV];
+    for (int l = 0; l < lv.nlev; ++l) {
+        const double pl = l < nq ? pct[l] : (l == nq ? lower_p : upper_p);
+        const double x = pl / 100.0 * (n_samples - 1);
+        r0[l] = (int)floor(x);
+        r1[l] = r0[l] + 1 < n_samples - 1 ? r0[l] + 1 : n_samples - 1;
+        lv.frac[l] = x - floor(x);
+    }
+    int rk[MC_QRANK];
+    int nr = 0;
+    for (int l = 0; l < lv.nlev; ++l) { rk[nr++] = r0[l]; rk[nr++] = r1[l]; }
+    std::sort(rk, rk + nr);
+    lv.nrank = (int)(std::unique(rk, rk + nr) - rk);
+    for (int t = 0; t < MC_QRANK; ++t) lv.rank[t] = t < lv.nrank ? rk[t] : 0;
+    for (int l = 0; l < MC_QLEV; ++l) {
+        lv.ia[l] = l < lv.nlev ? (unsigned char)(std::lower_bound(rk, rk + lv.nrank, r0[l]) - rk) : 0;
+        lv.ib[l] = l < lv.nlev ? (unsigned char)(std::lower_bound(rk, rk + lv.nrank, r1[l]) - rk) : 0;
+        if (l >= lv.nlev) lv.frac[l] = 0.0;
+    }
     a.seed = seed;
-    a.lower = a.upper = a.tlower = a.tupper = nullptr;
+    a.lower = a.upper = a.tlower = a.tupper = a.planes = nullptr;
     return true;
 }
 
-// returns 0 ok, -1 sample count or interval width out of range, 1 CUDA error.  tlower / tupper: trend bounds, or both null
+// returns 0 ok, -1 sample count, interval width or level count out of range, 1 CUDA error.  lower / upper: the bounds, or
+// both null; tlower / tupper: trend bounds (with the bounds), or both null; nq > 0: the quantile planes at the percentiles
+// pct [nq] (not with the trend bounds)
 inline int launch_mc(cudaStream_t st, int sms, const PredictArgs& p, int n_samples, double width, uint64_t seed,
-                     double* lower, double* upper, double* tlower = nullptr, double* tupper = nullptr) {
+                     double* lower, double* upper, double* tlower = nullptr, double* tupper = nullptr, int nq = 0,
+                     const double* pct = nullptr, double* planes = nullptr) {
     McArgs a;
-    if (!mc_args(a, p, n_samples, width, seed)) return -1;
+    const bool bounds = lower && upper;
+    if ((!bounds && nq == 0) || (tlower && (!bounds || nq > 0))) return -1;
+    if (!mc_args(a, p, n_samples, width, seed, bounds, nq, pct)) return -1;
     a.lower = lower;
     a.upper = upper;
     a.tlower = tlower;
     a.tupper = tupper;
+    a.planes = planes;
     const bool trend = tlower && tupper;
     const int grid = p.n_models < sms ? p.n_models : sms;
     const bool logi = p.growth == PB200_GROWTH_LOGISTIC;

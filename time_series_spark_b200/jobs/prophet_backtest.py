@@ -15,9 +15,14 @@ Keys (``backtest.*``):
   aggregate          a fixed-width duration W dividing the horizon ('1h', '8h', '1D'): also the held-out totals per
                      window (c + j W, c + (j + 1) W] after each cutoff c and their metrics by horizon (j + 1) W, with
                      intervals the coverage of the totals' joint-draw intervals (DESIGN §14); needs io.window_metrics
+  quantiles          a list of 1 to 32 levels in [0, 1]: the held-out quantiles of each level from uncertainty_samples
+                     draws (with or without intervals) and their pinball loss and share of y at or below them by
+                     horizon (DESIGN §15); needs io.quantile_metrics, not with aggregate
 Outputs (parquet, one part file per rank):
   io.metrics          series_id, dim_id, horizon duration[ns], mse, rmse, mae, mape[, coverage]
-  io.cv_rows          (optional) series_id, dim_id, ds, cutoff, y, yhat[, yhat_lower, yhat_upper]
+  io.cv_rows          (optional) series_id, dim_id, ds, cutoff, y, yhat[, yhat_lower, yhat_upper][, yhat_q<level>...]
+  io.quantile_metrics (with quantiles) series_id, dim_id, horizon duration[ns], quantile, pinball_loss, share_below: one
+                      row per (horizon, level)
   io.window_metrics   (with aggregate) series_id, dim_id, horizon duration[ns], mse, rmse, mae, mape[, coverage]
   io.window_rows      (optional, with aggregate) series_id, dim_id, cutoff, horizon, window_points, y, yhat[,
                       yhat_lower, yhat_upper]
@@ -37,6 +42,7 @@ from .. import batched
 from .. import dist as pdist
 from ..pack import pack_groups_cuda
 from .prophet_modeler import ProphetModeler, get_context, options_from_config
+from .prophet_scorer import quantile_column, quantile_levels
 
 
 def _duration_ns(key: str, value) -> int:
@@ -69,15 +75,24 @@ def backtest_spec_from_config(config) -> dict:
     intervals = bool(b.get("intervals", False))
     spec = {"horizon": horizon, "period": period, "initial": initial, "rolling_window": rw, "intervals": intervals,
             "uncertainty_samples": 0, "interval_width": 0.8, "seed": int(b.get("seed", 0))}
+    levels = quantile_levels(b, "backtest.quantiles")
     if intervals:
         width = float(b.get("interval_width", 0.8))
         if not (0.0 <= width <= 1.0):
             raise ValueError(f"backtest.interval_width must be in [0, 1] (got {b.get('interval_width')!r})")
+        spec["interval_width"] = width
+    if intervals or levels is not None:
         ns = int(b.get("uncertainty_samples", 1000))
         if not (2 <= ns <= 1024):
             raise ValueError(f"backtest.uncertainty_samples must be in [2, 1024] (got {b.get('uncertainty_samples')!r})")
-        spec["interval_width"], spec["uncertainty_samples"] = width, ns
+        spec["uncertainty_samples"] = ns
     spec["aggregate"] = _aggregate_width(config, b, horizon)
+    if levels is not None:
+        if spec["aggregate"] is not None:
+            raise ValueError("backtest.quantiles cannot be combined with backtest.aggregate")
+        if not (config.get("io", {}) or {}).get("quantile_metrics"):
+            raise ValueError("backtest.quantiles needs io.quantile_metrics, the directory the quantile metrics are written to")
+    spec["quantiles"] = levels
     return spec
 
 
@@ -169,9 +184,30 @@ def assemble_window_outputs(series_id, dim_id, res: batched.CvResult, with_rows:
     return metrics, rows
 
 
-def assemble_outputs(series_id, dim_id, res: batched.CvResult, y_dtype, with_rows: bool = True):
+QUANTILE_METRICS_SCHEMA = pa.schema([("series_id", pa.int32()), ("dim_id", pa.int32()), ("horizon", pa.duration("ns")),
+                                     ("quantile", pa.float64()), ("pinball_loss", pa.float64()),
+                                     ("share_below", pa.float64())])
+
+
+def quantile_metrics_table(series_id, dim_id, res: batched.CvResult) -> pa.Table:
+    """io.quantile_metrics of a CvResult made with quantiles: one row per (series, horizon, level); the same failed-fit
+    rule as assemble_outputs (which prints the lines)."""
+    failed = _failed_series(series_id, dim_id, res, announce=False)
+    m = res.quantile_metrics
+    keep = ~failed[m["series"]]
+    ms = m["series"][keep]
+    return pa.table({"series_id": pa.array(np.asarray(series_id)[ms], pa.int32()),
+                     "dim_id": pa.array(np.asarray(dim_id)[ms], pa.int32()),
+                     "horizon": pa.array(m["horizon"][keep], pa.duration("ns")),
+                     "quantile": pa.array(m["level"][keep], pa.float64()),
+                     "pinball_loss": pa.array(m["pinball"][keep], pa.float64()),
+                     "share_below": pa.array(m["share_below"][keep], pa.float64())}, schema=QUANTILE_METRICS_SCHEMA)
+
+
+def assemble_outputs(series_id, dim_id, res: batched.CvResult, y_dtype, with_rows: bool = True, levels=None):
     """Metrics (and row) tables of a CvResult.  A series with a failed cutoff fit (status < 0) -- where fbprophet's
-    cross_validation would raise -- gets no row in either table, and a printed line names it and the cutoff."""
+    cross_validation would raise -- gets no row in either table, and a printed line names it and the cutoff.  ``levels``
+    (the CvResult made with them): the rows get a yhat_q<level> column per level."""
     failed = _failed_series(series_id, dim_id, res)
     metrics = _metrics_table(series_id, dim_id, res.metrics, failed)
     rows = None
@@ -187,6 +223,8 @@ def assemble_outputs(series_id, dim_id, res: batched.CvResult, y_dtype, with_row
         if res.yhat_lower is not None:
             rc["yhat_lower"] = pa.array(res.yhat_lower[keep], pa.float64())
             rc["yhat_upper"] = pa.array(res.yhat_upper[keep], pa.float64())
+        for q, lv in enumerate(levels or ()):
+            rc[quantile_column(lv)] = pa.array(res.yhat_q[q][keep], pa.float64())
         rows = pa.table(rc)
     return metrics, rows
 
@@ -199,6 +237,7 @@ class ProphetBacktester:
         self.config = config
         self.rank_local_input = False
         self.window_outputs = None     # (window metrics, window rows or None) with backtest.aggregate
+        self.quantile_metrics = None   # with backtest.quantiles
 
     def read_input_dataframe(self, spark=None):
         reader = ProphetModeler(self.config)
@@ -227,6 +266,7 @@ class ProphetBacktester:
         io = self.config.get("io", {}) or {}
         with_rows = bool(io.get("cv_rows"))
         W = spec["aggregate"]
+        levels = spec["quantiles"]
         if pk.n == 0:
             empty_metrics = lambda: dict({k: np.zeros(0, np.int64 if k in ("series", "horizon") else np.float64)  # noqa: E731
                                           for k in ("series", "horizon", "mse", "rmse", "mae", "mape")},
@@ -240,7 +280,11 @@ class ProphetBacktester:
                 res.windows = batched.CvWindows(W, *(np.zeros(0, np.int64),) * 3, np.zeros(0, np.int32), np.zeros(0),
                                                 np.zeros(0), iv, iv, empty_metrics())
                 self.window_outputs = assemble_window_outputs(pk.series_id, pk.dim_id, res, bool(io.get("window_rows")))
-            return assemble_outputs(pk.series_id, pk.dim_id, res, np.dtype(str(pk.y.dtype).replace("torch.", "")), with_rows)
+            if levels is not None:
+                res.yhat_q = np.zeros((len(levels), 0))
+                self.quantile_metrics = QUANTILE_METRICS_SCHEMA.empty_table()
+            return assemble_outputs(pk.series_id, pk.dim_id, res, np.dtype(str(pk.y.dtype).replace("torch.", "")), with_rows,
+                                    levels)
         ds, y = pk.ds.contiguous(), pk.y.contiguous()
         short = np.diff(pk.offsets) < 2
         if np.any(short):
@@ -255,26 +299,31 @@ class ProphetBacktester:
         print(f"Backtesting {pk.n} series at {plan.n_pairs} cutoffs")
         res = batched.cross_validation_device(ctx, opts, ds, y, pk.offsets, floor, cap, spec["horizon"], spec["period"],
                                               spec["initial"], intervals=spec["intervals"], seed=spec["seed"],
-                                              rolling_window=spec["rolling_window"], plan=plan, aggregate_ns=W)
+                                              rolling_window=spec["rolling_window"], plan=plan, aggregate_ns=W,
+                                              quantiles=levels)
         for code, msg in ((L.ST_CAP_LE_FLOOR, "cap must be greater than floor (which defaults to 0)."),
                           (L.ST_BAD_INPUT, "Found non-finite y or a zero time span in a series.")):
             hit = np.zeros(pk.n, bool)
             hit[res.pair_series[res.pair_status == code]] = True
             if hit.any():
                 raise ValueError(msg + _who(pk.series_id, pk.dim_id, hit))
-        out = assemble_outputs(pk.series_id, pk.dim_id, res, np.dtype(str(y.dtype).replace("torch.", "")), with_rows)
+        out = assemble_outputs(pk.series_id, pk.dim_id, res, np.dtype(str(y.dtype).replace("torch.", "")), with_rows,
+                               levels)
+        if levels is not None:
+            self.quantile_metrics = quantile_metrics_table(pk.series_id, pk.dim_id, res)
         if W is not None:
             self.window_outputs = assemble_window_outputs(pk.series_id, pk.dim_id, res, bool(io.get("window_rows")))
         print(f"Backtest: {out[0].num_rows} metrics rows in {time.time() - t0:.1f} s")
         return out
 
     def persist(self, metrics: pa.Table, rows) -> None:
-        """Parquet part file per rank under io.metrics (and io.cv_rows, and with backtest.aggregate io.window_metrics
-        and io.window_rows)."""
+        """Parquet part file per rank under io.metrics (and io.cv_rows, with backtest.aggregate io.window_metrics and
+        io.window_rows, with backtest.quantiles io.quantile_metrics)."""
         io = self.config["io"]
         rank = pdist.world()[0]
         wm, wr = self.window_outputs or (None, None)
-        for key, tbl in (("metrics", metrics), ("cv_rows", rows), ("window_metrics", wm), ("window_rows", wr)):
+        for key, tbl in (("metrics", metrics), ("cv_rows", rows), ("window_metrics", wm), ("window_rows", wr),
+                         ("quantile_metrics", self.quantile_metrics)):
             if tbl is None or not io.get(key):
                 continue
             pdist.prepare_output_dir(io[key])

@@ -15,7 +15,9 @@ computes yhat_lower/yhat_upper inside Prophet.predict and drops them at :86; set
 component columns ``trend, yearly, weekly, daily, multiplicative_terms, additive_terms``, and ``trend_lower`` /
 ``trend_upper`` with intervals -- DESIGN §12), ``forecast.aggregate`` (a fixed-width duration such as ``'1D'``: also
 write, to ``io.aggregates``, the forecast total of every such window of every model with the interval of the total from
-the joint draws -- DESIGN §13) and ``forecast.aggregate_origin`` (where window 0 starts, default 1970-01-01).
+the joint draws -- DESIGN §13), ``forecast.aggregate_origin`` (where window 0 starts, default 1970-01-01) and
+``forecast.quantiles`` (a list of 1 to 32 levels in [0, 1]: one float64 column ``yhat_q<level>`` per level, the
+percentile 100 level of the point's ``uncertainty_samples`` draws -- DESIGN §15).
 """
 from __future__ import annotations
 
@@ -56,6 +58,31 @@ def _want_components(fc) -> bool:
     return bool(v)
 
 
+def quantile_levels(section: dict, key: str):
+    """``<section>.quantiles`` checked (``key`` is its full name for the messages): None without it, else the list of
+    levels, 1 to 32 numbers in [0, 1], whose column names ``quantile_column`` are distinct."""
+    v = section.get("quantiles")
+    if v is None:
+        return None
+    if not isinstance(v, (list, tuple)) or not 1 <= len(v) <= batched.QUANTILES_MAX:
+        raise ValueError(f"{key} must be a list of 1 to {batched.QUANTILES_MAX} levels in [0, 1] (got {v!r})")
+    levels = []
+    for q in v:
+        if isinstance(q, (bool, np.bool_)) or not isinstance(q, (int, float, np.integer, np.floating)) or \
+                not 0.0 <= float(q) <= 1.0:
+            raise ValueError(f"{key} must hold levels in [0, 1] (got {q!r})")
+        levels.append(float(q))
+    names = [quantile_column(q) for q in levels]
+    if len(set(names)) != len(names):
+        raise ValueError(f"{key} names a level twice (columns {names})")
+    return levels
+
+
+def quantile_column(q: float) -> str:
+    """The forecast column of level q: yhat_q0.1, yhat_q0.5, yhat_q0.975."""
+    return "yhat_q" + repr(float(q))
+
+
 def _component_fields(intervals: bool):
     names = COMPONENT_COLUMNS + (("trend_lower", "trend_upper") if intervals else ())
     return [pa.field(n, pa.float64()) for n in names]
@@ -81,6 +108,18 @@ AGGREGATE_SCHEMA = pa.schema([
     pa.field("window_points", pa.int32()), pa.field("forecast_quantity", pa.int64()), pa.field("yhat", pa.float64()),
     pa.field("yhat_lower", pa.float64()), pa.field("yhat_upper", pa.float64()),
 ])
+
+
+def forecast_quantiles(config):
+    """``forecast.quantiles`` checked (quantile_levels), or None; it does not combine with forecast.components or
+    forecast.aggregate."""
+    fc = config.get("forecast", {}) or {}
+    levels = quantile_levels(fc, "forecast.quantiles")
+    if levels is not None and _want_components(fc):
+        raise ValueError("forecast.quantiles cannot be combined with forecast.components")
+    if levels is not None and fc.get("aggregate") is not None:
+        raise ValueError("forecast.quantiles cannot be combined with forecast.aggregate")
+    return levels
 
 
 def aggregate_rule(config):
@@ -196,7 +235,8 @@ class _ForecastTimeSeriesOp:
         want_intervals = bool(fc.get("intervals", False))
         rule = aggregate_rule(self.config)
         self.aggregates = AGGREGATE_SCHEMA.empty_table() if rule else None
-        if want_intervals or rule:
+        levels = forecast_quantiles(self.config)
+        if want_intervals or rule or levels:
             width = float(fc.get("interval_width", 0.8))
             if not 0.0 <= width <= 1.0:     # fbprophet refuses it too (numpy's percentile range check); NaN fails here
                 raise ValueError(f"forecast.interval_width must be in [0, 1] (got {fc.get('interval_width')!r})")
@@ -210,6 +250,8 @@ class _ForecastTimeSeriesOp:
         empty_schema = FORECAST_SCHEMA
         if want_intervals:
             empty_schema = empty_schema.append(pa.field("yhat_lower", pa.float64())).append(pa.field("yhat_upper", pa.float64()))
+        for q in levels or ():
+            empty_schema = empty_schema.append(pa.field(quantile_column(q), pa.float64()))
         if want_components:
             for f in _component_fields(want_intervals):
                 empty_schema = empty_schema.append(f)
@@ -229,7 +271,8 @@ class _ForecastTimeSeriesOp:
                                     seasonality_mode="multiplicative" if info["multiplicative"] else "additive",
                                     n_changepoints=info["n_changepoints"],
                                     interval_width=fc.get("interval_width", 0.8),
-                                    uncertainty_samples=fc.get("uncertainty_samples", 1000) if want_intervals or rule else 0)
+                                    uncertainty_samples=fc.get("uncertainty_samples", 1000) if want_intervals or rule or levels
+                                    else 0)
         opts.yearly, opts.weekly, opts.daily = info["yearly"], info["weekly"], info["daily"]
         # reference :46-47: floor / cap are read back from the FLOAT32 columns of the models table
         floor = table["floor"].combine_chunks().to_numpy(zero_copy_only=False).astype(np.float64)
@@ -244,6 +287,9 @@ class _ForecastTimeSeriesOp:
             res, sums = batched.predict_sums_host(ctx, opts, fitted, future, floor, cap, rule[0], rule[1],
                                                   seed=int(fc.get("seed", 0)), intervals=want_intervals)
             self.aggregates = aggregate_table(sid, did, ok, sums)
+        elif levels:
+            res = batched.predict_quantiles_host(ctx, opts, fitted, future, floor, cap, levels, seed=int(fc.get("seed", 0)),
+                                                 intervals=want_intervals)
         else:
             res = batched.predict_batch_host(ctx, opts, fitted, future, floor, cap, seed=int(fc.get("seed", 0)),
                                              intervals=want_intervals, components=want_components)
@@ -260,6 +306,8 @@ class _ForecastTimeSeriesOp:
         if want_intervals:
             cols["yhat_lower"] = pa.array(res.yhat_lower.reshape(-1), pa.float64())
             cols["yhat_upper"] = pa.array(res.yhat_upper.reshape(-1), pa.float64())
+        for q, lv in enumerate(levels or ()):
+            cols[quantile_column(lv)] = pa.array(res.quantiles[q].reshape(-1), pa.float64())
         if want_components:
             cols.update(component_columns(res, fitted.meta_i32[:, 3], periods, want_intervals))
         out = pa.table(cols)
@@ -414,7 +462,8 @@ class ProphetScorer:
             "forecast_timestamp": ds,
             "forecast_quantity": t["yhat"],
         }
-        for extra in ("yhat_lower", "yhat_upper") + COMPONENT_COLUMNS + ("trend_lower", "trend_upper"):
+        quants = tuple(c for c in t.column_names if c.startswith("yhat_q"))
+        for extra in ("yhat_lower", "yhat_upper") + quants + COMPONENT_COLUMNS + ("trend_lower", "trend_upper"):
             if extra in t.column_names:
                 cols[extra] = t[extra]
         out = Frame(pa.table(cols))
@@ -476,7 +525,8 @@ class ProphetScorer:
 
     @staticmethod
     def score(spark_session, config):
-        aggregate_rule(config)              # a bad forecast.aggregate fails before anything is read
+        aggregate_rule(config)              # a bad forecast.aggregate or forecast.quantiles fails before anything is read
+        forecast_quantiles(config)
         pdist.init_process_group()          # no-op unless launched by torchrun with WORLD_SIZE > 1
         scorer = ProphetScorer(config)
         model_df = scorer.read_model_dataframe(spark_session)
