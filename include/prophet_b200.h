@@ -545,6 +545,50 @@ PB200_API int pb200_cv_quantile_metrics_device(pb200_ctx* ctx, const int64_t* d_
                                                double rolling_window, int64_t* d_out_horizon, int64_t* d_scratch,
                                                double* d_pinball, double* d_share_below, int32_t* d_valid);
 
+/*
+ * In-sample predict over ragged frames (DESIGN §16): fbprophet's m.predict() with no frame, for every model's own history.
+ * The arguments of pb200_predict_device, with the fixed (d_future_ds, horizon) replaced by a ragged frame: model i's rows
+ * are [h_offsets[i], h_offsets[i + 1]) of d_ds (int64 ns, ascending per model), h_offsets a host int64 array
+ * [n_models + 1] as pb200_fit_device's (the call makes the device copy).  Outputs, each indexed like d_ds:
+ *   d_yhat                       double, pb200_predict_device's yhat
+ *   d_yhat_lower / d_yhat_upper  double, the interval (NULL or uncertainty_samples = 0 to skip)
+ * The key, the counters and Tmax are those of the model's own frame, so every value is bit-identical to what
+ * pb200_predict_device gives when that model's rows are its frame, padded to any longer horizon by repeating its last
+ * timestamp.  Failed models (status < 0) get NaN rows.  Argument checks are pb200_predict_device's, plus monotone
+ * offsets; nothing is launched on an error.  The _host form takes host arrays (h_ds [h_offsets[n_models]]).
+ */
+PB200_API int pb200_predict_history_device(pb200_ctx* ctx, const pb200_options* opts,
+                         const double* d_params, const double* d_tchange,
+                         const int32_t* d_meta_i32, const int64_t* d_meta_i64,
+                         const double* d_meta_f64, int64_t n_models,
+                         const int64_t* d_ds, const int64_t* h_offsets,
+                         const double* d_floor, const double* d_cap, uint64_t seed,
+                         double* d_yhat, double* d_yhat_lower, double* d_yhat_upper);
+
+PB200_API int pb200_predict_history_host(pb200_ctx* ctx, const pb200_options* opts,
+                       const double* h_params, const double* h_tchange,
+                       const int32_t* h_meta_i32, const int64_t* h_meta_i64,
+                       const double* h_meta_f64, int64_t n_models,
+                       const int64_t* h_ds, const int64_t* h_offsets,
+                       const double* h_floor, const double* h_cap, uint64_t seed,
+                       double* h_yhat, double* h_yhat_lower, double* h_yhat_upper);
+
+/*
+ * Outlier flags and the kept rows (DESIGN §16), two passes over series i's rows [d_offsets[i], d_offsets[i + 1]):
+ *   pb200_outlier_counts_device   d_flag[r] = (double)y[r] < d_lower[r] || (double)y[r] > d_upper[r] (uint8; a NaN
+ *                                 bound never flags), d_kept[i] = the series' rows not flagged (int32)
+ *   pb200_outlier_compact_device  given d_kept_off = exclusive scan of d_kept ([n_series + 1], int64), writes the kept
+ *                                 rows' ds and y (y in its element type y_dtype) to [d_kept_off[i], d_kept_off[i + 1]) of
+ *                                 d_ds_out / d_y_out in their order: a packed batch pb200_fit_device takes as it is.
+ * One warp per series, no atomics: a series' outputs depend on its own rows only.
+ */
+PB200_API int pb200_outlier_counts_device(pb200_ctx* ctx, const void* d_y, int32_t y_dtype, const int64_t* d_offsets,
+                                          int64_t n_series, const double* d_lower, const double* d_upper, uint8_t* d_flag,
+                                          int32_t* d_kept);
+PB200_API int pb200_outlier_compact_device(pb200_ctx* ctx, const int64_t* d_ds, const void* d_y, int32_t y_dtype,
+                                           const int64_t* d_offsets, int64_t n_series, const uint8_t* d_flag,
+                                           const int64_t* d_kept_off, int64_t* d_ds_out, void* d_y_out);
+
 #ifdef __cplusplus
 }
 #endif

@@ -57,7 +57,8 @@ EXPORTS = [
     "pb200_fit_trace_host", "pb200_forecast_csv_lengths_device", "pb200_forecast_csv_rows_device", "pb200_forecast_csv_row_host",
     "pb200_cv_plan_counts_device", "pb200_cv_plan_device", "pb200_cv_gather_device", "pb200_cv_metrics_device",
     "pb200_predict_sums_anchored_device", "pb200_cv_windows_device", "pb200_predict_quantiles_device",
-    "pb200_predict_quantiles_host", "pb200_cv_quantile_metrics_device",
+    "pb200_predict_quantiles_host", "pb200_cv_quantile_metrics_device", "pb200_predict_history_device",
+    "pb200_predict_history_host", "pb200_outlier_counts_device", "pb200_outlier_compact_device",
 ]
 CV_ERR_HORIZON, CV_ERR_INITIAL, CV_ERR_FEW = 1, 2, 4
 
@@ -124,6 +125,15 @@ def load() -> C.CDLL:
     lib.pb200_predict_quantiles_device.restype = C.c_int
     lib.pb200_predict_quantiles_host.argtypes = pred_args + [i32, vp, vp]
     lib.pb200_predict_quantiles_host.restype = C.c_int
+    hist_args = [vp, OP, vp, vp, vp, vp, vp, i64, vp, vp, vp, vp, u64, vp, vp, vp]
+    lib.pb200_predict_history_device.argtypes = hist_args
+    lib.pb200_predict_history_device.restype = C.c_int
+    lib.pb200_predict_history_host.argtypes = hist_args
+    lib.pb200_predict_history_host.restype = C.c_int
+    lib.pb200_outlier_counts_device.argtypes = [vp, vp, i32, vp, i64, vp, vp, vp, vp]
+    lib.pb200_outlier_counts_device.restype = C.c_int
+    lib.pb200_outlier_compact_device.argtypes = [vp, vp, vp, i32, vp, i64, vp, vp, vp, vp]
+    lib.pb200_outlier_compact_device.restype = C.c_int
     lib.pb200_make_future_device.argtypes = [vp, vp, i64, i32, i64, vp]
     lib.pb200_make_future_device.restype = C.c_int
     lib.pb200_objective_host.argtypes = [vp, OP, vp, vp, i32, vp, i64, dbl, dbl, vp, vp, vp, vp]

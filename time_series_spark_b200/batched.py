@@ -505,6 +505,127 @@ def predict_quantiles_device(ctx: L.Context, opts: L.Options, fitted: FittedBatc
 
 
 @dataclass
+class HistoryForecast:
+    """The in-sample predict of pb200_predict_history_* (DESIGN §16): one value per history row, model i's rows at
+    [offsets[i], offsets[i + 1]) as in the batch that was fitted."""
+    offsets: np.ndarray      # [N + 1] int64 (host)
+    yhat: object             # [rows] f64
+    yhat_lower: object       # [rows] f64, or None without intervals
+    yhat_upper: object
+
+
+def _history_offsets(offsets, n: int) -> np.ndarray:
+    offsets = np.ascontiguousarray(offsets, dtype=np.int64)
+    if offsets.shape != (n + 1,):
+        raise ValueError(f"offsets must have n_models + 1 = {n + 1} entries (got shape {offsets.shape})")
+    return offsets
+
+
+def predict_history_host(ctx: L.Context, opts: L.Options, fitted: FittedBatch, ds_ns: np.ndarray, offsets: np.ndarray,
+                         floor, cap, seed: int = 0, intervals: bool = True) -> HistoryForecast:
+    """pb200_predict_history_host: fbprophet's ``m.predict()`` (no frame: the history itself) for every model of
+    ``fitted`` over its rows ``[offsets[i], offsets[i + 1])`` of ``ds_ns``; ``floor`` / ``cap`` per model (the fit's:
+    ``fitted.meta_f64[:, 1]`` / ``[:, 2]``).  With ``intervals`` the bounds of ``opts.interval_width`` from
+    ``opts.uncertainty_samples`` draws, bit-identical to predict_batch_host on the history padded by its last timestamp."""
+    fitted = fitted.to_host()
+    n = fitted.n
+    offsets = _history_offsets(offsets, n)
+    ds_ns = np.ascontiguousarray(ds_ns, dtype=np.int64)
+    rows = int(offsets[-1])
+    floor = np.ascontiguousarray(np.broadcast_to(np.asarray(floor, dtype=np.float64), (n,)))
+    cap = np.ascontiguousarray(np.broadcast_to(np.asarray(cap, dtype=np.float64), (n,)))
+    do_mc = intervals and opts.uncertainty_samples > 0
+    yhat = np.empty(rows, np.float64)
+    lo = np.empty(rows, np.float64) if do_mc else None
+    hi = np.empty(rows, np.float64) if do_mc else None
+    if n > 0 and rows > 0:
+        rc = L.load().pb200_predict_history_host(
+            ctx.handle, C.byref(opts), _np_ptr(np.ascontiguousarray(fitted.params)),
+            _np_ptr(np.ascontiguousarray(fitted.tchange)), _np_ptr(np.ascontiguousarray(fitted.meta_i32)),
+            _np_ptr(np.ascontiguousarray(fitted.meta_i64)), _np_ptr(np.ascontiguousarray(fitted.meta_f64)), n,
+            _np_ptr(ds_ns), _np_ptr(offsets), _np_ptr(floor), _np_ptr(cap), int(seed) & (2**64 - 1), _np_ptr(yhat),
+            _np_ptr(lo) if do_mc else None, _np_ptr(hi) if do_mc else None)
+        L.check(rc, "pb200_predict_history_host")
+    return HistoryForecast(offsets, yhat, lo, hi)
+
+
+def predict_history_device(ctx: L.Context, opts: L.Options, fitted: FittedBatch, ds_ns, offsets_host: np.ndarray, floor,
+                           cap, seed: int = 0, intervals: bool = True, sync: bool = True) -> HistoryForecast:
+    """pb200_predict_history_device: predict_history_host with torch CUDA tensors (``fitted`` on the device, ``ds_ns``
+    the packed history, ``floor`` / ``cap`` float64 [N]); the offsets stay on the host."""
+    import torch
+    n = fitted.n
+    offsets_host = _history_offsets(offsets_host, n)
+    rows = int(offsets_host[-1])
+    dev = ds_ns.device
+    do_mc = intervals and opts.uncertainty_samples > 0
+    yhat = torch.empty(rows, dtype=torch.float64, device=dev)
+    lo = torch.empty(rows, dtype=torch.float64, device=dev) if do_mc else None
+    hi = torch.empty(rows, dtype=torch.float64, device=dev) if do_mc else None
+    if n > 0 and rows > 0:
+        torch.cuda.current_stream(dev).synchronize()
+        rc = L.load().pb200_predict_history_device(
+            ctx.handle, C.byref(opts), fitted.params.data_ptr(), fitted.tchange.data_ptr(), fitted.meta_i32.data_ptr(),
+            fitted.meta_i64.data_ptr(), fitted.meta_f64.data_ptr(), n, ds_ns.data_ptr(), _np_ptr(offsets_host),
+            floor.data_ptr(), cap.data_ptr(), int(seed) & (2**64 - 1), yhat.data_ptr(),
+            lo.data_ptr() if do_mc else None, hi.data_ptr() if do_mc else None)
+        L.check(rc, "pb200_predict_history_device")
+        if sync:
+            ctx.synchronize()
+    return HistoryForecast(offsets_host, yhat, lo, hi)
+
+
+@dataclass
+class Outliers:
+    """The rows outside their in-sample interval and the batch without them (pb200_outlier_*_device, DESIGN §16)."""
+    flag: object             # [rows] uint8 CUDA: 1 where y < lower or y > upper
+    kept: np.ndarray         # [N] int64 (host): rows kept per series
+    offsets: np.ndarray      # [N + 1] int64 (host): the kept batch's offsets, for fit_batch_device
+    ds: object               # [offsets[-1]] int64 CUDA: the kept rows in their order
+    y: object                # [offsets[-1]] CUDA, y's dtype
+
+
+def outliers_device(ctx: L.Context, ds_ns, y, offsets_host: np.ndarray, lower, upper) -> Outliers:
+    """Flags each row whose y lies outside ``[lower, upper]`` (a NaN bound never flags) and packs the other rows into a
+    batch that ``fit_batch_device`` takes as it is.  Counts, scan, rows: the kept counts are the only device-to-host
+    copy, for the host offsets of the new batch; ds / y never leave the device."""
+    import torch
+    offsets_host = np.ascontiguousarray(offsets_host, dtype=np.int64)
+    n = offsets_host.size - 1
+    rows = int(offsets_host[-1])
+    dev = ds_ns.device
+    for t, what in ((lower, "lower"), (upper, "upper")):
+        if t.dtype != torch.float64 or not t.is_contiguous() or t.device != dev or int(t.numel()) < rows:
+            raise ValueError(f"{what} must be a contiguous float64 tensor of at least {rows} rows on {dev}")
+    lib = L.load()
+    ydt = _y_dtype(y)
+    flag = torch.empty(rows, dtype=torch.uint8, device=dev)
+    kept = torch.empty(n, dtype=torch.int32, device=dev)
+    d_off = torch.from_numpy(offsets_host).to(dev)
+    if n > 0:
+        torch.cuda.current_stream(dev).synchronize()
+        L.check(lib.pb200_outlier_counts_device(ctx.handle, y.data_ptr(), ydt, d_off.data_ptr(), n, lower.data_ptr(),
+                                                upper.data_ptr(), flag.data_ptr(), kept.data_ptr()),
+                "pb200_outlier_counts_device")
+        ctx.synchronize()
+    kept_h = kept.cpu().numpy().astype(np.int64)
+    new_off = np.zeros(n + 1, np.int64)
+    np.cumsum(kept_h, out=new_off[1:])
+    total = int(new_off[-1])
+    ds_out = torch.empty(total, dtype=torch.int64, device=dev)
+    y_out = torch.empty(total, dtype=y.dtype, device=dev)
+    if total > 0:
+        d_kept_off = torch.from_numpy(new_off).to(dev)
+        torch.cuda.current_stream(dev).synchronize()
+        L.check(lib.pb200_outlier_compact_device(ctx.handle, ds_ns.data_ptr(), y.data_ptr(), ydt, d_off.data_ptr(), n,
+                                                 flag.data_ptr(), d_kept_off.data_ptr(), ds_out.data_ptr(),
+                                                 y_out.data_ptr()),
+                "pb200_outlier_compact_device")
+        ctx.synchronize()
+    return Outliers(flag, kept_h, new_off, ds_out, y_out)
+
+
+@dataclass
 class WindowSums:
     """Forecast totals over fixed-width time windows (pb200_predict_sums_*), each [N, wmax]; slots at or past a model's
     ``n_windows`` hold INT64_MIN / 0 / NaN."""

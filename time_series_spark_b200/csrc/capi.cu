@@ -8,6 +8,7 @@
 #include "newton_kernel.cuh"
 #include "csv_kernel.cuh"
 #include "cv_kernel.cuh"
+#include "insample_kernel.cuh"
 
 #include <algorithm>
 #include <cstdio>
@@ -109,6 +110,7 @@ struct pb200_ctx {
     DevBuf d_mc;     // MC workspace
     DevBuf d_sums;   // staging of pb200_predict_sums_host's window outputs
     DevBuf d_quant;  // staging of pb200_predict_quantiles_host's planes
+    DevBuf d_hoff;   // device copy of pb200_predict_history_*'s frame offsets
     int lc0_max = 1 << 30; // PB200_LC0_MAX: longest series on one warp per series, longer ones get four (unset: no limit)
     bool lc_auto = true;   // false when PB200_LC0_MAX pins the CTA width
     bool tab_on = true;    // PB200_NO_TAB=1 disables the seasonal-table variants (A/B runs)
@@ -1452,6 +1454,205 @@ PB200_API int pb200_cv_windows_device(pb200_ctx* c, const int64_t* d_ds, const v
     a.yhat_sum = d_yhat_sum;
     const int grid = (int)std::min<int64_t>((n + 7) / 8, (int64_t)c->sms * 4);   // 8 warps per CTA, one per entry
     pb200::cv::cv_window_kernel<<<grid, 256, 0, c->stream>>>(a);
+    CK(cudaGetLastError());
+    c->launches++;
+    return PB200_OK;
+}
+
+}  // extern "C"
+
+// ---- in-sample predict over ragged frames, outlier flags and the kept rows (DESIGN §16) ----
+namespace {
+
+// pb200_predict_history_device: pb200_predict_device's checks, then the ragged instances of predict_kernel and mc_kernel
+// over model i's rows [h_offsets[i], h_offsets[i + 1]) of d_ds; the offsets are copied to the device here
+int predict_history_device(pb200_ctx* c, const pb200_options* opts, const double* d_params, const double* d_tchange,
+                           const int32_t* d_meta_i32, const int64_t* d_meta_i64, const double* d_meta_f64,
+                           int64_t n_models, const int64_t* d_ds, const int64_t* h_offsets, const double* d_floor,
+                           const double* d_cap, uint64_t seed, double* d_yhat, double* d_yhat_lower, double* d_yhat_upper) {
+    if (!c) return fail(PB200_E_ARG, "ctx is null");
+    int rc = check_opts(opts);
+    if (rc) return rc;
+    if (n_models < 0 || n_models > (1LL << 30)) return fail(PB200_E_ARG, "sizes");
+    if (n_models == 0) return PB200_OK;
+    if (!h_offsets) return fail(PB200_E_ARG, "null pointer (offsets)");
+    if (h_offsets[0] < 0) return fail(PB200_E_ARG, "offsets[0] < 0");
+    int64_t tmax = 0;
+    for (int64_t i = 0; i < n_models; ++i) {
+        const int64_t T = h_offsets[i + 1] - h_offsets[i];
+        if (T < 0) return fail(PB200_E_ARG, "offsets not monotone");
+        if (T > INT32_MAX) return fail(PB200_E_UNSUPPORTED, "a frame longer than 2^31 - 1 rows");
+        tmax = std::max(tmax, T);
+    }
+    if (tmax == 0) return PB200_OK;
+    if (!d_params || !d_tchange || !d_meta_i32 || !d_meta_i64 || !d_meta_f64 || !d_floor || !d_cap || !d_ds || !d_yhat)
+        return fail(PB200_E_ARG, "null pointer");
+    const bool mc = d_yhat_lower && d_yhat_upper && opts->uncertainty_samples > 0;
+    if (mc && (rc = check_mc_opts(opts))) return rc;
+    pb200_layout L;
+    pb200_get_layout(opts, &L);
+    CK(cudaSetDevice(c->device));
+    const size_t N = (size_t)n_models;
+    CK(c->d_hoff.reserve((N + 1) * 8));
+    CK(cudaMemcpyAsync(c->d_hoff.p, h_offsets, (N + 1) * 8, cudaMemcpyHostToDevice, c->stream));
+    pb200::RaggedPredictArgs a;
+    a.params = d_params;
+    a.tchange = d_tchange;
+    a.meta_i32 = d_meta_i32;
+    a.meta_i64 = (const long long*)d_meta_i64;
+    a.meta_f64 = d_meta_f64;
+    a.future_ds = (const long long*)d_ds;
+    a.floor = d_floor;
+    a.cap = d_cap;
+    a.n_models = (int)n_models;
+    a.horizon = 0;                 // the frames are the offsets'
+    a.smax = L.smax;
+    a.kmax = L.kmax;
+    a.pstride = L.pstride;
+    a.growth = opts->growth;
+    a.mult = opts->multiplicative ? 1 : 0;
+    a.yhat = d_yhat;
+    a.trend = nullptr;
+    a.yhat_int = nullptr;
+    a.offsets = (const long long*)c->d_hoff.p;
+    // the fixed frame's geometry over the longest frame: CTAs past a shorter model's rows leave at once
+    dim3 grid((unsigned)n_models, (unsigned)std::min<int64_t>((tmax + 1023) / 1024, 64));
+    pb200::predict_kernel<false, true><<<grid, 256, 0, c->stream>>>(a);
+    CK(cudaGetLastError());
+    c->launches++;
+    if (mc) {
+        rc = pb200::launch_mc_ragged(c->stream, c->sms, a, a.offsets, opts->uncertainty_samples, opts->interval_width, seed,
+                                     d_yhat_lower, d_yhat_upper);
+        if (rc == -1) return fail(PB200_E_ARG, "uncertainty_samples / interval_width out of range");
+        if (rc) return fail(PB200_E_CUDA, "mc kernel launch", cudaGetLastError());
+        c->launches++;
+    }
+    return PB200_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+PB200_API int pb200_predict_history_device(pb200_ctx* c, const pb200_options* opts, const double* d_params,
+                                           const double* d_tchange, const int32_t* d_meta_i32, const int64_t* d_meta_i64,
+                                           const double* d_meta_f64, int64_t n_models, const int64_t* d_ds,
+                                           const int64_t* h_offsets, const double* d_floor, const double* d_cap,
+                                           uint64_t seed, double* d_yhat, double* d_yhat_lower, double* d_yhat_upper) {
+    return predict_history_device(c, opts, d_params, d_tchange, d_meta_i32, d_meta_i64, d_meta_f64, n_models, d_ds,
+                                  h_offsets, d_floor, d_cap, seed, d_yhat, d_yhat_lower, d_yhat_upper);
+}
+
+PB200_API int pb200_predict_history_host(pb200_ctx* c, const pb200_options* opts, const double* h_params,
+                                         const double* h_tchange, const int32_t* h_meta_i32, const int64_t* h_meta_i64,
+                                         const double* h_meta_f64, int64_t n_models, const int64_t* h_ds,
+                                         const int64_t* h_offsets, const double* h_floor, const double* h_cap,
+                                         uint64_t seed, double* h_yhat, double* h_yhat_lower, double* h_yhat_upper) {
+    if (!c) return fail(PB200_E_ARG, "ctx is null");
+    int rc = check_opts(opts);
+    if (rc) return rc;
+    if (n_models < 0 || n_models > (1LL << 30)) return fail(PB200_E_ARG, "sizes");
+    if (n_models == 0) return PB200_OK;
+    if (!h_offsets) return fail(PB200_E_ARG, "null pointer (offsets)");
+    const int64_t rows = h_offsets[n_models];
+    if (rows < 0) return fail(PB200_E_ARG, "offsets");
+    if (!h_params || !h_tchange || !h_meta_i32 || !h_meta_i64 || !h_meta_f64 || !h_floor || !h_cap ||
+        (rows > 0 && (!h_ds || !h_yhat)))
+        return fail(PB200_E_ARG, "null pointer");
+    const bool mc = h_yhat_lower && h_yhat_upper && opts->uncertainty_samples > 0;
+    if (mc && (rc = check_mc_opts(opts))) return rc;
+    pb200_layout L;
+    pb200_get_layout(opts, &L);
+    CK(cudaSetDevice(c->device));
+    const size_t N = (size_t)n_models, R = (size_t)std::max<int64_t>(rows, 0);
+    CK(c->d_params.reserve(N * L.pstride * 8));
+    CK(c->d_tchange.reserve(N * L.smax * 8));
+    CK(c->d_mi32.reserve(N * 8 * 4));
+    CK(c->d_mi64.reserve(N * 2 * 8));
+    CK(c->d_mf64.reserve(N * 4 * 8));
+    CK(c->d_floor.reserve(N * 8));
+    CK(c->d_cap.reserve(N * 8));
+    CK(c->d_fut.reserve(R * 8));
+    CK(c->d_yhat.reserve(R * 8));
+    if (mc) {
+        CK(c->d_lo.reserve(R * 8));
+        CK(c->d_hi.reserve(R * 8));
+    }
+    cudaStream_t st = c->stream;
+    CK(cudaMemcpyAsync(c->d_params.p, h_params, N * L.pstride * 8, cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(c->d_tchange.p, h_tchange, N * L.smax * 8, cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(c->d_mi32.p, h_meta_i32, N * 8 * 4, cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(c->d_mi64.p, h_meta_i64, N * 2 * 8, cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(c->d_mf64.p, h_meta_f64, N * 4 * 8, cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(c->d_floor.p, h_floor, N * 8, cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(c->d_cap.p, h_cap, N * 8, cudaMemcpyHostToDevice, st));
+    if (R) CK(cudaMemcpyAsync(c->d_fut.p, h_ds, R * 8, cudaMemcpyHostToDevice, st));
+    rc = predict_history_device(c, opts, (const double*)c->d_params.p, (const double*)c->d_tchange.p,
+                                (const int32_t*)c->d_mi32.p, (const int64_t*)c->d_mi64.p, (const double*)c->d_mf64.p,
+                                n_models, (const int64_t*)c->d_fut.p, h_offsets, (const double*)c->d_floor.p,
+                                (const double*)c->d_cap.p, seed, (double*)c->d_yhat.p, mc ? (double*)c->d_lo.p : nullptr,
+                                mc ? (double*)c->d_hi.p : nullptr);
+    if (rc) return rc;
+    if (R) {
+        CK(cudaMemcpyAsync(h_yhat, c->d_yhat.p, R * 8, cudaMemcpyDeviceToHost, st));
+        if (mc) {
+            CK(cudaMemcpyAsync(h_yhat_lower, c->d_lo.p, R * 8, cudaMemcpyDeviceToHost, st));
+            CK(cudaMemcpyAsync(h_yhat_upper, c->d_hi.p, R * 8, cudaMemcpyDeviceToHost, st));
+        }
+    }
+    CK(cudaStreamSynchronize(st));
+    return PB200_OK;
+}
+
+static int outlier_grid(const pb200_ctx* c, int64_t n_series) {   // one warp per series, 8 per CTA
+    return (int)std::max<int64_t>(1, std::min<int64_t>((n_series + pb200::insample::WARPS - 1) / pb200::insample::WARPS,
+                                                       (int64_t)c->sms * 16));
+}
+
+PB200_API int pb200_outlier_counts_device(pb200_ctx* c, const void* d_y, int32_t y_dtype, const int64_t* d_offsets,
+                                          int64_t n_series, const double* d_lower, const double* d_upper, uint8_t* d_flag,
+                                          int32_t* d_kept) {
+    if (!c) return fail(PB200_E_ARG, "ctx is null");
+    if (n_series < 0) return fail(PB200_E_ARG, "n_series");
+    if (y_dtype < 0 || y_dtype > 2) return fail(PB200_E_ARG, "y_dtype");
+    if (n_series == 0) return PB200_OK;
+    if (!d_y || !d_offsets || !d_lower || !d_upper || !d_flag || !d_kept) return fail(PB200_E_ARG, "null pointer");
+    CK(cudaSetDevice(c->device));
+    pb200::insample::FlagArgs a;
+    a.y = d_y;
+    a.y_dtype = y_dtype;
+    a.offsets = (const long long*)d_offsets;
+    a.n_series = n_series;
+    a.lower = d_lower;
+    a.upper = d_upper;
+    a.flag = d_flag;
+    a.kept = d_kept;
+    pb200::insample::outlier_counts_kernel<<<outlier_grid(c, n_series), pb200::insample::THREADS, 0, c->stream>>>(a);
+    CK(cudaGetLastError());
+    c->launches++;
+    return PB200_OK;
+}
+
+PB200_API int pb200_outlier_compact_device(pb200_ctx* c, const int64_t* d_ds, const void* d_y, int32_t y_dtype,
+                                           const int64_t* d_offsets, int64_t n_series, const uint8_t* d_flag,
+                                           const int64_t* d_kept_off, int64_t* d_ds_out, void* d_y_out) {
+    if (!c) return fail(PB200_E_ARG, "ctx is null");
+    if (n_series < 0) return fail(PB200_E_ARG, "n_series");
+    if (y_dtype < 0 || y_dtype > 2) return fail(PB200_E_ARG, "y_dtype");
+    if (n_series == 0) return PB200_OK;
+    if (!d_ds || !d_y || !d_offsets || !d_flag || !d_kept_off || !d_ds_out || !d_y_out) return fail(PB200_E_ARG, "null pointer");
+    CK(cudaSetDevice(c->device));
+    pb200::insample::CompactArgs a;
+    a.ds = (const long long*)d_ds;
+    a.y = d_y;
+    a.y_dtype = y_dtype;
+    a.offsets = (const long long*)d_offsets;
+    a.n_series = n_series;
+    a.flag = d_flag;
+    a.kept_off = (const long long*)d_kept_off;
+    a.ds_out = (long long*)d_ds_out;
+    a.y_out = d_y_out;
+    pb200::insample::outlier_compact_kernel<<<outlier_grid(c, n_series), pb200::insample::THREADS, 0, c->stream>>>(a);
     CK(cudaGetLastError());
     c->launches++;
     return PB200_OK;

@@ -90,6 +90,15 @@ struct McArgs {
     double* planes;       // [nq][n_models * horizon]: the quantile planes (mc_kernel<LOGI, false> only)
 };
 
+// mc_kernel's ragged instance (pb200_predict_history_*): model i's frame is rows [offsets[i], offsets[i + 1]) of
+// p.future_ds and of lower / upper.  Derived, as RaggedPredictArgs, so that McArgs and the fixed-frame instances keep
+// their layout and code.
+struct RaggedMcArgs : McArgs {
+    const long long* offsets;   // [n_models + 1]
+};
+template <bool RAGGED>
+using McArgsT = std::conditional_t<RAGGED, RaggedMcArgs, McArgs>;
+
 __device__ __forceinline__ uint64_t splitmix64(uint64_t z) {
     z += 0x9E3779B97F4A7C15ull;
     z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
@@ -313,14 +322,28 @@ __device__ __forceinline__ void row_levels(double* row, const int n, const McLev
     __syncwarp();
 }
 
+// model i's frame: its first row and its points, model * H and H of a fixed frame of H points (RAGGED: the rows
+// [offsets[i], offsets[i + 1]))
+template <bool RAGGED>
+__device__ __forceinline__ size_t frame_base(const McArgsT<RAGGED>& a, const int model, const int H) {
+    if constexpr (RAGGED) return (size_t)a.offsets[model];
+    else return (size_t)model * H;
+}
+template <bool RAGGED>
+__device__ __forceinline__ int frame_len(const McArgsT<RAGGED>& a, const int model, const int H) {
+    if constexpr (RAGGED) return (int)(a.offsets[model + 1] - a.offsets[model]);
+    else return H;
+}
+
 // What a CTA does for a model before its first point: Tmax = max t over the whole frame, the model's Philox key, and
 // the state of this thread's two draws (tid and tid + MC_THREADS) with the time of their first simulated changepoint.
 // red_t [MC_THREADS / 32] and key_sm are shared scratch; every thread of the CTA calls it.
-__device__ __forceinline__ void start_draws(const McArgs& a, const ModelSm& ms, const int model, const int tid,
+template <bool RAGGED = false>
+__device__ __forceinline__ void start_draws(const McArgsT<RAGGED>& a, const ModelSm& ms, const int model, const int tid,
                                             double* red_t, uint64_t* key_sm, Philox& ph, DrawState* d, bool* live) {
     const int lane = tid & 31, warp = tid >> 5;
-    const int H = a.p.horizon;
-    const size_t base = (size_t)model * H;
+    const size_t base = frame_base<RAGGED>(a, model, a.p.horizon);
+    const int H = frame_len<RAGGED>(a, model, a.p.horizon);
     double tm = -INFINITY;
     for (int h = tid; h < H; h += MC_THREADS) tm = fmax(tm, (double)(a.p.future_ds[base + h] - ms.start) / ms.t_scale);
 #pragma unroll
@@ -377,8 +400,10 @@ __device__ __forceinline__ double draw_point(DrawState& d, const ModelSm& ms, co
 // draws and rows [8, 16) the trend draws of the same points, in the same 128 KB, and warp w still selects row w.  The
 // yhat draws are the same numbers (the noise counters go by pairs of points and 8 is even; the trend state advances per
 // draw across tiles; Tmax is over the whole frame), so are their bounds.
-template <bool LOGI, bool TREND>
-__global__ void __launch_bounds__(MC_THREADS, 1) mc_kernel(const McArgs a) {
+// RAGGED: model i's frame is its own rows [offsets[i], offsets[i + 1]) (RaggedMcArgs), walked as a frame of that length:
+// the same Tmax, key and counters as a fixed frame holding those rows first, so the same draws at those points.
+template <bool LOGI, bool TREND, bool RAGGED = false>
+__global__ void __launch_bounds__(MC_THREADS, 1) mc_kernel(const McArgsT<RAGGED> a) {
     constexpr int TILE = TREND ? MC_TILE / 2 : MC_TILE;
     extern __shared__ __align__(16) unsigned char mc_smem[];
     double* rows = (double*)mc_smem;                       // [MC_TILE][MC_NP]
@@ -400,10 +425,11 @@ __global__ void __launch_bounds__(MC_THREADS, 1) mc_kernel(const McArgs a) {
     for (int model = blockIdx.x; model < a.p.n_models; model += gridDim.x) {
         __syncthreads();
         load_model(ms, a.p, model, tid, MC_THREADS);
-        const size_t base = (size_t)model * H;
+        const size_t base = frame_base<RAGGED>(a, model, H);
+        const int HM = frame_len<RAGGED>(a, model, H);     // the model's points
         if (ms.status < 0) {
             for (int l = 0; l < lv.nlev; ++l)
-                for (int h = tid; h < H; h += MC_THREADS) {
+                for (int h = tid; h < HM; h += MC_THREADS) {
                     out(l, base + h, false) = NAN;
                     if (TREND) out(l, base + h, true) = NAN;
                 }
@@ -412,10 +438,10 @@ __global__ void __launch_bounds__(MC_THREADS, 1) mc_kernel(const McArgs a) {
         Philox ph;
         DrawState d[2];
         bool live[2];
-        start_draws(a, ms, model, tid, red_t, &key_sm, ph, d, live);
+        start_draws<RAGGED>(a, ms, model, tid, red_t, &key_sm, ph, d, live);
         const double rate = (double)ms.S, nscale = ms.sigma * ms.y_scale;
-        for (int h0 = 0; h0 < H; h0 += TILE) {
-            const int np = min(TILE, H - h0);
+        for (int h0 = 0; h0 < HM; h0 += TILE) {
+            const int np = min(TILE, HM - h0);
             if (tid < np) {
                 const long long dsv = a.p.future_ds[base + h0 + tid];
                 tt[tid] = (double)(dsv - ms.start) / ms.t_scale;
@@ -596,11 +622,12 @@ __global__ void __launch_bounds__(MC_THREADS, 1) mc_sum_kernel(const McSumArgs a
     }
 }
 
-template <bool LOGI, bool TREND>
-cudaError_t launch_mc_inst(cudaStream_t st, int grid, size_t smem, const McArgs& a) {
-    const cudaError_t e = cudaFuncSetAttribute(mc_kernel<LOGI, TREND>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+template <bool LOGI, bool TREND, bool RAGGED = false>
+cudaError_t launch_mc_inst(cudaStream_t st, int grid, size_t smem, const McArgsT<RAGGED>& a) {
+    const cudaError_t e = cudaFuncSetAttribute(mc_kernel<LOGI, TREND, RAGGED>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                               (int)smem);
     if (e != cudaSuccess) return e;
-    mc_kernel<LOGI, TREND><<<grid, MC_THREADS, smem, st>>>(a);
+    mc_kernel<LOGI, TREND, RAGGED><<<grid, MC_THREADS, smem, st>>>(a);
     return cudaGetLastError();
 }
 
@@ -670,6 +697,21 @@ inline int launch_mc(cudaStream_t st, int sms, const PredictArgs& p, int n_sampl
     const bool logi = p.growth == PB200_GROWTH_LOGISTIC;
     const cudaError_t e = logi ? (trend ? launch_mc_inst<true, true>(st, grid, MC_SMEM, a) : launch_mc_inst<true, false>(st, grid, MC_SMEM, a))
                                : (trend ? launch_mc_inst<false, true>(st, grid, MC_SMEM, a) : launch_mc_inst<false, false>(st, grid, MC_SMEM, a));
+    return e == cudaSuccess ? 0 : 1;
+}
+
+// the bounds of mc_kernel's ragged instance over model i's rows [offsets[i], offsets[i + 1]) of p.future_ds (device
+// array [n_models + 1]).  Returns as launch_mc
+inline int launch_mc_ragged(cudaStream_t st, int sms, const PredictArgs& p, const long long* offsets, int n_samples,
+                            double width, uint64_t seed, double* lower, double* upper) {
+    RaggedMcArgs a;
+    if (!mc_args(a, p, n_samples, width, seed)) return -1;
+    a.lower = lower;
+    a.upper = upper;
+    a.offsets = offsets;
+    const int grid = p.n_models < sms ? p.n_models : sms;
+    const cudaError_t e = p.growth == PB200_GROWTH_LOGISTIC ? launch_mc_inst<true, false, true>(st, grid, MC_SMEM, a)
+                                                            : launch_mc_inst<false, false, true>(st, grid, MC_SMEM, a);
     return e == cudaSuccess ? 0 : 1;
 }
 

@@ -13,6 +13,8 @@
 #include <math.h>
 #include <stdint.h>
 
+#include <type_traits>
+
 #include "../../include/prophet_b200.h"
 
 namespace pb200 {
@@ -35,6 +37,15 @@ struct PredictArgs {
     double* trend;
     int* yhat_int;
 };
+
+// The ragged instances (pb200_predict_history_*): model i's frame is rows [offsets[i], offsets[i + 1]) of future_ds and of
+// the outputs, in place of [i * horizon, (i + 1) * horizon).  A derived type, so that PredictArgs -- and with it the code of
+// every fixed-frame instance -- stays as it is.
+struct RaggedPredictArgs : PredictArgs {
+    const long long* offsets;   // [n_models + 1]
+};
+template <bool RAGGED>
+using PredictArgsT = std::conditional_t<RAGGED, RaggedPredictArgs, PredictArgs>;
 
 constexpr double PI_FL = 3.141592653589793;
 
@@ -156,20 +167,30 @@ __device__ __forceinline__ double seasonal_parts(const ModelSm& ms, const long l
     return acc;
 }
 
-// COMP: also write fbprophet's component columns -- planes PB200_COMP_* of a.trend, each [n_models * horizon]
-template <bool COMP>
-__global__ void __launch_bounds__(256) predict_kernel(const PredictArgs a) {
+// COMP: also write fbprophet's component columns -- planes PB200_COMP_* of a.trend, each [n_models * horizon].
+// RAGGED: model i's own rows [offsets[i], offsets[i + 1]) (RaggedPredictArgs); yhat only (no yhat_int, no trend).  A CTA
+// whose first point lies past its model's rows leaves before the model's prologue.
+template <bool COMP, bool RAGGED = false>
+__global__ void __launch_bounds__(256) predict_kernel(const PredictArgsT<RAGGED> a) {
     __shared__ ModelSm ms;
     const int model = blockIdx.x;
     const int tid = threadIdx.x;
+    long long r0 = 0;
+    int H = a.horizon;
+    if constexpr (RAGGED) {
+        r0 = a.offsets[model];
+        H = (int)(a.offsets[model + 1] - r0);
+        if ((int)(blockIdx.y * blockDim.x) >= H) return;
+    }
     load_model(ms, a, model, tid, blockDim.x);
     const bool ok = ms.status >= 0;
     const int S = ms.S;
     const size_t plane = (size_t)a.n_models * a.horizon;
-    for (int h = blockIdx.y * blockDim.x + tid; h < a.horizon; h += gridDim.y * blockDim.x) {
-        const size_t o = (size_t)model * a.horizon + h;
+    for (int h = blockIdx.y * blockDim.x + tid; h < H; h += gridDim.y * blockDim.x) {
+        const size_t o = RAGGED ? (size_t)(r0 + h) : (size_t)model * a.horizon + h;
         if (!ok) {
             a.yhat[o] = NAN;
+            if (RAGGED) continue;
             if (COMP) {
 #pragma unroll
                 for (int c = 0; c < PB200_N_COMPONENTS; ++c) a.trend[c * plane + o] = NAN;
@@ -210,6 +231,7 @@ __global__ void __launch_bounds__(256) predict_kernel(const PredictArgs a) {
             a.trend[PB200_COMP_DAILY * plane + o] = cd * s;
         }
         a.yhat[o] = yh;
+        if (RAGGED) continue;
         if (!COMP && a.trend) a.trend[o] = tr;
         // prophet_scorer.py:73 astype(int) truncates toward zero; :76-84 values < floor -> floor
         double yt = trunc(yh);

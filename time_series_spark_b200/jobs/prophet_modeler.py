@@ -21,6 +21,18 @@ fit from its row of that table when the row's changepoint count and seasonalitie
 how many table rows matched no input group.  The table must have been fitted with the job's growth, seasonality mode,
 seasonality switches and ``n_changepoints``.  It may be ``io.models`` itself: the old table is read before it is
 replaced.  Without the key the job is the cold fit it has always been.
+
+``insample`` (optional section): fbprophet's in-sample predict, ``m.predict()`` with no frame, for every fitted group
+(DESIGN §16).  ``insample.interval_width`` (required, in [0, 1]) decides what counts as an outlier: a history row whose
+y lies outside its ``yhat_lower`` / ``yhat_upper``, from ``insample.uncertainty_samples`` draws (default 1000, in
+[2, 1024]) keyed by ``insample.seed`` (default 0).  ``io.fitted`` (optional) receives one parquet part file per rank with
+one row per history row of every group that got a model, in the packed order: ``series_id, dim_id, ds, y`` (y in the
+input column's type), ``yhat, yhat_lower, yhat_upper`` (float64) and ``outlier`` (bool).  ``insample.refit: true``
+(default false) drops the flagged rows and fits again on the device, with the same options and ``io.warm_start``:
+``io.models`` then holds the models a plain run gives on the input without those rows (a group left with fewer than 2
+rows raises), while ``io.fitted`` still describes the first fit, the one the flags come from.  The section needs
+``io.fitted`` or ``refit: true``; one line reports the rows predicted and flagged and the series flagged and refitted.
+Without the section the job is what it was.
 """
 from __future__ import annotations
 
@@ -95,6 +107,76 @@ def who(series_id, dim_id, mask) -> str:
 def _group_keys(series_id, dim_id) -> np.ndarray:
     """One int64 key per (series_id, dim_id) group."""
     return (np.asarray(series_id, dtype=np.int64) << 32) | (np.asarray(dim_id, dtype=np.int64) & 0xFFFFFFFF)
+
+
+INSAMPLE_KEYS = ("interval_width", "uncertainty_samples", "seed", "refit")
+
+# the io.fitted frame, but for y, which keeps the input column's type
+FITTED_COLUMNS = [("series_id", pa.int32()), ("dim_id", pa.int32()), ("ds", pa.timestamp("ns")), ("y", None),
+                  ("yhat", pa.float64()), ("yhat_lower", pa.float64()), ("yhat_upper", pa.float64()),
+                  ("outlier", pa.bool_())]
+
+
+def fitted_schema(y_type) -> pa.Schema:
+    """The schema of the io.fitted frame for an input y column of type ``y_type``."""
+    return pa.schema([pa.field(n, y_type if t is None else t, True) for n, t in FITTED_COLUMNS])
+
+
+def insample_options(config):
+    """The ``insample`` section as ``{interval_width, uncertainty_samples, seed, refit}`` with its defaults, or None when
+    the config has no such section.  Raises ValueError naming the key for an unknown key, a missing or out-of-range
+    ``interval_width``, ``uncertainty_samples`` outside [2, 1024], a bad ``seed`` or ``refit``, and for a section that
+    would write nothing (neither ``io.fitted`` nor ``refit: true``)."""
+    if "insample" not in config:
+        return None
+    sec = config["insample"]
+    if not isinstance(sec, dict):
+        raise ValueError(f"insample must be a mapping with at least insample.interval_width (got {sec!r})")
+    unknown = sorted(set(sec) - set(INSAMPLE_KEYS))
+    if unknown:
+        raise ValueError(f"insample.{unknown[0]} is not a known key (known: {', '.join(INSAMPLE_KEYS)})")
+    if "interval_width" not in sec:
+        raise ValueError("insample.interval_width is required: it decides which history rows are outliers")
+    w = sec["interval_width"]
+    if isinstance(w, bool) or not isinstance(w, (int, float)) or not 0.0 <= float(w) <= 1.0:
+        raise ValueError(f"insample.interval_width must be a number in [0, 1] (got {w!r})")
+    n = sec.get("uncertainty_samples", 1000)
+    if isinstance(n, bool) or not isinstance(n, int) or not 2 <= n <= 1024:
+        raise ValueError(f"insample.uncertainty_samples must be an integer in [2, 1024] (got {n!r})")
+    seed = sec.get("seed", 0)
+    if isinstance(seed, bool) or not isinstance(seed, int) or not 0 <= seed < 2**64:
+        raise ValueError(f"insample.seed must be an integer in [0, 2^64) (got {seed!r})")
+    refit = sec.get("refit", False)
+    if not isinstance(refit, bool):
+        raise ValueError(f"insample.refit must be true or false (got {refit!r})")
+    if not refit and not (config.get("io") or {}).get("fitted"):
+        raise ValueError("insample needs io.fitted or insample.refit: true; as configured it would do nothing")
+    return {"interval_width": float(w), "uncertainty_samples": int(n), "seed": int(seed), "refit": refit}
+
+
+def insample_report(rows: int, flagged: int, series_flagged: int, refitted: int) -> str:
+    """The job's one line about the in-sample predict."""
+    return (f"In-sample: {rows} rows predicted, {flagged} flagged as outliers in {series_flagged} series; "
+            f"{refitted} series refitted without them")
+
+
+def null_rows_last_ds(table: pa.Table, series_id, dim_id) -> np.ndarray:
+    """Per packed group ``(series_id, dim_id)``, the latest ds (ns) of its rows whose y is null or NaN, INT64_MIN for a
+    group without one.  The pack drops those rows, but they count for the group's ``last_ds``, and a refit keeps them."""
+    import pyarrow.compute as pc
+    out = np.full(len(series_id), np.iinfo(np.int64).min, np.int64)
+    null = pc.is_null(table["y"], nan_is_null=True)
+    if not pc.any(null).as_py():
+        return out
+    sub = table.filter(null)
+    ds = pc.cast(pc.cast(sub["ds"], pa.timestamp("ns")), pa.int64()).to_numpy()
+    key = _group_keys(sub["series_id"].to_numpy(), sub["dim_id"].to_numpy())
+    gkey = _group_keys(series_id, dim_id)
+    order = np.argsort(gkey, kind="stable")
+    pos = np.minimum(np.searchsorted(gkey[order], key), gkey.size - 1)
+    hit = gkey[order][pos] == key
+    np.maximum.at(out, order[pos[hit]], ds[hit])
+    return out
 
 
 def warm_start_init(table: pa.Table, opts: L.Options, series_id, dim_id, path: str = "io.warm_start"):
@@ -198,6 +280,10 @@ class _ModelTimeSeriesOp:
             raise ValueError("model_time_series groups by ('series_id', 'dim_id')")
         floor = self.config["model"]["floor"]
         cap_multiplier = self.config["model"]["cap_multiplier"]
+        ins = insample_options(self.config)
+        with_frame = ins is not None and bool((self.config.get("io") or {}).get("fitted"))
+        # this rank's io.fitted frame (empty until a group is predicted)
+        self.fitted_table = fitted_schema(table.schema.field("y").type).empty_table() if with_frame else None
         ctx = get_context()
         # group + sort on the GPU (two radix sorts), ds / y stay in HBM for the fit
         import torch
@@ -224,15 +310,65 @@ class _ModelTimeSeriesOp:
         init = None
         if warm_path:
             init, unmatched = warm_start_init(read_warm_start(warm_path, pk.series_id), opts, pk.series_id, pk.dim_id)
-        fitted = batched.fit_batch_device(ctx, opts, pk.ds.contiguous(), pk.y.contiguous(), pk.offsets,
-                                          float(floor), float(cap_multiplier), init=init).to_host()
+        fitted_d = batched.fit_batch_device(ctx, opts, pk.ds.contiguous(), pk.y.contiguous(), pk.offsets,
+                                            float(floor), float(cap_multiplier), init=init)
+        fitted = fitted_d.to_host()
         if warm_path:
             print(warm_report(fitted.warm, unmatched))
         t_fit = time.time()
-        out = models_table(fitted, pk.series_id, pk.dim_id, pk.last_ds, opts, floor)
+        if ins is None:
+            out = models_table(fitted, pk.series_id, pk.dim_id, pk.last_ds, opts, floor)
+        else:
+            out = self._insample(ctx, opts, ins, table, pk, fitted_d, fitted, floor, cap_multiplier, init,
+                                 unmatched if warm_path else 0)
         # wall time per stage of the last call (tools/e2e_scaling.py reports them): upload + group + sort, GPU fit + D2H, encode
         self.last_timings = {"pack_s": t_pack - execution_time, "fit_s": t_fit - t_pack, "encode_s": time.time() - t_fit}
         print(f"Output df {out.num_rows} models trained in {time.time() - execution_time}")
+        return out
+
+    def _insample(self, ctx, opts, ins, table, pk, fitted_d, fitted, floor, cap_multiplier, init, unmatched):
+        """The in-sample predict of the fitted batch, its outlier flags, the io.fitted frame and (insample.refit) the
+        fit without the flagged rows; returns the models table the job writes."""
+        import torch
+        iopts = L.Options.from_buffer_copy(opts)
+        iopts.interval_width = ins["interval_width"]
+        iopts.uncertainty_samples = ins["uncertainty_samples"]
+        # fbprophet predicts the history with the floor and cap it was fitted on: the fit's own (float64) values
+        fl = fitted_d.meta_f64[:, 1].contiguous()
+        cp = fitted_d.meta_f64[:, 2].contiguous()
+        hf = batched.predict_history_device(ctx, iopts, fitted_d, pk.ds, pk.offsets, fl, cp, seed=ins["seed"])
+        ol = batched.outliers_device(ctx, pk.ds, pk.y, pk.offsets, hf.yhat_lower, hf.yhat_upper)
+        ok = fitted.meta_i32[:, 4] >= 0
+        T = np.diff(pk.offsets)
+        lost = T - ol.kept                                  # flagged rows per group (0 for a failed fit: NaN bounds)
+        if self.fitted_table is not None:
+            row_ok = np.repeat(ok, T)
+            y_type = self.fitted_table.schema.field("y").type
+            cols = {
+                "series_id": np.repeat(pk.series_id, T), "dim_id": np.repeat(pk.dim_id, T),
+                "ds": pk.ds.cpu().numpy().view("datetime64[ns]"), "y": pk.y.cpu().numpy(),
+                "yhat": hf.yhat.cpu().numpy(), "yhat_lower": hf.yhat_lower.cpu().numpy(),
+                "yhat_upper": hf.yhat_upper.cpu().numpy(), "outlier": ol.flag.cpu().numpy().astype(bool),
+            }
+            arrays = [pa.array(cols[n][row_ok], type=y_type if t is None else t) if n != "y"
+                      else pa.array(cols[n][row_ok]).cast(y_type) for n, t in FITTED_COLUMNS]
+            self.fitted_table = pa.Table.from_arrays(arrays, schema=self.fitted_table.schema)
+        refitted = 0
+        if not ins["refit"]:
+            out = models_table(fitted, pk.series_id, pk.dim_id, pk.last_ds, opts, floor)
+        else:
+            short = np.diff(ol.offsets) < 2
+            if np.any(short):
+                raise ValueError("Dataframe has less than 2 non-NaN rows." + who(pk.series_id, pk.dim_id, short))
+            refit = batched.fit_batch_device(ctx, opts, ol.ds, ol.y, ol.offsets, float(floor), float(cap_multiplier),
+                                             init=init).to_host()
+            if init is not None:
+                print(warm_report(refit.warm, unmatched))
+            kept_last = ol.ds[torch.from_numpy(ol.offsets[1:] - 1).to(ol.ds.device)].cpu().numpy()
+            last_ds = np.maximum(kept_last, null_rows_last_ds(table, pk.series_id, pk.dim_id))
+            out = models_table(refit, pk.series_id, pk.dim_id, last_ds, opts, floor)
+            refitted = pk.n
+        print(insample_report(int(T[ok].sum()), int(lost.sum()), int(np.count_nonzero(lost > 0)), refitted))
         return out
 
     def __call__(self, pdf):
@@ -323,6 +459,12 @@ class ProphetModeler:
         pdist.prepare_output_dir(out)
         pq.write_table(model_df.table, os.path.join(out, f"part-{rank:05d}.parquet"))
 
+    def persist_fitted(self, fitted: pa.Table):
+        """The in-sample frame (insample with io.fitted): parquet, mode='overwrite', one part file per rank."""
+        out = self.config["io"]["fitted"]
+        pdist.prepare_output_dir(out)
+        pq.write_table(fitted, os.path.join(out, f"part-{pdist.world()[0]:05d}.parquet"))
+
     @staticmethod
     def model(spark_session, config):
         """Create the trained time series models (reference :127-143)."""
@@ -333,3 +475,5 @@ class ProphetModeler:
         op.rank_local_input = getattr(scorer, "rank_local_input", False)
         model_df = input_df.groupby("series_id", "dim_id").apply(op)
         scorer.persist_models(model_df)
+        if getattr(op, "fitted_table", None) is not None:
+            scorer.persist_fitted(op.fitted_table)
