@@ -402,6 +402,47 @@ PB200_API int pb200_predict_sums_anchored_device(pb200_ctx* ctx, const pb200_opt
                          double* d_yhat_sum, int64_t* d_quantity_sum, double* d_sum_lower, double* d_sum_upper);
 
 /*
+ * pb200_predict_sums_* over calendar periods (DESIGN §17): months, quarters and years of any anchor.  The arguments and
+ * outputs are pb200_predict_sums_*'s with (months, month_shift) in place of (width_ns, origin_ns):
+ *   months in {1, 3, 12}, 0 <= month_shift < months   the period of a point is floor((mi + month_shift) / months), mi the
+ *                 months of ds's proleptic Gregorian civil date since 1970-01 (mathematical floor: also before 1970); a
+ *                 model's windows are the maximal runs of equal period in its (ascending) frame, in order
+ *   d_win_start   the period's start: 00:00 on day 1 of month p * months - month_shift since 1970-01
+ * pandas' 'M' is (1, 0), 'Q-<MON>' (3, (12 - E) mod 3) and 'Y-<MON>' (12, (12 - E) mod 12), E the end month (1..12).  A
+ * period start before the int64-ns minimum is not representable: such a slot holds the start taken mod 2^64 (the callers
+ * refuse such frames).  A bad rule is PB200_E_ARG; the other checks are pb200_predict_sums_*'s.  Nothing is launched on
+ * an error.
+ */
+PB200_API int pb200_predict_period_sums_device(pb200_ctx* ctx, const pb200_options* opts,
+                         const double* d_params, const double* d_tchange,
+                         const int32_t* d_meta_i32, const int64_t* d_meta_i64,
+                         const double* d_meta_f64, int64_t n_models,
+                         const int64_t* d_future_ds, int32_t horizon,
+                         const double* d_floor, const double* d_cap, uint64_t seed,
+                         double* d_yhat, double* d_yhat_lower, double* d_yhat_upper,
+                         int32_t* d_yhat_int, int32_t months, int32_t month_shift, int32_t wmax,
+                         int32_t* d_n_windows, int64_t* d_win_start, int32_t* d_win_points,
+                         double* d_yhat_sum, int64_t* d_quantity_sum, double* d_sum_lower, double* d_sum_upper);
+
+PB200_API int pb200_predict_period_sums_host(pb200_ctx* ctx, const pb200_options* opts,
+                       const double* h_params, const double* h_tchange,
+                       const int32_t* h_meta_i32, const int64_t* h_meta_i64,
+                       const double* h_meta_f64, int64_t n_models,
+                       const int64_t* h_future_ds, int32_t horizon,
+                       const double* h_floor, const double* h_cap, uint64_t seed,
+                       double* h_yhat, double* h_yhat_lower, double* h_yhat_upper,
+                       int32_t* h_yhat_int, int32_t months, int32_t month_shift, int32_t wmax,
+                       int32_t* h_n_windows, int64_t* h_win_start, int32_t* h_win_points,
+                       double* h_yhat_sum, int64_t* h_quantity_sum, double* h_sum_lower, double* h_sum_upper);
+
+/*
+ * The period of each of n timestamps under (months, month_shift) and its start, by the very __host__ __device__ functions
+ * the calendar kernel runs (csrc/calendar.cuh); host arrays.  Needs no context or device.  PB200_E_ARG on a bad rule.
+ */
+PB200_API int pb200_period_host(const int64_t* ds, int64_t n, int32_t months, int32_t month_shift, int64_t* period,
+                                int64_t* start);
+
+/*
  * pb200_predict_* plus forecast quantiles at n_q levels from the same draws (DESIGN §15): fbprophet's
  * np.percentile(predictive_samples(future)['yhat'], p, axis=1) for each p of h_percentiles, in one pass over the draws.
  * Same arguments and the same yhat / yhat_lower / yhat_upper / yhat_int bits as pb200_predict_* (the bounds optional as

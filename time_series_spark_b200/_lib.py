@@ -59,6 +59,7 @@ EXPORTS = [
     "pb200_predict_sums_anchored_device", "pb200_cv_windows_device", "pb200_predict_quantiles_device",
     "pb200_predict_quantiles_host", "pb200_cv_quantile_metrics_device", "pb200_predict_history_device",
     "pb200_predict_history_host", "pb200_outlier_counts_device", "pb200_outlier_compact_device",
+    "pb200_predict_period_sums_device", "pb200_predict_period_sums_host", "pb200_period_host",
 ]
 CV_ERR_HORIZON, CV_ERR_INITIAL, CV_ERR_FEW = 1, 2, 4
 
@@ -121,6 +122,12 @@ def load() -> C.CDLL:
     lib.pb200_predict_sums_host.restype = C.c_int
     lib.pb200_predict_sums_anchored_device.argtypes = pred_args + [i64, vp, vp, i32, vp, vp, vp, vp, vp, vp, vp]
     lib.pb200_predict_sums_anchored_device.restype = C.c_int
+    lib.pb200_predict_period_sums_device.argtypes = pred_args + [i32, i32, i32, vp, vp, vp, vp, vp, vp, vp]
+    lib.pb200_predict_period_sums_device.restype = C.c_int
+    lib.pb200_predict_period_sums_host.argtypes = pred_args + [i32, i32, i32, vp, vp, vp, vp, vp, vp, vp]
+    lib.pb200_predict_period_sums_host.restype = C.c_int
+    lib.pb200_period_host.argtypes = [vp, i64, i32, i32, vp, vp]
+    lib.pb200_period_host.restype = C.c_int
     lib.pb200_predict_quantiles_device.argtypes = pred_args + [i32, vp, vp]
     lib.pb200_predict_quantiles_device.restype = C.c_int
     lib.pb200_predict_quantiles_host.argtypes = pred_args + [i32, vp, vp]

@@ -627,10 +627,10 @@ def outliers_device(ctx: L.Context, ds_ns, y, offsets_host: np.ndarray, lower, u
 
 @dataclass
 class WindowSums:
-    """Forecast totals over fixed-width time windows (pb200_predict_sums_*), each [N, wmax]; slots at or past a model's
-    ``n_windows`` hold INT64_MIN / 0 / NaN."""
+    """Forecast totals over fixed-width time windows (pb200_predict_sums_*) or calendar periods
+    (pb200_predict_period_sums_*), each [N, wmax]; slots at or past a model's ``n_windows`` hold INT64_MIN / 0 / NaN."""
     n_windows: object     # [N] int32
-    start: object         # int64 ns: origin + window index * width
+    start: object         # int64 ns: origin + window index * width, or the period's start
     points: object        # int32: frame points in the window
     yhat_sum: object      # f64: yhat summed in frame order
     quantity_sum: object  # int64: yhat_int summed
@@ -653,12 +653,43 @@ def _check_window_slots(wmax: int, n_windows_max: int) -> None:
                          "last columns: is every model's future frame ascending?")
 
 
-def predict_sums_host(ctx: L.Context, opts: L.Options, fitted: FittedBatch, future_ds: np.ndarray, floor: np.ndarray,
-                      cap: np.ndarray, width_ns: int, origin_ns: int = 0, seed: int = 0, intervals: bool = False):
-    """pb200_predict_sums_host: predict_batch_host's ForecastBatch and the WindowSums of the windows
-    floor((ds - origin_ns) / width_ns) of each model's ascending frame -- totals of yhat / yhat_int per window and the
-    interval of each total from the joint draws (fbprophet's predictive_samples summed per window).  Needs
-    ``opts.uncertainty_samples`` in [2, 1024]; ``intervals`` asks for the pointwise yhat_lower / yhat_upper as well."""
+def _period_rule_checked(months: int, month_shift: int):
+    months, month_shift = int(months), int(month_shift)
+    if months not in (1, 3, 12) or not 0 <= month_shift < months:
+        raise ValueError(f"months must be 1, 3 or 12 and month_shift in [0, months) (got {months}, {month_shift})")
+    return months, month_shift
+
+
+def periods_host(ds, months: int, month_shift: int):
+    """pb200_period_host: the calendar period of each timestamp (int64 ns) under (months, month_shift) and the period's
+    start, computed by the functions the calendar kernel runs.  Returns (period, start), int64 arrays of ds's shape."""
+    months, month_shift = _period_rule_checked(months, month_shift)
+    ds = np.ascontiguousarray(ds, dtype=np.int64)
+    period = np.empty(ds.shape, np.int64)
+    start = np.empty(ds.shape, np.int64)
+    L.check(L.load().pb200_period_host(_np_ptr(ds), ds.size, months, month_shift, _np_ptr(period), _np_ptr(start)),
+            "pb200_period_host")
+    return period, start
+
+
+def period_slots(first_ds, last_ds, months: int, month_shift: int) -> int:
+    """window_slots for calendar periods: max_i (p(last_i) - p(first_i) + 1).  Refuses, with a ValueError, a frame whose
+    first point's period starts before the int64-ns minimum (1677-09-21), where its start is not representable."""
+    first_ds = np.asarray(first_ds, np.int64)
+    if first_ds.size == 0:
+        return 1
+    p0, s0 = periods_host(first_ds, months, month_shift)
+    bad = np.flatnonzero(s0 > first_ds)         # the start wrapped: it lies before the int64-ns minimum
+    if bad.size:
+        raise ValueError(f"the period of {int(first_ds[bad[0]])} ns starts before the earliest representable timestamp "
+                         "(1677-09-21): no window_start can be written for it")
+    p1, _ = periods_host(last_ds, months, month_shift)
+    return int((p1 - p0).max()) + 1
+
+
+def _sums_host(ctx, opts, fitted, future_ds, floor, cap, seed, intervals, entry: str, rule, slots):
+    """The body of predict_sums_host / predict_period_sums_host: ``entry`` the C function, ``rule`` its two rule arguments,
+    ``slots(first_ds, last_ds)`` the slots per model."""
     fitted = fitted.to_host()
     n = fitted.n
     future_ds = np.ascontiguousarray(future_ds, dtype=np.int64)
@@ -666,10 +697,7 @@ def predict_sums_host(ctx: L.Context, opts: L.Options, fitted: FittedBatch, futu
     h = future_ds.shape[1]
     floor = np.ascontiguousarray(np.broadcast_to(np.asarray(floor, dtype=np.float64), (n,)))
     cap = np.ascontiguousarray(np.broadcast_to(np.asarray(cap, dtype=np.float64), (n,)))
-    width_ns, origin_ns = int(width_ns), int(origin_ns)
-    if width_ns <= 0:
-        raise ValueError(f"width_ns must be > 0 (got {width_ns})")
-    wmax = window_slots(future_ds[:, 0], future_ds[:, -1], width_ns, origin_ns) if h else 1
+    wmax = slots(future_ds[:, 0], future_ds[:, -1]) if h else 1
     yhat = np.empty((n, h), np.float64)
     yint = np.empty((n, h), np.int32)
     lo = np.empty((n, h), np.float64) if intervals else None
@@ -677,33 +705,52 @@ def predict_sums_host(ctx: L.Context, opts: L.Options, fitted: FittedBatch, futu
     ws = WindowSums(np.zeros(n, np.int32), np.empty((n, wmax), np.int64), np.empty((n, wmax), np.int32),
                     np.empty((n, wmax), np.float64), np.empty((n, wmax), np.int64), np.empty((n, wmax), np.float64),
                     np.empty((n, wmax), np.float64))
-    rc = L.load().pb200_predict_sums_host(
+    rc = getattr(L.load(), entry)(
         ctx.handle, C.byref(opts), _np_ptr(np.ascontiguousarray(fitted.params)),
         _np_ptr(np.ascontiguousarray(fitted.tchange)), _np_ptr(np.ascontiguousarray(fitted.meta_i32)),
         _np_ptr(np.ascontiguousarray(fitted.meta_i64)), _np_ptr(np.ascontiguousarray(fitted.meta_f64)),
         n, _np_ptr(future_ds), h, _np_ptr(floor), _np_ptr(cap), int(seed) & (2**64 - 1),
         _np_ptr(yhat), _np_ptr(lo) if intervals else None, _np_ptr(hi) if intervals else None, _np_ptr(yint),
-        width_ns, origin_ns, wmax, _np_ptr(ws.n_windows), _np_ptr(ws.start), _np_ptr(ws.points), _np_ptr(ws.yhat_sum),
+        *rule, wmax, _np_ptr(ws.n_windows), _np_ptr(ws.start), _np_ptr(ws.points), _np_ptr(ws.yhat_sum),
         _np_ptr(ws.quantity_sum), _np_ptr(ws.lower), _np_ptr(ws.upper))
-    L.check(rc, "pb200_predict_sums_host")
+    L.check(rc, entry)
     _check_window_slots(wmax, int(ws.n_windows.max()) if n else 0)
     return ForecastBatch(future_ds, yhat, lo, hi, yint), ws
 
 
-def predict_sums_device(ctx: L.Context, opts: L.Options, fitted: FittedBatch, future_ds, floor, cap, width_ns: int,
-                        origin_ns: int = 0, seed: int = 0, intervals: bool = False):
-    """pb200_predict_sums_device with torch CUDA tensors; as predict_sums_host."""
+def predict_sums_host(ctx: L.Context, opts: L.Options, fitted: FittedBatch, future_ds: np.ndarray, floor: np.ndarray,
+                      cap: np.ndarray, width_ns: int, origin_ns: int = 0, seed: int = 0, intervals: bool = False):
+    """pb200_predict_sums_host: predict_batch_host's ForecastBatch and the WindowSums of the windows
+    floor((ds - origin_ns) / width_ns) of each model's ascending frame -- totals of yhat / yhat_int per window and the
+    interval of each total from the joint draws (fbprophet's predictive_samples summed per window).  Needs
+    ``opts.uncertainty_samples`` in [2, 1024]; ``intervals`` asks for the pointwise yhat_lower / yhat_upper as well."""
+    width_ns, origin_ns = int(width_ns), int(origin_ns)
+    if width_ns <= 0:
+        raise ValueError(f"width_ns must be > 0 (got {width_ns})")
+    return _sums_host(ctx, opts, fitted, future_ds, floor, cap, seed, intervals, "pb200_predict_sums_host",
+                      (width_ns, origin_ns), lambda a, b: window_slots(a, b, width_ns, origin_ns))
+
+
+def predict_period_sums_host(ctx: L.Context, opts: L.Options, fitted: FittedBatch, future_ds: np.ndarray, floor, cap,
+                             months: int, month_shift: int, seed: int = 0, intervals: bool = False):
+    """pb200_predict_period_sums_host: predict_sums_host over calendar periods (DESIGN §17) -- the windows are the
+    periods floor((mi + month_shift) / months) of each model's ascending frame, mi the months of ds's civil date since
+    1970-01, and ``WindowSums.start`` holds each period's start.  ``period_rule`` turns a pandas alias into the rule."""
+    months, month_shift = _period_rule_checked(months, month_shift)
+    return _sums_host(ctx, opts, fitted, future_ds, floor, cap, seed, intervals, "pb200_predict_period_sums_host",
+                      (months, month_shift), lambda a, b: period_slots(a, b, months, month_shift))
+
+
+def _sums_device(ctx, opts, fitted, future_ds, floor, cap, seed, intervals, entry: str, rule, slots):
+    """The body of predict_sums_device / predict_period_sums_device, as _sums_host."""
     import torch
     n = fitted.n
     h = int(future_ds.shape[1])
     dev = future_ds.device
-    width_ns, origin_ns = int(width_ns), int(origin_ns)
-    if width_ns <= 0:
-        raise ValueError(f"width_ns must be > 0 (got {width_ns})")
     wmax = 1
     if n and h:
         ends = future_ds[:, [0, -1]].cpu().numpy()
-        wmax = window_slots(ends[:, 0], ends[:, 1], width_ns, origin_ns)
+        wmax = slots(ends[:, 0], ends[:, 1])
     f64 = dict(dtype=torch.float64, device=dev)
     yhat = torch.empty((n, h), **f64)
     yint = torch.empty((n, h), dtype=torch.int32, device=dev)
@@ -714,17 +761,59 @@ def predict_sums_device(ctx: L.Context, opts: L.Options, fitted: FittedBatch, fu
                     torch.empty((n, wmax), dtype=torch.int64, device=dev), torch.empty((n, wmax), **f64),
                     torch.empty((n, wmax), **f64))
     torch.cuda.current_stream(dev).synchronize()
-    rc = L.load().pb200_predict_sums_device(
+    rc = getattr(L.load(), entry)(
         ctx.handle, C.byref(opts), fitted.params.data_ptr(), fitted.tchange.data_ptr(), fitted.meta_i32.data_ptr(),
         fitted.meta_i64.data_ptr(), fitted.meta_f64.data_ptr(), n, future_ds.data_ptr(), h, floor.data_ptr(),
         cap.data_ptr(), int(seed) & (2**64 - 1), yhat.data_ptr(), lo.data_ptr() if intervals else None,
-        hi.data_ptr() if intervals else None, yint.data_ptr(), width_ns, origin_ns, wmax, ws.n_windows.data_ptr(),
+        hi.data_ptr() if intervals else None, yint.data_ptr(), *rule, wmax, ws.n_windows.data_ptr(),
         ws.start.data_ptr(), ws.points.data_ptr(), ws.yhat_sum.data_ptr(), ws.quantity_sum.data_ptr(), ws.lower.data_ptr(),
         ws.upper.data_ptr())
-    L.check(rc, "pb200_predict_sums_device")
+    L.check(rc, entry)
     ctx.synchronize()
     _check_window_slots(wmax, int(ws.n_windows.max().item()) if n else 0)
     return ForecastBatch(future_ds, yhat, lo, hi, yint), ws
+
+
+def predict_sums_device(ctx: L.Context, opts: L.Options, fitted: FittedBatch, future_ds, floor, cap, width_ns: int,
+                        origin_ns: int = 0, seed: int = 0, intervals: bool = False):
+    """pb200_predict_sums_device with torch CUDA tensors; as predict_sums_host."""
+    width_ns, origin_ns = int(width_ns), int(origin_ns)
+    if width_ns <= 0:
+        raise ValueError(f"width_ns must be > 0 (got {width_ns})")
+    return _sums_device(ctx, opts, fitted, future_ds, floor, cap, seed, intervals, "pb200_predict_sums_device",
+                        (width_ns, origin_ns), lambda a, b: window_slots(a, b, width_ns, origin_ns))
+
+
+def predict_period_sums_device(ctx: L.Context, opts: L.Options, fitted: FittedBatch, future_ds, floor, cap, months: int,
+                               month_shift: int, seed: int = 0, intervals: bool = False):
+    """pb200_predict_period_sums_device with torch CUDA tensors; as predict_period_sums_host."""
+    months, month_shift = _period_rule_checked(months, month_shift)
+    return _sums_device(ctx, opts, fitted, future_ds, floor, cap, seed, intervals, "pb200_predict_period_sums_device",
+                        (months, month_shift), lambda a, b: period_slots(a, b, months, month_shift))
+
+
+_MONTHS = ("JAN", "FEB", "MAR", "APR", "MAY", "JUN", "JUL", "AUG", "SEP", "OCT", "NOV", "DEC")
+_WEEKDAYS = ("MON", "TUE", "WED", "THU", "FRI", "SAT", "SUN")
+
+
+def period_rule(alias: str):
+    """A pandas period alias as a window rule (DESIGN §17): ``("months", months, shift)`` for 'M', 'Q', 'Q-<MON>', 'Y'
+    and 'Y-<MON>' (the periods of predict_period_sums_*), ``("fixed", width_ns, origin_ns)`` for 'W' and 'W-<DAY>' (a
+    week is the fixed rule 7D whose origin is the day after <DAY>: W-SUN weeks start on Monday, origin 1970-01-05).
+    Anything else -- 'D', 'h', '7D', 'MS', 'QS', 'A', 'B', multiples such as '2M' -- is refused with a ValueError."""
+    import re
+    m = re.fullmatch(r"([A-Z])(?:-([A-Z]{3}))?", alias) if isinstance(alias, str) else None
+    kind, anchor = (m.group(1), m.group(2)) if m else (None, None)
+    if kind == "W" and (anchor is None or anchor in _WEEKDAYS):
+        d = _WEEKDAYS.index(anchor or "SUN")
+        return "fixed", 7 * 86400 * 10**9, ((d + 1 - 3) % 7) * 86400 * 10**9     # 1970-01-01 was a Thursday (3)
+    if kind == "M" and anchor is None:
+        return "months", 1, 0
+    if kind in ("Q", "Y") and (anchor is None or anchor in _MONTHS):
+        months = 3 if kind == "Q" else 12
+        end = _MONTHS.index(anchor or "DEC") + 1
+        return "months", months, (12 - end) % months
+    raise ValueError(f"{alias!r} is not a period alias: use 'W', 'W-<DAY>', 'M', 'Q', 'Q-<MON>', 'Y' or 'Y-<MON>'")
 
 
 def predict_sums_anchored_device(ctx: L.Context, opts: L.Options, fitted: FittedBatch, future_ds, floor, cap,

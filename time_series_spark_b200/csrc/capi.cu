@@ -840,13 +840,20 @@ struct SumOut {
     // pb200_predict_sums_anchored_device: an origin and a frame length per model, in place of origin_ns and the horizon
     const int64_t* origins = nullptr;
     const int32_t* frame_len = nullptr;
+    // pb200_predict_period_sums_*: the calendar periods of (months, month_shift), in place of width_ns / origin_ns
+    int32_t months = 0, month_shift = 0;
 };
 
 // checked before anything is copied or launched
 int check_sum_args(const pb200_options* o, const SumOut& s) {
     const int rc = check_mc_opts(o);
     if (rc) return rc;
-    if (s.width_ns <= 0) return fail(PB200_E_ARG, "width_ns must be > 0");
+    if (s.months != 0) {
+        if (!(s.months == 1 || s.months == 3 || s.months == 12) || s.month_shift < 0 || s.month_shift >= s.months)
+            return fail(PB200_E_ARG, "months must be 1, 3 or 12 and month_shift in [0, months)");
+    } else if (s.width_ns <= 0) {
+        return fail(PB200_E_ARG, "width_ns must be > 0");
+    }
     if (s.wmax <= 0) return fail(PB200_E_ARG, "wmax must be > 0");
     if (!s.n_windows || !s.win_start || !s.win_points || !s.yhat_sum || !s.quantity_sum || !s.sum_lower || !s.sum_upper)
         return fail(PB200_E_ARG, "null pointer (window outputs)");
@@ -874,7 +881,8 @@ int check_quant_args(const pb200_options* o, const QuantOut& q) {
 
 // pb200_predict_device; d_comp != null: the components instance of predict_kernel, d_tlo / d_thi != null: the
 // trend-bounds instance of mc_kernel; sums != null: mc_sum_kernel after them (it also runs on an empty frame, where
-// every model has no window), its per-model instance when sums->origins != null; quant != null: mc_kernel also writes the
+// every model has no window), its per-model instance when sums->origins != null, its calendar instance when
+// sums->months != 0; quant != null: mc_kernel also writes the
 // quantile planes, from the same selection as the bounds
 int predict_device(pb200_ctx* c, const pb200_options* opts, const double* d_params, const double* d_tchange,
                    const int32_t* d_meta_i32, const int64_t* d_meta_i64, const double* d_meta_f64, int64_t n_models,
@@ -946,7 +954,8 @@ int predict_device(pb200_ctx* c, const pb200_options* opts, const double* d_para
         s.quantity_sum = (long long*)sums->quantity_sum;
         s.origins = (const long long*)sums->origins;
         s.frame_len = sums->frame_len;
-        rc = pb200::launch_mc_sum(c->stream, c->sms, a, opts->uncertainty_samples, opts->interval_width, seed, s);
+        rc = pb200::launch_mc_sum(c->stream, c->sms, a, opts->uncertainty_samples, opts->interval_width, seed, s,
+                                  sums->months, sums->month_shift);
         if (rc == -1) return fail(PB200_E_ARG, "uncertainty_samples / interval_width out of range");
         if (rc) return fail(PB200_E_CUDA, "mc sum kernel launch", cudaGetLastError());
         c->launches++;
@@ -1152,6 +1161,49 @@ PB200_API int pb200_predict_sums_host(pb200_ctx* c, const pb200_options* opts, c
                       h_sum_lower, h_sum_upper};
     return predict_host(c, opts, h_params, h_tchange, h_meta_i32, h_meta_i64, h_meta_f64, n_models, h_future_ds, horizon,
                         h_floor, h_cap, seed, h_yhat, h_yhat_lower, h_yhat_upper, h_yhat_int, nullptr, nullptr, nullptr, &s);
+}
+
+PB200_API int pb200_predict_period_sums_device(pb200_ctx* c, const pb200_options* opts, const double* d_params,
+                         const double* d_tchange, const int32_t* d_meta_i32, const int64_t* d_meta_i64,
+                         const double* d_meta_f64, int64_t n_models, const int64_t* d_future_ds, int32_t horizon,
+                         const double* d_floor, const double* d_cap, uint64_t seed, double* d_yhat, double* d_yhat_lower,
+                         double* d_yhat_upper, int32_t* d_yhat_int, int32_t months, int32_t month_shift, int32_t wmax,
+                         int32_t* d_n_windows, int64_t* d_win_start, int32_t* d_win_points, double* d_yhat_sum,
+                         int64_t* d_quantity_sum, double* d_sum_lower, double* d_sum_upper) {
+    SumOut s = {0, 0, wmax, d_n_windows, d_win_start, d_win_points, d_yhat_sum, d_quantity_sum, d_sum_lower, d_sum_upper};
+    s.months = months;
+    s.month_shift = month_shift;
+    if (months == 0) return fail(PB200_E_ARG, "months must be 1, 3 or 12 and month_shift in [0, months)");
+    return predict_device(c, opts, d_params, d_tchange, d_meta_i32, d_meta_i64, d_meta_f64, n_models, d_future_ds, horizon,
+                          d_floor, d_cap, seed, d_yhat, d_yhat_lower, d_yhat_upper, d_yhat_int, nullptr, nullptr, nullptr, &s);
+}
+
+PB200_API int pb200_predict_period_sums_host(pb200_ctx* c, const pb200_options* opts, const double* h_params,
+                       const double* h_tchange, const int32_t* h_meta_i32, const int64_t* h_meta_i64,
+                       const double* h_meta_f64, int64_t n_models, const int64_t* h_future_ds, int32_t horizon,
+                       const double* h_floor, const double* h_cap, uint64_t seed, double* h_yhat, double* h_yhat_lower,
+                       double* h_yhat_upper, int32_t* h_yhat_int, int32_t months, int32_t month_shift, int32_t wmax,
+                       int32_t* h_n_windows, int64_t* h_win_start, int32_t* h_win_points, double* h_yhat_sum,
+                       int64_t* h_quantity_sum, double* h_sum_lower, double* h_sum_upper) {
+    SumOut s = {0, 0, wmax, h_n_windows, h_win_start, h_win_points, h_yhat_sum, h_quantity_sum, h_sum_lower, h_sum_upper};
+    s.months = months;
+    s.month_shift = month_shift;
+    if (months == 0) return fail(PB200_E_ARG, "months must be 1, 3 or 12 and month_shift in [0, months)");
+    return predict_host(c, opts, h_params, h_tchange, h_meta_i32, h_meta_i64, h_meta_f64, n_models, h_future_ds, horizon,
+                        h_floor, h_cap, seed, h_yhat, h_yhat_lower, h_yhat_upper, h_yhat_int, nullptr, nullptr, nullptr, &s);
+}
+
+PB200_API int pb200_period_host(const int64_t* ds, int64_t n, int32_t months, int32_t month_shift, int64_t* period,
+                                int64_t* start) {
+    if (!(months == 1 || months == 3 || months == 12) || month_shift < 0 || month_shift >= months)
+        return fail(PB200_E_ARG, "months must be 1, 3 or 12 and month_shift in [0, months)");
+    if (n < 0) return fail(PB200_E_ARG, "sizes");
+    if (n > 0 && (!ds || !period || !start)) return fail(PB200_E_ARG, "null pointer");
+    for (int64_t i = 0; i < n; ++i) {
+        period[i] = pb200::period_of(ds[i], months, month_shift);
+        start[i] = pb200::period_start(period[i], months, month_shift);
+    }
+    return PB200_OK;
 }
 
 PB200_API int pb200_predict_quantiles_device(pb200_ctx* c, const pb200_options* opts, const double* d_params,

@@ -12,6 +12,8 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include "calendar.cuh"     // civil_from_days
+
 namespace pb200 {
 namespace csv {
 
@@ -39,19 +41,6 @@ __host__ __device__ __forceinline__ char* put_2(char* p, int v) {
     p[0] = (char)('0' + v / 10);
     p[1] = (char)('0' + v % 10);
     return p + 2;
-}
-
-// civil date of a day count since 1970-01-01 (proleptic Gregorian; days >= 0 here)
-__host__ __device__ __forceinline__ void civil_from_days(int64_t z, int& y, int& m, int& d) {
-    z += 719468;
-    const int64_t era = z / 146097;
-    const unsigned doe = (unsigned)(z - era * 146097);
-    const unsigned yoe = (doe - doe / 1460 + doe / 36524 - doe / 146096) / 365;
-    const unsigned doy = doe - (365 * yoe + yoe / 4 - yoe / 100);
-    const unsigned mp = (5 * doy + 2) / 153;
-    d = (int)(doy - (153 * mp + 2) / 5 + 1);
-    m = (int)(mp < 10 ? mp + 3 : mp - 9);
-    y = (int)(yoe + era * 400) + (m <= 2 ? 1 : 0);
 }
 
 __host__ __device__ __forceinline__ int row_len(int32_t sid, int32_t did, int32_t qty, int created_len) {

@@ -25,6 +25,7 @@
 
 #include <algorithm>
 
+#include "calendar.cuh"
 #include "predict_kernel.cuh"
 
 namespace pb200 {
@@ -499,6 +500,15 @@ struct McSumArgs {
     const int* frame_len;         // [n_models]
 };
 
+// mc_sum_kernel's calendar instance (DESIGN §17): the windows are the calendar periods of the rule (months, month_shift)
+// (calendar.cuh) in place of floor((ds - origin_ns) / width_ns).  Derived, as RaggedMcArgs, so that McSumArgs and the
+// fixed-width instances keep their layout and code.
+struct PeriodSumArgs : McSumArgs {
+    int months, month_shift;
+};
+template <bool CAL>
+using McSumArgsT = std::conditional_t<CAL, PeriodSumArgs, McSumArgs>;
+
 constexpr int MC_SUM_TILE = 512;  // points whose t, seasonal term, window and predict outputs are staged at once (even: noise pairs)
 
 // mathematical floor((ds - origin) / width), width > 0
@@ -516,8 +526,10 @@ __device__ __forceinline__ long long window_of(const long long ds, const long lo
 // PER_MODEL: model i's windows are taken from origins[i] over its first frame_len[i] points only.  Tmax, the key and the
 // counters stay those of the whole frame, so the draws at the walked points are unchanged (the backtest pads a frame by
 // repeating its last timestamp, which leaves Tmax as it is).
-template <bool LOGI, bool PER_MODEL>
-__global__ void __launch_bounds__(MC_THREADS, 1) mc_sum_kernel(const McSumArgs a) {
+// CAL: the windows are the calendar periods of a.months / a.month_shift (PeriodSumArgs), each starting at its period start;
+// the draws, the sums and the selection are those of the fixed-width instance.
+template <bool LOGI, bool PER_MODEL, bool CAL = false>
+__global__ void __launch_bounds__(MC_THREADS, 1) mc_sum_kernel(const McSumArgsT<CAL> a) {
     extern __shared__ __align__(16) unsigned char mc_smem[];
     double* rows = (double*)mc_smem;                       // [MC_TILE][MC_NP], as mc_kernel
     const SelScratch sw = sel_scratch(mc_smem, threadIdx.x >> 5);
@@ -562,7 +574,8 @@ __global__ void __launch_bounds__(MC_THREADS, 1) mc_sum_kernel(const McSumArgs a
                     s[q] = 0.0;
                 }
                 if (tid == 0 && nw < a.wmax) {
-                    a.win_start[wbase + nw] = (PER_MODEL ? a.origins[model] : a.origin_ns) + cur_w * a.width_ns;
+                    if constexpr (CAL) a.win_start[wbase + nw] = period_start(cur_w, a.months, a.month_shift);
+                    else a.win_start[wbase + nw] = (PER_MODEL ? a.origins[model] : a.origin_ns) + cur_w * a.width_ns;
                     a.win_points[wbase + nw] = pts;
                     a.yhat_sum[wbase + nw] = ys;
                     a.quantity_sum[wbase + nw] = qs;
@@ -578,7 +591,8 @@ __global__ void __launch_bounds__(MC_THREADS, 1) mc_sum_kernel(const McSumArgs a
                     const long long dsv = mc.p.future_ds[base + h0 + tid];
                     tt[tid] = (double)(dsv - ms.start) / ms.t_scale;
                     seas[tid] = ms.K > 0 ? seasonal_term(ms, dsv) : 0.0;
-                    win[tid] = window_of(dsv, PER_MODEL ? a.origins[model] : a.origin_ns, a.width_ns);
+                    if constexpr (CAL) win[tid] = period_of(dsv, a.months, a.month_shift);
+                    else win[tid] = window_of(dsv, PER_MODEL ? a.origins[model] : a.origin_ns, a.width_ns);
                     yh_t[tid] = mc.p.yhat[base + h0 + tid];
                     yi_t[tid] = mc.p.yhat_int[base + h0 + tid];
                 }
@@ -631,12 +645,12 @@ cudaError_t launch_mc_inst(cudaStream_t st, int grid, size_t smem, const McArgsT
     return cudaGetLastError();
 }
 
-template <bool LOGI, bool PER_MODEL>
-cudaError_t launch_mc_sum_inst(cudaStream_t st, int grid, const McSumArgs& a) {
-    const cudaError_t e = cudaFuncSetAttribute(mc_sum_kernel<LOGI, PER_MODEL>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                               (int)MC_SMEM);
+template <bool LOGI, bool PER_MODEL, bool CAL = false>
+cudaError_t launch_mc_sum_inst(cudaStream_t st, int grid, const McSumArgsT<CAL>& a) {
+    const cudaError_t e = cudaFuncSetAttribute(mc_sum_kernel<LOGI, PER_MODEL, CAL>,
+                                               cudaFuncAttributeMaxDynamicSharedMemorySize, (int)MC_SMEM);
     if (e != cudaSuccess) return e;
-    mc_sum_kernel<LOGI, PER_MODEL><<<grid, MC_THREADS, MC_SMEM, st>>>(a);
+    mc_sum_kernel<LOGI, PER_MODEL, CAL><<<grid, MC_THREADS, MC_SMEM, st>>>(a);
     return cudaGetLastError();
 }
 
@@ -716,10 +730,11 @@ inline int launch_mc_ragged(cudaStream_t st, int sms, const PredictArgs& p, cons
 }
 
 // mc_sum_kernel over the frame of p, whose yhat / yhat_int predict_kernel has written on the same stream; s.mc is filled
-// here but for its lower / upper (the window bounds).  s.origins != null: the per-model instance (s.frame_len as well).
+// here but for its lower / upper (the window bounds).  s.origins != null: the per-model instance (s.frame_len as well);
+// months > 0: the calendar instance over the periods of (months, month_shift), whose width_ns / origin_ns are unused.
 // Returns as launch_mc
 inline int launch_mc_sum(cudaStream_t st, int sms, const PredictArgs& p, int n_samples, double width, uint64_t seed,
-                         McSumArgs& s) {
+                         McSumArgs& s, int months = 0, int month_shift = 0) {
     double* const lo = s.mc.lower;
     double* const hi = s.mc.upper;
     if (!mc_args(s.mc, p, n_samples, width, seed)) return -1;
@@ -727,8 +742,17 @@ inline int launch_mc_sum(cudaStream_t st, int sms, const PredictArgs& p, int n_s
     s.mc.upper = hi;
     const int grid = p.n_models < sms ? p.n_models : sms;
     const bool logi = p.growth == PB200_GROWTH_LOGISTIC, per_model = s.origins != nullptr;
-    const cudaError_t e = logi ? (per_model ? launch_mc_sum_inst<true, true>(st, grid, s) : launch_mc_sum_inst<true, false>(st, grid, s))
-                               : (per_model ? launch_mc_sum_inst<false, true>(st, grid, s) : launch_mc_sum_inst<false, false>(st, grid, s));
+    cudaError_t e;
+    if (months > 0) {
+        PeriodSumArgs c;
+        static_cast<McSumArgs&>(c) = s;
+        c.months = months;
+        c.month_shift = month_shift;
+        e = logi ? launch_mc_sum_inst<true, false, true>(st, grid, c) : launch_mc_sum_inst<false, false, true>(st, grid, c);
+    } else {
+        e = logi ? (per_model ? launch_mc_sum_inst<true, true>(st, grid, s) : launch_mc_sum_inst<true, false>(st, grid, s))
+                 : (per_model ? launch_mc_sum_inst<false, true>(st, grid, s) : launch_mc_sum_inst<false, false>(st, grid, s));
+    }
     return e == cudaSuccess ? 0 : 1;
 }
 

@@ -15,7 +15,9 @@ computes yhat_lower/yhat_upper inside Prophet.predict and drops them at :86; set
 component columns ``trend, yearly, weekly, daily, multiplicative_terms, additive_terms``, and ``trend_lower`` /
 ``trend_upper`` with intervals -- DESIGN §12), ``forecast.aggregate`` (a fixed-width duration such as ``'1D'``: also
 write, to ``io.aggregates``, the forecast total of every such window of every model with the interval of the total from
-the joint draws -- DESIGN §13), ``forecast.aggregate_origin`` (where window 0 starts, default 1970-01-01) and
+the joint draws -- DESIGN §13), ``forecast.aggregate_origin`` (where window 0 starts, default 1970-01-01),
+``forecast.aggregate_period`` (a pandas period alias such as ``'M'``, ``'Q-NOV'``, ``'Y'`` or ``'W-SUN'``: the same
+``io.aggregates`` table over calendar months, quarters, years or weeks -- DESIGN §17) and
 ``forecast.quantiles`` (a list of 1 to 32 levels in [0, 1]: one float64 column ``yhat_q<level>`` per level, the
 percentile 100 level of the point's ``uncertainty_samples`` draws -- DESIGN §15).
 """
@@ -154,6 +156,27 @@ def aggregate_rule(config):
     return width, origin_ns
 
 
+def aggregate_period(config):
+    """``forecast.aggregate_period``, a pandas period alias ('M', 'Q-NOV', 'Y', 'W-SUN'), as batched.period_rule's tuple,
+    or None without the key.  It writes io.aggregates as forecast.aggregate does, so it needs io.aggregates and combines
+    with none of forecast.aggregate, forecast.aggregate_origin, forecast.components and forecast.quantiles."""
+    fc = config.get("forecast", {}) or {}
+    spec = fc.get("aggregate_period")
+    if spec is None:
+        return None
+    for other in ("aggregate", "aggregate_origin", "quantiles"):
+        if fc.get(other) is not None:
+            raise ValueError(f"forecast.aggregate_period cannot be combined with forecast.{other}")
+    if _want_components(fc):
+        raise ValueError("forecast.aggregate_period cannot be combined with forecast.components")
+    if not (config.get("io", {}) or {}).get("aggregates"):
+        raise ValueError("forecast.aggregate_period needs io.aggregates, the directory the period totals are written to")
+    try:
+        return batched.period_rule(spec)
+    except ValueError as e:
+        raise ValueError(f"forecast.aggregate_period: {e}") from None
+
+
 def aggregate_table(sid, did, ok, ws: "batched.WindowSums") -> pa.Table:
     """One row per (model, window) of the models that have a forecast, from a shard's WindowSums."""
     wmax = ws.start.shape[1]
@@ -233,10 +256,13 @@ class _ForecastTimeSeriesOp:
             raise ValueError("forecast_time_series groups by ('series_id', 'dim_id')")
         fc = self.config["forecast"]
         want_intervals = bool(fc.get("intervals", False))
-        rule = aggregate_rule(self.config)
-        self.aggregates = AGGREGATE_SCHEMA.empty_table() if rule else None
+        # forecast.aggregate_period: weeks are a fixed-width rule, months / quarters / years the calendar call
+        period = aggregate_period(self.config)
+        rule = period[1:] if period and period[0] == "fixed" else aggregate_rule(self.config)
+        months = period[1:] if period and period[0] == "months" else None
+        self.aggregates = AGGREGATE_SCHEMA.empty_table() if rule or months else None
         levels = forecast_quantiles(self.config)
-        if want_intervals or rule or levels:
+        if want_intervals or rule or months or levels:
             width = float(fc.get("interval_width", 0.8))
             if not 0.0 <= width <= 1.0:     # fbprophet refuses it too (numpy's percentile range check); NaN fails here
                 raise ValueError(f"forecast.interval_width must be in [0, 1] (got {fc.get('interval_width')!r})")
@@ -271,8 +297,8 @@ class _ForecastTimeSeriesOp:
                                     seasonality_mode="multiplicative" if info["multiplicative"] else "additive",
                                     n_changepoints=info["n_changepoints"],
                                     interval_width=fc.get("interval_width", 0.8),
-                                    uncertainty_samples=fc.get("uncertainty_samples", 1000) if want_intervals or rule or levels
-                                    else 0)
+                                    uncertainty_samples=fc.get("uncertainty_samples", 1000)
+                                    if want_intervals or rule or months or levels else 0)
         opts.yearly, opts.weekly, opts.daily = info["yearly"], info["weekly"], info["daily"]
         # reference :46-47: floor / cap are read back from the FLOAT32 columns of the models table
         floor = table["floor"].combine_chunks().to_numpy(zero_copy_only=False).astype(np.float64)
@@ -286,6 +312,10 @@ class _ForecastTimeSeriesOp:
         if rule:
             res, sums = batched.predict_sums_host(ctx, opts, fitted, future, floor, cap, rule[0], rule[1],
                                                   seed=int(fc.get("seed", 0)), intervals=want_intervals)
+            self.aggregates = aggregate_table(sid, did, ok, sums)
+        elif months:
+            res, sums = batched.predict_period_sums_host(ctx, opts, fitted, future, floor, cap, months[0], months[1],
+                                                         seed=int(fc.get("seed", 0)), intervals=want_intervals)
             self.aggregates = aggregate_table(sid, did, ok, sums)
         elif levels:
             res = batched.predict_quantiles_host(ctx, opts, fitted, future, floor, cap, levels, seed=int(fc.get("seed", 0)),
@@ -525,7 +555,8 @@ class ProphetScorer:
 
     @staticmethod
     def score(spark_session, config):
-        aggregate_rule(config)              # a bad forecast.aggregate or forecast.quantiles fails before anything is read
+        aggregate_period(config)            # a bad forecast.aggregate_period, forecast.aggregate or forecast.quantiles
+        aggregate_rule(config)              # fails before anything is read
         forecast_quantiles(config)
         pdist.init_process_group()          # no-op unless launched by torchrun with WORLD_SIZE > 1
         scorer = ProphetScorer(config)
