@@ -85,8 +85,8 @@ extern "C" {
 #define PB200_GROWTH_LOGISTIC 1
 
 /* seasonality switch: PB200_SEAS_AUTO follows Prophet.set_auto_seasonalities,
- * 0 disables, > 0 forces the default Fourier order of that seasonality on
- * (yearly 10, weekly 3, daily 4).  Other orders are not compiled in. */
+ * 0 disables, 1 forces that seasonality on.  Its Fourier order is the default
+ * (yearly 10, weekly 3, daily 4) unless a pb200_options_v2 sets another. */
 #define PB200_SEAS_AUTO (-1)
 
 /* Options = Prophet.__init__ arguments the reference fixes at
@@ -118,9 +118,50 @@ typedef struct pb200_options {
 /* Fills *o with the reference's defaults. */
 PB200_API void pb200_default_options(pb200_options* o);
 
+/*
+ * Seasonality table (DESIGN §18): fbprophet's add_seasonality(name, period, fourier_order, prior_scale) and non-default
+ * built-in Fourier orders.  A pb200_options_v2 with v1.abi_version = PB200_ABI_VERSION_TABLE is accepted by every entry
+ * point that takes a const pb200_options* (pass &o.v1); the tail is read only at that version.
+ *   yearly_order / weekly_order / daily_order  Fourier order of the built-in when its switch (v1.yearly ...) is on or
+ *                 AUTO; 0 = the default (10, 3, 4)
+ *   seasonalities[n_seasonalities]  custom seasonalities in the order they were added: name (NUL-terminated, <= 15
+ *                 bytes, unique), period in days > 0, fourier_order > 0, prior_scale > 0 or 0 for
+ *                 v1.seasonality_prior_scale.  Never auto-disabled.  A name equal to a built-in's replaces it when that
+ *                 built-in's switch is AUTO; with an explicit switch (0 or 1) it is refused.
+ * The model's columns are the custom entries in order, then yearly, weekly and daily: at most PB200_MAX_SEASONALITIES
+ * entries, K = sum of 2 * order <= 64 and 3 + max(1, n_changepoints) + K <= 96, else PB200_E_UNSUPPORTED before any
+ * launch.  All seasonalities share v1.multiplicative.  A table that restates the defaults (no custom entry, orders
+ * 0 or default) is the v1 model; any other is a table model: its series are fitted by a one-warp-per-series kernel
+ * whatever their grid, meta_i32[3] holds one bit per table entry (bit j: entry j active), and the params row packs
+ * the betas of the active entries in table order.
+ * Components add one plane per custom entry (pb200_component_count).  The Newton retry and PB200_ALG_NEWTON evaluate
+ * the table as the fit does.  Not yet for table models (PB200_E_UNSUPPORTED): per-series prior scales and warm starts
+ * (pb200_fit_prior_device / pb200_fit_warm_* with a prior or an init).
+ */
+#define PB200_ABI_VERSION_TABLE 2
+#define PB200_MAX_SEASONALITIES 8
+typedef struct pb200_seasonality {
+    char    name[16];
+    double  period;                 /* days */
+    double  prior_scale;            /* 0 = seasonality_prior_scale */
+    int32_t fourier_order;
+    int32_t reserved;
+} pb200_seasonality;
+
+typedef struct pb200_options_v2 {
+    pb200_options v1;               /* v1.abi_version = PB200_ABI_VERSION_TABLE */
+    int32_t yearly_order, weekly_order, daily_order;
+    int32_t n_seasonalities;        /* 0 .. PB200_MAX_SEASONALITIES */
+    const pb200_seasonality* seasonalities;
+} pb200_options_v2;
+
+/* Series of the context's LAST fit that went to the seasonality-table class (0 for a v1 model).  Synchronises. */
+PB200_API int pb200_last_fit_table_count(struct pb200_ctx* ctx, int64_t* h_count);
+
 /* Layout of one fitted-model record (the arrays fit writes and predict reads).
  * smax = max(1, n_changepoints); kmax = 2*(10+3+4) = 34 or fewer when
- * seasonalities are forced off; params row = [k, m, sigma_obs, delta[smax], beta[kmax]]. */
+ * seasonalities are forced off, or the sum of 2 * order over a seasonality table;
+ * params row = [k, m, sigma_obs, delta[smax], beta[kmax]]. */
 typedef struct pb200_layout {
     int32_t smax;
     int32_t kmax;
@@ -321,6 +362,12 @@ PB200_API int pb200_predict_host(pb200_ctx* ctx, const pb200_options* opts,
 #define PB200_COMP_YEARLY         3
 #define PB200_COMP_WEEKLY         4
 #define PB200_COMP_DAILY          5
+/* Planes of pb200_predict_components_* for these options: PB200_N_COMPONENTS, plus one per custom seasonality of a
+ * seasonality table not named like a built-in, in table order (a custom 'yearly' / 'weekly' / 'daily' fills that
+ * built-in's plane); d_components holds that many planes.  Each is X_c beta_c of its seasonality as the built-ins' planes
+ * are (0 where the model's mask lacks it), and in table order they add up to multiplicative_terms (multiplicative mode)
+ * or to additive_terms / y_scale's unrounded sum.  A negative PB200_E_* for bad options. */
+PB200_API int32_t pb200_component_count(const pb200_options* o);
 PB200_API int pb200_predict_components_device(pb200_ctx* ctx, const pb200_options* opts,
                          const double* d_params, const double* d_tchange,
                          const int32_t* d_meta_i32, const int64_t* d_meta_i64,

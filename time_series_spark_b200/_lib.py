@@ -43,6 +43,22 @@ class Options(C.Structure):
     ]
 
 
+ABI_VERSION_TABLE = 2
+MAX_SEASONALITIES = 8
+
+
+class Seasonality(C.Structure):
+    """struct pb200_seasonality."""
+    _fields_ = [("name", C.c_char * 16), ("period", C.c_double), ("prior_scale", C.c_double),
+                ("fourier_order", C.c_int32), ("reserved", C.c_int32)]
+
+
+class OptionsV2(Options):
+    """struct pb200_options_v2: pb200_options followed by the seasonality table (passed where an Options is taken)."""
+    _fields_ = [("yearly_order", C.c_int32), ("weekly_order", C.c_int32), ("daily_order", C.c_int32),
+                ("n_seasonalities", C.c_int32), ("seasonalities", C.POINTER(Seasonality))]
+
+
 class Layout(C.Structure):
     """struct pb200_layout."""
     _fields_ = [("smax", C.c_int32), ("kmax", C.c_int32), ("pstride", C.c_int32),
@@ -60,6 +76,7 @@ EXPORTS = [
     "pb200_predict_quantiles_host", "pb200_cv_quantile_metrics_device", "pb200_predict_history_device",
     "pb200_predict_history_host", "pb200_outlier_counts_device", "pb200_outlier_compact_device",
     "pb200_predict_period_sums_device", "pb200_predict_period_sums_host", "pb200_period_host",
+    "pb200_last_fit_table_count", "pb200_component_count",
 ]
 CV_ERR_HORIZON, CV_ERR_INITIAL, CV_ERR_FEW = 1, 2, 4
 
@@ -95,6 +112,10 @@ def load() -> C.CDLL:
     lib.pb200_tab_chunk.argtypes = [i32, i32]
     lib.pb200_tab_chunk.restype = i32
     lib.pb200_last_fit_variant_counts.argtypes = [vp, vp]
+    lib.pb200_last_fit_table_count.restype = C.c_int
+    lib.pb200_last_fit_table_count.argtypes = [vp, vp]
+    lib.pb200_component_count.restype = i32
+    lib.pb200_component_count.argtypes = [OP]
     lib.pb200_last_fit_variant_counts.restype = C.c_int
     fit_args = [vp, OP, vp, vp, i32, vp, i64, dbl, dbl, vp, vp, vp, vp, vp, vp]
     lib.pb200_fit_device.argtypes = fit_args

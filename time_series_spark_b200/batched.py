@@ -58,6 +58,105 @@ def make_options(growth: str = "logistic", seasonality_mode: str = "multiplicati
     return o
 
 
+# fbprophet 0.5's validate_column_name: names a seasonality may not take (they are columns of its predict frame)
+_RESERVED_NAMES = frozenset([
+    "trend", "additive_terms", "multiplicative_terms", "holidays", "zeros", "extra_regressors_additive",
+    "extra_regressors_multiplicative", "yhat", "ds", "y", "cap", "floor", "y_scaled", "cap_scaled"])
+
+
+def _number(v, key: str) -> float:
+    if isinstance(v, (bool, np.bool_)) or not isinstance(v, (int, float, np.integer, np.floating)):
+        raise ValueError(f"{key} must be a number (got {v!r})")
+    return float(v)
+
+
+def make_table_options(seasonalities=(), yearly_seasonality="auto", weekly_seasonality="auto",
+                       daily_seasonality="auto", seasonality_mode: str = "multiplicative",
+                       seasonality_prior_scale: float = 10.0, **kw) -> L.OptionsV2:
+    """make_options plus fbprophet's add_seasonality and any built-in Fourier order (DESIGN §18): a pb200_options_v2.
+
+    ``yearly_seasonality`` / ``weekly_seasonality`` / ``daily_seasonality``: 'auto', True, False or an int order (> 0
+    forces it on at that order, 0 is off).  ``seasonalities``: dicts ``{name, period, fourier_order, prior_scale?,
+    mode?}`` in the order they were added; ``prior_scale`` defaults to ``seasonality_prior_scale`` and ``mode`` must be
+    ``seasonality_mode``.  Other keyword arguments are make_options'.  A table that restates the defaults gives the
+    default model; the limits (8 seasonalities, K <= 64, P <= 96) are checked here and by the library."""
+    builtin = {}
+    for key, v, dflt in (("yearly_seasonality", yearly_seasonality, 10), ("weekly_seasonality", weekly_seasonality, 3),
+                         ("daily_seasonality", daily_seasonality, 4)):
+        if isinstance(v, str):
+            if v != "auto":
+                raise ValueError(f"{key} must be 'auto', a bool or an int order (got {v!r})")
+            builtin[key] = ("auto", 0)
+        elif isinstance(v, (bool, np.bool_)):
+            builtin[key] = (bool(v), 0)
+        else:
+            if not isinstance(v, (int, np.integer)):
+                raise ValueError(f"{key} must be 'auto', a bool or an int order (got {v!r})")
+            n = int(v)
+            if n < 0:
+                raise ValueError(f"{key} must be >= 0 (got {n})")
+            builtin[key] = (n > 0, n if n > 0 else 0)
+    o1 = make_options(yearly_seasonality=builtin["yearly_seasonality"][0],
+                      weekly_seasonality=builtin["weekly_seasonality"][0],
+                      daily_seasonality=builtin["daily_seasonality"][0], seasonality_mode=seasonality_mode,
+                      seasonality_prior_scale=seasonality_prior_scale, **kw)
+    o = L.OptionsV2()
+    for name, _ in L.Options._fields_:
+        setattr(o, name, getattr(o1, name))
+    o.abi_version = L.ABI_VERSION_TABLE
+    o.yearly_order = builtin["yearly_seasonality"][1]
+    o.weekly_order = builtin["weekly_seasonality"][1]
+    o.daily_order = builtin["daily_seasonality"][1]
+    seasonalities = list(seasonalities or ())
+    if len(seasonalities) > L.MAX_SEASONALITIES:
+        raise ValueError(f"seasonalities: at most {L.MAX_SEASONALITIES} entries (got {len(seasonalities)})")
+    arr = (L.Seasonality * max(1, len(seasonalities)))()
+    names = set()
+    for i, spec in enumerate(seasonalities):
+        key = f"seasonalities[{i}]"
+        if not isinstance(spec, dict):
+            raise ValueError(f"{key} must be a mapping with name, period and fourier_order")
+        unknown = set(spec) - {"name", "period", "fourier_order", "prior_scale", "mode"}
+        if unknown:
+            raise ValueError(f"{key}: unknown key(s) {sorted(unknown)}")
+        for req in ("name", "period", "fourier_order"):
+            if req not in spec:
+                raise ValueError(f"{key}.{req} is required")
+        name = spec["name"]
+        if not isinstance(name, str) or not name or len(name.encode()) > 15:
+            raise ValueError(f"{key}.name must be a non-empty string of at most 15 bytes (got {name!r})")
+        if name in names:
+            raise ValueError(f"{key}.name: seasonality {name!r} is added twice")
+        if name in _RESERVED_NAMES or name.endswith(("_lower", "_upper")):
+            raise ValueError(f"{key}.name: {name!r} is reserved (fbprophet's validate_column_name)")
+        names.add(name)
+        for b, bkey in (("yearly", "yearly_seasonality"), ("weekly", "weekly_seasonality"), ("daily", "daily_seasonality")):
+            if name == b and builtin[bkey][0] != "auto":
+                raise ValueError(f"{key}.name: {name!r} replaces the built-in only when {bkey} is 'auto'")
+        period = _number(spec["period"], f"{key}.period")
+        if not (np.isfinite(period) and period > 0):
+            raise ValueError(f"{key}.period must be finite and > 0 (got {spec['period']!r})")
+        order = spec["fourier_order"]
+        if isinstance(order, (bool, np.bool_)) or not isinstance(order, (int, np.integer)) or int(order) <= 0:
+            raise ValueError(f"{key}.fourier_order must be an int > 0 (got {order!r})")
+        ps = spec.get("prior_scale")
+        if ps is not None and not (np.isfinite(_number(ps, f"{key}.prior_scale")) and float(ps) > 0):
+            raise ValueError(f"{key}.prior_scale must be > 0 (got {ps!r})")
+        mode = spec.get("mode")
+        if mode is not None and mode != seasonality_mode:
+            raise ValueError(f"{key}.mode: every seasonality takes the model's seasonality_mode {seasonality_mode!r} "
+                             f"(got {mode!r})")
+        arr[i].name = name.encode()
+        arr[i].period = period
+        arr[i].fourier_order = int(order)
+        arr[i].prior_scale = 0.0 if ps is None else float(ps)
+    o.n_seasonalities = len(seasonalities)
+    o.seasonalities = C.cast(arr, C.POINTER(L.Seasonality))
+    o._table = arr      # keeps the entries alive as long as the options
+    L.get_layout(o)     # the library's checks: the limits and the refusals, before any GPU call
+    return o
+
+
 @dataclass
 class FittedBatch:
     """Fitted-model arrays of one shard (numpy on host, or torch tensors on device)."""
@@ -294,15 +393,30 @@ class ForecastBatch:
     yhat_lower: object   # [N, H] f64 or None
     yhat_upper: object
     yhat_int: object     # [N, H] int32 (truncated, floor-clamped)
-    components: object = None   # [6, N, H] f64, planes in L.COMPONENTS order (components=True), else None
+    components: object = None   # [C, N, H] f64, planes in component_names(opts) order (components=True), else None
     trend_lower: object = None  # [N, H] f64 (components=True with intervals), else None
     trend_upper: object = None
     quantiles: object = None    # [Q, N, H] f64 (predict_quantiles_*), else None
+    names: tuple = L.COMPONENTS  # the component planes' names
 
     def component(self, name: str):
         """One component plane by its fbprophet column name (trend, multiplicative_terms, additive_terms, yearly, weekly,
-        daily)."""
-        return self.components[L.COMPONENTS.index(name)]
+        daily, and a seasonality table's custom entries)."""
+        return self.components[self.names.index(name)]
+
+
+def component_names(opts: L.Options) -> tuple:
+    """The planes of pb200_predict_components_* for these options: L.COMPONENTS, then each custom seasonality of a
+    seasonality table not named like a built-in, in table order."""
+    n = L.load().pb200_component_count(C.byref(opts))
+    L.check(min(n, 0), "pb200_component_count")
+    extra = []
+    if getattr(opts, "abi_version", L.ABI_VERSION) == L.ABI_VERSION_TABLE:
+        extra = [opts.seasonalities[i].name.decode() for i in range(opts.n_seasonalities)]
+        extra = [x for x in extra if x not in ("yearly", "weekly", "daily")]
+    names = L.COMPONENTS + tuple(extra)
+    assert len(names) == n
+    return names
 
 
 def make_future(last_ds_ns: np.ndarray, periods: int, freq_ns: int) -> np.ndarray:
@@ -383,7 +497,8 @@ def predict_batch_host(ctx: L.Context, opts: L.Options, fitted: FittedBatch, fut
     do_mc = intervals and opts.uncertainty_samples > 0
     lo = np.empty((n, h), np.float64) if do_mc else None
     hi = np.empty((n, h), np.float64) if do_mc else None
-    comp = np.empty((L.N_COMPONENTS, n, h), np.float64) if components else None
+    names = component_names(opts) if components else L.COMPONENTS
+    comp = np.empty((len(names), n, h), np.float64) if components else None
     tlo = np.empty((n, h), np.float64) if components and do_mc else None
     thi = np.empty((n, h), np.float64) if components and do_mc else None
     if n > 0 and h > 0:
@@ -398,7 +513,8 @@ def predict_batch_host(ctx: L.Context, opts: L.Options, fitted: FittedBatch, fut
             L.check(rc, "pb200_predict_components_host")
         else:
             L.check(L.load().pb200_predict_host(*args), "pb200_predict_host")
-    return ForecastBatch(future_ds, yhat, lo, hi, yint, comp, tlo, thi)
+    return ForecastBatch(future_ds, yhat, lo, hi, yint, comp, tlo, thi,
+                         names=component_names(opts) if components else L.COMPONENTS)
 
 
 def predict_batch_device(ctx: L.Context, opts: L.Options, fitted: FittedBatch, future_ds, floor, cap,
@@ -419,7 +535,7 @@ def predict_batch_device(ctx: L.Context, opts: L.Options, fitted: FittedBatch, f
         yint = torch.empty((n, h), dtype=torch.int32, device=dev)
         lo = torch.empty((n, h), dtype=torch.float64, device=dev) if do_mc else None
         hi = torch.empty((n, h), dtype=torch.float64, device=dev) if do_mc else None
-        comp = torch.empty((L.N_COMPONENTS, n, h), dtype=torch.float64, device=dev) if components else None
+        comp = torch.empty((len(component_names(opts)), n, h), dtype=torch.float64, device=dev) if components else None
         tlo = torch.empty((n, h), dtype=torch.float64, device=dev) if components and do_mc else None
         thi = torch.empty((n, h), dtype=torch.float64, device=dev) if components and do_mc else None
     if n > 0 and h > 0:
@@ -437,7 +553,8 @@ def predict_batch_device(ctx: L.Context, opts: L.Options, fitted: FittedBatch, f
             L.check(L.load().pb200_predict_device(*args), "pb200_predict_device")
         if sync:
             ctx.synchronize()
-    return ForecastBatch(future_ds, yhat, lo, hi, yint, comp, tlo, thi)
+    return ForecastBatch(future_ds, yhat, lo, hi, yint, comp, tlo, thi,
+                         names=component_names(opts) if components else L.COMPONENTS)
 
 
 QUANTILES_MAX = 32

@@ -3,8 +3,8 @@
     python -m time_series_spark_b200.build [--force]
 
 nvcc cross-compiles without a GPU.  The eight seasonality-class translation units
-(fit_inst.cu with -DPB200_MASK=0..7), capi.cu and the grouped-lanes kernels (fit_group_inst.cu) are compiled in
-parallel, then linked.
+(fit_inst.cu with -DPB200_MASK=0..7), capi.cu, the grouped-lanes kernels (fit_group_inst.cu) and the
+seasonality-table class (fit_table.cu) are compiled in parallel, then linked.
 """
 from __future__ import annotations
 
@@ -63,6 +63,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
                       "-o", os.path.join(OBJ, f"fit_inst_{m}.o")]))
     jobs.append([nvcc, *NVCC_FLAGS, "-c", os.path.join(CSRC, "capi.cu"), "-o", os.path.join(OBJ, "capi.o")])
     jobs.append([nvcc, *NVCC_FLAGS, "-c", os.path.join(CSRC, "fit_group_inst.cu"), "-o", os.path.join(OBJ, "fit_group_inst.o")])
+    jobs.append([nvcc, *NVCC_FLAGS, "-c", os.path.join(CSRC, "fit_table.cu"), "-o", os.path.join(OBJ, "fit_table.o")])
     if verbose:
         jobs = [j[:1] + ["-Xptxas", "-v"] + j[1:] for j in jobs]
 
@@ -77,7 +78,8 @@ def build(force: bool = False, verbose: bool = False) -> str:
             if r.returncode != 0:
                 raise RuntimeError("nvcc failed: " + " ".join(cmd))
     objs = [os.path.join(OBJ, f"fit_inst_{m}.o") for m in range(8)] + [os.path.join(OBJ, "capi.o"),
-                                                                      os.path.join(OBJ, "fit_group_inst.o")]
+                                                                      os.path.join(OBJ, "fit_group_inst.o"),
+                                                                      os.path.join(OBJ, "fit_table.o")]
     link = [nvcc, "-shared", *ARCH, "-o", LIB, *objs, "-lcudart"]
     r = subprocess.run(link, capture_output=True, text=True)
     if r.returncode != 0:

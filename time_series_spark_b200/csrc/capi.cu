@@ -147,18 +147,123 @@ const launch_fn LAUNCH[8] = {pb200::launch_fit_mask0, pb200::launch_fit_mask1, p
                              pb200::launch_fit_mask3, pb200::launch_fit_mask4, pb200::launch_fit_mask5,
                              pb200::launch_fit_mask6, pb200::launch_fit_mask7};
 
+int opts_table(const pb200_options* o, pb200::SeasTab* t);
+
 int check_opts(const pb200_options* o) {
     if (!o) return fail(PB200_E_ARG, "options is null");
-    if (o->abi_version != PB200_ABI_VERSION) return fail(PB200_E_ARG, "options.abi_version mismatch");
+    if (o->abi_version != PB200_ABI_VERSION && o->abi_version != PB200_ABI_VERSION_TABLE)
+        return fail(PB200_E_ARG, "options.abi_version mismatch");
     if (o->growth != PB200_GROWTH_LINEAR && o->growth != PB200_GROWTH_LOGISTIC) return fail(PB200_E_ARG, "growth");
     if (o->n_changepoints < 0 || o->n_changepoints > 30) return fail(PB200_E_UNSUPPORTED, "n_changepoints must be in [0, 30]");
     if (o->history_size < 1 || o->history_size > pb200::HMAX) return fail(PB200_E_UNSUPPORTED, "history_size must be in [1, 5]");
     if (!(o->changepoint_range > 0.0 && o->changepoint_range <= 1.0)) return fail(PB200_E_ARG, "changepoint_range");
     if (!(o->changepoint_prior_scale > 0.0) || !(o->seasonality_prior_scale > 0.0)) return fail(PB200_E_ARG, "prior scales");
-    for (int v : {o->yearly, o->weekly, o->daily})
+    for (int v : {o->yearly, o->weekly, o->daily})   // at version 2 the orders are v2's *_order
         if (v != PB200_SEAS_AUTO && v != 0 && v != 1) return fail(PB200_E_UNSUPPORTED, "seasonality switch must be AUTO, 0 or 1");
     if (o->max_iter < 1) return fail(PB200_E_ARG, "max_iter");
     if (o->algorithm < PB200_ALG_LBFGS_NEWTON || o->algorithm > PB200_ALG_NEWTON) return fail(PB200_E_ARG, "algorithm");
+    pb200::SeasTab t;
+    return opts_table(o, &t);
+}
+
+// The seasonality table of *o, normalised to fbprophet's column order (custom entries as added, then yearly, weekly,
+// daily) and checked against the limits.  t->n = 0 for a v1 model and for a v2 one that restates the defaults.
+int opts_table(const pb200_options* o, pb200::SeasTab* t) {
+    t->n = 0;
+    if (o->abi_version != PB200_ABI_VERSION_TABLE) return PB200_OK;
+    const pb200_options_v2* v = reinterpret_cast<const pb200_options_v2*>(o);
+    char msg[160];
+    const int ns = v->n_seasonalities;
+    if (ns < 0 || ns > PB200_MAX_SEASONALITIES) {
+        snprintf(msg, sizeof msg, "n_seasonalities must be in [0, %d] (got %d)", PB200_MAX_SEASONALITIES, ns);
+        return fail(PB200_E_UNSUPPORTED, msg);
+    }
+    if (ns > 0 && !v->seasonalities) return fail(PB200_E_ARG, "seasonalities is null");
+    static const char* const BNAME[3] = {"yearly", "weekly", "daily"};
+    const int dflt[3] = {10, 3, 4}, ord[3] = {v->yearly_order, v->weekly_order, v->daily_order};
+    const int sw[3] = {o->yearly, o->weekly, o->daily};
+    bool replaced[3] = {false, false, false};
+    for (int b = 0; b < 3; ++b)
+        if (ord[b] < 0) {
+            snprintf(msg, sizeof msg, "%s_order must be >= 0 (got %d)", BNAME[b], ord[b]);
+            return fail(PB200_E_ARG, msg);
+        }
+    for (int i = 0; i < ns; ++i) {
+        const pb200_seasonality& e = v->seasonalities[i];
+        const size_t len = strnlen(e.name, sizeof e.name);
+        if (len == 0 || len == sizeof e.name) return fail(PB200_E_ARG, "seasonality name must be 1 to 15 bytes, NUL-terminated");
+        for (int j = 0; j < i; ++j)
+            if (strncmp(e.name, v->seasonalities[j].name, sizeof e.name) == 0) {
+                snprintf(msg, sizeof msg, "seasonality '%s' is added twice", e.name);
+                return fail(PB200_E_ARG, msg);
+            }
+        if (!(e.period > 0.0 && e.period < INFINITY)) {
+            snprintf(msg, sizeof msg, "seasonality '%s': period must be finite and > 0 (got %g)", e.name, e.period);
+            return fail(PB200_E_ARG, msg);
+        }
+        if (e.fourier_order <= 0) {
+            snprintf(msg, sizeof msg, "seasonality '%s': fourier_order must be > 0 (got %d)", e.name, e.fourier_order);
+            return fail(PB200_E_ARG, msg);
+        }
+        if (!(e.prior_scale >= 0.0 && e.prior_scale < INFINITY)) {
+            snprintf(msg, sizeof msg, "seasonality '%s': prior_scale must be > 0 (got %g)", e.name, e.prior_scale);
+            return fail(PB200_E_ARG, msg);
+        }
+        for (int b = 0; b < 3; ++b)
+            if (strcmp(e.name, BNAME[b]) == 0) {
+                if (sw[b] != PB200_SEAS_AUTO) {
+                    snprintf(msg, sizeof msg, "custom seasonality '%s' replaces the built-in only when its switch is AUTO", e.name);
+                    return fail(PB200_E_UNSUPPORTED, msg);
+                }
+                replaced[b] = true;
+            }
+    }
+    bool restates = ns == 0;
+    for (int b = 0; b < 3; ++b) restates = restates && (ord[b] == 0 || ord[b] == dflt[b] || sw[b] == 0);
+    if (restates) return PB200_OK;
+    int n = 0;
+    double ps[PB200_MAX_SEASONALITIES + 3];
+    int order[PB200_MAX_SEASONALITIES + 3], kind[PB200_MAX_SEASONALITIES + 3];
+    double period[PB200_MAX_SEASONALITIES + 3];
+    for (int i = 0; i < ns; ++i) {
+        const pb200_seasonality& e = v->seasonalities[i];
+        period[n] = e.period; order[n] = e.fourier_order; kind[n] = 0;
+        ps[n++] = e.prior_scale > 0.0 ? e.prior_scale : o->seasonality_prior_scale;
+    }
+    const double bper[3] = {365.25, 7.0, 1.0};
+    for (int b = 0; b < 3; ++b) {
+        if (sw[b] == 0 || replaced[b]) continue;
+        period[n] = bper[b]; order[n] = ord[b] > 0 ? ord[b] : dflt[b]; kind[n] = 1 << b;
+        ps[n++] = o->seasonality_prior_scale;
+    }
+    if (n > PB200_MAX_SEASONALITIES) {
+        snprintf(msg, sizeof msg, "the model has %d seasonalities; at most %d", n, PB200_MAX_SEASONALITIES);
+        return fail(PB200_E_UNSUPPORTED, msg);
+    }
+    int K = 0;
+    for (int i = 0; i < n; ++i) K += 2 * order[i];
+    if (K > pb200::SEAS_KMAX) {
+        snprintf(msg, sizeof msg, "the seasonalities have K = %d Fourier columns; at most %d", K, pb200::SEAS_KMAX);
+        return fail(PB200_E_UNSUPPORTED, msg);
+    }
+    const int P = 3 + (o->n_changepoints > 0 ? o->n_changepoints : 1) + K;
+    if (P > pb200::SEAS_PMAX) {
+        snprintf(msg, sizeof msg, "the model has P = 3 + S + K = %d parameters; at most %d", P, pb200::SEAS_PMAX);
+        return fail(PB200_E_UNSUPPORTED, msg);
+    }
+    t->n = n;
+    int extra = 0;
+    for (int i = 0; i < n; ++i) {
+        t->period[i] = period[i];
+        t->order[i] = order[i];
+        t->kind[i] = kind[i];
+        t->inv_sig2[i] = 1.0 / (ps[i] * ps[i]);
+        int pl = -1;
+        for (int b = 0; b < 3; ++b)
+            if (kind[i] == 1 << b || (i < ns && strcmp(v->seasonalities[i].name, BNAME[b]) == 0)) pl = PB200_COMP_YEARLY + b;
+        t->plane[i] = pl >= 0 ? pl : PB200_N_COMPONENTS + extra++;
+    }
+    t->nplanes = PB200_N_COMPONENTS + extra;
     return PB200_OK;
 }
 
@@ -237,6 +342,9 @@ PB200_API int pb200_get_layout(const pb200_options* o, pb200_layout* out) {
     if (o->yearly != 0) k += 20;
     if (o->weekly != 0) k += 6;
     if (o->daily != 0) k += 8;
+    pb200::SeasTab t;
+    opts_table(o, &t);
+    if (t.n > 0) k = pb200::tab_k(t, (1 << t.n) - 1);
     out->kmax = k > 0 ? k : 1;
     out->pstride = 3 + out->smax + out->kmax;
     out->meta_i32_stride = 8;
@@ -325,6 +433,26 @@ PB200_API int pb200_last_fit_variant_counts(pb200_ctx* c, int32_t* h_counts) {
     return PB200_OK;
 }
 
+PB200_API int32_t pb200_component_count(const pb200_options* o) {
+    int rc = check_opts(o);
+    if (rc) return rc;
+    pb200::SeasTab t;
+    opts_table(o, &t);
+    return t.n > 0 ? t.nplanes : PB200_N_COMPONENTS;
+}
+
+PB200_API int pb200_last_fit_table_count(pb200_ctx* c, int64_t* h_count) {
+    if (!c || !h_count) return fail(PB200_E_ARG, "null argument");
+    *h_count = 0;
+    if (!c->d_vcount.p) return PB200_OK;      // no fit yet
+    int32_t n = 0;
+    CK(cudaSetDevice(c->device));
+    CK(cudaStreamSynchronize(c->stream));
+    CK(cudaMemcpy(&n, (const int32_t*)c->d_vcount.p + NQ, 4, cudaMemcpyDeviceToHost));
+    *h_count = n;
+    return PB200_OK;
+}
+
 PB200_API int pb200_synchronize(pb200_ctx* c) {
     if (!c) return fail(PB200_E_ARG, "ctx is null");
     CK(cudaSetDevice(c->device));
@@ -338,7 +466,7 @@ PB200_API int pb200_synchronize(pb200_ctx* c) {
 static int launch_newton(pb200_ctx* c, const pb200_options* opts, const int64_t* d_ds, const void* d_y,
                          int32_t y_dtype, const int64_t* d_offsets, int64_t n_series, int* d_nq, const double* d_prior,
                          const double* d_x0, double* d_params, double* d_tchange, int32_t* d_meta_i32, int64_t* d_meta_i64, double* d_meta_f64) {
-    static_assert(30 + 34 + 3 <= pb200::nw::NW_PMAX, "newton_kernel holds every P check_opts admits");
+    static_assert(pb200::SEAS_PMAX <= pb200::nw::NW_PMAX, "newton_kernel holds every P check_opts admits");
     pb200_layout L;
     pb200_get_layout(opts, &L);
     if (opts->algorithm == PB200_ALG_LBFGS) return PB200_OK;
@@ -361,6 +489,7 @@ static int launch_newton(pb200_ctx* c, const pb200_options* opts, const int64_t*
     na.prior = d_prior;
     na.x0 = d_x0;
     na.o = to_dev(opts);
+    opts_table(opts, &na.tab);
     const size_t nsm = pb200::nw::newton_smem_bytes(L.pstride);
     CK(cudaFuncSetAttribute(pb200::nw::newton_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)nsm));
     int ngrid = (int)std::min<int64_t>(n_series, opts->algorithm == PB200_ALG_NEWTON ? (int64_t)c->sms * 2 : (int64_t)c->sms);
@@ -382,10 +511,17 @@ static int fit_impl(pb200_ctx* c, const pb200_options* opts, const int64_t* d_ds
                     const int32_t* d_init_meta = nullptr, int32_t* d_warm = nullptr) {
     if (!c) return fail(PB200_E_ARG, "ctx is null");
     CK(cudaSetDevice(c->device));
-    CK(c->d_vcount.reserve(NQ * 4));
-    CK(cudaMemsetAsync(c->d_vcount.p, 0, NQ * 4, c->stream));
+    CK(c->d_vcount.reserve((NQ + 1) * 4));     // [NQ]: the table class
+    CK(cudaMemsetAsync(c->d_vcount.p, 0, (NQ + 1) * 4, c->stream));
     int rc = check_opts(opts);
     if (rc) return rc;
+    pb200::SeasTab tab;
+    opts_table(opts, &tab);
+    if (tab.n > 0) {
+        if (d_prior) return fail(PB200_E_UNSUPPORTED, "per-series prior scales are not supported with a seasonality table");
+        if (d_init_params) return fail(PB200_E_UNSUPPORTED, "warm start is not supported with a seasonality table");
+    }
+    const int NQT = NLC * NQ + 1;    // the work queues: (length class, variant, mask), then the table class
     if (n_series < 0 || n_series > (1LL << 30)) return fail(PB200_E_ARG, "n_series");
     if (n_series == 0) return PB200_OK;
     if (!d_ds || !d_y || !h_offsets || !d_params || !d_tchange || !d_meta_i32 || !d_meta_i64 || !d_meta_f64)
@@ -442,12 +578,12 @@ static int fit_impl(pb200_ctx* c, const pb200_options* opts, const int64_t* d_ds
     CK(c->d_offsets.reserve((size_t)(N + 1) * 8));
     CK(c->d_order.reserve((size_t)N * 4));
     CK(c->d_lenclass.reserve((size_t)N * 4));
-    CK(c->d_qitems.reserve((size_t)NLC * NQ * N * 4));
-    CK(c->d_qctl.reserve((size_t)NLC * NQ * 2 * 4));
+    CK(c->d_qitems.reserve((size_t)NQT * N * 4));
+    CK(c->d_qctl.reserve((size_t)NQT * 2 * 4));
     CK(c->d_qkey.reserve((size_t)N * 4));
-    CK(c->d_qhist.reserve((size_t)NLC * NQ * pb200::QBINS * 4));
+    CK(c->d_qhist.reserve((size_t)NQT * pb200::QBINS * 4));
     CK(cudaMemsetAsync(c->d_qkey.p, 0xff, (size_t)N * 4, c->stream));
-    CK(cudaMemsetAsync(c->d_qhist.p, 0, (size_t)NLC * NQ * pb200::QBINS * 4, c->stream));
+    CK(cudaMemsetAsync(c->d_qhist.p, 0, (size_t)NQT * pb200::QBINS * 4, c->stream));
     CK(c->d_nq.reserve((size_t)(N + 2) * 4));             // count, head, items[N]
     int* nq = (int*)c->d_nq.p;
     CK(cudaMemsetAsync(nq, 0, 8, c->stream));
@@ -456,11 +592,11 @@ static int fit_impl(pb200_ctx* c, const pb200_options* opts, const int64_t* d_ds
     CK(cudaMemcpyAsync(c->d_lenclass.p, hlc, (size_t)N * 4, cudaMemcpyHostToDevice, c->stream));
     CK(cudaEventRecord(c->ctl_ev, c->stream));
     c->ctl_pending = true;
-    CK(cudaMemsetAsync(c->d_qctl.p, 0, (size_t)NLC * NQ * 2 * 4, c->stream));
+    CK(cudaMemsetAsync(c->d_qctl.p, 0, (size_t)NQT * 2 * 4, c->stream));
     CK(cudaMemsetAsync(d_params, 0, (size_t)N * L.pstride * 8, c->stream));
     CK(cudaMemsetAsync(d_tchange, 0, (size_t)N * L.smax * 8, c->stream));
     int* q_count = (int*)c->d_qctl.p;
-    int* q_head = q_count + NLC * NQ;
+    int* q_head = q_count + NQT;
 
     const FitOptsDev od = to_dev(opts);
     // lanes per series of the grouped day-table kernel
@@ -503,12 +639,14 @@ static int fit_impl(pb200_ctx* c, const pb200_options* opts, const int64_t* d_ds
         pa.warm = d_warm;
         pa.smax = L.smax;
         pa.pstride = L.pstride;
+        pa.tab = tab;
+        pa.tab_queue = NLC * NQ;
         const int warps_per_block = 8;
         int grid = (N + warps_per_block - 1) / warps_per_block;
         grid = std::min(grid, c->sms * 8);
         pb200::prep_kernel<<<grid, warps_per_block * 32, 0, c->stream>>>(pa);
         CK(cudaGetLastError());
-        pb200::queue_scan_kernel<<<(NLC * NQ + 127) / 128, 128, 0, c->stream>>>((int*)c->d_qhist.p, NLC * NQ);
+        pb200::queue_scan_kernel<<<(NQT + 127) / 128, 128, 0, c->stream>>>((int*)c->d_qhist.p, NQT);
         CK(cudaGetLastError());
         pb200::queue_scatter_kernel<<<std::min((N + 255) / 256, c->sms * 8), 256, 0, c->stream>>>(
             (const int*)c->d_qkey.p, (int*)c->d_qhist.p, (int*)c->d_qitems.p, N);
@@ -527,7 +665,7 @@ static int fit_impl(pb200_ctx* c, const pb200_options* opts, const int64_t* d_ds
             Geo& g = geo[lc][rm];
             g.on = false;
             g.grouped = false;
-            if (lc_n[lc] == 0) continue;
+            if (lc_n[lc] == 0 || tab.n > 0) continue;
             const bool plain_grp = reg == 3 && mask == 0 && grp_g > 0 && c->plain_grp;   // grouped kernel's class without seasonality
             if (reg && mask == 0 && !plain_grp) continue;                // no Fourier features: nothing to regenerate
             if (reg >= 2 && ((mask != 6 && !plain_grp) || LC_NT[lc] != 32 || !c->tab_on)) continue;   // seasonal-table variants
@@ -564,8 +702,58 @@ static int fit_impl(pb200_ctx* c, const pb200_options* opts, const int64_t* d_ds
             planes_bytes += (size_t)g.grid * g.slice * 16;
             g.on = true;
         }
+    // the table class: one warp per series, (t, y) and one base (sin, cos) plane per table entry in each slice
+    int tab_grid = 0, tab_Tp = 0, tab_ppad = 0;
+    size_t tab_smem = 0, tab_off = 0;
+    if (tab.n > 0) {
+        tab_Tp = (int)(((tmax_all + (tmax_all + 31) / 32 + 7) / 8) * 8);
+        tab_ppad = (L.pstride + 1) & ~1;
+        tab_smem = pb200::fit_table_smem(tab_ppad);
+        int occ = 0;
+        pb200::TableFitArgs dummy{};
+        CK(pb200::launch_fit_table(opts->growth, dummy, 0, tab_smem, c->stream, &occ));
+        if (occ < 1) return fail(PB200_E_UNSUPPORTED, "table fit kernel does not fit on an SM");
+        tab_grid = cap_grid(std::min<int64_t>((int64_t)N, (int64_t)c->sms * occ));
+        tab_off = planes_bytes;
+        planes_bytes += (size_t)tab_grid * (1 + tab.n) * tab_Tp * 16;
+    }
     CK(c->d_planes.reserve(planes_bytes));
-    for (int lc = 0; lc < NLC; ++lc) {
+    if (tab.n > 0) {
+        pb200::TableFitArgs fa;
+        fa.ds = (const long long*)d_ds;
+        fa.y = d_y;
+        fa.y_dtype = y_dtype;
+        fa.offsets = (const long long*)c->d_offsets.p;
+        const int q = NLC * NQ;
+        fa.q_items = (const int*)c->d_qitems.p + (size_t)q * N;
+        fa.q_count = q_count + q;
+        fa.q_head = q_head + q;
+        fa.params = d_params;
+        fa.tchange = d_tchange;
+        fa.meta_i32 = d_meta_i32;
+        fa.meta_i64 = (long long*)d_meta_i64;
+        fa.meta_f64 = d_meta_f64;
+        fa.smax = L.smax;
+        fa.kmax = L.kmax;
+        fa.pstride = L.pstride;
+        fa.Tp = tab_Tp;
+        fa.ppad = tab_ppad;
+        fa.planes = (double2*)((char*)c->d_planes.p + tab_off);
+        fa.nseas_stride = (1 + tab.n) * tab_Tp;
+        fa.theta_in = d_theta_in;
+        fa.grad_out = d_grad_out;
+        fa.trace = d_trace;
+        fa.trace_cap = trace_cap;
+        fa.nq_count = nq;
+        fa.nq_items = opts->algorithm == PB200_ALG_LBFGS_NEWTON ? nq + 2 : nullptr;
+        fa.o = od;
+        fa.l2_keep = fa.l2_rest_first = 0;
+        fa.prior = nullptr;
+        fa.tab = tab;
+        CK(pb200::launch_fit_table(opts->growth, fa, tab_grid, tab_smem, c->stream, nullptr));
+        c->launches++;
+    }
+    for (int lc = 0; lc < NLC && tab.n == 0; ++lc) {
         if (lc_n[lc] == 0) continue;
         const int NT = LC_NT[lc];
         for (int rm = 0; rm < NQ; ++rm) {
@@ -903,8 +1091,9 @@ int predict_device(pb200_ctx* c, const pb200_options* opts, const double* d_para
     if (mc && (rc = check_mc_opts(opts))) return rc;
     pb200_layout L;
     pb200_get_layout(opts, &L);
-    CK(cudaSetDevice(c->device));
     pb200::PredictArgs a;
+    opts_table(opts, &a.tab);
+    CK(cudaSetDevice(c->device));
     a.params = d_params;
     a.tchange = d_tchange;
     a.meta_i32 = d_meta_i32;
@@ -1017,7 +1206,8 @@ int predict_host(pb200_ctx* c, const pb200_options* opts, const double* h_params
         CK(c->d_lo.reserve(NH * 8));
         CK(c->d_hi.reserve(NH * 8));
     }
-    if (h_comp) CK(c->d_comp.reserve(NH * 8 * PB200_N_COMPONENTS));
+    const int ncomp = pb200_component_count(opts);
+    if (h_comp) CK(c->d_comp.reserve(NH * 8 * ncomp));
     QuantOut dquant;
     if (quant) {
         CK(c->d_quant.reserve(NH * 8 * (size_t)quant->n_q));
@@ -1061,7 +1251,7 @@ int predict_host(pb200_ctx* c, const pb200_options* opts, const double* h_params
         CK(cudaMemcpyAsync(h_yhat_lower, c->d_lo.p, NH * 8, cudaMemcpyDeviceToHost, st));
         CK(cudaMemcpyAsync(h_yhat_upper, c->d_hi.p, NH * 8, cudaMemcpyDeviceToHost, st));
     }
-    if (h_comp) CK(cudaMemcpyAsync(h_comp, c->d_comp.p, NH * 8 * PB200_N_COMPONENTS, cudaMemcpyDeviceToHost, st));
+    if (h_comp) CK(cudaMemcpyAsync(h_comp, c->d_comp.p, NH * 8 * ncomp, cudaMemcpyDeviceToHost, st));
     if (quant) CK(cudaMemcpyAsync(quant->planes, dquant.planes, NH * 8 * (size_t)quant->n_q, cudaMemcpyDeviceToHost, st));
     if (h_tlo) {
         CK(cudaMemcpyAsync(h_tlo, c->d_tlo.p, NH * 8, cudaMemcpyDeviceToHost, st));
@@ -1548,6 +1738,7 @@ int predict_history_device(pb200_ctx* c, const pb200_options* opts, const double
     CK(c->d_hoff.reserve((N + 1) * 8));
     CK(cudaMemcpyAsync(c->d_hoff.p, h_offsets, (N + 1) * 8, cudaMemcpyHostToDevice, c->stream));
     pb200::RaggedPredictArgs a;
+    opts_table(opts, &a.tab);
     a.params = d_params;
     a.tchange = d_tchange;
     a.meta_i32 = d_meta_i32;

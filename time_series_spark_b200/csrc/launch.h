@@ -15,3 +15,11 @@ namespace pb200 {
 cudaError_t launch_fit_group(int g, int logi, int mult, int seas, const FitArgs& a, int grid, cudaStream_t st, int* occ);
 size_t fit_group_plane_doubles(int tmax, int g);      // global workspace per series slot (y pairs + L-BFGS history)
 }  // namespace pb200
+
+namespace pb200 {
+// fit class of the models with a seasonality table (fit_table.cu): one warp per series, dynamic shared memory of
+// fit_table_smem(ppad) bytes
+struct TableFitArgs;
+cudaError_t launch_fit_table(int logi, const TableFitArgs& a, int grid, size_t smem, cudaStream_t st, int* occ);
+size_t fit_table_smem(int ppad);
+}  // namespace pb200

@@ -23,7 +23,7 @@ namespace pb200 {
 namespace nw {
 
 constexpr int NW_WARPS = 16;
-constexpr int NW_PMAX = 68;          // S + K + 3 <= 30 + 34 + 3 = 67 (yearly + weekly + daily, 30 changepoints)
+constexpr int NW_PMAX = SEAS_PMAX;   // S + K + 3 <= 96: a seasonality table's limit (default models: 30 + 34 + 3 = 67)
 constexpr int NW_SEG = 32;
 
 struct NewtonArgs {
@@ -43,6 +43,7 @@ struct NewtonArgs {
     const double* prior;     // per-series prior scales (FitArgs::prior); null: o's
     const double* x0;        // warm start points (PrepArgs::warm_x, k = NaN: cold); null: every series from stan_init
     FitOptsDev o;
+    SeasTab tab;             // the models' seasonality table (n = 0: the compiled-in orders); mask = the table mask
 };
 
 struct WarpScratch {     // per warp
@@ -61,6 +62,7 @@ struct Series {          // per CTA
     double x[NW_PMAX], g0[NW_PMAX], u[NW_PMAX], w[NW_PMAX], xn[NW_PMAX];
     double f, f0, f1, last;
     int it, nev, status, moved, stop, err;
+    double isig[SEAS_KMAX];      // a table model's 1 / prior_scale^2 per packed column
 };
 
 inline size_t newton_smem_bytes(int P) {
@@ -99,9 +101,10 @@ __device__ __noinline__ void nw_eval(const NewtonArgs& a, const Series& sr, Warp
     int j = 0;
     for (int s = 0; s < S; ++s) j += sr.bidx[s] < i0 ? 1 : 0;
     const int j0 = j;
-    double gb[34];                                   // fixed layout: yearly 0..19, weekly 20..25, daily 26..33
+    const bool tab = a.tab.n > 0;
+    double gb[SEAS_KMAX];      // fixed layout: yearly 0..19, weekly 20..25, daily 26..33; a table model: its packed columns
 #pragma unroll
-    for (int q = 0; q < 34; ++q) gb[q] = 0.0;
+    for (int q = 0; q < SEAS_KMAX; ++q) gb[q] = 0.0;
     double ss = 0.0, locU = 0.0, locV = 0.0;
     const double dspan = (double)sr.span;
     const double* beta = th + 3 + S;
@@ -112,24 +115,42 @@ __device__ __noinline__ void nw_eval(const NewtonArgs& a, const Series& sr, Warp
         const long long d = a.ds[sr.off + i];
         const double t = (double)(d - sr.start) / dspan;
         const double yv = (load_y(a.y, a.y_dtype, sr.off + i) - sr.fl) / sr.y_scale;
-        double Xy[20], Xw[6], Xd[8];
+        double Xy[20], Xw[6], Xd[8], Xt[SEAS_KMAX];
         double dot = 0.0;
         const double tau_d = (1e-9 * (double)d) / 86400.0;
-        if (sr.mask & 1) {
+        if (tab) {
+            // the active entries in column order: one sincos per seasonality, harmonics by the three-term recurrence
+            int col = 0;
+            for (int e = 0; e < a.tab.n; ++e) {
+                if (!((sr.mask >> e) & 1)) continue;
+                double s_, c_;
+                sincos(TWO_PI_FL * tau_d / a.tab.period[e], &s_, &c_);
+                const double c2 = c_ + c_;
+                double sp = 0.0, cp = 1.0, sn = s_, cn = c_;
+                for (int h = 0; h < a.tab.order[e]; ++h, col += 2) {
+                    Xt[col] = sn;
+                    Xt[col + 1] = cn;
+                    const double s2 = fma(c2, sn, -sp), cc = fma(c2, cn, -cp);
+                    sp = sn; cp = cn; sn = s2; cn = cc;
+                }
+            }
+            for (int q = 0; q < Kreal; ++q) dot = fma(Xt[q], beta[q], dot);
+        }
+        if (!tab && (sr.mask & 1)) {
             double s_, c_;
             sincos(TWO_PI_FL * tau_d / 365.25, &s_, &c_);
             harmonics<10>(make_double2(s_, c_), Xy);
 #pragma unroll
             for (int q = 0; q < 20; ++q) dot = fma(Xy[q], beta[q], dot);
         }
-        if (sr.mask & 2) {
+        if (!tab && (sr.mask & 2)) {
             double s_, c_;
             sincos(TWO_PI_FL * tau_d / 7.0, &s_, &c_);
             harmonics<3>(make_double2(s_, c_), Xw);
 #pragma unroll
             for (int q = 0; q < 6; ++q) dot = fma(Xw[q], beta[bw + q], dot);
         }
-        if (sr.mask & 4) {
+        if (!tab && (sr.mask & 4)) {
             double s_, c_;
             sincos(TWO_PI_FL * tau_d / 1.0, &s_, &c_);
             harmonics<4>(make_double2(s_, c_), Xd);
@@ -146,15 +167,17 @@ __device__ __noinline__ void nw_eval(const NewtonArgs& a, const Series& sr, Warp
         const double r = yv - yhat;
         ss = fma(r, r, ss);
         const double cb = sr.mult ? r * gtr : r;
-        if (sr.mask & 1) {
+        if (tab) {
+            for (int q = 0; q < Kreal; ++q) gb[q] = fma(cb, Xt[q], gb[q]);
+        } else if (sr.mask & 1) {
 #pragma unroll
             for (int q = 0; q < 20; ++q) gb[q] = fma(cb, Xy[q], gb[q]);
         }
-        if (sr.mask & 2) {
+        if (!tab && (sr.mask & 2)) {
 #pragma unroll
             for (int q = 0; q < 6; ++q) gb[20 + q] = fma(cb, Xw[q], gb[20 + q]);
         }
-        if (sr.mask & 4) {
+        if (!tab && (sr.mask & 4)) {
 #pragma unroll
             for (int q = 0; q < 8; ++q) gb[26 + q] = fma(cb, Xd[q], gb[26 + q]);
         }
@@ -174,7 +197,9 @@ __device__ __noinline__ void nw_eval(const NewtonArgs& a, const Series& sr, Warp
     // boundaries beyond the last point owned by anybody cannot occur (changepoints lie in the first 80 % of the history)
     if (lane == 31) { ws.U[S] = incU; ws.V[S] = incV; }
     ss = wsum(ss);
-    if (Kreal) {
+    if (tab) {
+        for (int q = 0; q < Kreal; ++q) gb[q] = wsum(gb[q]);
+    } else if (Kreal) {
 #pragma unroll
         for (int q = 0; q < 34; ++q) gb[q] = wsum(gb[q]);
     }
@@ -225,6 +250,12 @@ __device__ __noinline__ void nw_eval(const NewtonArgs& a, const Series& sr, Warp
             const double b = beta[0];
             g[3 + S] = b * isg;
             pb = 0.5 * b * b * isg;
+        } else if (tab) {
+            for (int c = 0; c < Kreal; ++c) {
+                const double b = beta[c];
+                g[3 + S + c] = scale * gb[c] + b * sr.isig[c];
+                pb += 0.5 * b * b * sr.isig[c];
+            }
         } else {
 #pragma unroll
             for (int q = 0; q < 34; ++q) {
@@ -313,6 +344,13 @@ __global__ void __launch_bounds__(32 * NW_WARPS, 1) newton_kernel(const NewtonAr
         if (tid == 0) {
             sr.T = mi[0]; sr.S = mi[1]; sr.ncp = mi[2]; sr.mask = mi[3];
             sr.K = sr.mask ? ((sr.mask & 1) ? 20 : 0) + ((sr.mask & 2) ? 6 : 0) + ((sr.mask & 4) ? 8 : 0) : 1;
+            if (a.tab.n > 0) {
+                const int K = tab_k(a.tab, sr.mask);
+                sr.K = K > 0 ? K : 1;
+                for (int e = 0, c = 0; e < a.tab.n; ++e)
+                    if ((sr.mask >> e) & 1)
+                        for (int q = 0; q < 2 * a.tab.order[e]; ++q) sr.isig[c++] = a.tab.inv_sig2[e];
+            }
             sr.P = sr.S + sr.K + 3;
             sr.logistic = a.o.growth == PB200_GROWTH_LOGISTIC;
             sr.mult = a.o.mult;

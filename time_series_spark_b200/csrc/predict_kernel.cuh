@@ -16,6 +16,7 @@
 #include <type_traits>
 
 #include "../../include/prophet_b200.h"
+#include "seas_table.cuh"
 
 namespace pb200 {
 
@@ -36,6 +37,8 @@ struct PredictArgs {
     // planes after it, at a stride of n_models * horizon (PB200_COMP_* order)
     double* trend;
     int* yhat_int;
+    // the models' seasonality table (n = 0: the compiled-in orders); a model's meta_i32[3] is then its table mask
+    SeasTab tab;
 };
 
 // The ragged instances (pb200_predict_history_*): model i's frame is rows [offsets[i], offsets[i + 1]) of future_ds and of
@@ -89,7 +92,11 @@ struct ModelSm {
     double delta[32];
     double tc[32];
     double gamma[32];
-    double beta[40];
+    double beta[SEAS_KMAX];
+    // seasonality table (tn = 0: the compiled-in orders)
+    int tn;
+    int order[SEAS_TMAX], plane[SEAS_TMAX];
+    double period[SEAS_TMAX];
 };
 
 __device__ __forceinline__ void load_model(ModelSm& ms, const PredictArgs& a, const int model, const int tid, const int nt) {
@@ -113,13 +120,22 @@ __device__ __forceinline__ void load_model(ModelSm& ms, const PredictArgs& a, co
         if (ms.mask & 1) K += 20;
         if (ms.mask & 2) K += 6;
         if (ms.mask & 4) K += 8;
+        ms.tn = a.tab.n;
+        if (a.tab.n > 0) {
+            K = tab_k(a.tab, ms.mask);
+            for (int e = 0; e < a.tab.n; ++e) {
+                ms.order[e] = a.tab.order[e];
+                ms.period[e] = a.tab.period[e];
+                ms.plane[e] = a.tab.plane[e];
+            }
+        }
         ms.K = K;
     }
     for (int s = tid; s < 32; s += nt) {
         ms.delta[s] = s < a.smax ? pr[3 + s] : 0.0;
         ms.tc[s] = s < a.smax ? a.tchange[(size_t)model * a.smax + s] : 0.0;
     }
-    for (int q = tid; q < 40; q += nt) ms.beta[q] = q < a.kmax ? pr[3 + a.smax + q] : 0.0;
+    for (int q = tid; q < SEAS_KMAX; q += nt) ms.beta[q] = q < a.kmax ? pr[3 + a.smax + q] : 0.0;
     __syncthreads();
     if (tid == 0) {
         const int S = ms.S;
@@ -147,6 +163,14 @@ __device__ __forceinline__ double seasonal_term(const ModelSm& ms, const long lo
     const double tau = (1e-9 * (double)d) / 86400.0;
     double acc = 0.0;
     int col = 0;
+    if (ms.tn > 0) {     // a table model: its active entries in column order
+        for (int e = 0; e < ms.tn; ++e) {
+            if (!((ms.mask >> e) & 1)) continue;
+            acc += seas_dot(tau, ms.period[e], ms.order[e], ms.beta + col);
+            col += 2 * ms.order[e];
+        }
+        return acc;
+    }
     if (ms.mask & 1) { acc += seas_dot(tau, 365.25, 10, ms.beta + col); col += 20; }
     if (ms.mask & 2) { acc += seas_dot(tau, 7.0, 3, ms.beta + col); col += 6; }
     if (ms.mask & 4) { acc += seas_dot(tau, 1.0, 4, ms.beta + col); col += 8; }
@@ -157,10 +181,11 @@ __device__ __forceinline__ double seasonal_term(const ModelSm& ms, const long lo
 // the same order, so it is seasonal_term's value bit for bit
 __device__ __forceinline__ double seasonal_parts(const ModelSm& ms, const long long d, double* yearly, double* weekly,
                                                  double* daily) {
+    *yearly = *weekly = *daily = 0.0;
+    if (ms.tn > 0) return seasonal_term(ms, d);    // a table model: predict_kernel<true> writes its planes per entry
     const double tau = (1e-9 * (double)d) / 86400.0;
     double acc = 0.0;
     int col = 0;
-    *yearly = *weekly = *daily = 0.0;
     if (ms.mask & 1) { *yearly = seas_dot(tau, 365.25, 10, ms.beta + col); acc += *yearly; col += 20; }
     if (ms.mask & 2) { *weekly = seas_dot(tau, 7.0, 3, ms.beta + col); acc += *weekly; col += 6; }
     if (ms.mask & 4) { *daily = seas_dot(tau, 1.0, 4, ms.beta + col); acc += *daily; col += 8; }
@@ -192,8 +217,8 @@ __global__ void __launch_bounds__(256) predict_kernel(const PredictArgsT<RAGGED>
             a.yhat[o] = NAN;
             if (RAGGED) continue;
             if (COMP) {
-#pragma unroll
-                for (int c = 0; c < PB200_N_COMPONENTS; ++c) a.trend[c * plane + o] = NAN;
+                const int nc = a.tab.n > 0 ? a.tab.nplanes : PB200_N_COMPONENTS;
+                for (int c = 0; c < nc; ++c) a.trend[c * plane + o] = NAN;
             } else if (a.trend) {
                 a.trend[o] = NAN;
             }
@@ -226,9 +251,28 @@ __global__ void __launch_bounds__(256) predict_kernel(const PredictArgsT<RAGGED>
             a.trend[o] = tr;
             a.trend[PB200_COMP_MULTIPLICATIVE * plane + o] = a.mult ? sd : 0.0;
             a.trend[PB200_COMP_ADDITIVE * plane + o] = a.mult ? 0.0 : add;
-            a.trend[PB200_COMP_YEARLY * plane + o] = cy * s;
-            a.trend[PB200_COMP_WEEKLY * plane + o] = cw * s;
-            a.trend[PB200_COMP_DAILY * plane + o] = cd * s;
+            if (ms.tn > 0) {
+                // a table model: each entry's X_c beta_c into its plane (seasonal_term's terms, in table order); the
+                // built-in planes no entry fills are 0
+                const double tau = (1e-9 * (double)d) / 86400.0;
+                unsigned filled = 0;
+                int col = 0;
+                for (int e = 0; e < ms.tn; ++e) {
+                    double v = 0.0;
+                    if ((ms.mask >> e) & 1) {
+                        v = seas_dot(tau, ms.period[e], ms.order[e], ms.beta + col);
+                        col += 2 * ms.order[e];
+                    }
+                    a.trend[ms.plane[e] * plane + o] = v * s;
+                    filled |= 1u << ms.plane[e];
+                }
+                for (int c = PB200_COMP_YEARLY; c <= PB200_COMP_DAILY; ++c)
+                    if (!((filled >> c) & 1)) a.trend[c * plane + o] = 0.0;
+            } else {
+                a.trend[PB200_COMP_YEARLY * plane + o] = cy * s;
+                a.trend[PB200_COMP_WEEKLY * plane + o] = cw * s;
+                a.trend[PB200_COMP_DAILY * plane + o] = cd * s;
+            }
         }
         a.yhat[o] = yh;
         if (RAGGED) continue;
