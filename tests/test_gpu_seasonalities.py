@@ -178,31 +178,6 @@ def test_series_alone_and_in_a_batch_give_the_same_bits(gpu_ctx):
         assert np.array_equal(one.params[0], fa.params[i]) and np.array_equal(one.meta_f64[0], fa.meta_f64[i])
 
 
-def _table_seasonal(opts):
-    """mc_stream's seasonal term for a table model: the active entries of the table mask in table order."""
-    from seasonality_table import BUILTINS
-    ents = [(opts.seasonalities[i].period, opts.seasonalities[i].fourier_order) for i in range(opts.n_seasonalities)]
-    names = {opts.seasonalities[i].name.decode() for i in range(opts.n_seasonalities)}
-    for (name, period, order), sw, o in zip(BUILTINS, (opts.yearly, opts.weekly, opts.daily),
-                                            (opts.yearly_order, opts.weekly_order, opts.daily_order)):
-        if sw != 0 and name not in names:
-            ents.append((period, o or order))
-
-    def seasonal(ds_ns, mask, beta):
-        tau = (1e-9 * np.asarray(ds_ns, np.int64).astype(np.float64)) / 86400.0
-        acc, col = np.zeros(tau.size), 0
-        for e, (period, order) in enumerate(ents):
-            if (mask >> e) & 1:
-                blk = np.zeros(tau.size)
-                for i in range(order):
-                    arg = (2.0 * (i + 1)) * np.pi * tau / period
-                    blk = blk + np.sin(arg) * beta[col + 2 * i] + np.cos(arg) * beta[col + 2 * i + 1]
-                acc = acc + blk
-                col += 2 * order
-        return acc
-    return seasonal
-
-
 @pytest.mark.parametrize("table, growth, mode", [("monthly", "logistic", "multiplicative"), ("k64", "linear", "additive"),
                                                  ("quarterly", "logistic", "additive")])
 def test_bounds_and_window_sums_match_mc_stream(gpu_ctx, monkeypatch, table, growth, mode):
@@ -218,7 +193,7 @@ def test_bounds_and_window_sums_match_mc_stream(gpu_ctx, monkeypatch, table, gro
     fc = batched.predict_batch_host(gpu_ctx, opts, fb, fut, fl, cap32, seed=7, intervals=True)
     fs, ws = batched.predict_sums_host(gpu_ctx, opts, fb, fut, fl, cap32, 7 * DAY, seed=7, intervals=True)
     assert np.array_equal(fs.yhat, fc.yhat)
-    monkeypatch.setattr(mc_stream, "_seasonal", _table_seasonal(opts))
+    monkeypatch.setattr(mc_stream, "_seasonal", st.table_seasonal(opts, "numpy"))
     for i in range(b.n):
         ys = fb.meta_f64[i, 0]
         d = mc_stream.draws(fb, i, fut[i], 0.0, cap32[i], growth == "logistic", mode == "multiplicative",
