@@ -157,6 +157,60 @@ def make_table_options(seasonalities=(), yearly_seasonality="auto", weekly_seaso
     return o
 
 
+_BUILTINS = (("yearly", 1, 365.25, 10), ("weekly", 2, 7.0, 3), ("daily", 4, 1.0, 4))
+
+
+def is_table(opts) -> bool:
+    """Whether ``opts`` is a pb200_options_v2 whose table is not a restatement of the default model."""
+    return seasonality_table(opts) is not None
+
+
+def seasonality_table(opts):
+    """The seasonality table of ``opts`` as the library normalises it (DESIGN §18): a list of entries
+    ``(name, period, fourier_order, kind)`` in column order -- the custom entries as added, then the built-ins that are
+    not off and not replaced by a custom entry of their name -- where ``kind`` is 0 for a custom entry and the built-in's
+    mask bit (1 yearly, 2 weekly, 4 daily) otherwise.  None for v1 options and for a table that restates the defaults
+    (the v1 model)."""
+    if getattr(opts, "abi_version", L.ABI_VERSION) != L.ABI_VERSION_TABLE:
+        return None
+    custom = [opts.seasonalities[i] for i in range(opts.n_seasonalities)]
+    orders = (opts.yearly_order, opts.weekly_order, opts.daily_order)
+    switches = (opts.yearly, opts.weekly, opts.daily)
+    if not custom and all(o == 0 or o == d or s == 0 for o, s, (_, _, _, d) in zip(orders, switches, _BUILTINS)):
+        return None
+    names = [e.name.decode() for e in custom]
+    out = [(e.name.decode(), float(e.period), int(e.fourier_order), 0) for e in custom]
+    for (name, bit, period, dflt), order, sw in zip(_BUILTINS, orders, switches):
+        if sw != 0 and name not in names:
+            out.append((name, period, order or dflt, bit))
+    return out
+
+
+def table_mask(table, builtin_mask):
+    """The table mask (bit j: entry j of ``seasonality_table`` active) of histories with built-in mask ``builtin_mask``
+    (scalar or array): the library's tab_mask."""
+    bm = np.asarray(builtin_mask)
+    m = np.zeros(bm.shape, np.int32)
+    for j, (_, _, _, kind) in enumerate(table):
+        m |= np.where((kind == 0) | ((bm & kind) != 0), np.int32(1 << j), np.int32(0))
+    return m
+
+
+def copy_options(opts):
+    """A copy of ``opts`` that shares nothing mutable with it: the whole pb200_options_v2 for a table (its entries kept
+    alive by the copy), pb200_options otherwise."""
+    if getattr(opts, "abi_version", L.ABI_VERSION) != L.ABI_VERSION_TABLE:
+        return L.Options.from_buffer_copy(opts)
+    o = L.OptionsV2.from_buffer_copy(opts)
+    n = opts.n_seasonalities
+    arr = (L.Seasonality * max(1, n))()
+    for i in range(n):
+        arr[i] = L.Seasonality.from_buffer_copy(opts.seasonalities[i])
+    o.seasonalities = C.cast(arr, C.POINTER(L.Seasonality))
+    o._table = arr
+    return o
+
+
 @dataclass
 class FittedBatch:
     """Fitted-model arrays of one shard (numpy on host, or torch tensors on device)."""
@@ -1073,9 +1127,18 @@ def cv_plan_errors(plan: CvPlan):
 
 
 def _with_mask(opts: L.Options, mask: int) -> L.Options:
-    """The options of a cutoff fit: the full model's, seasonalities forced to the full history's auto mask."""
-    o = L.Options.from_buffer_copy(opts)
-    o.yearly, o.weekly, o.daily = int(mask & 1 != 0), int(mask & 2 != 0), int(mask & 4 != 0)
+    """The options of a cutoff fit: the full model's, seasonalities forced to the full history's auto mask (fbprophet
+    0.5's prophet_copy, which gives the copy the fitted model's seasonalities and turns the built-in switches off).  For
+    a seasonality table the cutoff fit keeps every custom entry and the orders; a built-in is forced on or off by the
+    mask only where no custom entry carries its name -- such an entry replaces the built-in, whose switch must stay
+    AUTO."""
+    o = copy_options(opts)
+    custom = set()
+    if getattr(opts, "abi_version", L.ABI_VERSION) == L.ABI_VERSION_TABLE:
+        custom = {opts.seasonalities[i].name.decode() for i in range(opts.n_seasonalities)}
+    for name, bit, _, _ in _BUILTINS:
+        if name not in custom:
+            setattr(o, name, int(mask & bit != 0))
     return o
 
 
@@ -1084,7 +1147,8 @@ class CvResult:
     """Output of cross_validation_device (host numpy).
 
     Pairs, in plan order (series ascending, cutoffs ascending): ``pair_series``, ``pair_cutoff``, ``pair_status`` (the
-    cutoff fit's solver status; < 0: failed), ``pair_mask`` (the seasonality mask it was fitted with).
+    cutoff fit's solver status; < 0: failed), ``pair_mask`` (the built-in seasonality mask it was fitted with; with a
+    seasonality table the kept fits' meta_i32[:, 3] holds the table mask of ``opts``).
     Held-out rows, ordered by (series, cutoff, ds): ``row_series``, ``ds``, ``cutoff``, ``y`` (float64 of the input
     value), ``yhat`` and, with intervals, ``yhat_lower`` / ``yhat_upper``.
     Metrics rows (when requested), ordered by (series, horizon): ``m_series``, ``horizon`` (ns), ``mse``, ``rmse``,
@@ -1241,6 +1305,7 @@ def cross_validation_device(ctx: L.Context, opts: L.Options, ds_ns, y, offsets_h
                          f"{int(bad[1].sum())} series in all)")
     lib = L.load()
     lay = L.get_layout(opts)
+    table = seasonality_table(opts)
     ydt = _y_dtype(y)
     d_off = torch.from_numpy(offsets_host).to(dev)
     n_grid, grid_h = 1, None
@@ -1308,10 +1373,16 @@ def cross_validation_device(ctx: L.Context, opts: L.Options, ds_ns, y, offsets_h
             r0, r1 = int(fit_off[a]), int(fit_off[b])
             fc = fit_batch_device(ctx, oc, ds_g[r0:r1], y_g[r0:r1], fit_off[a:b + 1] - r0, float(floor), 1.0,
                                   cap=cap_p[a:b], prior=prior_p[a:b] if prior_p is not None else None)
+            # a table's cutoff fit packs the same active columns as the full model (never more: every entry of its
+            # table is an active entry of the full one); its table drops the built-ins forced off and so numbers the
+            # entries differently, and the mask is restated in the full table's entries
             w = fc.params.shape[1]
+            assert w <= lay.pstride, (w, lay.pstride)
             fitted.params[a:b, :w] = fc.params
             fitted.tchange[a:b] = fc.tchange
             fitted.meta_i32[a:b] = fc.meta_i32
+            if table is not None:
+                fitted.meta_i32[a:b, 3] = int(table_mask(table, int(sp[a])))
             fitted.meta_i64[a:b] = fc.meta_i64
             fitted.meta_f64[a:b] = fc.meta_f64
         torch.cuda.current_stream(dev).synchronize()

@@ -4,6 +4,9 @@ Reads the modeler's input (``io.input``, same header-less hive-partitioned CSV) 
 its history with the modeler's options (``model.*``), then predicts the held-out rows after each cutoff and reduces
 the errors to metrics by forecast horizon.  All of it on the GPU: the cutoff plan, the gathered truncated histories,
 the fits, the prediction and the metrics (time_series_spark_b200/csrc/cv_kernel.cuh; semantics in DESIGN §9).
+A seasonality table (``model.seasonalities`` or an int built-in order, DESIGN §18) is backtested as fbprophet's
+prophet_copy does it: every cutoff fit takes the full history's active seasonalities and nothing else, with every
+``backtest.*`` option below.
 
 Keys (``backtest.*``):
   horizon            pandas Timedelta string, required ("1 days")

@@ -14,6 +14,17 @@ Optional keys beyond the reference (defaults reproduce prophet_modeler.py:65 exa
 ``model.weekly_seasonality``, ``model.daily_seasonality``, ``model.n_changepoints``,
 ``model.changepoint_range``, ``model.changepoint_prior_scale``, ``model.seasonality_prior_scale``.
 
+Seasonality tables (DESIGN §18): ``model.yearly_seasonality`` / ``weekly_seasonality`` / ``daily_seasonality`` also take
+an int Fourier order (> 0 forces the built-in on at that order, 0 is off), and ``model.seasonalities`` is a list of
+fbprophet ``add_seasonality`` calls in the order they are made: ``{name, period (days), fourier_order, prior_scale?
+(default model.seasonality_prior_scale), mode? (must be model.seasonality_mode)}``.  With either key the options come
+from ``batched.make_table_options`` and every error names the YAML key.  A custom name that is a column of the scorer's
+frames (series_id, dim_id, ds, yhat, created_timestamp, forecast_date, forecast_timestamp, forecast_quantity, yhat_q...)
+is refused here, since the scorer writes one component column per custom seasonality.  The models table then holds
+version-2 records, which carry the table to the scorer; a table that restates the defaults (``yearly_seasonality: 10``)
+is the default model and writes the same version-1 bytes as ``yearly_seasonality: true``.  ``io.warm_start`` (and so
+``insample.refit`` with a warm start) is refused for a table; ``insample`` without it serves table models unchanged.
+
 ``io.warm_start`` (optional): the path of a previous models table, for a job re-run on a schedule over the same groups
 plus new rows (fbprophet's "updating fitted models", ``m.fit(df, init=stan_init(m_old))``).  Every group starts its
 fit from its row of that table when the row's changepoint count and seasonalities are those of the new history
@@ -82,19 +93,78 @@ def get_context(device=None) -> L.Context:
     return _contexts[device]
 
 
+_BUILTIN_KEYS = ("yearly_seasonality", "weekly_seasonality", "daily_seasonality")
+
+# columns of the scorer's frames a custom seasonality's component column must not shadow: the internal frame's and the
+# written CSV's (convert_forecasts); names starting with yhat_q are the quantile columns
+SCORER_COLUMNS = frozenset(["series_id", "dim_id", "ds", "yhat", "created_timestamp", "forecast_date",
+                            "forecast_timestamp", "forecast_quantity"])
+
+
+def table_keys(config) -> list:
+    """The ``model.*`` keys that make the job's model a seasonality table: ``model.seasonalities`` and the built-in
+    switches given as an int order."""
+    m = config.get("model", {}) or {}
+    keys = [f"model.{k}" for k in _BUILTIN_KEYS
+            if isinstance(m.get(k), (int, np.integer)) and not isinstance(m.get(k), (bool, np.bool_))]
+    return keys + (["model.seasonalities"] if "seasonalities" in m else [])
+
+
+def _model_key_error(e: ValueError, keys) -> ValueError:
+    """make_table_options' message with each key it names spelled as its YAML key (model.<key>); a message that names
+    none (the library's limits) is prefixed with the table's keys."""
+    import re
+    msg = str(e)
+    named = re.sub(r"(?<![\w.])(seasonalities(?=[\[:])|yearly_seasonality|weekly_seasonality|daily_seasonality|"
+                   r"seasonality_mode)", r"model.\1", msg)
+    return ValueError(named if named != msg else f"{' / '.join(keys)}: {msg}")
+
+
 def options_from_config(config) -> L.Options:
+    """The job's fit options from ``model.*``.  Without ``model.seasonalities`` and without an int order for a built-in,
+    batched.make_options as always; with either, batched.make_table_options (DESIGN §18), whose errors name the YAML key.
+    A table that restates the default model gives the same pb200_options as the switches alone."""
     m = dict(config.get("model", {}) or {})
-    return batched.make_options(
-        growth=m.get("growth", "logistic"),
-        seasonality_mode=m.get("seasonality_mode", "multiplicative"),
-        yearly_seasonality=m.get("yearly_seasonality", "auto"),
-        weekly_seasonality=m.get("weekly_seasonality", "auto"),
-        daily_seasonality=m.get("daily_seasonality", "auto"),
-        n_changepoints=m.get("n_changepoints", 25),
-        changepoint_range=m.get("changepoint_range", 0.8),
-        changepoint_prior_scale=m.get("changepoint_prior_scale", 0.05),
-        seasonality_prior_scale=m.get("seasonality_prior_scale", 10.0),
-    )
+    kw = dict(growth=m.get("growth", "logistic"),
+              seasonality_mode=m.get("seasonality_mode", "multiplicative"),
+              n_changepoints=m.get("n_changepoints", 25),
+              changepoint_range=m.get("changepoint_range", 0.8),
+              changepoint_prior_scale=m.get("changepoint_prior_scale", 0.05),
+              seasonality_prior_scale=m.get("seasonality_prior_scale", 10.0))
+    keys = table_keys(config)
+    if not keys:
+        return batched.make_options(yearly_seasonality=m.get("yearly_seasonality", "auto"),
+                                    weekly_seasonality=m.get("weekly_seasonality", "auto"),
+                                    daily_seasonality=m.get("daily_seasonality", "auto"), **kw)
+    seas = m.get("seasonalities")
+    if seas is None:
+        seas = []
+    if not isinstance(seas, (list, tuple)):
+        raise ValueError(f"model.seasonalities must be a list of {{name, period, fourier_order, prior_scale?, mode?}} "
+                         f"(got {seas!r})")
+    for i, spec in enumerate(seas):
+        name = spec.get("name") if isinstance(spec, dict) else None
+        if isinstance(name, str) and (name in SCORER_COLUMNS or name.startswith("yhat_q")):
+            raise ValueError(f"model.seasonalities[{i}].name: {name!r} is a column of the scorer's forecast frames; its "
+                             "component column would shadow it")
+    try:
+        opts = batched.make_table_options(seasonalities=seas, **{k: m.get(k, "auto") for k in _BUILTIN_KEYS}, **kw)
+    except ValueError as e:
+        raise _model_key_error(e, keys) from None
+    if batched.is_table(opts):
+        return opts
+    v1 = L.Options.from_buffer_copy(opts)
+    v1.abi_version = L.ABI_VERSION
+    return v1
+
+
+def refuse_table_warm_start(config, opts) -> None:
+    """Warm start needs the previous optimum in the options' layout, which the library takes for the default model only:
+    a seasonality table with ``io.warm_start`` (also under ``insample.refit``) raises, naming both keys."""
+    if batched.is_table(opts) and (config.get("io") or {}).get("warm_start"):
+        raise ValueError(f"io.warm_start is not available for a model with a seasonality table "
+                         f"({', '.join(table_keys(config))}): warm start serves the default seasonalities only"
+                         + (" (insample.refit would start from it too)" if "insample" in config else ""))
 
 
 def who(series_id, dim_id, mask) -> str:
@@ -183,7 +253,8 @@ def warm_start_init(table: pa.Table, opts: L.Options, series_id, dim_id, path: s
     """The previous models of the packed groups ``(series_id, dim_id)`` from a models table (MODEL_OUTPUT_SCHEMA), as
     the ``init`` of ``batched.fit_batch_device``: a host FittedBatch in the groups' order whose rows without a previous
     model have status -1.  Returns ``(init, unmatched)``, ``unmatched`` the number of table rows that match no group.
-    Raises ValueError (naming ``path``) for a table fitted with other options, and for duplicate keys."""
+    Raises ValueError (naming ``path``) for a table fitted with other options or with a seasonality table, and for
+    duplicate keys."""
     lay = L.get_layout(opts)
     n = len(series_id)
     gkey = _group_keys(series_id, dim_id)
@@ -202,6 +273,10 @@ def warm_start_init(table: pa.Table, opts: L.Options, series_id, dim_id, path: s
     if dup.any():
         raise ValueError(f"{path} holds more than one model for a (series_id, dim_id) group." + who(tsid, tdid, dup))
     prev, _, info = model_record.decode(table["model"])
+    if "table" in info:
+        # a seasonality table's records hold its mask and betas in the table's column order, not the default model's
+        raise ValueError(f"{path} holds models fitted with a seasonality table (version-2 records); warm start serves "
+                         "the default seasonalities only")
     want = {"logistic": opts.growth == L.GROWTH_LOGISTIC, "multiplicative": bool(opts.multiplicative),
             "yearly": int(opts.yearly), "weekly": int(opts.weekly), "daily": int(opts.daily),
             "n_changepoints": int(opts.n_changepoints)}
@@ -281,6 +356,8 @@ class _ModelTimeSeriesOp:
         floor = self.config["model"]["floor"]
         cap_multiplier = self.config["model"]["cap_multiplier"]
         ins = insample_options(self.config)
+        if table_keys(self.config):         # a table's refusals come before any GPU work
+            refuse_table_warm_start(self.config, options_from_config(self.config))
         with_frame = ins is not None and bool((self.config.get("io") or {}).get("fitted"))
         # this rank's io.fitted frame (empty until a group is predicted)
         self.fitted_table = fitted_schema(table.schema.field("y").type).empty_table() if with_frame else None
@@ -330,7 +407,7 @@ class _ModelTimeSeriesOp:
         """The in-sample predict of the fitted batch, its outlier flags, the io.fitted frame and (insample.refit) the
         fit without the flagged rows; returns the models table the job writes."""
         import torch
-        iopts = L.Options.from_buffer_copy(opts)
+        iopts = batched.copy_options(opts)
         iopts.interval_width = ins["interval_width"]
         iopts.uncertainty_samples = ins["uncertainty_samples"]
         # fbprophet predicts the history with the floor and cap it was fitted on: the fit's own (float64) values

@@ -20,6 +20,12 @@ the joint draws -- DESIGN §13), ``forecast.aggregate_origin`` (where window 0 s
 ``io.aggregates`` table over calendar months, quarters, years or weeks -- DESIGN §17) and
 ``forecast.quantiles`` (a list of 1 to 32 levels in [0, 1]: one float64 column ``yhat_q<level>`` per level, the
 percentile 100 level of the point's ``uncertainty_samples`` draws -- DESIGN §15).
+
+Models with a seasonality table (version-2 records, written by the modeler from ``model.seasonalities`` or an int
+built-in order -- DESIGN §18) are scored with the table the record carries; no scorer key is needed, and every mode
+above serves them.  With ``forecast.components`` each custom seasonality not named like a built-in adds one float64
+column of its name after ``additive_terms`` (in table order); a custom ``yearly`` / ``weekly`` / ``daily`` fills that
+built-in's column, which is null where the model's entry of that name is inactive.
 """
 from __future__ import annotations
 
@@ -85,20 +91,40 @@ def quantile_column(q: float) -> str:
     return "yhat_q" + repr(float(q))
 
 
-def _component_fields(intervals: bool):
-    names = COMPONENT_COLUMNS + (("trend_lower", "trend_upper") if intervals else ())
+def _component_fields(intervals: bool, custom=()):
+    names = COMPONENT_COLUMNS + tuple(custom) + (("trend_lower", "trend_upper") if intervals else ())
     return [pa.field(n, pa.float64()) for n in names]
 
 
-def component_columns(res: "batched.ForecastBatch", mask: np.ndarray, periods: int, intervals: bool) -> dict:
+def custom_component_names(opts) -> tuple:
+    """The component columns a seasonality table adds to COMPONENT_COLUMNS: one per custom entry not named like a
+    built-in, in table order (batched.component_names past the six planes)."""
+    return tuple(batched.component_names(opts)[L.N_COMPONENTS:])
+
+
+def component_columns(res: "batched.ForecastBatch", mask: np.ndarray, periods: int, intervals: bool, table=None) -> dict:
     """The component columns of one shard's forecast frame, one row per (model, period), from a components predict
-    (``res``) and the models' seasonality masks (meta_i32[:, 3])."""
+    (``res``) and the models' seasonality masks (meta_i32[:, 3]).  With a seasonality table (``table``:
+    batched.seasonality_table) the mask is the table mask: a built-in's column is null where the entry of its name (the
+    built-in's own, or a custom entry replacing it) is inactive or absent, and each custom entry not named like a
+    built-in adds its column after additive_terms."""
     mask = np.asarray(mask)
     cols = {}
+    entry = {e[0]: j for j, e in enumerate(table or ())}
     for name in COMPONENT_COLUMNS:
         v = np.ascontiguousarray(res.component(name)).reshape(-1)
-        absent = np.repeat((mask & _SEASONAL_BIT[name]) == 0, periods) if name in _SEASONAL_BIT else None
+        absent = None
+        if name in _SEASONAL_BIT:
+            if table is None:
+                off = (mask & _SEASONAL_BIT[name]) == 0
+            elif name in entry:
+                off = ((mask >> entry[name]) & 1) == 0
+            else:
+                off = np.ones(mask.shape, bool)
+            absent = np.repeat(off, periods)
         cols[name] = pa.array(v, pa.float64(), mask=absent)
+    for name in res.names[L.N_COMPONENTS:]:
+        cols[name] = pa.array(np.ascontiguousarray(res.component(name)).reshape(-1), pa.float64())
     if intervals:
         cols["trend_lower"] = pa.array(res.trend_lower.reshape(-1), pa.float64())
         cols["trend_upper"] = pa.array(res.trend_upper.reshape(-1), pa.float64())
@@ -267,7 +293,20 @@ class _ForecastTimeSeriesOp:
             if not 0.0 <= width <= 1.0:     # fbprophet refuses it too (numpy's percentile range check); NaN fails here
                 raise ValueError(f"forecast.interval_width must be in [0, 1] (got {fc.get('interval_width')!r})")
         want_components = _want_components(fc)
+        # every rank scores a shard of the whole table, so the model class (version 1, or version 2 with one seasonality
+        # table) is checked over all of it, and a table's custom component columns come from its first model: every
+        # rank's frame (an empty shard's too) then has the same columns
         rank, ws, _ = pdist.world()
+        custom = ()
+        if (want_components or ws > 1) and table.num_rows:
+            valid = table["model"].filter(pc.is_valid(table["model"]))
+            if len(valid):
+                if ws > 1:
+                    model_record.check_one_class(valid)
+                if want_components:
+                    _, _, info0 = model_record.decode(valid.slice(0, 1))
+                    if "table" in info0:
+                        custom = custom_component_names(model_record.table_options(info0))
         if ws > 1 and table.num_rows:      # shard the model rows across ranks (equal horizon => equal work)
             lo, hi = pdist.shard_bounds(np.arange(table.num_rows + 1, dtype=np.int64), ws)[rank]
             table = table.slice(lo, hi - lo)
@@ -279,7 +318,7 @@ class _ForecastTimeSeriesOp:
         for q in levels or ():
             empty_schema = empty_schema.append(pa.field(quantile_column(q), pa.float64()))
         if want_components:
-            for f in _component_fields(want_intervals):
+            for f in _component_fields(want_intervals, custom):
                 empty_schema = empty_schema.append(f)
         if table.num_rows == 0:
             return empty_schema.empty_table()
@@ -293,13 +332,15 @@ class _ForecastTimeSeriesOp:
             if table.num_rows == 0:
                 return empty_schema.empty_table()
         fitted, last_ds, info = model_record.decode(table["model"])
-        opts = batched.make_options(growth="logistic" if info["logistic"] else "linear",
-                                    seasonality_mode="multiplicative" if info["multiplicative"] else "additive",
-                                    n_changepoints=info["n_changepoints"],
-                                    interval_width=fc.get("interval_width", 0.8),
-                                    uncertainty_samples=fc.get("uncertainty_samples", 1000)
-                                    if want_intervals or rule or months or levels else 0)
-        opts.yearly, opts.weekly, opts.daily = info["yearly"], info["weekly"], info["daily"]
+        mc = dict(interval_width=fc.get("interval_width", 0.8),
+                  uncertainty_samples=fc.get("uncertainty_samples", 1000) if want_intervals or rule or months or levels else 0)
+        if "table" in info:          # a version-2 record: the fit's seasonality table (DESIGN §18)
+            opts = model_record.table_options(info, **mc)
+        else:
+            opts = batched.make_options(growth="logistic" if info["logistic"] else "linear",
+                                        seasonality_mode="multiplicative" if info["multiplicative"] else "additive",
+                                        n_changepoints=info["n_changepoints"], **mc)
+            opts.yearly, opts.weekly, opts.daily = info["yearly"], info["weekly"], info["daily"]
         # reference :46-47: floor / cap are read back from the FLOAT32 columns of the models table
         floor = table["floor"].combine_chunks().to_numpy(zero_copy_only=False).astype(np.float64)
         cap = table["cap"].combine_chunks().to_numpy(zero_copy_only=False).astype(np.float64)
@@ -339,7 +380,8 @@ class _ForecastTimeSeriesOp:
         for q, lv in enumerate(levels or ()):
             cols[quantile_column(lv)] = pa.array(res.quantiles[q].reshape(-1), pa.float64())
         if want_components:
-            cols.update(component_columns(res, fitted.meta_i32[:, 3], periods, want_intervals))
+            cols.update(component_columns(res, fitted.meta_i32[:, 3], periods, want_intervals,
+                                          batched.seasonality_table(opts)))
         out = pa.table(cols)
         if not ok.all():
             out = out.filter(pa.array(np.repeat(ok, periods)))
@@ -493,7 +535,10 @@ class ProphetScorer:
             "forecast_quantity": t["yhat"],
         }
         quants = tuple(c for c in t.column_names if c.startswith("yhat_q"))
-        for extra in ("yhat_lower", "yhat_upper") + quants + COMPONENT_COLUMNS + ("trend_lower", "trend_upper"):
+        known = {"series_id", "dim_id", "ds", "yhat", "yhat_lower", "yhat_upper", "trend_lower", "trend_upper",
+                 *quants, *COMPONENT_COLUMNS}
+        custom = tuple(c for c in t.column_names if c not in known)   # a seasonality table's component columns
+        for extra in ("yhat_lower", "yhat_upper") + quants + COMPONENT_COLUMNS + custom + ("trend_lower", "trend_upper"):
             if extra in t.column_names:
                 cols[extra] = t[extra]
         out = Frame(pa.table(cols))

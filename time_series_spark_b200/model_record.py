@@ -12,6 +12,15 @@ the record is a fixed-layout little-endian struct (about 0.7 KB):
     | f64[4] meta_f64 (y_scale, floor, cap, neg_log_posterior)
     | f64[pstride] params (k, m, sigma_obs, delta[smax], beta[kmax]) | f64[smax] t_change
 
+Version 2 is the record of a model with a seasonality table (DESIGN §18): the version-1 fields (meta_i32[3] then holds
+the table mask, bit j = entry j of the normalised table active), followed by the table as it was given:
+
+    | i32[3] built-in orders (yearly, weekly, daily; 0 = default) | i32 entry count
+    | 8 x (name[16] NUL-padded | f64 period (days) | f64 prior_scale (0 = seasonality_prior_scale) | i32 fourier_order)
+
+Options without a table, and a table that restates the default model, write version 1.  Every record of a table
+has one version, and the version-2 records of a table one seasonality table.
+
 Encoding / decoding is vectorised over the whole batch (one numpy structured array),
 never a per-row Python loop.
 """
@@ -20,35 +29,103 @@ from __future__ import annotations
 import numpy as np
 import pyarrow as pa
 
+from . import _lib as L
+from . import batched
 from .batched import FittedBatch
 
 MAGIC = b"PB2M"
 VERSION = 1
+VERSION_TABLE = 2
 FLAG_LOGISTIC, FLAG_MULT = 1, 2
+_BUILTIN_KEYS = ("yearly_seasonality", "weekly_seasonality", "daily_seasonality")
+ENTRY_DTYPE = np.dtype([("name", "S16"), ("period", "<f8"), ("prior_scale", "<f8"), ("fourier_order", "<i4")])
 
 
-def record_dtype(smax: int, kmax: int) -> np.dtype:
+def record_dtype(smax: int, kmax: int, version: int = VERSION) -> np.dtype:
     pstride = 3 + smax + kmax
-    return np.dtype([("magic", "S4"), ("version", "<u2"), ("flags", "<u2"), ("smax", "<i4"), ("kmax", "<i4"),
-                     ("switches", "<i4", (4,)), ("meta_i32", "<i4", (8,)), ("meta_i64", "<i8", (2,)), ("last_ds", "<i8"),
-                     ("meta_f64", "<f8", (4,)), ("params", "<f8", (pstride,)), ("tchange", "<f8", (smax,))])
+    fields = [("magic", "S4"), ("version", "<u2"), ("flags", "<u2"), ("smax", "<i4"), ("kmax", "<i4"),
+              ("switches", "<i4", (4,)), ("meta_i32", "<i4", (8,)), ("meta_i64", "<i8", (2,)), ("last_ds", "<i8"),
+              ("meta_f64", "<f8", (4,)), ("params", "<f8", (pstride,)), ("tchange", "<f8", (smax,))]
+    if version == VERSION_TABLE:
+        fields += [("orders", "<i4", (3,)), ("n_entries", "<i4"), ("entries", ENTRY_DTYPE, (L.MAX_SEASONALITIES,))]
+    elif version != VERSION:
+        raise ValueError(f"unknown model record version {version}")
+    return np.dtype(fields)
+
+
+def _table_spec(opts) -> dict:
+    """The seasonality table of pb200_options_v2 as make_table_options' keyword arguments."""
+    spec = {}
+    for key, sw, order in zip(_BUILTIN_KEYS, (opts.yearly, opts.weekly, opts.daily),
+                              (opts.yearly_order, opts.weekly_order, opts.daily_order)):
+        if sw == L.SEAS_AUTO:
+            if order != 0:
+                raise ValueError(f"{key}: an order ({order}) under an AUTO switch (make_table_options forces a "
+                                 "built-in on when it is given an order)")
+            spec[key] = "auto"
+        else:
+            spec[key] = (int(order) if order > 0 else True) if sw == 1 else False
+    seas = []
+    for i in range(opts.n_seasonalities):
+        e = opts.seasonalities[i]
+        d = {"name": e.name.decode(), "period": float(e.period), "fourier_order": int(e.fourier_order)}
+        if e.prior_scale != 0.0:
+            d["prior_scale"] = float(e.prior_scale)
+        seas.append(d)
+    spec["seasonalities"] = seas
+    return spec
+
+
+def table_options(info: dict, **kw):
+    """The options of a decoded table (``info["table"]``) for make_table_options' other keyword arguments ``kw``
+    (make_options'): the fit's seasonality table, layout and component names."""
+    return batched.make_table_options(
+        growth="logistic" if info["logistic"] else "linear",
+        seasonality_mode="multiplicative" if info["multiplicative"] else "additive",
+        n_changepoints=info["n_changepoints"], **info["table"], **kw)
 
 
 def encode(fitted: FittedBatch, last_ds_ns: np.ndarray, opts) -> pa.Array:
-    """FittedBatch (+ the pb200 Options it was fitted with) -> Arrow binary array, one record per model."""
+    """FittedBatch (+ the pb200 Options it was fitted with) -> Arrow binary array, one record per model.  Options the
+    record cannot represent -- a decoded record would rebuild another model from them -- raise ValueError."""
     logistic, multiplicative = opts.growth == 1, bool(opts.multiplicative)
     fitted = fitted.to_host()
     n = fitted.n
-    dt = record_dtype(fitted.smax, fitted.kmax)
+    table = batched.seasonality_table(opts)
+    version = VERSION if table is None else VERSION_TABLE
+    if table is not None:
+        try:
+            spec = _table_spec(opts)
+            rebuilt = batched.make_table_options(
+                growth="logistic" if logistic else "linear",
+                seasonality_mode="multiplicative" if multiplicative else "additive",
+                n_changepoints=opts.n_changepoints, seasonality_prior_scale=opts.seasonality_prior_scale, **spec)
+        except ValueError as e:
+            raise ValueError(f"these options have no model record: {e}") from None
+        if batched.seasonality_table(rebuilt) != table:
+            raise ValueError("these options have no model record: their seasonality table does not rebuild")
+        lay = L.get_layout(opts)
+        if (lay.smax, lay.kmax) != (fitted.smax, fitted.kmax):
+            raise ValueError(f"the fitted batch's layout (smax {fitted.smax}, kmax {fitted.kmax}) is not the options' "
+                             f"(smax {lay.smax}, kmax {lay.kmax})")
+    dt = record_dtype(fitted.smax, fitted.kmax, version)
     rec = np.zeros(n, dtype=dt)
     rec["magic"] = MAGIC
-    rec["version"] = VERSION
+    rec["version"] = version
     rec["flags"] = (FLAG_LOGISTIC if logistic else 0) | (FLAG_MULT if multiplicative else 0)
     rec["smax"], rec["kmax"] = fitted.smax, fitted.kmax
     rec["switches"] = np.array([opts.yearly, opts.weekly, opts.daily, opts.n_changepoints], dtype=np.int32)
     rec["meta_i32"], rec["meta_i64"], rec["meta_f64"] = fitted.meta_i32, fitted.meta_i64, fitted.meta_f64
     rec["last_ds"] = np.asarray(last_ds_ns, dtype=np.int64)
     rec["params"], rec["tchange"] = fitted.params, fitted.tchange
+    if table is not None:
+        rec["orders"] = np.array([opts.yearly_order, opts.weekly_order, opts.daily_order], dtype=np.int32)
+        rec["n_entries"] = opts.n_seasonalities
+        ent = np.zeros(L.MAX_SEASONALITIES, ENTRY_DTYPE)
+        for i in range(opts.n_seasonalities):
+            e = opts.seasonalities[i]
+            ent[i] = (e.name, e.period, e.prior_scale, e.fourier_order)
+        rec["entries"] = ent
     size = dt.itemsize
     offsets = pa.py_buffer((np.arange(n + 1, dtype=np.int64) * size).astype(np.int32).tobytes()) \
         if n * size < 2**31 else None
@@ -59,27 +136,74 @@ def encode(fitted: FittedBatch, last_ds_ns: np.ndarray, opts) -> pa.Array:
     return pa.Array.from_buffers(pa.large_binary(), n, [None, off64, data])
 
 
-def decode(col) -> tuple:
-    """Arrow binary column -> (FittedBatch, last_ds_ns, dict of the fit-time options)."""
+_TABLE_TAIL = 16 + ENTRY_DTYPE.itemsize * L.MAX_SEASONALITIES     # orders, n_entries, entries: a v2 record's end
+
+
+def _column(col):
+    """One Arrow array of the records, refused when empty or holding nulls."""
     if isinstance(col, pa.ChunkedArray):
         col = col.combine_chunks() if col.num_chunks != 1 else col.chunk(0)
-    n = len(col)
-    if n == 0:
+    if len(col) == 0:
         raise ValueError("empty model column")
     if col.null_count:
         raise ValueError("model column holds nulls (the reference returns an empty frame for those rows)")
-    first = col[0].as_py()
-    if first[:4] != MAGIC:
+    return col
+
+
+def _one_class(col):
+    """(record offsets, data bytes, version) of a column whose records are one model class: a PB2M first record, every
+    record's version known and the same, and for version 2 one seasonality table.  Reads only the records' headers and
+    table bytes, whatever their layouts."""
+    n = len(col)
+    if col[0].as_py()[:4] != MAGIC:
         raise ValueError("model blob is not a PB2M record (fbprophet pickles cannot be scored on this path)")
-    smax, kmax = np.frombuffer(first[8:16], dtype="<i4")
-    dt = record_dtype(int(smax), int(kmax))
     bufs = col.buffers()
     off_dt = np.int64 if pa.types.is_large_binary(col.type) else np.int32
-    offs = np.frombuffer(bufs[1], dtype=off_dt)[col.offset:col.offset + n + 1]
+    offs = np.frombuffer(bufs[1], dtype=off_dt)[col.offset:col.offset + n + 1].astype(np.int64)
+    if np.any(np.diff(offs) < 16):
+        raise ValueError("bad model record header")
+    # every record's version, read before the record layout it decides
+    raw = np.frombuffer(bufs[2], dtype=np.uint8)
+    ver = raw[offs[:-1] + 4].astype(np.int64) | (raw[offs[:-1] + 5].astype(np.int64) << 8)
+    known = (ver == VERSION) | (ver == VERSION_TABLE)
+    if not known.all():
+        raise ValueError(f"model record version {int(ver[~known][0])} is unknown to this library (it reads versions "
+                         f"{VERSION} and {VERSION_TABLE})")
+    version = int(ver[0])
+    if not np.all(ver == version):
+        raise ValueError("version-1 and version-2 model records in one table: models without and with a seasonality "
+                         "table cannot be scored in one call")
+    if version == VERSION_TABLE:
+        if np.any(np.diff(offs) < 16 + _TABLE_TAIL):
+            raise ValueError("bad model record header")
+        tab = raw[(offs[1:] - _TABLE_TAIL)[:, None] + np.arange(_TABLE_TAIL)[None, :]]
+        if not np.all(tab == tab[0]):
+            raise ValueError("model records with different seasonality tables in one table: each table's models are "
+                             "scored with one set of options")
+    return offs, bufs, version
+
+
+def check_one_class(col) -> None:
+    """Refuse, as decode does, a models column that mixes version-1 and version-2 records or holds two seasonality
+    tables, without decoding the records: for callers that decode the column in shards (one per rank) but must agree
+    on the model class of the whole table."""
+    _one_class(_column(col))
+
+
+def decode(col) -> tuple:
+    """Arrow binary column -> (FittedBatch, last_ds_ns, dict of the fit-time options).  Version-2 records add ``info["table"]``,
+    the seasonality table as make_table_options' keyword arguments (``table_options`` rebuilds the fit's options from
+    it); version-1 records have no such key."""
+    col = _column(col)
+    n = len(col)
+    offs, bufs, version = _one_class(col)
+    first = col[0].as_py()
+    smax, kmax = np.frombuffer(first[8:16], dtype="<i4")
+    dt = record_dtype(int(smax), int(kmax), version)
     if not np.all(np.diff(offs) == dt.itemsize):
         raise ValueError("model records of differing layout in one table")
     rec = np.frombuffer(bufs[2], dtype=dt, count=n, offset=int(offs[0]))
-    if not (np.all(rec["magic"] == MAGIC) and np.all(rec["version"] == VERSION)):
+    if not (np.all(rec["magic"] == MAGIC) and np.all(rec["version"] == version)):
         raise ValueError("bad model record header")
     flags = int(rec["flags"][0])
     fb = FittedBatch(np.ascontiguousarray(rec["params"]), np.ascontiguousarray(rec["tchange"]),
@@ -90,6 +214,18 @@ def decode(col) -> tuple:
     sw = rec["switches"][0]
     info = {"logistic": bool(flags & FLAG_LOGISTIC), "multiplicative": bool(flags & FLAG_MULT),
             "yearly": int(sw[0]), "weekly": int(sw[1]), "daily": int(sw[2]), "n_changepoints": int(sw[3])}
+    if version == VERSION_TABLE:
+        ne = int(rec["n_entries"][0])
+        if not 0 <= ne <= L.MAX_SEASONALITIES:
+            raise ValueError(f"bad model record: {ne} seasonality entries")
+        table = {}
+        for key, s, order in zip(_BUILTIN_KEYS, sw[:3], rec["orders"][0]):
+            table[key] = "auto" if s == L.SEAS_AUTO else ((int(order) if order > 0 else True) if s == 1 else False)
+        table["seasonalities"] = [
+            dict({"name": e["name"].decode(), "period": float(e["period"]), "fourier_order": int(e["fourier_order"])},
+                 **({"prior_scale": float(e["prior_scale"])} if e["prior_scale"] != 0.0 else {}))
+            for e in rec["entries"][0][:ne]]
+        info["table"] = table
     return fb, np.ascontiguousarray(rec["last_ds"]), info
 
 
