@@ -68,6 +68,7 @@ extern "C" {
 #define PB200_ST_CAP_LE_FLOOR -4  /* cap <= floor (fbprophet ValueError) */
 #define PB200_ST_BAD_INPUT   -5   /* unsorted timestamps / non-finite y / zero time span */
 #define PB200_ST_BAD_PRIOR   -6   /* pb200_fit_prior_device: the series' prior scales are not finite and > 0 */
+/* -7 PB200_ST_BAD_REGRESSOR: see the regressor entry points at the end of this header */
 
 /* where a series of pb200_fit_warm_device started (d_warm) */
 #define PB200_WARM_USED       1   /* from its previous model */
@@ -676,6 +677,102 @@ PB200_API int pb200_outlier_counts_device(pb200_ctx* ctx, const void* d_y, int32
 PB200_API int pb200_outlier_compact_device(pb200_ctx* ctx, const int64_t* d_ds, const void* d_y, int32_t y_dtype,
                                            const int64_t* d_offsets, int64_t n_series, const uint8_t* d_flag,
                                            const int64_t* d_kept_off, int64_t* d_ds_out, void* d_y_out);
+
+/*
+ * Extra regressors (DESIGN §19): fbprophet 0.5's add_regressor(name, prior_scale, standardize, mode).  A
+ * pb200_options_v3 with v2.v1.abi_version = PB200_ABI_VERSION_REGRESSORS embeds a pb200_options_v2 (its table may
+ * restate the defaults) and adds:
+ *   holidays_prior_scale  the prior scale of a regressor whose prior_scale is 0 (fbprophet's default 10.0)
+ *   regressors[n_regressors]  in the order they were added, at most PB200_MAX_REGRESSORS: name (NUL-terminated, <= 15
+ *                 bytes, unique, not a seasonality's), prior_scale > 0 or 0, standardize PB200_STD_AUTO / 0 / 1.  Every
+ *                 regressor takes v1.multiplicative.
+ * With n_regressors = 0 a v3 options is exactly its v2 part.  With n_regressors = R > 0 the model is a table model
+ * (even when its seasonalities restate the defaults) whose columns are the active seasonal columns, then the R
+ * regressors: regressor r of series i is beta[K_seas(mask_i) + r] of its params row and of the objective hook's theta.
+ * Limits: K_seas + R <= 64 and 3 + max(1, n_changepoints) + K_seas + R <= 96, else PB200_E_UNSUPPORTED before any
+ * launch.  pb200_get_layout counts R in kmax.  Only the entry points below take such options; every other entry point
+ * that takes options refuses them with PB200_E_UNSUPPORTED before any launch (components, window and period sums,
+ * quantiles, in-sample predict, the backtest, per-series prior scales and warm start have no regressor values).
+ *
+ * Standardisation (fbprophet's initialize_scales, on the rows the fit sees): a regressor with fewer than 2 distinct
+ * values, or under PB200_STD_AUTO one whose values are exactly {0, 1}, is used as it is (mu = 0, std = 1); any other is
+ * (x - mu) / std with mu its mean and std its sample standard deviation (ddof = 1).
+ */
+#define PB200_ABI_VERSION_REGRESSORS 3
+#define PB200_MAX_REGRESSORS 16
+#define PB200_STD_AUTO (-1)
+#define PB200_ST_BAD_REGRESSOR -7  /* a regressor value of the series' history is not finite (fbprophet: "Found NaN") */
+
+typedef struct pb200_regressor {
+    char    name[16];
+    double  prior_scale;            /* 0 = holidays_prior_scale */
+    int32_t standardize;            /* PB200_STD_AUTO | 0 | 1 */
+    int32_t reserved;
+} pb200_regressor;
+
+typedef struct pb200_options_v3 {
+    pb200_options_v2 v2;            /* v2.v1.abi_version = PB200_ABI_VERSION_REGRESSORS */
+    double  holidays_prior_scale;   /* 10.0 */
+    int32_t n_regressors;           /* 0 .. PB200_MAX_REGRESSORS */
+    int32_t reserved;
+    const pb200_regressor* regressors;
+} pb200_options_v3;
+
+/* pb200_fit_device with the regressors' values:
+ *   d_reg        double [R][n_rows] (device), plane r aligned with d_ds (n_rows = h_offsets[n_series])
+ *   d_reg_scale  double [n_series][R][2] (device, out): (mu, std) of each regressor of each series; (0, 1) where it is
+ *                not standardised.  A series with a non-finite value gets status PB200_ST_BAD_REGRESSOR and no fit; the
+ *                other series are not affected. */
+PB200_API int pb200_fit_regressors_device(pb200_ctx* ctx, const pb200_options* opts,
+                     const int64_t* d_ds, const void* d_y, int32_t y_dtype,
+                     const int64_t* h_offsets, int64_t n_series,
+                     double floor, double cap_multiplier, const double* d_cap,
+                     const double* d_reg, double* d_reg_scale,
+                     double* d_params, double* d_tchange,
+                     int32_t* d_meta_i32, int64_t* d_meta_i64, double* d_meta_f64);
+
+/* The same on host buffers, plus pb200_fit_trace_host's trajectory rows when h_trace != NULL and trace_cap > 0. */
+PB200_API int pb200_fit_regressors_host(pb200_ctx* ctx, const pb200_options* opts,
+                     const int64_t* h_ds, const void* h_y, int32_t y_dtype,
+                     const int64_t* h_offsets, int64_t n_series,
+                     double floor, double cap_multiplier, const double* h_cap,
+                     const double* h_reg, double* h_reg_scale,
+                     double* h_params, double* h_tchange,
+                     int32_t* h_meta_i32, int64_t* h_meta_i64, double* h_meta_f64,
+                     double* h_trace, int32_t trace_cap);
+
+/* pb200_objective_host with the regressors' values (h_reg as h_ds); h_reg_scale [n_series][R][2] receives the
+ * standardisation the objective used. */
+PB200_API int pb200_objective_regressors_host(pb200_ctx* ctx, const pb200_options* opts,
+                     const int64_t* h_ds, const void* h_y, int32_t y_dtype,
+                     const int64_t* h_offsets, int64_t n_series,
+                     double floor, double cap_multiplier, const double* h_reg, double* h_reg_scale,
+                     const double* h_theta, double* h_f, double* h_grad, int32_t* h_meta_i32);
+
+/* pb200_predict_* with the regressors' future values:
+ *   d_future_reg  double [R][n_models * horizon], plane r aligned with d_future_ds
+ *   d_reg_scale   double [n_models][R][2], the fit's (mu, std)
+ * yhat adds sum_r beta_r (x_r - mu_r) / std_r to the seasonal term.  A model with a non-finite future regressor value
+ * gets the rows of a failed model (NaN, INT32_MIN). */
+PB200_API int pb200_predict_regressors_device(pb200_ctx* ctx, const pb200_options* opts,
+                         const double* d_params, const double* d_tchange,
+                         const int32_t* d_meta_i32, const int64_t* d_meta_i64,
+                         const double* d_meta_f64, int64_t n_models,
+                         const int64_t* d_future_ds, int32_t horizon,
+                         const double* d_floor, const double* d_cap, uint64_t seed,
+                         const double* d_future_reg, const double* d_reg_scale,
+                         double* d_yhat, double* d_yhat_lower, double* d_yhat_upper,
+                         int32_t* d_yhat_int);
+
+PB200_API int pb200_predict_regressors_host(pb200_ctx* ctx, const pb200_options* opts,
+                       const double* h_params, const double* h_tchange,
+                       const int32_t* h_meta_i32, const int64_t* h_meta_i64,
+                       const double* h_meta_f64, int64_t n_models,
+                       const int64_t* h_future_ds, int32_t horizon,
+                       const double* h_floor, const double* h_cap, uint64_t seed,
+                       const double* h_future_reg, const double* h_reg_scale,
+                       double* h_yhat, double* h_yhat_lower, double* h_yhat_upper,
+                       int32_t* h_yhat_int);
 
 #ifdef __cplusplus
 }

@@ -59,6 +59,24 @@ class OptionsV2(Options):
                 ("n_seasonalities", C.c_int32), ("seasonalities", C.POINTER(Seasonality))]
 
 
+ABI_VERSION_REGRESSORS = 3
+MAX_REGRESSORS = 16
+STD_AUTO = -1
+ST_BAD_REGRESSOR = -7
+
+
+class Regressor(C.Structure):
+    """struct pb200_regressor."""
+    _fields_ = [("name", C.c_char * 16), ("prior_scale", C.c_double), ("standardize", C.c_int32),
+                ("reserved", C.c_int32)]
+
+
+class OptionsV3(OptionsV2):
+    """struct pb200_options_v3: pb200_options_v2 followed by the extra regressors (DESIGN §19)."""
+    _fields_ = [("holidays_prior_scale", C.c_double), ("n_regressors", C.c_int32), ("reserved", C.c_int32),
+                ("regressors", C.POINTER(Regressor))]
+
+
 class Layout(C.Structure):
     """struct pb200_layout."""
     _fields_ = [("smax", C.c_int32), ("kmax", C.c_int32), ("pstride", C.c_int32),
@@ -76,7 +94,8 @@ EXPORTS = [
     "pb200_predict_quantiles_host", "pb200_cv_quantile_metrics_device", "pb200_predict_history_device",
     "pb200_predict_history_host", "pb200_outlier_counts_device", "pb200_outlier_compact_device",
     "pb200_predict_period_sums_device", "pb200_predict_period_sums_host", "pb200_period_host",
-    "pb200_last_fit_table_count", "pb200_component_count",
+    "pb200_last_fit_table_count", "pb200_component_count", "pb200_fit_regressors_device", "pb200_fit_regressors_host",
+    "pb200_objective_regressors_host", "pb200_predict_regressors_device", "pb200_predict_regressors_host",
 ]
 CV_ERR_HORIZON, CV_ERR_INITIAL, CV_ERR_FEW = 1, 2, 4
 
@@ -166,6 +185,16 @@ def load() -> C.CDLL:
     lib.pb200_make_future_device.restype = C.c_int
     lib.pb200_objective_host.argtypes = [vp, OP, vp, vp, i32, vp, i64, dbl, dbl, vp, vp, vp, vp]
     lib.pb200_objective_host.restype = C.c_int
+    lib.pb200_objective_regressors_host.argtypes = [vp, OP, vp, vp, i32, vp, i64, dbl, dbl, vp, vp, vp, vp, vp, vp]
+    lib.pb200_objective_regressors_host.restype = C.c_int
+    lib.pb200_fit_regressors_device.argtypes = fit_args[:10] + [vp, vp] + fit_args[10:]
+    lib.pb200_fit_regressors_device.restype = C.c_int
+    lib.pb200_fit_regressors_host.argtypes = fit_args[:10] + [vp, vp] + fit_args[10:] + [vp, i32]
+    lib.pb200_fit_regressors_host.restype = C.c_int
+    lib.pb200_predict_regressors_device.argtypes = pred_args[:13] + [vp, vp] + pred_args[13:]
+    lib.pb200_predict_regressors_device.restype = C.c_int
+    lib.pb200_predict_regressors_host.argtypes = pred_args[:13] + [vp, vp] + pred_args[13:]
+    lib.pb200_predict_regressors_host.restype = C.c_int
     lib.pb200_fit_trace_host.argtypes = [vp, OP, vp, vp, i32, vp, i64, dbl, dbl, vp, vp, vp, vp, vp, vp, i32]
     lib.pb200_fit_trace_host.restype = C.c_int
     lib.pb200_forecast_csv_lengths_device.argtypes = [vp, vp, vp, vp, i64, i32, vp]

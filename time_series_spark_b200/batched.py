@@ -157,6 +157,106 @@ def make_table_options(seasonalities=(), yearly_seasonality="auto", weekly_seaso
     return o
 
 
+def make_regressor_options(regressors=(), holidays_prior_scale: float = 10.0, **kw) -> L.OptionsV3:
+    """make_table_options plus fbprophet's add_regressor (DESIGN §19): a pb200_options_v3.
+
+    ``regressors``: dicts ``{name, prior_scale?, standardize?, mode?}`` in the order they were added.  ``prior_scale``
+    defaults to ``holidays_prior_scale``; ``standardize`` is 'auto' (the default), True or False; ``mode`` must be the
+    model's ``seasonality_mode``.  Other keyword arguments are make_table_options'.  With no regressor the options are
+    exactly make_table_options'.  The limits (16 regressors, K + R <= 64, P <= 96) are checked here and by the library.
+    The regressor values go to the ``regressors=`` argument of the fit and predict calls."""
+    mode = kw.get("seasonality_mode", "multiplicative")
+    o2 = make_table_options(**kw)
+    o = L.OptionsV3()
+    C.memmove(C.addressof(o), C.addressof(o2), C.sizeof(L.OptionsV2))
+    o._table = o2._table
+    o.abi_version = L.ABI_VERSION_REGRESSORS
+    hps = _number(holidays_prior_scale, "holidays_prior_scale")
+    if not (np.isfinite(hps) and hps > 0):
+        raise ValueError(f"holidays_prior_scale must be finite and > 0 (got {holidays_prior_scale!r})")
+    o.holidays_prior_scale = hps
+    regressors = list(regressors or ())
+    if len(regressors) > L.MAX_REGRESSORS:
+        raise ValueError(f"regressors: at most {L.MAX_REGRESSORS} entries (got {len(regressors)})")
+    seas_names = {o.seasonalities[i].name.decode() for i in range(o.n_seasonalities)} | {"yearly", "weekly", "daily"}
+    arr = (L.Regressor * max(1, len(regressors)))()
+    names = set()
+    for i, spec in enumerate(regressors):
+        key = f"regressors[{i}]"
+        if not isinstance(spec, dict):
+            raise ValueError(f"{key} must be a mapping with a name")
+        unknown = set(spec) - {"name", "prior_scale", "standardize", "mode"}
+        if unknown:
+            raise ValueError(f"{key}: unknown key(s) {sorted(unknown)}")
+        if "name" not in spec:
+            raise ValueError(f"{key}.name is required")
+        name = spec["name"]
+        if not isinstance(name, str) or not name or len(name.encode()) > 15:
+            raise ValueError(f"{key}.name must be a non-empty string of at most 15 bytes (got {name!r})")
+        if name in _RESERVED_NAMES or name.endswith(("_lower", "_upper")):
+            raise ValueError(f"{key}.name: {name!r} is reserved (fbprophet's validate_column_name)")
+        if name in seas_names:
+            raise ValueError(f"{key}.name: {name!r} is already used as a seasonality name")
+        if name in names:
+            raise ValueError(f"{key}.name: regressor {name!r} is added twice")
+        names.add(name)
+        ps = spec.get("prior_scale")
+        if ps is not None and not (np.isfinite(_number(ps, f"{key}.prior_scale")) and float(ps) > 0):
+            raise ValueError(f"{key}.prior_scale must be > 0 (got {ps!r})")
+        st = spec.get("standardize", "auto")
+        if not ((isinstance(st, str) and st == "auto") or isinstance(st, (bool, np.bool_))):
+            raise ValueError(f"{key}.standardize must be 'auto', True or False (got {st!r})")
+        rmode = spec.get("mode")
+        if rmode is not None and rmode != mode:
+            raise ValueError(f"{key}.mode: every regressor takes the model's seasonality_mode {mode!r} (got {rmode!r})")
+        arr[i].name = name.encode()
+        arr[i].prior_scale = 0.0 if ps is None else float(ps)
+        arr[i].standardize = L.STD_AUTO if isinstance(st, str) else int(bool(st))
+    o.n_regressors = len(regressors)
+    o.regressors = C.cast(arr, C.POINTER(L.Regressor))
+    o._regressors = arr     # keeps the entries alive as long as the options
+    L.get_layout(o)         # the library's checks: the limits and the refusals, before any GPU call
+    return o
+
+
+def _has_table(opts) -> bool:
+    """Whether ``opts`` carries a seasonality table: a pb200_options_v2, or a v3 (which embeds one)."""
+    return getattr(opts, "abi_version", L.ABI_VERSION) in (L.ABI_VERSION_TABLE, L.ABI_VERSION_REGRESSORS)
+
+
+def n_regressors(opts) -> int:
+    """R of ``opts``: its regressor count at version 3, else 0."""
+    return int(opts.n_regressors) if getattr(opts, "abi_version", L.ABI_VERSION) == L.ABI_VERSION_REGRESSORS else 0
+
+
+def regressor_scales(reg, offsets, standardize) -> np.ndarray:
+    """fbprophet 0.5's initialize_scales for the regressors, restated on the host (the test reference of the library's
+    standardisation): ``[n, R, 2]`` (mu, std) per series.  ``reg``: ``[R, n_rows]`` values aligned with the batch's rows;
+    ``standardize``: per regressor 'auto', True or False.  Fewer than two distinct values, or 'auto' on values that are
+    exactly {0, 1}: (0, 1); else the mean and the sample standard deviation (ddof = 1).  A non-finite value: (NaN, NaN)."""
+    reg = np.asarray(reg, np.float64)
+    offsets = np.asarray(offsets, np.int64)
+    n, R = offsets.size - 1, reg.shape[0]
+    out = np.zeros((n, R, 2))
+    out[:, :, 1] = 1.0
+    for i in range(n):
+        for r in range(R):
+            x = reg[r, offsets[i]:offsets[i + 1]]
+            if not np.all(np.isfinite(x)):
+                out[i, r] = np.nan
+                continue
+            vals = np.unique(x)
+            st = standardize[r]
+            if vals.size < 2:
+                continue
+            if isinstance(st, str):
+                st = set(vals.tolist()) != {0.0, 1.0}
+            if st:
+                mu = x.sum() / x.size
+                out[i, r] = mu, np.sqrt(((x - mu) ** 2).sum() / (x.size - 1))
+    return out
+
+
 _BUILTINS = (("yearly", 1, 365.25, 10), ("weekly", 2, 7.0, 3), ("daily", 4, 1.0, 4))
 
 
@@ -170,13 +270,14 @@ def seasonality_table(opts):
     ``(name, period, fourier_order, kind)`` in column order -- the custom entries as added, then the built-ins that are
     not off and not replaced by a custom entry of their name -- where ``kind`` is 0 for a custom entry and the built-in's
     mask bit (1 yearly, 2 weekly, 4 daily) otherwise.  None for v1 options and for a table that restates the defaults
-    (the v1 model)."""
-    if getattr(opts, "abi_version", L.ABI_VERSION) != L.ABI_VERSION_TABLE:
+    (the v1 model).  With regressors (version 3) it is never None: such a model is a table model even when its table
+    restates the defaults."""
+    if not _has_table(opts):
         return None
     custom = [opts.seasonalities[i] for i in range(opts.n_seasonalities)]
     orders = (opts.yearly_order, opts.weekly_order, opts.daily_order)
     switches = (opts.yearly, opts.weekly, opts.daily)
-    if not custom and all(o == 0 or o == d or s == 0 for o, s, (_, _, _, d) in zip(orders, switches, _BUILTINS)):
+    if not custom and not n_regressors(opts) and all(o == 0 or o == d or s == 0 for o, s, (_, _, _, d) in zip(orders, switches, _BUILTINS)):
         return None
     names = [e.name.decode() for e in custom]
     out = [(e.name.decode(), float(e.period), int(e.fourier_order), 0) for e in custom]
@@ -199,15 +300,22 @@ def table_mask(table, builtin_mask):
 def copy_options(opts):
     """A copy of ``opts`` that shares nothing mutable with it: the whole pb200_options_v2 for a table (its entries kept
     alive by the copy), pb200_options otherwise."""
-    if getattr(opts, "abi_version", L.ABI_VERSION) != L.ABI_VERSION_TABLE:
+    version = getattr(opts, "abi_version", L.ABI_VERSION)
+    if not _has_table(opts):
         return L.Options.from_buffer_copy(opts)
-    o = L.OptionsV2.from_buffer_copy(opts)
+    o = (L.OptionsV2 if version == L.ABI_VERSION_TABLE else L.OptionsV3).from_buffer_copy(opts)
     n = opts.n_seasonalities
     arr = (L.Seasonality * max(1, n))()
     for i in range(n):
         arr[i] = L.Seasonality.from_buffer_copy(opts.seasonalities[i])
     o.seasonalities = C.cast(arr, C.POINTER(L.Seasonality))
     o._table = arr
+    if version == L.ABI_VERSION_REGRESSORS:
+        regs = (L.Regressor * max(1, opts.n_regressors))()
+        for i in range(opts.n_regressors):
+            regs[i] = L.Regressor.from_buffer_copy(opts.regressors[i])
+        o.regressors = C.cast(regs, C.POINTER(L.Regressor))
+        o._regressors = regs
     return o
 
 
@@ -222,6 +330,7 @@ class FittedBatch:
     smax: int
     kmax: int
     warm: object = None  # [N] int32 L.WARM_* of a warm-started fit (where each series started); None for a cold fit
+    reg_scale: object = None  # [N, R, 2] f64 (mu, std) of each regressor (a fit with regressors), else None
 
     @property
     def n(self) -> int:
@@ -236,7 +345,8 @@ class FittedBatch:
             return self
         return FittedBatch(*(x.cpu().numpy() for x in (self.params, self.tchange, self.meta_i32,
                                                        self.meta_i64, self.meta_f64)),
-                           smax=self.smax, kmax=self.kmax, warm=None if self.warm is None else self.warm.cpu().numpy())
+                           smax=self.smax, kmax=self.kmax, warm=None if self.warm is None else self.warm.cpu().numpy(),
+                           reg_scale=None if self.reg_scale is None else self.reg_scale.cpu().numpy())
 
 
 def _seasonal_k(mask):
@@ -302,9 +412,35 @@ def _np_ptr(a: np.ndarray) -> int:
     return a.ctypes.data
 
 
+def _host_regressors(opts, regressors, rows: int) -> np.ndarray:
+    """The ``regressors=`` values of a host call: float64 ``[R, rows]``."""
+    R = n_regressors(opts)
+    reg = np.ascontiguousarray(regressors, dtype=np.float64)
+    if reg.size != R * rows:
+        raise ValueError(f"regressors must hold [{R}, {rows}] values (got shape {reg.shape})")
+    return reg.reshape(R, rows)
+
+
+def _check_reg_scale(reg_scale, n: int, R: int, what: str, dev=None) -> None:
+    """A (mu, std) array the library reads or writes as [n][R][2] doubles: float64, that shape, contiguous (and on ``dev``
+    for a device call)."""
+    if reg_scale is None:
+        raise ValueError(f"{what} is missing (a fit with regressors)")
+    dt = str(reg_scale.dtype).replace("torch.", "")
+    contiguous = reg_scale.is_contiguous() if dev is not None else True
+    if (dt != "float64" or tuple(reg_scale.shape) != (n, R, 2) or not contiguous
+            or (dev is not None and getattr(reg_scale, "device", None) != dev)):
+        raise ValueError(f"{what} must be a contiguous float64 array of shape ({n}, {R}, 2)"
+                         + (f" on {dev}" if dev is not None else "") + f" (got {dt} {tuple(reg_scale.shape)})")
+
+
 def fit_batch_host(ctx: L.Context, opts: L.Options, ds_ns: np.ndarray, y: np.ndarray, offsets: np.ndarray,
-                   floor: float, cap_multiplier: float, cap: Optional[np.ndarray] = None) -> FittedBatch:
-    """pb200_fit_host: numpy (ideally pinned) buffers in, numpy out; copies inside the call."""
+                   floor: float, cap_multiplier: float, cap: Optional[np.ndarray] = None, regressors=None) -> FittedBatch:
+    """pb200_fit_host: numpy (ideally pinned) buffers in, numpy out; copies inside the call.  ``regressors``: None, or
+    for options with regressors (make_regressor_options) their values ``[R, n_rows]`` aligned with ``ds_ns``
+    (pb200_fit_regressors_host); ``FittedBatch.reg_scale`` then holds each series' standardisation."""
+    if regressors is not None:
+        return _fit_regressors_host(ctx, opts, ds_ns, y, offsets, floor, cap_multiplier, cap, regressors, 0)[0]
     ds_ns = np.ascontiguousarray(ds_ns, dtype=np.int64)
     y = np.ascontiguousarray(y)
     offsets = np.ascontiguousarray(offsets, dtype=np.int64)
@@ -327,10 +463,39 @@ def fit_batch_host(ctx: L.Context, opts: L.Options, ds_ns: np.ndarray, y: np.nda
     return FittedBatch(params, tchange, mi32, mi64, mf64, lay.smax, lay.kmax)
 
 
+def _fit_regressors_host(ctx, opts, ds_ns, y, offsets, floor, cap_multiplier, cap, regressors, trace_cap: int):
+    ds_ns = np.ascontiguousarray(ds_ns, dtype=np.int64)
+    y = np.ascontiguousarray(y)
+    offsets = np.ascontiguousarray(offsets, dtype=np.int64)
+    n = offsets.size - 1
+    lay = L.get_layout(opts)
+    reg = _host_regressors(opts, regressors, ds_ns.size)
+    params = np.empty((n, lay.pstride), np.float64)
+    tchange = np.empty((n, lay.smax), np.float64)
+    mi32 = np.empty((n, 8), np.int32)
+    mi64 = np.empty((n, 2), np.int64)
+    mf64 = np.empty((n, 4), np.float64)
+    rsc = np.empty((n, reg.shape[0], 2), np.float64)
+    trace = np.zeros((n, trace_cap, 4), np.float64) if trace_cap > 0 else None
+    if cap is not None:
+        cap = np.ascontiguousarray(cap, dtype=np.float64)
+    if n > 0:
+        ptr = lambda a: None if a is None else _np_ptr(a)     # noqa: E731
+        rc = L.load().pb200_fit_regressors_host(ctx.handle, C.byref(opts), _np_ptr(ds_ns), _np_ptr(y), _y_dtype(y),
+                                                _np_ptr(offsets), n, float(floor), float(cap_multiplier), ptr(cap),
+                                                _np_ptr(reg), _np_ptr(rsc), _np_ptr(params), _np_ptr(tchange),
+                                                _np_ptr(mi32), _np_ptr(mi64), _np_ptr(mf64), ptr(trace), int(trace_cap))
+        L.check(rc, "pb200_fit_regressors_host")
+    return FittedBatch(params, tchange, mi32, mi64, mf64, lay.smax, lay.kmax, reg_scale=rsc), trace
+
+
 def fit_batch_trace_host(ctx: L.Context, opts: L.Options, ds_ns: np.ndarray, y: np.ndarray, offsets: np.ndarray,
-                         floor: float, cap_multiplier: float, trace_cap: int = 256):
+                         floor: float, cap_multiplier: float, trace_cap: int = 256, regressors=None):
     """pb200_fit_trace_host (parity-test hook): the fit plus, per series, one row
-    ``(iteration, f_k, alpha_k, n_evals)`` per accepted L-BFGS iteration (``[n, trace_cap, 4]``)."""
+    ``(iteration, f_k, alpha_k, n_evals)`` per accepted L-BFGS iteration (``[n, trace_cap, 4]``).  ``regressors``: as
+    fit_batch_host's (pb200_fit_regressors_host with the trajectory)."""
+    if regressors is not None:
+        return _fit_regressors_host(ctx, opts, ds_ns, y, offsets, floor, cap_multiplier, None, regressors, int(trace_cap))
     ds_ns = np.ascontiguousarray(ds_ns, dtype=np.int64)
     y = np.ascontiguousarray(y)
     offsets = np.ascontiguousarray(offsets, dtype=np.int64)
@@ -393,18 +558,51 @@ def fit_batch_warm_host(ctx: L.Context, opts: L.Options, ds_ns: np.ndarray, y: n
 
 def fit_batch_device(ctx: L.Context, opts: L.Options, ds_ns, y, offsets_host: np.ndarray,
                      floor: float, cap_multiplier: float, cap=None, out: Optional[FittedBatch] = None,
-                     sync: bool = True, prior=None, init: Optional[FittedBatch] = None) -> FittedBatch:
+                     sync: bool = True, prior=None, init: Optional[FittedBatch] = None, regressors=None) -> FittedBatch:
     """pb200_fit_warm_device: ``ds_ns`` / ``y`` / ``cap`` are torch CUDA tensors already in HBM.  ``prior``: None (the
     options' prior scales) or a float64 CUDA tensor ``[n, 2]`` of (changepoint_prior_scale, seasonality_prior_scale)
     per series; a series whose pair is not finite and > 0 gets status ``L.ST_BAD_PRIOR``.  ``init``: None (every
     series starts from fbprophet's stan_init) or the previous models, a FittedBatch (host or device) whose rows are
     aligned with the batch and whose layout is the options'; each series then starts from its previous optimum when
-    DESIGN §11's rule allows, and ``out.warm`` receives the ``L.WARM_*`` code of every series."""
+    DESIGN §11's rule allows, and ``out.warm`` receives the ``L.WARM_*`` code of every series.  ``regressors``: None, or
+    for options with regressors (make_regressor_options) a contiguous float64 CUDA tensor ``[R, n_rows]`` of their
+    values aligned with ``ds_ns`` (pb200_fit_regressors_device; not with ``prior`` or ``init``); ``out.reg_scale``
+    then receives each series' standardisation ``[n, R, 2]``."""
     import torch
     offsets_host = np.ascontiguousarray(offsets_host, dtype=np.int64)
     n = offsets_host.size - 1
     lay = L.get_layout(opts)
     dev = ds_ns.device
+    if regressors is not None:
+        if prior is not None or init is not None:
+            raise ValueError("regressors are not supported with prior or init")
+        R = n_regressors(opts)
+        rows = int(offsets_host[-1])
+        if (regressors.dtype != torch.float64 or tuple(regressors.shape) != (R, rows) or not regressors.is_contiguous()
+                or regressors.device != dev):
+            raise ValueError(f"regressors must be a contiguous float64 tensor of shape ({R}, {rows}) on {dev}")
+        if out is None:
+            out = FittedBatch(torch.empty((n, lay.pstride), dtype=torch.float64, device=dev),
+                              torch.empty((n, lay.smax), dtype=torch.float64, device=dev),
+                              torch.empty((n, 8), dtype=torch.int32, device=dev),
+                              torch.empty((n, 2), dtype=torch.int64, device=dev),
+                              torch.empty((n, 4), dtype=torch.float64, device=dev), lay.smax, lay.kmax)
+        if out.reg_scale is None:
+            out.reg_scale = torch.empty((n, R, 2), dtype=torch.float64, device=dev)
+        _check_reg_scale(out.reg_scale, n, R, "out.reg_scale", dev)
+        if n > 0:
+            torch.cuda.current_stream(dev).synchronize()
+            rc = L.load().pb200_fit_regressors_device(ctx.handle, C.byref(opts), ds_ns.data_ptr(), y.data_ptr(),
+                                                      _y_dtype(y), _np_ptr(offsets_host), n, float(floor),
+                                                      float(cap_multiplier), cap.data_ptr() if cap is not None else None,
+                                                      regressors.data_ptr(), out.reg_scale.data_ptr(),
+                                                      out.params.data_ptr(), out.tchange.data_ptr(),
+                                                      out.meta_i32.data_ptr(), out.meta_i64.data_ptr(),
+                                                      out.meta_f64.data_ptr())
+            L.check(rc, "pb200_fit_regressors_device")
+            if sync:
+                ctx.synchronize()
+        return out
     if init is not None:
         _check_init(init, n, lay)
     if out is None:
@@ -465,7 +663,7 @@ def component_names(opts: L.Options) -> tuple:
     n = L.load().pb200_component_count(C.byref(opts))
     L.check(min(n, 0), "pb200_component_count")
     extra = []
-    if getattr(opts, "abi_version", L.ABI_VERSION) == L.ABI_VERSION_TABLE:
+    if _has_table(opts):
         extra = [opts.seasonalities[i].name.decode() for i in range(opts.n_seasonalities)]
         extra = [x for x in extra if x not in ("yearly", "weekly", "daily")]
     names = L.COMPONENTS + tuple(extra)
@@ -536,10 +734,12 @@ def forecast_csv_row_host(series_id: int, dim_id: int, ds_ns: int, quantity: int
 
 def predict_batch_host(ctx: L.Context, opts: L.Options, fitted: FittedBatch, future_ds: np.ndarray,
                        floor: np.ndarray, cap: np.ndarray, seed: int = 0, intervals: bool = True,
-                       components: bool = False) -> ForecastBatch:
+                       components: bool = False, regressors=None) -> ForecastBatch:
     """pb200_predict_host.  ``floor`` / ``cap`` per model as the scorer reads them back from
     the float32 model-table columns (prophet_scorer.py:46-47,67-68).  ``components``: pb200_predict_components_host,
-    which also fills ``components`` and, with intervals, ``trend_lower`` / ``trend_upper``."""
+    which also fills ``components`` and, with intervals, ``trend_lower`` / ``trend_upper``.  ``regressors``: None, or
+    for a fit with regressors their future values ``[R, N, H]`` (pb200_predict_regressors_host, with the fit's
+    ``reg_scale``; not with ``components``)."""
     fitted = fitted.to_host()
     n = fitted.n
     future_ds = np.ascontiguousarray(future_ds, dtype=np.int64).reshape(n, -1)
@@ -555,13 +755,22 @@ def predict_batch_host(ctx: L.Context, opts: L.Options, fitted: FittedBatch, fut
     comp = np.empty((len(names), n, h), np.float64) if components else None
     tlo = np.empty((n, h), np.float64) if components and do_mc else None
     thi = np.empty((n, h), np.float64) if components and do_mc else None
+    if regressors is not None:
+        if components:
+            raise ValueError("components are not supported with regressors")
+        _check_reg_scale(fitted.reg_scale, n, n_regressors(opts), "fitted.reg_scale")
+        freg = _host_regressors(opts, regressors, n * h)
+        rsc = np.ascontiguousarray(fitted.reg_scale)
     if n > 0 and h > 0:
         args = (ctx.handle, C.byref(opts), _np_ptr(np.ascontiguousarray(fitted.params)),
                 _np_ptr(np.ascontiguousarray(fitted.tchange)), _np_ptr(np.ascontiguousarray(fitted.meta_i32)),
                 _np_ptr(np.ascontiguousarray(fitted.meta_i64)), _np_ptr(np.ascontiguousarray(fitted.meta_f64)),
                 n, _np_ptr(future_ds), h, _np_ptr(floor), _np_ptr(cap), int(seed) & (2**64 - 1),
                 _np_ptr(yhat), _np_ptr(lo) if do_mc else None, _np_ptr(hi) if do_mc else None, _np_ptr(yint))
-        if components:
+        if regressors is not None:
+            rc = L.load().pb200_predict_regressors_host(*args[:13], _np_ptr(freg), _np_ptr(rsc), *args[13:])
+            L.check(rc, "pb200_predict_regressors_host")
+        elif components:
             rc = L.load().pb200_predict_components_host(*args, _np_ptr(comp), _np_ptr(tlo) if do_mc else None,
                                                         _np_ptr(thi) if do_mc else None)
             L.check(rc, "pb200_predict_components_host")
@@ -573,9 +782,12 @@ def predict_batch_host(ctx: L.Context, opts: L.Options, fitted: FittedBatch, fut
 
 def predict_batch_device(ctx: L.Context, opts: L.Options, fitted: FittedBatch, future_ds, floor, cap,
                          seed: int = 0, intervals: bool = True, sync: bool = True,
-                         out: Optional["ForecastBatch"] = None, components: bool = False) -> ForecastBatch:
+                         out: Optional["ForecastBatch"] = None, components: bool = False,
+                         regressors=None) -> ForecastBatch:
     """pb200_predict_device with torch CUDA tensors (``out`` reuses a previous result's buffers, which must have been
-    made with the same ``components``).  ``components``: pb200_predict_components_device, as in predict_batch_host."""
+    made with the same ``components``).  ``components``: pb200_predict_components_device, as in predict_batch_host.
+    ``regressors``: None, or for a fit with regressors a contiguous float64 CUDA tensor ``[R, N, H]`` of their future
+    values (pb200_predict_regressors_device, with ``fitted.reg_scale``; not with ``components``)."""
     import torch
     n = fitted.n
     h = int(future_ds.shape[1])
@@ -599,7 +811,18 @@ def predict_batch_device(ctx: L.Context, opts: L.Options, fitted: FittedBatch, f
                 fitted.meta_i32.data_ptr(), fitted.meta_i64.data_ptr(), fitted.meta_f64.data_ptr(), n,
                 future_ds.data_ptr(), h, floor.data_ptr(), cap.data_ptr(), int(seed) & (2**64 - 1),
                 yhat.data_ptr(), lo.data_ptr() if do_mc else None, hi.data_ptr() if do_mc else None, yint.data_ptr())
-        if components:
+        if regressors is not None:
+            R = n_regressors(opts)
+            if components:
+                raise ValueError("components are not supported with regressors")
+            _check_reg_scale(fitted.reg_scale, n, R, "fitted.reg_scale", dev)
+            if (regressors.dtype != torch.float64 or regressors.numel() != R * n * h or not regressors.is_contiguous()
+                    or regressors.device != dev):
+                raise ValueError(f"regressors must be a contiguous float64 tensor of shape ({R}, {n}, {h}) on {dev}")
+            rc = L.load().pb200_predict_regressors_device(*args[:13], regressors.data_ptr(), fitted.reg_scale.data_ptr(),
+                                                          *args[13:])
+            L.check(rc, "pb200_predict_regressors_device")
+        elif components:
             rc = L.load().pb200_predict_components_device(*args, comp.data_ptr(), tlo.data_ptr() if do_mc else None,
                                                           thi.data_ptr() if do_mc else None)
             L.check(rc, "pb200_predict_components_device")
@@ -1034,9 +1257,11 @@ def predict_sums_anchored_device(ctx: L.Context, opts: L.Options, fitted: Fitted
 
 
 def objective_host(ctx: L.Context, opts: L.Options, ds_ns: np.ndarray, y: np.ndarray, offsets: np.ndarray,
-                   floor: float, cap_multiplier: float, theta: np.ndarray):
+                   floor: float, cap_multiplier: float, theta: np.ndarray, regressors=None):
     """pb200_objective_host (parity-test hook): objective and gradient at ``theta`` rows
-    (Stan unconstrained order k, m, delta[S], log sigma, beta[K], zero-padded to pstride)."""
+    (Stan unconstrained order k, m, delta[S], log sigma, beta[K], zero-padded to pstride).  ``regressors``: None, or
+    their values ``[R, n_rows]`` (pb200_objective_regressors_host: beta[K] is then the seasonal columns followed by the
+    R regressors); the standardisation used, ``[n, R, 2]``, is returned as a fourth value."""
     ds_ns = np.ascontiguousarray(ds_ns, dtype=np.int64)
     y = np.ascontiguousarray(y)
     offsets = np.ascontiguousarray(offsets, dtype=np.int64)
@@ -1047,6 +1272,15 @@ def objective_host(ctx: L.Context, opts: L.Options, ds_ns: np.ndarray, y: np.nda
     f = np.empty(n, np.float64)
     g = np.empty((n, lay.pstride), np.float64)
     mi32 = np.empty((n, 8), np.int32)
+    if regressors is not None:
+        reg = _host_regressors(opts, regressors, ds_ns.size)
+        rsc = np.empty((n, reg.shape[0], 2), np.float64)
+        rc = L.load().pb200_objective_regressors_host(ctx.handle, C.byref(opts), _np_ptr(ds_ns), _np_ptr(y), _y_dtype(y),
+                                                      _np_ptr(offsets), n, float(floor), float(cap_multiplier),
+                                                      _np_ptr(reg), _np_ptr(rsc), _np_ptr(th), _np_ptr(f), _np_ptr(g),
+                                                      _np_ptr(mi32))
+        L.check(rc, "pb200_objective_regressors_host")
+        return f, g, mi32, rsc
     rc = L.load().pb200_objective_host(ctx.handle, C.byref(opts), _np_ptr(ds_ns), _np_ptr(y), _y_dtype(y),
                                        _np_ptr(offsets), n, float(floor), float(cap_multiplier), _np_ptr(th),
                                        _np_ptr(f), _np_ptr(g), _np_ptr(mi32))
@@ -1134,7 +1368,7 @@ def _with_mask(opts: L.Options, mask: int) -> L.Options:
     AUTO."""
     o = copy_options(opts)
     custom = set()
-    if getattr(opts, "abi_version", L.ABI_VERSION) == L.ABI_VERSION_TABLE:
+    if _has_table(opts):
         custom = {opts.seasonalities[i].name.decode() for i in range(opts.n_seasonalities)}
     for name, bit, _, _ in _BUILTINS:
         if name not in custom:

@@ -9,6 +9,7 @@
 #include "csv_kernel.cuh"
 #include "cv_kernel.cuh"
 #include "insample_kernel.cuh"
+#include "reg_scale_kernel.cuh"
 
 #include <algorithm>
 #include <cstdio>
@@ -111,6 +112,8 @@ struct pb200_ctx {
     DevBuf d_sums;   // staging of pb200_predict_sums_host's window outputs
     DevBuf d_quant;  // staging of pb200_predict_quantiles_host's planes
     DevBuf d_hoff;   // device copy of pb200_predict_history_*'s frame offsets
+    DevBuf d_regbad;                // regressor fits: series with a non-finite regressor value (reg_scale_kernel -> prep_kernel)
+    DevBuf d_reg, d_regsc;          // staging of the regressor entry points' values and (mu, std)
     int lc0_max = 1 << 30; // PB200_LC0_MAX: longest series on one warp per series, longer ones get four (unset: no limit)
     bool lc_auto = true;   // false when PB200_LC0_MAX pins the CTA width
     bool tab_on = true;    // PB200_NO_TAB=1 disables the seasonal-table variants (A/B runs)
@@ -148,11 +151,18 @@ const launch_fn LAUNCH[8] = {pb200::launch_fit_mask0, pb200::launch_fit_mask1, p
                              pb200::launch_fit_mask6, pb200::launch_fit_mask7};
 
 int opts_table(const pb200_options* o, pb200::SeasTab* t);
+int opts_reg(const pb200_options* o, pb200::RegSpec* r);
 
-int check_opts(const pb200_options* o) {
+// options of version 2 and 3 carry a seasonality table (version 3 also the regressors)
+bool has_table(const pb200_options* o) {
+    return o->abi_version == PB200_ABI_VERSION_TABLE || o->abi_version == PB200_ABI_VERSION_REGRESSORS;
+}
+
+// regs: the caller is a regressor entry point (pb200_*_regressors_*) or pb200_get_layout.  Every other entry point refuses
+// options with regressors: it has nowhere to receive their values
+int check_opts(const pb200_options* o, bool regs = false) {
     if (!o) return fail(PB200_E_ARG, "options is null");
-    if (o->abi_version != PB200_ABI_VERSION && o->abi_version != PB200_ABI_VERSION_TABLE)
-        return fail(PB200_E_ARG, "options.abi_version mismatch");
+    if (o->abi_version != PB200_ABI_VERSION && !has_table(o)) return fail(PB200_E_ARG, "options.abi_version mismatch");
     if (o->growth != PB200_GROWTH_LINEAR && o->growth != PB200_GROWTH_LOGISTIC) return fail(PB200_E_ARG, "growth");
     if (o->n_changepoints < 0 || o->n_changepoints > 30) return fail(PB200_E_UNSUPPORTED, "n_changepoints must be in [0, 30]");
     if (o->history_size < 1 || o->history_size > pb200::HMAX) return fail(PB200_E_UNSUPPORTED, "history_size must be in [1, 5]");
@@ -162,16 +172,74 @@ int check_opts(const pb200_options* o) {
         if (v != PB200_SEAS_AUTO && v != 0 && v != 1) return fail(PB200_E_UNSUPPORTED, "seasonality switch must be AUTO, 0 or 1");
     if (o->max_iter < 1) return fail(PB200_E_ARG, "max_iter");
     if (o->algorithm < PB200_ALG_LBFGS_NEWTON || o->algorithm > PB200_ALG_NEWTON) return fail(PB200_E_ARG, "algorithm");
+    pb200::RegSpec r;
+    int rc = opts_reg(o, &r);
+    if (rc) return rc;
+    if (r.R > 0 && !regs)
+        return fail(PB200_E_UNSUPPORTED, "options with regressors (n_regressors > 0) are taken only by pb200_fit_regressors_*, "
+                                         "pb200_objective_regressors_host and pb200_predict_regressors_*");
     pb200::SeasTab t;
     return opts_table(o, &t);
 }
 
+// The regressors of *o (DESIGN §19), checked: r->R = 0 below version 3
+int opts_reg(const pb200_options* o, pb200::RegSpec* r) {
+    r->R = 0;
+    if (o->abi_version != PB200_ABI_VERSION_REGRESSORS) return PB200_OK;
+    const pb200_options_v3* v = reinterpret_cast<const pb200_options_v3*>(o);
+    char msg[200];
+    const int n = v->n_regressors;
+    if (n < 0 || n > PB200_MAX_REGRESSORS) {
+        snprintf(msg, sizeof msg, "n_regressors must be in [0, %d] (got %d)", PB200_MAX_REGRESSORS, n);
+        return fail(PB200_E_UNSUPPORTED, msg);
+    }
+    if (n == 0) return PB200_OK;
+    if (!v->regressors) return fail(PB200_E_ARG, "regressors is null");
+    if (!(v->holidays_prior_scale > 0.0 && v->holidays_prior_scale < INFINITY))
+        return fail(PB200_E_ARG, "holidays_prior_scale must be finite and > 0");
+    for (int i = 0; i < n; ++i) {
+        const pb200_regressor& e = v->regressors[i];
+        const size_t len = strnlen(e.name, sizeof e.name);
+        if (len == 0 || len == sizeof e.name) return fail(PB200_E_ARG, "regressor name must be 1 to 15 bytes, NUL-terminated");
+        for (int j = 0; j < i; ++j)
+            if (strncmp(e.name, v->regressors[j].name, sizeof e.name) == 0) {
+                snprintf(msg, sizeof msg, "regressor '%s' is added twice", e.name);
+                return fail(PB200_E_ARG, msg);
+            }
+        bool seas_name = strcmp(e.name, "yearly") == 0 || strcmp(e.name, "weekly") == 0 || strcmp(e.name, "daily") == 0;
+        for (int j = 0; j < v->v2.n_seasonalities && v->v2.seasonalities; ++j)
+            seas_name = seas_name || strncmp(e.name, v->v2.seasonalities[j].name, sizeof e.name) == 0;
+        if (seas_name) {
+            snprintf(msg, sizeof msg, "regressor '%s' has a seasonality's name", e.name);
+            return fail(PB200_E_ARG, msg);
+        }
+        if (!(e.prior_scale >= 0.0 && e.prior_scale < INFINITY)) {
+            snprintf(msg, sizeof msg, "regressor '%s': prior_scale must be > 0 (got %g)", e.name, e.prior_scale);
+            return fail(PB200_E_ARG, msg);
+        }
+        if (e.standardize != PB200_STD_AUTO && e.standardize != 0 && e.standardize != 1) {
+            snprintf(msg, sizeof msg, "regressor '%s': standardize must be AUTO, 0 or 1", e.name);
+            return fail(PB200_E_ARG, msg);
+        }
+        const double ps = e.prior_scale > 0.0 ? e.prior_scale : v->holidays_prior_scale;
+        r->standardize[i] = e.standardize;
+        r->inv_sig2[i] = 1.0 / (ps * ps);
+    }
+    r->R = n;
+    return PB200_OK;
+}
+
 // The seasonality table of *o, normalised to fbprophet's column order (custom entries as added, then yearly, weekly,
 // daily) and checked against the limits.  t->n = 0 for a v1 model and for a v2 one that restates the defaults.
+//
+// Options of version 3 with regressors are table models even when the table restates the defaults; their limits count
+// the R regressor columns with the seasonal ones.
 int opts_table(const pb200_options* o, pb200::SeasTab* t) {
     t->n = 0;
-    if (o->abi_version != PB200_ABI_VERSION_TABLE) return PB200_OK;
+    if (!has_table(o)) return PB200_OK;
     const pb200_options_v2* v = reinterpret_cast<const pb200_options_v2*>(o);
+    const int R = o->abi_version == PB200_ABI_VERSION_REGRESSORS
+                      ? std::max(0, reinterpret_cast<const pb200_options_v3*>(o)->n_regressors) : 0;
     char msg[160];
     const int ns = v->n_seasonalities;
     if (ns < 0 || ns > PB200_MAX_SEASONALITIES) {
@@ -218,7 +286,7 @@ int opts_table(const pb200_options* o, pb200::SeasTab* t) {
                 replaced[b] = true;
             }
     }
-    bool restates = ns == 0;
+    bool restates = ns == 0 && R == 0;
     for (int b = 0; b < 3; ++b) restates = restates && (ord[b] == 0 || ord[b] == dflt[b] || sw[b] == 0);
     if (restates) return PB200_OK;
     int n = 0;
@@ -246,9 +314,16 @@ int opts_table(const pb200_options* o, pb200::SeasTab* t) {
         snprintf(msg, sizeof msg, "the seasonalities have K = %d Fourier columns; at most %d", K, pb200::SEAS_KMAX);
         return fail(PB200_E_UNSUPPORTED, msg);
     }
+    if (R > 0 && K + R > pb200::SEAS_KMAX) {
+        snprintf(msg, sizeof msg, "the seasonalities' K = %d columns and the %d regressors make %d; at most %d", K, R, K + R,
+                 pb200::SEAS_KMAX);
+        return fail(PB200_E_UNSUPPORTED, msg);
+    }
+    K += R;
     const int P = 3 + (o->n_changepoints > 0 ? o->n_changepoints : 1) + K;
     if (P > pb200::SEAS_PMAX) {
-        snprintf(msg, sizeof msg, "the model has P = 3 + S + K = %d parameters; at most %d", P, pb200::SEAS_PMAX);
+        snprintf(msg, sizeof msg, R > 0 ? "the model has P = 3 + S + K + R = %d parameters; at most %d"
+                                        : "the model has P = 3 + S + K = %d parameters; at most %d", P, pb200::SEAS_PMAX);
         return fail(PB200_E_UNSUPPORTED, msg);
     }
     t->n = n;
@@ -334,7 +409,7 @@ PB200_API void pb200_default_options(pb200_options* o) {
 }
 
 PB200_API int pb200_get_layout(const pb200_options* o, pb200_layout* out) {
-    int rc = check_opts(o);
+    int rc = check_opts(o, true);
     if (rc) return rc;
     if (!out) return fail(PB200_E_ARG, "layout is null");
     out->smax = o->n_changepoints > 0 ? o->n_changepoints : 1;
@@ -344,7 +419,9 @@ PB200_API int pb200_get_layout(const pb200_options* o, pb200_layout* out) {
     if (o->daily != 0) k += 8;
     pb200::SeasTab t;
     opts_table(o, &t);
-    if (t.n > 0) k = pb200::tab_k(t, (1 << t.n) - 1);
+    pb200::RegSpec r;
+    opts_reg(o, &r);
+    if (t.n > 0 || r.R > 0) k = pb200::tab_k(t, (1 << t.n) - 1) + r.R;
     out->kmax = k > 0 ? k : 1;
     out->pstride = 3 + out->smax + out->kmax;
     out->meta_i32_stride = 8;
@@ -406,7 +483,8 @@ PB200_API void pb200_destroy(pb200_ctx* c) {
     cudaStreamSynchronize(c->stream);
     for (DevBuf* b : {&c->d_ds, &c->d_y, &c->d_cap, &c->d_params, &c->d_tchange, &c->d_mi32, &c->d_mi64, &c->d_mf64, &c->d_fut,
                       &c->d_floor, &c->d_yhat, &c->d_lo, &c->d_hi, &c->d_yint, &c->d_comp, &c->d_tlo, &c->d_thi, &c->d_mc, &c->d_sums, &c->d_trace, &c->d_warm_x, &c->d_prior, &c->d_iparams, &c->d_imeta, &c->d_warm, &c->d_vcount, &c->d_offsets,
-                      &c->d_order, &c->d_lenclass, &c->d_qitems, &c->d_qctl, &c->d_nq, &c->d_planes, &c->d_qkey, &c->d_qhist})
+                      &c->d_order, &c->d_lenclass, &c->d_qitems, &c->d_qctl, &c->d_nq, &c->d_planes, &c->d_qkey, &c->d_qhist,
+                      &c->d_regbad, &c->d_reg, &c->d_regsc})
         b->release();
     c->h_ctl.release();
     cudaEventDestroy(c->ctl_ev);
@@ -465,7 +543,8 @@ PB200_API int pb200_synchronize(pb200_ctx* c) {
 // newton_kernel over the queue {count, head, items...} at d_nq (16-warp CTAs with up to ~113 KB of shared memory, at P = 67)
 static int launch_newton(pb200_ctx* c, const pb200_options* opts, const int64_t* d_ds, const void* d_y,
                          int32_t y_dtype, const int64_t* d_offsets, int64_t n_series, int* d_nq, const double* d_prior,
-                         const double* d_x0, double* d_params, double* d_tchange, int32_t* d_meta_i32, int64_t* d_meta_i64, double* d_meta_f64) {
+                         const double* d_x0, double* d_params, double* d_tchange, int32_t* d_meta_i32, int64_t* d_meta_i64, double* d_meta_f64,
+                         const double* d_reg, const double* d_reg_scale, int64_t n_rows) {
     static_assert(pb200::SEAS_PMAX <= pb200::nw::NW_PMAX, "newton_kernel holds every P check_opts admits");
     pb200_layout L;
     pb200_get_layout(opts, &L);
@@ -490,6 +569,10 @@ static int launch_newton(pb200_ctx* c, const pb200_options* opts, const int64_t*
     na.x0 = d_x0;
     na.o = to_dev(opts);
     opts_table(opts, &na.tab);
+    opts_reg(opts, &na.reg);
+    na.reg_x = d_reg;
+    na.reg_scale = d_reg_scale;
+    na.n_rows = n_rows;
     const size_t nsm = pb200::nw::newton_smem_bytes(L.pstride);
     CK(cudaFuncSetAttribute(pb200::nw::newton_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)nsm));
     int ngrid = (int)std::min<int64_t>(n_series, opts->algorithm == PB200_ALG_NEWTON ? (int64_t)c->sms * 2 : (int64_t)c->sms);
@@ -508,16 +591,20 @@ static int fit_impl(pb200_ctx* c, const pb200_options* opts, const int64_t* d_ds
                     const double* d_cap, const double* d_prior, double* d_params, double* d_tchange, int32_t* d_meta_i32,
                     int64_t* d_meta_i64, double* d_meta_f64, const double* d_theta_in, double* d_grad_out,
                     double* d_trace = nullptr, int trace_cap = 0, const double* d_init_params = nullptr,
-                    const int32_t* d_init_meta = nullptr, int32_t* d_warm = nullptr) {
+                    const int32_t* d_init_meta = nullptr, int32_t* d_warm = nullptr, bool regs = false,
+                    const double* d_reg = nullptr, double* d_reg_scale = nullptr) {
     if (!c) return fail(PB200_E_ARG, "ctx is null");
     CK(cudaSetDevice(c->device));
     CK(c->d_vcount.reserve((NQ + 1) * 4));     // [NQ]: the table class
     CK(cudaMemsetAsync(c->d_vcount.p, 0, (NQ + 1) * 4, c->stream));
-    int rc = check_opts(opts);
+    int rc = check_opts(opts, regs);
     if (rc) return rc;
     pb200::SeasTab tab;
     opts_table(opts, &tab);
-    if (tab.n > 0) {
+    pb200::RegSpec reg;
+    opts_reg(opts, &reg);
+    const bool tabcls = tab.n > 0 || reg.R > 0;     // the table class (fit_table.cu)
+    if (tabcls) {
         if (d_prior) return fail(PB200_E_UNSUPPORTED, "per-series prior scales are not supported with a seasonality table");
         if (d_init_params) return fail(PB200_E_UNSUPPORTED, "warm start is not supported with a seasonality table");
     }
@@ -528,6 +615,7 @@ static int fit_impl(pb200_ctx* c, const pb200_options* opts, const int64_t* d_ds
         return fail(PB200_E_ARG, "null pointer");
     if (y_dtype < 0 || y_dtype > 2) return fail(PB200_E_ARG, "y_dtype");
     if (d_init_params && !d_init_meta) return fail(PB200_E_ARG, "d_init_meta_i32 is null");
+    if (reg.R > 0 && (!d_reg || !d_reg_scale)) return fail(PB200_E_ARG, "null pointer (regressors / reg_scale)");
     pb200_layout L;
     pb200_get_layout(opts, &L);
     const int N = (int)n_series;
@@ -597,6 +685,22 @@ static int fit_impl(pb200_ctx* c, const pb200_options* opts, const int64_t* d_ds
     CK(cudaMemsetAsync(d_tchange, 0, (size_t)N * L.smax * 8, c->stream));
     int* q_count = (int*)c->d_qctl.p;
     int* q_head = q_count + NQT;
+    const int64_t n_rows = ho[N];
+    // ---- the regressors' standardisation, which prep_kernel's status and every evaluation read ----
+    if (reg.R > 0) {
+        CK(c->d_regbad.reserve((size_t)N));
+        pb200::RegScaleArgs ra;
+        ra.reg = d_reg;
+        ra.n_rows = n_rows;
+        ra.offsets = (const long long*)c->d_offsets.p;
+        ra.n_series = N;
+        ra.spec = reg;
+        ra.reg_scale = d_reg_scale;
+        ra.bad = (unsigned char*)c->d_regbad.p;
+        pb200::reg_scale_kernel<<<std::min((N + 7) / 8, c->sms * 8), 256, 0, c->stream>>>(ra);
+        CK(cudaGetLastError());
+        c->launches++;
+    }
 
     const FitOptsDev od = to_dev(opts);
     // lanes per series of the grouped day-table kernel
@@ -641,6 +745,7 @@ static int fit_impl(pb200_ctx* c, const pb200_options* opts, const int64_t* d_ds
         pa.pstride = L.pstride;
         pa.tab = tab;
         pa.tab_queue = NLC * NQ;
+        pa.reg_bad = reg.R > 0 ? (const unsigned char*)c->d_regbad.p : nullptr;
         const int warps_per_block = 8;
         int grid = (N + warps_per_block - 1) / warps_per_block;
         grid = std::min(grid, c->sms * 8);
@@ -665,7 +770,7 @@ static int fit_impl(pb200_ctx* c, const pb200_options* opts, const int64_t* d_ds
             Geo& g = geo[lc][rm];
             g.on = false;
             g.grouped = false;
-            if (lc_n[lc] == 0 || tab.n > 0) continue;
+            if (lc_n[lc] == 0 || tabcls) continue;
             const bool plain_grp = reg == 3 && mask == 0 && grp_g > 0 && c->plain_grp;   // grouped kernel's class without seasonality
             if (reg && mask == 0 && !plain_grp) continue;                // no Fourier features: nothing to regenerate
             if (reg >= 2 && ((mask != 6 && !plain_grp) || LC_NT[lc] != 32 || !c->tab_on)) continue;   // seasonal-table variants
@@ -702,23 +807,30 @@ static int fit_impl(pb200_ctx* c, const pb200_options* opts, const int64_t* d_ds
             planes_bytes += (size_t)g.grid * g.slice * 16;
             g.on = true;
         }
-    // the table class: one warp per series, (t, y) and one base (sin, cos) plane per table entry in each slice
-    int tab_grid = 0, tab_Tp = 0, tab_ppad = 0;
+    // the table class: one warp per series, (t, y) and one base (sin, cos) plane per table entry in each slice, then
+    // ceil(R / 2) planes of the standardised regressors
+    int tab_grid = 0, tab_Tp = 0, tab_ppad = 0, tab_planes = 0;
     size_t tab_smem = 0, tab_off = 0;
-    if (tab.n > 0) {
+    if (tabcls) {
         tab_Tp = (int)(((tmax_all + (tmax_all + 31) / 32 + 7) / 8) * 8);
         tab_ppad = (L.pstride + 1) & ~1;
-        tab_smem = pb200::fit_table_smem(tab_ppad);
+        tab_planes = 1 + tab.n + (reg.R + 1) / 2;
+        tab_smem = reg.R > 0 ? pb200::fit_table_reg_smem(tab_ppad) : pb200::fit_table_smem(tab_ppad);
         int occ = 0;
-        pb200::TableFitArgs dummy{};
-        CK(pb200::launch_fit_table(opts->growth, dummy, 0, tab_smem, c->stream, &occ));
+        if (reg.R > 0) {
+            pb200::RegTableFitArgs dummy{};
+            CK(pb200::launch_fit_table_reg(opts->growth, dummy, 0, tab_smem, c->stream, &occ));
+        } else {
+            pb200::TableFitArgs dummy{};
+            CK(pb200::launch_fit_table(opts->growth, dummy, 0, tab_smem, c->stream, &occ));
+        }
         if (occ < 1) return fail(PB200_E_UNSUPPORTED, "table fit kernel does not fit on an SM");
         tab_grid = cap_grid(std::min<int64_t>((int64_t)N, (int64_t)c->sms * occ));
         tab_off = planes_bytes;
-        planes_bytes += (size_t)tab_grid * (1 + tab.n) * tab_Tp * 16;
+        planes_bytes += (size_t)tab_grid * tab_planes * tab_Tp * 16;
     }
     CK(c->d_planes.reserve(planes_bytes));
-    if (tab.n > 0) {
+    if (tabcls) {
         pb200::TableFitArgs fa;
         fa.ds = (const long long*)d_ds;
         fa.y = d_y;
@@ -739,7 +851,7 @@ static int fit_impl(pb200_ctx* c, const pb200_options* opts, const int64_t* d_ds
         fa.Tp = tab_Tp;
         fa.ppad = tab_ppad;
         fa.planes = (double2*)((char*)c->d_planes.p + tab_off);
-        fa.nseas_stride = (1 + tab.n) * tab_Tp;
+        fa.nseas_stride = tab_planes * tab_Tp;
         fa.theta_in = d_theta_in;
         fa.grad_out = d_grad_out;
         fa.trace = d_trace;
@@ -750,10 +862,20 @@ static int fit_impl(pb200_ctx* c, const pb200_options* opts, const int64_t* d_ds
         fa.l2_keep = fa.l2_rest_first = 0;
         fa.prior = nullptr;
         fa.tab = tab;
-        CK(pb200::launch_fit_table(opts->growth, fa, tab_grid, tab_smem, c->stream, nullptr));
+        if (reg.R > 0) {
+            pb200::RegTableFitArgs ra;
+            static_cast<pb200::TableFitArgs&>(ra) = fa;
+            ra.reg = d_reg;
+            ra.reg_scale = d_reg_scale;
+            ra.n_rows = n_rows;
+            ra.spec = reg;
+            CK(pb200::launch_fit_table_reg(opts->growth, ra, tab_grid, tab_smem, c->stream, nullptr));
+        } else {
+            CK(pb200::launch_fit_table(opts->growth, fa, tab_grid, tab_smem, c->stream, nullptr));
+        }
         c->launches++;
     }
-    for (int lc = 0; lc < NLC && tab.n == 0; ++lc) {
+    for (int lc = 0; lc < NLC && !tabcls; ++lc) {
         if (lc_n[lc] == 0) continue;
         const int NT = LC_NT[lc];
         for (int rm = 0; rm < NQ; ++rm) {
@@ -811,15 +933,15 @@ static int fit_impl(pb200_ctx* c, const pb200_options* opts, const int64_t* d_ds
     // ---- fbprophet's Newton retry over the series whose L-BFGS failed its line search (normally an empty queue) ----
     if (!d_grad_out)
         return launch_newton(c, opts, d_ds, d_y, y_dtype, (const int64_t*)c->d_offsets.p, n_series, nq, d_prior, warm_x,
-                             d_params, d_tchange, d_meta_i32, d_meta_i64, d_meta_f64);
+                             d_params, d_tchange, d_meta_i32, d_meta_i64, d_meta_f64, d_reg, d_reg_scale, n_rows);
     return PB200_OK;
 }
 
 // argument checks of the *_host fit entry points (outs: the caller's own pointers are all set); n_series == 0 passes
 static int check_host_fit(pb200_ctx* c, const pb200_options* opts, const int64_t* h_ds, const void* h_y, int32_t y_dtype,
-                          const int64_t* h_offsets, int64_t n_series, bool outs) {
+                          const int64_t* h_offsets, int64_t n_series, bool outs, bool regs = false) {
     if (!c) return fail(PB200_E_ARG, "ctx is null");
-    int rc = check_opts(opts);
+    int rc = check_opts(opts, regs);
     if (rc) return rc;
     if (n_series <= 0) return n_series == 0 ? PB200_OK : fail(PB200_E_ARG, "n_series");
     if (!h_ds || !h_y || !h_offsets || !outs) return fail(PB200_E_ARG, "null pointer");
@@ -827,9 +949,11 @@ static int check_host_fit(pb200_ctx* c, const pb200_options* opts, const int64_t
     return PB200_OK;
 }
 
-// ... and their common staging: ds and y copied in, room for the fitted records
+// ... and their common staging: ds and y copied in, room for the fitted records; with regressors (h_reg, h_reg_scale
+// non-null) their values copied in and room for their (mu, std)
 static int stage_host_fit(pb200_ctx* c, const pb200_options* opts, const int64_t* h_ds, const void* h_y, int32_t y_dtype,
-                          const int64_t* h_offsets, int64_t n_series) {
+                          const int64_t* h_offsets, int64_t n_series, const double* h_reg = nullptr,
+                          const double* h_reg_scale = nullptr) {
     pb200_layout L;
     pb200_get_layout(opts, &L);
     CK(cudaSetDevice(c->device));
@@ -844,6 +968,14 @@ static int stage_host_fit(pb200_ctx* c, const pb200_options* opts, const int64_t
     CK(c->d_mf64.reserve(N * 4 * 8));
     CK(cudaMemcpyAsync(c->d_ds.p, h_ds, (size_t)R * 8, cudaMemcpyHostToDevice, c->stream));
     CK(cudaMemcpyAsync(c->d_y.p, h_y, (size_t)R * y_elem(y_dtype), cudaMemcpyHostToDevice, c->stream));
+    pb200::RegSpec reg;
+    opts_reg(opts, &reg);
+    if (reg.R > 0) {
+        if (!h_reg || !h_reg_scale) return fail(PB200_E_ARG, "null pointer (regressors / reg_scale)");
+        CK(c->d_reg.reserve((size_t)reg.R * R * 8));
+        CK(c->d_regsc.reserve(N * reg.R * 2 * 8));
+        CK(cudaMemcpyAsync(c->d_reg.p, h_reg, (size_t)reg.R * R * 8, cudaMemcpyHostToDevice, c->stream));
+    }
     return PB200_OK;
 }
 
@@ -853,13 +985,16 @@ static int fit_host(pb200_ctx* c, const pb200_options* opts, const int64_t* h_ds
                     const int64_t* h_offsets, int64_t n_series, double floor, double cap_multiplier, const double* h_cap,
                     double* h_params, double* h_tchange, int32_t* h_meta_i32, int64_t* h_meta_i64, double* h_meta_f64,
                     bool traced, double* h_trace, int32_t trace_cap, const double* h_prior = nullptr,
-                    const double* h_init_params = nullptr, const int32_t* h_init_meta = nullptr, int32_t* h_warm = nullptr) {
+                    const double* h_init_params = nullptr, const int32_t* h_init_meta = nullptr, int32_t* h_warm = nullptr,
+                    bool regs = false, const double* h_reg = nullptr, double* h_reg_scale = nullptr) {
     int rc = check_host_fit(c, opts, h_ds, h_y, y_dtype, h_offsets, n_series,
-                            h_params && h_tchange && h_meta_i32 && h_meta_i64 && h_meta_f64 && (h_trace || !traced));
+                            h_params && h_tchange && h_meta_i32 && h_meta_i64 && h_meta_f64 && (h_trace || !traced), regs);
     if (rc || n_series == 0) return rc;
     if (h_init_params && !h_init_meta) return fail(PB200_E_ARG, "h_init_meta_i32 is null");
     if (traced && (trace_cap < 1 || (int64_t)trace_cap * n_series > (1LL << 26))) return fail(PB200_E_ARG, "trace_cap");
-    if ((rc = stage_host_fit(c, opts, h_ds, h_y, y_dtype, h_offsets, n_series))) return rc;
+    if ((rc = stage_host_fit(c, opts, h_ds, h_y, y_dtype, h_offsets, n_series, h_reg, h_reg_scale))) return rc;
+    pb200::RegSpec reg;
+    opts_reg(opts, &reg);
     pb200_layout L;
     pb200_get_layout(opts, &L);
     const size_t N = (size_t)n_series, tbytes = traced ? N * (size_t)trace_cap * 4 * 8 : 0;
@@ -889,9 +1024,11 @@ static int fit_host(pb200_ctx* c, const pb200_options* opts, const int64_t* h_ds
                   (int32_t*)c->d_mi32.p, (int64_t*)c->d_mi64.p, (double*)c->d_mf64.p, nullptr, nullptr,
                   traced ? (double*)c->d_trace.p : nullptr, trace_cap,
                   h_init_params ? (const double*)c->d_iparams.p : nullptr,
-                  h_init_params ? (const int32_t*)c->d_imeta.p : nullptr, warm_out ? (int32_t*)c->d_warm.p : nullptr);
+                  h_init_params ? (const int32_t*)c->d_imeta.p : nullptr, warm_out ? (int32_t*)c->d_warm.p : nullptr, regs,
+                  reg.R > 0 ? (const double*)c->d_reg.p : nullptr, reg.R > 0 ? (double*)c->d_regsc.p : nullptr);
     if (rc) return rc;
     if (warm_out) CK(cudaMemcpyAsync(h_warm, c->d_warm.p, N * 4, cudaMemcpyDeviceToHost, c->stream));
+    if (reg.R > 0) CK(cudaMemcpyAsync(h_reg_scale, c->d_regsc.p, N * reg.R * 2 * 8, cudaMemcpyDeviceToHost, c->stream));
     CK(cudaMemcpyAsync(h_params, c->d_params.p, N * L.pstride * 8, cudaMemcpyDeviceToHost, c->stream));
     CK(cudaMemcpyAsync(h_tchange, c->d_tchange.p, N * L.smax * 8, cudaMemcpyDeviceToHost, c->stream));
     CK(cudaMemcpyAsync(h_meta_i32, c->d_mi32.p, N * 8 * 4, cudaMemcpyDeviceToHost, c->stream));
@@ -942,13 +1079,18 @@ PB200_API int pb200_fit_device(pb200_ctx* c, const pb200_options* opts, const in
                                   d_params, d_tchange, d_meta_i32, d_meta_i64, d_meta_f64);
 }
 
-PB200_API int pb200_objective_host(pb200_ctx* c, const pb200_options* opts, const int64_t* h_ds, const void* h_y,
-                                   int32_t y_dtype, const int64_t* h_offsets, int64_t n_series, double floor,
-                                   double cap_multiplier, const double* h_theta, double* h_f, double* h_grad,
-                                   int32_t* h_meta_i32) {
-    int rc = check_host_fit(c, opts, h_ds, h_y, y_dtype, h_offsets, n_series, h_theta && h_f && h_grad && h_meta_i32);
+}  // extern "C"
+
+// pb200_objective_host and pb200_objective_regressors_host (regs; h_reg / h_reg_scale as pb200_fit_regressors_host's)
+static int objective_host(pb200_ctx* c, const pb200_options* opts, const int64_t* h_ds, const void* h_y, int32_t y_dtype,
+                          const int64_t* h_offsets, int64_t n_series, double floor, double cap_multiplier,
+                          const double* h_theta, double* h_f, double* h_grad, int32_t* h_meta_i32, bool regs = false,
+                          const double* h_reg = nullptr, double* h_reg_scale = nullptr) {
+    int rc = check_host_fit(c, opts, h_ds, h_y, y_dtype, h_offsets, n_series, h_theta && h_f && h_grad && h_meta_i32, regs);
     if (rc || n_series == 0) return rc;
-    if ((rc = stage_host_fit(c, opts, h_ds, h_y, y_dtype, h_offsets, n_series))) return rc;
+    if ((rc = stage_host_fit(c, opts, h_ds, h_y, y_dtype, h_offsets, n_series, h_reg, h_reg_scale))) return rc;
+    pb200::RegSpec reg;
+    opts_reg(opts, &reg);
     pb200_layout L;
     pb200_get_layout(opts, &L);
     const size_t N = (size_t)n_series;
@@ -958,8 +1100,11 @@ PB200_API int pb200_objective_host(pb200_ctx* c, const pb200_options* opts, cons
     CK(cudaMemsetAsync(c->d_lo.p, 0, N * L.pstride * 8, c->stream));
     rc = fit_impl(c, opts, (const int64_t*)c->d_ds.p, c->d_y.p, y_dtype, h_offsets, n_series, floor, cap_multiplier,
                   nullptr, nullptr, (double*)c->d_params.p, (double*)c->d_tchange.p, (int32_t*)c->d_mi32.p,
-                  (int64_t*)c->d_mi64.p, (double*)c->d_mf64.p, (const double*)c->d_yhat.p, (double*)c->d_lo.p);
+                  (int64_t*)c->d_mi64.p, (double*)c->d_mf64.p, (const double*)c->d_yhat.p, (double*)c->d_lo.p, nullptr, 0,
+                  nullptr, nullptr, nullptr, regs, reg.R > 0 ? (const double*)c->d_reg.p : nullptr,
+                  reg.R > 0 ? (double*)c->d_regsc.p : nullptr);
     if (rc) return rc;
+    if (reg.R > 0) CK(cudaMemcpyAsync(h_reg_scale, c->d_regsc.p, N * reg.R * 2 * 8, cudaMemcpyDeviceToHost, c->stream));
     std::vector<double> mf(N * 4);
     CK(cudaMemcpyAsync(h_grad, c->d_lo.p, N * L.pstride * 8, cudaMemcpyDeviceToHost, c->stream));
     CK(cudaMemcpyAsync(h_meta_i32, c->d_mi32.p, N * 8 * 4, cudaMemcpyDeviceToHost, c->stream));
@@ -967,6 +1112,44 @@ PB200_API int pb200_objective_host(pb200_ctx* c, const pb200_options* opts, cons
     CK(cudaStreamSynchronize(c->stream));
     for (size_t i = 0; i < N; ++i) h_f[i] = mf[i * 4 + 3];
     return PB200_OK;
+}
+
+extern "C" {
+
+PB200_API int pb200_objective_host(pb200_ctx* c, const pb200_options* opts, const int64_t* h_ds, const void* h_y,
+                                   int32_t y_dtype, const int64_t* h_offsets, int64_t n_series, double floor,
+                                   double cap_multiplier, const double* h_theta, double* h_f, double* h_grad,
+                                   int32_t* h_meta_i32) {
+    return objective_host(c, opts, h_ds, h_y, y_dtype, h_offsets, n_series, floor, cap_multiplier, h_theta, h_f, h_grad,
+                          h_meta_i32);
+}
+
+PB200_API int pb200_objective_regressors_host(pb200_ctx* c, const pb200_options* opts, const int64_t* h_ds, const void* h_y,
+                                              int32_t y_dtype, const int64_t* h_offsets, int64_t n_series, double floor,
+                                              double cap_multiplier, const double* h_reg, double* h_reg_scale,
+                                              const double* h_theta, double* h_f, double* h_grad, int32_t* h_meta_i32) {
+    return objective_host(c, opts, h_ds, h_y, y_dtype, h_offsets, n_series, floor, cap_multiplier, h_theta, h_f, h_grad,
+                          h_meta_i32, true, h_reg, h_reg_scale);
+}
+
+PB200_API int pb200_fit_regressors_device(pb200_ctx* c, const pb200_options* opts, const int64_t* d_ds, const void* d_y,
+                                          int32_t y_dtype, const int64_t* h_offsets, int64_t n_series, double floor,
+                                          double cap_multiplier, const double* d_cap, const double* d_reg, double* d_reg_scale,
+                                          double* d_params, double* d_tchange, int32_t* d_meta_i32, int64_t* d_meta_i64,
+                                          double* d_meta_f64) {
+    return fit_impl(c, opts, d_ds, d_y, y_dtype, h_offsets, n_series, floor, cap_multiplier, d_cap, nullptr, d_params,
+                    d_tchange, d_meta_i32, d_meta_i64, d_meta_f64, nullptr, nullptr, nullptr, 0, nullptr, nullptr, nullptr,
+                    true, d_reg, d_reg_scale);
+}
+
+PB200_API int pb200_fit_regressors_host(pb200_ctx* c, const pb200_options* opts, const int64_t* h_ds, const void* h_y,
+                                        int32_t y_dtype, const int64_t* h_offsets, int64_t n_series, double floor,
+                                        double cap_multiplier, const double* h_cap, const double* h_reg, double* h_reg_scale,
+                                        double* h_params, double* h_tchange, int32_t* h_meta_i32, int64_t* h_meta_i64,
+                                        double* h_meta_f64, double* h_trace, int32_t trace_cap) {
+    return fit_host(c, opts, h_ds, h_y, y_dtype, h_offsets, n_series, floor, cap_multiplier, h_cap, h_params, h_tchange,
+                    h_meta_i32, h_meta_i64, h_meta_f64, h_trace != nullptr && trace_cap > 0, h_trace, trace_cap, nullptr,
+                    nullptr, nullptr, nullptr, true, h_reg, h_reg_scale);
 }
 
 PB200_API int pb200_fit_host(pb200_ctx* c, const pb200_options* opts, const int64_t* h_ds, const void* h_y, int32_t y_dtype,
@@ -1076,9 +1259,10 @@ int predict_device(pb200_ctx* c, const pb200_options* opts, const double* d_para
                    const int32_t* d_meta_i32, const int64_t* d_meta_i64, const double* d_meta_f64, int64_t n_models,
                    const int64_t* d_future_ds, int32_t horizon, const double* d_floor, const double* d_cap, uint64_t seed,
                    double* d_yhat, double* d_yhat_lower, double* d_yhat_upper, int32_t* d_yhat_int, double* d_comp,
-                   double* d_tlo, double* d_thi, const SumOut* sums = nullptr, const QuantOut* quant = nullptr) {
+                   double* d_tlo, double* d_thi, const SumOut* sums = nullptr, const QuantOut* quant = nullptr,
+                   bool regs = false, const double* d_future_reg = nullptr, const double* d_reg_scale = nullptr) {
     if (!c) return fail(PB200_E_ARG, "ctx is null");
-    int rc = check_opts(opts);
+    int rc = check_opts(opts, regs);
     if (rc) return rc;
     if (n_models < 0 || horizon < 0 || n_models > (1LL << 30)) return fail(PB200_E_ARG, "sizes");
     if (sums && (rc = check_sum_args(opts, *sums))) return rc;
@@ -1089,6 +1273,9 @@ int predict_device(pb200_ctx* c, const pb200_options* opts, const double* d_para
         return fail(PB200_E_ARG, "null pointer");
     const bool mc = horizon > 0 && d_yhat_lower && d_yhat_upper && opts->uncertainty_samples > 0;
     if (mc && (rc = check_mc_opts(opts))) return rc;
+    pb200::RegSpec reg;
+    opts_reg(opts, &reg);
+    if (reg.R > 0 && horizon > 0 && (!d_future_reg || !d_reg_scale)) return fail(PB200_E_ARG, "null pointer (regressors / reg_scale)");
     pb200_layout L;
     pb200_get_layout(opts, &L);
     pb200::PredictArgs a;
@@ -1112,6 +1299,27 @@ int predict_device(pb200_ctx* c, const pb200_options* opts, const double* d_para
     a.yhat = d_yhat;
     a.trend = d_comp;
     a.yhat_int = d_yhat_int;
+    if (reg.R > 0) {
+        // the regressor instances: yhat and its interval (every other output is refused for these options by check_opts)
+        pb200::RegPredictArgs ra;
+        static_cast<pb200::PredictArgs&>(ra) = a;
+        ra.reg.future_reg = d_future_reg;
+        ra.reg.reg_scale = d_reg_scale;
+        ra.reg.R = reg.R;
+        if (horizon == 0) return PB200_OK;
+        dim3 grid((unsigned)n_models, (unsigned)std::min((horizon + 1023) / 1024, 64));
+        pb200::predict_kernel<false, false, true><<<grid, 256, 0, c->stream>>>(ra);
+        CK(cudaGetLastError());
+        c->launches++;
+        if (mc) {
+            rc = pb200::launch_mc_reg(c->stream, c->sms, a, ra.reg, opts->uncertainty_samples, opts->interval_width, seed,
+                                      d_yhat_lower, d_yhat_upper);
+            if (rc == -1) return fail(PB200_E_ARG, "uncertainty_samples / interval_width out of range");
+            if (rc) return fail(PB200_E_CUDA, "mc kernel launch", cudaGetLastError());
+            c->launches++;
+        }
+        return PB200_OK;
+    }
     if (horizon > 0) {
         // one CTA per (model, 1024 future points): the per-model prologue (parameters, the serial gamma recurrence) is paid
         // once for config #5's 672 periods instead of three times
@@ -1157,9 +1365,10 @@ int predict_host(pb200_ctx* c, const pb200_options* opts, const double* h_params
                  const int32_t* h_meta_i32, const int64_t* h_meta_i64, const double* h_meta_f64, int64_t n_models,
                  const int64_t* h_future_ds, int32_t horizon, const double* h_floor, const double* h_cap, uint64_t seed,
                  double* h_yhat, double* h_yhat_lower, double* h_yhat_upper, int32_t* h_yhat_int, double* h_comp,
-                 double* h_tlo, double* h_thi, const SumOut* sums = nullptr, const QuantOut* quant = nullptr) {
+                 double* h_tlo, double* h_thi, const SumOut* sums = nullptr, const QuantOut* quant = nullptr,
+                 bool regs = false, const double* h_future_reg = nullptr, const double* h_reg_scale = nullptr) {
     if (!c) return fail(PB200_E_ARG, "ctx is null");
-    int rc = check_opts(opts);
+    int rc = check_opts(opts, regs);
     if (rc) return rc;
     if (quant && (rc = check_quant_args(opts, *quant))) return rc;
     if (sums) {
@@ -1178,6 +1387,13 @@ int predict_host(pb200_ctx* c, const pb200_options* opts, const double* h_params
     const size_t N = (size_t)n_models, NH = N * (size_t)horizon;
     const bool mc = horizon > 0 && h_yhat_lower && h_yhat_upper && opts->uncertainty_samples > 0;
     if (mc && (rc = check_mc_opts(opts))) return rc;
+    pb200::RegSpec reg;
+    opts_reg(opts, &reg);
+    if (reg.R > 0) {
+        if (!h_future_reg || !h_reg_scale) return fail(PB200_E_ARG, "null pointer (regressors / reg_scale)");
+        CK(c->d_reg.reserve(NH * reg.R * 8));
+        CK(c->d_regsc.reserve(N * reg.R * 2 * 8));
+    }
     // the window outputs on the device: five 8-byte arrays [N * wmax], then win_points [N * wmax] and n_windows [N]
     const size_t NW = sums ? N * (size_t)sums->wmax : 0;
     SumOut dsum;
@@ -1227,12 +1443,17 @@ int predict_host(pb200_ctx* c, const pb200_options* opts, const double* h_params
     if (NH) CK(cudaMemcpyAsync(c->d_fut.p, h_future_ds, NH * 8, cudaMemcpyHostToDevice, st));
     CK(cudaMemcpyAsync(c->d_floor.p, h_floor, N * 8, cudaMemcpyHostToDevice, st));
     CK(cudaMemcpyAsync(c->d_cap.p, h_cap, N * 8, cudaMemcpyHostToDevice, st));
+    if (reg.R > 0) {
+        CK(cudaMemcpyAsync(c->d_reg.p, h_future_reg, NH * reg.R * 8, cudaMemcpyHostToDevice, st));
+        CK(cudaMemcpyAsync(c->d_regsc.p, h_reg_scale, N * reg.R * 2 * 8, cudaMemcpyHostToDevice, st));
+    }
     rc = predict_device(c, opts, (const double*)c->d_params.p, (const double*)c->d_tchange.p, (const int32_t*)c->d_mi32.p,
                         (const int64_t*)c->d_mi64.p, (const double*)c->d_mf64.p, n_models, (const int64_t*)c->d_fut.p,
                         horizon, (const double*)c->d_floor.p, (const double*)c->d_cap.p, seed, (double*)c->d_yhat.p,
                         mc ? (double*)c->d_lo.p : nullptr, mc ? (double*)c->d_hi.p : nullptr, (int32_t*)c->d_yint.p,
                         h_comp ? (double*)c->d_comp.p : nullptr, h_tlo ? (double*)c->d_tlo.p : nullptr,
-                        h_tlo ? (double*)c->d_thi.p : nullptr, sums ? &dsum : nullptr, quant ? &dquant : nullptr);
+                        h_tlo ? (double*)c->d_thi.p : nullptr, sums ? &dsum : nullptr, quant ? &dquant : nullptr, regs,
+                        reg.R > 0 ? (const double*)c->d_reg.p : nullptr, reg.R > 0 ? (const double*)c->d_regsc.p : nullptr);
     if (rc) return rc;
     if (sums) {
         CK(cudaMemcpyAsync(sums->win_start, dsum.win_start, NW * 8, cudaMemcpyDeviceToHost, st));
@@ -1278,6 +1499,28 @@ PB200_API int pb200_predict_host(pb200_ctx* c, const pb200_options* opts, const 
                        uint64_t seed, double* h_yhat, double* h_yhat_lower, double* h_yhat_upper, int32_t* h_yhat_int) {
     return predict_host(c, opts, h_params, h_tchange, h_meta_i32, h_meta_i64, h_meta_f64, n_models, h_future_ds, horizon,
                         h_floor, h_cap, seed, h_yhat, h_yhat_lower, h_yhat_upper, h_yhat_int, nullptr, nullptr, nullptr);
+}
+
+PB200_API int pb200_predict_regressors_device(pb200_ctx* c, const pb200_options* opts, const double* d_params,
+                         const double* d_tchange, const int32_t* d_meta_i32, const int64_t* d_meta_i64,
+                         const double* d_meta_f64, int64_t n_models, const int64_t* d_future_ds, int32_t horizon,
+                         const double* d_floor, const double* d_cap, uint64_t seed, const double* d_future_reg,
+                         const double* d_reg_scale, double* d_yhat, double* d_yhat_lower, double* d_yhat_upper,
+                         int32_t* d_yhat_int) {
+    return predict_device(c, opts, d_params, d_tchange, d_meta_i32, d_meta_i64, d_meta_f64, n_models, d_future_ds, horizon,
+                          d_floor, d_cap, seed, d_yhat, d_yhat_lower, d_yhat_upper, d_yhat_int, nullptr, nullptr, nullptr,
+                          nullptr, nullptr, true, d_future_reg, d_reg_scale);
+}
+
+PB200_API int pb200_predict_regressors_host(pb200_ctx* c, const pb200_options* opts, const double* h_params,
+                       const double* h_tchange, const int32_t* h_meta_i32, const int64_t* h_meta_i64,
+                       const double* h_meta_f64, int64_t n_models, const int64_t* h_future_ds, int32_t horizon,
+                       const double* h_floor, const double* h_cap, uint64_t seed, const double* h_future_reg,
+                       const double* h_reg_scale, double* h_yhat, double* h_yhat_lower, double* h_yhat_upper,
+                       int32_t* h_yhat_int) {
+    return predict_host(c, opts, h_params, h_tchange, h_meta_i32, h_meta_i64, h_meta_f64, n_models, h_future_ds, horizon,
+                        h_floor, h_cap, seed, h_yhat, h_yhat_lower, h_yhat_upper, h_yhat_int, nullptr, nullptr, nullptr,
+                        nullptr, nullptr, true, h_future_reg, h_reg_scale);
 }
 
 PB200_API int pb200_predict_components_device(pb200_ctx* c, const pb200_options* opts, const double* d_params,

@@ -7,6 +7,9 @@
 // The trend and sigma terms, Stan's L-BFGS (line search, update, stop rules) and the trajectory hook are the routines of
 // fit_kernel.cuh, called as they are: eval_setup / eval_finalize see a model without Fourier columns (K = 0) at a
 // shadow of the point whose beta is zero, and this file adds the beta terms with a prior scale per column.
+// The REG instances (DESIGN §19) add the model's extra regressors as R more columns after the seasonal ones.
+#include <type_traits>
+
 #include "fit_kernel.cuh"
 #include "launch.h"
 #include "seas_table.cuh"
@@ -32,9 +35,26 @@ __host__ __device__ inline size_t fit_table_smem_bytes(int ppad) {
 
 __device__ __forceinline__ TabExt& tab_ext() { return *reinterpret_cast<TabExt*>(smem_ring<1>(smem_hdr<1>().ppad)); }
 
+// behind TabExt in the instances with regressors (DESIGN §19).  Their columns follow the seasonal ones in TabExt's beta,
+// isig2 and gs (K_seas + R <= SEAS_KMAX); their standardised values are staged as ceil(R / 2) double2 planes after the
+// series' active seasonal planes, regressor r in component r & 1 of plane r >> 1
+struct RegExt {
+    int R;
+};
+static_assert(sizeof(TabExt) % 8 == 0, "RegExt follows TabExt");
+
+__device__ __forceinline__ RegExt& reg_ext() { return *reinterpret_cast<RegExt*>(&tab_ext() + 1); }
+
+// regressor r of the point at pt (its double2 of plane 0), in a slice whose active seasonal planes are ne
+template <class D2>
+__device__ __forceinline__ auto& reg_at(D2* pt, const int ne, const int Tp, const int r) {
+    using D = std::conditional_t<std::is_const_v<D2>, const double, double>;
+    return reinterpret_cast<D*>(pt + (size_t)(ne + 1 + (r >> 1)) * Tp)[r & 1];
+}
+
 // objective + gradient pass over lane's points [i0, i1): the trend partial sums as point_pass, the Fourier columns of
 // every active seasonality twice per point (for the dot product, then for the gradient once the residual is known)
-template <bool LOGI>
+template <bool LOGI, bool REG>
 PB200_EVAL_FN void table_point_pass(const int lane, const int i0, const int i1, const int j0) {
     Smem<1>& sm = smem_hdr<1>();
     TabExt& ex = tab_ext();
@@ -78,6 +98,11 @@ PB200_EVAL_FN void table_point_pass(const int lane, const int i0, const int i1, 
                     sp = sn; cp = cn; sn = s2; cn = cc;
                 }
             }
+            if constexpr (REG) {
+                const int R = reg_ext().R;
+#pragma unroll 1
+                for (int r = 0; r < R; ++r) dot = fma(ex.beta[col + r], reg_at(pt, ne, Tp, r), dot);
+            }
         }
         double g, sig = 0.0;
         const double tm = ty.x - mcj;
@@ -106,6 +131,11 @@ PB200_EVAL_FN void table_point_pass(const int lane, const int i0, const int i1, 
                     const double s2 = fma(c2, sn, -sp), cc = fma(c2, cn, -cp);
                     sp = sn; cp = cn; sn = s2; cn = cc;
                 }
+            }
+            if constexpr (REG) {
+                const int R = reg_ext().R;
+#pragma unroll 1
+                for (int r = 0; r < R; ++r) gs[(col + r) * GS_STRIDE] = fma(cb, reg_at(pt, ne, Tp, r), gs[(col + r) * GS_STRIDE]);
             }
         }
         const double qv = r * opm;
@@ -143,7 +173,7 @@ PB200_EVAL_FN void table_point_pass(const int lane, const int i0, const int i1, 
 }
 
 // one objective + gradient evaluation at vector xv -> gv, f -> *f_out; returns err (uniform)
-template <bool LOGI>
+template <bool LOGI, bool REG>
 __device__ __forceinline__ int table_eval(const double* xv, double* gv, double* f_out, const int lane, const int i0,
                                           const int i1, const int j0) {
     Smem<1>& sm = smem_hdr<1>();
@@ -156,7 +186,7 @@ __device__ __forceinline__ int table_eval(const double* xv, double* gv, double* 
     __syncwarp();
     eval_setup<1, LOGI>(ex.xs, lane, 0);
     if (lane == 0) sm.ls.nevals += 1;
-    table_point_pass<LOGI>(lane, i0, i1, j0);
+    table_point_pass<LOGI, REG>(lane, i0, i1, j0);
     double f0;
     int bad = eval_finalize<1, LOGI>(ex.xs, gv, lane, 0, &f0);
     // the beta terms: gradient scale * X'c + beta / sigma_c^2, prior sum of beta^2 / (2 sigma_c^2)
@@ -185,8 +215,12 @@ __device__ __forceinline__ int table_eval(const double* xv, double* gv, double* 
     return bad;
 }
 
-template <bool LOGI>
-__global__ void __launch_bounds__(32) fit_table_kernel(const TableFitArgs a) {
+template <bool REG>
+using TableFitArgsT = std::conditional_t<REG, RegTableFitArgs, TableFitArgs>;
+
+// REG: the model's regressors (RegTableFitArgs) as R more columns; <LOGI, false> is the table class without them
+template <bool LOGI, bool REG>
+__global__ void __launch_bounds__(32) fit_table_kernel(const TableFitArgsT<REG> a) {
     const int lane = threadIdx.x;
     Smem<1>& sm = smem_hdr<1>();
     TabExt& ex = *reinterpret_cast<TabExt*>(smem_ring<1>(a.ppad));
@@ -215,7 +249,9 @@ __global__ void __launch_bounds__(32) fit_table_kernel(const TableFitArgs a) {
         const int chunk = (T + 31) / 32;
         const int nact = (T + chunk - 1) / chunk;
         const double cap_s = LOGI ? (capv - fl) / y_scale : 0.0;
-        const int K = tab_k(a.tab, mask), KE = K > 0 ? K : 1;
+        int Kc = tab_k(a.tab, mask);
+        if constexpr (REG) Kc += a.spec.R;
+        const int K = Kc, KE = K > 0 ? K : 1;
         if (lane == 0) {
             sm.T = T; sm.S = S; sm.chunk = chunk; sm.nact = nact;
             sm.cap_s = cap_s;
@@ -229,6 +265,10 @@ __global__ void __launch_bounds__(32) fit_table_kernel(const TableFitArgs a) {
                 ex.order[ne] = a.tab.order[e];
                 for (int q = 0; q < 2 * a.tab.order[e]; ++q) ex.isig2[col++] = a.tab.inv_sig2[e];
                 ++ne;
+            }
+            if constexpr (REG) {
+                for (int r = 0; r < a.spec.R; ++r) ex.isig2[col++] = a.spec.inv_sig2[r];
+                reg_ext().R = a.spec.R;
             }
             if (K == 0) ex.isig2[0] = 1.0;      // fbprophet's zero column has prior scale 1
             ex.ne = ne;
@@ -250,6 +290,11 @@ __global__ void __launch_bounds__(32) fit_table_kernel(const TableFitArgs a) {
                 double s_, c_;
                 sincos(TWO_PI_FL * tau_d / ex.period[e], &s_, &c_);
                 TYp[(size_t)(e + 1) * a.Tp + ph] = make_double2(s_, c_);
+            }
+            if constexpr (REG) {
+                const double* sc = a.reg_scale + (size_t)sidx * a.spec.R * 2;
+                for (int r = 0; r < a.spec.R; ++r)
+                    reg_at(TYp + ph, ex.ne, a.Tp, r) = reg_value(a.reg[(size_t)r * a.n_rows + off + i], sc[2 * r], sc[2 * r + 1]);
             }
         }
         // ---- changepoints (Prophet.set_changepoints) and segment boundaries ----
@@ -320,14 +365,14 @@ __global__ void __launch_bounds__(32) fit_table_kernel(const TableFitArgs a) {
         }
         int status = st0;
         if (a.grad_out) {
-            const int err = table_eval<LOGI>(vecp<1>(0), vecp<1>(1), &ls.fk, lane, i0, i1, j0);
+            const int err = table_eval<LOGI, REG>(vecp<1>(0), vecp<1>(1), &ls.fk, lane, i0, i1, j0);
             status = err ? PB200_ST_INIT_ERROR : PB200_ST_SUCCESS;
             double* go = a.grad_out + (size_t)sidx * a.pstride;
 #pragma unroll 1
             for (int q = lane; q < a.pstride; q += 32) go[q] = q < P ? g[q] : 0.0;
         } else if (status != PB200_ST_CONST_LINEAR) {
             // ======== stan::optimization::BFGSMinimizer<..., LBFGSUpdate>, as fit_kernel ========
-            int err = table_eval<LOGI>(vecp<1>(0), vecp<1>(1), &ls.fk, lane, i0, i1, j0);
+            int err = table_eval<LOGI, REG>(vecp<1>(0), vecp<1>(1), &ls.fk, lane, i0, i1, j0);
             if (err) {
                 status = PB200_ST_INIT_ERROR;
             } else {
@@ -336,7 +381,7 @@ __global__ void __launch_bounds__(32) fit_table_kernel(const TableFitArgs a) {
                 __syncwarp();
                 ls_begin<1>(lane, P, a.o.init_alpha);
                 for (;;) {
-                    err = table_eval<LOGI>(vecp<1>(ls.ixt), vecp<1>(ls.igt), &ls.ft, lane, i0, i1, j0);
+                    err = table_eval<LOGI, REG>(vecp<1>(ls.ixt), vecp<1>(ls.igt), &ls.ft, lane, i0, i1, j0);
                     const int act = ls_step<1>(lane, P, err);
                     if (act == ACT_EVAL) continue;
                     if (act == ACT_FAIL) {
@@ -395,8 +440,9 @@ __global__ void __launch_bounds__(32) fit_table_kernel(const TableFitArgs a) {
     }
 }
 
-cudaError_t launch_fit_table(int logi, const TableFitArgs& a, int grid, size_t smem, cudaStream_t st, int* occ) {
-    auto kern = logi ? fit_table_kernel<true> : fit_table_kernel<false>;
+template <bool REG>
+static cudaError_t launch_table_inst(int logi, const TableFitArgsT<REG>& a, int grid, size_t smem, cudaStream_t st, int* occ) {
+    auto kern = logi ? fit_table_kernel<true, REG> : fit_table_kernel<false, REG>;
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return e;
     if (occ) return cudaOccupancyMaxActiveBlocksPerMultiprocessor(occ, kern, 32, smem);
@@ -404,6 +450,15 @@ cudaError_t launch_fit_table(int logi, const TableFitArgs& a, int grid, size_t s
     return cudaGetLastError();
 }
 
+cudaError_t launch_fit_table(int logi, const TableFitArgs& a, int grid, size_t smem, cudaStream_t st, int* occ) {
+    return launch_table_inst<false>(logi, a, grid, smem, st, occ);
+}
+
+cudaError_t launch_fit_table_reg(int logi, const RegTableFitArgs& a, int grid, size_t smem, cudaStream_t st, int* occ) {
+    return launch_table_inst<true>(logi, a, grid, smem, st, occ);
+}
+
 size_t fit_table_smem(int ppad) { return fit_table_smem_bytes(ppad); }
+size_t fit_table_reg_smem(int ppad) { return fit_table_smem_bytes(ppad) + sizeof(RegExt); }
 
 }  // namespace pb200

@@ -22,4 +22,8 @@ namespace pb200 {
 struct TableFitArgs;
 cudaError_t launch_fit_table(int logi, const TableFitArgs& a, int grid, size_t smem, cudaStream_t st, int* occ);
 size_t fit_table_smem(int ppad);
+// ... with regressors (DESIGN §19): fit_table_reg_smem(ppad) bytes of dynamic shared memory
+struct RegTableFitArgs;
+cudaError_t launch_fit_table_reg(int logi, const RegTableFitArgs& a, int grid, size_t smem, cudaStream_t st, int* occ);
+size_t fit_table_reg_smem(int ppad);
 }  // namespace pb200

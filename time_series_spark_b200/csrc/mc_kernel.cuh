@@ -97,8 +97,12 @@ struct McArgs {
 struct RaggedMcArgs : McArgs {
     const long long* offsets;   // [n_models + 1]
 };
-template <bool RAGGED>
-using McArgsT = std::conditional_t<RAGGED, RaggedMcArgs, McArgs>;
+// mc_kernel's instance with regressors (pb200_predict_regressors_*, DESIGN §19).  Derived, as RaggedMcArgs
+struct RegMcArgs : McArgs {
+    RegFrame reg;
+};
+template <bool RAGGED, bool REGR = false>
+using McArgsT = std::conditional_t<RAGGED, RaggedMcArgs, std::conditional_t<REGR, RegMcArgs, McArgs>>;
 
 __device__ __forceinline__ uint64_t splitmix64(uint64_t z) {
     z += 0x9E3779B97F4A7C15ull;
@@ -403,8 +407,10 @@ __device__ __forceinline__ double draw_point(DrawState& d, const ModelSm& ms, co
 // draw across tiles; Tmax is over the whole frame), so are their bounds.
 // RAGGED: model i's frame is its own rows [offsets[i], offsets[i + 1]) (RaggedMcArgs), walked as a frame of that length:
 // the same Tmax, key and counters as a fixed frame holding those rows first, so the same draws at those points.
-template <bool LOGI, bool TREND, bool RAGGED = false>
-__global__ void __launch_bounds__(MC_THREADS, 1) mc_kernel(const McArgsT<RAGGED> a) {
+// REGR: the models' regressors (RegMcArgs) added to the seasonal term of every draw, as predict_kernel adds them to yhat.
+template <bool LOGI, bool TREND, bool RAGGED = false, bool REGR = false>
+__global__ void __launch_bounds__(MC_THREADS, 1) mc_kernel(const McArgsT<RAGGED, REGR> a) {
+    static_assert(!REGR || (!TREND && !RAGGED), "the regressor instance is the fixed-frame interval");
     constexpr int TILE = TREND ? MC_TILE / 2 : MC_TILE;
     extern __shared__ __align__(16) unsigned char mc_smem[];
     double* rows = (double*)mc_smem;                       // [MC_TILE][MC_NP]
@@ -428,7 +434,9 @@ __global__ void __launch_bounds__(MC_THREADS, 1) mc_kernel(const McArgsT<RAGGED>
         load_model(ms, a.p, model, tid, MC_THREADS);
         const size_t base = frame_base<RAGGED>(a, model, H);
         const int HM = frame_len<RAGGED>(a, model, H);     // the model's points
-        if (ms.status < 0) {
+        bool failed = ms.status < 0;
+        if constexpr (REGR) failed = !reg_finite(a.reg, NH, model, H, tid, MC_THREADS) || failed;
+        if (failed) {
             for (int l = 0; l < lv.nlev; ++l)
                 for (int h = tid; h < HM; h += MC_THREADS) {
                     out(l, base + h, false) = NAN;
@@ -446,7 +454,9 @@ __global__ void __launch_bounds__(MC_THREADS, 1) mc_kernel(const McArgsT<RAGGED>
             if (tid < np) {
                 const long long dsv = a.p.future_ds[base + h0 + tid];
                 tt[tid] = (double)(dsv - ms.start) / ms.t_scale;
-                seas[tid] = ms.K > 0 ? seasonal_term(ms, dsv) : 0.0;
+                double sv = ms.K > 0 ? seasonal_term(ms, dsv) : 0.0;
+                if constexpr (REGR) sv += reg_term(a.reg, NH, ms, model, base + h0 + tid);
+                seas[tid] = sv;
             }
             __syncthreads();
 #pragma unroll
@@ -636,12 +646,12 @@ __global__ void __launch_bounds__(MC_THREADS, 1) mc_sum_kernel(const McSumArgsT<
     }
 }
 
-template <bool LOGI, bool TREND, bool RAGGED = false>
-cudaError_t launch_mc_inst(cudaStream_t st, int grid, size_t smem, const McArgsT<RAGGED>& a) {
-    const cudaError_t e = cudaFuncSetAttribute(mc_kernel<LOGI, TREND, RAGGED>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                               (int)smem);
+template <bool LOGI, bool TREND, bool RAGGED = false, bool REGR = false>
+cudaError_t launch_mc_inst(cudaStream_t st, int grid, size_t smem, const McArgsT<RAGGED, REGR>& a) {
+    const cudaError_t e = cudaFuncSetAttribute(mc_kernel<LOGI, TREND, RAGGED, REGR>,
+                                               cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return e;
-    mc_kernel<LOGI, TREND, RAGGED><<<grid, MC_THREADS, smem, st>>>(a);
+    mc_kernel<LOGI, TREND, RAGGED, REGR><<<grid, MC_THREADS, smem, st>>>(a);
     return cudaGetLastError();
 }
 
@@ -726,6 +736,20 @@ inline int launch_mc_ragged(cudaStream_t st, int sms, const PredictArgs& p, cons
     const int grid = p.n_models < sms ? p.n_models : sms;
     const cudaError_t e = p.growth == PB200_GROWTH_LOGISTIC ? launch_mc_inst<true, false, true>(st, grid, MC_SMEM, a)
                                                             : launch_mc_inst<false, false, true>(st, grid, MC_SMEM, a);
+    return e == cudaSuccess ? 0 : 1;
+}
+
+// the bounds of mc_kernel's instance with regressors over p's fixed frame.  Returns as launch_mc
+inline int launch_mc_reg(cudaStream_t st, int sms, const PredictArgs& p, const RegFrame& reg, int n_samples, double width,
+                         uint64_t seed, double* lower, double* upper) {
+    RegMcArgs a;
+    if (!mc_args(a, p, n_samples, width, seed)) return -1;
+    a.lower = lower;
+    a.upper = upper;
+    a.reg = reg;
+    const int grid = p.n_models < sms ? p.n_models : sms;
+    const cudaError_t e = p.growth == PB200_GROWTH_LOGISTIC ? launch_mc_inst<true, false, false, true>(st, grid, MC_SMEM, a)
+                                                            : launch_mc_inst<false, false, false, true>(st, grid, MC_SMEM, a);
     return e == cudaSuccess ? 0 : 1;
 }
 

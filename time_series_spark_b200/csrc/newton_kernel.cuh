@@ -18,6 +18,7 @@
 // ... so every sum has a fixed order); the eigen-decomposition is cyclic Jacobi by warp 0.
 #pragma once
 #include "fit_kernel.cuh"
+#include "regressors.cuh"
 
 namespace pb200 {
 namespace nw {
@@ -44,6 +45,12 @@ struct NewtonArgs {
     const double* x0;        // warm start points (PrepArgs::warm_x, k = NaN: cold); null: every series from stan_init
     FitOptsDev o;
     SeasTab tab;             // the models' seasonality table (n = 0: the compiled-in orders); mask = the table mask
+    // the models' regressors (DESIGN §19; reg.R = 0: none): their columns follow the active seasonal ones, standardised
+    // with the fit's reg_scale
+    RegSpec reg;
+    const double* reg_x;     // [R][n_rows]
+    const double* reg_scale; // [n_series][R][2]
+    long long n_rows;
 };
 
 struct WarpScratch {     // per warp
@@ -63,6 +70,7 @@ struct Series {          // per CTA
     double f, f0, f1, last;
     int it, nev, status, moved, stop, err;
     double isig[SEAS_KMAX];      // a table model's 1 / prior_scale^2 per packed column
+    double rsc[2 * REG_MAX];     // the series' (mu, std) per regressor
 };
 
 inline size_t newton_smem_bytes(int P) {
@@ -71,7 +79,8 @@ inline size_t newton_smem_bytes(int P) {
 
 // objective + gradient at ws.x -> ws.g, ws.f, ws.err (Stan ModelAdaptor error convention: nonzero = reject)
 __device__ __noinline__ void nw_eval(const NewtonArgs& a, const Series& sr, WarpScratch& ws, const int lane) {
-    const int S = sr.S, T = sr.T, Kreal = sr.mask ? sr.K : 0;
+    const int R = a.reg.R;
+    const int S = sr.S, T = sr.T, Kreal = (sr.mask || R) ? sr.K : 0;
     const double* th = ws.x;
     int bad = 0;
     for (int q = lane; q < sr.P; q += 32) if (!isfinite(th[q])) bad = 1;
@@ -101,7 +110,7 @@ __device__ __noinline__ void nw_eval(const NewtonArgs& a, const Series& sr, Warp
     int j = 0;
     for (int s = 0; s < S; ++s) j += sr.bidx[s] < i0 ? 1 : 0;
     const int j0 = j;
-    const bool tab = a.tab.n > 0;
+    const bool tab = a.tab.n > 0 || R > 0;
     double gb[SEAS_KMAX];      // fixed layout: yearly 0..19, weekly 20..25, daily 26..33; a table model: its packed columns
 #pragma unroll
     for (int q = 0; q < SEAS_KMAX; ++q) gb[q] = 0.0;
@@ -134,6 +143,8 @@ __device__ __noinline__ void nw_eval(const NewtonArgs& a, const Series& sr, Warp
                     sp = sn; cp = cn; sn = s2; cn = cc;
                 }
             }
+            for (int r = 0; r < R; ++r)
+                Xt[col + r] = reg_value(a.reg_x[(size_t)r * a.n_rows + sr.off + i], sr.rsc[2 * r], sr.rsc[2 * r + 1]);
             for (int q = 0; q < Kreal; ++q) dot = fma(Xt[q], beta[q], dot);
         }
         if (!tab && (sr.mask & 1)) {
@@ -344,12 +355,18 @@ __global__ void __launch_bounds__(32 * NW_WARPS, 1) newton_kernel(const NewtonAr
         if (tid == 0) {
             sr.T = mi[0]; sr.S = mi[1]; sr.ncp = mi[2]; sr.mask = mi[3];
             sr.K = sr.mask ? ((sr.mask & 1) ? 20 : 0) + ((sr.mask & 2) ? 6 : 0) + ((sr.mask & 4) ? 8 : 0) : 1;
-            if (a.tab.n > 0) {
-                const int K = tab_k(a.tab, sr.mask);
+            if (a.tab.n > 0 || a.reg.R > 0) {
+                const int K = tab_k(a.tab, sr.mask) + a.reg.R;
                 sr.K = K > 0 ? K : 1;
-                for (int e = 0, c = 0; e < a.tab.n; ++e)
+                int c = 0;
+                for (int e = 0; e < a.tab.n; ++e)
                     if ((sr.mask >> e) & 1)
                         for (int q = 0; q < 2 * a.tab.order[e]; ++q) sr.isig[c++] = a.tab.inv_sig2[e];
+                for (int r = 0; r < a.reg.R; ++r) {
+                    sr.isig[c++] = a.reg.inv_sig2[r];
+                    sr.rsc[2 * r] = a.reg_scale[((size_t)sidx * a.reg.R + r) * 2];
+                    sr.rsc[2 * r + 1] = a.reg_scale[((size_t)sidx * a.reg.R + r) * 2 + 1];
+                }
             }
             sr.P = sr.S + sr.K + 3;
             sr.logistic = a.o.growth == PB200_GROWTH_LOGISTIC;

@@ -16,6 +16,7 @@
 #include <type_traits>
 
 #include "../../include/prophet_b200.h"
+#include "regressors.cuh"
 #include "seas_table.cuh"
 
 namespace pb200 {
@@ -47,8 +48,18 @@ struct PredictArgs {
 struct RaggedPredictArgs : PredictArgs {
     const long long* offsets;   // [n_models + 1]
 };
-template <bool RAGGED>
-using PredictArgsT = std::conditional_t<RAGGED, RaggedPredictArgs, PredictArgs>;
+// The models' future regressor values and the fit's standardisation (pb200_predict_regressors_*, DESIGN §19), which the
+// regressor instances of predict_kernel and mc_kernel take in a derived argument type, for the same reason.
+struct RegFrame {
+    const double* future_reg;    // [R][n_models * horizon], aligned with future_ds
+    const double* reg_scale;     // [n_models][R][2] (mu, std)
+    int R;
+};
+struct RegPredictArgs : PredictArgs {
+    RegFrame reg;
+};
+template <bool RAGGED, bool REGR = false>
+using PredictArgsT = std::conditional_t<RAGGED, RaggedPredictArgs, std::conditional_t<REGR, RegPredictArgs, PredictArgs>>;
 
 constexpr double PI_FL = 3.141592653589793;
 
@@ -193,11 +204,36 @@ __device__ __forceinline__ double seasonal_parts(const ModelSm& ms, const long l
     return acc;
 }
 
+// sum_r beta_r (x_r - mu_r) / std_r at row o of the frame (NH rows per plane): the regressors' betas follow the model's
+// seasonal ones.  predict_kernel and mc_kernel add it to the seasonal term
+__device__ __forceinline__ double reg_term(const RegFrame& a, const size_t NH, const ModelSm& ms, const int model,
+                                           const size_t o) {
+    const double* sc = a.reg_scale + (size_t)model * a.R * 2;
+    double acc = 0.0;
+    for (int r = 0; r < a.R; ++r)
+        acc = fma(ms.beta[ms.K + r], reg_value(a.future_reg[(size_t)r * NH + o], sc[2 * r], sc[2 * r + 1]), acc);
+    return acc;
+}
+
+// whether every future regressor value of the model's H rows is finite; every thread of the CTA calls it.  A model with
+// one that is not gets the rows of a failed model, so that no NaN reaches yhat_int or the interval selection
+__device__ __forceinline__ bool reg_finite(const RegFrame& a, const size_t NH, const int model, const int H,
+                                           const int tid, const int nt) {
+    const size_t base = (size_t)model * H;
+    int bad = 0;
+    for (int r = 0; r < a.R; ++r)
+        for (int h = tid; h < H; h += nt)
+            if (!isfinite(a.future_reg[(size_t)r * NH + base + h])) bad = 1;
+    return !__syncthreads_or(bad);
+}
+
 // COMP: also write fbprophet's component columns -- planes PB200_COMP_* of a.trend, each [n_models * horizon].
 // RAGGED: model i's own rows [offsets[i], offsets[i + 1]) (RaggedPredictArgs); yhat only (no yhat_int, no trend).  A CTA
 // whose first point lies past its model's rows leaves before the model's prologue.
-template <bool COMP, bool RAGGED = false>
-__global__ void __launch_bounds__(256) predict_kernel(const PredictArgsT<RAGGED> a) {
+// REGR: the models' regressors (RegPredictArgs) added to the seasonal term; yhat, yhat_int and the trend plane only.
+template <bool COMP, bool RAGGED = false, bool REGR = false>
+__global__ void __launch_bounds__(256) predict_kernel(const PredictArgsT<RAGGED, REGR> a) {
+    static_assert(!REGR || (!COMP && !RAGGED), "the regressor instance is the fixed-frame forecast");
     __shared__ ModelSm ms;
     const int model = blockIdx.x;
     const int tid = threadIdx.x;
@@ -209,7 +245,9 @@ __global__ void __launch_bounds__(256) predict_kernel(const PredictArgsT<RAGGED>
         if ((int)(blockIdx.y * blockDim.x) >= H) return;
     }
     load_model(ms, a, model, tid, blockDim.x);
-    const bool ok = ms.status >= 0;
+    bool okm = ms.status >= 0;
+    if constexpr (REGR) okm = reg_finite(a.reg, (size_t)a.n_models * a.horizon, model, a.horizon, tid, blockDim.x) && okm;
+    const bool ok = okm;
     const int S = ms.S;
     const size_t plane = (size_t)a.n_models * a.horizon;
     for (int h = blockIdx.y * blockDim.x + tid; h < H; h += gridDim.y * blockDim.x) {
@@ -242,6 +280,7 @@ __global__ void __launch_bounds__(256) predict_kernel(const PredictArgsT<RAGGED>
         double sd, cy = 0.0, cw = 0.0, cd = 0.0;
         if (COMP) sd = ms.K > 0 ? seasonal_parts(ms, d, &cy, &cw, &cd) : 0.0;
         else sd = ms.K > 0 ? seasonal_term(ms, d) : 0.0;
+        if constexpr (REGR) sd += reg_term(a.reg, plane, ms, model, o);
         // the expression of predict_kernel<false>, so that yhat keeps its bits.  In additive mode the compiler fuses it
         // into fma(sd, y_scale, trend): the product is not rounded on its own, while the additive_terms plane holds it
         // rounded (fbprophet's value), so yhat and trend + additive_terms may differ by that one rounding (DESIGN §12)
