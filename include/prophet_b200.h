@@ -774,6 +774,53 @@ PB200_API int pb200_predict_regressors_host(pb200_ctx* ctx, const pb200_options*
                        double* h_yhat, double* h_yhat_lower, double* h_yhat_upper,
                        int32_t* h_yhat_int);
 
+/*
+ * The regressors' future values of every model's forecast grid, joined on the device (DESIGN §20).  The table: n_rows
+ * rows packed by group, group g owning rows [d_tab_offsets[g], d_tab_offsets[g + 1]) of d_tab_ds (int64 ns, ascending
+ * within a group) and of each plane of d_tab_reg (double [n_regressors][n_rows]).  d_model_group [n_models] (int64) is
+ * each model's group, -1 for none; d_future_ds [n_models][horizon] its grid.  For every grid point the row of the
+ * model's group with exactly its timestamp gives the point's values in d_future_reg (double [n_regressors][n_models *
+ * horizon], the layout pb200_predict_regressors_* reads); a point without one gets NaN.  d_missing [n_models] (int32)
+ * receives the model's points without a row, d_first_missing [n_models] (int64) the timestamp of the first of them
+ * (INT64_MIN when there is none).  Rows that are no grid point are ignored.  The group's timestamps must be distinct:
+ * with a repeated one, which of its rows is taken is not specified.  One warp per model, no atomics.
+ */
+PB200_API int pb200_join_future_regressors_device(pb200_ctx* ctx, const int64_t* d_tab_ds, const int64_t* d_tab_offsets,
+                                                  const double* d_tab_reg, int64_t n_rows, int32_t n_regressors,
+                                                  const int64_t* d_model_group, const int64_t* d_future_ds,
+                                                  int64_t n_models, int32_t horizon, double* d_future_reg,
+                                                  int32_t* d_missing, int64_t* d_first_missing);
+
+/*
+ * The backtest with regressors (DESIGN §20), fbprophet 0.5's cross_validation: the cutoff fits take the full history's
+ * standardised values z = (x - mu_full) / std_full and keep the full model's (mu_full, std_full) where they do not
+ * standardise (prophet_copy copies extra_regressors; initialize_scales overwrites mu / std only where it standardises).
+ *   pb200_regressor_scales_device      reg_scale_kernel alone over full histories (h_offsets as pb200_fit_device's):
+ *                                      d_reg_scale [n_series][R][2] (mu, std) as pb200_fit_regressors_device gives
+ *                                      them, d_bad [n_series] (uint8) 1 where a value is not finite.
+ *   pb200_cv_gather_regressors_device  beside pb200_cv_gather_device, for the same entries: z of each truncated history
+ *                                      as d_reg_fit [R][d_fit_off[n]] and of each held-out window as d_reg_future
+ *                                      [R][n * hmax] (pb200_predict_regressors_*'s layout), short windows padded with
+ *                                      0.0; d_reg_scale_full [n_series][R][2].
+ *   pb200_fit_regressors_copy_device   pb200_fit_regressors_device whose regressors keep d_reg_scale_copy
+ *                                      [n_series][R][2] where they are not standardised, instead of (0, 1).
+ */
+PB200_API int pb200_regressor_scales_device(pb200_ctx* ctx, const pb200_options* opts, const double* d_reg,
+                                            const int64_t* h_offsets, int64_t n_series, double* d_reg_scale,
+                                            uint8_t* d_bad);
+PB200_API int pb200_cv_gather_regressors_device(pb200_ctx* ctx, const double* d_reg, int64_t n_rows, int32_t n_regressors,
+                                                const double* d_reg_scale_full, const int64_t* d_offsets,
+                                                const int32_t* d_pair_series, const int64_t* d_hist_end,
+                                                const int64_t* d_win_end, const int64_t* d_pairs, int64_t n,
+                                                const int64_t* d_fit_off, int32_t hmax, double* d_reg_fit,
+                                                double* d_reg_future);
+PB200_API int pb200_fit_regressors_copy_device(pb200_ctx* ctx, const pb200_options* opts, const int64_t* d_ds,
+                                               const void* d_y, int32_t y_dtype, const int64_t* h_offsets,
+                                               int64_t n_series, double floor, double cap_multiplier, const double* d_cap,
+                                               const double* d_reg, const double* d_reg_scale_copy, double* d_reg_scale,
+                                               double* d_params, double* d_tchange, int32_t* d_meta_i32,
+                                               int64_t* d_meta_i64, double* d_meta_f64);
+
 #ifdef __cplusplus
 }
 #endif

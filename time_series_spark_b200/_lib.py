@@ -96,6 +96,8 @@ EXPORTS = [
     "pb200_predict_period_sums_device", "pb200_predict_period_sums_host", "pb200_period_host",
     "pb200_last_fit_table_count", "pb200_component_count", "pb200_fit_regressors_device", "pb200_fit_regressors_host",
     "pb200_objective_regressors_host", "pb200_predict_regressors_device", "pb200_predict_regressors_host",
+    "pb200_join_future_regressors_device", "pb200_regressor_scales_device", "pb200_cv_gather_regressors_device",
+    "pb200_fit_regressors_copy_device",
 ]
 CV_ERR_HORIZON, CV_ERR_INITIAL, CV_ERR_FEW = 1, 2, 4
 
@@ -195,6 +197,14 @@ def load() -> C.CDLL:
     lib.pb200_predict_regressors_device.restype = C.c_int
     lib.pb200_predict_regressors_host.argtypes = pred_args[:13] + [vp, vp] + pred_args[13:]
     lib.pb200_predict_regressors_host.restype = C.c_int
+    lib.pb200_join_future_regressors_device.argtypes = [vp, vp, vp, vp, i64, i32, vp, vp, i64, i32, vp, vp, vp]
+    lib.pb200_join_future_regressors_device.restype = C.c_int
+    lib.pb200_regressor_scales_device.argtypes = [vp, OP, vp, vp, i64, vp, vp]
+    lib.pb200_regressor_scales_device.restype = C.c_int
+    lib.pb200_cv_gather_regressors_device.argtypes = [vp, vp, i64, i32, vp, vp, vp, vp, vp, vp, i64, vp, i32, vp, vp]
+    lib.pb200_cv_gather_regressors_device.restype = C.c_int
+    lib.pb200_fit_regressors_copy_device.argtypes = fit_args[:10] + [vp, vp, vp] + fit_args[10:]
+    lib.pb200_fit_regressors_copy_device.restype = C.c_int
     lib.pb200_fit_trace_host.argtypes = [vp, OP, vp, vp, i32, vp, i64, dbl, dbl, vp, vp, vp, vp, vp, vp, i32]
     lib.pb200_fit_trace_host.restype = C.c_int
     lib.pb200_forecast_csv_lengths_device.argtypes = [vp, vp, vp, vp, i64, i32, vp]

@@ -229,16 +229,19 @@ def n_regressors(opts) -> int:
     return int(opts.n_regressors) if getattr(opts, "abi_version", L.ABI_VERSION) == L.ABI_VERSION_REGRESSORS else 0
 
 
-def regressor_scales(reg, offsets, standardize) -> np.ndarray:
+def regressor_scales(reg, offsets, standardize, copy=None) -> np.ndarray:
     """fbprophet 0.5's initialize_scales for the regressors, restated on the host (the test reference of the library's
     standardisation): ``[n, R, 2]`` (mu, std) per series.  ``reg``: ``[R, n_rows]`` values aligned with the batch's rows;
     ``standardize``: per regressor 'auto', True or False.  Fewer than two distinct values, or 'auto' on values that are
-    exactly {0, 1}: (0, 1); else the mean and the sample standard deviation (ddof = 1).  A non-finite value: (NaN, NaN)."""
+    exactly {0, 1}: (0, 1), or with ``copy`` (``[n, R, 2]``, a prophet_copy's scales, DESIGN §20) the series' copy
+    entry; else the mean and the sample standard deviation (ddof = 1).  A non-finite value: (NaN, NaN)."""
     reg = np.asarray(reg, np.float64)
     offsets = np.asarray(offsets, np.int64)
     n, R = offsets.size - 1, reg.shape[0]
     out = np.zeros((n, R, 2))
     out[:, :, 1] = 1.0
+    if copy is not None:
+        out[:] = np.asarray(copy, np.float64)
     for i in range(n):
         for r in range(R):
             x = reg[r, offsets[i]:offsets[i + 1]]
@@ -556,9 +559,32 @@ def fit_batch_warm_host(ctx: L.Context, opts: L.Options, ds_ns: np.ndarray, y: n
     return FittedBatch(params, tchange, mi32, mi64, mf64, lay.smax, lay.kmax, warm=warm), trace
 
 
+def regressor_scales_device(ctx: L.Context, opts, regressors, offsets_host: np.ndarray):
+    """pb200_regressor_scales_device: the standardisation a fit with ``regressors`` (a contiguous float64 CUDA tensor
+    ``[R, n_rows]``) gives each series, without the fit: ``(reg_scale [n, R, 2] float64, bad [n] bool)`` CUDA tensors,
+    ``bad`` where a value of the series is not finite."""
+    import torch
+    offsets_host = np.ascontiguousarray(offsets_host, dtype=np.int64)
+    n = offsets_host.size - 1
+    R = n_regressors(opts)
+    dev = regressors.device
+    rows = int(offsets_host[-1])
+    if (regressors.dtype != torch.float64 or tuple(regressors.shape) != (R, rows) or not regressors.is_contiguous()):
+        raise ValueError(f"regressors must be a contiguous float64 tensor of shape ({R}, {rows})")
+    scale = torch.empty((n, R, 2), dtype=torch.float64, device=dev)
+    bad = torch.zeros(n, dtype=torch.uint8, device=dev)
+    if n:
+        torch.cuda.current_stream(dev).synchronize()
+        L.check(L.load().pb200_regressor_scales_device(ctx.handle, C.byref(opts), regressors.data_ptr(),
+                                                       _np_ptr(offsets_host), n, scale.data_ptr(), bad.data_ptr()),
+                "pb200_regressor_scales_device")
+    return scale, bad.bool()
+
+
 def fit_batch_device(ctx: L.Context, opts: L.Options, ds_ns, y, offsets_host: np.ndarray,
                      floor: float, cap_multiplier: float, cap=None, out: Optional[FittedBatch] = None,
-                     sync: bool = True, prior=None, init: Optional[FittedBatch] = None, regressors=None) -> FittedBatch:
+                     sync: bool = True, prior=None, init: Optional[FittedBatch] = None, regressors=None,
+                     reg_scale_copy=None) -> FittedBatch:
     """pb200_fit_warm_device: ``ds_ns`` / ``y`` / ``cap`` are torch CUDA tensors already in HBM.  ``prior``: None (the
     options' prior scales) or a float64 CUDA tensor ``[n, 2]`` of (changepoint_prior_scale, seasonality_prior_scale)
     per series; a series whose pair is not finite and > 0 gets status ``L.ST_BAD_PRIOR``.  ``init``: None (every
@@ -567,12 +593,16 @@ def fit_batch_device(ctx: L.Context, opts: L.Options, ds_ns, y, offsets_host: np
     DESIGN §11's rule allows, and ``out.warm`` receives the ``L.WARM_*`` code of every series.  ``regressors``: None, or
     for options with regressors (make_regressor_options) a contiguous float64 CUDA tensor ``[R, n_rows]`` of their
     values aligned with ``ds_ns`` (pb200_fit_regressors_device; not with ``prior`` or ``init``); ``out.reg_scale``
-    then receives each series' standardisation ``[n, R, 2]``."""
+    then receives each series' standardisation ``[n, R, 2]``.  ``reg_scale_copy`` (with ``regressors``): a float64 CUDA
+    tensor ``[n, R, 2]``, the (mu, std) each regressor keeps where it is not standardised instead of (0, 1)
+    (pb200_fit_regressors_copy_device; the backtest's prophet_copy, DESIGN §20)."""
     import torch
     offsets_host = np.ascontiguousarray(offsets_host, dtype=np.int64)
     n = offsets_host.size - 1
     lay = L.get_layout(opts)
     dev = ds_ns.device
+    if reg_scale_copy is not None and regressors is None:
+        raise ValueError("reg_scale_copy goes with regressors")
     if regressors is not None:
         if prior is not None or init is not None:
             raise ValueError("regressors are not supported with prior or init")
@@ -590,16 +620,20 @@ def fit_batch_device(ctx: L.Context, opts: L.Options, ds_ns, y, offsets_host: np
         if out.reg_scale is None:
             out.reg_scale = torch.empty((n, R, 2), dtype=torch.float64, device=dev)
         _check_reg_scale(out.reg_scale, n, R, "out.reg_scale", dev)
+        if reg_scale_copy is not None:
+            _check_reg_scale(reg_scale_copy, n, R, "reg_scale_copy", dev)
         if n > 0:
             torch.cuda.current_stream(dev).synchronize()
-            rc = L.load().pb200_fit_regressors_device(ctx.handle, C.byref(opts), ds_ns.data_ptr(), y.data_ptr(),
-                                                      _y_dtype(y), _np_ptr(offsets_host), n, float(floor),
-                                                      float(cap_multiplier), cap.data_ptr() if cap is not None else None,
-                                                      regressors.data_ptr(), out.reg_scale.data_ptr(),
-                                                      out.params.data_ptr(), out.tchange.data_ptr(),
-                                                      out.meta_i32.data_ptr(), out.meta_i64.data_ptr(),
-                                                      out.meta_f64.data_ptr())
-            L.check(rc, "pb200_fit_regressors_device")
+            lib = L.load()
+            head = (ctx.handle, C.byref(opts), ds_ns.data_ptr(), y.data_ptr(), _y_dtype(y), _np_ptr(offsets_host), n,
+                    float(floor), float(cap_multiplier), cap.data_ptr() if cap is not None else None, regressors.data_ptr())
+            tail = (out.reg_scale.data_ptr(), out.params.data_ptr(), out.tchange.data_ptr(), out.meta_i32.data_ptr(),
+                    out.meta_i64.data_ptr(), out.meta_f64.data_ptr())
+            if reg_scale_copy is not None:
+                rc = lib.pb200_fit_regressors_copy_device(*head, reg_scale_copy.data_ptr(), *tail)
+                L.check(rc, "pb200_fit_regressors_copy_device")
+            else:
+                L.check(lib.pb200_fit_regressors_device(*head, *tail), "pb200_fit_regressors_device")
             if sync:
                 ctx.synchronize()
         return out
@@ -690,6 +724,39 @@ def make_future_device(ctx: L.Context, last_ds_ns, periods: int, freq_ns: int):
         L.check(rc, "pb200_make_future_device")
         ctx.synchronize()
     return out
+
+
+def join_future_regressors_device(ctx: L.Context, tab_ds, tab_offsets_host: np.ndarray, tab_reg, model_group,
+                                  future_ds):
+    """pb200_join_future_regressors_device (DESIGN §20): the regressors' values of every model's forecast grid from a
+    packed table.  ``tab_ds`` int64 ``[rows]`` and ``tab_reg`` float64 ``[R, rows]`` CUDA tensors packed by group
+    (``tab_offsets_host`` ``[n_groups + 1]``, timestamps ascending and distinct within a group); ``model_group`` int64
+    ``[n]`` each model's group (-1: none); ``future_ds`` int64 ``[n, H]``.  Returns ``(future_reg [R, n, H] float64,
+    missing [n] int32, first_missing [n] int64)`` CUDA tensors: NaN where a grid point has no row, the count of such
+    points per model and the first one's timestamp (INT64_MIN where there is none); rows off the grid are ignored.
+    ``future_reg`` is what predict_batch_device's ``regressors=`` takes."""
+    import torch
+    dev = future_ds.device
+    n, h = int(future_ds.shape[0]), int(future_ds.shape[1])
+    R = int(tab_reg.shape[0])
+    rows = int(tab_ds.shape[0])
+    for t, dt, shape in ((tab_ds, torch.int64, (rows,)), (tab_reg, torch.float64, (R, rows)),
+                         (model_group, torch.int64, (n,)), (future_ds, torch.int64, (n, h))):
+        if t.dtype != dt or tuple(t.shape) != shape or not t.is_contiguous() or t.device != dev:
+            raise ValueError(f"join_future_regressors_device wants contiguous {dt} tensors of shape {shape} on {dev}")
+    offs = torch.from_numpy(np.ascontiguousarray(tab_offsets_host, dtype=np.int64)).to(dev)
+    out = torch.empty((R, n, h), dtype=torch.float64, device=dev)
+    missing = torch.empty(n, dtype=torch.int32, device=dev)
+    first = torch.empty(n, dtype=torch.int64, device=dev)
+    if n:
+        torch.cuda.current_stream(dev).synchronize()
+        rc = L.load().pb200_join_future_regressors_device(ctx.handle, tab_ds.data_ptr() if rows else None,
+                                                          offs.data_ptr(), tab_reg.data_ptr() if rows else None, rows, R,
+                                                          model_group.data_ptr(), future_ds.data_ptr(), n, h,
+                                                          out.data_ptr(), missing.data_ptr(), first.data_ptr())
+        L.check(rc, "pb200_join_future_regressors_device")
+        ctx.synchronize()
+    return out, missing, first
 
 
 def forecast_csv_device(ctx: L.Context, series_id, dim_id, ds_ns, quantity, created: bytes):
@@ -1349,6 +1416,17 @@ def cv_plan_device(ctx: L.Context, opts: L.Options, ds_ns, offsets_host: np.ndar
     return CvPlan(counts, mask.cpu().numpy(), err.cpu().numpy(), pair_off, ps, cut, he, we)
 
 
+def plan_options(opts):
+    """The options cv_plan_device takes for ``opts``: the plan reads the seasonalities only, so options with regressors
+    give their pb200_options_v2 part (version 2, the same table); any other options are returned as they are."""
+    if not n_regressors(opts):
+        return opts
+    o = L.OptionsV2.from_buffer_copy(opts)
+    o.abi_version = L.ABI_VERSION_TABLE
+    o._source = opts        # keeps the table entries alive as long as the copy
+    return o
+
+
 def cv_plan_errors(plan: CvPlan):
     """(message, per-series bool mask) of the first kind of plan error present, or None: fbprophet's exceptions."""
     for bit, msg in ((L.CV_ERR_HORIZON, "Less data than horizon."),
@@ -1388,7 +1466,7 @@ class CvResult:
     Metrics rows (when requested), ordered by (series, horizon): ``m_series``, ``horizon`` (ns), ``mse``, ``rmse``,
     ``mae``, ``mape``, ``coverage`` (None without intervals).
     ``fitted``: with ``keep_fits``, the cutoff fits in plan order, each record in the layout of ``opts`` (beta packed
-    by its mask, zero beyond).
+    by its mask, zero beyond); with regressors its ``reg_scale`` is each cutoff fit's (mu, std).
     With a ``grid`` of n_grid prior-scale pairs every series index above is a virtual one, ``s * n_grid + g`` for series
     ``s`` fitted with grid point ``g``, and "plan order" is (series, grid point, cutoff)."""
     pair_series: np.ndarray
@@ -1501,7 +1579,7 @@ def cross_validation_device(ctx: L.Context, opts: L.Options, ds_ns, y, offsets_h
                             rolling_window: Optional[float] = None, plan: Optional[CvPlan] = None,
                             keep_fits: bool = False, timings: Optional[dict] = None,
                             _row_budget: Optional[int] = None, grid=None,
-                            aggregate_ns: Optional[int] = None, quantiles=None) -> CvResult:
+                            aggregate_ns: Optional[int] = None, quantiles=None, regressors=None) -> CvResult:
     """fbprophet.diagnostics.cross_validation (and, with ``rolling_window``, performance_metrics) for every series of a
     packed batch: ``ds_ns`` / ``y`` CUDA tensors sorted within each series, ``cap`` the float64 CUDA tensor of each
     series' full-history cap.  Per chunk of series: one gather, one pb200_fit_device per full-history seasonality mask
@@ -1518,7 +1596,14 @@ def cross_validation_device(ctx: L.Context, opts: L.Options, ds_ns, y, offsets_h
     after each cutoff c, with their metrics, as ``CvResult.windows`` (DESIGN §14).  Every other output is unchanged.
     With intervals the chunk's predict is pb200_predict_sums_anchored_device, whose pointwise outputs are
     pb200_predict_device's; the window totals are pb200_cv_windows_device's (stages ``windows`` and
-    ``window_metrics``)."""
+    ``window_metrics``).
+    ``regressors`` (for options with regressors, required with them): a contiguous float64 CUDA tensor ``[R, rows]``
+    aligned with ``ds_ns``.  fbprophet 0.5's cross_validation with prophet_copy (DESIGN §20): the full histories' (mu,
+    std) by pb200_regressor_scales_device (a non-finite value raises ValueError), the cutoff fits on z = (x - mu_full) /
+    std_full gathered by pb200_cv_gather_regressors_device and fitted with those scales as their copy
+    (pb200_fit_regressors_copy_device), the held-out rows' z predicted with each cutoff fit's own (mu, std).  The plan
+    is made with ``plan_options(opts)``; ``CvResult.fitted`` carries ``reg_scale``.  Not with ``grid``,
+    ``aggregate_ns`` or ``quantiles``."""
     import time
     import torch
     tm = timings if timings is not None else {}
@@ -1530,8 +1615,13 @@ def cross_validation_device(ctx: L.Context, opts: L.Options, ds_ns, y, offsets_h
         clock[0] = t
     offsets_host = np.ascontiguousarray(offsets_host, dtype=np.int64)
     dev = ds_ns.device
+    R = n_regressors(opts)
+    if (regressors is None) != (R == 0):
+        raise ValueError("regressors= is required with options that have regressors, and taken only with them")
+    if R and (grid is not None or aggregate_ns is not None or quantiles is not None):
+        raise ValueError("grid, aggregate_ns and quantiles are not supported with regressors")
     if plan is None:
-        plan = cv_plan_device(ctx, opts, ds_ns, offsets_host, horizon_ns, period_ns, initial_ns)
+        plan = cv_plan_device(ctx, plan_options(opts), ds_ns, offsets_host, horizon_ns, period_ns, initial_ns)
         lap("plan")
     bad = cv_plan_errors(plan)
     if bad is not None:
@@ -1561,6 +1651,19 @@ def cross_validation_device(ctx: L.Context, opts: L.Options, ds_ns, y, offsets_h
             raise ValueError("quantiles do not combine with aggregate_ns or grid")
         levels = np.asarray(quantiles, dtype=np.float64)
         quantile_percentiles(levels)
+    if R:
+        rows_all = int(offsets_host[-1])
+        if (regressors.dtype != torch.float64 or tuple(regressors.shape) != (R, rows_all)
+                or not regressors.is_contiguous() or regressors.device != dev):
+            raise ValueError(f"regressors must be a contiguous float64 tensor of shape ({R}, {rows_all}) on {dev}")
+        scale_full, bad_reg = regressor_scales_device(ctx, opts, regressors, offsets_host)
+        bad_h = bad_reg.cpu().numpy()
+        if bad_h.any():
+            i = int(np.flatnonzero(bad_h)[0])
+            r = int(torch.nonzero(torch.isnan(scale_full[i, :, 0]))[0, 0])
+            raise ValueError(f"Found NaN in column {opts.regressors[r].name.decode()} (first offender: series {i}; "
+                             f"{int(bad_h.sum())} series in all)")
+        lap("scales")
     chunks, he_h, we_h = _cv_chunks(plan, offsets_host, int(_row_budget or CV_ROW_BUDGET), n_grid)
     cap = cap.to(device=dev, dtype=torch.float64)
     pieces = []
@@ -1590,6 +1693,14 @@ def cross_validation_device(ctx: L.Context, opts: L.Options, ds_ns, y, offsets_h
                                            plan.pair_series.data_ptr(), plan.hist_end.data_ptr(), plan.win_end.data_ptr(),
                                            d_pairs.data_ptr(), n, d_fit_off.data_ptr(), hmax, ds_g.data_ptr(),
                                            y_g.data_ptr(), fut.data_ptr()), "pb200_cv_gather_device")
+        if R:
+            reg_g = torch.empty((R, int(fit_off[-1])), dtype=torch.float64, device=dev)
+            reg_f = torch.empty((R, n, hmax), dtype=torch.float64, device=dev)
+            L.check(lib.pb200_cv_gather_regressors_device(
+                ctx.handle, regressors.data_ptr(), int(offsets_host[-1]), R, scale_full.data_ptr(), d_off.data_ptr(),
+                plan.pair_series.data_ptr(), plan.hist_end.data_ptr(), plan.win_end.data_ptr(), d_pairs.data_ptr(), n,
+                d_fit_off.data_ptr(), hmax, reg_g.data_ptr(), reg_f.data_ptr()), "pb200_cv_gather_regressors_device")
+            copy_p = scale_full[torch.from_numpy(ps_h[perm]).to(dev)].contiguous()
         ctx.synchronize()
         lap("gather")
         # fits, one call per mask class; records re-laid into the layout of ``opts`` for the one predict call
@@ -1598,7 +1709,8 @@ def cross_validation_device(ctx: L.Context, opts: L.Options, ds_ns, y, offsets_h
                              torch.zeros((n, lay.smax), dtype=torch.float64, device=dev),
                              torch.empty((n, 8), dtype=torch.int32, device=dev),
                              torch.empty((n, 2), dtype=torch.int64, device=dev),
-                             torch.empty((n, 4), dtype=torch.float64, device=dev), lay.smax, lay.kmax)
+                             torch.empty((n, 4), dtype=torch.float64, device=dev), lay.smax, lay.kmax,
+                             reg_scale=torch.empty((n, R, 2), dtype=torch.float64, device=dev) if R else None)
         cap_p = cap[torch.from_numpy(ps_h[perm]).to(dev)].contiguous()
         prior_p = torch.from_numpy(grid_h[g_h[perm]]).to(dev) if grid_h is not None else None
         bounds = np.flatnonzero(np.diff(np.concatenate(([-1], sp, [-1])))).tolist()
@@ -1606,7 +1718,11 @@ def cross_validation_device(ctx: L.Context, opts: L.Options, ds_ns, y, offsets_h
             oc = _with_mask(opts, int(sp[a]))
             r0, r1 = int(fit_off[a]), int(fit_off[b])
             fc = fit_batch_device(ctx, oc, ds_g[r0:r1], y_g[r0:r1], fit_off[a:b + 1] - r0, float(floor), 1.0,
-                                  cap=cap_p[a:b], prior=prior_p[a:b] if prior_p is not None else None)
+                                  cap=cap_p[a:b], prior=prior_p[a:b] if prior_p is not None else None,
+                                  regressors=reg_g[:, r0:r1].contiguous() if R else None,
+                                  reg_scale_copy=copy_p[a:b] if R else None)
+            if R:
+                fitted.reg_scale[a:b] = fc.reg_scale
             # a table's cutoff fit packs the same active columns as the full model (never more: every entry of its
             # table is an active entry of the full one); its table drops the built-ins forced off and so numbers the
             # entries differently, and the mask is restated in the full table's entries
@@ -1633,7 +1749,8 @@ def cross_validation_device(ctx: L.Context, opts: L.Options, ds_ns, y, offsets_h
             fcst = predict_quantiles_device(ctx, opts, fitted, fut, floor_p, cap_p, levels, seed=seed,
                                             intervals=intervals and opts.uncertainty_samples > 0)
         else:
-            fcst = predict_batch_device(ctx, opts, fitted, fut, floor_p, cap_p, seed=seed, intervals=intervals)
+            fcst = predict_batch_device(ctx, opts, fitted, fut, floor_p, cap_p, seed=seed, intervals=intervals,
+                                        regressors=reg_f if R else None)
         lap("predict")
         # back to plan order, then the held-out rows
         inv = torch.from_numpy(np.argsort(perm, kind="stable")).to(dev)
@@ -1690,7 +1807,8 @@ def cross_validation_device(ctx: L.Context, opts: L.Options, ds_ns, y, offsets_h
         fh = None
         if keep_fits:
             fh = FittedBatch(*(x[inv].cpu().numpy() for x in (fitted.params, fitted.tchange, fitted.meta_i32,
-                                                               fitted.meta_i64, fitted.meta_f64)), lay.smax, lay.kmax)
+                                                               fitted.meta_i64, fitted.meta_f64)), lay.smax, lay.kmax,
+                             reg_scale=fitted.reg_scale[inv].cpu().numpy() if R else None)
         pieces.append(({k: (v.cpu().numpy() if v is not None else None) for k, v in rows.items()}, met,
                        fitted.meta_i32[inv, 4].cpu().numpy(), fh, wpiece, qpiece))
         lap("rows")
@@ -1711,7 +1829,8 @@ def cross_validation_device(ctx: L.Context, opts: L.Options, ds_ns, y, offsets_h
     fitted_all = None
     if keep_fits and pieces:
         fitted_all = FittedBatch(*(np.concatenate([getattr(p[3], f) for p in pieces])
-                                   for f in ("params", "tchange", "meta_i32", "meta_i64", "meta_f64")), lay.smax, lay.kmax)
+                                   for f in ("params", "tchange", "meta_i32", "meta_i64", "meta_f64")), lay.smax, lay.kmax,
+                                 reg_scale=np.concatenate([p[3].reg_scale for p in pieces]) if R else None)
     ent_all, ps_all, g_all = _cv_entries(plan, 0, plan.n_cutoffs.size, n_grid)
     status = cat([p[2] for p in pieces]) if pieces else np.zeros(0, np.int32)
     windows = None

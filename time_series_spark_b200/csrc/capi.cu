@@ -10,6 +10,7 @@
 #include "cv_kernel.cuh"
 #include "insample_kernel.cuh"
 #include "reg_scale_kernel.cuh"
+#include "join_kernel.cuh"
 
 #include <algorithm>
 #include <cstdio>
@@ -592,7 +593,8 @@ static int fit_impl(pb200_ctx* c, const pb200_options* opts, const int64_t* d_ds
                     int64_t* d_meta_i64, double* d_meta_f64, const double* d_theta_in, double* d_grad_out,
                     double* d_trace = nullptr, int trace_cap = 0, const double* d_init_params = nullptr,
                     const int32_t* d_init_meta = nullptr, int32_t* d_warm = nullptr, bool regs = false,
-                    const double* d_reg = nullptr, double* d_reg_scale = nullptr) {
+                    const double* d_reg = nullptr, double* d_reg_scale = nullptr,
+                    const double* d_reg_scale_copy = nullptr) {
     if (!c) return fail(PB200_E_ARG, "ctx is null");
     CK(cudaSetDevice(c->device));
     CK(c->d_vcount.reserve((NQ + 1) * 4));     // [NQ]: the table class
@@ -697,6 +699,7 @@ static int fit_impl(pb200_ctx* c, const pb200_options* opts, const int64_t* d_ds
         ra.spec = reg;
         ra.reg_scale = d_reg_scale;
         ra.bad = (unsigned char*)c->d_regbad.p;
+        ra.scale_copy = d_reg_scale_copy;
         pb200::reg_scale_kernel<<<std::min((N + 7) / 8, c->sms * 8), 256, 0, c->stream>>>(ra);
         CK(cudaGetLastError());
         c->launches++;
@@ -1140,6 +1143,88 @@ PB200_API int pb200_fit_regressors_device(pb200_ctx* c, const pb200_options* opt
     return fit_impl(c, opts, d_ds, d_y, y_dtype, h_offsets, n_series, floor, cap_multiplier, d_cap, nullptr, d_params,
                     d_tchange, d_meta_i32, d_meta_i64, d_meta_f64, nullptr, nullptr, nullptr, 0, nullptr, nullptr, nullptr,
                     true, d_reg, d_reg_scale);
+}
+
+PB200_API int pb200_fit_regressors_copy_device(pb200_ctx* c, const pb200_options* opts, const int64_t* d_ds,
+                                               const void* d_y, int32_t y_dtype, const int64_t* h_offsets,
+                                               int64_t n_series, double floor, double cap_multiplier, const double* d_cap,
+                                               const double* d_reg, const double* d_reg_scale_copy, double* d_reg_scale,
+                                               double* d_params, double* d_tchange, int32_t* d_meta_i32,
+                                               int64_t* d_meta_i64, double* d_meta_f64) {
+    if (!d_reg_scale_copy && n_series > 0) return fail(PB200_E_ARG, "null pointer (reg_scale_copy)");
+    return fit_impl(c, opts, d_ds, d_y, y_dtype, h_offsets, n_series, floor, cap_multiplier, d_cap, nullptr, d_params,
+                    d_tchange, d_meta_i32, d_meta_i64, d_meta_f64, nullptr, nullptr, nullptr, 0, nullptr, nullptr, nullptr,
+                    true, d_reg, d_reg_scale, d_reg_scale_copy);
+}
+
+PB200_API int pb200_regressor_scales_device(pb200_ctx* c, const pb200_options* opts, const double* d_reg,
+                                            const int64_t* h_offsets, int64_t n_series, double* d_reg_scale,
+                                            uint8_t* d_bad) {
+    if (!c) return fail(PB200_E_ARG, "ctx is null");
+    int rc = check_opts(opts, true);
+    if (rc) return rc;
+    pb200::RegSpec reg;
+    opts_reg(opts, &reg);
+    if (reg.R < 1) return fail(PB200_E_ARG, "options without regressors");
+    if (n_series < 0 || n_series > (1LL << 30)) return fail(PB200_E_ARG, "n_series");
+    if (n_series == 0) return PB200_OK;
+    if (!d_reg || !h_offsets || !d_reg_scale || !d_bad) return fail(PB200_E_ARG, "null pointer");
+    for (int64_t i = 0; i < n_series; ++i)
+        if (h_offsets[i + 1] < h_offsets[i] || h_offsets[0] != 0) return fail(PB200_E_ARG, "offsets");
+    CK(cudaSetDevice(c->device));
+    CK(c->d_offsets.reserve((size_t)(n_series + 1) * 8));
+    CK(cudaMemcpyAsync(c->d_offsets.p, h_offsets, (size_t)(n_series + 1) * 8, cudaMemcpyHostToDevice, c->stream));
+    pb200::RegScaleArgs ra;
+    ra.reg = d_reg;
+    ra.n_rows = h_offsets[n_series];
+    ra.offsets = (const long long*)c->d_offsets.p;
+    ra.n_series = (int)n_series;
+    ra.spec = reg;
+    ra.reg_scale = d_reg_scale;
+    ra.bad = d_bad;
+    ra.scale_copy = nullptr;
+    const int N = (int)n_series;
+    pb200::reg_scale_kernel<<<std::min((N + 7) / 8, c->sms * 8), 256, 0, c->stream>>>(ra);
+    CK(cudaGetLastError());
+    c->launches++;
+    CK(cudaStreamSynchronize(c->stream));      // the offsets' staging buffer is the context's
+    return PB200_OK;
+}
+
+PB200_API int pb200_cv_gather_regressors_device(pb200_ctx* c, const double* d_reg, int64_t n_rows, int32_t n_regressors,
+                                                const double* d_reg_scale_full, const int64_t* d_offsets,
+                                                const int32_t* d_pair_series, const int64_t* d_hist_end,
+                                                const int64_t* d_win_end, const int64_t* d_pairs, int64_t n,
+                                                const int64_t* d_fit_off, int32_t hmax, double* d_reg_fit,
+                                                double* d_reg_future) {
+    if (!c) return fail(PB200_E_ARG, "ctx is null");
+    if (n < 0 || hmax < 1 || n_rows < 0) return fail(PB200_E_ARG, "sizes");
+    if (n_regressors < 1 || n_regressors > PB200_MAX_REGRESSORS) return fail(PB200_E_ARG, "n_regressors");
+    if (n == 0) return PB200_OK;
+    if (!d_reg || !d_reg_scale_full || !d_offsets || !d_pair_series || !d_hist_end || !d_win_end || !d_pairs ||
+        !d_fit_off || !d_reg_fit || !d_reg_future)
+        return fail(PB200_E_ARG, "null pointer");
+    CK(cudaSetDevice(c->device));
+    pb200::CvRegGatherArgs a;
+    a.reg = d_reg;
+    a.n_rows = n_rows;
+    a.R = n_regressors;
+    a.scale_full = d_reg_scale_full;
+    a.offsets = (const long long*)d_offsets;
+    a.pair_series = d_pair_series;
+    a.hist_end = (const long long*)d_hist_end;
+    a.win_end = (const long long*)d_win_end;
+    a.pairs = (const long long*)d_pairs;
+    a.n = n;
+    a.fit_off = (const long long*)d_fit_off;
+    a.hmax = hmax;
+    a.reg_fit = d_reg_fit;
+    a.reg_fut = d_reg_future;
+    const int grid = (int)std::min<int64_t>(n, (int64_t)c->sms * 32);
+    pb200::cv_gather_regressors_kernel<<<grid, 256, 0, c->stream>>>(a);
+    CK(cudaGetLastError());
+    c->launches++;
+    return PB200_OK;
 }
 
 PB200_API int pb200_fit_regressors_host(pb200_ctx* c, const pb200_options* opts, const int64_t* h_ds, const void* h_y,
@@ -2139,6 +2224,40 @@ PB200_API int pb200_outlier_compact_device(pb200_ctx* c, const int64_t* d_ds, co
     a.ds_out = (long long*)d_ds_out;
     a.y_out = d_y_out;
     pb200::insample::outlier_compact_kernel<<<outlier_grid(c, n_series), pb200::insample::THREADS, 0, c->stream>>>(a);
+    CK(cudaGetLastError());
+    c->launches++;
+    return PB200_OK;
+}
+
+PB200_API int pb200_join_future_regressors_device(pb200_ctx* c, const int64_t* d_tab_ds, const int64_t* d_tab_offsets,
+                                                  const double* d_tab_reg, int64_t n_rows, int32_t n_regressors,
+                                                  const int64_t* d_model_group, const int64_t* d_future_ds,
+                                                  int64_t n_models, int32_t horizon, double* d_future_reg,
+                                                  int32_t* d_missing, int64_t* d_first_missing) {
+    if (!c) return fail(PB200_E_ARG, "ctx is null");
+    if (n_rows < 0 || n_models < 0 || horizon < 0) return fail(PB200_E_ARG, "sizes");
+    if (n_regressors < 1 || n_regressors > PB200_MAX_REGRESSORS) return fail(PB200_E_ARG, "n_regressors");
+    if (n_models == 0) return PB200_OK;
+    if (!d_tab_offsets || !d_model_group || !d_missing || !d_first_missing || (n_rows > 0 && (!d_tab_ds || !d_tab_reg)) ||
+        (horizon > 0 && (!d_future_ds || !d_future_reg)))
+        return fail(PB200_E_ARG, "null pointer");
+    CK(cudaSetDevice(c->device));
+    pb200::join::JoinArgs a;
+    a.tab_ds = (const long long*)d_tab_ds;
+    a.tab_offsets = (const long long*)d_tab_offsets;
+    a.tab_reg = d_tab_reg;
+    a.rows = n_rows;
+    a.R = n_regressors;
+    a.model_group = (const long long*)d_model_group;
+    a.future_ds = (const long long*)d_future_ds;
+    a.n_models = n_models;
+    a.horizon = horizon;
+    a.future_reg = d_future_reg;
+    a.missing = d_missing;
+    a.first_missing = (long long*)d_first_missing;
+    const int grid = (int)std::max<int64_t>(1, std::min<int64_t>((n_models + pb200::join::WARPS - 1) / pb200::join::WARPS,
+                                                                 (int64_t)c->sms * 16));
+    pb200::join::join_future_regressors_kernel<<<grid, pb200::join::THREADS, 0, c->stream>>>(a);
     CK(cudaGetLastError());
     c->launches++;
     return PB200_OK;

@@ -13,11 +13,14 @@ struct RegScaleArgs {
     RegSpec spec;
     double* reg_scale;           // [n_series][R][2] out
     unsigned char* bad;          // [n_series] out: 1 if a value of the series' history is not finite
+    const double* scale_copy;    // [n_series][R][2]: the (mu, std) a regressor keeps where it is not standardised
+                                 // (fbprophet's prophet_copy of the full model's scales, DESIGN §20); null: (0, 1)
 };
 
 // fbprophet's initialize_scales for the regressors, one warp per series: a first pass for min, max, the {0, 1} test,
 // non-finite values and the sum, a second for sum (x - mu)^2 (the two-pass form of pandas' nanvar).  Fewer than two
-// distinct values, or a binary column under 'auto', or standardize = 0: (mu, std) = (0, 1).  A non-finite value: (NaN,
+// distinct values, or a binary column under 'auto', or standardize = 0: (mu, std) = (0, 1), or the series' scale_copy
+// entry when there is one (initialize_scales overwrites mu / std only where it standardises).  A non-finite value: (NaN,
 // NaN) and the series is flagged, so that prep_kernel gives it PB200_ST_BAD_REGRESSOR
 __global__ void __launch_bounds__(256) reg_scale_kernel(const RegScaleArgs a) {
     const int lane = threadIdx.x & 31;
@@ -46,6 +49,10 @@ __global__ void __launch_bounds__(256) reg_scale_kernel(const RegScaleArgs a) {
             mx = wmax(mx);
             sum = wsum(sum);
             double mu = 0.0, sd = 1.0;
+            if (a.scale_copy) {
+                mu = a.scale_copy[((size_t)s * R + r) * 2];
+                sd = a.scale_copy[((size_t)s * R + r) * 2 + 1];
+            }
             const int st = a.spec.standardize[r];
             if (nonfin) {
                 mu = sd = NAN;
@@ -66,6 +73,46 @@ __global__ void __launch_bounds__(256) reg_scale_kernel(const RegScaleArgs a) {
             }
         }
         if (lane == 0) a.bad[s] = (unsigned char)bad_any;
+    }
+}
+
+// The backtest's regressor values (DESIGN §20): fbprophet 0.5's cross_validation slices model.history, whose regressor
+// columns setup_dataframe has replaced by z = (x - mu_full) / std_full.  For each gathered entry (a plan pair, as
+// cv_gather_kernel's), z of its truncated history packed as the fit batch's planes and z of its held-out rows as
+// [n][hmax] frames; a short window's padding is 0.0, a finite value (a non-finite one would fail the whole model in
+// predict).  One CTA per entry.
+struct CvRegGatherArgs {
+    const double* reg;           // [R][n_rows] the original values
+    long long n_rows;
+    int R;
+    const double* scale_full;    // [n_series][R][2] (mu_full, std_full) of the full histories
+    const long long* offsets;    // [n_series + 1]
+    const int* pair_series;      // [pairs] (plan)
+    const long long* hist_end;
+    const long long* win_end;
+    const long long* pairs;      // [n]
+    long long n;
+    const long long* fit_off;    // [n + 1]
+    int hmax;
+    double* reg_fit;             // [R][fit_off[n]]
+    double* reg_fut;             // [R][n * hmax]
+};
+
+__global__ void __launch_bounds__(256) cv_gather_regressors_kernel(const CvRegGatherArgs a) {
+    const long long fit_rows = a.fit_off[a.n];
+    for (long long k = blockIdx.x; k < a.n; k += gridDim.x) {
+        const long long p = a.pairs[k];
+        const int s = a.pair_series[p];
+        const long long off = a.offsets[s], he = a.hist_end[p], we = a.win_end[p];
+        const long long dst = a.fit_off[k], len = he - off;
+        for (int r = 0; r < a.R; ++r) {
+            const double mu = a.scale_full[((size_t)s * a.R + r) * 2], sd = a.scale_full[((size_t)s * a.R + r) * 2 + 1];
+            const double* x = a.reg + (size_t)r * a.n_rows;
+            for (long long i = threadIdx.x; i < len; i += blockDim.x)
+                a.reg_fit[(size_t)r * fit_rows + dst + i] = reg_value(x[off + i], mu, sd);
+            for (int j = threadIdx.x; j < a.hmax; j += blockDim.x)
+                a.reg_fut[(size_t)r * a.n * a.hmax + k * a.hmax + j] = he + j < we ? reg_value(x[he + j], mu, sd) : 0.0;
+        }
     }
 }
 

@@ -6,7 +6,10 @@ the errors to metrics by forecast horizon.  All of it on the GPU: the cutoff pla
 the fits, the prediction and the metrics (time_series_spark_b200/csrc/cv_kernel.cuh; semantics in DESIGN §9).
 A seasonality table (``model.seasonalities`` or an int built-in order, DESIGN §18) is backtested as fbprophet's
 prophet_copy does it: every cutoff fit takes the full history's active seasonalities and nothing else, with every
-``backtest.*`` option below.
+``backtest.*`` option below.  With ``model.regressors`` (DESIGN §20) the input's regressor columns are read as the
+modeler reads them and every cutoff is fitted as fbprophet 0.5's cross_validation does it: on the full history's
+standardised values, keeping the full model's (mu, std) where the cutoff's history is not standardised;
+``backtest.aggregate`` and ``backtest.quantiles`` are refused with it.
 
 Keys (``backtest.*``):
   horizon            pandas Timedelta string, required ("1 days")
@@ -44,7 +47,7 @@ from .. import _lib as L
 from .. import batched
 from .. import dist as pdist
 from ..pack import pack_groups_cuda
-from .prophet_modeler import ProphetModeler, get_context, options_from_config
+from .prophet_modeler import ProphetModeler, get_context, options_from_config, regressor_names
 from .prophet_scorer import quantile_column, quantile_levels
 
 
@@ -253,6 +256,12 @@ class ProphetBacktester:
         backtest.aggregate, ``self.window_outputs`` gets the (window metrics, window rows or None) tables."""
         t0 = time.time()
         spec = backtest_spec_from_config(self.config)
+        reg_names = regressor_names(self.config)
+        if reg_names:
+            for key in ("aggregate", "quantiles"):
+                if spec[key] is not None:
+                    raise ValueError(f"backtest.{key} is not available with model.regressors: the window totals and "
+                                     "quantiles of a model with extra regressors are not implemented")
         floor = float(self.config["model"]["floor"])
         cap_multiplier = float(self.config["model"]["cap_multiplier"])
         opts = options_from_config(self.config)
@@ -261,7 +270,7 @@ class ProphetBacktester:
         ctx = get_context()
         import torch
         torch.cuda.set_device(ctx.device)
-        pk = pack_groups_cuda(table, device=f"cuda:{ctx.device}")
+        pk = pack_groups_cuda(table, device=f"cuda:{ctx.device}", reg_cols=reg_names)
         rank, ws, _ = pdist.world()
         if ws > 1 and not self.rank_local_input:
             lo, hi = pdist.shard_bounds(pk.offsets, ws)[rank]
@@ -292,7 +301,15 @@ class ProphetBacktester:
         short = np.diff(pk.offsets) < 2
         if np.any(short):
             raise ValueError("Dataframe has less than 2 non-NaN rows." + _who(pk.series_id, pk.dim_id, short))
-        plan = batched.cv_plan_device(ctx, opts, ds, pk.offsets, spec["horizon"], spec["period"], spec["initial"])
+        if reg_names:
+            # fbprophet's setup_dataframe on the full history: "Found NaN in column <name>", as the modeler says it
+            scale, nan = batched.regressor_scales_device(ctx, opts, pk.regressors, pk.offsets)
+            nan = nan.cpu().numpy()
+            if nan.any():
+                r = int(np.flatnonzero(np.isnan(scale[int(np.flatnonzero(nan)[0]), :, 0].cpu().numpy()))[0])
+                raise ValueError(f"Found NaN in column {reg_names[r]}" + _who(pk.series_id, pk.dim_id, nan))
+        plan = batched.cv_plan_device(ctx, batched.plan_options(opts), ds, pk.offsets, spec["horizon"], spec["period"],
+                                      spec["initial"])
         bad = batched.cv_plan_errors(plan)
         if bad is not None:
             raise ValueError(bad[0] + _who(pk.series_id, pk.dim_id, bad[1]))
@@ -303,7 +320,7 @@ class ProphetBacktester:
         res = batched.cross_validation_device(ctx, opts, ds, y, pk.offsets, floor, cap, spec["horizon"], spec["period"],
                                               spec["initial"], intervals=spec["intervals"], seed=spec["seed"],
                                               rolling_window=spec["rolling_window"], plan=plan, aggregate_ns=W,
-                                              quantiles=levels)
+                                              quantiles=levels, regressors=pk.regressors)
         for code, msg in ((L.ST_CAP_LE_FLOOR, "cap must be greater than floor (which defaults to 0)."),
                           (L.ST_BAD_INPUT, "Found non-finite y or a zero time span in a series.")):
             hit = np.zeros(pk.n, bool)

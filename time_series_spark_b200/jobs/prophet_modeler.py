@@ -25,6 +25,17 @@ version-2 records, which carry the table to the scorer; a table that restates th
 is the default model and writes the same version-1 bytes as ``yearly_seasonality: true``.  ``io.warm_start`` (and so
 ``insample.refit`` with a warm start) is refused for a table; ``insample`` without it serves table models unchanged.
 
+Extra regressors (DESIGN §20): ``model.regressors`` is a list of fbprophet ``add_regressor`` calls in the order they are
+made, ``{name, prior_scale? (default model.holidays_prior_scale, 10.0), standardize? ('auto', true, false), mode? (must be
+model.seasonality_mode)}``.  With it, regressor r is header-less CSV column 4 + r of the input (after ``quantity``), read
+as float64; an empty field is null (NaN).  The options come from ``batched.make_regressor_options`` and every error names
+the YAML key; a name that is a column of the input or the internal frame (series_id, dim_id, start_time, quantity, ds, y)
+is refused.  Rows whose y is null are dropped before the values are looked at, as fbprophet fits on
+``df[df['y'].notnull()]``; a NaN value on a kept row fails the job with fbprophet's ``ValueError("Found NaN in column
+<name>")``.  The models table then holds version-4 records, which carry each series' standardisation (mu, std) and the
+regressors to the scorer.  ``io.warm_start`` and the ``insample`` section are refused with regressors; the backtest takes them (DESIGN §20).  Without
+``model.regressors`` (or with an empty list) the job reads, fits and writes what it did before.
+
 ``io.warm_start`` (optional): the path of a previous models table, for a job re-run on a schedule over the same groups
 plus new rows (fbprophet's "updating fitted models", ``m.fit(df, init=stan_init(m_old))``).  Every group starts its
 fit from its row of that table when the row's changepoint count and seasonalities are those of the new history
@@ -111,19 +122,50 @@ def table_keys(config) -> list:
 
 
 def _model_key_error(e: ValueError, keys) -> ValueError:
-    """make_table_options' message with each key it names spelled as its YAML key (model.<key>); a message that names
-    none (the library's limits) is prefixed with the table's keys."""
+    """make_table_options' (or make_regressor_options') message with each key it names spelled as its YAML key
+    (model.<key>); a message that names none (the library's limits) is prefixed with the table's keys."""
     import re
     msg = str(e)
-    named = re.sub(r"(?<![\w.])(seasonalities(?=[\[:])|yearly_seasonality|weekly_seasonality|daily_seasonality|"
-                   r"seasonality_mode)", r"model.\1", msg)
+    named = re.sub(r"(?<![\w.])(seasonalities(?=[\[:])|regressors(?=[\[:])|yearly_seasonality|weekly_seasonality|"
+                   r"daily_seasonality|seasonality_mode|holidays_prior_scale)", r"model.\1", msg)
     return ValueError(named if named != msg else f"{' / '.join(keys)}: {msg}")
+
+
+# columns of the modeler's input and internal frames a regressor's column must not be named like (fbprophet's
+# validate_column_name refuses ds and y itself)
+INPUT_COLUMNS = frozenset(["series_id", "dim_id", "start_time", "quantity"])
+
+
+def regressor_keys(config) -> list:
+    """The ``model.*`` keys of extra regressors the config gives: ``model.regressors``, ``model.holidays_prior_scale``."""
+    m = config.get("model", {}) or {}
+    return [f"model.{k}" for k in ("regressors", "holidays_prior_scale") if k in m]
+
+
+def regressor_names(config) -> list:
+    """The names of ``model.regressors`` in order (the input's extra columns), [] without regressors; raises ValueError
+    naming the key for a value that is not a list and for a name that is a column of the input or internal frames."""
+    regs = (config.get("model", {}) or {}).get("regressors")
+    if regs is None:
+        return []
+    if not isinstance(regs, (list, tuple)):
+        raise ValueError(f"model.regressors must be a list of {{name, prior_scale?, standardize?, mode?}} (got {regs!r})")
+    names = []
+    for i, spec in enumerate(regs):
+        name = spec.get("name") if isinstance(spec, dict) else None
+        if isinstance(name, str) and name in INPUT_COLUMNS:
+            raise ValueError(f"model.regressors[{i}].name: {name!r} is a column of the modeler's input; a regressor "
+                             "column must have a name of its own")
+        names.append(name)
+    return names
 
 
 def options_from_config(config) -> L.Options:
     """The job's fit options from ``model.*``.  Without ``model.seasonalities`` and without an int order for a built-in,
     batched.make_options as always; with either, batched.make_table_options (DESIGN §18), whose errors name the YAML key.
-    A table that restates the default model gives the same pb200_options as the switches alone."""
+    A table that restates the default model gives the same pb200_options as the switches alone.  With
+    ``model.regressors`` (DESIGN §20), batched.make_regressor_options with the same table keywords; an empty list (or
+    ``model.holidays_prior_scale`` alone) is checked and then gives the options without it."""
     m = dict(config.get("model", {}) or {})
     kw = dict(growth=m.get("growth", "logistic"),
               seasonality_mode=m.get("seasonality_mode", "multiplicative"),
@@ -132,6 +174,22 @@ def options_from_config(config) -> L.Options:
               changepoint_prior_scale=m.get("changepoint_prior_scale", 0.05),
               seasonality_prior_scale=m.get("seasonality_prior_scale", 10.0))
     keys = table_keys(config)
+    rkeys = regressor_keys(config)
+    if rkeys:
+        names = regressor_names(config)
+        seas = m.get("seasonalities")
+        if seas is not None and not isinstance(seas, (list, tuple)):
+            raise ValueError(f"model.seasonalities must be a list of {{name, period, fourier_order, prior_scale?, "
+                             f"mode?}} (got {seas!r})")
+        try:
+            ropts = batched.make_regressor_options(regressors=m.get("regressors") or [],
+                                                   holidays_prior_scale=m.get("holidays_prior_scale", 10.0),
+                                                   seasonalities=seas or [],
+                                                   **{k: m.get(k, "auto") for k in _BUILTIN_KEYS}, **kw)
+        except ValueError as e:
+            raise _model_key_error(e, keys + rkeys) from None
+        if names:
+            return ropts
     if not keys:
         return batched.make_options(yearly_seasonality=m.get("yearly_seasonality", "auto"),
                                     weekly_seasonality=m.get("weekly_seasonality", "auto"),
@@ -165,6 +223,19 @@ def refuse_table_warm_start(config, opts) -> None:
         raise ValueError(f"io.warm_start is not available for a model with a seasonality table "
                          f"({', '.join(table_keys(config))}): warm start serves the default seasonalities only"
                          + (" (insample.refit would start from it too)" if "insample" in config else ""))
+
+
+def refuse_regressors(config) -> None:
+    """Warm start and the in-sample predict have no regressor values: ``io.warm_start`` (and so ``insample.refit`` with
+    it) and the ``insample`` section raise with ``model.regressors``, naming both keys, before any GPU work."""
+    if not regressor_names(config):
+        return
+    if (config.get("io") or {}).get("warm_start"):
+        raise ValueError("io.warm_start is not available with model.regressors: warm start serves models without extra "
+                         "regressors only" + (" (insample.refit would start from it too)" if "insample" in config else ""))
+    if "insample" in config:
+        raise ValueError("insample is not available with model.regressors: the in-sample predict of a model with extra "
+                         "regressors is not implemented")
 
 
 def who(series_id, dim_id, mask) -> str:
@@ -325,6 +396,12 @@ def models_table(fitted: batched.FittedBatch, series_id, dim_id, last_ds, opts: 
         raise ValueError("cap must be greater than floor (which defaults to 0)." + who(series_id, dim_id, status == L.ST_CAP_LE_FLOOR))
     if np.any(status == L.ST_BAD_INPUT):
         raise ValueError("Found non-finite y or a zero time span in a series." + who(series_id, dim_id, status == L.ST_BAD_INPUT))
+    bad = status == L.ST_BAD_REGRESSOR
+    if np.any(bad):
+        # fbprophet's setup_dataframe: "Found NaN in column <name>"; the regressor is the first one whose scale is NaN
+        i = int(np.flatnonzero(bad)[0])
+        r = int(np.flatnonzero(np.isnan(np.asarray(fitted.reg_scale)[i, :, 0]))[0])
+        raise ValueError(f"Found NaN in column {opts.regressors[r].name.decode()}" + who(series_id, dim_id, bad))
     ok = status >= 0
     for i in np.flatnonzero(~ok):
         print(f"Runtime error (solver status {int(status[i])}) for series_id: {int(series_id[i])}, "
@@ -358,6 +435,10 @@ class _ModelTimeSeriesOp:
         ins = insample_options(self.config)
         if table_keys(self.config):         # a table's refusals come before any GPU work
             refuse_table_warm_start(self.config, options_from_config(self.config))
+        reg_names = regressor_names(self.config)
+        if reg_names:                       # and so do the regressors'
+            refuse_regressors(self.config)
+            options_from_config(self.config)
         with_frame = ins is not None and bool((self.config.get("io") or {}).get("fitted"))
         # this rank's io.fitted frame (empty until a group is predicted)
         self.fitted_table = fitted_schema(table.schema.field("y").type).empty_table() if with_frame else None
@@ -365,7 +446,7 @@ class _ModelTimeSeriesOp:
         # group + sort on the GPU (two radix sorts), ds / y stay in HBM for the fit
         import torch
         torch.cuda.set_device(ctx.device)
-        pk = pack_groups_cuda(table, device=f"cuda:{ctx.device}")
+        pk = pack_groups_cuda(table, device=f"cuda:{ctx.device}", reg_cols=reg_names)
         torch.cuda.synchronize()
         t_pack = time.time()
         rank, ws, _ = pdist.world()
@@ -388,7 +469,7 @@ class _ModelTimeSeriesOp:
         if warm_path:
             init, unmatched = warm_start_init(read_warm_start(warm_path, pk.series_id), opts, pk.series_id, pk.dim_id)
         fitted_d = batched.fit_batch_device(ctx, opts, pk.ds.contiguous(), pk.y.contiguous(), pk.offsets,
-                                            float(floor), float(cap_multiplier), init=init)
+                                            float(floor), float(cap_multiplier), init=init, regressors=pk.regressors)
         fitted = fitted_d.to_host()
         if warm_path:
             print(warm_report(fitted.warm, unmatched))
@@ -495,16 +576,19 @@ class ProphetModeler:
     def read_input_dataframe(self, spark=None) -> Frame:
         """Header-less CSV ``dim_id,timestamp,quantity`` under hive dirs ``series_id=<int>/``
         (reference :102-116; fixture tests/fixtures/model-input).  Returns columns
-        series_id, dim_id, ds, y."""
+        series_id, dim_id, ds, y -- and with ``model.regressors`` one float64 column per regressor, named as it is,
+        read from the CSV columns after quantity (an empty field is null)."""
         pdist.size_host_pools()             # pyarrow threads = this rank's share of the lease, not os.cpu_count()
         path = self.config["io"]["input"]
         part = pads.partitioning(pa.schema([("series_id", pa.int32())]), flavor="hive")
-        names = [f.name for f in MODEL_INPUT_SCHEMA if f.name != "series_id"]
+        regs = regressor_names(self.config)
+        names = [f.name for f in MODEL_INPUT_SCHEMA if f.name != "series_id"] + regs
+        types = {f.name: f.type for f in MODEL_INPUT_SCHEMA if f.name != "series_id"}
+        types.update({r: pa.float64() for r in regs})
         fmt = pads.CsvFileFormat(
             read_options=pacsv.ReadOptions(column_names=names),
             convert_options=pacsv.ConvertOptions(
-                column_types={f.name: f.type for f in MODEL_INPUT_SCHEMA if f.name != "series_id"},
-                timestamp_parsers=["%Y-%m-%d %H:%M:%S", pacsv.ISO8601]))
+                column_types=types, timestamp_parsers=["%Y-%m-%d %H:%M:%S", pacsv.ISO8601]))
         dset = pads.dataset(path, format=fmt, partitioning=part, exclude_invalid_files=False,
                             ignore_prefixes=[".", "_"])
         # Rank-local ingestion (SURVEY 8e): a group never spans two ``series_id=`` directories, so under torchrun each
@@ -519,12 +603,12 @@ class ProphetModeler:
                 self.rank_local_input = True
                 if not mine:
                     empty = pa.schema([("series_id", pa.int32()), ("dim_id", pa.int32()), ("ds", pa.timestamp("ns")),
-                                       ("y", pa.int32())]).empty_table()
+                                       ("y", pa.int32())] + [(r, pa.float64()) for r in regs]).empty_table()
                     return Frame(empty)
                 dset = pads.dataset(mine, format=fmt, partitioning=part, partition_base_dir=path,
                                     exclude_invalid_files=False)
-        tbl = dset.to_table(columns=["series_id", "dim_id", "start_time", "quantity"])
-        tbl = tbl.rename_columns(["series_id", "dim_id", "ds", "y"])
+        tbl = dset.to_table(columns=["series_id", "dim_id", "start_time", "quantity"] + regs)
+        tbl = tbl.rename_columns(["series_id", "dim_id", "ds", "y"] + regs)
         return Frame(tbl)
 
     def persist_models(self, model_df: Frame):

@@ -26,6 +26,15 @@ built-in order -- DESIGN §18) are scored with the table the record carries; no 
 above serves them.  With ``forecast.components`` each custom seasonality not named like a built-in adds one float64
 column of its name after ``additive_terms`` (in table order); a custom ``yearly`` / ``weekly`` / ``daily`` fills that
 built-in's column, which is null where the model's entry of that name is inactive.
+
+Models with extra regressors (version-4 records, written by the modeler from ``model.regressors`` -- DESIGN §20) need
+``io.future_regressors``: the regressors' values on the forecast grid, as hive dirs ``series_id=<id>/`` of header-less
+CSV ``dim_id,timestamp,<one value per regressor in the record's order>``.  Each rank reads the series_ids of its own
+models.  The values are joined onto every model's grid on the GPU by exact timestamp; rows off the grid are ignored.  A
+grid point without a row, a NaN value on one and a repeated ``(series_id, dim_id, timestamp)`` raise ValueError before
+any predict, naming the regressor or the row.  Point forecasts and ``forecast.intervals`` serve such models;
+``forecast.components``, ``forecast.aggregate``, ``forecast.aggregate_period`` and ``forecast.quantiles`` are refused
+with them, and ``io.future_regressors`` is refused for models without regressors.
 """
 from __future__ import annotations
 
@@ -270,6 +279,94 @@ def frequency_to_future(last_ds_ns: np.ndarray, periods: int, frequency) -> np.n
     return out
 
 
+def refuse_regressor_modes(config, regressors: bool) -> None:
+    """The scorer's keys that do not go with the models' class: with extra regressors (version-4 records) the modes
+    without regressor values (components, window and period totals, quantiles) and a missing io.future_regressors;
+    without them an io.future_regressors, which would be ignored.  Each raises ValueError naming the key."""
+    fc = config.get("forecast", {}) or {}
+    path = (config.get("io", {}) or {}).get("future_regressors")
+    if not regressors:
+        if path:
+            raise ValueError("io.future_regressors is given, but the models have no extra regressors (they are not "
+                             "version-4 records)")
+        return
+    for key in ("aggregate", "aggregate_period", "quantiles"):
+        if fc.get(key) is not None:
+            raise ValueError(f"forecast.{key} is not available for models with extra regressors (model.regressors)")
+    if _want_components(fc):
+        raise ValueError("forecast.components is not available for models with extra regressors (model.regressors)")
+    if not path:
+        raise ValueError("io.future_regressors is required: the models have extra regressors (model.regressors), "
+                         "whose values on the forecast grid it holds")
+
+
+def read_future_regressors(path: str, names, series_id) -> pa.Table:
+    """The rows of io.future_regressors (hive dirs ``series_id=<id>/``, header-less CSV ``dim_id,timestamp,<values>``)
+    whose series_id is one of ``series_id``: columns series_id, dim_id, ds and one float64 column per name (an empty
+    field is null)."""
+    part = pads.partitioning(pa.schema([("series_id", pa.int32())]), flavor="hive")
+    cols = ["dim_id", "ds"] + list(names)
+    types = dict({"dim_id": pa.int32(), "ds": pa.timestamp("ns")}, **{n: pa.float64() for n in names})
+    fmt = pads.CsvFileFormat(read_options=pacsv.ReadOptions(column_names=cols),
+                             convert_options=pacsv.ConvertOptions(
+                                 column_types=types, timestamp_parsers=["%Y-%m-%d %H:%M:%S", pacsv.ISO8601]))
+    dset = pads.dataset(path, format=fmt, partitioning=part, exclude_invalid_files=False, ignore_prefixes=[".", "_"])
+    sids = pa.array(np.unique(np.asarray(series_id, dtype=np.int32)), pa.int32())
+    return dset.to_table(columns=["series_id"] + cols, filter=pc.field("series_id").isin(sids))
+
+
+def _at(sid, did, i, ts) -> str:
+    return f"series_id {int(sid[i])}, dim_id {int(did[i])}, ds {np.datetime64(int(ts), 'ns')}"
+
+
+def future_regressor_values(ctx, table: pa.Table, names, sid, did, future_ds, ok):
+    """The future values ``[R, n, H]`` (a CUDA tensor) of the models ``(sid, did)`` on their grids ``future_ds`` (a CUDA
+    int64 tensor ``[n, H]``) from the rows of io.future_regressors in ``table``: packed on the GPU, matched to the models
+    on the host and joined by pb200_join_future_regressors_device.  Raises ValueError, naming the row, for a repeated
+    (series_id, dim_id, timestamp), and -- over the models ``ok`` -- naming the regressor, the first model and
+    timestamp and the count, for a grid point without a row or with a NaN value (fbprophet: "Found NaN in column")."""
+    import torch
+    from ..pack import pack_groups_cuda
+    from .prophet_modeler import _group_keys
+    dev = future_ds.device
+    pk = pack_groups_cuda(table, device=dev, y_col=None, reg_cols=list(names))
+    if pk.ds.numel() > 1:
+        starts = torch.zeros(pk.ds.numel(), dtype=torch.bool, device=dev)
+        starts[torch.from_numpy(pk.offsets[:-1]).to(dev)] = True
+        dup = (pk.ds[1:] == pk.ds[:-1]) & ~starts[1:]
+        if bool(dup.any()):
+            r = int(torch.nonzero(dup)[0, 0]) + 1
+            g = int(np.searchsorted(pk.offsets, r, side="right") - 1)
+            raise ValueError("io.future_regressors holds more than one row for "
+                             f"{_at(pk.series_id, pk.dim_id, g, pk.ds[r].item())} ({int(dup.sum())} repeated row(s) in all)")
+    gkey = _group_keys(pk.series_id, pk.dim_id)
+    mkey = _group_keys(sid, did)
+    order = np.argsort(gkey, kind="stable")
+    group = np.full(mkey.size, -1, np.int64)
+    if gkey.size:
+        pos = np.minimum(np.searchsorted(gkey[order], mkey), gkey.size - 1)
+        hit = gkey[order][pos] == mkey
+        group[hit] = order[pos[hit]]
+    fut, missing, first = batched.join_future_regressors_device(
+        ctx, pk.ds.contiguous(), pk.offsets, pk.regressors.contiguous(), torch.from_numpy(group).to(dev),
+        future_ds.contiguous())
+    missing = missing.cpu().numpy()
+    bad = (missing > 0) & ok
+    if bad.any():
+        i = int(np.flatnonzero(bad)[0])
+        raise ValueError(f"Found NaN in column {names[0]}: io.future_regressors has no row for {int(missing[bad].sum())} "
+                         f"forecast point(s) of {int(bad.sum())} model(s) (first: "
+                         f"{_at(sid, did, i, first[i].item())})")
+    okd = torch.from_numpy(ok).to(dev)
+    for r, name in enumerate(names):
+        nan = torch.isnan(fut[r]) & okd[:, None]
+        if bool(nan.any()):
+            i, h = (int(v) for v in torch.nonzero(nan)[0])
+            raise ValueError(f"Found NaN in column {name}: io.future_regressors holds NaN for {int(nan.sum())} forecast "
+                             f"point(s) (first: {_at(sid, did, i, future_ds[i, h].item())})")
+    return fut
+
+
 class _ForecastTimeSeriesOp:
     """Batched GROUPED_MAP operator over the models table."""
 
@@ -298,15 +395,16 @@ class _ForecastTimeSeriesOp:
         # rank's frame (an empty shard's too) then has the same columns
         rank, ws, _ = pdist.world()
         custom = ()
-        if (want_components or ws > 1) and table.num_rows:
+        if table.num_rows:
             valid = table["model"].filter(pc.is_valid(table["model"]))
             if len(valid):
                 if ws > 1:
                     model_record.check_one_class(valid)
-                if want_components:
-                    _, _, info0 = model_record.decode(valid.slice(0, 1))
-                    if "table" in info0:
-                        custom = custom_component_names(model_record.table_options(info0))
+                _, _, info0 = model_record.decode(valid.slice(0, 1))
+                # a version-4 record's refusals come before any GPU work, on every rank
+                refuse_regressor_modes(self.config, "regressors" in info0)
+                if want_components and "table" in info0:
+                    custom = custom_component_names(model_record.table_options(info0))
         if ws > 1 and table.num_rows:      # shard the model rows across ranks (equal horizon => equal work)
             lo, hi = pdist.shard_bounds(np.arange(table.num_rows + 1, dtype=np.int64), ws)[rank]
             table = table.slice(lo, hi - lo)
@@ -334,7 +432,9 @@ class _ForecastTimeSeriesOp:
         fitted, last_ds, info = model_record.decode(table["model"])
         mc = dict(interval_width=fc.get("interval_width", 0.8),
                   uncertainty_samples=fc.get("uncertainty_samples", 1000) if want_intervals or rule or months or levels else 0)
-        if "table" in info:          # a version-2 record: the fit's seasonality table (DESIGN §18)
+        if "regressors" in info:     # a version-4 record: the fit's table and regressors (DESIGN §20)
+            opts = model_record.regressor_options(info, **mc)
+        elif "table" in info:        # a version-2 record: the fit's seasonality table (DESIGN §18)
             opts = model_record.table_options(info, **mc)
         else:
             opts = batched.make_options(growth="logistic" if info["logistic"] else "linear",
@@ -350,7 +450,9 @@ class _ForecastTimeSeriesOp:
         sid = table["series_id"].combine_chunks().to_numpy(zero_copy_only=False).astype(np.int32)
         did = table["dim_id"].combine_chunks().to_numpy(zero_copy_only=False).astype(np.int32)
         ok = fitted.meta_i32[:, 4] >= 0
-        if rule:
+        if "regressors" in info:
+            res = self._predict_regressors(ctx, opts, info, fitted, future, floor, cap, sid, did, ok, want_intervals)
+        elif rule:
             res, sums = batched.predict_sums_host(ctx, opts, fitted, future, floor, cap, rule[0], rule[1],
                                                   seed=int(fc.get("seed", 0)), intervals=want_intervals)
             self.aggregates = aggregate_table(sid, did, ok, sums)
@@ -386,6 +488,26 @@ class _ForecastTimeSeriesOp:
         if not ok.all():
             out = out.filter(pa.array(np.repeat(ok, periods)))
         return out
+
+    def _predict_regressors(self, ctx, opts, info, fitted, future, floor, cap, sid, did, ok, intervals):
+        """Point forecasts (and intervals) of version-4 models: io.future_regressors joined onto the grids on the GPU,
+        then pb200_predict_regressors_device with each record's (mu, std); the result on the host."""
+        import torch
+        torch.cuda.set_device(ctx.device)
+        dev = torch.device("cuda", ctx.device)
+        names = [r["name"] for r in info["regressors"]]
+        tab = read_future_regressors(self.config["io"]["future_regressors"], names, sid)
+        fut = torch.from_numpy(np.ascontiguousarray(future)).to(dev)
+        freg = future_regressor_values(ctx, tab, names, sid, did, fut, ok)
+        fd = batched.FittedBatch(*(torch.from_numpy(np.ascontiguousarray(x)).to(dev) for x in (
+            fitted.params, fitted.tchange, fitted.meta_i32, fitted.meta_i64, fitted.meta_f64)), fitted.smax, fitted.kmax,
+            reg_scale=torch.from_numpy(np.ascontiguousarray(fitted.reg_scale)).to(dev))
+        res = batched.predict_batch_device(ctx, opts, fd, fut, torch.from_numpy(floor).to(dev),
+                                           torch.from_numpy(cap).to(dev), seed=int(self.config["forecast"].get("seed", 0)),
+                                           intervals=intervals, regressors=freg)
+        host = lambda t: None if t is None else t.cpu().numpy()  # noqa: E731
+        return batched.ForecastBatch(future, host(res.yhat), host(res.yhat_lower), host(res.yhat_upper),
+                                     host(res.yhat_int))
 
     def __call__(self, pdf):
         tbl = pa.Table.from_pandas(pdf, preserve_index=False)

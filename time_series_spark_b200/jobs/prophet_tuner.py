@@ -8,7 +8,7 @@ that pair.  A group with no eligible grid point (a failed cutoff fit, or a score
 with a zero) keeps the ``model.*`` prior scales.  All of it is one batched GPU job (batched.tune_device; DESIGN §10).
 
 Keys: ``io.input``, ``model.*`` as the modeler, but for a seasonality table (``model.seasonalities`` or an int order
-for a built-in, which raises: per-series prior scales are not available for tables); ``backtest.horizon`` / ``period`` / ``initial`` as the backtest; and
+for a built-in, which raises: per-series prior scales are not available for tables; ``model.regressors`` raises too); ``backtest.horizon`` / ``period`` / ``initial`` as the backtest; and
 ``tune.*``:
   changepoint_prior_scale   list of values > 0, default [0.001, 0.01, 0.1, 0.5]
   seasonality_prior_scale   list of values > 0, default [0.01, 0.1, 1.0, 10.0]
@@ -36,7 +36,7 @@ from .. import dist as pdist
 from ..pack import pack_groups_cuda
 from .prophet_backtest import backtest_spec_from_config
 from .prophet_modeler import (MODEL_OUTPUT_SCHEMA, ProphetModeler, get_context, models_table, options_from_config,
-                              table_keys, who)
+                              regressor_names, table_keys, who)
 
 # fbprophet's documentation: "Hyperparameter tuning"
 DEFAULT_CHANGEPOINT_PRIOR_SCALES = (0.001, 0.01, 0.1, 0.5)
@@ -117,6 +117,9 @@ class ProphetTuner:
         floor = self.config["model"]["floor"]
         cap_multiplier = float(self.config["model"]["cap_multiplier"])
         opts = options_from_config(self.config)
+        if regressor_names(self.config):
+            raise ValueError("model.regressors: the tuner fits every grid point with per-series prior scales, which a "
+                             "model with extra regressors does not take; fit it with the modeler")
         if batched.is_table(opts):
             raise ValueError(f"{' / '.join(table_keys(self.config))}: the tuner fits every grid point with per-series "
                              "prior scales, which a model with a seasonality table does not take; tune the default "

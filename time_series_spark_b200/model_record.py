@@ -21,6 +21,15 @@ the table mask, bit j = entry j of the normalised table active), followed by the
 Options without a table, and a table that restates the default model, write version 1.  Every record of a table
 has one version, and the version-2 records of a table one seasonality table.
 
+Version 4 is the record of a model with extra regressors (DESIGN §20; version 3 was never written): the version-1
+fields, each series' standardisation, then the bytes every record of the fit shares -- the table tail of version 2
+(always present; it may restate the defaults) and the regressors as they were given:
+
+    | f64[16][2] reg_scale (mu, std of regressor r; unused slots 0)
+    | i32[3] built-in orders | i32 entry count | 8 x seasonality entry          (as version 2)
+    | f64 holidays_prior_scale | i32 regressor count
+    | 16 x (name[16] NUL-padded | f64 prior_scale (0 = holidays_prior_scale) | i32 standardize (-1 auto, 0, 1))
+
 Encoding / decoding is vectorised over the whole batch (one numpy structured array),
 never a per-row Python loop.
 """
@@ -36,9 +45,11 @@ from .batched import FittedBatch
 MAGIC = b"PB2M"
 VERSION = 1
 VERSION_TABLE = 2
+VERSION_REGRESSORS = 4
 FLAG_LOGISTIC, FLAG_MULT = 1, 2
 _BUILTIN_KEYS = ("yearly_seasonality", "weekly_seasonality", "daily_seasonality")
 ENTRY_DTYPE = np.dtype([("name", "S16"), ("period", "<f8"), ("prior_scale", "<f8"), ("fourier_order", "<i4")])
+REGRESSOR_DTYPE = np.dtype([("name", "S16"), ("prior_scale", "<f8"), ("standardize", "<i4")])
 
 
 def record_dtype(smax: int, kmax: int, version: int = VERSION) -> np.dtype:
@@ -46,8 +57,12 @@ def record_dtype(smax: int, kmax: int, version: int = VERSION) -> np.dtype:
     fields = [("magic", "S4"), ("version", "<u2"), ("flags", "<u2"), ("smax", "<i4"), ("kmax", "<i4"),
               ("switches", "<i4", (4,)), ("meta_i32", "<i4", (8,)), ("meta_i64", "<i8", (2,)), ("last_ds", "<i8"),
               ("meta_f64", "<f8", (4,)), ("params", "<f8", (pstride,)), ("tchange", "<f8", (smax,))]
+    table = [("orders", "<i4", (3,)), ("n_entries", "<i4"), ("entries", ENTRY_DTYPE, (L.MAX_SEASONALITIES,))]
     if version == VERSION_TABLE:
-        fields += [("orders", "<i4", (3,)), ("n_entries", "<i4"), ("entries", ENTRY_DTYPE, (L.MAX_SEASONALITIES,))]
+        fields += table
+    elif version == VERSION_REGRESSORS:
+        fields = fields + [("reg_scale", "<f8", (L.MAX_REGRESSORS, 2))] + table + [
+            ("holidays_prior_scale", "<f8"), ("n_regressors", "<i4"), ("regressors", REGRESSOR_DTYPE, (L.MAX_REGRESSORS,))]
     elif version != VERSION:
         raise ValueError(f"unknown model record version {version}")
     return np.dtype(fields)
@@ -76,6 +91,29 @@ def _table_spec(opts) -> dict:
     return spec
 
 
+def _regressor_spec(opts) -> list:
+    """The regressors of pb200_options_v3 as make_regressor_options' ``regressors``."""
+    out = []
+    for i in range(opts.n_regressors):
+        e = opts.regressors[i]
+        d = {"name": e.name.decode()}
+        if e.prior_scale != 0.0:
+            d["prior_scale"] = float(e.prior_scale)
+        d["standardize"] = "auto" if e.standardize == L.STD_AUTO else bool(e.standardize)
+        out.append(d)
+    return out
+
+
+def regressor_options(info: dict, **kw):
+    """The options of a decoded version-4 record (``info["table"]``, ``info["regressors"]``,
+    ``info["holidays_prior_scale"]``) for make_table_options' other keyword arguments ``kw``: the fit's options."""
+    return batched.make_regressor_options(
+        regressors=info["regressors"], holidays_prior_scale=info["holidays_prior_scale"],
+        growth="logistic" if info["logistic"] else "linear",
+        seasonality_mode="multiplicative" if info["multiplicative"] else "additive",
+        n_changepoints=info["n_changepoints"], **info["table"], **kw)
+
+
 def table_options(info: dict, **kw):
     """The options of a decoded table (``info["table"]``) for make_table_options' other keyword arguments ``kw``
     (make_options'): the fit's seasonality table, layout and component names."""
@@ -92,18 +130,29 @@ def encode(fitted: FittedBatch, last_ds_ns: np.ndarray, opts) -> pa.Array:
     fitted = fitted.to_host()
     n = fitted.n
     table = batched.seasonality_table(opts)
-    version = VERSION if table is None else VERSION_TABLE
+    R = batched.n_regressors(opts)
+    version = VERSION if table is None else VERSION_REGRESSORS if R else VERSION_TABLE
     if table is not None:
         try:
             spec = _table_spec(opts)
-            rebuilt = batched.make_table_options(
-                growth="logistic" if logistic else "linear",
-                seasonality_mode="multiplicative" if multiplicative else "additive",
-                n_changepoints=opts.n_changepoints, seasonality_prior_scale=opts.seasonality_prior_scale, **spec)
+            kw = dict(growth="logistic" if logistic else "linear",
+                      seasonality_mode="multiplicative" if multiplicative else "additive",
+                      n_changepoints=opts.n_changepoints, seasonality_prior_scale=opts.seasonality_prior_scale, **spec)
+            if R:
+                rspec = _regressor_spec(opts)
+                rebuilt = batched.make_regressor_options(regressors=rspec,
+                                                         holidays_prior_scale=opts.holidays_prior_scale, **kw)
+            else:
+                rebuilt = batched.make_table_options(**kw)
         except ValueError as e:
             raise ValueError(f"these options have no model record: {e}") from None
         if batched.seasonality_table(rebuilt) != table:
             raise ValueError("these options have no model record: their seasonality table does not rebuild")
+        if R:
+            if fitted.reg_scale is None:
+                raise ValueError("a fit with regressors needs its reg_scale (FittedBatch.reg_scale) in the model record")
+            if np.shape(fitted.reg_scale) != (n, R, 2):
+                raise ValueError(f"the fitted batch's reg_scale has shape {np.shape(fitted.reg_scale)}, not ({n}, {R}, 2)")
         lay = L.get_layout(opts)
         if (lay.smax, lay.kmax) != (fitted.smax, fitted.kmax):
             raise ValueError(f"the fitted batch's layout (smax {fitted.smax}, kmax {fitted.kmax}) is not the options' "
@@ -126,6 +175,15 @@ def encode(fitted: FittedBatch, last_ds_ns: np.ndarray, opts) -> pa.Array:
             e = opts.seasonalities[i]
             ent[i] = (e.name, e.period, e.prior_scale, e.fourier_order)
         rec["entries"] = ent
+    if version == VERSION_REGRESSORS:
+        rec["reg_scale"][:, :R, :] = fitted.reg_scale
+        rec["holidays_prior_scale"] = opts.holidays_prior_scale
+        rec["n_regressors"] = R
+        regs = np.zeros(L.MAX_REGRESSORS, REGRESSOR_DTYPE)
+        for i in range(R):
+            e = opts.regressors[i]
+            regs[i] = (e.name, e.prior_scale, e.standardize)
+        rec["regressors"] = regs
     size = dt.itemsize
     offsets = pa.py_buffer((np.arange(n + 1, dtype=np.int64) * size).astype(np.int32).tobytes()) \
         if n * size < 2**31 else None
@@ -137,6 +195,7 @@ def encode(fitted: FittedBatch, last_ds_ns: np.ndarray, opts) -> pa.Array:
 
 
 _TABLE_TAIL = 16 + ENTRY_DTYPE.itemsize * L.MAX_SEASONALITIES     # orders, n_entries, entries: a v2 record's end
+_REG_TAIL = 12 + REGRESSOR_DTYPE.itemsize * L.MAX_REGRESSORS      # holidays_prior_scale, n_regressors, regressors
 
 
 def _column(col):
@@ -152,8 +211,8 @@ def _column(col):
 
 def _one_class(col):
     """(record offsets, data bytes, version) of a column whose records are one model class: a PB2M first record, every
-    record's version known and the same, and for version 2 one seasonality table.  Reads only the records' headers and
-    table bytes, whatever their layouts."""
+    record's version known and the same, for version 2 one seasonality table, and for version 4 one seasonality table
+    and one set of regressors.  Reads only the records' headers and shared tails, whatever their layouts."""
     n = len(col)
     if col[0].as_py()[:4] != MAGIC:
         raise ValueError("model blob is not a PB2M record (fbprophet pickles cannot be scored on this path)")
@@ -165,27 +224,36 @@ def _one_class(col):
     # every record's version, read before the record layout it decides
     raw = np.frombuffer(bufs[2], dtype=np.uint8)
     ver = raw[offs[:-1] + 4].astype(np.int64) | (raw[offs[:-1] + 5].astype(np.int64) << 8)
-    known = (ver == VERSION) | (ver == VERSION_TABLE)
+    known = (ver == VERSION) | (ver == VERSION_TABLE) | (ver == VERSION_REGRESSORS)
     if not known.all():
         raise ValueError(f"model record version {int(ver[~known][0])} is unknown to this library (it reads versions "
-                         f"{VERSION} and {VERSION_TABLE})")
+                         f"{VERSION}, {VERSION_TABLE} and {VERSION_REGRESSORS})")
     version = int(ver[0])
     if not np.all(ver == version):
+        if np.any(ver == VERSION_REGRESSORS):
+            raise ValueError("version-4 model records with records of another version in one table: models with and "
+                             "without extra regressors cannot be scored in one call")
         raise ValueError("version-1 and version-2 model records in one table: models without and with a seasonality "
                          "table cannot be scored in one call")
-    if version == VERSION_TABLE:
-        if np.any(np.diff(offs) < 16 + _TABLE_TAIL):
+    if version != VERSION:
+        reg = _REG_TAIL if version == VERSION_REGRESSORS else 0
+        if np.any(np.diff(offs) < 16 + _TABLE_TAIL + reg):
             raise ValueError("bad model record header")
-        tab = raw[(offs[1:] - _TABLE_TAIL)[:, None] + np.arange(_TABLE_TAIL)[None, :]]
+        tab = raw[(offs[1:] - reg - _TABLE_TAIL)[:, None] + np.arange(_TABLE_TAIL)[None, :]]
         if not np.all(tab == tab[0]):
             raise ValueError("model records with different seasonality tables in one table: each table's models are "
                              "scored with one set of options")
+        if reg:
+            regs = raw[(offs[1:] - reg)[:, None] + np.arange(reg)[None, :]]
+            if not np.all(regs == regs[0]):
+                raise ValueError("model records with different regressors in one table: each set of regressors' models "
+                                 "is scored with one set of options and one io.future_regressors layout")
     return offs, bufs, version
 
 
 def check_one_class(col) -> None:
-    """Refuse, as decode does, a models column that mixes version-1 and version-2 records or holds two seasonality
-    tables, without decoding the records: for callers that decode the column in shards (one per rank) but must agree
+    """Refuse, as decode does, a models column that mixes record versions or holds two seasonality tables or two sets
+    of regressors, without decoding the records: for callers that decode the column in shards (one per rank) but must agree
     on the model class of the whole table."""
     _one_class(_column(col))
 
@@ -193,7 +261,9 @@ def check_one_class(col) -> None:
 def decode(col) -> tuple:
     """Arrow binary column -> (FittedBatch, last_ds_ns, dict of the fit-time options).  Version-2 records add ``info["table"]``,
     the seasonality table as make_table_options' keyword arguments (``table_options`` rebuilds the fit's options from
-    it); version-1 records have no such key."""
+    it); version-1 records have no such key.  Version-4 records add the table too, ``info["regressors"]`` (make_regressor_options'
+    entries), ``info["holidays_prior_scale"]`` and the FittedBatch's ``reg_scale`` (``regressor_options`` rebuilds
+    the fit's options)."""
     col = _column(col)
     n = len(col)
     offs, bufs, version = _one_class(col)
@@ -214,7 +284,7 @@ def decode(col) -> tuple:
     sw = rec["switches"][0]
     info = {"logistic": bool(flags & FLAG_LOGISTIC), "multiplicative": bool(flags & FLAG_MULT),
             "yearly": int(sw[0]), "weekly": int(sw[1]), "daily": int(sw[2]), "n_changepoints": int(sw[3])}
-    if version == VERSION_TABLE:
+    if version in (VERSION_TABLE, VERSION_REGRESSORS):
         ne = int(rec["n_entries"][0])
         if not 0 <= ne <= L.MAX_SEASONALITIES:
             raise ValueError(f"bad model record: {ne} seasonality entries")
@@ -226,6 +296,17 @@ def decode(col) -> tuple:
                  **({"prior_scale": float(e["prior_scale"])} if e["prior_scale"] != 0.0 else {}))
             for e in rec["entries"][0][:ne]]
         info["table"] = table
+    if version == VERSION_REGRESSORS:
+        R = int(rec["n_regressors"][0])
+        if not 1 <= R <= L.MAX_REGRESSORS:
+            raise ValueError(f"bad model record: {R} regressors")
+        info["regressors"] = [
+            dict({"name": e["name"].decode()}, **({"prior_scale": float(e["prior_scale"])} if e["prior_scale"] != 0.0
+                                                  else {}),
+                 standardize="auto" if e["standardize"] == L.STD_AUTO else bool(e["standardize"]))
+            for e in rec["regressors"][0][:R]]
+        info["holidays_prior_scale"] = float(rec["holidays_prior_scale"][0])
+        fb.reg_scale = np.ascontiguousarray(rec["reg_scale"][:, :R, :])
     return fb, np.ascontiguousarray(rec["last_ds"]), info
 
 

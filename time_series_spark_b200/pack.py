@@ -24,6 +24,7 @@ class PackedGroups:
     y: np.ndarray            # [R] int32 (or float64 when the input was not integral)
     last_ds: np.ndarray      # [N] int64: max ds of the group INCLUDING null-y rows
     n_rows_in: np.ndarray    # [N] rows of the group before dropping nulls
+    regressors: object = None  # [R, rows] float64 CUDA tensor aligned with ds (pack_groups_cuda's reg_cols), else None
 
     @property
     def n(self) -> int:
@@ -33,7 +34,9 @@ class PackedGroups:
         """Groups [lo, hi) (a rank's shard; see dist.shard_bounds)."""
         a, b = int(self.offsets[lo]), int(self.offsets[hi])
         return PackedGroups(self.series_id[lo:hi], self.dim_id[lo:hi], self.offsets[lo:hi + 1] - a,
-                            self.ds[a:b], self.y[a:b], self.last_ds[lo:hi], self.n_rows_in[lo:hi])
+                            self.ds[a:b], None if self.y is None else self.y[a:b], self.last_ds[lo:hi],
+                            self.n_rows_in[lo:hi],
+                            None if self.regressors is None else self.regressors[:, a:b].contiguous())
 
     @property
     def on_device(self) -> bool:
@@ -187,16 +190,26 @@ def _device_column(col, arrow_type, dev):
     return out
 
 
-def pack_groups_cuda(table: pa.Table, device=None, keys=("series_id", "dim_id"), ds_col="ds", y_col="y"):
+def pack_groups_cuda(table: pa.Table, device=None, keys=("series_id", "dim_id"), ds_col="ds", y_col="y", reg_cols=()):
     """GPU version of :func:`pack_groups` (SURVEY 8f-2): the columns go to HBM as they are (32-bit ids and y, 64-bit
     ds), the sort key is formed there and the (series_id, dim_id, ds) sort of the whole frame runs on the GPU as two
     stable radix sorts (``torch.sort`` -- plumbing, not a hand-written kernel; skipped when the frame already is in
     that order, as a hive-partitioned input written per series is).  ``ds`` / ``y`` stay resident in HBM for
     ``pb200_fit_device``.  Returns a PackedGroups whose ``ds`` / ``y`` are CUDA tensors; ids, offsets and last_ds are
-    host numpy arrays.  Null ``y`` rows are dropped exactly as on the host path."""
+    host numpy arrays.  Null ``y`` rows are dropped exactly as on the host path.
+
+    ``reg_cols``: the extra regressors' columns (DESIGN §20), carried as one float64 ``[R, rows]`` tensor
+    (``regressors``) through the same permutation and the same null-y row drop; a null value becomes NaN.
+    ``y_col=None`` packs a table without y (the scorer's future regressor values): no y, no row dropped."""
     import torch
     if table.num_rows == 0:
-        return pack_groups(table, keys, ds_col, y_col, pin=False)
+        pk = pack_groups(table, keys, ds_col, y_col, pin=False)
+        if reg_cols:
+            pk.regressors = torch.zeros((len(reg_cols), 0), dtype=torch.float64,
+                                        device=torch.device("cuda", torch.cuda.current_device()) if device is None else device)
+        if y_col is None:
+            pk.y = None
+        return pk
     dev = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
     if dev.index is None:
         dev = torch.device("cuda", torch.cuda.current_device())
@@ -210,10 +223,10 @@ def pack_groups_cuda(table: pa.Table, device=None, keys=("series_id", "dim_id"),
         if table[k].null_count:
             raise ValueError(f"group key column {k!r} holds {table[k].null_count} null value(s); every row needs both "
                              f"{keys[0]!r} and {keys[1]!r}")
-    ycol = table[y_col]
-    integral = pa.types.is_integer(ycol.type)
+    ycol = table[y_col] if y_col is not None else None
+    integral = ycol is not None and pa.types.is_integer(ycol.type)
     y_null = None
-    if ycol.null_count:
+    if ycol is not None and ycol.null_count:
         y_null = np.asarray(ycol.combine_chunks().is_null().to_numpy(zero_copy_only=False))
         ycol = pc.fill_null(ycol, 0)
     ds_t = _device_column(ds_arr, pa.int64(), dev)
@@ -221,8 +234,14 @@ def pack_groups_cuda(table: pa.Table, device=None, keys=("series_id", "dim_id"),
         ds_t *= mult                                       # timestamp[s|ms|us] -> ns, on the device
     k0 = _device_column(table[keys[0]], pa.int32(), dev)
     k1 = _device_column(table[keys[1]], pa.int32(), dev)
-    y_t = _device_column(ycol, pa.int32() if integral else pa.float64(), dev)
-    if not integral:
+    y_t = _device_column(ycol, pa.int32() if integral else pa.float64(), dev) if ycol is not None else None
+    reg = None
+    if reg_cols:
+        reg = torch.empty((len(reg_cols), ds_t.numel()), dtype=torch.float64, device=dev)
+        for r, name in enumerate(reg_cols):
+            col = pc.fill_null(pc.cast(table[name], pa.float64()), float("nan"))
+            reg[r] = _device_column(col, pa.float64(), dev)
+    if ycol is not None and not integral:
         nan = torch.isnan(y_t)
         if bool(nan.any()):
             nan_h = nan.cpu().numpy()
@@ -237,7 +256,11 @@ def pack_groups_cuda(table: pa.Table, device=None, keys=("series_id", "dim_id"),
         i1 = torch.argsort(ds_t, stable=True)
         i2 = torch.argsort(key[i1], stable=True)
         order = i1[i2]
-        key, ds_t, y_t = key[order], ds_t[order], y_t[order]
+        key, ds_t = key[order], ds_t[order]
+        if y_t is not None:
+            y_t = y_t[order]
+        if reg is not None:
+            reg = reg[:, order]
     new_grp = torch.ones(key.numel(), dtype=torch.bool, device=dev)
     new_grp[1:] = key[1:] != key[:-1]
     starts = torch.nonzero(new_grp).flatten()
@@ -253,8 +276,11 @@ def pack_groups_cuda(table: pa.Table, device=None, keys=("series_id", "dim_id"),
         grp_id = torch.cumsum(new_grp.to(torch.int64), 0) - 1
         counts = torch.bincount(grp_id[keep], minlength=starts.numel()).cpu().numpy().astype(np.int64)
         ds_t, y_t = ds_t[keep].contiguous(), y_t[keep].contiguous()
+        if reg is not None:
+            reg = reg[:, keep]
     else:
         counts = n_rows_in
     offsets = np.zeros(sid.size + 1, np.int64)
     np.cumsum(counts, out=offsets[1:])
-    return PackedGroups(sid, did, offsets, ds_t.contiguous(), y_t.contiguous(), last_ds.astype(np.int64), n_rows_in)
+    return PackedGroups(sid, did, offsets, ds_t.contiguous(), None if y_t is None else y_t.contiguous(),
+                        last_ds.astype(np.int64), n_rows_in, None if reg is None else reg.contiguous())
