@@ -89,6 +89,16 @@ int env_int(const char* name, int dflt) {
     return v && *v ? atoi(v) : dflt;
 }
 
+// the arrays the *_host entry points stage on the device (Staging), one growth-only buffer per role: repeated identical
+// calls allocate nothing after the first
+enum StageRole {
+    ST_DS, ST_Y, ST_REG, ST_REGSC, ST_CAP, ST_PRIOR, ST_IPARAMS, ST_IMETA, ST_WARM, ST_THETA, ST_GRAD, ST_TRACE,   // fit inputs
+    ST_PARAMS, ST_TCHANGE, ST_MI32, ST_MI64, ST_MF64,   // the model records
+    ST_FUT, ST_FLOOR,                                   // predict inputs (ST_FUT: the predicted rows' ds)
+    ST_YHAT, ST_LO, ST_HI, ST_YINT, ST_COMP, ST_TLO, ST_THI, ST_SUMS, ST_QUANT,   // predict outputs
+    N_STAGE
+};
+
 }  // namespace
 
 struct pb200_ctx {
@@ -105,24 +115,15 @@ struct pb200_ctx {
     DevBuf d_planes;                // fit kernels' per-series workspace (one slice per resident CTA / series slot)
     HostBuf h_ctl;                  // pinned staging for offsets / order / lenclass
     DevBuf d_vcount;                // series of the last fit call per kernel variant x seasonality class
-    // data staging for the *_host entry points
-    DevBuf d_ds, d_y, d_cap, d_params, d_tchange, d_mi32, d_mi64, d_mf64;
-    DevBuf d_fut, d_floor, d_yhat, d_lo, d_hi, d_yint;
-    DevBuf d_comp, d_tlo, d_thi;   // staging of pb200_predict_components_host's planes and trend bounds
-    DevBuf d_mc;     // MC workspace
-    DevBuf d_sums;   // staging of pb200_predict_sums_host's window outputs
-    DevBuf d_quant;  // staging of pb200_predict_quantiles_host's planes
-    DevBuf d_hoff;   // device copy of pb200_predict_history_*'s frame offsets
+    DevBuf d_warm_x;                // warm start points of pb200_fit_warm_* (prep_kernel -> fit kernels, Newton retry)
     DevBuf d_regbad;                // regressor fits: series with a non-finite regressor value (reg_scale_kernel -> prep_kernel)
-    DevBuf d_reg, d_regsc;          // staging of the regressor entry points' values and (mu, std)
+    DevBuf d_hoff;                  // device copy of pb200_predict_history_*'s frame offsets
+    DevBuf stage[N_STAGE];          // the *_host entry points' arrays, by StageRole
     int lc0_max = 1 << 30; // PB200_LC0_MAX: longest series on one warp per series, longer ones get four (unset: no limit)
     bool lc_auto = true;   // false when PB200_LC0_MAX pins the CTA width
     bool tab_on = true;    // PB200_NO_TAB=1 disables the seasonal-table variants (A/B runs)
     int grp_g = -1;        // lanes per series of the grouped day-table kernel (fit_group.cuh); PB200_GROUP=0|8|16 pins it
                            // (0 = point_pass_tab), unset = by batch size: 8 from grp_min series on, 16 below
-    DevBuf d_trace;        // trajectory rows of pb200_fit_trace_host
-    DevBuf d_warm_x;       // warm start points of pb200_fit_warm_* (prep_kernel -> fit kernels, Newton retry)
-    DevBuf d_prior, d_iparams, d_imeta, d_warm;   // staging of pb200_fit_warm_host's prior scales, previous models, warm codes
     int plain_grp = 0;     // PB200_PLAIN_GROUP=1: the class WITHOUT seasonality (regular grid; reference config #4) on the grouped kernel
                            // too.  Off: it beat one warp per series only at the largest batches measured (500k short series) --
                            // its rounds are longer, and small batches are latency bound
@@ -382,6 +383,76 @@ int mask_k(int m) { return ((m & 1) ? 20 : 0) + ((m & 2) ? 6 : 0) + ((m & 4) ? 8
 
 size_t y_elem(int dt) { return dt == PB200_Y_F64 ? 8 : 4; }
 
+// The staging of one *_host call on the context's stream.  in() copies a host array into its role's buffer; out() makes
+// room for an output (zeroed on the device when asked) and records its copy back; finish() enqueues the recorded copies
+// and synchronises once.  A null host array stages nothing and gives a null device pointer, a count of 0 copies nothing.
+// The first CUDA error is kept and every later step skips: status() reports it before the device body runs.
+struct Staging {
+    struct Copy { void* h; const void* d; size_t bytes; };
+    pb200_ctx* c;
+    cudaError_t err;
+    std::vector<Copy> outs;
+
+    explicit Staging(pb200_ctx* ctx) : c(ctx), err(cudaSetDevice(ctx->device)) {}
+    void* reserve(StageRole role, size_t bytes) {
+        if (err == cudaSuccess) err = c->stage[role].reserve(bytes);
+        return err == cudaSuccess ? c->stage[role].p : nullptr;
+    }
+    template <class T> T* in(StageRole role, const T* h, size_t n) {
+        if (!h) return nullptr;
+        T* d = (T*)reserve(role, n * sizeof(T));
+        if (n && err == cudaSuccess) err = cudaMemcpyAsync(d, h, n * sizeof(T), cudaMemcpyHostToDevice, c->stream);
+        return d;
+    }
+    template <class T> T* out(StageRole role, T* h, size_t n, bool zero = false) {
+        if (!h) return nullptr;
+        T* d = (T*)reserve(role, n * sizeof(T));
+        if (zero && n && err == cudaSuccess) err = cudaMemsetAsync(d, 0, n * sizeof(T), c->stream);
+        later(h, d, n);
+        return d;
+    }
+    template <class T> void later(T* h, const T* d, size_t n) {
+        if (n) outs.push_back({h, d, n * sizeof(T)});
+    }
+    int status() const { return err == cudaSuccess ? PB200_OK : fail(PB200_E_CUDA, "staging of the host arrays", err); }
+    int finish() {
+        for (const Copy& o : outs)
+            if (err == cudaSuccess) err = cudaMemcpyAsync(o.h, o.d, o.bytes, cudaMemcpyDeviceToHost, c->stream);
+        if (err == cudaSuccess) err = cudaStreamSynchronize(c->stream);
+        return status();
+    }
+};
+
+// One fit request (fit_impl): device arrays, or host arrays in fit_host / objective_host.  The leading members are the
+// arguments every fit entry point takes, in their order; the others are optional.  offsets is always a host array.
+struct FitCall {
+    const pb200_options* opts;
+    const int64_t* ds;
+    const void* y;
+    int32_t y_dtype;
+    const int64_t* offsets;
+    int64_t n_series;
+    double floor, cap_multiplier;
+    const double* cap;
+    double* params;
+    double* tchange;
+    int32_t* meta_i32;
+    int64_t* meta_i64;
+    double* meta_f64;
+    const double* prior = nullptr;         // per-series prior scales [n_series][2]; null: the options'
+    const double* init_params = nullptr;   // warm start: the previous models (pb200_fit_warm_*), their meta and codes
+    const int32_t* init_meta = nullptr;
+    int32_t* warm = nullptr;
+    const double* theta = nullptr;         // an objective evaluation: -log p and its gradient at theta, no fit
+    double* grad = nullptr;
+    double* trace = nullptr;               // trace_cap trajectory rows per series
+    int32_t trace_cap = 0;
+    bool regs = false;                     // a regressor entry point: the options may carry regressors
+    const double* reg = nullptr;           // their values [R][rows] and (mu, std) [n_series][R][2]
+    double* reg_scale = nullptr;
+    const double* reg_scale_copy = nullptr;   // pb200_fit_regressors_copy_device's scales
+};
+
 }  // namespace
 
 extern "C" {
@@ -482,11 +553,10 @@ PB200_API void pb200_destroy(pb200_ctx* c) {
     if (!c) return;
     cudaSetDevice(c->device);
     cudaStreamSynchronize(c->stream);
-    for (DevBuf* b : {&c->d_ds, &c->d_y, &c->d_cap, &c->d_params, &c->d_tchange, &c->d_mi32, &c->d_mi64, &c->d_mf64, &c->d_fut,
-                      &c->d_floor, &c->d_yhat, &c->d_lo, &c->d_hi, &c->d_yint, &c->d_comp, &c->d_tlo, &c->d_thi, &c->d_mc, &c->d_sums, &c->d_trace, &c->d_warm_x, &c->d_prior, &c->d_iparams, &c->d_imeta, &c->d_warm, &c->d_vcount, &c->d_offsets,
-                      &c->d_order, &c->d_lenclass, &c->d_qitems, &c->d_qctl, &c->d_nq, &c->d_planes, &c->d_qkey, &c->d_qhist,
-                      &c->d_regbad, &c->d_reg, &c->d_regsc})
+    for (DevBuf* b : {&c->d_offsets, &c->d_order, &c->d_lenclass, &c->d_qitems, &c->d_qctl, &c->d_qkey, &c->d_qhist,
+                      &c->d_nq, &c->d_planes, &c->d_vcount, &c->d_warm_x, &c->d_regbad, &c->d_hoff})
         b->release();
+    for (DevBuf& b : c->stage) b.release();
     c->h_ctl.release();
     cudaEventDestroy(c->ctl_ev);
     cudaStreamDestroy(c->stream);
@@ -542,41 +612,40 @@ PB200_API int pb200_synchronize(pb200_ctx* c) {
 }  // extern "C"
 
 // newton_kernel over the queue {count, head, items...} at d_nq (16-warp CTAs with up to ~113 KB of shared memory, at P = 67)
-static int launch_newton(pb200_ctx* c, const pb200_options* opts, const int64_t* d_ds, const void* d_y,
-                         int32_t y_dtype, const int64_t* d_offsets, int64_t n_series, int* d_nq, const double* d_prior,
-                         const double* d_x0, double* d_params, double* d_tchange, int32_t* d_meta_i32, int64_t* d_meta_i64, double* d_meta_f64,
-                         const double* d_reg, const double* d_reg_scale, int64_t n_rows) {
+// (f's series, offsets and queue as fit_impl staged them; x0: the warm start points, or null)
+static int launch_newton(pb200_ctx* c, const FitCall& f, const double* x0) {
     static_assert(pb200::SEAS_PMAX <= pb200::nw::NW_PMAX, "newton_kernel holds every P check_opts admits");
     pb200_layout L;
-    pb200_get_layout(opts, &L);
-    if (opts->algorithm == PB200_ALG_LBFGS) return PB200_OK;
+    pb200_get_layout(f.opts, &L);
+    if (f.opts->algorithm == PB200_ALG_LBFGS) return PB200_OK;
+    int* nq = (int*)c->d_nq.p;
     pb200::nw::NewtonArgs na;
-    na.ds = (const long long*)d_ds;
-    na.y = d_y;
-    na.y_dtype = y_dtype;
-    na.offsets = (const long long*)d_offsets;
-    na.nq_count = d_nq;
-    na.nq_head = d_nq + 1;
-    na.nq_items = d_nq + 2;
-    na.params = d_params;
-    na.tchange = d_tchange;
-    na.meta_i32 = d_meta_i32;
-    na.meta_i64 = (const long long*)d_meta_i64;
-    na.meta_f64 = d_meta_f64;
+    na.ds = (const long long*)f.ds;
+    na.y = f.y;
+    na.y_dtype = f.y_dtype;
+    na.offsets = (const long long*)c->d_offsets.p;
+    na.nq_count = nq;
+    na.nq_head = nq + 1;
+    na.nq_items = nq + 2;
+    na.params = f.params;
+    na.tchange = f.tchange;
+    na.meta_i32 = f.meta_i32;
+    na.meta_i64 = (const long long*)f.meta_i64;
+    na.meta_f64 = f.meta_f64;
     na.smax = L.smax;
     na.kmax = L.kmax;
     na.pstride = L.pstride;
-    na.prior = d_prior;
-    na.x0 = d_x0;
-    na.o = to_dev(opts);
-    opts_table(opts, &na.tab);
-    opts_reg(opts, &na.reg);
-    na.reg_x = d_reg;
-    na.reg_scale = d_reg_scale;
-    na.n_rows = n_rows;
+    na.prior = f.prior;
+    na.x0 = x0;
+    na.o = to_dev(f.opts);
+    opts_table(f.opts, &na.tab);
+    opts_reg(f.opts, &na.reg);
+    na.reg_x = f.reg;
+    na.reg_scale = f.reg_scale;
+    na.n_rows = f.offsets[f.n_series];
     const size_t nsm = pb200::nw::newton_smem_bytes(L.pstride);
     CK(cudaFuncSetAttribute(pb200::nw::newton_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)nsm));
-    int ngrid = (int)std::min<int64_t>(n_series, opts->algorithm == PB200_ALG_NEWTON ? (int64_t)c->sms * 2 : (int64_t)c->sms);
+    int ngrid = (int)std::min<int64_t>(f.n_series, f.opts->algorithm == PB200_ALG_NEWTON ? (int64_t)c->sms * 2 : (int64_t)c->sms);
     if (c->grid_max > 0) ngrid = std::min(ngrid, c->grid_max);
     pb200::nw::newton_kernel<<<ngrid, 32 * pb200::nw::NW_WARPS, nsm, c->stream>>>(na);
     CK(cudaGetLastError());
@@ -585,44 +654,36 @@ static int launch_newton(pb200_ctx* c, const pb200_options* opts, const int64_t*
 }
 
 // every fit call: zeroes the variant counters, then queues, fit kernels and (unless this is an objective evaluation,
-// d_grad_out set) the Newton retry on the context's stream.  d_prior: per-series prior scales, or null for the options'.
-// d_init_params / d_init_meta: previous models to start from (pb200_fit_warm_device), or null
-static int fit_impl(pb200_ctx* c, const pb200_options* opts, const int64_t* d_ds, const void* d_y, int32_t y_dtype,
-                    const int64_t* h_offsets, int64_t n_series, double floor, double cap_multiplier,
-                    const double* d_cap, const double* d_prior, double* d_params, double* d_tchange, int32_t* d_meta_i32,
-                    int64_t* d_meta_i64, double* d_meta_f64, const double* d_theta_in, double* d_grad_out,
-                    double* d_trace = nullptr, int trace_cap = 0, const double* d_init_params = nullptr,
-                    const int32_t* d_init_meta = nullptr, int32_t* d_warm = nullptr, bool regs = false,
-                    const double* d_reg = nullptr, double* d_reg_scale = nullptr,
-                    const double* d_reg_scale_copy = nullptr) {
+// f.grad set) the Newton retry on the context's stream
+static int fit_impl(pb200_ctx* c, const FitCall& f) {
     if (!c) return fail(PB200_E_ARG, "ctx is null");
     CK(cudaSetDevice(c->device));
     CK(c->d_vcount.reserve((NQ + 1) * 4));     // [NQ]: the table class
     CK(cudaMemsetAsync(c->d_vcount.p, 0, (NQ + 1) * 4, c->stream));
-    int rc = check_opts(opts, regs);
+    int rc = check_opts(f.opts, f.regs);
     if (rc) return rc;
     pb200::SeasTab tab;
-    opts_table(opts, &tab);
+    opts_table(f.opts, &tab);
     pb200::RegSpec reg;
-    opts_reg(opts, &reg);
+    opts_reg(f.opts, &reg);
     const bool tabcls = tab.n > 0 || reg.R > 0;     // the table class (fit_table.cu)
     if (tabcls) {
-        if (d_prior) return fail(PB200_E_UNSUPPORTED, "per-series prior scales are not supported with a seasonality table");
-        if (d_init_params) return fail(PB200_E_UNSUPPORTED, "warm start is not supported with a seasonality table");
+        if (f.prior) return fail(PB200_E_UNSUPPORTED, "per-series prior scales are not supported with a seasonality table");
+        if (f.init_params) return fail(PB200_E_UNSUPPORTED, "warm start is not supported with a seasonality table");
     }
     const int NQT = NLC * NQ + 1;    // the work queues: (length class, variant, mask), then the table class
-    if (n_series < 0 || n_series > (1LL << 30)) return fail(PB200_E_ARG, "n_series");
-    if (n_series == 0) return PB200_OK;
-    if (!d_ds || !d_y || !h_offsets || !d_params || !d_tchange || !d_meta_i32 || !d_meta_i64 || !d_meta_f64)
+    if (f.n_series < 0 || f.n_series > (1LL << 30)) return fail(PB200_E_ARG, "n_series");
+    if (f.n_series == 0) return PB200_OK;
+    if (!f.ds || !f.y || !f.offsets || !f.params || !f.tchange || !f.meta_i32 || !f.meta_i64 || !f.meta_f64)
         return fail(PB200_E_ARG, "null pointer");
-    if (y_dtype < 0 || y_dtype > 2) return fail(PB200_E_ARG, "y_dtype");
-    if (d_init_params && !d_init_meta) return fail(PB200_E_ARG, "d_init_meta_i32 is null");
-    if (reg.R > 0 && (!d_reg || !d_reg_scale)) return fail(PB200_E_ARG, "null pointer (regressors / reg_scale)");
+    if (f.y_dtype < 0 || f.y_dtype > 2) return fail(PB200_E_ARG, "y_dtype");
+    if (f.init_params && !f.init_meta) return fail(PB200_E_ARG, "d_init_meta_i32 is null");
+    if (reg.R > 0 && (!f.reg || !f.reg_scale)) return fail(PB200_E_ARG, "null pointer (regressors / reg_scale)");
     pb200_layout L;
-    pb200_get_layout(opts, &L);
-    const int N = (int)n_series;
+    pb200_get_layout(f.opts, &L);
+    const int N = (int)f.n_series;
     const double* warm_x = nullptr;     // the start points prep_kernel writes for the fit kernels and the Newton retry
-    if (d_init_params) {
+    if (f.init_params) {
         CK(c->d_warm_x.reserve((size_t)N * L.pstride * 8));
         warm_x = (const double*)c->d_warm_x.p;
     }
@@ -637,7 +698,7 @@ static int fit_impl(pb200_ctx* c, const pb200_options* opts, const int64_t* d_ds
     int64_t* ho = (int64_t*)c->h_ctl.p;
     int* horder = (int*)(ho + N + 1);
     int* hlc = horder + N;
-    memcpy(ho, h_offsets, (size_t)(N + 1) * 8);
+    memcpy(ho, f.offsets, (size_t)(N + 1) * 8);
     int lc_n[NLC] = {0, 0}, lc_tmax[NLC] = {0, 0};
     int64_t tmax_all = 0;
     for (int i = 0; i < N; ++i) {
@@ -683,8 +744,8 @@ static int fit_impl(pb200_ctx* c, const pb200_options* opts, const int64_t* d_ds
     CK(cudaEventRecord(c->ctl_ev, c->stream));
     c->ctl_pending = true;
     CK(cudaMemsetAsync(c->d_qctl.p, 0, (size_t)NQT * 2 * 4, c->stream));
-    CK(cudaMemsetAsync(d_params, 0, (size_t)N * L.pstride * 8, c->stream));
-    CK(cudaMemsetAsync(d_tchange, 0, (size_t)N * L.smax * 8, c->stream));
+    CK(cudaMemsetAsync(f.params, 0, (size_t)N * L.pstride * 8, c->stream));
+    CK(cudaMemsetAsync(f.tchange, 0, (size_t)N * L.smax * 8, c->stream));
     int* q_count = (int*)c->d_qctl.p;
     int* q_head = q_count + NQT;
     const int64_t n_rows = ho[N];
@@ -692,37 +753,37 @@ static int fit_impl(pb200_ctx* c, const pb200_options* opts, const int64_t* d_ds
     if (reg.R > 0) {
         CK(c->d_regbad.reserve((size_t)N));
         pb200::RegScaleArgs ra;
-        ra.reg = d_reg;
+        ra.reg = f.reg;
         ra.n_rows = n_rows;
         ra.offsets = (const long long*)c->d_offsets.p;
         ra.n_series = N;
         ra.spec = reg;
-        ra.reg_scale = d_reg_scale;
+        ra.reg_scale = f.reg_scale;
         ra.bad = (unsigned char*)c->d_regbad.p;
-        ra.scale_copy = d_reg_scale_copy;
+        ra.scale_copy = f.reg_scale_copy;
         pb200::reg_scale_kernel<<<std::min((N + 7) / 8, c->sms * 8), 256, 0, c->stream>>>(ra);
         CK(cudaGetLastError());
         c->launches++;
     }
 
-    const FitOptsDev od = to_dev(opts);
+    const FitOptsDev od = to_dev(f.opts);
     // lanes per series of the grouped day-table kernel
     const int grp_g = !c->tab_on ? 0 : (c->grp_g >= 0 ? c->grp_g : (N >= c->grp_min ? 8 : 16));
     // ---- prep kernel ----
     {
         pb200::PrepArgs pa;
-        pa.ds = (const long long*)d_ds;
-        pa.y = d_y;
-        pa.y_dtype = y_dtype;
+        pa.ds = (const long long*)f.ds;
+        pa.y = f.y;
+        pa.y_dtype = f.y_dtype;
         pa.offsets = (const long long*)c->d_offsets.p;
         pa.order = (const int*)c->d_order.p;
-        pa.cap = d_cap;
-        pa.floor = floor;
-        pa.cap_multiplier = cap_multiplier;
+        pa.cap = f.cap;
+        pa.floor = f.floor;
+        pa.cap_multiplier = f.cap_multiplier;
         pa.n_series = N;
-        pa.meta_i32 = d_meta_i32;
-        pa.meta_i64 = (long long*)d_meta_i64;
-        pa.meta_f64 = d_meta_f64;
+        pa.meta_i32 = f.meta_i32;
+        pa.meta_i64 = (long long*)f.meta_i64;
+        pa.meta_f64 = f.meta_f64;
         pa.lenclass = (const int*)c->d_lenclass.p;
         pa.q_items = (int*)c->d_qitems.p;
         pa.q_count = q_count;
@@ -733,17 +794,17 @@ static int fit_impl(pb200_ctx* c, const pb200_options* opts, const int64_t* d_ds
         pa.grp_g = grp_g;
         pa.grp_plain = (c->plain_grp && grp_g > 0) ? 1 : 0;
         pa.cv_weight = QKEY_CV_WEIGHT;
-        pa.newton_only = (opts->algorithm == PB200_ALG_NEWTON && !d_grad_out) ? 1 : 0;
+        pa.newton_only = (f.opts->algorithm == PB200_ALG_NEWTON && !f.grad) ? 1 : 0;
         pa.nq_count = nq;
         pa.nq_items = nq + 2;
         pa.vcount = (int*)c->d_vcount.p;
         pa.qkey = (int*)c->d_qkey.p;
         pa.qhist = (int*)c->d_qhist.p;
-        pa.prior = d_prior;
-        pa.init_params = d_init_params;
-        pa.init_meta = d_init_meta;
+        pa.prior = f.prior;
+        pa.init_params = f.init_params;
+        pa.init_meta = f.init_meta;
         pa.warm_x = (double*)warm_x;
-        pa.warm = d_warm;
+        pa.warm = f.warm;
         pa.smax = L.smax;
         pa.pstride = L.pstride;
         pa.tab = tab;
@@ -778,7 +839,7 @@ static int fit_impl(pb200_ctx* c, const pb200_options* opts, const int64_t* d_ds
             if (reg && mask == 0 && !plain_grp) continue;                // no Fourier features: nothing to regenerate
             if (reg >= 2 && ((mask != 6 && !plain_grp) || LC_NT[lc] != 32 || !c->tab_on)) continue;   // seasonal-table variants
             auto impossible = [&](int bit, int sw) { return (sw == 0 && (mask & bit)) || (sw == 1 && !(mask & bit)); };
-            if (impossible(1, opts->yearly) || impossible(2, opts->weekly) || impossible(4, opts->daily)) continue;
+            if (impossible(1, f.opts->yearly) || impossible(2, f.opts->weekly) || impossible(4, f.opts->daily)) continue;
             const int NT = LC_NT[lc];
             const int chunk = std::max((lc_tmax[lc] + NT - 1) / NT, 1);
             g.Tp = ((lc_tmax[lc] + chunk + pb200::TAB_CHUNK_SLACK + 1 + 7) / 8) * 8;   // the table variants may widen a chunk
@@ -795,7 +856,7 @@ static int fit_impl(pb200_ctx* c, const pb200_options* opts, const int64_t* d_ds
             if (reg == 3 && grp_g > 0) {
                 // grouped day-table kernel: one warp per CTA, 32 / grp_g series per warp, one workspace slot per series
                 const int nser = 32 / grp_g;
-                CK(pb200::launch_fit_group(grp_g, opts->growth, opts->multiplicative ? 1 : 0, mask != 0, dummy, 0, c->stream, &occ));
+                CK(pb200::launch_fit_group(grp_g, f.opts->growth, f.opts->multiplicative ? 1 : 0, mask != 0, dummy, 0, c->stream, &occ));
                 if (occ < 1) return fail(PB200_E_UNSUPPORTED, "grouped fit kernel does not fit on an SM");
                 g.grouped = true;
                 g.slice = pb200::fit_group_plane_doubles(lc_tmax[lc], grp_g);           // doubles per slot
@@ -804,7 +865,7 @@ static int fit_impl(pb200_ctx* c, const pb200_options* opts, const int64_t* d_ds
                 g.on = true;
                 continue;
             }
-            CK(LAUNCH[mask](NT, opts->growth, reg, dummy, 0, g.smem, c->stream, &occ));
+            CK(LAUNCH[mask](NT, f.opts->growth, reg, dummy, 0, g.smem, c->stream, &occ));
             if (occ < 1) return fail(PB200_E_UNSUPPORTED, "fit kernel does not fit on an SM");
             g.grid = cap_grid(std::min<int64_t>((int64_t)lc_n[lc], (int64_t)c->sms * occ));
             planes_bytes += (size_t)g.grid * g.slice * 16;
@@ -822,10 +883,10 @@ static int fit_impl(pb200_ctx* c, const pb200_options* opts, const int64_t* d_ds
         int occ = 0;
         if (reg.R > 0) {
             pb200::RegTableFitArgs dummy{};
-            CK(pb200::launch_fit_table_reg(opts->growth, dummy, 0, tab_smem, c->stream, &occ));
+            CK(pb200::launch_fit_table_reg(f.opts->growth, dummy, 0, tab_smem, c->stream, &occ));
         } else {
             pb200::TableFitArgs dummy{};
-            CK(pb200::launch_fit_table(opts->growth, dummy, 0, tab_smem, c->stream, &occ));
+            CK(pb200::launch_fit_table(f.opts->growth, dummy, 0, tab_smem, c->stream, &occ));
         }
         if (occ < 1) return fail(PB200_E_UNSUPPORTED, "table fit kernel does not fit on an SM");
         tab_grid = cap_grid(std::min<int64_t>((int64_t)N, (int64_t)c->sms * occ));
@@ -833,48 +894,52 @@ static int fit_impl(pb200_ctx* c, const pb200_options* opts, const int64_t* d_ds
         planes_bytes += (size_t)tab_grid * tab_planes * tab_Tp * 16;
     }
     CK(c->d_planes.reserve(planes_bytes));
+    // the arguments every fit launch shares; each launch adds its queue, workspace and geometry.  The table class has no
+    // warm start and no per-series prior scales (refused above), so it gets theta and a null prior from here too
+    FitArgs base{};
+    base.ds = (const long long*)f.ds;
+    base.y = f.y;
+    base.y_dtype = f.y_dtype;
+    base.offsets = (const long long*)c->d_offsets.p;
+    base.params = f.params;
+    base.tchange = f.tchange;
+    base.meta_i32 = f.meta_i32;
+    base.meta_i64 = (long long*)f.meta_i64;
+    base.meta_f64 = f.meta_f64;
+    base.smax = L.smax;
+    base.kmax = L.kmax;
+    base.pstride = L.pstride;
+    base.theta_in = f.theta ? f.theta : warm_x;
+    base.grad_out = f.grad;
+    base.trace = f.trace;
+    base.trace_cap = f.trace_cap;
+    base.nq_count = nq;
+    base.nq_items = f.opts->algorithm == PB200_ALG_LBFGS_NEWTON ? nq + 2 : nullptr;
+    base.o = od;
+    base.prior = f.prior;
+    base.l2_keep = base.l2_rest_first = 0;
     if (tabcls) {
         pb200::TableFitArgs fa;
-        fa.ds = (const long long*)d_ds;
-        fa.y = d_y;
-        fa.y_dtype = y_dtype;
-        fa.offsets = (const long long*)c->d_offsets.p;
+        static_cast<FitArgs&>(fa) = base;
         const int q = NLC * NQ;
         fa.q_items = (const int*)c->d_qitems.p + (size_t)q * N;
         fa.q_count = q_count + q;
         fa.q_head = q_head + q;
-        fa.params = d_params;
-        fa.tchange = d_tchange;
-        fa.meta_i32 = d_meta_i32;
-        fa.meta_i64 = (long long*)d_meta_i64;
-        fa.meta_f64 = d_meta_f64;
-        fa.smax = L.smax;
-        fa.kmax = L.kmax;
-        fa.pstride = L.pstride;
         fa.Tp = tab_Tp;
         fa.ppad = tab_ppad;
         fa.planes = (double2*)((char*)c->d_planes.p + tab_off);
         fa.nseas_stride = tab_planes * tab_Tp;
-        fa.theta_in = d_theta_in;
-        fa.grad_out = d_grad_out;
-        fa.trace = d_trace;
-        fa.trace_cap = trace_cap;
-        fa.nq_count = nq;
-        fa.nq_items = opts->algorithm == PB200_ALG_LBFGS_NEWTON ? nq + 2 : nullptr;
-        fa.o = od;
-        fa.l2_keep = fa.l2_rest_first = 0;
-        fa.prior = nullptr;
         fa.tab = tab;
         if (reg.R > 0) {
             pb200::RegTableFitArgs ra;
             static_cast<pb200::TableFitArgs&>(ra) = fa;
-            ra.reg = d_reg;
-            ra.reg_scale = d_reg_scale;
+            ra.reg = f.reg;
+            ra.reg_scale = f.reg_scale;
             ra.n_rows = n_rows;
             ra.spec = reg;
-            CK(pb200::launch_fit_table_reg(opts->growth, ra, tab_grid, tab_smem, c->stream, nullptr));
+            CK(pb200::launch_fit_table_reg(f.opts->growth, ra, tab_grid, tab_smem, c->stream, nullptr));
         } else {
-            CK(pb200::launch_fit_table(opts->growth, fa, tab_grid, tab_smem, c->stream, nullptr));
+            CK(pb200::launch_fit_table(f.opts->growth, fa, tab_grid, tab_smem, c->stream, nullptr));
         }
         c->launches++;
     }
@@ -885,38 +950,15 @@ static int fit_impl(pb200_ctx* c, const pb200_options* opts, const int64_t* d_ds
             const int mask = rm & 7, reg = rm >> 3;
             const Geo& g = geo[lc][rm];
             if (!g.on) continue;
-            const int Tp = g.Tp, ppad = g.ppad;
-            const size_t smem = g.smem;
-            FitArgs fa;
-            fa.ds = (const long long*)d_ds;
-            fa.y = d_y;
-            fa.y_dtype = y_dtype;
-            fa.offsets = (const long long*)c->d_offsets.p;
+            FitArgs fa = base;
             const int q = lc * NQ + rm;
             fa.q_items = (const int*)c->d_qitems.p + (size_t)q * N;
             fa.q_count = q_count + q;
             fa.q_head = q_head + q;
-            fa.params = d_params;
-            fa.tchange = d_tchange;
-            fa.meta_i32 = d_meta_i32;
-            fa.meta_i64 = (long long*)d_meta_i64;
-            fa.meta_f64 = d_meta_f64;
-            fa.smax = L.smax;
-            fa.kmax = L.kmax;
-            fa.pstride = L.pstride;
-            fa.Tp = Tp;
-            fa.ppad = ppad;
+            fa.Tp = g.Tp;
+            fa.ppad = g.ppad;
             fa.planes = (double2*)((char*)c->d_planes.p + g.off);
             fa.nseas_stride = (int)g.slice;
-            fa.theta_in = d_theta_in ? d_theta_in : warm_x;
-            fa.grad_out = d_grad_out;
-            fa.trace = d_trace;
-            fa.trace_cap = trace_cap;
-            fa.nq_count = nq;
-            fa.nq_items = opts->algorithm == PB200_ALG_LBFGS_NEWTON ? nq + 2 : nullptr;
-            fa.o = od;
-            fa.prior = d_prior;
-            fa.l2_keep = fa.l2_rest_first = 0;
             if (g.grouped && c->l2_keep_pct >= 0) {
                 // the slots' y planes are read once per evaluation round, cyclically: an LRU-like L2 smaller than all of them
                 // would miss on nearly every line.  A fixed subset that fits stays resident (evict_last); the rest streams
@@ -926,119 +968,94 @@ static int fit_impl(pb200_ctx* c, const pb200_options* opts, const int64_t* d_ds
                 fa.l2_rest_first = 1;
             }
             if (g.grouped) {
-                CK(pb200::launch_fit_group(grp_g, opts->growth, opts->multiplicative ? 1 : 0, mask != 0, fa, g.grid, c->stream, nullptr));
+                CK(pb200::launch_fit_group(grp_g, f.opts->growth, f.opts->multiplicative ? 1 : 0, mask != 0, fa, g.grid, c->stream, nullptr));
             } else {
-                CK(LAUNCH[mask](NT, opts->growth, reg, fa, g.grid, smem, c->stream, nullptr));
+                CK(LAUNCH[mask](NT, f.opts->growth, reg, fa, g.grid, g.smem, c->stream, nullptr));
             }
             c->launches++;
         }
     }
     // ---- fbprophet's Newton retry over the series whose L-BFGS failed its line search (normally an empty queue) ----
-    if (!d_grad_out)
-        return launch_newton(c, opts, d_ds, d_y, y_dtype, (const int64_t*)c->d_offsets.p, n_series, nq, d_prior, warm_x,
-                             d_params, d_tchange, d_meta_i32, d_meta_i64, d_meta_f64, d_reg, d_reg_scale, n_rows);
+    if (!f.grad) return launch_newton(c, f, warm_x);
     return PB200_OK;
 }
 
 // argument checks of the *_host fit entry points (outs: the caller's own pointers are all set); n_series == 0 passes
-static int check_host_fit(pb200_ctx* c, const pb200_options* opts, const int64_t* h_ds, const void* h_y, int32_t y_dtype,
-                          const int64_t* h_offsets, int64_t n_series, bool outs, bool regs = false) {
+static int check_host_fit(pb200_ctx* c, const FitCall& h, bool outs) {
     if (!c) return fail(PB200_E_ARG, "ctx is null");
-    int rc = check_opts(opts, regs);
+    int rc = check_opts(h.opts, h.regs);
     if (rc) return rc;
-    if (n_series <= 0) return n_series == 0 ? PB200_OK : fail(PB200_E_ARG, "n_series");
-    if (!h_ds || !h_y || !h_offsets || !outs) return fail(PB200_E_ARG, "null pointer");
-    if (y_dtype < 0 || y_dtype > 2) return fail(PB200_E_ARG, "y_dtype");
+    if (h.n_series <= 0) return h.n_series == 0 ? PB200_OK : fail(PB200_E_ARG, "n_series");
+    if (!h.ds || !h.y || !h.offsets || !outs) return fail(PB200_E_ARG, "null pointer");
+    if (h.y_dtype < 0 || h.y_dtype > 2) return fail(PB200_E_ARG, "y_dtype");
     return PB200_OK;
 }
 
-// ... and their common staging: ds and y copied in, room for the fitted records; with regressors (h_reg, h_reg_scale
-// non-null) their values copied in and room for their (mu, std)
-static int stage_host_fit(pb200_ctx* c, const pb200_options* opts, const int64_t* h_ds, const void* h_y, int32_t y_dtype,
-                          const int64_t* h_offsets, int64_t n_series, const double* h_reg = nullptr,
-                          const double* h_reg_scale = nullptr) {
-    pb200_layout L;
-    pb200_get_layout(opts, &L);
-    CK(cudaSetDevice(c->device));
-    const int64_t R = h_offsets[n_series];
-    const size_t N = (size_t)n_series;
-    CK(c->d_ds.reserve((size_t)R * 8));
-    CK(c->d_y.reserve((size_t)R * y_elem(y_dtype)));
-    CK(c->d_params.reserve(N * L.pstride * 8));
-    CK(c->d_tchange.reserve(N * L.smax * 8));
-    CK(c->d_mi32.reserve(N * 8 * 4));
-    CK(c->d_mi64.reserve(N * 2 * 8));
-    CK(c->d_mf64.reserve(N * 4 * 8));
-    CK(cudaMemcpyAsync(c->d_ds.p, h_ds, (size_t)R * 8, cudaMemcpyHostToDevice, c->stream));
-    CK(cudaMemcpyAsync(c->d_y.p, h_y, (size_t)R * y_elem(y_dtype), cudaMemcpyHostToDevice, c->stream));
-    pb200::RegSpec reg;
-    opts_reg(opts, &reg);
-    if (reg.R > 0) {
-        if (!h_reg || !h_reg_scale) return fail(PB200_E_ARG, "null pointer (regressors / reg_scale)");
-        CK(c->d_reg.reserve((size_t)reg.R * R * 8));
-        CK(c->d_regsc.reserve(N * reg.R * 2 * 8));
-        CK(cudaMemcpyAsync(c->d_reg.p, h_reg, (size_t)reg.R * R * 8, cudaMemcpyHostToDevice, c->stream));
-    }
-    return PB200_OK;
+// ... and their common staging of d's series (host arrays in, device arrays after): ds and y in, with R regressors their
+// values in and their (mu, std) out
+static void stage_series(Staging& s, FitCall& d, int R) {
+    const size_t N = (size_t)d.n_series, rows = (size_t)d.offsets[d.n_series];
+    d.ds = s.in(ST_DS, d.ds, rows);
+    d.y = s.in(ST_Y, (const char*)d.y, rows * y_elem(d.y_dtype));
+    d.reg = s.in(ST_REG, R > 0 ? d.reg : nullptr, (size_t)R * rows);
+    d.reg_scale = s.out(ST_REGSC, R > 0 ? d.reg_scale : nullptr, N * R * 2);
 }
 
-// pb200_fit_host, pb200_fit_trace_host and pb200_fit_warm_host (traced: trace_cap trajectory rows per series into h_trace;
-// h_prior, h_init_params / h_init_meta, h_warm optional): copy in, fit, copy out
-static int fit_host(pb200_ctx* c, const pb200_options* opts, const int64_t* h_ds, const void* h_y, int32_t y_dtype,
-                    const int64_t* h_offsets, int64_t n_series, double floor, double cap_multiplier, const double* h_cap,
-                    double* h_params, double* h_tchange, int32_t* h_meta_i32, int64_t* h_meta_i64, double* h_meta_f64,
-                    bool traced, double* h_trace, int32_t trace_cap, const double* h_prior = nullptr,
-                    const double* h_init_params = nullptr, const int32_t* h_init_meta = nullptr, int32_t* h_warm = nullptr,
-                    bool regs = false, const double* h_reg = nullptr, double* h_reg_scale = nullptr) {
-    int rc = check_host_fit(c, opts, h_ds, h_y, y_dtype, h_offsets, n_series,
-                            h_params && h_tchange && h_meta_i32 && h_meta_i64 && h_meta_f64 && (h_trace || !traced), regs);
-    if (rc || n_series == 0) return rc;
-    if (h_init_params && !h_init_meta) return fail(PB200_E_ARG, "h_init_meta_i32 is null");
-    if (traced && (trace_cap < 1 || (int64_t)trace_cap * n_series > (1LL << 26))) return fail(PB200_E_ARG, "trace_cap");
-    if ((rc = stage_host_fit(c, opts, h_ds, h_y, y_dtype, h_offsets, n_series, h_reg, h_reg_scale))) return rc;
+// pb200_fit_host, pb200_fit_trace_host, pb200_fit_warm_host and pb200_fit_regressors_host (h: host arrays; traced:
+// h.trace_cap trajectory rows per series into h.trace): copy in, fit, copy out
+static int fit_host(pb200_ctx* c, const FitCall& h, bool traced) {
+    int rc = check_host_fit(c, h, h.params && h.tchange && h.meta_i32 && h.meta_i64 && h.meta_f64 && (h.trace || !traced));
+    if (rc || h.n_series == 0) return rc;
+    if (h.init_params && !h.init_meta) return fail(PB200_E_ARG, "h_init_meta_i32 is null");
+    if (traced && (h.trace_cap < 1 || (int64_t)h.trace_cap * h.n_series > (1LL << 26))) return fail(PB200_E_ARG, "trace_cap");
     pb200::RegSpec reg;
-    opts_reg(opts, &reg);
+    opts_reg(h.opts, &reg);
+    if (reg.R > 0 && (!h.reg || !h.reg_scale)) return fail(PB200_E_ARG, "null pointer (regressors / reg_scale)");
     pb200_layout L;
-    pb200_get_layout(opts, &L);
-    const size_t N = (size_t)n_series, tbytes = traced ? N * (size_t)trace_cap * 4 * 8 : 0;
-    if (h_cap) {
-        CK(c->d_cap.reserve(N * 8));
-        CK(cudaMemcpyAsync(c->d_cap.p, h_cap, N * 8, cudaMemcpyHostToDevice, c->stream));
-    }
-    if (traced) {
-        CK(c->d_trace.reserve(tbytes));
-        CK(cudaMemsetAsync(c->d_trace.p, 0, tbytes, c->stream));
-    }
-    if (h_prior) {
-        CK(c->d_prior.reserve(N * 2 * 8));
-        CK(cudaMemcpyAsync(c->d_prior.p, h_prior, N * 2 * 8, cudaMemcpyHostToDevice, c->stream));
-    }
-    if (h_init_params) {
-        CK(c->d_iparams.reserve(N * L.pstride * 8));
-        CK(c->d_imeta.reserve(N * 8 * 4));
-        CK(cudaMemcpyAsync(c->d_iparams.p, h_init_params, N * L.pstride * 8, cudaMemcpyHostToDevice, c->stream));
-        CK(cudaMemcpyAsync(c->d_imeta.p, h_init_meta, N * 8 * 4, cudaMemcpyHostToDevice, c->stream));
-    }
-    const bool warm_out = h_init_params && h_warm;
-    if (warm_out) CK(c->d_warm.reserve(N * 4));
-    rc = fit_impl(c, opts, (const int64_t*)c->d_ds.p, c->d_y.p, y_dtype, h_offsets, n_series, floor, cap_multiplier,
-                  h_cap ? (const double*)c->d_cap.p : nullptr, h_prior ? (const double*)c->d_prior.p : nullptr,
-                  (double*)c->d_params.p, (double*)c->d_tchange.p,
-                  (int32_t*)c->d_mi32.p, (int64_t*)c->d_mi64.p, (double*)c->d_mf64.p, nullptr, nullptr,
-                  traced ? (double*)c->d_trace.p : nullptr, trace_cap,
-                  h_init_params ? (const double*)c->d_iparams.p : nullptr,
-                  h_init_params ? (const int32_t*)c->d_imeta.p : nullptr, warm_out ? (int32_t*)c->d_warm.p : nullptr, regs,
-                  reg.R > 0 ? (const double*)c->d_reg.p : nullptr, reg.R > 0 ? (double*)c->d_regsc.p : nullptr);
-    if (rc) return rc;
-    if (warm_out) CK(cudaMemcpyAsync(h_warm, c->d_warm.p, N * 4, cudaMemcpyDeviceToHost, c->stream));
-    if (reg.R > 0) CK(cudaMemcpyAsync(h_reg_scale, c->d_regsc.p, N * reg.R * 2 * 8, cudaMemcpyDeviceToHost, c->stream));
-    CK(cudaMemcpyAsync(h_params, c->d_params.p, N * L.pstride * 8, cudaMemcpyDeviceToHost, c->stream));
-    CK(cudaMemcpyAsync(h_tchange, c->d_tchange.p, N * L.smax * 8, cudaMemcpyDeviceToHost, c->stream));
-    CK(cudaMemcpyAsync(h_meta_i32, c->d_mi32.p, N * 8 * 4, cudaMemcpyDeviceToHost, c->stream));
-    CK(cudaMemcpyAsync(h_meta_i64, c->d_mi64.p, N * 2 * 8, cudaMemcpyDeviceToHost, c->stream));
-    CK(cudaMemcpyAsync(h_meta_f64, c->d_mf64.p, N * 4 * 8, cudaMemcpyDeviceToHost, c->stream));
-    if (traced) CK(cudaMemcpyAsync(h_trace, c->d_trace.p, tbytes, cudaMemcpyDeviceToHost, c->stream));
-    CK(cudaStreamSynchronize(c->stream));
+    pb200_get_layout(h.opts, &L);
+    const size_t N = (size_t)h.n_series;
+    Staging s(c);
+    FitCall d = h;
+    stage_series(s, d, reg.R);
+    d.cap = s.in(ST_CAP, h.cap, N);
+    d.prior = s.in(ST_PRIOR, h.prior, N * 2);
+    d.init_params = s.in(ST_IPARAMS, h.init_params, N * L.pstride);
+    d.init_meta = s.in(ST_IMETA, h.init_params ? h.init_meta : nullptr, N * 8);
+    d.warm = s.out(ST_WARM, h.init_params ? h.warm : nullptr, N);
+    d.trace = s.out(ST_TRACE, traced ? h.trace : nullptr, N * (size_t)h.trace_cap * 4, true);
+    d.params = s.out(ST_PARAMS, h.params, N * L.pstride);
+    d.tchange = s.out(ST_TCHANGE, h.tchange, N * L.smax);
+    d.meta_i32 = s.out(ST_MI32, h.meta_i32, N * 8);
+    d.meta_i64 = s.out(ST_MI64, h.meta_i64, N * 2);
+    d.meta_f64 = s.out(ST_MF64, h.meta_f64, N * 4);
+    if ((rc = s.status()) || (rc = fit_impl(c, d))) return rc;
+    return s.finish();
+}
+
+// pb200_objective_host and pb200_objective_regressors_host (h: host arrays; the objective goes to h_f): -log p and its
+// gradient at h.theta
+static int objective_host(pb200_ctx* c, const FitCall& h, double* h_f) {
+    int rc = check_host_fit(c, h, h.theta && h_f && h.grad && h.meta_i32);
+    if (rc || h.n_series == 0) return rc;
+    pb200::RegSpec reg;
+    opts_reg(h.opts, &reg);
+    if (reg.R > 0 && (!h.reg || !h.reg_scale)) return fail(PB200_E_ARG, "null pointer (regressors / reg_scale)");
+    pb200_layout L;
+    pb200_get_layout(h.opts, &L);
+    const size_t N = (size_t)h.n_series;
+    std::vector<double> mf(N * 4);
+    Staging s(c);
+    FitCall d = h;
+    stage_series(s, d, reg.R);
+    d.theta = s.in(ST_THETA, h.theta, N * L.pstride);
+    d.grad = s.out(ST_GRAD, h.grad, N * L.pstride, true);
+    d.params = (double*)s.reserve(ST_PARAMS, N * L.pstride * 8);
+    d.tchange = (double*)s.reserve(ST_TCHANGE, N * L.smax * 8);
+    d.meta_i32 = s.out(ST_MI32, h.meta_i32, N * 8);
+    d.meta_i64 = (int64_t*)s.reserve(ST_MI64, N * 2 * 8);
+    d.meta_f64 = s.out(ST_MF64, mf.data(), N * 4);
+    if ((rc = s.status()) || (rc = fit_impl(c, d)) || (rc = s.finish())) return rc;
+    for (size_t i = 0; i < N; ++i) h_f[i] = mf[i * 4 + 3];
     return PB200_OK;
 }
 
@@ -1048,8 +1065,10 @@ PB200_API int pb200_fit_prior_device(pb200_ctx* c, const pb200_options* opts, co
                                      int32_t y_dtype, const int64_t* h_offsets, int64_t n_series, double floor,
                                      double cap_multiplier, const double* d_cap, const double* d_prior, double* d_params,
                                      double* d_tchange, int32_t* d_meta_i32, int64_t* d_meta_i64, double* d_meta_f64) {
-    return fit_impl(c, opts, d_ds, d_y, y_dtype, h_offsets, n_series, floor, cap_multiplier, d_cap, d_prior, d_params,
-                    d_tchange, d_meta_i32, d_meta_i64, d_meta_f64, nullptr, nullptr);
+    FitCall f = {opts, d_ds, d_y, y_dtype, h_offsets, n_series, floor, cap_multiplier, d_cap, d_params, d_tchange,
+                 d_meta_i32, d_meta_i64, d_meta_f64};
+    f.prior = d_prior;
+    return fit_impl(c, f);
 }
 
 PB200_API int pb200_fit_warm_device(pb200_ctx* c, const pb200_options* opts, const int64_t* d_ds, const void* d_y,
@@ -1058,9 +1077,13 @@ PB200_API int pb200_fit_warm_device(pb200_ctx* c, const pb200_options* opts, con
                                     const double* d_init_params, const int32_t* d_init_meta_i32, double* d_params,
                                     double* d_tchange, int32_t* d_meta_i32, int64_t* d_meta_i64, double* d_meta_f64,
                                     int32_t* d_warm) {
-    return fit_impl(c, opts, d_ds, d_y, y_dtype, h_offsets, n_series, floor, cap_multiplier, d_cap, d_prior, d_params,
-                    d_tchange, d_meta_i32, d_meta_i64, d_meta_f64, nullptr, nullptr, nullptr, 0, d_init_params,
-                    d_init_meta_i32, d_init_params ? d_warm : nullptr);
+    FitCall f = {opts, d_ds, d_y, y_dtype, h_offsets, n_series, floor, cap_multiplier, d_cap, d_params, d_tchange,
+                 d_meta_i32, d_meta_i64, d_meta_f64};
+    f.prior = d_prior;
+    f.init_params = d_init_params;
+    f.init_meta = d_init_meta_i32;
+    f.warm = d_init_params ? d_warm : nullptr;
+    return fit_impl(c, f);
 }
 
 PB200_API int pb200_fit_warm_host(pb200_ctx* c, const pb200_options* opts, const int64_t* h_ds, const void* h_y,
@@ -1069,70 +1092,49 @@ PB200_API int pb200_fit_warm_host(pb200_ctx* c, const pb200_options* opts, const
                                   const double* h_init_params, const int32_t* h_init_meta_i32, double* h_params,
                                   double* h_tchange, int32_t* h_meta_i32, int64_t* h_meta_i64, double* h_meta_f64,
                                   int32_t* h_warm, double* h_trace, int32_t trace_cap) {
-    return fit_host(c, opts, h_ds, h_y, y_dtype, h_offsets, n_series, floor, cap_multiplier, h_cap, h_params, h_tchange,
-                    h_meta_i32, h_meta_i64, h_meta_f64, h_trace != nullptr, h_trace, trace_cap, h_prior, h_init_params,
-                    h_init_meta_i32, h_warm);
+    FitCall h = {opts, h_ds, h_y, y_dtype, h_offsets, n_series, floor, cap_multiplier, h_cap, h_params, h_tchange,
+                 h_meta_i32, h_meta_i64, h_meta_f64};
+    h.prior = h_prior;
+    h.init_params = h_init_params;
+    h.init_meta = h_init_meta_i32;
+    h.warm = h_warm;
+    h.trace = h_trace;
+    h.trace_cap = trace_cap;
+    return fit_host(c, h, h_trace != nullptr);
 }
 
 PB200_API int pb200_fit_device(pb200_ctx* c, const pb200_options* opts, const int64_t* d_ds, const void* d_y, int32_t y_dtype,
                      const int64_t* h_offsets, int64_t n_series, double floor, double cap_multiplier,
                      const double* d_cap, double* d_params, double* d_tchange, int32_t* d_meta_i32,
                      int64_t* d_meta_i64, double* d_meta_f64) {
-    return pb200_fit_prior_device(c, opts, d_ds, d_y, y_dtype, h_offsets, n_series, floor, cap_multiplier, d_cap, nullptr,
-                                  d_params, d_tchange, d_meta_i32, d_meta_i64, d_meta_f64);
+    const FitCall f = {opts, d_ds, d_y, y_dtype, h_offsets, n_series, floor, cap_multiplier, d_cap, d_params, d_tchange,
+                       d_meta_i32, d_meta_i64, d_meta_f64};
+    return fit_impl(c, f);
 }
-
-}  // extern "C"
-
-// pb200_objective_host and pb200_objective_regressors_host (regs; h_reg / h_reg_scale as pb200_fit_regressors_host's)
-static int objective_host(pb200_ctx* c, const pb200_options* opts, const int64_t* h_ds, const void* h_y, int32_t y_dtype,
-                          const int64_t* h_offsets, int64_t n_series, double floor, double cap_multiplier,
-                          const double* h_theta, double* h_f, double* h_grad, int32_t* h_meta_i32, bool regs = false,
-                          const double* h_reg = nullptr, double* h_reg_scale = nullptr) {
-    int rc = check_host_fit(c, opts, h_ds, h_y, y_dtype, h_offsets, n_series, h_theta && h_f && h_grad && h_meta_i32, regs);
-    if (rc || n_series == 0) return rc;
-    if ((rc = stage_host_fit(c, opts, h_ds, h_y, y_dtype, h_offsets, n_series, h_reg, h_reg_scale))) return rc;
-    pb200::RegSpec reg;
-    opts_reg(opts, &reg);
-    pb200_layout L;
-    pb200_get_layout(opts, &L);
-    const size_t N = (size_t)n_series;
-    CK(c->d_yhat.reserve(N * L.pstride * 8));   // theta_in
-    CK(c->d_lo.reserve(N * L.pstride * 8));     // grad_out
-    CK(cudaMemcpyAsync(c->d_yhat.p, h_theta, N * L.pstride * 8, cudaMemcpyHostToDevice, c->stream));
-    CK(cudaMemsetAsync(c->d_lo.p, 0, N * L.pstride * 8, c->stream));
-    rc = fit_impl(c, opts, (const int64_t*)c->d_ds.p, c->d_y.p, y_dtype, h_offsets, n_series, floor, cap_multiplier,
-                  nullptr, nullptr, (double*)c->d_params.p, (double*)c->d_tchange.p, (int32_t*)c->d_mi32.p,
-                  (int64_t*)c->d_mi64.p, (double*)c->d_mf64.p, (const double*)c->d_yhat.p, (double*)c->d_lo.p, nullptr, 0,
-                  nullptr, nullptr, nullptr, regs, reg.R > 0 ? (const double*)c->d_reg.p : nullptr,
-                  reg.R > 0 ? (double*)c->d_regsc.p : nullptr);
-    if (rc) return rc;
-    if (reg.R > 0) CK(cudaMemcpyAsync(h_reg_scale, c->d_regsc.p, N * reg.R * 2 * 8, cudaMemcpyDeviceToHost, c->stream));
-    std::vector<double> mf(N * 4);
-    CK(cudaMemcpyAsync(h_grad, c->d_lo.p, N * L.pstride * 8, cudaMemcpyDeviceToHost, c->stream));
-    CK(cudaMemcpyAsync(h_meta_i32, c->d_mi32.p, N * 8 * 4, cudaMemcpyDeviceToHost, c->stream));
-    CK(cudaMemcpyAsync(mf.data(), c->d_mf64.p, N * 4 * 8, cudaMemcpyDeviceToHost, c->stream));
-    CK(cudaStreamSynchronize(c->stream));
-    for (size_t i = 0; i < N; ++i) h_f[i] = mf[i * 4 + 3];
-    return PB200_OK;
-}
-
-extern "C" {
 
 PB200_API int pb200_objective_host(pb200_ctx* c, const pb200_options* opts, const int64_t* h_ds, const void* h_y,
                                    int32_t y_dtype, const int64_t* h_offsets, int64_t n_series, double floor,
                                    double cap_multiplier, const double* h_theta, double* h_f, double* h_grad,
                                    int32_t* h_meta_i32) {
-    return objective_host(c, opts, h_ds, h_y, y_dtype, h_offsets, n_series, floor, cap_multiplier, h_theta, h_f, h_grad,
-                          h_meta_i32);
+    FitCall h = {opts, h_ds, h_y, y_dtype, h_offsets, n_series, floor, cap_multiplier};
+    h.theta = h_theta;
+    h.grad = h_grad;
+    h.meta_i32 = h_meta_i32;
+    return objective_host(c, h, h_f);
 }
 
 PB200_API int pb200_objective_regressors_host(pb200_ctx* c, const pb200_options* opts, const int64_t* h_ds, const void* h_y,
                                               int32_t y_dtype, const int64_t* h_offsets, int64_t n_series, double floor,
                                               double cap_multiplier, const double* h_reg, double* h_reg_scale,
                                               const double* h_theta, double* h_f, double* h_grad, int32_t* h_meta_i32) {
-    return objective_host(c, opts, h_ds, h_y, y_dtype, h_offsets, n_series, floor, cap_multiplier, h_theta, h_f, h_grad,
-                          h_meta_i32, true, h_reg, h_reg_scale);
+    FitCall h = {opts, h_ds, h_y, y_dtype, h_offsets, n_series, floor, cap_multiplier};
+    h.regs = true;
+    h.reg = h_reg;
+    h.reg_scale = h_reg_scale;
+    h.theta = h_theta;
+    h.grad = h_grad;
+    h.meta_i32 = h_meta_i32;
+    return objective_host(c, h, h_f);
 }
 
 PB200_API int pb200_fit_regressors_device(pb200_ctx* c, const pb200_options* opts, const int64_t* d_ds, const void* d_y,
@@ -1140,9 +1142,12 @@ PB200_API int pb200_fit_regressors_device(pb200_ctx* c, const pb200_options* opt
                                           double cap_multiplier, const double* d_cap, const double* d_reg, double* d_reg_scale,
                                           double* d_params, double* d_tchange, int32_t* d_meta_i32, int64_t* d_meta_i64,
                                           double* d_meta_f64) {
-    return fit_impl(c, opts, d_ds, d_y, y_dtype, h_offsets, n_series, floor, cap_multiplier, d_cap, nullptr, d_params,
-                    d_tchange, d_meta_i32, d_meta_i64, d_meta_f64, nullptr, nullptr, nullptr, 0, nullptr, nullptr, nullptr,
-                    true, d_reg, d_reg_scale);
+    FitCall f = {opts, d_ds, d_y, y_dtype, h_offsets, n_series, floor, cap_multiplier, d_cap, d_params, d_tchange,
+                 d_meta_i32, d_meta_i64, d_meta_f64};
+    f.regs = true;
+    f.reg = d_reg;
+    f.reg_scale = d_reg_scale;
+    return fit_impl(c, f);
 }
 
 PB200_API int pb200_fit_regressors_copy_device(pb200_ctx* c, const pb200_options* opts, const int64_t* d_ds,
@@ -1152,9 +1157,13 @@ PB200_API int pb200_fit_regressors_copy_device(pb200_ctx* c, const pb200_options
                                                double* d_params, double* d_tchange, int32_t* d_meta_i32,
                                                int64_t* d_meta_i64, double* d_meta_f64) {
     if (!d_reg_scale_copy && n_series > 0) return fail(PB200_E_ARG, "null pointer (reg_scale_copy)");
-    return fit_impl(c, opts, d_ds, d_y, y_dtype, h_offsets, n_series, floor, cap_multiplier, d_cap, nullptr, d_params,
-                    d_tchange, d_meta_i32, d_meta_i64, d_meta_f64, nullptr, nullptr, nullptr, 0, nullptr, nullptr, nullptr,
-                    true, d_reg, d_reg_scale, d_reg_scale_copy);
+    FitCall f = {opts, d_ds, d_y, y_dtype, h_offsets, n_series, floor, cap_multiplier, d_cap, d_params, d_tchange,
+                 d_meta_i32, d_meta_i64, d_meta_f64};
+    f.regs = true;
+    f.reg = d_reg;
+    f.reg_scale = d_reg_scale;
+    f.reg_scale_copy = d_reg_scale_copy;
+    return fit_impl(c, f);
 }
 
 PB200_API int pb200_regressor_scales_device(pb200_ctx* c, const pb200_options* opts, const double* d_reg,
@@ -1232,24 +1241,37 @@ PB200_API int pb200_fit_regressors_host(pb200_ctx* c, const pb200_options* opts,
                                         double cap_multiplier, const double* h_cap, const double* h_reg, double* h_reg_scale,
                                         double* h_params, double* h_tchange, int32_t* h_meta_i32, int64_t* h_meta_i64,
                                         double* h_meta_f64, double* h_trace, int32_t trace_cap) {
-    return fit_host(c, opts, h_ds, h_y, y_dtype, h_offsets, n_series, floor, cap_multiplier, h_cap, h_params, h_tchange,
-                    h_meta_i32, h_meta_i64, h_meta_f64, h_trace != nullptr && trace_cap > 0, h_trace, trace_cap, nullptr,
-                    nullptr, nullptr, nullptr, true, h_reg, h_reg_scale);
+    FitCall h = {opts, h_ds, h_y, y_dtype, h_offsets, n_series, floor, cap_multiplier, h_cap, h_params, h_tchange,
+                 h_meta_i32, h_meta_i64, h_meta_f64};
+    h.regs = true;
+    h.reg = h_reg;
+    h.reg_scale = h_reg_scale;
+    h.trace = h_trace;
+    h.trace_cap = trace_cap;
+    return fit_host(c, h, h_trace != nullptr && trace_cap > 0);
 }
 
 PB200_API int pb200_fit_host(pb200_ctx* c, const pb200_options* opts, const int64_t* h_ds, const void* h_y, int32_t y_dtype,
                    const int64_t* h_offsets, int64_t n_series, double floor, double cap_multiplier, const double* h_cap,
                    double* h_params, double* h_tchange, int32_t* h_meta_i32, int64_t* h_meta_i64, double* h_meta_f64) {
-    return fit_host(c, opts, h_ds, h_y, y_dtype, h_offsets, n_series, floor, cap_multiplier, h_cap, h_params, h_tchange,
-                    h_meta_i32, h_meta_i64, h_meta_f64, false, nullptr, 0);
+    const FitCall h = {opts, h_ds, h_y, y_dtype, h_offsets, n_series, floor, cap_multiplier, h_cap, h_params, h_tchange,
+                       h_meta_i32, h_meta_i64, h_meta_f64};
+    return fit_host(c, h, false);
 }
 
 PB200_API int pb200_fit_trace_host(pb200_ctx* c, const pb200_options* opts, const int64_t* h_ds, const void* h_y, int32_t y_dtype,
                          const int64_t* h_offsets, int64_t n_series, double floor, double cap_multiplier, double* h_params,
                          double* h_tchange, int32_t* h_meta_i32, int64_t* h_meta_i64, double* h_meta_f64, double* h_trace,
                          int32_t trace_cap) {
-    return fit_host(c, opts, h_ds, h_y, y_dtype, h_offsets, n_series, floor, cap_multiplier, nullptr, h_params, h_tchange,
-                    h_meta_i32, h_meta_i64, h_meta_f64, true, h_trace, trace_cap);
+    FitCall h = {opts, h_ds, h_y, y_dtype, h_offsets, n_series, floor, cap_multiplier};
+    h.params = h_params;
+    h.tchange = h_tchange;
+    h.meta_i32 = h_meta_i32;
+    h.meta_i64 = h_meta_i64;
+    h.meta_f64 = h_meta_f64;
+    h.trace = h_trace;
+    h.trace_cap = trace_cap;
+    return fit_host(c, h, true);
 }
 
 PB200_API int pb200_make_future_device(pb200_ctx* c, const int64_t* d_last_ds, int64_t n_models, int32_t horizon, int64_t freq_ns,
@@ -1335,94 +1357,124 @@ int check_quant_args(const pb200_options* o, const QuantOut& q) {
     return PB200_OK;
 }
 
-// pb200_predict_device; d_comp != null: the components instance of predict_kernel, d_tlo / d_thi != null: the
-// trend-bounds instance of mc_kernel; sums != null: mc_sum_kernel after them (it also runs on an empty frame, where
-// every model has no window), its per-model instance when sums->origins != null, its calendar instance when
-// sums->months != 0; quant != null: mc_kernel also writes the
-// quantile planes, from the same selection as the bounds
-int predict_device(pb200_ctx* c, const pb200_options* opts, const double* d_params, const double* d_tchange,
-                   const int32_t* d_meta_i32, const int64_t* d_meta_i64, const double* d_meta_f64, int64_t n_models,
-                   const int64_t* d_future_ds, int32_t horizon, const double* d_floor, const double* d_cap, uint64_t seed,
-                   double* d_yhat, double* d_yhat_lower, double* d_yhat_upper, int32_t* d_yhat_int, double* d_comp,
-                   double* d_tlo, double* d_thi, const SumOut* sums = nullptr, const QuantOut* quant = nullptr,
-                   bool regs = false, const double* d_future_reg = nullptr, const double* d_reg_scale = nullptr) {
-    if (!c) return fail(PB200_E_ARG, "ctx is null");
-    int rc = check_opts(opts, regs);
-    if (rc) return rc;
-    if (n_models < 0 || horizon < 0 || n_models > (1LL << 30)) return fail(PB200_E_ARG, "sizes");
-    if (sums && (rc = check_sum_args(opts, *sums))) return rc;
-    if (quant && (rc = check_quant_args(opts, *quant))) return rc;
-    if (n_models == 0 || (horizon == 0 && !sums)) return PB200_OK;
-    if (!d_params || !d_tchange || !d_meta_i32 || !d_meta_i64 || !d_meta_f64 || !d_floor || !d_cap ||
-        (horizon > 0 && (!d_future_ds || !d_yhat || !d_yhat_int)))
-        return fail(PB200_E_ARG, "null pointer");
-    const bool mc = horizon > 0 && d_yhat_lower && d_yhat_upper && opts->uncertainty_samples > 0;
-    if (mc && (rc = check_mc_opts(opts))) return rc;
-    pb200::RegSpec reg;
-    opts_reg(opts, &reg);
-    if (reg.R > 0 && horizon > 0 && (!d_future_reg || !d_reg_scale)) return fail(PB200_E_ARG, "null pointer (regressors / reg_scale)");
+// One predict request: device arrays in predict_device / predict_history_device, host arrays in predict_host /
+// pb200_predict_history_host.  The leading members are the arguments every predict entry point takes, in their order;
+// the others are optional
+struct PredictCall {
+    const pb200_options* opts;
+    const double* params;
+    const double* tchange;
+    const int32_t* meta_i32;
+    const int64_t* meta_i64;
+    const double* meta_f64;
+    int64_t n_models;
+    const int64_t* future_ds;
+    int32_t horizon;
+    const double* floor;
+    const double* cap;
+    uint64_t seed;
+    double* yhat;
+    double* yhat_lower;
+    double* yhat_upper;
+    int32_t* yhat_int;
+    double* comp = nullptr;          // the component planes and the trend bounds (pb200_predict_components_*)
+    double* tlo = nullptr;
+    double* thi = nullptr;
+    const SumOut* sums = nullptr;    // window totals (pb200_predict_sums_*, pb200_predict_period_sums_*)
+    const QuantOut* quant = nullptr;
+    bool regs = false;               // a regressor entry point: the options may carry regressors
+    const double* future_reg = nullptr;
+    const double* reg_scale = nullptr;
+    const int64_t* offsets = nullptr;   // pb200_predict_history_*: model i's rows of future_ds (a host array)
+};
+
+// the arguments every predict_kernel and mc_kernel instance takes
+void predict_args(pb200::PredictArgs& a, const PredictCall& p) {
     pb200_layout L;
-    pb200_get_layout(opts, &L);
-    pb200::PredictArgs a;
-    opts_table(opts, &a.tab);
-    CK(cudaSetDevice(c->device));
-    a.params = d_params;
-    a.tchange = d_tchange;
-    a.meta_i32 = d_meta_i32;
-    a.meta_i64 = (const long long*)d_meta_i64;
-    a.meta_f64 = d_meta_f64;
-    a.future_ds = (const long long*)d_future_ds;
-    a.floor = d_floor;
-    a.cap = d_cap;
-    a.n_models = (int)n_models;
-    a.horizon = horizon;
+    pb200_get_layout(p.opts, &L);
+    opts_table(p.opts, &a.tab);
+    a.params = p.params;
+    a.tchange = p.tchange;
+    a.meta_i32 = p.meta_i32;
+    a.meta_i64 = (const long long*)p.meta_i64;
+    a.meta_f64 = p.meta_f64;
+    a.future_ds = (const long long*)p.future_ds;
+    a.floor = p.floor;
+    a.cap = p.cap;
+    a.n_models = (int)p.n_models;
+    a.horizon = p.horizon;
     a.smax = L.smax;
     a.kmax = L.kmax;
     a.pstride = L.pstride;
-    a.growth = opts->growth;
-    a.mult = opts->multiplicative ? 1 : 0;
-    a.yhat = d_yhat;
-    a.trend = d_comp;
-    a.yhat_int = d_yhat_int;
+    a.growth = p.opts->growth;
+    a.mult = p.opts->multiplicative ? 1 : 0;
+    a.yhat = p.yhat;
+    a.trend = p.comp;
+    a.yhat_int = p.yhat_int;
+}
+
+// pb200_predict_device; p.comp != null: the components instance of predict_kernel, p.tlo / p.thi != null: the
+// trend-bounds instance of mc_kernel; p.sums != null: mc_sum_kernel after them (it also runs on an empty frame, where
+// every model has no window), its per-model instance when sums->origins != null, its calendar instance when
+// sums->months != 0; p.quant != null: mc_kernel also writes the quantile planes, from the same selection as the bounds
+int predict_device(pb200_ctx* c, const PredictCall& p) {
+    if (!c) return fail(PB200_E_ARG, "ctx is null");
+    int rc = check_opts(p.opts, p.regs);
+    if (rc) return rc;
+    if (p.n_models < 0 || p.horizon < 0 || p.n_models > (1LL << 30)) return fail(PB200_E_ARG, "sizes");
+    if (p.sums && (rc = check_sum_args(p.opts, *p.sums))) return rc;
+    if (p.quant && (rc = check_quant_args(p.opts, *p.quant))) return rc;
+    if (p.n_models == 0 || (p.horizon == 0 && !p.sums)) return PB200_OK;
+    if (!p.params || !p.tchange || !p.meta_i32 || !p.meta_i64 || !p.meta_f64 || !p.floor || !p.cap ||
+        (p.horizon > 0 && (!p.future_ds || !p.yhat || !p.yhat_int)))
+        return fail(PB200_E_ARG, "null pointer");
+    const bool mc = p.horizon > 0 && p.yhat_lower && p.yhat_upper && p.opts->uncertainty_samples > 0;
+    if (mc && (rc = check_mc_opts(p.opts))) return rc;
+    pb200::RegSpec reg;
+    opts_reg(p.opts, &reg);
+    if (reg.R > 0 && p.horizon > 0 && (!p.future_reg || !p.reg_scale)) return fail(PB200_E_ARG, "null pointer (regressors / reg_scale)");
+    pb200::PredictArgs a;
+    predict_args(a, p);
+    CK(cudaSetDevice(c->device));
     if (reg.R > 0) {
         // the regressor instances: yhat and its interval (every other output is refused for these options by check_opts)
         pb200::RegPredictArgs ra;
         static_cast<pb200::PredictArgs&>(ra) = a;
-        ra.reg.future_reg = d_future_reg;
-        ra.reg.reg_scale = d_reg_scale;
+        ra.reg.future_reg = p.future_reg;
+        ra.reg.reg_scale = p.reg_scale;
         ra.reg.R = reg.R;
-        if (horizon == 0) return PB200_OK;
-        dim3 grid((unsigned)n_models, (unsigned)std::min((horizon + 1023) / 1024, 64));
+        if (p.horizon == 0) return PB200_OK;
+        dim3 grid((unsigned)p.n_models, (unsigned)std::min((p.horizon + 1023) / 1024, 64));
         pb200::predict_kernel<false, false, true><<<grid, 256, 0, c->stream>>>(ra);
         CK(cudaGetLastError());
         c->launches++;
         if (mc) {
-            rc = pb200::launch_mc_reg(c->stream, c->sms, a, ra.reg, opts->uncertainty_samples, opts->interval_width, seed,
-                                      d_yhat_lower, d_yhat_upper);
+            rc = pb200::launch_mc_reg(c->stream, c->sms, a, ra.reg, p.opts->uncertainty_samples, p.opts->interval_width, p.seed,
+                                      p.yhat_lower, p.yhat_upper);
             if (rc == -1) return fail(PB200_E_ARG, "uncertainty_samples / interval_width out of range");
             if (rc) return fail(PB200_E_CUDA, "mc kernel launch", cudaGetLastError());
             c->launches++;
         }
         return PB200_OK;
     }
-    if (horizon > 0) {
+    if (p.horizon > 0) {
         // one CTA per (model, 1024 future points): the per-model prologue (parameters, the serial gamma recurrence) is paid
         // once for config #5's 672 periods instead of three times
-        dim3 grid((unsigned)n_models, (unsigned)std::min((horizon + 1023) / 1024, 64));
-        if (d_comp) pb200::predict_kernel<true><<<grid, 256, 0, c->stream>>>(a);
+        dim3 grid((unsigned)p.n_models, (unsigned)std::min((p.horizon + 1023) / 1024, 64));
+        if (p.comp) pb200::predict_kernel<true><<<grid, 256, 0, c->stream>>>(a);
         else pb200::predict_kernel<false><<<grid, 256, 0, c->stream>>>(a);
         CK(cudaGetLastError());
         c->launches++;
     }
-    if (mc || (quant && horizon > 0)) {
-        rc = pb200::launch_mc(c->stream, c->sms, a, opts->uncertainty_samples, opts->interval_width, seed,
-                              mc ? d_yhat_lower : nullptr, mc ? d_yhat_upper : nullptr, d_tlo, d_thi, quant ? quant->n_q : 0,
-                              quant ? quant->percentiles : nullptr, quant ? quant->planes : nullptr);
+    if (mc || (p.quant && p.horizon > 0)) {
+        rc = pb200::launch_mc(c->stream, c->sms, a, p.opts->uncertainty_samples, p.opts->interval_width, p.seed,
+                              mc ? p.yhat_lower : nullptr, mc ? p.yhat_upper : nullptr, p.tlo, p.thi, p.quant ? p.quant->n_q : 0,
+                              p.quant ? p.quant->percentiles : nullptr, p.quant ? p.quant->planes : nullptr);
         if (rc == -1) return fail(PB200_E_ARG, "uncertainty_samples / interval_width / n_q out of range");
         if (rc) return fail(PB200_E_CUDA, "mc kernel launch", cudaGetLastError());
         c->launches++;
     }
-    if (sums) {
+    if (const SumOut* sums = p.sums) {
         pb200::McSumArgs s;
         s.mc.lower = sums->sum_lower;
         s.mc.upper = sums->sum_upper;
@@ -1436,7 +1488,7 @@ int predict_device(pb200_ctx* c, const pb200_options* opts, const double* d_para
         s.quantity_sum = (long long*)sums->quantity_sum;
         s.origins = (const long long*)sums->origins;
         s.frame_len = sums->frame_len;
-        rc = pb200::launch_mc_sum(c->stream, c->sms, a, opts->uncertainty_samples, opts->interval_width, seed, s,
+        rc = pb200::launch_mc_sum(c->stream, c->sms, a, p.opts->uncertainty_samples, p.opts->interval_width, p.seed, s,
                                   sums->months, sums->month_shift);
         if (rc == -1) return fail(PB200_E_ARG, "uncertainty_samples / interval_width out of range");
         if (rc) return fail(PB200_E_CUDA, "mc sum kernel launch", cudaGetLastError());
@@ -1445,126 +1497,79 @@ int predict_device(pb200_ctx* c, const pb200_options* opts, const double* d_para
     return PB200_OK;
 }
 
-// pb200_predict_host; h_comp / h_tlo / h_thi as predict_device's d_comp / d_tlo / d_thi
-int predict_host(pb200_ctx* c, const pb200_options* opts, const double* h_params, const double* h_tchange,
-                 const int32_t* h_meta_i32, const int64_t* h_meta_i64, const double* h_meta_f64, int64_t n_models,
-                 const int64_t* h_future_ds, int32_t horizon, const double* h_floor, const double* h_cap, uint64_t seed,
-                 double* h_yhat, double* h_yhat_lower, double* h_yhat_upper, int32_t* h_yhat_int, double* h_comp,
-                 double* h_tlo, double* h_thi, const SumOut* sums = nullptr, const QuantOut* quant = nullptr,
-                 bool regs = false, const double* h_future_reg = nullptr, const double* h_reg_scale = nullptr) {
+// pb200_predict_host and the other fixed-frame *_host predict calls (h: host arrays): copy in, predict, copy out
+int predict_host(pb200_ctx* c, const PredictCall& h) {
     if (!c) return fail(PB200_E_ARG, "ctx is null");
-    int rc = check_opts(opts, regs);
+    int rc = check_opts(h.opts, h.regs);
     if (rc) return rc;
-    if (quant && (rc = check_quant_args(opts, *quant))) return rc;
-    if (sums) {
-        if (n_models < 0 || horizon < 0) return fail(PB200_E_ARG, "sizes");
-        if ((rc = check_sum_args(opts, *sums))) return rc;
-        if (n_models == 0) return PB200_OK;
-    } else if (n_models <= 0 || horizon <= 0) {
-        return (n_models == 0 || horizon == 0) ? PB200_OK : fail(PB200_E_ARG, "sizes");
+    if (h.quant && (rc = check_quant_args(h.opts, *h.quant))) return rc;
+    if (h.sums) {
+        if (h.n_models < 0 || h.horizon < 0) return fail(PB200_E_ARG, "sizes");
+        if ((rc = check_sum_args(h.opts, *h.sums))) return rc;
+        if (h.n_models == 0) return PB200_OK;
+    } else if (h.n_models <= 0 || h.horizon <= 0) {
+        return (h.n_models == 0 || h.horizon == 0) ? PB200_OK : fail(PB200_E_ARG, "sizes");
     }
-    if (!h_params || !h_tchange || !h_meta_i32 || !h_meta_i64 || !h_meta_f64 || !h_floor || !h_cap ||
-        (horizon > 0 && (!h_future_ds || !h_yhat || !h_yhat_int)))
+    if (!h.params || !h.tchange || !h.meta_i32 || !h.meta_i64 || !h.meta_f64 || !h.floor || !h.cap ||
+        (h.horizon > 0 && (!h.future_ds || !h.yhat || !h.yhat_int)))
         return fail(PB200_E_ARG, "null pointer");
-    pb200_layout L;
-    pb200_get_layout(opts, &L);
-    CK(cudaSetDevice(c->device));
-    const size_t N = (size_t)n_models, NH = N * (size_t)horizon;
-    const bool mc = horizon > 0 && h_yhat_lower && h_yhat_upper && opts->uncertainty_samples > 0;
-    if (mc && (rc = check_mc_opts(opts))) return rc;
+    const bool mc = h.horizon > 0 && h.yhat_lower && h.yhat_upper && h.opts->uncertainty_samples > 0;
+    if (mc && (rc = check_mc_opts(h.opts))) return rc;
     pb200::RegSpec reg;
-    opts_reg(opts, &reg);
-    if (reg.R > 0) {
-        if (!h_future_reg || !h_reg_scale) return fail(PB200_E_ARG, "null pointer (regressors / reg_scale)");
-        CK(c->d_reg.reserve(NH * reg.R * 8));
-        CK(c->d_regsc.reserve(N * reg.R * 2 * 8));
-    }
-    // the window outputs on the device: five 8-byte arrays [N * wmax], then win_points [N * wmax] and n_windows [N]
-    const size_t NW = sums ? N * (size_t)sums->wmax : 0;
-    SumOut dsum;
-    if (sums) {
-        CK(c->d_sums.reserve(NW * 44 + N * 4));
-        dsum = *sums;
-        dsum.win_start = (int64_t*)c->d_sums.p;
-        dsum.quantity_sum = dsum.win_start + NW;
-        dsum.yhat_sum = (double*)(dsum.quantity_sum + NW);
-        dsum.sum_lower = dsum.yhat_sum + NW;
-        dsum.sum_upper = dsum.sum_lower + NW;
-        dsum.win_points = (int32_t*)(dsum.sum_upper + NW);
-        dsum.n_windows = dsum.win_points + NW;
-    }
-    CK(c->d_params.reserve(N * L.pstride * 8));
-    CK(c->d_tchange.reserve(N * L.smax * 8));
-    CK(c->d_mi32.reserve(N * 8 * 4));
-    CK(c->d_mi64.reserve(N * 2 * 8));
-    CK(c->d_mf64.reserve(N * 4 * 8));
-    CK(c->d_fut.reserve(NH * 8));
-    CK(c->d_floor.reserve(N * 8));
-    CK(c->d_cap.reserve(N * 8));
-    CK(c->d_yhat.reserve(NH * 8));
-    CK(c->d_yint.reserve(NH * 4));
-    if (mc) {
-        CK(c->d_lo.reserve(NH * 8));
-        CK(c->d_hi.reserve(NH * 8));
-    }
-    const int ncomp = pb200_component_count(opts);
-    if (h_comp) CK(c->d_comp.reserve(NH * 8 * ncomp));
+    opts_reg(h.opts, &reg);
+    if (reg.R > 0 && (!h.future_reg || !h.reg_scale)) return fail(PB200_E_ARG, "null pointer (regressors / reg_scale)");
+    pb200_layout L;
+    pb200_get_layout(h.opts, &L);
+    const size_t N = (size_t)h.n_models, NH = N * (size_t)h.horizon;
+    Staging s(c);
+    PredictCall d = h;
+    d.params = s.in(ST_PARAMS, h.params, N * L.pstride);
+    d.tchange = s.in(ST_TCHANGE, h.tchange, N * L.smax);
+    d.meta_i32 = s.in(ST_MI32, h.meta_i32, N * 8);
+    d.meta_i64 = s.in(ST_MI64, h.meta_i64, N * 2);
+    d.meta_f64 = s.in(ST_MF64, h.meta_f64, N * 4);
+    d.future_ds = s.in(ST_FUT, h.future_ds, NH);
+    d.floor = s.in(ST_FLOOR, h.floor, N);
+    d.cap = s.in(ST_CAP, h.cap, N);
+    d.future_reg = s.in(ST_REG, reg.R > 0 ? h.future_reg : nullptr, NH * reg.R);
+    d.reg_scale = s.in(ST_REGSC, reg.R > 0 ? h.reg_scale : nullptr, N * reg.R * 2);
+    d.yhat = s.out(ST_YHAT, h.yhat, NH);
+    d.yhat_int = s.out(ST_YINT, h.yhat_int, NH);
+    d.yhat_lower = s.out(ST_LO, mc ? h.yhat_lower : nullptr, NH);
+    d.yhat_upper = s.out(ST_HI, mc ? h.yhat_upper : nullptr, NH);
+    d.comp = s.out(ST_COMP, h.comp, NH * pb200_component_count(h.opts));
+    d.tlo = s.out(ST_TLO, h.tlo, NH);
+    d.thi = s.out(ST_THI, h.thi, NH);
     QuantOut dquant;
-    if (quant) {
-        CK(c->d_quant.reserve(NH * 8 * (size_t)quant->n_q));
-        dquant = *quant;
-        dquant.planes = (double*)c->d_quant.p;
+    if (h.quant) {
+        dquant = *h.quant;
+        dquant.planes = s.out(ST_QUANT, h.quant->planes, NH * h.quant->n_q);
+        d.quant = &dquant;
     }
-    if (h_tlo) {
-        CK(c->d_tlo.reserve(NH * 8));
-        CK(c->d_thi.reserve(NH * 8));
+    SumOut dsum;
+    if (const SumOut* hs = h.sums) {
+        // on the device: five 8-byte arrays [N * wmax], then win_points [N * wmax] and n_windows [N]
+        const size_t NW = N * (size_t)hs->wmax;
+        char* next = (char*)s.reserve(ST_SUMS, NW * 44 + N * 4);
+        if ((rc = s.status())) return rc;
+        auto carve = [&](auto* h, size_t n) {   // the next n elements of the buffer, copied back to h
+            auto* dp = (decltype(h))next;
+            next += n * sizeof *h;
+            s.later(h, dp, n);
+            return dp;
+        };
+        dsum = *hs;
+        dsum.win_start = carve(hs->win_start, NW);
+        dsum.quantity_sum = carve(hs->quantity_sum, NW);
+        dsum.yhat_sum = carve(hs->yhat_sum, NW);
+        dsum.sum_lower = carve(hs->sum_lower, NW);
+        dsum.sum_upper = carve(hs->sum_upper, NW);
+        dsum.win_points = carve(hs->win_points, NW);
+        dsum.n_windows = carve(hs->n_windows, N);
+        d.sums = &dsum;
     }
-    cudaStream_t st = c->stream;
-    CK(cudaMemcpyAsync(c->d_params.p, h_params, N * L.pstride * 8, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(c->d_tchange.p, h_tchange, N * L.smax * 8, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(c->d_mi32.p, h_meta_i32, N * 8 * 4, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(c->d_mi64.p, h_meta_i64, N * 2 * 8, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(c->d_mf64.p, h_meta_f64, N * 4 * 8, cudaMemcpyHostToDevice, st));
-    if (NH) CK(cudaMemcpyAsync(c->d_fut.p, h_future_ds, NH * 8, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(c->d_floor.p, h_floor, N * 8, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(c->d_cap.p, h_cap, N * 8, cudaMemcpyHostToDevice, st));
-    if (reg.R > 0) {
-        CK(cudaMemcpyAsync(c->d_reg.p, h_future_reg, NH * reg.R * 8, cudaMemcpyHostToDevice, st));
-        CK(cudaMemcpyAsync(c->d_regsc.p, h_reg_scale, N * reg.R * 2 * 8, cudaMemcpyHostToDevice, st));
-    }
-    rc = predict_device(c, opts, (const double*)c->d_params.p, (const double*)c->d_tchange.p, (const int32_t*)c->d_mi32.p,
-                        (const int64_t*)c->d_mi64.p, (const double*)c->d_mf64.p, n_models, (const int64_t*)c->d_fut.p,
-                        horizon, (const double*)c->d_floor.p, (const double*)c->d_cap.p, seed, (double*)c->d_yhat.p,
-                        mc ? (double*)c->d_lo.p : nullptr, mc ? (double*)c->d_hi.p : nullptr, (int32_t*)c->d_yint.p,
-                        h_comp ? (double*)c->d_comp.p : nullptr, h_tlo ? (double*)c->d_tlo.p : nullptr,
-                        h_tlo ? (double*)c->d_thi.p : nullptr, sums ? &dsum : nullptr, quant ? &dquant : nullptr, regs,
-                        reg.R > 0 ? (const double*)c->d_reg.p : nullptr, reg.R > 0 ? (const double*)c->d_regsc.p : nullptr);
-    if (rc) return rc;
-    if (sums) {
-        CK(cudaMemcpyAsync(sums->win_start, dsum.win_start, NW * 8, cudaMemcpyDeviceToHost, st));
-        CK(cudaMemcpyAsync(sums->quantity_sum, dsum.quantity_sum, NW * 8, cudaMemcpyDeviceToHost, st));
-        CK(cudaMemcpyAsync(sums->yhat_sum, dsum.yhat_sum, NW * 8, cudaMemcpyDeviceToHost, st));
-        CK(cudaMemcpyAsync(sums->sum_lower, dsum.sum_lower, NW * 8, cudaMemcpyDeviceToHost, st));
-        CK(cudaMemcpyAsync(sums->sum_upper, dsum.sum_upper, NW * 8, cudaMemcpyDeviceToHost, st));
-        CK(cudaMemcpyAsync(sums->win_points, dsum.win_points, NW * 4, cudaMemcpyDeviceToHost, st));
-        CK(cudaMemcpyAsync(sums->n_windows, dsum.n_windows, N * 4, cudaMemcpyDeviceToHost, st));
-    }
-    if (NH) {     // an empty frame (window sums only: every model then has no window) has nothing to copy
-        CK(cudaMemcpyAsync(h_yhat, c->d_yhat.p, NH * 8, cudaMemcpyDeviceToHost, st));
-        CK(cudaMemcpyAsync(h_yhat_int, c->d_yint.p, NH * 4, cudaMemcpyDeviceToHost, st));
-    }
-    if (mc) {
-        CK(cudaMemcpyAsync(h_yhat_lower, c->d_lo.p, NH * 8, cudaMemcpyDeviceToHost, st));
-        CK(cudaMemcpyAsync(h_yhat_upper, c->d_hi.p, NH * 8, cudaMemcpyDeviceToHost, st));
-    }
-    if (h_comp) CK(cudaMemcpyAsync(h_comp, c->d_comp.p, NH * 8 * ncomp, cudaMemcpyDeviceToHost, st));
-    if (quant) CK(cudaMemcpyAsync(quant->planes, dquant.planes, NH * 8 * (size_t)quant->n_q, cudaMemcpyDeviceToHost, st));
-    if (h_tlo) {
-        CK(cudaMemcpyAsync(h_tlo, c->d_tlo.p, NH * 8, cudaMemcpyDeviceToHost, st));
-        CK(cudaMemcpyAsync(h_thi, c->d_thi.p, NH * 8, cudaMemcpyDeviceToHost, st));
-    }
-    CK(cudaStreamSynchronize(st));
-    return PB200_OK;
+    if ((rc = s.status()) || (rc = predict_device(c, d))) return rc;
+    return s.finish();
 }
 
 }  // namespace
@@ -1574,16 +1579,18 @@ PB200_API int pb200_predict_device(pb200_ctx* c, const pb200_options* opts, cons
                          int64_t n_models, const int64_t* d_future_ds, int32_t horizon, const double* d_floor,
                          const double* d_cap, uint64_t seed, double* d_yhat, double* d_yhat_lower, double* d_yhat_upper,
                          int32_t* d_yhat_int) {
-    return predict_device(c, opts, d_params, d_tchange, d_meta_i32, d_meta_i64, d_meta_f64, n_models, d_future_ds, horizon,
-                          d_floor, d_cap, seed, d_yhat, d_yhat_lower, d_yhat_upper, d_yhat_int, nullptr, nullptr, nullptr);
+    const PredictCall p = {opts, d_params, d_tchange, d_meta_i32, d_meta_i64, d_meta_f64, n_models, d_future_ds,
+                           horizon, d_floor, d_cap, seed, d_yhat, d_yhat_lower, d_yhat_upper, d_yhat_int};
+    return predict_device(c, p);
 }
 
 PB200_API int pb200_predict_host(pb200_ctx* c, const pb200_options* opts, const double* h_params, const double* h_tchange,
                        const int32_t* h_meta_i32, const int64_t* h_meta_i64, const double* h_meta_f64, int64_t n_models,
                        const int64_t* h_future_ds, int32_t horizon, const double* h_floor, const double* h_cap,
                        uint64_t seed, double* h_yhat, double* h_yhat_lower, double* h_yhat_upper, int32_t* h_yhat_int) {
-    return predict_host(c, opts, h_params, h_tchange, h_meta_i32, h_meta_i64, h_meta_f64, n_models, h_future_ds, horizon,
-                        h_floor, h_cap, seed, h_yhat, h_yhat_lower, h_yhat_upper, h_yhat_int, nullptr, nullptr, nullptr);
+    const PredictCall p = {opts, h_params, h_tchange, h_meta_i32, h_meta_i64, h_meta_f64, n_models, h_future_ds,
+                           horizon, h_floor, h_cap, seed, h_yhat, h_yhat_lower, h_yhat_upper, h_yhat_int};
+    return predict_host(c, p);
 }
 
 PB200_API int pb200_predict_regressors_device(pb200_ctx* c, const pb200_options* opts, const double* d_params,
@@ -1592,9 +1599,12 @@ PB200_API int pb200_predict_regressors_device(pb200_ctx* c, const pb200_options*
                          const double* d_floor, const double* d_cap, uint64_t seed, const double* d_future_reg,
                          const double* d_reg_scale, double* d_yhat, double* d_yhat_lower, double* d_yhat_upper,
                          int32_t* d_yhat_int) {
-    return predict_device(c, opts, d_params, d_tchange, d_meta_i32, d_meta_i64, d_meta_f64, n_models, d_future_ds, horizon,
-                          d_floor, d_cap, seed, d_yhat, d_yhat_lower, d_yhat_upper, d_yhat_int, nullptr, nullptr, nullptr,
-                          nullptr, nullptr, true, d_future_reg, d_reg_scale);
+    PredictCall p = {opts, d_params, d_tchange, d_meta_i32, d_meta_i64, d_meta_f64, n_models, d_future_ds,
+                     horizon, d_floor, d_cap, seed, d_yhat, d_yhat_lower, d_yhat_upper, d_yhat_int};
+    p.regs = true;
+    p.future_reg = d_future_reg;
+    p.reg_scale = d_reg_scale;
+    return predict_device(c, p);
 }
 
 PB200_API int pb200_predict_regressors_host(pb200_ctx* c, const pb200_options* opts, const double* h_params,
@@ -1603,9 +1613,12 @@ PB200_API int pb200_predict_regressors_host(pb200_ctx* c, const pb200_options* o
                        const double* h_floor, const double* h_cap, uint64_t seed, const double* h_future_reg,
                        const double* h_reg_scale, double* h_yhat, double* h_yhat_lower, double* h_yhat_upper,
                        int32_t* h_yhat_int) {
-    return predict_host(c, opts, h_params, h_tchange, h_meta_i32, h_meta_i64, h_meta_f64, n_models, h_future_ds, horizon,
-                        h_floor, h_cap, seed, h_yhat, h_yhat_lower, h_yhat_upper, h_yhat_int, nullptr, nullptr, nullptr,
-                        nullptr, nullptr, true, h_future_reg, h_reg_scale);
+    PredictCall p = {opts, h_params, h_tchange, h_meta_i32, h_meta_i64, h_meta_f64, n_models, h_future_ds,
+                     horizon, h_floor, h_cap, seed, h_yhat, h_yhat_lower, h_yhat_upper, h_yhat_int};
+    p.regs = true;
+    p.future_reg = h_future_reg;
+    p.reg_scale = h_reg_scale;
+    return predict_host(c, p);
 }
 
 PB200_API int pb200_predict_components_device(pb200_ctx* c, const pb200_options* opts, const double* d_params,
@@ -1618,9 +1631,12 @@ PB200_API int pb200_predict_components_device(pb200_ctx* c, const pb200_options*
     int rc = check_opts(opts);
     if (rc) return rc;
     if ((rc = check_comp_args(opts, d_components, d_yhat_lower, d_yhat_upper, d_trend_lower, d_trend_upper))) return rc;
-    return predict_device(c, opts, d_params, d_tchange, d_meta_i32, d_meta_i64, d_meta_f64, n_models, d_future_ds, horizon,
-                          d_floor, d_cap, seed, d_yhat, d_yhat_lower, d_yhat_upper, d_yhat_int, d_components, d_trend_lower,
-                          d_trend_upper);
+    PredictCall p = {opts, d_params, d_tchange, d_meta_i32, d_meta_i64, d_meta_f64, n_models, d_future_ds,
+                     horizon, d_floor, d_cap, seed, d_yhat, d_yhat_lower, d_yhat_upper, d_yhat_int};
+    p.comp = d_components;
+    p.tlo = d_trend_lower;
+    p.thi = d_trend_upper;
+    return predict_device(c, p);
 }
 
 PB200_API int pb200_predict_components_host(pb200_ctx* c, const pb200_options* opts, const double* h_params,
@@ -1633,9 +1649,12 @@ PB200_API int pb200_predict_components_host(pb200_ctx* c, const pb200_options* o
     int rc = check_opts(opts);
     if (rc) return rc;
     if ((rc = check_comp_args(opts, h_components, h_yhat_lower, h_yhat_upper, h_trend_lower, h_trend_upper))) return rc;
-    return predict_host(c, opts, h_params, h_tchange, h_meta_i32, h_meta_i64, h_meta_f64, n_models, h_future_ds, horizon,
-                        h_floor, h_cap, seed, h_yhat, h_yhat_lower, h_yhat_upper, h_yhat_int, h_components, h_trend_lower,
-                        h_trend_upper);
+    PredictCall p = {opts, h_params, h_tchange, h_meta_i32, h_meta_i64, h_meta_f64, n_models, h_future_ds,
+                     horizon, h_floor, h_cap, seed, h_yhat, h_yhat_lower, h_yhat_upper, h_yhat_int};
+    p.comp = h_components;
+    p.tlo = h_trend_lower;
+    p.thi = h_trend_upper;
+    return predict_host(c, p);
 }
 
 PB200_API int pb200_predict_sums_device(pb200_ctx* c, const pb200_options* opts, const double* d_params, const double* d_tchange,
@@ -1647,8 +1666,10 @@ PB200_API int pb200_predict_sums_device(pb200_ctx* c, const pb200_options* opts,
                          double* d_sum_lower, double* d_sum_upper) {
     const SumOut s = {width_ns, origin_ns, wmax, d_n_windows, d_win_start, d_win_points, d_yhat_sum, d_quantity_sum,
                       d_sum_lower, d_sum_upper};
-    return predict_device(c, opts, d_params, d_tchange, d_meta_i32, d_meta_i64, d_meta_f64, n_models, d_future_ds, horizon,
-                          d_floor, d_cap, seed, d_yhat, d_yhat_lower, d_yhat_upper, d_yhat_int, nullptr, nullptr, nullptr, &s);
+    PredictCall p = {opts, d_params, d_tchange, d_meta_i32, d_meta_i64, d_meta_f64, n_models, d_future_ds,
+                     horizon, d_floor, d_cap, seed, d_yhat, d_yhat_lower, d_yhat_upper, d_yhat_int};
+    p.sums = &s;
+    return predict_device(c, p);
 }
 
 PB200_API int pb200_predict_sums_anchored_device(pb200_ctx* c, const pb200_options* opts, const double* d_params,
@@ -1664,8 +1685,10 @@ PB200_API int pb200_predict_sums_anchored_device(pb200_ctx* c, const pb200_optio
                 d_sum_upper};
     s.origins = d_origin_ns;
     s.frame_len = d_frame_len;
-    return predict_device(c, opts, d_params, d_tchange, d_meta_i32, d_meta_i64, d_meta_f64, n_models, d_future_ds, horizon,
-                          d_floor, d_cap, seed, d_yhat, d_yhat_lower, d_yhat_upper, d_yhat_int, nullptr, nullptr, nullptr, &s);
+    PredictCall p = {opts, d_params, d_tchange, d_meta_i32, d_meta_i64, d_meta_f64, n_models, d_future_ds,
+                     horizon, d_floor, d_cap, seed, d_yhat, d_yhat_lower, d_yhat_upper, d_yhat_int};
+    p.sums = &s;
+    return predict_device(c, p);
 }
 
 PB200_API int pb200_predict_sums_host(pb200_ctx* c, const pb200_options* opts, const double* h_params, const double* h_tchange,
@@ -1677,8 +1700,10 @@ PB200_API int pb200_predict_sums_host(pb200_ctx* c, const pb200_options* opts, c
                        double* h_sum_upper) {
     const SumOut s = {width_ns, origin_ns, wmax, h_n_windows, h_win_start, h_win_points, h_yhat_sum, h_quantity_sum,
                       h_sum_lower, h_sum_upper};
-    return predict_host(c, opts, h_params, h_tchange, h_meta_i32, h_meta_i64, h_meta_f64, n_models, h_future_ds, horizon,
-                        h_floor, h_cap, seed, h_yhat, h_yhat_lower, h_yhat_upper, h_yhat_int, nullptr, nullptr, nullptr, &s);
+    PredictCall p = {opts, h_params, h_tchange, h_meta_i32, h_meta_i64, h_meta_f64, n_models, h_future_ds,
+                     horizon, h_floor, h_cap, seed, h_yhat, h_yhat_lower, h_yhat_upper, h_yhat_int};
+    p.sums = &s;
+    return predict_host(c, p);
 }
 
 PB200_API int pb200_predict_period_sums_device(pb200_ctx* c, const pb200_options* opts, const double* d_params,
@@ -1692,8 +1717,10 @@ PB200_API int pb200_predict_period_sums_device(pb200_ctx* c, const pb200_options
     s.months = months;
     s.month_shift = month_shift;
     if (months == 0) return fail(PB200_E_ARG, "months must be 1, 3 or 12 and month_shift in [0, months)");
-    return predict_device(c, opts, d_params, d_tchange, d_meta_i32, d_meta_i64, d_meta_f64, n_models, d_future_ds, horizon,
-                          d_floor, d_cap, seed, d_yhat, d_yhat_lower, d_yhat_upper, d_yhat_int, nullptr, nullptr, nullptr, &s);
+    PredictCall p = {opts, d_params, d_tchange, d_meta_i32, d_meta_i64, d_meta_f64, n_models, d_future_ds,
+                     horizon, d_floor, d_cap, seed, d_yhat, d_yhat_lower, d_yhat_upper, d_yhat_int};
+    p.sums = &s;
+    return predict_device(c, p);
 }
 
 PB200_API int pb200_predict_period_sums_host(pb200_ctx* c, const pb200_options* opts, const double* h_params,
@@ -1707,8 +1734,10 @@ PB200_API int pb200_predict_period_sums_host(pb200_ctx* c, const pb200_options* 
     s.months = months;
     s.month_shift = month_shift;
     if (months == 0) return fail(PB200_E_ARG, "months must be 1, 3 or 12 and month_shift in [0, months)");
-    return predict_host(c, opts, h_params, h_tchange, h_meta_i32, h_meta_i64, h_meta_f64, n_models, h_future_ds, horizon,
-                        h_floor, h_cap, seed, h_yhat, h_yhat_lower, h_yhat_upper, h_yhat_int, nullptr, nullptr, nullptr, &s);
+    PredictCall p = {opts, h_params, h_tchange, h_meta_i32, h_meta_i64, h_meta_f64, n_models, h_future_ds,
+                     horizon, h_floor, h_cap, seed, h_yhat, h_yhat_lower, h_yhat_upper, h_yhat_int};
+    p.sums = &s;
+    return predict_host(c, p);
 }
 
 PB200_API int pb200_period_host(const int64_t* ds, int64_t n, int32_t months, int32_t month_shift, int64_t* period,
@@ -1731,9 +1760,10 @@ PB200_API int pb200_predict_quantiles_device(pb200_ctx* c, const pb200_options* 
                          double* d_yhat_upper, int32_t* d_yhat_int, int32_t n_q, const double* h_percentiles,
                          double* d_quantiles) {
     const QuantOut q = {n_q, h_percentiles, d_quantiles};
-    return predict_device(c, opts, d_params, d_tchange, d_meta_i32, d_meta_i64, d_meta_f64, n_models, d_future_ds, horizon,
-                          d_floor, d_cap, seed, d_yhat, d_yhat_lower, d_yhat_upper, d_yhat_int, nullptr, nullptr, nullptr,
-                          nullptr, &q);
+    PredictCall p = {opts, d_params, d_tchange, d_meta_i32, d_meta_i64, d_meta_f64, n_models, d_future_ds,
+                     horizon, d_floor, d_cap, seed, d_yhat, d_yhat_lower, d_yhat_upper, d_yhat_int};
+    p.quant = &q;
+    return predict_device(c, p);
 }
 
 PB200_API int pb200_predict_quantiles_host(pb200_ctx* c, const pb200_options* opts, const double* h_params,
@@ -1743,9 +1773,10 @@ PB200_API int pb200_predict_quantiles_host(pb200_ctx* c, const pb200_options* op
                        double* h_yhat_upper, int32_t* h_yhat_int, int32_t n_q, const double* h_percentiles,
                        double* h_quantiles) {
     const QuantOut q = {n_q, h_percentiles, h_quantiles};
-    return predict_host(c, opts, h_params, h_tchange, h_meta_i32, h_meta_i64, h_meta_f64, n_models, h_future_ds, horizon,
-                        h_floor, h_cap, seed, h_yhat, h_yhat_lower, h_yhat_upper, h_yhat_int, nullptr, nullptr, nullptr,
-                        nullptr, &q);
+    PredictCall p = {opts, h_params, h_tchange, h_meta_i32, h_meta_i64, h_meta_f64, n_models, h_future_ds,
+                     horizon, h_floor, h_cap, seed, h_yhat, h_yhat_lower, h_yhat_upper, h_yhat_int};
+    p.quant = &q;
+    return predict_host(c, p);
 }
 
 // ---- forecast CSV rows formatted on the device (csv_kernel.cuh) ----
@@ -2035,56 +2066,35 @@ PB200_API int pb200_cv_windows_device(pb200_ctx* c, const int64_t* d_ds, const v
 namespace {
 
 // pb200_predict_history_device: pb200_predict_device's checks, then the ragged instances of predict_kernel and mc_kernel
-// over model i's rows [h_offsets[i], h_offsets[i + 1]) of d_ds; the offsets are copied to the device here
-int predict_history_device(pb200_ctx* c, const pb200_options* opts, const double* d_params, const double* d_tchange,
-                           const int32_t* d_meta_i32, const int64_t* d_meta_i64, const double* d_meta_f64,
-                           int64_t n_models, const int64_t* d_ds, const int64_t* h_offsets, const double* d_floor,
-                           const double* d_cap, uint64_t seed, double* d_yhat, double* d_yhat_lower, double* d_yhat_upper) {
+// over model i's rows [p.offsets[i], p.offsets[i + 1]) of p.future_ds (the history's ds; p.horizon is 0); the offsets
+// are copied to the device here
+int predict_history_device(pb200_ctx* c, const PredictCall& p) {
     if (!c) return fail(PB200_E_ARG, "ctx is null");
-    int rc = check_opts(opts);
+    int rc = check_opts(p.opts);
     if (rc) return rc;
+    const int64_t n_models = p.n_models;
     if (n_models < 0 || n_models > (1LL << 30)) return fail(PB200_E_ARG, "sizes");
     if (n_models == 0) return PB200_OK;
-    if (!h_offsets) return fail(PB200_E_ARG, "null pointer (offsets)");
-    if (h_offsets[0] < 0) return fail(PB200_E_ARG, "offsets[0] < 0");
+    if (!p.offsets) return fail(PB200_E_ARG, "null pointer (offsets)");
+    if (p.offsets[0] < 0) return fail(PB200_E_ARG, "offsets[0] < 0");
     int64_t tmax = 0;
     for (int64_t i = 0; i < n_models; ++i) {
-        const int64_t T = h_offsets[i + 1] - h_offsets[i];
+        const int64_t T = p.offsets[i + 1] - p.offsets[i];
         if (T < 0) return fail(PB200_E_ARG, "offsets not monotone");
         if (T > INT32_MAX) return fail(PB200_E_UNSUPPORTED, "a frame longer than 2^31 - 1 rows");
         tmax = std::max(tmax, T);
     }
     if (tmax == 0) return PB200_OK;
-    if (!d_params || !d_tchange || !d_meta_i32 || !d_meta_i64 || !d_meta_f64 || !d_floor || !d_cap || !d_ds || !d_yhat)
+    if (!p.params || !p.tchange || !p.meta_i32 || !p.meta_i64 || !p.meta_f64 || !p.floor || !p.cap || !p.future_ds || !p.yhat)
         return fail(PB200_E_ARG, "null pointer");
-    const bool mc = d_yhat_lower && d_yhat_upper && opts->uncertainty_samples > 0;
-    if (mc && (rc = check_mc_opts(opts))) return rc;
-    pb200_layout L;
-    pb200_get_layout(opts, &L);
+    const bool mc = p.yhat_lower && p.yhat_upper && p.opts->uncertainty_samples > 0;
+    if (mc && (rc = check_mc_opts(p.opts))) return rc;
     CK(cudaSetDevice(c->device));
     const size_t N = (size_t)n_models;
     CK(c->d_hoff.reserve((N + 1) * 8));
-    CK(cudaMemcpyAsync(c->d_hoff.p, h_offsets, (N + 1) * 8, cudaMemcpyHostToDevice, c->stream));
+    CK(cudaMemcpyAsync(c->d_hoff.p, p.offsets, (N + 1) * 8, cudaMemcpyHostToDevice, c->stream));
     pb200::RaggedPredictArgs a;
-    opts_table(opts, &a.tab);
-    a.params = d_params;
-    a.tchange = d_tchange;
-    a.meta_i32 = d_meta_i32;
-    a.meta_i64 = (const long long*)d_meta_i64;
-    a.meta_f64 = d_meta_f64;
-    a.future_ds = (const long long*)d_ds;
-    a.floor = d_floor;
-    a.cap = d_cap;
-    a.n_models = (int)n_models;
-    a.horizon = 0;                 // the frames are the offsets'
-    a.smax = L.smax;
-    a.kmax = L.kmax;
-    a.pstride = L.pstride;
-    a.growth = opts->growth;
-    a.mult = opts->multiplicative ? 1 : 0;
-    a.yhat = d_yhat;
-    a.trend = nullptr;
-    a.yhat_int = nullptr;
+    predict_args(a, p);
     a.offsets = (const long long*)c->d_hoff.p;
     // the fixed frame's geometry over the longest frame: CTAs past a shorter model's rows leave at once
     dim3 grid((unsigned)n_models, (unsigned)std::min<int64_t>((tmax + 1023) / 1024, 64));
@@ -2092,8 +2102,8 @@ int predict_history_device(pb200_ctx* c, const pb200_options* opts, const double
     CK(cudaGetLastError());
     c->launches++;
     if (mc) {
-        rc = pb200::launch_mc_ragged(c->stream, c->sms, a, a.offsets, opts->uncertainty_samples, opts->interval_width, seed,
-                                     d_yhat_lower, d_yhat_upper);
+        rc = pb200::launch_mc_ragged(c->stream, c->sms, a, a.offsets, p.opts->uncertainty_samples, p.opts->interval_width,
+                                     p.seed, p.yhat_lower, p.yhat_upper);
         if (rc == -1) return fail(PB200_E_ARG, "uncertainty_samples / interval_width out of range");
         if (rc) return fail(PB200_E_CUDA, "mc kernel launch", cudaGetLastError());
         c->launches++;
@@ -2110,8 +2120,10 @@ PB200_API int pb200_predict_history_device(pb200_ctx* c, const pb200_options* op
                                            const double* d_meta_f64, int64_t n_models, const int64_t* d_ds,
                                            const int64_t* h_offsets, const double* d_floor, const double* d_cap,
                                            uint64_t seed, double* d_yhat, double* d_yhat_lower, double* d_yhat_upper) {
-    return predict_history_device(c, opts, d_params, d_tchange, d_meta_i32, d_meta_i64, d_meta_f64, n_models, d_ds,
-                                  h_offsets, d_floor, d_cap, seed, d_yhat, d_yhat_lower, d_yhat_upper);
+    PredictCall p = {opts, d_params, d_tchange, d_meta_i32, d_meta_i64, d_meta_f64, n_models, d_ds, 0, d_floor, d_cap,
+                     seed, d_yhat, d_yhat_lower, d_yhat_upper};
+    p.offsets = h_offsets;
+    return predict_history_device(c, p);
 }
 
 PB200_API int pb200_predict_history_host(pb200_ctx* c, const pb200_options* opts, const double* h_params,
@@ -2134,45 +2146,25 @@ PB200_API int pb200_predict_history_host(pb200_ctx* c, const pb200_options* opts
     if (mc && (rc = check_mc_opts(opts))) return rc;
     pb200_layout L;
     pb200_get_layout(opts, &L);
-    CK(cudaSetDevice(c->device));
-    const size_t N = (size_t)n_models, R = (size_t)std::max<int64_t>(rows, 0);
-    CK(c->d_params.reserve(N * L.pstride * 8));
-    CK(c->d_tchange.reserve(N * L.smax * 8));
-    CK(c->d_mi32.reserve(N * 8 * 4));
-    CK(c->d_mi64.reserve(N * 2 * 8));
-    CK(c->d_mf64.reserve(N * 4 * 8));
-    CK(c->d_floor.reserve(N * 8));
-    CK(c->d_cap.reserve(N * 8));
-    CK(c->d_fut.reserve(R * 8));
-    CK(c->d_yhat.reserve(R * 8));
-    if (mc) {
-        CK(c->d_lo.reserve(R * 8));
-        CK(c->d_hi.reserve(R * 8));
-    }
-    cudaStream_t st = c->stream;
-    CK(cudaMemcpyAsync(c->d_params.p, h_params, N * L.pstride * 8, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(c->d_tchange.p, h_tchange, N * L.smax * 8, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(c->d_mi32.p, h_meta_i32, N * 8 * 4, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(c->d_mi64.p, h_meta_i64, N * 2 * 8, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(c->d_mf64.p, h_meta_f64, N * 4 * 8, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(c->d_floor.p, h_floor, N * 8, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(c->d_cap.p, h_cap, N * 8, cudaMemcpyHostToDevice, st));
-    if (R) CK(cudaMemcpyAsync(c->d_fut.p, h_ds, R * 8, cudaMemcpyHostToDevice, st));
-    rc = predict_history_device(c, opts, (const double*)c->d_params.p, (const double*)c->d_tchange.p,
-                                (const int32_t*)c->d_mi32.p, (const int64_t*)c->d_mi64.p, (const double*)c->d_mf64.p,
-                                n_models, (const int64_t*)c->d_fut.p, h_offsets, (const double*)c->d_floor.p,
-                                (const double*)c->d_cap.p, seed, (double*)c->d_yhat.p, mc ? (double*)c->d_lo.p : nullptr,
-                                mc ? (double*)c->d_hi.p : nullptr);
-    if (rc) return rc;
-    if (R) {
-        CK(cudaMemcpyAsync(h_yhat, c->d_yhat.p, R * 8, cudaMemcpyDeviceToHost, st));
-        if (mc) {
-            CK(cudaMemcpyAsync(h_yhat_lower, c->d_lo.p, R * 8, cudaMemcpyDeviceToHost, st));
-            CK(cudaMemcpyAsync(h_yhat_upper, c->d_hi.p, R * 8, cudaMemcpyDeviceToHost, st));
-        }
-    }
-    CK(cudaStreamSynchronize(st));
-    return PB200_OK;
+    const size_t N = (size_t)n_models, R = (size_t)rows;
+    Staging s(c);
+    PredictCall d = {opts};
+    d.params = s.in(ST_PARAMS, h_params, N * L.pstride);
+    d.tchange = s.in(ST_TCHANGE, h_tchange, N * L.smax);
+    d.meta_i32 = s.in(ST_MI32, h_meta_i32, N * 8);
+    d.meta_i64 = s.in(ST_MI64, h_meta_i64, N * 2);
+    d.meta_f64 = s.in(ST_MF64, h_meta_f64, N * 4);
+    d.n_models = n_models;
+    d.future_ds = s.in(ST_FUT, h_ds, R);
+    d.offsets = h_offsets;
+    d.floor = s.in(ST_FLOOR, h_floor, N);
+    d.cap = s.in(ST_CAP, h_cap, N);
+    d.seed = seed;
+    d.yhat = s.out(ST_YHAT, h_yhat, R);
+    d.yhat_lower = s.out(ST_LO, mc ? h_yhat_lower : nullptr, R);
+    d.yhat_upper = s.out(ST_HI, mc ? h_yhat_upper : nullptr, R);
+    if ((rc = s.status()) || (rc = predict_history_device(c, d))) return rc;
+    return s.finish();
 }
 
 static int outlier_grid(const pb200_ctx* c, int64_t n_series) {   // one warp per series, 8 per CTA
