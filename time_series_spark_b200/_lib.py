@@ -116,117 +116,68 @@ def load() -> C.CDLL:
     lib = C.CDLL(LIB_PATH)
     vp, i64, i32, dbl, u64 = C.c_void_p, C.c_int64, C.c_int32, C.c_double, C.c_uint64
     OP = C.POINTER(Options)
-    lib.pb200_default_options.argtypes = [OP]
-    lib.pb200_default_options.restype = None
-    lib.pb200_get_layout.argtypes = [OP, C.POINTER(Layout)]
-    lib.pb200_get_layout.restype = C.c_int
-    lib.pb200_create.argtypes = [C.c_int]
-    lib.pb200_create.restype = vp
-    lib.pb200_destroy.argtypes = [vp]
-    lib.pb200_destroy.restype = None
-    lib.pb200_last_error.argtypes = []
-    lib.pb200_last_error.restype = C.c_char_p
-    lib.pb200_stream.argtypes = [vp]
-    lib.pb200_stream.restype = vp
-    lib.pb200_launch_count.argtypes = [vp]
-    lib.pb200_launch_count.restype = i64
-    lib.pb200_tab_chunk.argtypes = [i32, i32]
-    lib.pb200_tab_chunk.restype = i32
-    lib.pb200_last_fit_variant_counts.argtypes = [vp, vp]
-    lib.pb200_last_fit_table_count.restype = C.c_int
-    lib.pb200_last_fit_table_count.argtypes = [vp, vp]
-    lib.pb200_component_count.restype = i32
-    lib.pb200_component_count.argtypes = [OP]
-    lib.pb200_last_fit_variant_counts.restype = C.c_int
     fit_args = [vp, OP, vp, vp, i32, vp, i64, dbl, dbl, vp, vp, vp, vp, vp, vp]
-    lib.pb200_fit_device.argtypes = fit_args
-    lib.pb200_fit_device.restype = C.c_int
-    lib.pb200_fit_prior_device.argtypes = fit_args[:10] + [vp] + fit_args[10:]
-    lib.pb200_fit_prior_device.restype = C.c_int
-    lib.pb200_fit_warm_device.argtypes = fit_args[:10] + [vp, vp, vp] + fit_args[10:] + [vp]
-    lib.pb200_fit_warm_device.restype = C.c_int
-    lib.pb200_fit_warm_host.argtypes = fit_args[:10] + [vp, vp, vp] + fit_args[10:] + [vp, vp, i32]
-    lib.pb200_fit_warm_host.restype = C.c_int
-    lib.pb200_fit_host.argtypes = fit_args
-    lib.pb200_fit_host.restype = C.c_int
     pred_args = [vp, OP, vp, vp, vp, vp, vp, i64, vp, i32, vp, vp, u64, vp, vp, vp, vp]
-    lib.pb200_predict_device.argtypes = pred_args
-    lib.pb200_predict_device.restype = C.c_int
-    lib.pb200_predict_host.argtypes = pred_args
-    lib.pb200_predict_host.restype = C.c_int
-    lib.pb200_predict_components_device.argtypes = pred_args + [vp, vp, vp]
-    lib.pb200_predict_components_device.restype = C.c_int
-    lib.pb200_predict_components_host.argtypes = pred_args + [vp, vp, vp]
-    lib.pb200_predict_components_host.restype = C.c_int
-    lib.pb200_predict_sums_device.argtypes = pred_args + [i64, i64, i32, vp, vp, vp, vp, vp, vp, vp]
-    lib.pb200_predict_sums_device.restype = C.c_int
-    lib.pb200_predict_sums_host.argtypes = pred_args + [i64, i64, i32, vp, vp, vp, vp, vp, vp, vp]
-    lib.pb200_predict_sums_host.restype = C.c_int
-    lib.pb200_predict_sums_anchored_device.argtypes = pred_args + [i64, vp, vp, i32, vp, vp, vp, vp, vp, vp, vp]
-    lib.pb200_predict_sums_anchored_device.restype = C.c_int
-    lib.pb200_predict_period_sums_device.argtypes = pred_args + [i32, i32, i32, vp, vp, vp, vp, vp, vp, vp]
-    lib.pb200_predict_period_sums_device.restype = C.c_int
-    lib.pb200_predict_period_sums_host.argtypes = pred_args + [i32, i32, i32, vp, vp, vp, vp, vp, vp, vp]
-    lib.pb200_predict_period_sums_host.restype = C.c_int
-    lib.pb200_period_host.argtypes = [vp, i64, i32, i32, vp, vp]
-    lib.pb200_period_host.restype = C.c_int
-    lib.pb200_predict_quantiles_device.argtypes = pred_args + [i32, vp, vp]
-    lib.pb200_predict_quantiles_device.restype = C.c_int
-    lib.pb200_predict_quantiles_host.argtypes = pred_args + [i32, vp, vp]
-    lib.pb200_predict_quantiles_host.restype = C.c_int
     hist_args = [vp, OP, vp, vp, vp, vp, vp, i64, vp, vp, vp, vp, u64, vp, vp, vp]
-    lib.pb200_predict_history_device.argtypes = hist_args
-    lib.pb200_predict_history_device.restype = C.c_int
-    lib.pb200_predict_history_host.argtypes = hist_args
-    lib.pb200_predict_history_host.restype = C.c_int
-    lib.pb200_outlier_counts_device.argtypes = [vp, vp, i32, vp, i64, vp, vp, vp, vp]
-    lib.pb200_outlier_counts_device.restype = C.c_int
-    lib.pb200_outlier_compact_device.argtypes = [vp, vp, vp, i32, vp, i64, vp, vp, vp, vp]
-    lib.pb200_outlier_compact_device.restype = C.c_int
-    lib.pb200_make_future_device.argtypes = [vp, vp, i64, i32, i64, vp]
-    lib.pb200_make_future_device.restype = C.c_int
-    lib.pb200_objective_host.argtypes = [vp, OP, vp, vp, i32, vp, i64, dbl, dbl, vp, vp, vp, vp]
-    lib.pb200_objective_host.restype = C.c_int
-    lib.pb200_objective_regressors_host.argtypes = [vp, OP, vp, vp, i32, vp, i64, dbl, dbl, vp, vp, vp, vp, vp, vp]
-    lib.pb200_objective_regressors_host.restype = C.c_int
-    lib.pb200_fit_regressors_device.argtypes = fit_args[:10] + [vp, vp] + fit_args[10:]
-    lib.pb200_fit_regressors_device.restype = C.c_int
-    lib.pb200_fit_regressors_host.argtypes = fit_args[:10] + [vp, vp] + fit_args[10:] + [vp, i32]
-    lib.pb200_fit_regressors_host.restype = C.c_int
-    lib.pb200_predict_regressors_device.argtypes = pred_args[:13] + [vp, vp] + pred_args[13:]
-    lib.pb200_predict_regressors_device.restype = C.c_int
-    lib.pb200_predict_regressors_host.argtypes = pred_args[:13] + [vp, vp] + pred_args[13:]
-    lib.pb200_predict_regressors_host.restype = C.c_int
-    lib.pb200_join_future_regressors_device.argtypes = [vp, vp, vp, vp, i64, i32, vp, vp, i64, i32, vp, vp, vp]
-    lib.pb200_join_future_regressors_device.restype = C.c_int
-    lib.pb200_regressor_scales_device.argtypes = [vp, OP, vp, vp, i64, vp, vp]
-    lib.pb200_regressor_scales_device.restype = C.c_int
-    lib.pb200_cv_gather_regressors_device.argtypes = [vp, vp, i64, i32, vp, vp, vp, vp, vp, vp, i64, vp, i32, vp, vp]
-    lib.pb200_cv_gather_regressors_device.restype = C.c_int
-    lib.pb200_fit_regressors_copy_device.argtypes = fit_args[:10] + [vp, vp, vp] + fit_args[10:]
-    lib.pb200_fit_regressors_copy_device.restype = C.c_int
-    lib.pb200_fit_trace_host.argtypes = [vp, OP, vp, vp, i32, vp, i64, dbl, dbl, vp, vp, vp, vp, vp, vp, i32]
-    lib.pb200_fit_trace_host.restype = C.c_int
-    lib.pb200_forecast_csv_lengths_device.argtypes = [vp, vp, vp, vp, i64, i32, vp]
-    lib.pb200_forecast_csv_lengths_device.restype = C.c_int
-    lib.pb200_forecast_csv_rows_device.argtypes = [vp, vp, vp, vp, vp, i64, C.c_char_p, i32, vp, vp]
-    lib.pb200_forecast_csv_rows_device.restype = C.c_int
-    lib.pb200_forecast_csv_row_host.argtypes = [i32, i32, i64, i32, C.c_char_p, i32, C.c_char_p]
-    lib.pb200_forecast_csv_row_host.restype = i32
-    lib.pb200_cv_plan_counts_device.argtypes = [vp, OP, vp, vp, i64, i64, i64, i64, vp, vp, vp]
-    lib.pb200_cv_plan_counts_device.restype = C.c_int
-    lib.pb200_cv_plan_device.argtypes = [vp, OP, vp, vp, i64, i64, i64, i64, vp, vp, vp, vp, vp, vp]
-    lib.pb200_cv_plan_device.restype = C.c_int
-    lib.pb200_cv_gather_device.argtypes = [vp, vp, vp, i32, vp, vp, vp, vp, vp, i64, vp, i32, vp, vp, vp]
-    lib.pb200_cv_gather_device.restype = C.c_int
-    lib.pb200_cv_metrics_device.argtypes = [vp, vp, vp, vp, vp, vp, vp, vp, i64, dbl, vp, vp, vp, vp, vp, vp, vp, vp]
-    lib.pb200_cv_metrics_device.restype = C.c_int
-    lib.pb200_cv_windows_device.argtypes = [vp, vp, vp, i32, vp, vp, vp, vp, i64, vp, i32, i64, i32, vp, vp, vp, vp, vp]
-    lib.pb200_cv_windows_device.restype = C.c_int
-    lib.pb200_cv_quantile_metrics_device.argtypes = [vp, vp, vp, vp, i64, i32, vp, vp, vp, i64, dbl, vp, vp, vp, vp, vp]
-    lib.pb200_cv_quantile_metrics_device.restype = C.c_int
-    lib.pb200_synchronize.argtypes = [vp]
-    lib.pb200_synchronize.restype = C.c_int
+    twins = {      # the same arguments at both suffixes, _host and _device
+        "pb200_predict": pred_args,
+        "pb200_predict_components": pred_args + [vp, vp, vp],
+        "pb200_predict_sums": pred_args + [i64, i64, i32] + [vp] * 7,
+        "pb200_predict_period_sums": pred_args + [i32, i32, i32] + [vp] * 7,
+        "pb200_predict_quantiles": pred_args + [i32, vp, vp],
+        "pb200_predict_history": hist_args,
+        "pb200_predict_regressors": pred_args[:13] + [vp, vp] + pred_args[13:],
+    }
+    prototypes = {name + s: args for name, args in twins.items() for s in ("_host", "_device")}
+    prototypes.update({
+        "pb200_default_options": [OP],
+        "pb200_get_layout": [OP, C.POINTER(Layout)],
+        "pb200_create": [C.c_int],
+        "pb200_destroy": [vp],
+        "pb200_last_error": [],
+        "pb200_stream": [vp],
+        "pb200_launch_count": [vp],
+        "pb200_tab_chunk": [i32, i32],
+        "pb200_last_fit_variant_counts": [vp, vp],
+        "pb200_last_fit_table_count": [vp, vp],
+        "pb200_component_count": [OP],
+        "pb200_synchronize": [vp],
+        "pb200_fit_device": fit_args,
+        "pb200_fit_host": fit_args,
+        "pb200_fit_prior_device": fit_args[:10] + [vp] + fit_args[10:],
+        "pb200_fit_warm_device": fit_args[:10] + [vp, vp, vp] + fit_args[10:] + [vp],
+        "pb200_fit_warm_host": fit_args[:10] + [vp, vp, vp] + fit_args[10:] + [vp, vp, i32],
+        "pb200_fit_trace_host": fit_args[:9] + fit_args[10:] + [vp, i32],
+        "pb200_fit_regressors_device": fit_args[:10] + [vp, vp] + fit_args[10:],
+        "pb200_fit_regressors_copy_device": fit_args[:10] + [vp, vp, vp] + fit_args[10:],
+        "pb200_fit_regressors_host": fit_args[:10] + [vp, vp] + fit_args[10:] + [vp, i32],
+        "pb200_objective_host": fit_args[:9] + [vp, vp, vp, vp],
+        "pb200_objective_regressors_host": fit_args[:9] + [vp, vp, vp, vp, vp, vp],
+        "pb200_predict_sums_anchored_device": pred_args + [i64, vp, vp, i32] + [vp] * 7,
+        "pb200_period_host": [vp, i64, i32, i32, vp, vp],
+        "pb200_make_future_device": [vp, vp, i64, i32, i64, vp],
+        "pb200_outlier_counts_device": [vp, vp, i32, vp, i64, vp, vp, vp, vp],
+        "pb200_outlier_compact_device": [vp, vp, vp, i32, vp, i64, vp, vp, vp, vp],
+        "pb200_join_future_regressors_device": [vp, vp, vp, vp, i64, i32, vp, vp, i64, i32, vp, vp, vp],
+        "pb200_regressor_scales_device": [vp, OP, vp, vp, i64, vp, vp],
+        "pb200_cv_gather_regressors_device": [vp, vp, i64, i32, vp, vp, vp, vp, vp, vp, i64, vp, i32, vp, vp],
+        "pb200_forecast_csv_lengths_device": [vp, vp, vp, vp, i64, i32, vp],
+        "pb200_forecast_csv_rows_device": [vp, vp, vp, vp, vp, i64, C.c_char_p, i32, vp, vp],
+        "pb200_forecast_csv_row_host": [i32, i32, i64, i32, C.c_char_p, i32, C.c_char_p],
+        "pb200_cv_plan_counts_device": [vp, OP, vp, vp, i64, i64, i64, i64, vp, vp, vp],
+        "pb200_cv_plan_device": [vp, OP, vp, vp, i64, i64, i64, i64, vp, vp, vp, vp, vp, vp],
+        "pb200_cv_gather_device": [vp, vp, vp, i32, vp, vp, vp, vp, vp, i64, vp, i32, vp, vp, vp],
+        "pb200_cv_metrics_device": [vp, vp, vp, vp, vp, vp, vp, vp, i64, dbl] + [vp] * 8,
+        "pb200_cv_windows_device": [vp, vp, vp, i32, vp, vp, vp, vp, i64, vp, i32, i64, i32, vp, vp, vp, vp, vp],
+        "pb200_cv_quantile_metrics_device": [vp, vp, vp, vp, i64, i32, vp, vp, vp, i64, dbl, vp, vp, vp, vp, vp],
+    })
+    restypes = {"pb200_default_options": None, "pb200_destroy": None, "pb200_create": vp, "pb200_last_error": C.c_char_p,
+                "pb200_stream": vp, "pb200_launch_count": i64, "pb200_tab_chunk": i32, "pb200_component_count": i32,
+                "pb200_forecast_csv_row_host": i32}     # every other entry point returns an int status
+    for name, args in prototypes.items():
+        f = getattr(lib, name)
+        f.argtypes = args
+        f.restype = restypes.get(name, C.c_int)
     _lib = lib
     return lib
 

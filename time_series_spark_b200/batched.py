@@ -437,59 +437,149 @@ def _check_reg_scale(reg_scale, n: int, R: int, what: str, dev=None) -> None:
                          + (f" on {dev}" if dev is not None else "") + f" (got {dt} {tuple(reg_scale.shape)})")
 
 
+class _Space:
+    """Where a call's arrays live: numpy on the host (``dev`` None), or torch tensors on the device ``dev``.  The
+    entry points of a call family differ only in this, and in their suffix."""
+
+    def __init__(self, dev=None):
+        self.dev = dev
+        self.suffix = "_host" if dev is None else "_device"
+
+    def empty(self, shape, dtype: str):
+        if self.dev is None:
+            return np.empty(shape, dtype)
+        import torch
+        return torch.empty(shape, dtype=getattr(torch, dtype), device=self.dev)
+
+    def zeros(self, shape, dtype: str):
+        if self.dev is None:
+            return np.zeros(shape, dtype)
+        import torch
+        return torch.zeros(shape, dtype=getattr(torch, dtype), device=self.dev)
+
+    def asarray(self, a, dtype: str):
+        """``a`` (numpy, or a torch tensor for a device call) as a contiguous ``dtype`` array here; a copy only where
+        needed."""
+        if self.dev is None:
+            return np.ascontiguousarray(a, dtype=dtype)
+        import torch
+        return torch.as_tensor(a, dtype=getattr(torch, dtype), device=self.dev).contiguous()
+
+    def ptr(self, a):
+        if a is None:
+            return None
+        return a.ctypes.data if self.dev is None else a.data_ptr()
+
+    def sync_torch(self) -> None:
+        """Before a device call: its inputs were produced on torch's current stream; the library has its own stream."""
+        if self.dev is not None:
+            import torch
+            torch.cuda.current_stream(self.dev).synchronize()
+
+
+_HOST = _Space()
+
+
+def _call(entry: str, *args) -> None:
+    L.check(getattr(L.load(), entry)(*args), entry)
+
+
+_FIT_FIELDS = ("params", "tchange", "meta_i32", "meta_i64", "meta_f64")
+
+
+def _fitted_outputs(space: _Space, n: int, lay, R: int = 0, zeros: bool = False) -> FittedBatch:
+    """A FittedBatch for ``n`` series of layout ``lay`` for a fit to write, with ``reg_scale`` when R > 0.  ``zeros``:
+    params and tchange start zero-filled (a fit narrower than ``lay`` leaves their pad columns at 0)."""
+    pad = space.zeros if zeros else space.empty
+    return FittedBatch(pad((n, lay.pstride), "float64"), pad((n, lay.smax), "float64"), space.empty((n, 8), "int32"),
+                       space.empty((n, 2), "int64"), space.empty((n, 4), "float64"), lay.smax, lay.kmax,
+                       reg_scale=space.empty((n, R, 2), "float64") if R else None)
+
+
+def _fit(space: _Space, ctx, opts, ds_ns, y, offsets, floor, cap_multiplier, kind: str, cap=None, prior=None,
+         init=None, regressors=None, reg_scale_copy=None, trace_cap: int = 0, out=None, sync: bool = False):
+    """The body of the fit wrappers: pb200_fit[_<kind>][_copy]_host / _device, ``kind`` "fit", "trace" or "warm", or
+    "regressors" whenever ``regressors`` is given.  A host call converts its inputs and returns a trace array for the
+    trace, and for the warm and regressor fits with ``trace_cap`` > 0; a device call checks its inputs and synchronises
+    the context after the call with ``sync`` or ``init``.  Returns (FittedBatch, trace or None)."""
+    host = space.dev is None
+    if host:
+        ds_ns, y = np.ascontiguousarray(ds_ns, dtype=np.int64), np.ascontiguousarray(y)
+    offsets = np.ascontiguousarray(offsets, dtype=np.int64)
+    n = offsets.size - 1
+    lay = L.get_layout(opts)
+    R = 0
+    if reg_scale_copy is not None and regressors is None:
+        raise ValueError("reg_scale_copy goes with regressors")
+    if regressors is not None:
+        if prior is not None or init is not None:
+            raise ValueError("regressors are not supported with prior or init")
+        kind, R = "regressors", n_regressors(opts)
+        if host:
+            regressors = _host_regressors(opts, regressors, ds_ns.size)
+        else:
+            import torch
+            rows = int(offsets[-1])
+            if (regressors.dtype != torch.float64 or tuple(regressors.shape) != (R, rows)
+                    or not regressors.is_contiguous() or regressors.device != space.dev):
+                raise ValueError(f"regressors must be a contiguous float64 tensor of shape ({R}, {rows}) on {space.dev}")
+    if init is not None:
+        _check_init(init, n, lay)
+    if out is None:
+        out = _fitted_outputs(space, n, lay, R)
+    if R:
+        if out.reg_scale is None:
+            out.reg_scale = space.empty((n, R, 2), "float64")
+        if not host:
+            _check_reg_scale(out.reg_scale, n, R, "out.reg_scale", space.dev)
+            if reg_scale_copy is not None:
+                _check_reg_scale(reg_scale_copy, n, R, "reg_scale_copy", space.dev)
+    ip = im = None
+    if init is not None:
+        src = init.to_host() if host else init
+        ip, im = space.asarray(src.params, "float64"), space.asarray(src.meta_i32, "int32")
+        if out.warm is None:
+            out.warm = space.empty(n, "int32")
+    if host:
+        if cap is not None:
+            cap = np.ascontiguousarray(cap, dtype=np.float64)
+        if prior is not None:
+            prior = np.ascontiguousarray(prior, dtype=np.float64).reshape(n, 2)
+    trace = space.zeros((n, trace_cap, 4), "float64") if kind == "trace" or trace_cap > 0 else None
+    if n > 0:
+        if not host:
+            import torch
+            if prior is not None and (prior.dtype != torch.float64 or tuple(prior.shape) != (n, 2)
+                                      or not prior.is_contiguous() or prior.device != space.dev):
+                raise ValueError(f"prior must be a contiguous float64 tensor of shape ({n}, 2) on {space.dev}")
+            space.sync_torch()
+        p = space.ptr
+        args = [ctx.handle, C.byref(opts), p(ds_ns), p(y), _y_dtype(y), _np_ptr(offsets), n, float(floor),
+                float(cap_multiplier)]
+        if kind != "trace":
+            args.append(p(cap))
+        if kind == "warm":
+            args += [p(prior), p(ip), p(im)]
+        if kind == "regressors":
+            args += [p(regressors)] + ([p(reg_scale_copy)] if reg_scale_copy is not None else []) + [p(out.reg_scale)]
+        args += [p(getattr(out, f)) for f in _FIT_FIELDS]
+        if kind == "warm":
+            args.append(p(out.warm) if init is not None else None)
+        if host and kind != "fit":
+            args += [p(trace), int(trace_cap)]
+        entry = "pb200_fit" + ("" if kind == "fit" else "_" + kind) + ("_copy" if reg_scale_copy is not None else "")
+        _call(entry + space.suffix, *args)
+        if not host and (sync or init is not None):       # (the uploaded copies of init must outlive the call)
+            ctx.synchronize()
+    return out, trace
+
+
 def fit_batch_host(ctx: L.Context, opts: L.Options, ds_ns: np.ndarray, y: np.ndarray, offsets: np.ndarray,
                    floor: float, cap_multiplier: float, cap: Optional[np.ndarray] = None, regressors=None) -> FittedBatch:
     """pb200_fit_host: numpy (ideally pinned) buffers in, numpy out; copies inside the call.  ``regressors``: None, or
     for options with regressors (make_regressor_options) their values ``[R, n_rows]`` aligned with ``ds_ns``
     (pb200_fit_regressors_host); ``FittedBatch.reg_scale`` then holds each series' standardisation."""
-    if regressors is not None:
-        return _fit_regressors_host(ctx, opts, ds_ns, y, offsets, floor, cap_multiplier, cap, regressors, 0)[0]
-    ds_ns = np.ascontiguousarray(ds_ns, dtype=np.int64)
-    y = np.ascontiguousarray(y)
-    offsets = np.ascontiguousarray(offsets, dtype=np.int64)
-    n = offsets.size - 1
-    lay = L.get_layout(opts)
-    params = np.empty((n, lay.pstride), np.float64)
-    tchange = np.empty((n, lay.smax), np.float64)
-    mi32 = np.empty((n, 8), np.int32)
-    mi64 = np.empty((n, 2), np.int64)
-    mf64 = np.empty((n, 4), np.float64)
-    capp = None
-    if cap is not None:
-        cap = np.ascontiguousarray(cap, dtype=np.float64)
-        capp = _np_ptr(cap)
-    if n > 0:
-        rc = L.load().pb200_fit_host(ctx.handle, C.byref(opts), _np_ptr(ds_ns), _np_ptr(y), _y_dtype(y),
-                                     _np_ptr(offsets), n, float(floor), float(cap_multiplier), capp,
-                                     _np_ptr(params), _np_ptr(tchange), _np_ptr(mi32), _np_ptr(mi64), _np_ptr(mf64))
-        L.check(rc, "pb200_fit_host")
-    return FittedBatch(params, tchange, mi32, mi64, mf64, lay.smax, lay.kmax)
-
-
-def _fit_regressors_host(ctx, opts, ds_ns, y, offsets, floor, cap_multiplier, cap, regressors, trace_cap: int):
-    ds_ns = np.ascontiguousarray(ds_ns, dtype=np.int64)
-    y = np.ascontiguousarray(y)
-    offsets = np.ascontiguousarray(offsets, dtype=np.int64)
-    n = offsets.size - 1
-    lay = L.get_layout(opts)
-    reg = _host_regressors(opts, regressors, ds_ns.size)
-    params = np.empty((n, lay.pstride), np.float64)
-    tchange = np.empty((n, lay.smax), np.float64)
-    mi32 = np.empty((n, 8), np.int32)
-    mi64 = np.empty((n, 2), np.int64)
-    mf64 = np.empty((n, 4), np.float64)
-    rsc = np.empty((n, reg.shape[0], 2), np.float64)
-    trace = np.zeros((n, trace_cap, 4), np.float64) if trace_cap > 0 else None
-    if cap is not None:
-        cap = np.ascontiguousarray(cap, dtype=np.float64)
-    if n > 0:
-        ptr = lambda a: None if a is None else _np_ptr(a)     # noqa: E731
-        rc = L.load().pb200_fit_regressors_host(ctx.handle, C.byref(opts), _np_ptr(ds_ns), _np_ptr(y), _y_dtype(y),
-                                                _np_ptr(offsets), n, float(floor), float(cap_multiplier), ptr(cap),
-                                                _np_ptr(reg), _np_ptr(rsc), _np_ptr(params), _np_ptr(tchange),
-                                                _np_ptr(mi32), _np_ptr(mi64), _np_ptr(mf64), ptr(trace), int(trace_cap))
-        L.check(rc, "pb200_fit_regressors_host")
-    return FittedBatch(params, tchange, mi32, mi64, mf64, lay.smax, lay.kmax, reg_scale=rsc), trace
+    return _fit(_HOST, ctx, opts, ds_ns, y, offsets, floor, cap_multiplier, "fit", cap=cap, regressors=regressors)[0]
 
 
 def fit_batch_trace_host(ctx: L.Context, opts: L.Options, ds_ns: np.ndarray, y: np.ndarray, offsets: np.ndarray,
@@ -497,26 +587,8 @@ def fit_batch_trace_host(ctx: L.Context, opts: L.Options, ds_ns: np.ndarray, y: 
     """pb200_fit_trace_host (parity-test hook): the fit plus, per series, one row
     ``(iteration, f_k, alpha_k, n_evals)`` per accepted L-BFGS iteration (``[n, trace_cap, 4]``).  ``regressors``: as
     fit_batch_host's (pb200_fit_regressors_host with the trajectory)."""
-    if regressors is not None:
-        return _fit_regressors_host(ctx, opts, ds_ns, y, offsets, floor, cap_multiplier, None, regressors, int(trace_cap))
-    ds_ns = np.ascontiguousarray(ds_ns, dtype=np.int64)
-    y = np.ascontiguousarray(y)
-    offsets = np.ascontiguousarray(offsets, dtype=np.int64)
-    n = offsets.size - 1
-    lay = L.get_layout(opts)
-    params = np.empty((n, lay.pstride), np.float64)
-    tchange = np.empty((n, lay.smax), np.float64)
-    mi32 = np.empty((n, 8), np.int32)
-    mi64 = np.empty((n, 2), np.int64)
-    mf64 = np.empty((n, 4), np.float64)
-    trace = np.zeros((n, trace_cap, 4), np.float64)
-    if n > 0:
-        rc = L.load().pb200_fit_trace_host(ctx.handle, C.byref(opts), _np_ptr(ds_ns), _np_ptr(y), _y_dtype(y),
-                                           _np_ptr(offsets), n, float(floor), float(cap_multiplier),
-                                           _np_ptr(params), _np_ptr(tchange), _np_ptr(mi32), _np_ptr(mi64), _np_ptr(mf64),
-                                           _np_ptr(trace), int(trace_cap))
-        L.check(rc, "pb200_fit_trace_host")
-    return FittedBatch(params, tchange, mi32, mi64, mf64, lay.smax, lay.kmax), trace
+    return _fit(_HOST, ctx, opts, ds_ns, y, offsets, floor, cap_multiplier, "trace", regressors=regressors,
+                trace_cap=int(trace_cap))
 
 
 def fit_batch_warm_host(ctx: L.Context, opts: L.Options, ds_ns: np.ndarray, y: np.ndarray, offsets: np.ndarray,
@@ -525,38 +597,8 @@ def fit_batch_warm_host(ctx: L.Context, opts: L.Options, ds_ns: np.ndarray, y: n
     """pb200_fit_warm_host: ``fit_batch_device(init=...)`` on numpy buffers, plus (``trace_cap`` > 0) the trajectory rows
     of ``fit_batch_trace_host``.  Returns ``(FittedBatch, trace or None)``; ``FittedBatch.warm`` holds the
     ``L.WARM_*`` codes when ``init`` is given."""
-    ds_ns = np.ascontiguousarray(ds_ns, dtype=np.int64)
-    y = np.ascontiguousarray(y)
-    offsets = np.ascontiguousarray(offsets, dtype=np.int64)
-    n = offsets.size - 1
-    lay = L.get_layout(opts)
-    params = np.empty((n, lay.pstride), np.float64)
-    tchange = np.empty((n, lay.smax), np.float64)
-    mi32 = np.empty((n, 8), np.int32)
-    mi64 = np.empty((n, 2), np.int64)
-    mf64 = np.empty((n, 4), np.float64)
-    warm = trace = None
-    ip = im = None
-    if init is not None:
-        _check_init(init, n, lay)
-        init = init.to_host()
-        ip = np.ascontiguousarray(init.params, dtype=np.float64)
-        im = np.ascontiguousarray(init.meta_i32, dtype=np.int32)
-        warm = np.empty(n, np.int32)
-    if cap is not None:
-        cap = np.ascontiguousarray(cap, dtype=np.float64)
-    if prior is not None:
-        prior = np.ascontiguousarray(prior, dtype=np.float64).reshape(n, 2)
-    if trace_cap > 0:
-        trace = np.zeros((n, trace_cap, 4), np.float64)
-    if n > 0:
-        ptr = lambda a: None if a is None else _np_ptr(a)     # noqa: E731
-        rc = L.load().pb200_fit_warm_host(ctx.handle, C.byref(opts), _np_ptr(ds_ns), _np_ptr(y), _y_dtype(y),
-                                          _np_ptr(offsets), n, float(floor), float(cap_multiplier), ptr(cap), ptr(prior),
-                                          ptr(ip), ptr(im), _np_ptr(params), _np_ptr(tchange), _np_ptr(mi32), _np_ptr(mi64),
-                                          _np_ptr(mf64), ptr(warm), ptr(trace), int(trace_cap))
-        L.check(rc, "pb200_fit_warm_host")
-    return FittedBatch(params, tchange, mi32, mi64, mf64, lay.smax, lay.kmax, warm=warm), trace
+    return _fit(_HOST, ctx, opts, ds_ns, y, offsets, floor, cap_multiplier, "warm", cap=cap, prior=prior, init=init,
+                trace_cap=trace_cap)
 
 
 def regressor_scales_device(ctx: L.Context, opts, regressors, offsets_host: np.ndarray):
@@ -596,80 +638,8 @@ def fit_batch_device(ctx: L.Context, opts: L.Options, ds_ns, y, offsets_host: np
     then receives each series' standardisation ``[n, R, 2]``.  ``reg_scale_copy`` (with ``regressors``): a float64 CUDA
     tensor ``[n, R, 2]``, the (mu, std) each regressor keeps where it is not standardised instead of (0, 1)
     (pb200_fit_regressors_copy_device; the backtest's prophet_copy, DESIGN §20)."""
-    import torch
-    offsets_host = np.ascontiguousarray(offsets_host, dtype=np.int64)
-    n = offsets_host.size - 1
-    lay = L.get_layout(opts)
-    dev = ds_ns.device
-    if reg_scale_copy is not None and regressors is None:
-        raise ValueError("reg_scale_copy goes with regressors")
-    if regressors is not None:
-        if prior is not None or init is not None:
-            raise ValueError("regressors are not supported with prior or init")
-        R = n_regressors(opts)
-        rows = int(offsets_host[-1])
-        if (regressors.dtype != torch.float64 or tuple(regressors.shape) != (R, rows) or not regressors.is_contiguous()
-                or regressors.device != dev):
-            raise ValueError(f"regressors must be a contiguous float64 tensor of shape ({R}, {rows}) on {dev}")
-        if out is None:
-            out = FittedBatch(torch.empty((n, lay.pstride), dtype=torch.float64, device=dev),
-                              torch.empty((n, lay.smax), dtype=torch.float64, device=dev),
-                              torch.empty((n, 8), dtype=torch.int32, device=dev),
-                              torch.empty((n, 2), dtype=torch.int64, device=dev),
-                              torch.empty((n, 4), dtype=torch.float64, device=dev), lay.smax, lay.kmax)
-        if out.reg_scale is None:
-            out.reg_scale = torch.empty((n, R, 2), dtype=torch.float64, device=dev)
-        _check_reg_scale(out.reg_scale, n, R, "out.reg_scale", dev)
-        if reg_scale_copy is not None:
-            _check_reg_scale(reg_scale_copy, n, R, "reg_scale_copy", dev)
-        if n > 0:
-            torch.cuda.current_stream(dev).synchronize()
-            lib = L.load()
-            head = (ctx.handle, C.byref(opts), ds_ns.data_ptr(), y.data_ptr(), _y_dtype(y), _np_ptr(offsets_host), n,
-                    float(floor), float(cap_multiplier), cap.data_ptr() if cap is not None else None, regressors.data_ptr())
-            tail = (out.reg_scale.data_ptr(), out.params.data_ptr(), out.tchange.data_ptr(), out.meta_i32.data_ptr(),
-                    out.meta_i64.data_ptr(), out.meta_f64.data_ptr())
-            if reg_scale_copy is not None:
-                rc = lib.pb200_fit_regressors_copy_device(*head, reg_scale_copy.data_ptr(), *tail)
-                L.check(rc, "pb200_fit_regressors_copy_device")
-            else:
-                L.check(lib.pb200_fit_regressors_device(*head, *tail), "pb200_fit_regressors_device")
-            if sync:
-                ctx.synchronize()
-        return out
-    if init is not None:
-        _check_init(init, n, lay)
-    if out is None:
-        out = FittedBatch(torch.empty((n, lay.pstride), dtype=torch.float64, device=dev),
-                          torch.empty((n, lay.smax), dtype=torch.float64, device=dev),
-                          torch.empty((n, 8), dtype=torch.int32, device=dev),
-                          torch.empty((n, 2), dtype=torch.int64, device=dev),
-                          torch.empty((n, 4), dtype=torch.float64, device=dev), lay.smax, lay.kmax)
-    ip = im = None
-    if init is not None:
-        ip = torch.as_tensor(init.params, dtype=torch.float64, device=dev).contiguous()
-        im = torch.as_tensor(init.meta_i32, dtype=torch.int32, device=dev).contiguous()
-        if out.warm is None:
-            out.warm = torch.empty(n, dtype=torch.int32, device=dev)
-    if n > 0:
-        # inputs were produced on torch's current stream; the library has its own stream
-        if prior is not None and (prior.dtype != torch.float64 or tuple(prior.shape) != (n, 2) or not prior.is_contiguous()
-                                  or prior.device != dev):
-            raise ValueError(f"prior must be a contiguous float64 tensor of shape ({n}, 2) on {dev}")
-        torch.cuda.current_stream(dev).synchronize()
-        rc = L.load().pb200_fit_warm_device(ctx.handle, C.byref(opts), ds_ns.data_ptr(), y.data_ptr(), _y_dtype(y),
-                                            _np_ptr(offsets_host), n, float(floor), float(cap_multiplier),
-                                            cap.data_ptr() if cap is not None else None,
-                                            prior.data_ptr() if prior is not None else None,
-                                            ip.data_ptr() if ip is not None else None,
-                                            im.data_ptr() if im is not None else None,
-                                            out.params.data_ptr(), out.tchange.data_ptr(), out.meta_i32.data_ptr(),
-                                            out.meta_i64.data_ptr(), out.meta_f64.data_ptr(),
-                                            out.warm.data_ptr() if init is not None else None)
-        L.check(rc, "pb200_fit_warm_device")
-        if sync or init is not None:       # (the uploaded copies of init must outlive the call)
-            ctx.synchronize()
-    return out
+    return _fit(_Space(ds_ns.device), ctx, opts, ds_ns, y, offsets_host, floor, cap_multiplier, "warm", cap=cap,
+                prior=prior, init=init, regressors=regressors, reg_scale_copy=reg_scale_copy, out=out, sync=sync)[0]
 
 
 @dataclass
@@ -799,6 +769,90 @@ def forecast_csv_row_host(series_id: int, dim_id: int, ds_ns: int, quantity: int
     return buf.raw[:n]
 
 
+def _predict_head(space: _Space, ctx, opts, fitted: FittedBatch, grid, floor, cap, seed, shape, bounds: bool,
+                  yint: bool = True, out: Optional["ForecastBatch"] = None):
+    """What every predict entry point starts with: the arguments (handle, options, fitted's five arrays, n, the two
+    ``grid`` arguments, floor, cap, seed) and the outputs it writes first, yhat, the bounds (with ``bounds``, else None)
+    and (with ``yint``) yhat_int, each of ``shape``, or ``out``'s.  A host call takes ``fitted`` as contiguous numpy and
+    floor / cap broadcast to one float64 per model.  Returns (args, (yhat, lower, upper, yhat_int))."""
+    n = fitted.n
+    if space.dev is None:
+        fitted = fitted.to_host()
+        floor, cap = (np.ascontiguousarray(np.broadcast_to(np.asarray(v, dtype=np.float64), (n,))) for v in (floor, cap))
+        models = [np.ascontiguousarray(getattr(fitted, f)) for f in _FIT_FIELDS]
+    else:
+        models = (fitted.params, fitted.tchange, fitted.meta_i32, fitted.meta_i64, fitted.meta_f64)
+    if out is not None:
+        outputs = (out.yhat, out.yhat_lower, out.yhat_upper, out.yhat_int)
+    else:
+        outputs = (space.empty(shape, "float64"), space.empty(shape, "float64") if bounds else None,
+                   space.empty(shape, "float64") if bounds else None, space.empty(shape, "int32") if yint else None)
+    p = space.ptr
+    args = (ctx.handle, C.byref(opts), *map(p, models), n, *grid, p(floor), p(cap), int(seed) & (2**64 - 1))
+    return args, outputs
+
+
+def _future_host(future_ds, n: int) -> np.ndarray:
+    return np.ascontiguousarray(future_ds, dtype=np.int64).reshape(n, -1)
+
+
+def _predict_regressors(space: _Space, opts, fitted: FittedBatch, regressors, components: bool, n: int, h: int):
+    """The future regressor values and the fit's reg_scale a regressor predict reads: a host call's converted, a device
+    call's checked."""
+    if components:
+        raise ValueError("components are not supported with regressors")
+    R = n_regressors(opts)
+    _check_reg_scale(fitted.reg_scale, n, R, "fitted.reg_scale", space.dev)
+    if space.dev is None:
+        return _host_regressors(opts, regressors, n * h), np.ascontiguousarray(fitted.reg_scale)
+    import torch
+    if (regressors.dtype != torch.float64 or regressors.numel() != R * n * h or not regressors.is_contiguous()
+            or regressors.device != space.dev):
+        raise ValueError(f"regressors must be a contiguous float64 tensor of shape ({R}, {n}, {h}) on {space.dev}")
+    return regressors, fitted.reg_scale
+
+
+def _predict(space: _Space, ctx, opts, fitted, future_ds, floor, cap, seed, intervals, components, regressors,
+             out=None, sync=False) -> "ForecastBatch":
+    """The body of predict_batch_host / predict_batch_device: pb200_predict[_components|_regressors]_host / _device.
+    A device call synchronises torch's stream first unless it reuses ``out``, and the context after with ``sync``."""
+    host = space.dev is None
+    n = fitted.n
+    if host:
+        fitted = fitted.to_host()
+        future_ds = _future_host(future_ds, n)
+    h = int(future_ds.shape[1])
+    do_mc = intervals and opts.uncertainty_samples > 0
+    if out is not None:
+        comp, tlo, thi = out.components, out.trend_lower, out.trend_upper
+    else:
+        comp = space.empty((len(component_names(opts)), n, h), "float64") if components else None
+        tlo = space.empty((n, h), "float64") if components and do_mc else None
+        thi = space.empty((n, h), "float64") if components and do_mc else None
+    if host and regressors is not None:
+        regressors, reg_scale = _predict_regressors(space, opts, fitted, regressors, components, n, h)
+    args, (yhat, lo, hi, yint) = _predict_head(space, ctx, opts, fitted, (space.ptr(future_ds), h), floor, cap, seed,
+                                               (n, h), do_mc, out=out)
+    if n > 0 and h > 0:
+        if out is None:
+            space.sync_torch()
+        p = space.ptr
+        mc = p if do_mc else lambda a: None         # (``out`` may hold bounds this call does not write)
+        outputs = (p(yhat), mc(lo), mc(hi), p(yint))
+        if regressors is not None:
+            if not host:
+                regressors, reg_scale = _predict_regressors(space, opts, fitted, regressors, components, n, h)
+            _call("pb200_predict_regressors" + space.suffix, *args, p(regressors), p(reg_scale), *outputs)
+        elif components:
+            _call("pb200_predict_components" + space.suffix, *args, *outputs, p(comp), mc(tlo), mc(thi))
+        else:
+            _call("pb200_predict" + space.suffix, *args, *outputs)
+        if sync:
+            ctx.synchronize()
+    return ForecastBatch(future_ds, yhat, lo, hi, yint, comp, tlo, thi,
+                         names=component_names(opts) if components else L.COMPONENTS)
+
+
 def predict_batch_host(ctx: L.Context, opts: L.Options, fitted: FittedBatch, future_ds: np.ndarray,
                        floor: np.ndarray, cap: np.ndarray, seed: int = 0, intervals: bool = True,
                        components: bool = False, regressors=None) -> ForecastBatch:
@@ -807,44 +861,7 @@ def predict_batch_host(ctx: L.Context, opts: L.Options, fitted: FittedBatch, fut
     which also fills ``components`` and, with intervals, ``trend_lower`` / ``trend_upper``.  ``regressors``: None, or
     for a fit with regressors their future values ``[R, N, H]`` (pb200_predict_regressors_host, with the fit's
     ``reg_scale``; not with ``components``)."""
-    fitted = fitted.to_host()
-    n = fitted.n
-    future_ds = np.ascontiguousarray(future_ds, dtype=np.int64).reshape(n, -1)
-    h = future_ds.shape[1]
-    floor = np.ascontiguousarray(np.broadcast_to(np.asarray(floor, dtype=np.float64), (n,)))
-    cap = np.ascontiguousarray(np.broadcast_to(np.asarray(cap, dtype=np.float64), (n,)))
-    yhat = np.empty((n, h), np.float64)
-    yint = np.empty((n, h), np.int32)
-    do_mc = intervals and opts.uncertainty_samples > 0
-    lo = np.empty((n, h), np.float64) if do_mc else None
-    hi = np.empty((n, h), np.float64) if do_mc else None
-    names = component_names(opts) if components else L.COMPONENTS
-    comp = np.empty((len(names), n, h), np.float64) if components else None
-    tlo = np.empty((n, h), np.float64) if components and do_mc else None
-    thi = np.empty((n, h), np.float64) if components and do_mc else None
-    if regressors is not None:
-        if components:
-            raise ValueError("components are not supported with regressors")
-        _check_reg_scale(fitted.reg_scale, n, n_regressors(opts), "fitted.reg_scale")
-        freg = _host_regressors(opts, regressors, n * h)
-        rsc = np.ascontiguousarray(fitted.reg_scale)
-    if n > 0 and h > 0:
-        args = (ctx.handle, C.byref(opts), _np_ptr(np.ascontiguousarray(fitted.params)),
-                _np_ptr(np.ascontiguousarray(fitted.tchange)), _np_ptr(np.ascontiguousarray(fitted.meta_i32)),
-                _np_ptr(np.ascontiguousarray(fitted.meta_i64)), _np_ptr(np.ascontiguousarray(fitted.meta_f64)),
-                n, _np_ptr(future_ds), h, _np_ptr(floor), _np_ptr(cap), int(seed) & (2**64 - 1),
-                _np_ptr(yhat), _np_ptr(lo) if do_mc else None, _np_ptr(hi) if do_mc else None, _np_ptr(yint))
-        if regressors is not None:
-            rc = L.load().pb200_predict_regressors_host(*args[:13], _np_ptr(freg), _np_ptr(rsc), *args[13:])
-            L.check(rc, "pb200_predict_regressors_host")
-        elif components:
-            rc = L.load().pb200_predict_components_host(*args, _np_ptr(comp), _np_ptr(tlo) if do_mc else None,
-                                                        _np_ptr(thi) if do_mc else None)
-            L.check(rc, "pb200_predict_components_host")
-        else:
-            L.check(L.load().pb200_predict_host(*args), "pb200_predict_host")
-    return ForecastBatch(future_ds, yhat, lo, hi, yint, comp, tlo, thi,
-                         names=component_names(opts) if components else L.COMPONENTS)
+    return _predict(_HOST, ctx, opts, fitted, future_ds, floor, cap, seed, intervals, components, regressors)
 
 
 def predict_batch_device(ctx: L.Context, opts: L.Options, fitted: FittedBatch, future_ds, floor, cap,
@@ -855,50 +872,8 @@ def predict_batch_device(ctx: L.Context, opts: L.Options, fitted: FittedBatch, f
     made with the same ``components``).  ``components``: pb200_predict_components_device, as in predict_batch_host.
     ``regressors``: None, or for a fit with regressors a contiguous float64 CUDA tensor ``[R, N, H]`` of their future
     values (pb200_predict_regressors_device, with ``fitted.reg_scale``; not with ``components``)."""
-    import torch
-    n = fitted.n
-    h = int(future_ds.shape[1])
-    dev = future_ds.device
-    do_mc = intervals and opts.uncertainty_samples > 0
-    if out is not None:
-        yhat, yint, lo, hi = out.yhat, out.yhat_int, out.yhat_lower, out.yhat_upper
-        comp, tlo, thi = out.components, out.trend_lower, out.trend_upper
-    else:
-        yhat = torch.empty((n, h), dtype=torch.float64, device=dev)
-        yint = torch.empty((n, h), dtype=torch.int32, device=dev)
-        lo = torch.empty((n, h), dtype=torch.float64, device=dev) if do_mc else None
-        hi = torch.empty((n, h), dtype=torch.float64, device=dev) if do_mc else None
-        comp = torch.empty((len(component_names(opts)), n, h), dtype=torch.float64, device=dev) if components else None
-        tlo = torch.empty((n, h), dtype=torch.float64, device=dev) if components and do_mc else None
-        thi = torch.empty((n, h), dtype=torch.float64, device=dev) if components and do_mc else None
-    if n > 0 and h > 0:
-        if out is None:
-            torch.cuda.current_stream(dev).synchronize()
-        args = (ctx.handle, C.byref(opts), fitted.params.data_ptr(), fitted.tchange.data_ptr(),
-                fitted.meta_i32.data_ptr(), fitted.meta_i64.data_ptr(), fitted.meta_f64.data_ptr(), n,
-                future_ds.data_ptr(), h, floor.data_ptr(), cap.data_ptr(), int(seed) & (2**64 - 1),
-                yhat.data_ptr(), lo.data_ptr() if do_mc else None, hi.data_ptr() if do_mc else None, yint.data_ptr())
-        if regressors is not None:
-            R = n_regressors(opts)
-            if components:
-                raise ValueError("components are not supported with regressors")
-            _check_reg_scale(fitted.reg_scale, n, R, "fitted.reg_scale", dev)
-            if (regressors.dtype != torch.float64 or regressors.numel() != R * n * h or not regressors.is_contiguous()
-                    or regressors.device != dev):
-                raise ValueError(f"regressors must be a contiguous float64 tensor of shape ({R}, {n}, {h}) on {dev}")
-            rc = L.load().pb200_predict_regressors_device(*args[:13], regressors.data_ptr(), fitted.reg_scale.data_ptr(),
-                                                          *args[13:])
-            L.check(rc, "pb200_predict_regressors_device")
-        elif components:
-            rc = L.load().pb200_predict_components_device(*args, comp.data_ptr(), tlo.data_ptr() if do_mc else None,
-                                                          thi.data_ptr() if do_mc else None)
-            L.check(rc, "pb200_predict_components_device")
-        else:
-            L.check(L.load().pb200_predict_device(*args), "pb200_predict_device")
-        if sync:
-            ctx.synchronize()
-    return ForecastBatch(future_ds, yhat, lo, hi, yint, comp, tlo, thi,
-                         names=component_names(opts) if components else L.COMPONENTS)
+    return _predict(_Space(future_ds.device), ctx, opts, fitted, future_ds, floor, cap, seed, intervals, components,
+                    regressors, out=out, sync=sync)
 
 
 QUANTILES_MAX = 32
@@ -912,57 +887,37 @@ def quantile_percentiles(levels) -> np.ndarray:
     return np.ascontiguousarray(100.0 * lv)
 
 
+def _quantiles(space: _Space, ctx, opts, fitted, future_ds, floor, cap, levels, seed, intervals, sync=False):
+    """The body of predict_quantiles_host / predict_quantiles_device."""
+    pct = quantile_percentiles(levels)
+    n = fitted.n
+    if space.dev is None:
+        future_ds = _future_host(future_ds, n)
+    h = int(future_ds.shape[1])
+    p = space.ptr
+    args, (yhat, lo, hi, yint) = _predict_head(space, ctx, opts, fitted, (p(future_ds), h), floor, cap, seed, (n, h),
+                                               intervals)
+    qs = space.empty((pct.size, n, h), "float64")
+    space.sync_torch()
+    _call("pb200_predict_quantiles" + space.suffix, *args, p(yhat), p(lo), p(hi), p(yint), int(pct.size), _np_ptr(pct),
+          p(qs))
+    if sync:
+        ctx.synchronize()
+    return ForecastBatch(future_ds, yhat, lo, hi, yint, quantiles=qs)
+
+
 def predict_quantiles_host(ctx: L.Context, opts: L.Options, fitted: FittedBatch, future_ds: np.ndarray, floor, cap,
                            levels, seed: int = 0, intervals: bool = False) -> ForecastBatch:
     """pb200_predict_quantiles_host: predict_batch_host's ForecastBatch (the bounds with ``intervals``) and
     ``quantiles`` [Q, N, H], the percentile 100 q of each point's uncertainty_samples draws for each level q of
     ``levels`` (DESIGN §15).  The draws are those behind yhat_lower / yhat_upper."""
-    pct = quantile_percentiles(levels)
-    fitted = fitted.to_host()
-    n = fitted.n
-    future_ds = np.ascontiguousarray(future_ds, dtype=np.int64).reshape(n, -1)
-    h = future_ds.shape[1]
-    floor = np.ascontiguousarray(np.broadcast_to(np.asarray(floor, dtype=np.float64), (n,)))
-    cap = np.ascontiguousarray(np.broadcast_to(np.asarray(cap, dtype=np.float64), (n,)))
-    yhat = np.empty((n, h), np.float64)
-    yint = np.empty((n, h), np.int32)
-    lo = np.empty((n, h), np.float64) if intervals else None
-    hi = np.empty((n, h), np.float64) if intervals else None
-    qs = np.empty((pct.size, n, h), np.float64)
-    rc = L.load().pb200_predict_quantiles_host(
-        ctx.handle, C.byref(opts), _np_ptr(np.ascontiguousarray(fitted.params)),
-        _np_ptr(np.ascontiguousarray(fitted.tchange)), _np_ptr(np.ascontiguousarray(fitted.meta_i32)),
-        _np_ptr(np.ascontiguousarray(fitted.meta_i64)), _np_ptr(np.ascontiguousarray(fitted.meta_f64)), n,
-        _np_ptr(future_ds), h, _np_ptr(floor), _np_ptr(cap), int(seed) & (2**64 - 1), _np_ptr(yhat),
-        _np_ptr(lo) if intervals else None, _np_ptr(hi) if intervals else None, _np_ptr(yint), int(pct.size),
-        _np_ptr(pct), _np_ptr(qs))
-    L.check(rc, "pb200_predict_quantiles_host")
-    return ForecastBatch(future_ds, yhat, lo, hi, yint, quantiles=qs)
+    return _quantiles(_HOST, ctx, opts, fitted, future_ds, floor, cap, levels, seed, intervals)
 
 
 def predict_quantiles_device(ctx: L.Context, opts: L.Options, fitted: FittedBatch, future_ds, floor, cap, levels,
                              seed: int = 0, intervals: bool = False, sync: bool = True) -> ForecastBatch:
     """pb200_predict_quantiles_device with torch CUDA tensors; as predict_quantiles_host."""
-    import torch
-    pct = quantile_percentiles(levels)
-    n = fitted.n
-    h = int(future_ds.shape[1])
-    dev = future_ds.device
-    yhat = torch.empty((n, h), dtype=torch.float64, device=dev)
-    yint = torch.empty((n, h), dtype=torch.int32, device=dev)
-    lo = torch.empty((n, h), dtype=torch.float64, device=dev) if intervals else None
-    hi = torch.empty((n, h), dtype=torch.float64, device=dev) if intervals else None
-    qs = torch.empty((pct.size, n, h), dtype=torch.float64, device=dev)
-    torch.cuda.current_stream(dev).synchronize()
-    rc = L.load().pb200_predict_quantiles_device(
-        ctx.handle, C.byref(opts), fitted.params.data_ptr(), fitted.tchange.data_ptr(), fitted.meta_i32.data_ptr(),
-        fitted.meta_i64.data_ptr(), fitted.meta_f64.data_ptr(), n, future_ds.data_ptr(), h, floor.data_ptr(),
-        cap.data_ptr(), int(seed) & (2**64 - 1), yhat.data_ptr(), lo.data_ptr() if intervals else None,
-        hi.data_ptr() if intervals else None, yint.data_ptr(), int(pct.size), _np_ptr(pct), qs.data_ptr())
-    L.check(rc, "pb200_predict_quantiles_device")
-    if sync:
-        ctx.synchronize()
-    return ForecastBatch(future_ds, yhat, lo, hi, yint, quantiles=qs)
+    return _quantiles(_Space(future_ds.device), ctx, opts, fitted, future_ds, floor, cap, levels, seed, intervals, sync)
 
 
 @dataclass
@@ -982,58 +937,38 @@ def _history_offsets(offsets, n: int) -> np.ndarray:
     return offsets
 
 
+def _history(space: _Space, ctx, opts, fitted, ds_ns, offsets, floor, cap, seed, intervals, sync=False):
+    """The body of predict_history_host / predict_history_device."""
+    n = fitted.n
+    offsets = _history_offsets(offsets, n)
+    if space.dev is None:
+        ds_ns = np.ascontiguousarray(ds_ns, dtype=np.int64)
+    rows = int(offsets[-1])
+    p = space.ptr
+    args, (yhat, lo, hi, _) = _predict_head(space, ctx, opts, fitted, (p(ds_ns), _np_ptr(offsets)), floor, cap, seed,
+                                            rows, intervals and opts.uncertainty_samples > 0, yint=False)
+    if n > 0 and rows > 0:
+        space.sync_torch()
+        _call("pb200_predict_history" + space.suffix, *args, p(yhat), p(lo), p(hi))
+        if sync:
+            ctx.synchronize()
+    return HistoryForecast(offsets, yhat, lo, hi)
+
+
 def predict_history_host(ctx: L.Context, opts: L.Options, fitted: FittedBatch, ds_ns: np.ndarray, offsets: np.ndarray,
                          floor, cap, seed: int = 0, intervals: bool = True) -> HistoryForecast:
     """pb200_predict_history_host: fbprophet's ``m.predict()`` (no frame: the history itself) for every model of
     ``fitted`` over its rows ``[offsets[i], offsets[i + 1])`` of ``ds_ns``; ``floor`` / ``cap`` per model (the fit's:
     ``fitted.meta_f64[:, 1]`` / ``[:, 2]``).  With ``intervals`` the bounds of ``opts.interval_width`` from
     ``opts.uncertainty_samples`` draws, bit-identical to predict_batch_host on the history padded by its last timestamp."""
-    fitted = fitted.to_host()
-    n = fitted.n
-    offsets = _history_offsets(offsets, n)
-    ds_ns = np.ascontiguousarray(ds_ns, dtype=np.int64)
-    rows = int(offsets[-1])
-    floor = np.ascontiguousarray(np.broadcast_to(np.asarray(floor, dtype=np.float64), (n,)))
-    cap = np.ascontiguousarray(np.broadcast_to(np.asarray(cap, dtype=np.float64), (n,)))
-    do_mc = intervals and opts.uncertainty_samples > 0
-    yhat = np.empty(rows, np.float64)
-    lo = np.empty(rows, np.float64) if do_mc else None
-    hi = np.empty(rows, np.float64) if do_mc else None
-    if n > 0 and rows > 0:
-        rc = L.load().pb200_predict_history_host(
-            ctx.handle, C.byref(opts), _np_ptr(np.ascontiguousarray(fitted.params)),
-            _np_ptr(np.ascontiguousarray(fitted.tchange)), _np_ptr(np.ascontiguousarray(fitted.meta_i32)),
-            _np_ptr(np.ascontiguousarray(fitted.meta_i64)), _np_ptr(np.ascontiguousarray(fitted.meta_f64)), n,
-            _np_ptr(ds_ns), _np_ptr(offsets), _np_ptr(floor), _np_ptr(cap), int(seed) & (2**64 - 1), _np_ptr(yhat),
-            _np_ptr(lo) if do_mc else None, _np_ptr(hi) if do_mc else None)
-        L.check(rc, "pb200_predict_history_host")
-    return HistoryForecast(offsets, yhat, lo, hi)
+    return _history(_HOST, ctx, opts, fitted, ds_ns, offsets, floor, cap, seed, intervals)
 
 
 def predict_history_device(ctx: L.Context, opts: L.Options, fitted: FittedBatch, ds_ns, offsets_host: np.ndarray, floor,
                            cap, seed: int = 0, intervals: bool = True, sync: bool = True) -> HistoryForecast:
     """pb200_predict_history_device: predict_history_host with torch CUDA tensors (``fitted`` on the device, ``ds_ns``
     the packed history, ``floor`` / ``cap`` float64 [N]); the offsets stay on the host."""
-    import torch
-    n = fitted.n
-    offsets_host = _history_offsets(offsets_host, n)
-    rows = int(offsets_host[-1])
-    dev = ds_ns.device
-    do_mc = intervals and opts.uncertainty_samples > 0
-    yhat = torch.empty(rows, dtype=torch.float64, device=dev)
-    lo = torch.empty(rows, dtype=torch.float64, device=dev) if do_mc else None
-    hi = torch.empty(rows, dtype=torch.float64, device=dev) if do_mc else None
-    if n > 0 and rows > 0:
-        torch.cuda.current_stream(dev).synchronize()
-        rc = L.load().pb200_predict_history_device(
-            ctx.handle, C.byref(opts), fitted.params.data_ptr(), fitted.tchange.data_ptr(), fitted.meta_i32.data_ptr(),
-            fitted.meta_i64.data_ptr(), fitted.meta_f64.data_ptr(), n, ds_ns.data_ptr(), _np_ptr(offsets_host),
-            floor.data_ptr(), cap.data_ptr(), int(seed) & (2**64 - 1), yhat.data_ptr(),
-            lo.data_ptr() if do_mc else None, hi.data_ptr() if do_mc else None)
-        L.check(rc, "pb200_predict_history_device")
-        if sync:
-            ctx.synchronize()
-    return HistoryForecast(offsets_host, yhat, lo, hi)
+    return _history(_Space(ds_ns.device), ctx, opts, fitted, ds_ns, offsets_host, floor, cap, seed, intervals, sync)
 
 
 @dataclass
@@ -1148,33 +1083,31 @@ def period_slots(first_ds, last_ds, months: int, month_shift: int) -> int:
     return int((p1 - p0).max()) + 1
 
 
-def _sums_host(ctx, opts, fitted, future_ds, floor, cap, seed, intervals, entry: str, rule, slots):
-    """The body of predict_sums_host / predict_period_sums_host: ``entry`` the C function, ``rule`` its two rule arguments,
-    ``slots(first_ds, last_ds)`` the slots per model."""
-    fitted = fitted.to_host()
+def _window_sums(space: _Space, ctx, opts, fitted, future_ds, floor, cap, seed, intervals, entry: str, rule, wmax):
+    """The body of the predict_*sums_* wrappers: ``entry`` the C function without its suffix, ``rule`` its arguments
+    between yhat_int and wmax, ``wmax`` the slots per model or a function ``slots(first_ds, last_ds)`` of the frame's
+    first and last columns (numpy) that gives them.  A device call always synchronises the context."""
     n = fitted.n
-    future_ds = np.ascontiguousarray(future_ds, dtype=np.int64)
-    future_ds = future_ds.reshape(n, -1) if n else future_ds.reshape(0, future_ds.shape[-1] if future_ds.ndim == 2 else 0)
-    h = future_ds.shape[1]
-    floor = np.ascontiguousarray(np.broadcast_to(np.asarray(floor, dtype=np.float64), (n,)))
-    cap = np.ascontiguousarray(np.broadcast_to(np.asarray(cap, dtype=np.float64), (n,)))
-    wmax = slots(future_ds[:, 0], future_ds[:, -1]) if h else 1
-    yhat = np.empty((n, h), np.float64)
-    yint = np.empty((n, h), np.int32)
-    lo = np.empty((n, h), np.float64) if intervals else None
-    hi = np.empty((n, h), np.float64) if intervals else None
-    ws = WindowSums(np.zeros(n, np.int32), np.empty((n, wmax), np.int64), np.empty((n, wmax), np.int32),
-                    np.empty((n, wmax), np.float64), np.empty((n, wmax), np.int64), np.empty((n, wmax), np.float64),
-                    np.empty((n, wmax), np.float64))
-    rc = getattr(L.load(), entry)(
-        ctx.handle, C.byref(opts), _np_ptr(np.ascontiguousarray(fitted.params)),
-        _np_ptr(np.ascontiguousarray(fitted.tchange)), _np_ptr(np.ascontiguousarray(fitted.meta_i32)),
-        _np_ptr(np.ascontiguousarray(fitted.meta_i64)), _np_ptr(np.ascontiguousarray(fitted.meta_f64)),
-        n, _np_ptr(future_ds), h, _np_ptr(floor), _np_ptr(cap), int(seed) & (2**64 - 1),
-        _np_ptr(yhat), _np_ptr(lo) if intervals else None, _np_ptr(hi) if intervals else None, _np_ptr(yint),
-        *rule, wmax, _np_ptr(ws.n_windows), _np_ptr(ws.start), _np_ptr(ws.points), _np_ptr(ws.yhat_sum),
-        _np_ptr(ws.quantity_sum), _np_ptr(ws.lower), _np_ptr(ws.upper))
-    L.check(rc, entry)
+    if space.dev is None:
+        future_ds = np.ascontiguousarray(future_ds, dtype=np.int64)
+        future_ds = future_ds.reshape(n, -1) if n else future_ds.reshape(0, future_ds.shape[-1] if future_ds.ndim == 2 else 0)
+    h = int(future_ds.shape[1])
+    if callable(wmax):
+        slots, wmax = wmax, 1
+        if n and h:
+            ends = future_ds[:, [0, -1]]
+            ends = ends if space.dev is None else ends.cpu().numpy()
+            wmax = slots(ends[:, 0], ends[:, 1])
+    p = space.ptr
+    args, (yhat, lo, hi, yint) = _predict_head(space, ctx, opts, fitted, (p(future_ds), h), floor, cap, seed, (n, h),
+                                               intervals)
+    ws = WindowSums(space.zeros(n, "int32"), *(space.empty((n, wmax), dt) for dt in
+                                              ("int64", "int32", "float64", "int64", "float64", "float64")))
+    space.sync_torch()
+    _call(entry + space.suffix, *args, p(yhat), p(lo), p(hi), p(yint), *rule, wmax,
+          *(p(a) for a in (ws.n_windows, ws.start, ws.points, ws.yhat_sum, ws.quantity_sum, ws.lower, ws.upper)))
+    if space.dev is not None:
+        ctx.synchronize()
     _check_window_slots(wmax, int(ws.n_windows.max()) if n else 0)
     return ForecastBatch(future_ds, yhat, lo, hi, yint), ws
 
@@ -1185,11 +1118,7 @@ def predict_sums_host(ctx: L.Context, opts: L.Options, fitted: FittedBatch, futu
     floor((ds - origin_ns) / width_ns) of each model's ascending frame -- totals of yhat / yhat_int per window and the
     interval of each total from the joint draws (fbprophet's predictive_samples summed per window).  Needs
     ``opts.uncertainty_samples`` in [2, 1024]; ``intervals`` asks for the pointwise yhat_lower / yhat_upper as well."""
-    width_ns, origin_ns = int(width_ns), int(origin_ns)
-    if width_ns <= 0:
-        raise ValueError(f"width_ns must be > 0 (got {width_ns})")
-    return _sums_host(ctx, opts, fitted, future_ds, floor, cap, seed, intervals, "pb200_predict_sums_host",
-                      (width_ns, origin_ns), lambda a, b: window_slots(a, b, width_ns, origin_ns))
+    return _fixed_sums(_HOST, ctx, opts, fitted, future_ds, floor, cap, width_ns, origin_ns, seed, intervals)
 
 
 def predict_period_sums_host(ctx: L.Context, opts: L.Options, fitted: FittedBatch, future_ds: np.ndarray, floor, cap,
@@ -1197,60 +1126,35 @@ def predict_period_sums_host(ctx: L.Context, opts: L.Options, fitted: FittedBatc
     """pb200_predict_period_sums_host: predict_sums_host over calendar periods (DESIGN §17) -- the windows are the
     periods floor((mi + month_shift) / months) of each model's ascending frame, mi the months of ds's civil date since
     1970-01, and ``WindowSums.start`` holds each period's start.  ``period_rule`` turns a pandas alias into the rule."""
+    return _period_sums(_HOST, ctx, opts, fitted, future_ds, floor, cap, months, month_shift, seed, intervals)
+
+
+def _fixed_sums(space, ctx, opts, fitted, future_ds, floor, cap, width_ns, origin_ns, seed, intervals):
+    width_ns, origin_ns = int(width_ns), int(origin_ns)
+    if width_ns <= 0:
+        raise ValueError(f"width_ns must be > 0 (got {width_ns})")
+    return _window_sums(space, ctx, opts, fitted, future_ds, floor, cap, seed, intervals, "pb200_predict_sums",
+                        (width_ns, origin_ns), lambda a, b: window_slots(a, b, width_ns, origin_ns))
+
+
+def _period_sums(space, ctx, opts, fitted, future_ds, floor, cap, months, month_shift, seed, intervals):
     months, month_shift = _period_rule_checked(months, month_shift)
-    return _sums_host(ctx, opts, fitted, future_ds, floor, cap, seed, intervals, "pb200_predict_period_sums_host",
-                      (months, month_shift), lambda a, b: period_slots(a, b, months, month_shift))
-
-
-def _sums_device(ctx, opts, fitted, future_ds, floor, cap, seed, intervals, entry: str, rule, slots):
-    """The body of predict_sums_device / predict_period_sums_device, as _sums_host."""
-    import torch
-    n = fitted.n
-    h = int(future_ds.shape[1])
-    dev = future_ds.device
-    wmax = 1
-    if n and h:
-        ends = future_ds[:, [0, -1]].cpu().numpy()
-        wmax = slots(ends[:, 0], ends[:, 1])
-    f64 = dict(dtype=torch.float64, device=dev)
-    yhat = torch.empty((n, h), **f64)
-    yint = torch.empty((n, h), dtype=torch.int32, device=dev)
-    lo = torch.empty((n, h), **f64) if intervals else None
-    hi = torch.empty((n, h), **f64) if intervals else None
-    ws = WindowSums(torch.zeros(n, dtype=torch.int32, device=dev), torch.empty((n, wmax), dtype=torch.int64, device=dev),
-                    torch.empty((n, wmax), dtype=torch.int32, device=dev), torch.empty((n, wmax), **f64),
-                    torch.empty((n, wmax), dtype=torch.int64, device=dev), torch.empty((n, wmax), **f64),
-                    torch.empty((n, wmax), **f64))
-    torch.cuda.current_stream(dev).synchronize()
-    rc = getattr(L.load(), entry)(
-        ctx.handle, C.byref(opts), fitted.params.data_ptr(), fitted.tchange.data_ptr(), fitted.meta_i32.data_ptr(),
-        fitted.meta_i64.data_ptr(), fitted.meta_f64.data_ptr(), n, future_ds.data_ptr(), h, floor.data_ptr(),
-        cap.data_ptr(), int(seed) & (2**64 - 1), yhat.data_ptr(), lo.data_ptr() if intervals else None,
-        hi.data_ptr() if intervals else None, yint.data_ptr(), *rule, wmax, ws.n_windows.data_ptr(),
-        ws.start.data_ptr(), ws.points.data_ptr(), ws.yhat_sum.data_ptr(), ws.quantity_sum.data_ptr(), ws.lower.data_ptr(),
-        ws.upper.data_ptr())
-    L.check(rc, entry)
-    ctx.synchronize()
-    _check_window_slots(wmax, int(ws.n_windows.max().item()) if n else 0)
-    return ForecastBatch(future_ds, yhat, lo, hi, yint), ws
+    return _window_sums(space, ctx, opts, fitted, future_ds, floor, cap, seed, intervals, "pb200_predict_period_sums",
+                        (months, month_shift), lambda a, b: period_slots(a, b, months, month_shift))
 
 
 def predict_sums_device(ctx: L.Context, opts: L.Options, fitted: FittedBatch, future_ds, floor, cap, width_ns: int,
                         origin_ns: int = 0, seed: int = 0, intervals: bool = False):
     """pb200_predict_sums_device with torch CUDA tensors; as predict_sums_host."""
-    width_ns, origin_ns = int(width_ns), int(origin_ns)
-    if width_ns <= 0:
-        raise ValueError(f"width_ns must be > 0 (got {width_ns})")
-    return _sums_device(ctx, opts, fitted, future_ds, floor, cap, seed, intervals, "pb200_predict_sums_device",
-                        (width_ns, origin_ns), lambda a, b: window_slots(a, b, width_ns, origin_ns))
+    return _fixed_sums(_Space(future_ds.device), ctx, opts, fitted, future_ds, floor, cap, width_ns, origin_ns, seed,
+                       intervals)
 
 
 def predict_period_sums_device(ctx: L.Context, opts: L.Options, fitted: FittedBatch, future_ds, floor, cap, months: int,
                                month_shift: int, seed: int = 0, intervals: bool = False):
     """pb200_predict_period_sums_device with torch CUDA tensors; as predict_period_sums_host."""
-    months, month_shift = _period_rule_checked(months, month_shift)
-    return _sums_device(ctx, opts, fitted, future_ds, floor, cap, seed, intervals, "pb200_predict_period_sums_device",
-                        (months, month_shift), lambda a, b: period_slots(a, b, months, month_shift))
+    return _period_sums(_Space(future_ds.device), ctx, opts, fitted, future_ds, floor, cap, months, month_shift, seed,
+                        intervals)
 
 
 _MONTHS = ("JAN", "FEB", "MAR", "APR", "MAY", "JUN", "JUL", "AUG", "SEP", "OCT", "NOV", "DEC")
@@ -1299,28 +1203,8 @@ def predict_sums_anchored_device(ctx: L.Context, opts: L.Options, fitted: Fitted
             last = future_ds.gather(1, (frame_len.long().clamp(1, h) - 1)[:, None])[:, 0]
             w = (last - origins).div(width_ns, rounding_mode="floor") - (future_ds[:, 0] - origins).div(width_ns, rounding_mode="floor")
             wmax = max(1, int(w.max().item()) + 1)
-    wmax = int(wmax)
-    f64 = dict(dtype=torch.float64, device=dev)
-    yhat = torch.empty((n, h), **f64)
-    yint = torch.empty((n, h), dtype=torch.int32, device=dev)
-    lo = torch.empty((n, h), **f64) if intervals else None
-    hi = torch.empty((n, h), **f64) if intervals else None
-    ws = WindowSums(torch.zeros(n, dtype=torch.int32, device=dev), torch.empty((n, wmax), dtype=torch.int64, device=dev),
-                    torch.empty((n, wmax), dtype=torch.int32, device=dev), torch.empty((n, wmax), **f64),
-                    torch.empty((n, wmax), dtype=torch.int64, device=dev), torch.empty((n, wmax), **f64),
-                    torch.empty((n, wmax), **f64))
-    torch.cuda.current_stream(dev).synchronize()
-    rc = L.load().pb200_predict_sums_anchored_device(
-        ctx.handle, C.byref(opts), fitted.params.data_ptr(), fitted.tchange.data_ptr(), fitted.meta_i32.data_ptr(),
-        fitted.meta_i64.data_ptr(), fitted.meta_f64.data_ptr(), n, future_ds.data_ptr(), h, floor.data_ptr(),
-        cap.data_ptr(), int(seed) & (2**64 - 1), yhat.data_ptr(), lo.data_ptr() if intervals else None,
-        hi.data_ptr() if intervals else None, yint.data_ptr(), width_ns, origins.data_ptr(), frame_len.data_ptr(), wmax,
-        ws.n_windows.data_ptr(), ws.start.data_ptr(), ws.points.data_ptr(), ws.yhat_sum.data_ptr(),
-        ws.quantity_sum.data_ptr(), ws.lower.data_ptr(), ws.upper.data_ptr())
-    L.check(rc, "pb200_predict_sums_anchored_device")
-    ctx.synchronize()
-    _check_window_slots(wmax, int(ws.n_windows.max().item()) if n else 0)
-    return ForecastBatch(future_ds, yhat, lo, hi, yint), ws
+    return _window_sums(_Space(dev), ctx, opts, fitted, future_ds, floor, cap, seed, intervals,
+                        "pb200_predict_sums_anchored", (width_ns, origins.data_ptr(), frame_len.data_ptr()), int(wmax))
 
 
 def objective_host(ctx: L.Context, opts: L.Options, ds_ns: np.ndarray, y: np.ndarray, offsets: np.ndarray,
@@ -1339,20 +1223,18 @@ def objective_host(ctx: L.Context, opts: L.Options, ds_ns: np.ndarray, y: np.nda
     f = np.empty(n, np.float64)
     g = np.empty((n, lay.pstride), np.float64)
     mi32 = np.empty((n, 8), np.int32)
+    reg = rsc = None
     if regressors is not None:
         reg = _host_regressors(opts, regressors, ds_ns.size)
         rsc = np.empty((n, reg.shape[0], 2), np.float64)
-        rc = L.load().pb200_objective_regressors_host(ctx.handle, C.byref(opts), _np_ptr(ds_ns), _np_ptr(y), _y_dtype(y),
-                                                      _np_ptr(offsets), n, float(floor), float(cap_multiplier),
-                                                      _np_ptr(reg), _np_ptr(rsc), _np_ptr(th), _np_ptr(f), _np_ptr(g),
-                                                      _np_ptr(mi32))
-        L.check(rc, "pb200_objective_regressors_host")
-        return f, g, mi32, rsc
-    rc = L.load().pb200_objective_host(ctx.handle, C.byref(opts), _np_ptr(ds_ns), _np_ptr(y), _y_dtype(y),
-                                       _np_ptr(offsets), n, float(floor), float(cap_multiplier), _np_ptr(th),
-                                       _np_ptr(f), _np_ptr(g), _np_ptr(mi32))
-    L.check(rc, "pb200_objective_host")
-    return f, g, mi32
+    args = (ctx.handle, C.byref(opts), _np_ptr(ds_ns), _np_ptr(y), _y_dtype(y), _np_ptr(offsets), n, float(floor),
+            float(cap_multiplier))
+    outputs = (_np_ptr(th), _np_ptr(f), _np_ptr(g), _np_ptr(mi32))
+    if reg is None:
+        _call("pb200_objective_host", *args, *outputs)
+        return f, g, mi32
+    _call("pb200_objective_regressors_host", *args, _np_ptr(reg), _np_ptr(rsc), *outputs)
+    return f, g, mi32, rsc
 
 
 # ---------------------------------------------------------------------------------------------------------------------
@@ -1705,12 +1587,7 @@ def cross_validation_device(ctx: L.Context, opts: L.Options, ds_ns, y, offsets_h
         lap("gather")
         # fits, one call per mask class; records re-laid into the layout of ``opts`` for the one predict call
         sp = pmask[perm]
-        fitted = FittedBatch(torch.zeros((n, lay.pstride), dtype=torch.float64, device=dev),
-                             torch.zeros((n, lay.smax), dtype=torch.float64, device=dev),
-                             torch.empty((n, 8), dtype=torch.int32, device=dev),
-                             torch.empty((n, 2), dtype=torch.int64, device=dev),
-                             torch.empty((n, 4), dtype=torch.float64, device=dev), lay.smax, lay.kmax,
-                             reg_scale=torch.empty((n, R, 2), dtype=torch.float64, device=dev) if R else None)
+        fitted = _fitted_outputs(_Space(dev), n, lay, R, zeros=True)
         cap_p = cap[torch.from_numpy(ps_h[perm]).to(dev)].contiguous()
         prior_p = torch.from_numpy(grid_h[g_h[perm]]).to(dev) if grid_h is not None else None
         bounds = np.flatnonzero(np.diff(np.concatenate(([-1], sp, [-1])))).tolist()
@@ -1977,7 +1854,7 @@ def tune_device(ctx: L.Context, opts: L.Options, ds_ns, y, offsets_host: np.ndar
                 _row_budget: Optional[int] = None) -> TuneResult:
     """For every series of a packed batch: cross_validation + performance_metrics(rolling_window=1) at every grid point
     (one cross_validation_device call with ``grid``), the grid point with the lowest ``metric``, then one
-    pb200_fit_prior_device over the full histories, each series with its chosen pair (the options' for a series with no
+    pb200_fit_warm_device (fit_batch_device with ``prior``) over the full histories, each series with its chosen pair (the options' for a series with no
     eligible point).  ``cap_multiplier`` gives every fit the full history's cap, max(y) * cap_multiplier, as the modeler
     does.  ``timings`` as in cross_validation_device, plus ``final_fit``."""
     import time
