@@ -535,8 +535,10 @@ __global__ void __launch_bounds__(32 * NW_WARPS, 1) newton_kernel(const NewtonAr
                     const int c = q - 3;
                     v = (c < S && sr.ncp > 0) ? x[2 + c] : 0.0;
                 } else {
+                    // only fbprophet's zero column (no seasonality and no regressor) is recorded as 0: a history without
+                    // seasonality still has its R regressor betas in columns 0 .. R - 1
                     const int b = q - 3 - a.smax;
-                    v = (sr.mask && b < sr.K) ? x[3 + S + b] : 0.0;
+                    v = ((sr.mask || a.reg.R) && b < sr.K) ? x[3 + S + b] : 0.0;
                 }
                 pr[q] = v;
             }
