@@ -1,4 +1,4 @@
-"""ctypes binding of libprophet_b200.so (C ABI in include/prophet_b200.h).
+"""ctypes binding of libprophet_b200.so (C ABI in include/prophet_b200.h and include/prophet_b200_window_quantiles.h).
 
 There is no CPU fallback: importing this module never builds or emulates anything, and
 ``load()`` raises if the CUDA library is missing; ``Context()`` raises if no H100 is visible.
@@ -99,6 +99,12 @@ EXPORTS = [
     "pb200_join_future_regressors_device", "pb200_regressor_scales_device", "pb200_cv_gather_regressors_device",
     "pb200_fit_regressors_copy_device",
 ]
+# declared in include/prophet_b200_window_quantiles.h (DESIGN §21)
+WINDOW_QUANTILE_EXPORTS = [
+    "pb200_predict_sums_quantiles_device", "pb200_predict_sums_quantiles_host",
+    "pb200_predict_period_sums_quantiles_device", "pb200_predict_period_sums_quantiles_host",
+    "pb200_predict_sums_anchored_quantiles_device",
+]
 CV_ERR_HORIZON, CV_ERR_INITIAL, CV_ERR_FEW = 1, 2, 4
 
 _lib = None
@@ -125,6 +131,8 @@ def load() -> C.CDLL:
         "pb200_predict_sums": pred_args + [i64, i64, i32] + [vp] * 7,
         "pb200_predict_period_sums": pred_args + [i32, i32, i32] + [vp] * 7,
         "pb200_predict_quantiles": pred_args + [i32, vp, vp],
+        "pb200_predict_sums_quantiles": pred_args + [i64, i64, i32] + [vp] * 7 + [i32, vp, vp],
+        "pb200_predict_period_sums_quantiles": pred_args + [i32, i32, i32] + [vp] * 7 + [i32, vp, vp],
         "pb200_predict_history": hist_args,
         "pb200_predict_regressors": pred_args[:13] + [vp, vp] + pred_args[13:],
     }
@@ -154,6 +162,7 @@ def load() -> C.CDLL:
         "pb200_objective_host": fit_args[:9] + [vp, vp, vp, vp],
         "pb200_objective_regressors_host": fit_args[:9] + [vp, vp, vp, vp, vp, vp],
         "pb200_predict_sums_anchored_device": pred_args + [i64, vp, vp, i32] + [vp] * 7,
+        "pb200_predict_sums_anchored_quantiles_device": pred_args + [i64, vp, vp, i32] + [vp] * 7 + [i32, vp, vp],
         "pb200_period_host": [vp, i64, i32, i32, vp, vp],
         "pb200_make_future_device": [vp, vp, i64, i32, i64, vp],
         "pb200_outlier_counts_device": [vp, vp, i32, vp, i64, vp, vp, vp, vp],

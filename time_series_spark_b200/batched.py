@@ -9,7 +9,7 @@ the *_host entry points take numpy arrays and stage through the library's own bu
 from __future__ import annotations
 
 import ctypes as C
-from dataclasses import dataclass
+from dataclasses import dataclass, fields
 from typing import Optional
 
 import numpy as np
@@ -769,12 +769,19 @@ def forecast_csv_row_host(series_id: int, dim_id: int, ds_ns: int, quantity: int
     return buf.raw[:n]
 
 
+class _Args(tuple):
+    """A library call's arguments.  ``keep`` holds the arrays made for the call, which its pointers point into: they
+    must live until the call is made."""
+    keep = ()
+
+
 def _predict_head(space: _Space, ctx, opts, fitted: FittedBatch, grid, floor, cap, seed, shape, bounds: bool,
                   yint: bool = True, out: Optional["ForecastBatch"] = None):
     """What every predict entry point starts with: the arguments (handle, options, fitted's five arrays, n, the two
     ``grid`` arguments, floor, cap, seed) and the outputs it writes first, yhat, the bounds (with ``bounds``, else None)
     and (with ``yint``) yhat_int, each of ``shape``, or ``out``'s.  A host call takes ``fitted`` as contiguous numpy and
-    floor / cap broadcast to one float64 per model.  Returns (args, (yhat, lower, upper, yhat_int))."""
+    floor / cap broadcast to one float64 per model; the arguments (an _Args) keep those arrays alive.  Returns (args,
+    (yhat, lower, upper, yhat_int))."""
     n = fitted.n
     if space.dev is None:
         fitted = fitted.to_host()
@@ -788,7 +795,8 @@ def _predict_head(space: _Space, ctx, opts, fitted: FittedBatch, grid, floor, ca
         outputs = (space.empty(shape, "float64"), space.empty(shape, "float64") if bounds else None,
                    space.empty(shape, "float64") if bounds else None, space.empty(shape, "int32") if yint else None)
     p = space.ptr
-    args = (ctx.handle, C.byref(opts), *map(p, models), n, *grid, p(floor), p(cap), int(seed) & (2**64 - 1))
+    args = _Args((ctx.handle, C.byref(opts), *map(p, models), n, *grid, p(floor), p(cap), int(seed) & (2**64 - 1)))
+    args.keep = (models, floor, cap)
     return args, outputs
 
 
@@ -1034,6 +1042,14 @@ class WindowSums:
     upper: object
 
 
+@dataclass
+class WindowQuantiles(WindowSums):
+    """WindowSums plus the quantiles of each window's total at ``levels`` (DESIGN §21): the predict_*sums_* wrappers'
+    second result when called with ``levels``."""
+    levels: np.ndarray    # [Q] f64 fractions, as given
+    quantiles: object     # [Q, N, wmax] f64: percentile 100 q over the draws' window sums; NaN past n_windows
+
+
 def window_slots(first_ds, last_ds, width_ns: int, origin_ns: int) -> int:
     """An upper bound on a model's windows from the first and last column of an ascending frame:
     max_i (w(last_i) - w(first_i) + 1), w = floor((ds - origin) / width).  Exact when the grid is no coarser than the
@@ -1083,10 +1099,13 @@ def period_slots(first_ds, last_ds, months: int, month_shift: int) -> int:
     return int((p1 - p0).max()) + 1
 
 
-def _window_sums(space: _Space, ctx, opts, fitted, future_ds, floor, cap, seed, intervals, entry: str, rule, wmax):
+def _window_sums(space: _Space, ctx, opts, fitted, future_ds, floor, cap, seed, intervals, entry: str, rule, wmax,
+                 levels=None):
     """The body of the predict_*sums_* wrappers: ``entry`` the C function without its suffix, ``rule`` its arguments
     between yhat_int and wmax, ``wmax`` the slots per model or a function ``slots(first_ds, last_ds)`` of the frame's
-    first and last columns (numpy) that gives them.  A device call always synchronises the context."""
+    first and last columns (numpy) that gives them.  ``levels``: the ``entry``_quantiles twin, whose planes make the
+    result a WindowQuantiles.  A device call always synchronises the context."""
+    pct = quantile_percentiles(levels) if levels is not None else None
     n = fitted.n
     if space.dev is None:
         future_ds = np.ascontiguousarray(future_ds, dtype=np.int64)
@@ -1103,9 +1122,15 @@ def _window_sums(space: _Space, ctx, opts, fitted, future_ds, floor, cap, seed, 
                                                intervals)
     ws = WindowSums(space.zeros(n, "int32"), *(space.empty((n, wmax), dt) for dt in
                                               ("int64", "int32", "float64", "int64", "float64", "float64")))
+    quant = ()
+    if pct is not None:
+        ws = WindowQuantiles(*(getattr(ws, f.name) for f in fields(WindowSums)),
+                             np.asarray(levels, dtype=np.float64), space.empty((pct.size, n, wmax), "float64"))
+        entry += "_quantiles"
+        quant = (int(pct.size), _np_ptr(pct), p(ws.quantiles))
     space.sync_torch()
     _call(entry + space.suffix, *args, p(yhat), p(lo), p(hi), p(yint), *rule, wmax,
-          *(p(a) for a in (ws.n_windows, ws.start, ws.points, ws.yhat_sum, ws.quantity_sum, ws.lower, ws.upper)))
+          *(p(a) for a in (ws.n_windows, ws.start, ws.points, ws.yhat_sum, ws.quantity_sum, ws.lower, ws.upper)), *quant)
     if space.dev is not None:
         ctx.synchronize()
     _check_window_slots(wmax, int(ws.n_windows.max()) if n else 0)
@@ -1113,48 +1138,55 @@ def _window_sums(space: _Space, ctx, opts, fitted, future_ds, floor, cap, seed, 
 
 
 def predict_sums_host(ctx: L.Context, opts: L.Options, fitted: FittedBatch, future_ds: np.ndarray, floor: np.ndarray,
-                      cap: np.ndarray, width_ns: int, origin_ns: int = 0, seed: int = 0, intervals: bool = False):
+                      cap: np.ndarray, width_ns: int, origin_ns: int = 0, seed: int = 0, intervals: bool = False,
+                      levels=None):
     """pb200_predict_sums_host: predict_batch_host's ForecastBatch and the WindowSums of the windows
     floor((ds - origin_ns) / width_ns) of each model's ascending frame -- totals of yhat / yhat_int per window and the
     interval of each total from the joint draws (fbprophet's predictive_samples summed per window).  Needs
-    ``opts.uncertainty_samples`` in [2, 1024]; ``intervals`` asks for the pointwise yhat_lower / yhat_upper as well."""
-    return _fixed_sums(_HOST, ctx, opts, fitted, future_ds, floor, cap, width_ns, origin_ns, seed, intervals)
+    ``opts.uncertainty_samples`` in [2, 1024]; ``intervals`` asks for the pointwise yhat_lower / yhat_upper as well.
+    ``levels`` (1 to 32 fractions in [0, 1], any order): pb200_predict_sums_quantiles_host, which returns a
+    WindowQuantiles with each window total's quantiles at those levels from the same draws (DESIGN §21); every other
+    output is the same."""
+    return _fixed_sums(_HOST, ctx, opts, fitted, future_ds, floor, cap, width_ns, origin_ns, seed, intervals, levels)
 
 
 def predict_period_sums_host(ctx: L.Context, opts: L.Options, fitted: FittedBatch, future_ds: np.ndarray, floor, cap,
-                             months: int, month_shift: int, seed: int = 0, intervals: bool = False):
+                             months: int, month_shift: int, seed: int = 0, intervals: bool = False, levels=None):
     """pb200_predict_period_sums_host: predict_sums_host over calendar periods (DESIGN §17) -- the windows are the
     periods floor((mi + month_shift) / months) of each model's ascending frame, mi the months of ds's civil date since
-    1970-01, and ``WindowSums.start`` holds each period's start.  ``period_rule`` turns a pandas alias into the rule."""
-    return _period_sums(_HOST, ctx, opts, fitted, future_ds, floor, cap, months, month_shift, seed, intervals)
+    1970-01, and ``WindowSums.start`` holds each period's start.  ``period_rule`` turns a pandas alias into the rule.
+    ``levels``: pb200_predict_period_sums_quantiles_host, as in predict_sums_host."""
+    return _period_sums(_HOST, ctx, opts, fitted, future_ds, floor, cap, months, month_shift, seed, intervals, levels)
 
 
-def _fixed_sums(space, ctx, opts, fitted, future_ds, floor, cap, width_ns, origin_ns, seed, intervals):
+def _fixed_sums(space, ctx, opts, fitted, future_ds, floor, cap, width_ns, origin_ns, seed, intervals, levels=None):
     width_ns, origin_ns = int(width_ns), int(origin_ns)
     if width_ns <= 0:
         raise ValueError(f"width_ns must be > 0 (got {width_ns})")
     return _window_sums(space, ctx, opts, fitted, future_ds, floor, cap, seed, intervals, "pb200_predict_sums",
-                        (width_ns, origin_ns), lambda a, b: window_slots(a, b, width_ns, origin_ns))
+                        (width_ns, origin_ns), lambda a, b: window_slots(a, b, width_ns, origin_ns), levels)
 
 
-def _period_sums(space, ctx, opts, fitted, future_ds, floor, cap, months, month_shift, seed, intervals):
+def _period_sums(space, ctx, opts, fitted, future_ds, floor, cap, months, month_shift, seed, intervals, levels=None):
     months, month_shift = _period_rule_checked(months, month_shift)
     return _window_sums(space, ctx, opts, fitted, future_ds, floor, cap, seed, intervals, "pb200_predict_period_sums",
-                        (months, month_shift), lambda a, b: period_slots(a, b, months, month_shift))
+                        (months, month_shift), lambda a, b: period_slots(a, b, months, month_shift), levels)
 
 
 def predict_sums_device(ctx: L.Context, opts: L.Options, fitted: FittedBatch, future_ds, floor, cap, width_ns: int,
-                        origin_ns: int = 0, seed: int = 0, intervals: bool = False):
-    """pb200_predict_sums_device with torch CUDA tensors; as predict_sums_host."""
+                        origin_ns: int = 0, seed: int = 0, intervals: bool = False, levels=None):
+    """pb200_predict_sums_device with torch CUDA tensors; as predict_sums_host (``levels``:
+    pb200_predict_sums_quantiles_device)."""
     return _fixed_sums(_Space(future_ds.device), ctx, opts, fitted, future_ds, floor, cap, width_ns, origin_ns, seed,
-                       intervals)
+                       intervals, levels)
 
 
 def predict_period_sums_device(ctx: L.Context, opts: L.Options, fitted: FittedBatch, future_ds, floor, cap, months: int,
-                               month_shift: int, seed: int = 0, intervals: bool = False):
-    """pb200_predict_period_sums_device with torch CUDA tensors; as predict_period_sums_host."""
+                               month_shift: int, seed: int = 0, intervals: bool = False, levels=None):
+    """pb200_predict_period_sums_device with torch CUDA tensors; as predict_period_sums_host (``levels``:
+    pb200_predict_period_sums_quantiles_device)."""
     return _period_sums(_Space(future_ds.device), ctx, opts, fitted, future_ds, floor, cap, months, month_shift, seed,
-                        intervals)
+                        intervals, levels)
 
 
 _MONTHS = ("JAN", "FEB", "MAR", "APR", "MAY", "JUN", "JUL", "AUG", "SEP", "OCT", "NOV", "DEC")
@@ -1183,11 +1215,12 @@ def period_rule(alias: str):
 
 def predict_sums_anchored_device(ctx: L.Context, opts: L.Options, fitted: FittedBatch, future_ds, floor, cap,
                                  width_ns: int, origins, frame_len, seed: int = 0, intervals: bool = False,
-                                 wmax: Optional[int] = None):
+                                 wmax: Optional[int] = None, levels=None):
     """pb200_predict_sums_anchored_device with torch CUDA tensors: predict_sums_device with a window origin per model
     (``origins`` int64 [N]) whose windows cover only the first ``frame_len[i]`` points of row i (int32 [N]; the rest
     of the row is padding that is predicted but summed into no window).  ``wmax`` defaults to the bound
-    ``window_slots`` gives over each model's first and last walked point."""
+    ``window_slots`` gives over each model's first and last walked point.  ``levels``:
+    pb200_predict_sums_anchored_quantiles_device, as in predict_sums_host."""
     import torch
     n = fitted.n
     h = int(future_ds.shape[1])
@@ -1204,7 +1237,8 @@ def predict_sums_anchored_device(ctx: L.Context, opts: L.Options, fitted: Fitted
             w = (last - origins).div(width_ns, rounding_mode="floor") - (future_ds[:, 0] - origins).div(width_ns, rounding_mode="floor")
             wmax = max(1, int(w.max().item()) + 1)
     return _window_sums(_Space(dev), ctx, opts, fitted, future_ds, floor, cap, seed, intervals,
-                        "pb200_predict_sums_anchored", (width_ns, origins.data_ptr(), frame_len.data_ptr()), int(wmax))
+                        "pb200_predict_sums_anchored", (width_ns, origins.data_ptr(), frame_len.data_ptr()), int(wmax),
+                        levels)
 
 
 def objective_host(ctx: L.Context, opts: L.Options, ds_ns: np.ndarray, y: np.ndarray, offsets: np.ndarray,
@@ -1376,7 +1410,10 @@ class CvWindows:
     ``series`` (as CvResult.row_series), ``cutoff``, ``horizon`` ((j + 1) W, ns), ``points`` (held-out rows in the
     window), ``y`` / ``yhat`` (their float64 y / yhat summed in row order) and, with intervals, ``yhat_lower`` /
     ``yhat_upper`` (percentiles over the joint draws' window sums).  ``metrics`` (with ``rolling_window``):
-    performance_metrics over the window rows with ``horizon`` as the horizon, keyed as CvResult.metrics."""
+    performance_metrics over the window rows with ``horizon`` as the horizon, keyed as CvResult.metrics.
+    With ``window_quantiles`` (DESIGN §21): ``yhat_q`` [Q, rows], the quantiles of each window's total at those levels
+    from the same draws, and (with ``rolling_window``) ``quantile_metrics``, quantile_metrics_device over the window
+    rows with ``horizon`` as the horizon."""
     width_ns: int
     series: np.ndarray
     cutoff: np.ndarray
@@ -1387,6 +1424,8 @@ class CvWindows:
     yhat_lower: Optional[np.ndarray]
     yhat_upper: Optional[np.ndarray]
     metrics: Optional[dict] = None
+    yhat_q: Optional[np.ndarray] = None
+    quantile_metrics: Optional[dict] = None
 
 
 def cv_windows_device(ctx: L.Context, ds_ns, y, plan: CvPlan, pairs, yhat, width_ns: int, wmax: Optional[int] = None):
@@ -1461,7 +1500,8 @@ def cross_validation_device(ctx: L.Context, opts: L.Options, ds_ns, y, offsets_h
                             rolling_window: Optional[float] = None, plan: Optional[CvPlan] = None,
                             keep_fits: bool = False, timings: Optional[dict] = None,
                             _row_budget: Optional[int] = None, grid=None,
-                            aggregate_ns: Optional[int] = None, quantiles=None, regressors=None) -> CvResult:
+                            aggregate_ns: Optional[int] = None, quantiles=None, regressors=None,
+                            window_quantiles=None) -> CvResult:
     """fbprophet.diagnostics.cross_validation (and, with ``rolling_window``, performance_metrics) for every series of a
     packed batch: ``ds_ns`` / ``y`` CUDA tensors sorted within each series, ``cap`` the float64 CUDA tensor of each
     series' full-history cap.  Per chunk of series: one gather, one pb200_fit_device per full-history seasonality mask
@@ -1479,6 +1519,10 @@ def cross_validation_device(ctx: L.Context, opts: L.Options, ds_ns, y, offsets_h
     With intervals the chunk's predict is pb200_predict_sums_anchored_device, whose pointwise outputs are
     pb200_predict_device's; the window totals are pb200_cv_windows_device's (stages ``windows`` and
     ``window_metrics``).
+    ``window_quantiles`` (levels, fractions in [0, 1]; needs ``aggregate_ns``, ``intervals`` and uncertainty_samples
+    > 0): that anchored call is pb200_predict_sums_anchored_quantiles_device, whose other outputs are the same, and
+    ``CvWindows.yhat_q`` / ``CvWindows.quantile_metrics`` hold the totals' quantiles and, with ``rolling_window``,
+    their calibration by horizon (stage ``window_quantile_metrics``, DESIGN §21).
     ``regressors`` (for options with regressors, required with them): a contiguous float64 CUDA tensor ``[R, rows]``
     aligned with ``ds_ns``.  fbprophet 0.5's cross_validation with prophet_copy (DESIGN §20): the full histories' (mu,
     std) by pb200_regressor_scales_device (a non-finite value raises ValueError), the cutoff fits on z = (x - mu_full) /
@@ -1502,6 +1546,12 @@ def cross_validation_device(ctx: L.Context, opts: L.Options, ds_ns, y, offsets_h
         raise ValueError("regressors= is required with options that have regressors, and taken only with them")
     if R and (grid is not None or aggregate_ns is not None or quantiles is not None):
         raise ValueError("grid, aggregate_ns and quantiles are not supported with regressors")
+    wlevels = None
+    if window_quantiles is not None:
+        if aggregate_ns is None or not intervals or opts.uncertainty_samples <= 0:
+            raise ValueError("window_quantiles need aggregate_ns, intervals and uncertainty_samples > 0")
+        wlevels = np.asarray(window_quantiles, dtype=np.float64)
+        quantile_percentiles(wlevels)
     if plan is None:
         plan = cv_plan_device(ctx, plan_options(opts), ds_ns, offsets_host, horizon_ns, period_ns, initial_ns)
         lap("plan")
@@ -1621,7 +1671,7 @@ def cross_validation_device(ctx: L.Context, opts: L.Options, ds_ns, y, offsets_h
             origins = plan.cutoff[d_pairs] + 1
             flen = torch.from_numpy(win_len.astype(np.int32)).to(dev)
             fcst, ws = predict_sums_anchored_device(ctx, opts, fitted, fut, floor_p, cap_p, W, origins, flen, seed=seed,
-                                                    intervals=True, wmax=wmax)
+                                                    intervals=True, wmax=wmax, levels=wlevels)
         elif levels is not None:
             fcst = predict_quantiles_device(ctx, opts, fitted, fut, floor_p, cap_p, levels, seed=seed,
                                             intervals=intervals and opts.uncertainty_samples > 0)
@@ -1680,7 +1730,18 @@ def cross_validation_device(ctx: L.Context, opts: L.Options, ds_ns, y, offsets_h
                                                   rolling_window)
                 wmet["series"] = wmet["series"] + v0
                 lap("window_metrics")
-            wpiece = ({k: (v.cpu().numpy() if v is not None else None) for k, v in wrows.items()}, wmet)
+            wq = None
+            if wlevels is not None:
+                wyq = ws.quantiles[:, inv][:, wk, wj]
+                wqmet = None
+                if rolling_window is not None:
+                    v0 = s0 * n_grid
+                    wqmet = quantile_metrics_device(ctx, wrows["series"] - v0, wrows["horizon"], wrows["y"], wyq, wlevels,
+                                                    (s1 - s0) * n_grid, rolling_window)
+                    wqmet["series"] = wqmet["series"] + v0
+                    lap("window_quantile_metrics")
+                wq = (wyq.cpu().numpy(), wqmet)
+            wpiece = ({k: (v.cpu().numpy() if v is not None else None) for k, v in wrows.items()}, wmet, wq)
         fh = None
         if keep_fits:
             fh = FittedBatch(*(x[inv].cpu().numpy() for x in (fitted.params, fitted.tchange, fitted.meta_i32,
@@ -1728,6 +1789,14 @@ def cross_validation_device(ctx: L.Context, opts: L.Options, ds_ns, y, offsets_h
                                                   (None, None)), 0, rolling_window)
         windows = CvWindows(W, wr["series"], wr["cutoff"], wr["horizon"], wr["points"], wr["y"], wr["yhat"],
                             wr["yhat_lower"], wr["yhat_upper"], wm)
+        if wlevels is not None:
+            windows.yhat_q = (np.concatenate([p[4][2][0] for p in pieces], axis=1) if pieces
+                              else np.zeros((wlevels.size, 0)))
+            if rolling_window is not None:
+                keys = ("series", "horizon", "level", "pinball", "share_below")
+                windows.quantile_metrics = (
+                    {k: cat([p[4][2][1][k] for p in pieces]) for k in keys} if pieces else
+                    {k: np.zeros(0, np.int64 if k in ("series", "horizon") else np.float64) for k in keys})
     yhat_q = qmetrics = None
     if levels is not None:
         yhat_q = np.concatenate([p[5][0] for p in pieces], axis=1) if pieces else np.zeros((levels.size, 0))

@@ -11,6 +11,7 @@
 #include "insample_kernel.cuh"
 #include "reg_scale_kernel.cuh"
 #include "join_kernel.cuh"
+#include "../../include/prophet_b200_window_quantiles.h"
 
 #include <algorithm>
 #include <cstdio>
@@ -1303,6 +1304,8 @@ int check_comp_args(const pb200_options* o, const void* comp, const void* lo, co
     return PB200_OK;
 }
 
+struct QuantOut;
+
 // the window arguments of pb200_predict_sums_*: the rule, the slots per model and the seven outputs (device pointers in
 // predict_device, host pointers in predict_host)
 struct SumOut {
@@ -1320,6 +1323,8 @@ struct SumOut {
     const int32_t* frame_len = nullptr;
     // pb200_predict_period_sums_*: the calendar periods of (months, month_shift), in place of width_ns / origin_ns
     int32_t months = 0, month_shift = 0;
+    // pb200_predict_*sums*_quantiles_*: the levels and their planes [n_q][n_models * wmax] (DESIGN §21)
+    const QuantOut* quant = nullptr;
 };
 
 // checked before anything is copied or launched
@@ -1423,6 +1428,7 @@ int predict_device(pb200_ctx* c, const PredictCall& p) {
     if (rc) return rc;
     if (p.n_models < 0 || p.horizon < 0 || p.n_models > (1LL << 30)) return fail(PB200_E_ARG, "sizes");
     if (p.sums && (rc = check_sum_args(p.opts, *p.sums))) return rc;
+    if (p.sums && p.sums->quant && (rc = check_quant_args(p.opts, *p.sums->quant))) return rc;
     if (p.quant && (rc = check_quant_args(p.opts, *p.quant))) return rc;
     if (p.n_models == 0 || (p.horizon == 0 && !p.sums)) return PB200_OK;
     if (!p.params || !p.tchange || !p.meta_i32 || !p.meta_i64 || !p.meta_f64 || !p.floor || !p.cap ||
@@ -1488,9 +1494,12 @@ int predict_device(pb200_ctx* c, const PredictCall& p) {
         s.quantity_sum = (long long*)sums->quantity_sum;
         s.origins = (const long long*)sums->origins;
         s.frame_len = sums->frame_len;
+        const QuantOut* q = sums->quant;
         rc = pb200::launch_mc_sum(c->stream, c->sms, a, p.opts->uncertainty_samples, p.opts->interval_width, p.seed, s,
-                                  sums->months, sums->month_shift);
-        if (rc == -1) return fail(PB200_E_ARG, "uncertainty_samples / interval_width out of range");
+                                  sums->months, sums->month_shift, q ? q->n_q : 0, q ? q->percentiles : nullptr,
+                                  q ? q->planes : nullptr);
+        if (rc == -1) return fail(PB200_E_ARG, q ? "uncertainty_samples / interval_width / n_q out of range"
+                                                 : "uncertainty_samples / interval_width out of range");
         if (rc) return fail(PB200_E_CUDA, "mc sum kernel launch", cudaGetLastError());
         c->launches++;
     }
@@ -1506,6 +1515,7 @@ int predict_host(pb200_ctx* c, const PredictCall& h) {
     if (h.sums) {
         if (h.n_models < 0 || h.horizon < 0) return fail(PB200_E_ARG, "sizes");
         if ((rc = check_sum_args(h.opts, *h.sums))) return rc;
+        if (h.sums->quant && (rc = check_quant_args(h.opts, *h.sums->quant))) return rc;
         if (h.n_models == 0) return PB200_OK;
     } else if (h.n_models <= 0 || h.horizon <= 0) {
         return (h.n_models == 0 || h.horizon == 0) ? PB200_OK : fail(PB200_E_ARG, "sizes");
@@ -1547,10 +1557,12 @@ int predict_host(pb200_ctx* c, const PredictCall& h) {
         d.quant = &dquant;
     }
     SumOut dsum;
+    QuantOut dsq;
     if (const SumOut* hs = h.sums) {
-        // on the device: five 8-byte arrays [N * wmax], then win_points [N * wmax] and n_windows [N]
-        const size_t NW = N * (size_t)hs->wmax;
-        char* next = (char*)s.reserve(ST_SUMS, NW * 44 + N * 4);
+        // on the device: five 8-byte arrays [N * wmax], the n_q planes [n_q][N * wmax] of the levels, then win_points
+        // [N * wmax] and n_windows [N]
+        const size_t NW = N * (size_t)hs->wmax, nq = hs->quant ? (size_t)hs->quant->n_q : 0;
+        char* next = (char*)s.reserve(ST_SUMS, NW * (44 + 8 * nq) + N * 4);
         if ((rc = s.status())) return rc;
         auto carve = [&](auto* h, size_t n) {   // the next n elements of the buffer, copied back to h
             auto* dp = (decltype(h))next;
@@ -1564,6 +1576,11 @@ int predict_host(pb200_ctx* c, const PredictCall& h) {
         dsum.yhat_sum = carve(hs->yhat_sum, NW);
         dsum.sum_lower = carve(hs->sum_lower, NW);
         dsum.sum_upper = carve(hs->sum_upper, NW);
+        if (hs->quant) {
+            dsq = *hs->quant;
+            dsq.planes = carve(hs->quant->planes, NW * nq);
+            dsum.quant = &dsq;
+        }
         dsum.win_points = carve(hs->win_points, NW);
         dsum.n_windows = carve(hs->n_windows, N);
         d.sums = &dsum;
@@ -1776,6 +1793,105 @@ PB200_API int pb200_predict_quantiles_host(pb200_ctx* c, const pb200_options* op
     PredictCall p = {opts, h_params, h_tchange, h_meta_i32, h_meta_i64, h_meta_f64, n_models, h_future_ds,
                      horizon, h_floor, h_cap, seed, h_yhat, h_yhat_lower, h_yhat_upper, h_yhat_int};
     p.quant = &q;
+    return predict_host(c, p);
+}
+
+// ---- quantiles of the window totals (DESIGN §21): the sums entry points plus n_q levels and their planes ----
+PB200_API int pb200_predict_sums_quantiles_device(pb200_ctx* c, const pb200_options* opts, const double* d_params,
+                         const double* d_tchange, const int32_t* d_meta_i32, const int64_t* d_meta_i64,
+                         const double* d_meta_f64, int64_t n_models, const int64_t* d_future_ds, int32_t horizon,
+                         const double* d_floor, const double* d_cap, uint64_t seed, double* d_yhat, double* d_yhat_lower,
+                         double* d_yhat_upper, int32_t* d_yhat_int, int64_t width_ns, int64_t origin_ns, int32_t wmax,
+                         int32_t* d_n_windows, int64_t* d_win_start, int32_t* d_win_points, double* d_yhat_sum,
+                         int64_t* d_quantity_sum, double* d_sum_lower, double* d_sum_upper, int32_t n_q,
+                         const double* h_percentiles, double* d_sum_quantiles) {
+    const QuantOut q = {n_q, h_percentiles, d_sum_quantiles};
+    SumOut s = {width_ns, origin_ns, wmax, d_n_windows, d_win_start, d_win_points, d_yhat_sum, d_quantity_sum,
+                d_sum_lower, d_sum_upper};
+    s.quant = &q;
+    PredictCall p = {opts, d_params, d_tchange, d_meta_i32, d_meta_i64, d_meta_f64, n_models, d_future_ds,
+                     horizon, d_floor, d_cap, seed, d_yhat, d_yhat_lower, d_yhat_upper, d_yhat_int};
+    p.sums = &s;
+    return predict_device(c, p);
+}
+
+PB200_API int pb200_predict_sums_quantiles_host(pb200_ctx* c, const pb200_options* opts, const double* h_params,
+                       const double* h_tchange, const int32_t* h_meta_i32, const int64_t* h_meta_i64,
+                       const double* h_meta_f64, int64_t n_models, const int64_t* h_future_ds, int32_t horizon,
+                       const double* h_floor, const double* h_cap, uint64_t seed, double* h_yhat, double* h_yhat_lower,
+                       double* h_yhat_upper, int32_t* h_yhat_int, int64_t width_ns, int64_t origin_ns, int32_t wmax,
+                       int32_t* h_n_windows, int64_t* h_win_start, int32_t* h_win_points, double* h_yhat_sum,
+                       int64_t* h_quantity_sum, double* h_sum_lower, double* h_sum_upper, int32_t n_q,
+                       const double* h_percentiles, double* h_sum_quantiles) {
+    const QuantOut q = {n_q, h_percentiles, h_sum_quantiles};
+    SumOut s = {width_ns, origin_ns, wmax, h_n_windows, h_win_start, h_win_points, h_yhat_sum, h_quantity_sum,
+                h_sum_lower, h_sum_upper};
+    s.quant = &q;
+    PredictCall p = {opts, h_params, h_tchange, h_meta_i32, h_meta_i64, h_meta_f64, n_models, h_future_ds,
+                     horizon, h_floor, h_cap, seed, h_yhat, h_yhat_lower, h_yhat_upper, h_yhat_int};
+    p.sums = &s;
+    return predict_host(c, p);
+}
+
+PB200_API int pb200_predict_sums_anchored_quantiles_device(pb200_ctx* c, const pb200_options* opts,
+                         const double* d_params, const double* d_tchange, const int32_t* d_meta_i32,
+                         const int64_t* d_meta_i64, const double* d_meta_f64, int64_t n_models,
+                         const int64_t* d_future_ds, int32_t horizon, const double* d_floor, const double* d_cap,
+                         uint64_t seed, double* d_yhat, double* d_yhat_lower, double* d_yhat_upper, int32_t* d_yhat_int,
+                         int64_t width_ns, const int64_t* d_origin_ns, const int32_t* d_frame_len, int32_t wmax,
+                         int32_t* d_n_windows, int64_t* d_win_start, int32_t* d_win_points, double* d_yhat_sum,
+                         int64_t* d_quantity_sum, double* d_sum_lower, double* d_sum_upper, int32_t n_q,
+                         const double* h_percentiles, double* d_sum_quantiles) {
+    if (n_models > 0 && (!d_origin_ns || !d_frame_len)) return fail(PB200_E_ARG, "null pointer (origins / frame lengths)");
+    const QuantOut q = {n_q, h_percentiles, d_sum_quantiles};
+    SumOut s = {width_ns, 0, wmax, d_n_windows, d_win_start, d_win_points, d_yhat_sum, d_quantity_sum, d_sum_lower,
+                d_sum_upper};
+    s.origins = d_origin_ns;
+    s.frame_len = d_frame_len;
+    s.quant = &q;
+    PredictCall p = {opts, d_params, d_tchange, d_meta_i32, d_meta_i64, d_meta_f64, n_models, d_future_ds,
+                     horizon, d_floor, d_cap, seed, d_yhat, d_yhat_lower, d_yhat_upper, d_yhat_int};
+    p.sums = &s;
+    return predict_device(c, p);
+}
+
+PB200_API int pb200_predict_period_sums_quantiles_device(pb200_ctx* c, const pb200_options* opts,
+                         const double* d_params, const double* d_tchange, const int32_t* d_meta_i32,
+                         const int64_t* d_meta_i64, const double* d_meta_f64, int64_t n_models,
+                         const int64_t* d_future_ds, int32_t horizon, const double* d_floor, const double* d_cap,
+                         uint64_t seed, double* d_yhat, double* d_yhat_lower, double* d_yhat_upper, int32_t* d_yhat_int,
+                         int32_t months, int32_t month_shift, int32_t wmax, int32_t* d_n_windows, int64_t* d_win_start,
+                         int32_t* d_win_points, double* d_yhat_sum, int64_t* d_quantity_sum, double* d_sum_lower,
+                         double* d_sum_upper, int32_t n_q, const double* h_percentiles, double* d_sum_quantiles) {
+    if (months == 0) return fail(PB200_E_ARG, "months must be 1, 3 or 12 and month_shift in [0, months)");
+    const QuantOut q = {n_q, h_percentiles, d_sum_quantiles};
+    SumOut s = {0, 0, wmax, d_n_windows, d_win_start, d_win_points, d_yhat_sum, d_quantity_sum, d_sum_lower, d_sum_upper};
+    s.months = months;
+    s.month_shift = month_shift;
+    s.quant = &q;
+    PredictCall p = {opts, d_params, d_tchange, d_meta_i32, d_meta_i64, d_meta_f64, n_models, d_future_ds,
+                     horizon, d_floor, d_cap, seed, d_yhat, d_yhat_lower, d_yhat_upper, d_yhat_int};
+    p.sums = &s;
+    return predict_device(c, p);
+}
+
+PB200_API int pb200_predict_period_sums_quantiles_host(pb200_ctx* c, const pb200_options* opts,
+                       const double* h_params, const double* h_tchange, const int32_t* h_meta_i32,
+                       const int64_t* h_meta_i64, const double* h_meta_f64, int64_t n_models,
+                       const int64_t* h_future_ds, int32_t horizon, const double* h_floor, const double* h_cap,
+                       uint64_t seed, double* h_yhat, double* h_yhat_lower, double* h_yhat_upper, int32_t* h_yhat_int,
+                       int32_t months, int32_t month_shift, int32_t wmax, int32_t* h_n_windows, int64_t* h_win_start,
+                       int32_t* h_win_points, double* h_yhat_sum, int64_t* h_quantity_sum, double* h_sum_lower,
+                       double* h_sum_upper, int32_t n_q, const double* h_percentiles, double* h_sum_quantiles) {
+    if (months == 0) return fail(PB200_E_ARG, "months must be 1, 3 or 12 and month_shift in [0, months)");
+    const QuantOut q = {n_q, h_percentiles, h_sum_quantiles};
+    SumOut s = {0, 0, wmax, h_n_windows, h_win_start, h_win_points, h_yhat_sum, h_quantity_sum, h_sum_lower, h_sum_upper};
+    s.months = months;
+    s.month_shift = month_shift;
+    s.quant = &q;
+    PredictCall p = {opts, h_params, h_tchange, h_meta_i32, h_meta_i64, h_meta_f64, n_models, h_future_ds,
+                     horizon, h_floor, h_cap, seed, h_yhat, h_yhat_lower, h_yhat_upper, h_yhat_int};
+    p.sums = &s;
     return predict_host(c, p);
 }
 

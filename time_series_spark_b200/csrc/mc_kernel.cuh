@@ -538,7 +538,9 @@ __device__ __forceinline__ long long window_of(const long long ds, const long lo
 // repeating its last timestamp, which leaves Tmax as it is).
 // CAL: the windows are the calendar periods of a.months / a.month_shift (PeriodSumArgs), each starting at its period start;
 // the draws, the sums and the selection are those of the fixed-width instance.
-template <bool LOGI, bool PER_MODEL, bool CAL = false>
+// QUANT (DESIGN §21): the same selection also writes levels [0, mc.lv.nq) of each window's sums to the planes
+// mc.planes [nq][n_models * wmax] (the slot layout of lower / upper); the bounds are levels nq and nq + 1.
+template <bool LOGI, bool PER_MODEL, bool CAL = false, bool QUANT = false>
 __global__ void __launch_bounds__(MC_THREADS, 1) mc_sum_kernel(const McSumArgsT<CAL> a) {
     extern __shared__ __align__(16) unsigned char mc_smem[];
     double* rows = (double*)mc_smem;                       // [MC_TILE][MC_NP], as mc_kernel
@@ -572,7 +574,12 @@ __global__ void __launch_bounds__(MC_THREADS, 1) mc_sum_kernel(const McSumArgsT<
                 const int wi = nw - n + warp;
                 if (warp < n && wi < a.wmax)
                     row_levels<false>(rows + warp * MC_NP, mc.n_samples, mc.lv, sw, lane, [&](const int l, const double v) {
-                        (l == 0 ? mc.lower : mc.upper)[wbase + wi] = v;
+                        if constexpr (QUANT) {
+                            if (l < mc.lv.nq) mc.planes[(size_t)l * mc.p.n_models * a.wmax + wbase + wi] = v;
+                            else (l == mc.lv.nq ? mc.lower : mc.upper)[wbase + wi] = v;
+                        } else {
+                            (l == 0 ? mc.lower : mc.upper)[wbase + wi] = v;
+                        }
                     });
                 __syncthreads();
             };
@@ -642,6 +649,8 @@ __global__ void __launch_bounds__(MC_THREADS, 1) mc_sum_kernel(const McSumArgsT<
             a.quantity_sum[wbase + w] = INT64_MIN;
             mc.lower[wbase + w] = NAN;
             mc.upper[wbase + w] = NAN;
+            if constexpr (QUANT)
+                for (int l = 0; l < mc.lv.nq; ++l) mc.planes[(size_t)l * mc.p.n_models * a.wmax + wbase + w] = NAN;
         }
     }
 }
@@ -655,13 +664,31 @@ cudaError_t launch_mc_inst(cudaStream_t st, int grid, size_t smem, const McArgsT
     return cudaGetLastError();
 }
 
-template <bool LOGI, bool PER_MODEL, bool CAL = false>
+template <bool LOGI, bool PER_MODEL, bool CAL = false, bool QUANT = false>
 cudaError_t launch_mc_sum_inst(cudaStream_t st, int grid, const McSumArgsT<CAL>& a) {
-    const cudaError_t e = cudaFuncSetAttribute(mc_sum_kernel<LOGI, PER_MODEL, CAL>,
+    const cudaError_t e = cudaFuncSetAttribute(mc_sum_kernel<LOGI, PER_MODEL, CAL, QUANT>,
                                                cudaFuncAttributeMaxDynamicSharedMemorySize, (int)MC_SMEM);
     if (e != cudaSuccess) return e;
-    mc_sum_kernel<LOGI, PER_MODEL, CAL><<<grid, MC_THREADS, MC_SMEM, st>>>(a);
+    mc_sum_kernel<LOGI, PER_MODEL, CAL, QUANT><<<grid, MC_THREADS, MC_SMEM, st>>>(a);
     return cudaGetLastError();
+}
+
+// the instance of mc_sum_kernel for the growth, the window rule and the levels (nq > 0: QUANT)
+template <bool QUANT>
+cudaError_t launch_mc_sum_rule(cudaStream_t st, int grid, bool logi, bool per_model, const McSumArgs& s, int months,
+                               int month_shift) {
+    if (months > 0) {
+        PeriodSumArgs c;
+        static_cast<McSumArgs&>(c) = s;
+        c.months = months;
+        c.month_shift = month_shift;
+        return logi ? launch_mc_sum_inst<true, false, true, QUANT>(st, grid, c)
+                    : launch_mc_sum_inst<false, false, true, QUANT>(st, grid, c);
+    }
+    return logi ? (per_model ? launch_mc_sum_inst<true, true, false, QUANT>(st, grid, s)
+                             : launch_mc_sum_inst<true, false, false, QUANT>(st, grid, s))
+                : (per_model ? launch_mc_sum_inst<false, true, false, QUANT>(st, grid, s)
+                             : launch_mc_sum_inst<false, false, false, QUANT>(st, grid, s));
 }
 
 // the sample count, the levels (McLevels: the nq percentiles pct[0, nq), each in [0, 100], then with `bounds` the
@@ -756,27 +783,22 @@ inline int launch_mc_reg(cudaStream_t st, int sms, const PredictArgs& p, const R
 // mc_sum_kernel over the frame of p, whose yhat / yhat_int predict_kernel has written on the same stream; s.mc is filled
 // here but for its lower / upper (the window bounds).  s.origins != null: the per-model instance (s.frame_len as well);
 // months > 0: the calendar instance over the periods of (months, month_shift), whose width_ns / origin_ns are unused.
-// Returns as launch_mc
+// nq > 0: the QUANT instance, which also writes the window quantiles at the percentiles pct [nq] to planes
+// [nq][n_models * wmax].  Returns as launch_mc
 inline int launch_mc_sum(cudaStream_t st, int sms, const PredictArgs& p, int n_samples, double width, uint64_t seed,
-                         McSumArgs& s, int months = 0, int month_shift = 0) {
+                         McSumArgs& s, int months = 0, int month_shift = 0, int nq = 0, const double* pct = nullptr,
+                         double* planes = nullptr) {
     double* const lo = s.mc.lower;
     double* const hi = s.mc.upper;
-    if (!mc_args(s.mc, p, n_samples, width, seed)) return -1;
+    if ((nq > 0) != (planes != nullptr)) return -1;
+    if (!mc_args(s.mc, p, n_samples, width, seed, true, nq, pct)) return -1;
     s.mc.lower = lo;
     s.mc.upper = hi;
+    s.mc.planes = planes;
     const int grid = p.n_models < sms ? p.n_models : sms;
     const bool logi = p.growth == PB200_GROWTH_LOGISTIC, per_model = s.origins != nullptr;
-    cudaError_t e;
-    if (months > 0) {
-        PeriodSumArgs c;
-        static_cast<McSumArgs&>(c) = s;
-        c.months = months;
-        c.month_shift = month_shift;
-        e = logi ? launch_mc_sum_inst<true, false, true>(st, grid, c) : launch_mc_sum_inst<false, false, true>(st, grid, c);
-    } else {
-        e = logi ? (per_model ? launch_mc_sum_inst<true, true>(st, grid, s) : launch_mc_sum_inst<true, false>(st, grid, s))
-                 : (per_model ? launch_mc_sum_inst<false, true>(st, grid, s) : launch_mc_sum_inst<false, false>(st, grid, s));
-    }
+    const cudaError_t e = nq > 0 ? launch_mc_sum_rule<true>(st, grid, logi, per_model, s, months, month_shift)
+                                 : launch_mc_sum_rule<false>(st, grid, logi, per_model, s, months, month_shift);
     return e == cudaSuccess ? 0 : 1;
 }
 

@@ -9,7 +9,7 @@ prophet_copy does it: every cutoff fit takes the full history's active seasonali
 ``backtest.*`` option below.  With ``model.regressors`` (DESIGN §20) the input's regressor columns are read as the
 modeler reads them and every cutoff is fitted as fbprophet 0.5's cross_validation does it: on the full history's
 standardised values, keeping the full model's (mu, std) where the cutoff's history is not standardised;
-``backtest.aggregate`` and ``backtest.quantiles`` are refused with it.
+``backtest.aggregate`` (and so ``backtest.aggregate_quantiles``) and ``backtest.quantiles`` are refused with it.
 
 Keys (``backtest.*``):
   horizon            pandas Timedelta string, required ("1 days")
@@ -24,6 +24,9 @@ Keys (``backtest.*``):
   quantiles          a list of 1 to 32 levels in [0, 1]: the held-out quantiles of each level from uncertainty_samples
                      draws (with or without intervals) and their pinball loss and share of y at or below them by
                      horizon (DESIGN §15); needs io.quantile_metrics, not with aggregate
+  aggregate_quantiles  with aggregate and intervals, a list of 1 to 32 levels in [0, 1]: the quantiles of each
+                     window's total from the draws behind its interval, and their pinball loss and share of the held-out
+                     total at or below them by horizon (j + 1) W (DESIGN §21); needs io.window_quantile_metrics
 Outputs (parquet, one part file per rank):
   io.metrics          series_id, dim_id, horizon duration[ns], mse, rmse, mae, mape[, coverage]
   io.cv_rows          (optional) series_id, dim_id, ds, cutoff, y, yhat[, yhat_lower, yhat_upper][, yhat_q<level>...]
@@ -31,7 +34,8 @@ Outputs (parquet, one part file per rank):
                       row per (horizon, level)
   io.window_metrics   (with aggregate) series_id, dim_id, horizon duration[ns], mse, rmse, mae, mape[, coverage]
   io.window_rows      (optional, with aggregate) series_id, dim_id, cutoff, horizon, window_points, y, yhat[,
-                      yhat_lower, yhat_upper]
+                      yhat_lower, yhat_upper][, yhat_q<level>... with aggregate_quantiles]
+  io.window_quantile_metrics  (with aggregate_quantiles) io.quantile_metrics' columns over the window rows
 """
 from __future__ import annotations
 
@@ -99,6 +103,18 @@ def backtest_spec_from_config(config) -> dict:
         if not (config.get("io", {}) or {}).get("quantile_metrics"):
             raise ValueError("backtest.quantiles needs io.quantile_metrics, the directory the quantile metrics are written to")
     spec["quantiles"] = levels
+    wlevels = quantile_levels({"quantiles": b.get("aggregate_quantiles")}, "backtest.aggregate_quantiles")
+    if wlevels is not None:
+        if spec["aggregate"] is None:
+            raise ValueError("backtest.aggregate_quantiles needs backtest.aggregate: its levels are quantiles of the "
+                             "window totals")
+        if not intervals:
+            raise ValueError("backtest.aggregate_quantiles needs backtest.intervals: the levels come from the draws "
+                             "behind the window totals' intervals")
+        if not (config.get("io", {}) or {}).get("window_quantile_metrics"):
+            raise ValueError("backtest.aggregate_quantiles needs io.window_quantile_metrics, the directory the window "
+                             "quantile metrics are written to")
+        spec["aggregate_quantiles"] = wlevels
     return spec
 
 
@@ -166,9 +182,10 @@ def _metrics_table(series_id, dim_id, m: dict, failed) -> pa.Table:
     return pa.table(cols)
 
 
-def assemble_window_outputs(series_id, dim_id, res: batched.CvResult, with_rows: bool = True):
+def assemble_window_outputs(series_id, dim_id, res: batched.CvResult, with_rows: bool = True, levels=None):
     """Window metrics (and window row) tables of a CvResult made with aggregate_ns; the same failed-fit rule as
-    assemble_outputs (which prints the lines)."""
+    assemble_outputs (which prints the lines).  ``levels`` (the CvResult made with them as window_quantiles): the rows
+    get a yhat_q<level> column per level."""
     failed = _failed_series(series_id, dim_id, res, announce=False)
     w = res.windows
     metrics = _metrics_table(series_id, dim_id, w.metrics, failed)
@@ -186,6 +203,8 @@ def assemble_window_outputs(series_id, dim_id, res: batched.CvResult, with_rows:
         if w.yhat_lower is not None:
             rc["yhat_lower"] = pa.array(w.yhat_lower[keep], pa.float64())
             rc["yhat_upper"] = pa.array(w.yhat_upper[keep], pa.float64())
+        for q, lv in enumerate(levels or ()):
+            rc[quantile_column(lv)] = pa.array(w.yhat_q[q][keep], pa.float64())
         rows = pa.table(rc)
     return metrics, rows
 
@@ -198,8 +217,18 @@ QUANTILE_METRICS_SCHEMA = pa.schema([("series_id", pa.int32()), ("dim_id", pa.in
 def quantile_metrics_table(series_id, dim_id, res: batched.CvResult) -> pa.Table:
     """io.quantile_metrics of a CvResult made with quantiles: one row per (series, horizon, level); the same failed-fit
     rule as assemble_outputs (which prints the lines)."""
-    failed = _failed_series(series_id, dim_id, res, announce=False)
-    m = res.quantile_metrics
+    return _quantile_metrics_table(series_id, dim_id, res.quantile_metrics,
+                                   _failed_series(series_id, dim_id, res, announce=False))
+
+
+def window_quantile_metrics_table(series_id, dim_id, res: batched.CvResult) -> pa.Table:
+    """io.window_quantile_metrics of a CvResult made with window_quantiles: quantile_metrics_table's rows over the window
+    rows, horizon (j + 1) W."""
+    return _quantile_metrics_table(series_id, dim_id, res.windows.quantile_metrics,
+                                   _failed_series(series_id, dim_id, res, announce=False))
+
+
+def _quantile_metrics_table(series_id, dim_id, m: dict, failed) -> pa.Table:
     keep = ~failed[m["series"]]
     ms = m["series"][keep]
     return pa.table({"series_id": pa.array(np.asarray(series_id)[ms], pa.int32()),
@@ -244,6 +273,7 @@ class ProphetBacktester:
         self.rank_local_input = False
         self.window_outputs = None     # (window metrics, window rows or None) with backtest.aggregate
         self.quantile_metrics = None   # with backtest.quantiles
+        self.window_quantile_metrics = None   # with backtest.aggregate_quantiles
 
     def read_input_dataframe(self, spark=None):
         reader = ProphetModeler(self.config)
@@ -279,6 +309,7 @@ class ProphetBacktester:
         with_rows = bool(io.get("cv_rows"))
         W = spec["aggregate"]
         levels = spec["quantiles"]
+        wlevels = spec.get("aggregate_quantiles")
         if pk.n == 0:
             empty_metrics = lambda: dict({k: np.zeros(0, np.int64 if k in ("series", "horizon") else np.float64)  # noqa: E731
                                           for k in ("series", "horizon", "mse", "rmse", "mae", "mape")},
@@ -291,7 +322,11 @@ class ProphetBacktester:
                 iv = np.zeros(0) if spec["intervals"] else None
                 res.windows = batched.CvWindows(W, *(np.zeros(0, np.int64),) * 3, np.zeros(0, np.int32), np.zeros(0),
                                                 np.zeros(0), iv, iv, empty_metrics())
-                self.window_outputs = assemble_window_outputs(pk.series_id, pk.dim_id, res, bool(io.get("window_rows")))
+                if wlevels is not None:
+                    res.windows.yhat_q = np.zeros((len(wlevels), 0))
+                    self.window_quantile_metrics = QUANTILE_METRICS_SCHEMA.empty_table()
+                self.window_outputs = assemble_window_outputs(pk.series_id, pk.dim_id, res, bool(io.get("window_rows")),
+                                                              wlevels)
             if levels is not None:
                 res.yhat_q = np.zeros((len(levels), 0))
                 self.quantile_metrics = QUANTILE_METRICS_SCHEMA.empty_table()
@@ -320,7 +355,7 @@ class ProphetBacktester:
         res = batched.cross_validation_device(ctx, opts, ds, y, pk.offsets, floor, cap, spec["horizon"], spec["period"],
                                               spec["initial"], intervals=spec["intervals"], seed=spec["seed"],
                                               rolling_window=spec["rolling_window"], plan=plan, aggregate_ns=W,
-                                              quantiles=levels, regressors=pk.regressors)
+                                              quantiles=levels, regressors=pk.regressors, window_quantiles=wlevels)
         for code, msg in ((L.ST_CAP_LE_FLOOR, "cap must be greater than floor (which defaults to 0)."),
                           (L.ST_BAD_INPUT, "Found non-finite y or a zero time span in a series.")):
             hit = np.zeros(pk.n, bool)
@@ -332,18 +367,23 @@ class ProphetBacktester:
         if levels is not None:
             self.quantile_metrics = quantile_metrics_table(pk.series_id, pk.dim_id, res)
         if W is not None:
-            self.window_outputs = assemble_window_outputs(pk.series_id, pk.dim_id, res, bool(io.get("window_rows")))
+            self.window_outputs = assemble_window_outputs(pk.series_id, pk.dim_id, res, bool(io.get("window_rows")),
+                                                          wlevels)
+        if wlevels is not None:
+            self.window_quantile_metrics = window_quantile_metrics_table(pk.series_id, pk.dim_id, res)
         print(f"Backtest: {out[0].num_rows} metrics rows in {time.time() - t0:.1f} s")
         return out
 
     def persist(self, metrics: pa.Table, rows) -> None:
         """Parquet part file per rank under io.metrics (and io.cv_rows, with backtest.aggregate io.window_metrics and
-        io.window_rows, with backtest.quantiles io.quantile_metrics)."""
+        io.window_rows, with backtest.quantiles io.quantile_metrics, with backtest.aggregate_quantiles
+        io.window_quantile_metrics)."""
         io = self.config["io"]
         rank = pdist.world()[0]
         wm, wr = self.window_outputs or (None, None)
         for key, tbl in (("metrics", metrics), ("cv_rows", rows), ("window_metrics", wm), ("window_rows", wr),
-                         ("quantile_metrics", self.quantile_metrics)):
+                         ("quantile_metrics", self.quantile_metrics),
+                         ("window_quantile_metrics", self.window_quantile_metrics)):
             if tbl is None or not io.get(key):
                 continue
             pdist.prepare_output_dir(io[key])

@@ -17,7 +17,10 @@ component columns ``trend, yearly, weekly, daily, multiplicative_terms, additive
 write, to ``io.aggregates``, the forecast total of every such window of every model with the interval of the total from
 the joint draws -- DESIGN §13), ``forecast.aggregate_origin`` (where window 0 starts, default 1970-01-01),
 ``forecast.aggregate_period`` (a pandas period alias such as ``'M'``, ``'Q-NOV'``, ``'Y'`` or ``'W-SUN'``: the same
-``io.aggregates`` table over calendar months, quarters, years or weeks -- DESIGN §17) and
+``io.aggregates`` table over calendar months, quarters, years or weeks -- DESIGN §17),
+``forecast.aggregate_quantiles`` (with ``forecast.aggregate`` or ``forecast.aggregate_period``, a list of 1 to 32 levels
+in [0, 1]: one float64 column ``yhat_q<level>`` per level in ``io.aggregates``, after ``yhat_upper``, the percentile
+100 level of the window total's ``uncertainty_samples`` draws -- DESIGN §21) and
 ``forecast.quantiles`` (a list of 1 to 32 levels in [0, 1]: one float64 column ``yhat_q<level>`` per level, the
 percentile 100 level of the point's ``uncertainty_samples`` draws -- DESIGN §15).
 
@@ -212,11 +215,36 @@ def aggregate_period(config):
         raise ValueError(f"forecast.aggregate_period: {e}") from None
 
 
+def aggregate_quantiles(config):
+    """``forecast.aggregate_quantiles`` checked as quantile_levels checks forecast.quantiles, or None without it.  The
+    levels describe the window totals of io.aggregates, so the key needs forecast.aggregate or
+    forecast.aggregate_period."""
+    fc = config.get("forecast", {}) or {}
+    levels = quantile_levels({"quantiles": fc.get("aggregate_quantiles")}, "forecast.aggregate_quantiles")
+    if levels is not None and fc.get("aggregate") is None and fc.get("aggregate_period") is None:
+        raise ValueError("forecast.aggregate_quantiles needs forecast.aggregate or forecast.aggregate_period: its levels "
+                         "are quantiles of the window totals")
+    return levels
+
+
+def aggregate_schema(levels=None) -> pa.Schema:
+    """io.aggregates' schema: AGGREGATE_SCHEMA, then one float64 column quantile_column(q) per level of
+    forecast.aggregate_quantiles."""
+    schema = AGGREGATE_SCHEMA
+    for q in levels or ():
+        schema = schema.append(pa.field(quantile_column(q), pa.float64()))
+    return schema
+
+
 def aggregate_table(sid, did, ok, ws: "batched.WindowSums") -> pa.Table:
-    """One row per (model, window) of the models that have a forecast, from a shard's WindowSums."""
+    """One row per (model, window) of the models that have a forecast, from a shard's WindowSums (a WindowQuantiles
+    adds its levels' columns after yhat_upper)."""
     wmax = ws.start.shape[1]
     keep = (np.arange(wmax)[None, :] < ws.n_windows[:, None]) & ok[:, None]
     rows = np.nonzero(keep)[0]
+    quant = {}
+    if isinstance(ws, batched.WindowQuantiles):
+        quant = {quantile_column(q): pa.array(ws.quantiles[j][keep], pa.float64()) for j, q in enumerate(ws.levels)}
     return pa.table({
         "series_id": pa.array(sid[rows], pa.int32()),
         "dim_id": pa.array(did[rows], pa.int32()),
@@ -226,6 +254,7 @@ def aggregate_table(sid, did, ok, ws: "batched.WindowSums") -> pa.Table:
         "yhat": pa.array(ws.yhat_sum[keep], pa.float64()),
         "yhat_lower": pa.array(ws.lower[keep], pa.float64()),
         "yhat_upper": pa.array(ws.upper[keep], pa.float64()),
+        **quant,
     })
 
 
@@ -383,7 +412,8 @@ class _ForecastTimeSeriesOp:
         period = aggregate_period(self.config)
         rule = period[1:] if period and period[0] == "fixed" else aggregate_rule(self.config)
         months = period[1:] if period and period[0] == "months" else None
-        self.aggregates = AGGREGATE_SCHEMA.empty_table() if rule or months else None
+        alevels = aggregate_quantiles(self.config)
+        self.aggregates = aggregate_schema(alevels).empty_table() if rule or months else None
         levels = forecast_quantiles(self.config)
         if want_intervals or rule or months or levels:
             width = float(fc.get("interval_width", 0.8))
@@ -454,11 +484,12 @@ class _ForecastTimeSeriesOp:
             res = self._predict_regressors(ctx, opts, info, fitted, future, floor, cap, sid, did, ok, want_intervals)
         elif rule:
             res, sums = batched.predict_sums_host(ctx, opts, fitted, future, floor, cap, rule[0], rule[1],
-                                                  seed=int(fc.get("seed", 0)), intervals=want_intervals)
+                                                  seed=int(fc.get("seed", 0)), intervals=want_intervals, levels=alevels)
             self.aggregates = aggregate_table(sid, did, ok, sums)
         elif months:
             res, sums = batched.predict_period_sums_host(ctx, opts, fitted, future, floor, cap, months[0], months[1],
-                                                         seed=int(fc.get("seed", 0)), intervals=want_intervals)
+                                                         seed=int(fc.get("seed", 0)), intervals=want_intervals,
+                                                         levels=alevels)
             self.aggregates = aggregate_table(sid, did, ok, sums)
         elif levels:
             res = batched.predict_quantiles_host(ctx, opts, fitted, future, floor, cap, levels, seed=int(fc.get("seed", 0)),
@@ -708,7 +739,7 @@ class ProphetScorer:
     def write_aggregates(self, aggregates: pa.Table, created_timestamp: str):
         """The window totals of forecast.aggregate as CSV with header under io.aggregates: one part file per rank,
         ``created_timestamp, series_id, dim_id, window_start, window_points, forecast_quantity, yhat, yhat_lower,
-        yhat_upper``; window_start printed like forecast_timestamp."""
+        yhat_upper[, yhat_q<level>...]``; window_start printed like forecast_timestamp."""
         out = self.config["io"]["aggregates"]
         rank = pdist.world()[0]
         pdist.prepare_output_dir(out)
@@ -725,6 +756,7 @@ class ProphetScorer:
         aggregate_period(config)            # a bad forecast.aggregate_period, forecast.aggregate or forecast.quantiles
         aggregate_rule(config)              # fails before anything is read
         forecast_quantiles(config)
+        aggregate_quantiles(config)
         pdist.init_process_group()          # no-op unless launched by torchrun with WORLD_SIZE > 1
         scorer = ProphetScorer(config)
         model_df = scorer.read_model_dataframe(spark_session)
